@@ -15,6 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libfs2b200.so")
 
 FS2_DUR_I64, FS2_DUR_F32, FS2_DUR_I32 = 0, 1, 2
+FS2_PER_UTTERANCE = 1      # flag of fs2_encode_ex / fs2_decode_ex
 MATH_FP32, MATH_TF32, MATH_3XTF32, MATH_F16 = 0, 1, 2, 3
 # "3xtf32" is the historical name of the error-compensated mode (now three f16 products per term); "3xf16" is an alias
 MATH_MODES = {"fp32": MATH_FP32, "tf32": MATH_TF32, "3xtf32": MATH_3XTF32, "3xf16": MATH_3XTF32, "f16": MATH_F16}
@@ -48,9 +49,11 @@ SIGNATURES = {
     "fs2_load_weights": [_P, C.POINTER(WeightDesc), _I, _P],
     "fs2_workspace_bytes": [_P, _I, _I, _I, C.POINTER(_SZ)],
     "fs2_encode": [_P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _P],
+    "fs2_encode_ex": [_P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _I, _P],
     "fs2_length_plan": [_P, _I, _P, _F, _I, _I, _I, _P, _P, _P, _P],
     "fs2_length_gather": [_P, _P, _P, _I, _I, _I, _P, _I, _P],
     "fs2_decode": [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _SZ, _P],
+    "fs2_decode_ex": [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _SZ, _I, _P],
     "fs2_masked_losses": [_P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P],
     "fs2_bucketize": [_P, _P, _I, _L, _P, _P],
     "fs2_one_hot": [_P, _L, _I, _P, _P],

@@ -160,6 +160,15 @@ RowNorm make_norm(const Norm& n, const float* x, int ldx, int64_t rows, int C, f
   return r;
 }
 
+// Per-utterance mode (FS2_PER_UTTERANCE): zlens != nullptr.  Every tensor a convolution reads or the caller receives then
+// holds exact zeros at rows t >= zlens[b], so each convolution's "same" padding falls at the utterance's own length, as in
+// a B = 1 run.  zlens == nullptr leaves the kernels exactly as in the reference-semantics path.
+TapGemm masked(TapGemm g, const int64_t* zlens) { g.lens = zlens; return g; }
+RowNorm masked(RowNorm r, const int64_t* zlens, int L) {
+  if (zlens) { r.lens = zlens; r.L = L; }
+  return r;
+}
+
 struct BlockBufs {
   float *x, *y;            // fp32 rows [rows, C]: block input / output ping-pong (the residual stream)
   float *qkv, *vt, *ctx, *hid;   // fp32 families: q|k|v rows, transposed V, context, conv-FFN hidden
@@ -167,8 +176,8 @@ struct BlockBufs {
 };
 
 // FFT blocks of the fp32-FMA and tf32 families (fp32 rows everywhere); the result lands in *result
-int run_blocks(const std::vector<Block>& blocks, const BlockBufs& w, const int64_t* lens, int B, int L, int C, int heads,
-               int math_mode, bool is_dec, cudaStream_t st, float** result) {
+int run_blocks(const std::vector<Block>& blocks, const BlockBufs& w, const int64_t* lens, const int64_t* zlens, int B, int L,
+               int C, int heads, int math_mode, bool is_dec, cudaStream_t st, float** result) {
   const int64_t rows = (int64_t)B * L;
   const int c_qkv = is_dec ? P_DEC_QKV : P_ENC_QKV, c_att = is_dec ? P_DEC_ATTN : P_ENC_ATTN;
   const int c_out = is_dec ? P_DEC_OUT : P_ENC_OUT, c_w1 = is_dec ? P_DEC_W1 : P_ENC_W1, c_w2 = is_dec ? P_DEC_W2 : P_ENC_W2;
@@ -176,7 +185,7 @@ int run_blocks(const std::vector<Block>& blocks, const BlockBufs& w, const int64
   for (const Block& k : blocks) {
     int rc;
     // q | k | v projection (attention.py:48-50), one GEMM with N = 3C
-    TapGemm gq = make_gemm(k.qkv, x, C, B, L, ACT_NONE, nullptr, 0, w.qkv, 3 * C);
+    TapGemm gq = masked(make_gemm(k.qkv, x, C, B, L, ACT_NONE, nullptr, 0, w.qkv, 3 * C), zlens);
     if (math_mode == FS2_MATH_TF32) {  // V third stored transposed for the tensor-core attention (gemm_tc.cu epilogue)
       gq.vt_out = w.vt; gq.vt_col0 = 2 * C; gq.vt_dk = C / heads; gq.vt_heads = heads; gq.vt_lpad = round4(L);
     }
@@ -187,13 +196,15 @@ int run_blocks(const std::vector<Block>& blocks, const BlockBufs& w, const int64
                                       : attention_fp32(w.qkv, lens, B, L, C, heads, w.ctx, st);
       if (rc) return rc;
     }
-    // x = LN(x + linear_out(ctx)) (attention.py:74, encoder.py:60-62)
-    if ((rc = dense(make_gemm(k.out, w.ctx, C, B, L, ACT_NONE, x, C, y, C), math_mode, st, c_out))) return rc;
-    if ((rc = norm_rows(make_norm(k.ln1, y, C, rows, C, x, C), st))) return rc;
+    // x = LN(x + linear_out(ctx)) (attention.py:74, encoder.py:60-62).  Per-utterance mode: ctx rows past len are not
+    // guaranteed to be zero (the attention kernels scale whatever their query rows produced by 0, and those query rows
+    // may be unwritten); the out-projection reads each ctx row only for its own output row, which it writes as 0 there
+    if ((rc = dense(masked(make_gemm(k.out, w.ctx, C, B, L, ACT_NONE, x, C, y, C), zlens), math_mode, st, c_out))) return rc;
+    if ((rc = norm_rows(masked(make_norm(k.ln1, y, C, rows, C, x, C), zlens, L), st))) return rc;
     // conv-FFN: hid = relu(conv_k(x)); x = LN(x + conv_1(hid))  (modules.py:247-248, encoder.py:64-69)
-    if ((rc = dense(make_gemm(k.w1, x, C, B, L, ACT_RELU, nullptr, 0, w.hid, k.w1.N), math_mode, st, c_w1))) return rc;
-    if ((rc = dense(make_gemm(k.w2, w.hid, k.w1.N, B, L, ACT_NONE, x, C, y, C), math_mode, st, c_w2))) return rc;
-    if ((rc = norm_rows(make_norm(k.ln2, y, C, rows, C, x, C), st))) return rc;
+    if ((rc = dense(masked(make_gemm(k.w1, x, C, B, L, ACT_RELU, nullptr, 0, w.hid, k.w1.N), zlens), math_mode, st, c_w1))) return rc;
+    if ((rc = dense(masked(make_gemm(k.w2, w.hid, k.w1.N, B, L, ACT_NONE, x, C, y, C), zlens), math_mode, st, c_w2))) return rc;
+    if ((rc = norm_rows(masked(make_norm(k.ln2, y, C, rows, C, x, C), zlens, L), st))) return rc;
   }
   *result = x;
   return FS2_OK;
@@ -203,8 +214,8 @@ int run_blocks(const std::vector<Block>& blocks, const BlockBufs& w, const int64
 // planes its consumer reads; fp32 rows exist only for the residual stream (x, y).  x3: error-compensated (hi + lo planes,
 // fp32-class); else f16 on the hi planes; residual + LayerNorm run as a row kernel after each projection.
 // On entry w.xp holds the planes of w.x; on exit it holds the planes of *result.
-int run_blocks_planes(const std::vector<Block>& blocks, const BlockBufs& w, const int64_t* lens, int B, int L, int C, int heads,
-                      bool x3, bool is_dec, cudaStream_t st, float** result) {
+int run_blocks_planes(const std::vector<Block>& blocks, const BlockBufs& w, const int64_t* lens, const int64_t* zlens, int B,
+                      int L, int C, int heads, bool x3, bool is_dec, cudaStream_t st, float** result) {
   const int64_t rows = (int64_t)B * L;
   const int c_qkv = is_dec ? P_DEC_QKV : P_ENC_QKV, c_att = is_dec ? P_DEC_ATTN : P_ENC_ATTN;
   const int c_out = is_dec ? P_DEC_OUT : P_ENC_OUT, c_w1 = is_dec ? P_DEC_W1 : P_ENC_W1, c_w2 = is_dec ? P_DEC_W2 : P_ENC_W2;
@@ -214,7 +225,7 @@ int run_blocks_planes(const std::vector<Block>& blocks, const BlockBufs& w, cons
     int rc;
     // q | k | v projection (attention.py:48-50), one GEMM with N = 3C: q | k leave as planes [P][rows][2C], the V third
     // as transposed planes [P][B*heads][dk][lpad]; no fp32 copy exists
-    TapGemm gq = make_gemm_p(k.qkv, w.xp, B, L, x3, ACT_NONE, nullptr, 0, nullptr, 0);
+    TapGemm gq = masked(make_gemm_p(k.qkv, w.xp, B, L, x3, ACT_NONE, nullptr, 0, nullptr, 0), zlens);
     planes_out(gq, w.qkp, 2 * C, x3);
     gq.vtp = w.vtp; gq.vt_col0 = 2 * C; gq.vt_dk = C / heads; gq.vt_heads = heads; gq.vt_lpad = lpad;
     if ((rc = dense(gq, FS2_MATH_F16, st, c_qkv))) return rc;
@@ -223,17 +234,18 @@ int run_blocks_planes(const std::vector<Block>& blocks, const BlockBufs& w, cons
       if ((rc = attention_planes(w.qkp, w.vtp, lpad, lens, B, L, C, heads, x3, nullptr, w.ctxp, st))) return rc;
     }
     // x = LN(x + linear_out(ctx)) (attention.py:74, encoder.py:60-62); the LayerNorm also writes the conv-FFN's operand planes
-    if ((rc = dense(make_gemm_p(k.out, w.ctxp, B, L, x3, ACT_NONE, x, C, y, C), FS2_MATH_F16, st, c_out))) return rc;
-    RowNorm r1 = make_norm(k.ln1, y, C, rows, C, x, C);
+    // (per-utterance mode: see run_blocks on the ctx rows past len)
+    if ((rc = dense(masked(make_gemm_p(k.out, w.ctxp, B, L, x3, ACT_NONE, x, C, y, C), zlens), FS2_MATH_F16, st, c_out))) return rc;
+    RowNorm r1 = masked(make_norm(k.ln1, y, C, rows, C, x, C), zlens, L);
     r1.split_out = w.xp; r1.split_lo = x3;
     if ((rc = norm_rows(r1, st))) return rc;
     // conv-FFN: hid = relu(conv_k(x)); x = LN(x + conv_1(hid))  (modules.py:247-248, encoder.py:64-69); the hidden
     // activations exist only as planes
-    TapGemm g1 = make_gemm_p(k.w1, w.xp, B, L, x3, ACT_RELU, nullptr, 0, nullptr, 0);
+    TapGemm g1 = masked(make_gemm_p(k.w1, w.xp, B, L, x3, ACT_RELU, nullptr, 0, nullptr, 0), zlens);
     planes_out(g1, w.hidp, k.w1.N, x3);
     if ((rc = dense(g1, FS2_MATH_F16, st, c_w1))) return rc;
-    if ((rc = dense(make_gemm_p(k.w2, w.hidp, B, L, x3, ACT_NONE, x, C, y, C), FS2_MATH_F16, st, c_w2))) return rc;
-    RowNorm r2 = make_norm(k.ln2, y, C, rows, C, x, C);
+    if ((rc = dense(masked(make_gemm_p(k.w2, w.hidp, B, L, x3, ACT_NONE, x, C, y, C), zlens), FS2_MATH_F16, st, c_w2))) return rc;
+    RowNorm r2 = masked(make_norm(k.ln2, y, C, rows, C, x, C), zlens, L);
     r2.split_out = w.xp; r2.split_lo = x3;                 // planes of the block output: A operand of the next q|k|v / mel projection
     if ((rc = norm_rows(r2, st))) return rc;
   }
@@ -244,7 +256,7 @@ int run_blocks_planes(const std::vector<Block>& blocks, const BlockBufs& w, cons
 // conv stack + scalar head (duration_predictor.py:64-86 / variance_predictor.py:39-60).  xp == nullptr: exact fp32 FMA on
 // the rows x; else error-compensated 3xF16 on the planes xp (the LayerNorms write the next layer's planes into t2p)
 int run_predictor(const Predictor& p, const float* x, const __half* xp, int C, int B, int L, float* t1, float* t2, __half* t2p,
-                  const int64_t* lens, float* head_out, int64_t* dur_out, cudaStream_t st) {
+                  const int64_t* lens, const int64_t* zlens, float* head_out, int64_t* dur_out, cudaStream_t st) {
   const int64_t rows = (int64_t)B * L;
   const float* cur = x; const __half* cur_p = xp; int curC = C;
   for (int i = 0; i < p.layers; ++i) {
@@ -252,8 +264,8 @@ int run_predictor(const Predictor& p, const float* x, const __half* xp, int C, i
     const int N = p.conv[i].N;
     TapGemm g = xp ? make_gemm_p(p.conv[i], cur_p, B, L, true, ACT_RELU, nullptr, 0, t1, N)
                    : make_gemm(p.conv[i], cur, curC, B, L, ACT_RELU, nullptr, 0, t1, N);
-    if ((rc = dense(g, FS2_MATH_FP32, st, P_PRED_GEMM))) return rc;
-    RowNorm r = make_norm(p.ln[i], t1, N, rows, N, xp ? nullptr : t2, N);
+    if ((rc = dense(masked(g, zlens), FS2_MATH_FP32, st, P_PRED_GEMM))) return rc;
+    RowNorm r = masked(make_norm(p.ln[i], t1, N, rows, N, xp ? nullptr : t2, N), zlens, L);
     if (i == p.layers - 1) {  // last layer: only the scalar head leaves the kernel
       r.out = nullptr; r.head_w = p.head_w; r.head_b = p.head_b; r.head_out = head_out; r.dur_out = dur_out;
       r.lens = lens; r.L = L;
@@ -573,7 +585,13 @@ int fs2_workspace_bytes(fs2_handle* h, int B, int Tmax, int Lmax, size_t* out) {
 
 int fs2_encode(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B, int Tmax, float* hs, float* d_log,
                int64_t* d_int, void* ws, size_t ws_bytes, void* stream) {
+  return fs2_encode_ex(h, xs, ilens, B, Tmax, hs, d_log, d_int, ws, ws_bytes, 0, stream);
+}
+
+int fs2_encode_ex(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B, int Tmax, float* hs, float* d_log,
+                  int64_t* d_int, void* ws, size_t ws_bytes, int flags, void* stream) {
   FS2_REQUIRE(h && xs && ilens && hs && ws, "fs2_encode: null argument");
+  FS2_REQUIRE((flags & ~FS2_PER_UTTERANCE) == 0, "fs2_encode_ex: unknown flags 0x%x", flags);
   if (!h->loaded) { set_error("fs2_encode: weights not loaded"); return FS2_ERR_NOT_LOADED; }
   FS2_REQUIRE(Tmax <= h->enc_pe_len, "fs2_encode: Tmax=%d exceeds the positional table (%d rows)", Tmax, h->enc_pe_len);
   FS2_DEVICE_GUARD(h);
@@ -587,14 +605,15 @@ int fs2_encode(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B, in
   // the encoder's output feeds round() in the duration predictor: exact fp32 FMA in FS2_MATH_FP32,
   // error-compensated 3xF16 on the tensor cores in every other mode (never a plain 10-bit-mantissa product)
   const bool planes = c.math_mode != FS2_MATH_FP32;
+  const int64_t* zlens = (flags & FS2_PER_UTTERANCE) ? ilens : nullptr;
   { ProfScope prof_scope(P_EMBED, 0, (planes ? 12.0 : 8.0) * B * Tmax * c.adim, st);
-    if ((rc = embed_posenc(xs, h->emb, c.idim, h->enc_pe, h->enc_alpha, B, Tmax, c.adim, p.w.x, planes ? p.w.xp : nullptr, st))) return rc; }
+    if ((rc = embed_posenc(xs, h->emb, c.idim, h->enc_pe, h->enc_alpha, B, Tmax, c.adim, p.w.x, planes ? p.w.xp : nullptr, zlens, st))) return rc; }
   float* enc_out = nullptr;
-  if (planes) { if ((rc = run_blocks_planes(h->enc, p.w, ilens, B, Tmax, c.adim, c.aheads, true, false, st, &enc_out))) return rc; }
-  else { if ((rc = run_blocks(h->enc, p.w, ilens, B, Tmax, c.adim, c.aheads, FS2_MATH_FP32, false, st, &enc_out))) return rc; }
+  if (planes) { if ((rc = run_blocks_planes(h->enc, p.w, ilens, zlens, B, Tmax, c.adim, c.aheads, true, false, st, &enc_out))) return rc; }
+  else { if ((rc = run_blocks(h->enc, p.w, ilens, zlens, B, Tmax, c.adim, c.aheads, FS2_MATH_FP32, false, st, &enc_out))) return rc; }
   FS2_CUDA_CHECK(cudaMemcpyAsync(hs, enc_out, (size_t)B * Tmax * c.adim * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (d_log || d_int)
-    if ((rc = run_predictor(h->dur, enc_out, planes ? p.w.xp : nullptr, c.adim, B, Tmax, p.t1, p.t2, p.t2p, ilens, d_log, d_int, st))) return rc;
+    if ((rc = run_predictor(h->dur, enc_out, planes ? p.w.xp : nullptr, c.adim, B, Tmax, p.t1, p.t2, p.t2p, ilens, zlens, d_log, d_int, st))) return rc;
   return FS2_OK;
 }
 
@@ -613,8 +632,16 @@ int fs2_length_gather(const float* hs, const int32_t* cum, const int64_t* ilens,
 int fs2_decode(fs2_handle* h, const float* hm, const int64_t* olens, const float* es, const float* ps, int B, int L,
                float* before, float* after, float* e_out, float* p_out, int64_t* e_ids, int64_t* p_ids, void* ws,
                size_t ws_bytes, void* stream) {
+  return fs2_decode_ex(h, hm, olens, es, ps, B, L, before, after, e_out, p_out, e_ids, p_ids, ws, ws_bytes, 0, stream);
+}
+
+int fs2_decode_ex(fs2_handle* h, const float* hm, const int64_t* olens, const float* es, const float* ps, int B, int L,
+                  float* before, float* after, float* e_out, float* p_out, int64_t* e_ids, int64_t* p_ids, void* ws,
+                  size_t ws_bytes, int flags, void* stream) {
   FS2_REQUIRE(h && hm && before && after && e_out && p_out && ws, "fs2_decode: null argument");
   FS2_REQUIRE((es == nullptr) == (ps == nullptr), "fs2_decode: es and ps must both be given or both be NULL");
+  FS2_REQUIRE((flags & ~FS2_PER_UTTERANCE) == 0, "fs2_decode_ex: unknown flags 0x%x", flags);
+  FS2_REQUIRE(!(flags & FS2_PER_UTTERANCE) || olens, "fs2_decode_ex: FS2_PER_UTTERANCE needs olens");
   if (!h->loaded) { set_error("fs2_decode: weights not loaded"); return FS2_ERR_NOT_LOADED; }
   FS2_REQUIRE(L <= h->dec_pe_len, "fs2_decode: L=%d exceeds the positional table (%d rows)", L, h->dec_pe_len);
   FS2_DEVICE_GUARD(h);
@@ -629,6 +656,7 @@ int fs2_decode(fs2_handle* h, const float* hm, const int64_t* olens, const float
   const bool pred_planes = mode != FS2_MATH_FP32;                              // predictors: 3xF16 in every tensor-core mode
   const bool dec_planes = mode == FS2_MATH_3XTF32 || mode == FS2_MATH_F16;     // decoder side on operand planes
   const bool x3 = mode == FS2_MATH_3XTF32;
+  const int64_t* zlens = (flags & FS2_PER_UTTERANCE) ? olens : nullptr;   // hm rows past olens are zero (length_gather)
   int rc;
   // energy / pitch predictors on the length-regulated states (fastspeech.py:195-196,214-216); fp32-class.  hm enters the
   // library as fp32 rows (the LengthRegulator is its own ABI stage), so this is the one operand pre-pass left in a step
@@ -636,32 +664,32 @@ int fs2_decode(fs2_handle* h, const float* hm, const int64_t* olens, const float
     ProfScope prof_scope(P_ROWNORM, 0, 8.0 * rows * c.adim, st);
     if ((rc = split_rows(hm, c.adim, rows, c.adim, p.hmp, st))) return rc;
   }
-  if ((rc = run_predictor(h->energy, hm, pred_planes ? p.hmp : nullptr, c.adim, B, L, p.t1, p.t2, p.t2p, olens, e_out, nullptr, st))) return rc;
-  if ((rc = run_predictor(h->pitch, hm, pred_planes ? p.hmp : nullptr, c.adim, B, L, p.t1, p.t2, p.t2p, olens, p_out, nullptr, st))) return rc;
+  if ((rc = run_predictor(h->energy, hm, pred_planes ? p.hmp : nullptr, c.adim, B, L, p.t1, p.t2, p.t2p, olens, zlens, e_out, nullptr, st))) return rc;
+  if ((rc = run_predictor(h->pitch, hm, pred_planes ? p.hmp : nullptr, c.adim, B, L, p.t1, p.t2, p.t2p, olens, zlens, p_out, nullptr, st))) return rc;
   // hs + pitch_embed(one_hot) + energy_embed(one_hot) (fastspeech.py:218-219); plane families: straight to the decoder
   // input Linear's operand planes
   { ProfScope prof_scope(P_VAR_EMBED, 0, 4.0 * rows * c.adim * 4, st);
   if ((rc = variance_embed_add(hm, es ? es : e_out, ps ? ps : p_out, h->e_bins, h->p_bins, c.n_bins - 1, h->e_tab,
                                h->e_tab_bias, h->p_tab, h->p_tab_bias, rows, c.adim, dec_planes ? nullptr : p.hm2,
-                               dec_planes ? p.hm2p : nullptr, x3, e_ids, p_ids, st))) return rc; }
+                               dec_planes ? p.hm2p : nullptr, x3, e_ids, p_ids, zlens, L, st))) return rc; }
   // decoder input layer: Linear -> LayerNorm -> ReLU -> x + alpha*pe (core/encoder.py:118-125)
   {
     TapGemm g = dec_planes ? make_gemm_p(h->dec_in, p.hm2p, B, L, x3, ACT_NONE, nullptr, 0, p.w.y, c.ddim)
                            : make_gemm(h->dec_in, p.hm2, c.adim, B, L, ACT_NONE, nullptr, 0, p.w.y, c.ddim);
-    if ((rc = dense(g, mode, st, P_DEC_IN))) return rc;
-    RowNorm r = make_norm(h->dec_in_ln, p.w.y, c.ddim, rows, c.ddim, p.w.x, c.ddim);
+    if ((rc = dense(masked(g, zlens), mode, st, P_DEC_IN))) return rc;
+    RowNorm r = masked(make_norm(h->dec_in_ln, p.w.y, c.ddim, rows, c.ddim, p.w.x, c.ddim), zlens, L);
     r.relu_after = 1; r.pe = h->dec_pe; r.alpha = h->dec_alpha; r.L = L;
     if (dec_planes) { r.split_out = p.w.xp; r.split_lo = x3; }    // first block's q|k|v reads the planes
     if ((rc = norm_rows(r, st))) return rc;
   }
   float* dec_out = nullptr;
-  if (dec_planes) { if ((rc = run_blocks_planes(h->dec, p.w, olens, B, L, c.ddim, c.aheads, x3, true, st, &dec_out))) return rc; }
-  else { if ((rc = run_blocks(h->dec, p.w, olens, B, L, c.ddim, c.aheads, mode, true, st, &dec_out))) return rc; }
+  if (dec_planes) { if ((rc = run_blocks_planes(h->dec, p.w, olens, zlens, B, L, c.ddim, c.aheads, x3, true, st, &dec_out))) return rc; }
+  else { if ((rc = run_blocks(h->dec, p.w, olens, zlens, B, L, c.ddim, c.aheads, mode, true, st, &dec_out))) return rc; }
   // mel linear (fastspeech.py:228-230); plane families: from the planes of the last block's output, and the Postnet
   // chain stays in planes until the final residual layer
   {
-    TapGemm g = dec_planes ? make_gemm_p(h->feat_out, p.w.xp, B, L, x3, ACT_NONE, nullptr, 0, before, c.odim)
-                           : make_gemm(h->feat_out, dec_out, c.ddim, B, L, ACT_NONE, nullptr, 0, before, c.odim);
+    TapGemm g = masked(dec_planes ? make_gemm_p(h->feat_out, p.w.xp, B, L, x3, ACT_NONE, nullptr, 0, before, c.odim)
+                                  : make_gemm(h->feat_out, dec_out, c.ddim, B, L, ACT_NONE, nullptr, 0, before, c.odim), zlens);
     if (dec_planes) planes_out(g, p.beforep, c.odim, x3);
     if ((rc = dense(g, mode, st, P_FEAT_OUT))) return rc;
   }
@@ -676,7 +704,7 @@ int fs2_decode(fs2_handle* h, const float* hm, const int64_t* olens, const float
     TapGemm g = dec_planes ? make_gemm_p(h->postnet[i], cur_p, B, L, x3, last ? ACT_NONE : ACT_TANH, last ? before : nullptr, c.odim, last ? dst : nullptr, N)
                            : make_gemm(h->postnet[i], cur, curC, B, L, last ? ACT_NONE : ACT_TANH, last ? before : nullptr, c.odim, dst, N);
     if (dec_planes && !last) planes_out(g, reinterpret_cast<__half*>(dst), N, x3);
-    if ((rc = dense(g, mode, st, P_POSTNET))) return rc;
+    if ((rc = dense(masked(g, zlens), mode, st, P_POSTNET))) return rc;
     cur = dst; cur_p = reinterpret_cast<const __half*>(dst); curC = N;
   }
   return FS2_OK;

@@ -73,6 +73,9 @@ struct TapGemm {
   float a_inv = 1.0f;           // inverse of the A planes' scale (kPlaneInv for planes written by this library)
   __half* outp = nullptr; int ldo_p = 0; bool outp_lo = false;   // result as planes [P][B*L][ldo_p] (lo plane when outp_lo)
   bool precise = false;         // 3xF16 (hi + lo operands) instead of plain f16 on the hi planes
+  // per-utterance mode (FS2_PER_UTTERANCE): rows t >= lens[b] are written as exact zeros (fp32 rows and planes; the
+  // transposed V third is left unwritten there), and the tensor-core kernel skips row tiles that lie wholly past lens[b]
+  const int64_t* lens = nullptr;
 };
 int tap_gemm_fp32(const TapGemm& g, cudaStream_t st);
 int tap_gemm_tf32(const TapGemm& g, cudaStream_t st);   // wgmma + TMA, tf32 on fp32 data (gemm_tc.cu)
@@ -96,22 +99,24 @@ struct RowNorm {
   const float* pe; const float* alpha; int L;  // optional: y += alpha * pe[t], t = row % L
   // optional scalar head (predictors): s = y . head_w + head_b, 0 where t >= lens[b]
   const float* head_w; const float* head_b; float* head_out; int64_t* dur_out;
-  const int64_t* lens;            // optional mask for the head outputs
+  const int64_t* lens;            // optional mask (needs L > 0): rows t >= lens[b] write 0 to the head, out and split_out
   __half* split_out;              // optional operand planes of y (scaled by kPlaneScale): hi at [row][C], lo at [rows + row][C]
   int split_lo;                   // write the lo plane too (3xF16 consumer)
 };
 int row_norm(const RowNorm& r, cudaStream_t st);
 
+// lens (nullable): rows t >= lens[b] are written as zeros (per-utterance mode)
 int embed_posenc(const int64_t* xs, const float* table, int n_sym, const float* pe, const float* alpha, int B, int T,
-                 int C, float* out, __half* planes /*nullable: hi + lo*/, cudaStream_t st);
+                 int C, float* out, __half* planes /*nullable: hi + lo*/, const int64_t* lens, cudaStream_t st);
 
 int bucketize(const float* vals, const float* bins, int n_edges, int64_t n, int64_t* ids, cudaStream_t st);
 int one_hot(const int64_t* ids, int64_t n, int n_bins, float* out, cudaStream_t st);
-// out[r,:] = (hm[r,:] + (p_tab[p_id[r]] + p_bias)) + (e_tab[e_id[r]] + e_bias); ids from values (nullable id outs)
+// out[r,:] = (hm[r,:] + (p_tab[p_id[r]] + p_bias)) + (e_tab[e_id[r]] + e_bias); ids from values (nullable id outs).
+// lens (nullable, rows = B * L): frames t >= lens[b] get zero rows and id -1 (an all-zero one-hot)
 int variance_embed_add(const float* hm, const float* e_val, const float* p_val, const float* e_bins, const float* p_bins,
                        int n_edges, const float* e_tab, const float* e_bias, const float* p_tab, const float* p_bias,
                        int64_t rows, int C, float* out, __half* planes /*nullable: hi (+ lo)*/, int planes_lo, int64_t* e_ids,
-                       int64_t* p_ids, cudaStream_t st);
+                       int64_t* p_ids, const int64_t* lens, int L, cudaStream_t st);
 
 int attention_fp32(const float* qkv, const int64_t* lens, int B, int L, int C, int heads, float* ctx, cudaStream_t st);
 // tensor-core attention: q, k from qkv [B,L,3C]; v from the transposed buffer vt [B*heads, dk, lpad]

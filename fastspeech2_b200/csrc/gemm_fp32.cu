@@ -7,7 +7,8 @@
 // modules.py:283-348) of the reference.  Activations are [B, time, channel] with channels
 // innermost, so a k-tap convolution is `taps` GEMMs that read the same matrix at shifted rows;
 // rows outside [0, L) of the *same utterance* are zero ("same" padding at tensor edges only --
-// padded time steps inside the rectangle are real inputs, SURVEY.md section 8a row a7).
+// padded time steps inside the rectangle are real inputs, SURVEY.md section 8a row a7; in per-utterance mode,
+// TapGemm::lens, the epilogue writes them as zeros instead, so the next convolution's padding is the utterance's own).
 //
 // This is the exact-fp32 family (FMA on CUDA cores): used for the encoder and the predictors
 // in every mode (their outputs feed round()/bucketize(), where tf32 noise would flip integers)
@@ -117,6 +118,7 @@ tap_gemm_fp32_kernel(TapGemm g) {
   for (int i = 0; i < 8; ++i) {
     int m = m0 + (i < 4 ? ty * 4 + i : 64 + ty * 4 + (i - 4));
     if (m >= M) continue;
+    const bool padded = g.lens && m % g.L >= g.lens[m / g.L];   // per-utterance mode: exact zeros past the utterance
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       int n = n0 + h * 64 + tx * 4;
@@ -135,6 +137,7 @@ tap_gemm_fp32_kernel(TapGemm g) {
         float4 rv = __ldg(reinterpret_cast<const float4*>(g.resid + (long)m * g.ldr + n));
         v.x += rv.x; v.y += rv.y; v.z += rv.z; v.w += rv.w;
       }
+      if (padded) v = make_float4(0.f, 0.f, 0.f, 0.f);
       *reinterpret_cast<float4*>(g.out + (long)m * g.ldo + n) = v;
     }
   }

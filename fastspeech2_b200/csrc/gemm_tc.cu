@@ -29,7 +29,9 @@
 // Convolutions tile each utterance separately so the shifted boxes never cross an utterance boundary: floor(L/128) full
 // row tiles per utterance, and the tails (L % 128 rows, in 16-row granules loaded by separate small TMA boxes) of several
 // utterances packed into shared tiles, so no tensor-core rows are spent on padding.  Plain GEMMs (taps == 1) tile the flat
-// [B*L, K] matrix.  Every mbarrier wait is bounded: a pipeline bug traps instead of hanging the GPU.
+// [B*L, K] matrix, except in per-utterance mode (TapGemm::lens), where they tile per utterance as well so that tiles
+// wholly past an utterance's length can be skipped.  Every mbarrier wait is bounded: a pipeline bug traps instead of
+// hanging the GPU.
 // The 3xF16 lo planes are addressed through the same tensor map: plane stride = B*L rows, i.e. utterance index b + B.
 #include <stdlib.h>
 
@@ -59,6 +61,11 @@ struct TcParams {
   // optional: columns >= vt_col0 are the V third of a q|k|v projection and are stored transposed,
   // vt[(b*heads + h)*dk + d][t] with row pitch vt_lpad, for the attention kernel's P.V operand
   float* vt_out; __half* vtp; __half* vtp_lo; int vt_col0, vt_dk, vt_heads, vt_lpad, vt_L;
+  // per-utterance mode (nullable; needs the per-utterance tiling): rows t >= lens[b] are written as exact zeros, and an
+  // ordinary tile with t0 >= lens[b] is dead -- no TMA loads, no MMAs, only the zero stores.  The V third and the q|k
+  // planes of those rows are not needed as zeros (the attention kernels read no key or query row past len), so dead
+  // tiles leave them unwritten and live tiles skip the transposed V stores for them.
+  const int64_t* lens;
 };
 
 template <int BN, bool PRECISE, bool HALF = false>
@@ -116,14 +123,16 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   __syncthreads();
   pdl_wait();                                              // everything above overlapped the previous kernel's tail
 
-  // packed < 0: ordinary tile (utterance b, rows t0 .. t0+127); packed >= 0: index of a packed tail tile
-  auto tile_coords = [&](int tile, int& n0, int& b, int& t0, int& packed) {
+  // packed < 0: ordinary tile (utterance b, rows t0 .. t0+127); packed >= 0: index of a packed tail tile.
+  // Returns true for a dead tile (per-utterance mode: every row lies past lens[b]).
+  auto tile_coords = [&](int tile, int& n0, int& b, int& t0, int& packed) -> bool {
     const int mt = tile / p.n_tiles;
     n0 = (tile - mt * p.n_tiles) * BN;
     packed = -1;
     if (p.tiles_per_utt == 0) { b = 0; t0 = mt * BM; }
     else if (mt < p.full_tiles) { b = mt / p.full; t0 = (mt - b * p.full) * BM; }
     else { packed = mt - p.full_tiles; b = packed * p.upt; t0 = p.full * BM; }
+    return packed < 0 && p.lens != nullptr && t0 >= p.lens[b];
   };
 
   if (warp == 0) {
@@ -133,7 +142,7 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     int n = 0;      // ring position, runs across tiles
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int n0, b, t0, packed;
-      tile_coords(tile, n0, b, t0, packed);
+      if (tile_coords(tile, n0, b, t0, packed)) continue;   // dead tile: the consumers take no stage from the ring either
       int j = 0, kc = 0;                        // tap, K chunk of step s
       for (int s = 0; s < steps; ++s, ++n) {
         const int slot = n % C::STAGES, round = n / C::STAGES;
@@ -172,8 +181,8 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     int n = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int n0, b, t0, packed;
-      tile_coords(tile, n0, b, t0, packed);
-      long m[2]; bool row_ok[2];
+      const int tile_steps = tile_coords(tile, n0, b, t0, packed) ? 0 : steps;
+      long m[2]; bool row_ok[2], row_zero[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int row = r_lo + 8 * h;
@@ -186,10 +195,11 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           ok = u < p.upt && bb < p.B && t < p.L;
         }
         m[h] = (long)bb * p.L + t; row_ok[h] = ok;
+        row_zero[h] = ok && p.lens != nullptr && t >= p.lens[bb];
         if (has_res && ok) prefetch_l2(resid + m[h] * ldr + n0);   // residual rows -> L2 while the main loop runs
       }
       int prev = -1;
-      for (int s = 0; s < steps; ++s, ++n) {
+      for (int s = 0; s < tile_steps; ++s, ++n) {
         const int slot = n % C::STAGES, round = n / C::STAGES;
         const uint32_t base = smem_u32(tiles + (size_t)slot * C::STAGE_BYTES);
         const uint64_t a_hi = make_sw128_kmajor_desc(base + cg * (A_BYTES / 2)), b_hi = make_sw128_kmajor_desc(base + C::B_HI);
@@ -215,7 +225,7 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       wgmma_wait<0>();
       pin_regs<BN / 2>(d);
       if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
-      if (steps == 0) {
+      if (tile_steps == 0) {
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
       }
@@ -224,7 +234,7 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       const bool to_vt = (p.vt_out != nullptr || p.vtp != nullptr) && n0 >= p.vt_col0;   // tile-uniform (tile widths divide the V third)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        if (!row_ok[h]) continue;
+        if (!row_ok[h] || (to_vt && row_zero[h])) continue;
         const long mm = m[h];
 #pragma unroll
         for (int jj = 0; jj < BN / 8; ++jj) {
@@ -254,6 +264,7 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
             const float2 r = __ldg(reinterpret_cast<const float2*>(resid + mm * ldr + col));
             v0 += r.x; v1 += r.y;
           }
+          if (row_zero[h]) { v0 = 0.f; v1 = 0.f; }
           if (HALF && p.outp != nullptr) {       // operand planes of the next contraction
             const long off = mm * p.ldo_p + col;
             if (p.outp_lo != nullptr) {
@@ -310,12 +321,15 @@ int launch(const TapGemm& g, cudaStream_t st) {
   p.vt_out = HALF ? nullptr : g.vt_out; p.vtp = HALF ? g.vtp : nullptr;
   p.vtp_lo = (HALF && g.vtp && g.outp_lo) ? g.vtp + (long)g.B * g.vt_heads * g.vt_dk * g.vt_lpad : nullptr;
   p.vt_col0 = g.vt_col0; p.vt_dk = g.vt_dk; p.vt_heads = g.vt_heads; p.vt_lpad = g.vt_lpad; p.vt_L = g.L;
+  p.lens = g.lens;
   CUtensorMap ma, mb, mb_lo, ma16;
   const int esz = HALF ? 2 : 4;
   constexpr int planes = HALF && PRECISE ? 2 : 1;          // 3xF16: [hi plane][lo plane], each [B*L][K] fp16
   const void* xa = HALF ? (const void*)g.xp : (const void*)g.x;
   const uint64_t row_bytes = HALF ? (uint64_t)g.K * 2 : (uint64_t)g.ldx * 4;
-  if (g.taps == 1) {  // flat [B*L, K]
+  // with lens, plain GEMMs take the per-utterance tiling too, so that tiles past an utterance's length are dead; a row's
+  // K loop is the same in either tiling, so its result does not depend on it
+  if (g.taps == 1 && g.lens == nullptr) {  // flat [B*L, K]
     const uint64_t M = (uint64_t)g.B * g.L;
     p.L = (int)M; p.tiles_per_utt = 0;
     p.m_tiles = (int)((M + BM - 1) / BM);

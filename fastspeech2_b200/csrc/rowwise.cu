@@ -13,13 +13,14 @@ constexpr int ROWS_PER_CTA = 8;  // 8 warps
 template <int NV>  // float4 per lane
 __global__ void embed_posenc_kernel(const int64_t* __restrict__ xs, const float* __restrict__ table, int n_sym,
                                     const float* __restrict__ pe, const float* __restrict__ alpha, long rows, int T,
-                                    float* __restrict__ out, __half* __restrict__ planes) {
+                                    float* __restrict__ out, __half* __restrict__ planes, const int64_t* __restrict__ lens) {
   pdl_trigger(); pdl_wait();
   const int C = NV * 128;
   long row = (long)blockIdx.x * ROWS_PER_CTA + (threadIdx.x >> 5);
   if (row >= rows) return;
   int lane = threadIdx.x & 31;
   int t = (int)(row % T);
+  const bool padded = lens && t >= lens[row / T];
   long id = xs[row];
   if (id < 0 || id >= n_sym) id = 0;  // out-of-range ids behave like padding instead of faulting
   const float a = __ldg(alpha);
@@ -31,6 +32,7 @@ __global__ void embed_posenc_kernel(const int64_t* __restrict__ xs, const float*
     float4 o;  // x + (alpha * pe): two roundings like the reference's mul then add
     o.x = __fadd_rn(e.x, __fmul_rn(a, p.x)); o.y = __fadd_rn(e.y, __fmul_rn(a, p.y));
     o.z = __fadd_rn(e.z, __fmul_rn(a, p.z)); o.w = __fadd_rn(e.w, __fmul_rn(a, p.w));
+    if (padded) o = make_float4(0.f, 0.f, 0.f, 0.f);
     *reinterpret_cast<float4*>(out + row * C + c) = o;
     if (planes) {   // operand planes of the first q|k|v projection (3xF16)
       uint2 hv, lv;
@@ -73,6 +75,7 @@ __global__ void row_norm_kernel(RowNorm r) {
   const float rstd = 1.0f / sqrtf(warp_sum(ss) * (1.0f / C) + r.eps);
   int t = r.L > 0 ? (int)(row % r.L) : 0;
   long bidx = r.L > 0 ? row / r.L : 0;
+  const bool padded = r.lens && (long)t >= r.lens[bidx];
   const float alpha = r.pe ? __ldg(r.alpha) : 0.f;
   float dot = 0.f;
 #pragma unroll
@@ -93,6 +96,7 @@ __global__ void row_norm_kernel(RowNorm r) {
       float4 w = __ldg(reinterpret_cast<const float4*>(r.head_w + c));
       dot += (y.x * w.x + y.y * w.y) + (y.z * w.z + y.w * w.w);
     }
+    if (padded) y = make_float4(0.f, 0.f, 0.f, 0.f);
     if (r.out) *reinterpret_cast<float4*>(r.out + row * r.ldo + c) = y;
     if (r.split_out) {   // operand planes of the next contraction: hi = rn(s y), lo = rn(s y - hi), 8-byte stores
       uint2 hv, lv;
@@ -104,7 +108,6 @@ __global__ void row_norm_kernel(RowNorm r) {
   if (r.head_w) {
     dot = warp_sum(dot) + __ldg(r.head_b);
     if (lane == 0) {
-      bool padded = r.lens && (long)t >= r.lens[bidx];
       if (r.head_out) r.head_out[row] = padded ? 0.f : dot;
       if (r.dur_out) {
         // clamp(round(exp(x) - 1), min=0).long(), round = half to even (duration_predictor.py:77-81)
@@ -146,17 +149,19 @@ __global__ void variance_embed_add_kernel(const float* __restrict__ hm, const fl
                                           const float* __restrict__ e_bias, const float* __restrict__ p_tab,
                                           const float* __restrict__ p_bias, int64_t rows, float* __restrict__ out,
                                           __half* __restrict__ planes, int planes_lo,
-                                          int64_t* __restrict__ e_ids, int64_t* __restrict__ p_ids) {
+                                          int64_t* __restrict__ e_ids, int64_t* __restrict__ p_ids,
+                                          const int64_t* __restrict__ lens, int L) {
   pdl_trigger(); pdl_wait();
   const int C = NV * 128;
   int64_t row = (int64_t)blockIdx.x * ROWS_PER_CTA + (threadIdx.x >> 5);
   if (row >= rows) return;
   int lane = threadIdx.x & 31;
+  const bool padded = lens && row % L >= lens[row / L];
   int ide = bucket_of(__ldg(e_val + row), e_bins, n_edges);
   int idp = bucket_of(__ldg(p_val + row), p_bins, n_edges);
   if (lane == 0) {
-    if (e_ids) e_ids[row] = ide;
-    if (p_ids) p_ids[row] = idp;
+    if (e_ids) e_ids[row] = padded ? -1 : ide;
+    if (p_ids) p_ids[row] = padded ? -1 : idp;
   }
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
@@ -171,6 +176,7 @@ __global__ void variance_embed_add_kernel(const float* __restrict__ hm, const fl
     o.y = __fadd_rn(__fadd_rn(h.y, __fadd_rn(pw.y, pb.y)), __fadd_rn(ew.y, eb.y));
     o.z = __fadd_rn(__fadd_rn(h.z, __fadd_rn(pw.z, pb.z)), __fadd_rn(ew.z, eb.z));
     o.w = __fadd_rn(__fadd_rn(h.w, __fadd_rn(pw.w, pb.w)), __fadd_rn(ew.w, eb.w));
+    if (padded) o = make_float4(0.f, 0.f, 0.f, 0.f);
     if (out) *reinterpret_cast<float4*>(out + row * C + c) = o;
     if (planes) {   // operand planes of the decoder input Linear
       uint2 hv, lv;
@@ -280,12 +286,12 @@ inline int grid_for(long n, int block, int cap = 132 * 8) {
 }  // namespace
 
 int embed_posenc(const int64_t* xs, const float* table, int n_sym, const float* pe, const float* alpha, int B, int T,
-                 int C, float* out, __half* planes, cudaStream_t st) {
+                 int C, float* out, __half* planes, const int64_t* lens, cudaStream_t st) {
   long rows = (long)B * T;
   if (rows == 0) return FS2_OK;
   int grid = (int)((rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA);
-  if (C == 256) { FS2_CUDA_CHECK(launch_pdl(embed_posenc_kernel<2>, dim3(grid), dim3(256), 0, st, xs, table, n_sym, pe, alpha, rows, T, out, planes)); }
-  else if (C == 384) { FS2_CUDA_CHECK(launch_pdl(embed_posenc_kernel<3>, dim3(grid), dim3(256), 0, st, xs, table, n_sym, pe, alpha, rows, T, out, planes)); }
+  if (C == 256) { FS2_CUDA_CHECK(launch_pdl(embed_posenc_kernel<2>, dim3(grid), dim3(256), 0, st, xs, table, n_sym, pe, alpha, rows, T, out, planes, lens)); }
+  else if (C == 384) { FS2_CUDA_CHECK(launch_pdl(embed_posenc_kernel<3>, dim3(grid), dim3(256), 0, st, xs, table, n_sym, pe, alpha, rows, T, out, planes, lens)); }
   else { set_error("embed_posenc: C=%d unsupported (256 or 384)", C); return FS2_ERR_INVALID; }
   FS2_LAUNCH_CHECK();
   return FS2_OK;
@@ -295,6 +301,7 @@ int row_norm(const RowNorm& r, cudaStream_t st) {
   if (r.rows == 0) return FS2_OK;
   FS2_REQUIRE(r.ldx % 4 == 0 && (!r.out || r.ldo % 4 == 0) && (!r.resid || r.ldr % 4 == 0), "row_norm: strides must be 16-byte multiples");
   FS2_REQUIRE(!r.split_out || (reinterpret_cast<uintptr_t>(r.split_out) & 7) == 0, "row_norm: operand planes must be 8-byte aligned");
+  FS2_REQUIRE(!r.lens || r.L > 0, "row_norm: lens needs L > 0");
   int grid = (int)((r.rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA);
   if (r.C == 256) { FS2_CUDA_CHECK(launch_pdl(row_norm_kernel<2>, dim3(grid), dim3(256), 0, st, r)); }
   else if (r.C == 384) { FS2_CUDA_CHECK(launch_pdl(row_norm_kernel<3>, dim3(grid), dim3(256), 0, st, r)); }
@@ -321,15 +328,16 @@ int one_hot(const int64_t* ids, int64_t n, int n_bins, float* out, cudaStream_t 
 int variance_embed_add(const float* hm, const float* e_val, const float* p_val, const float* e_bins, const float* p_bins,
                        int n_edges, const float* e_tab, const float* e_bias, const float* p_tab, const float* p_bias,
                        int64_t rows, int C, float* out, __half* planes, int planes_lo, int64_t* e_ids, int64_t* p_ids,
-                       cudaStream_t st) {
+                       const int64_t* lens, int L, cudaStream_t st) {
   if (rows == 0) return FS2_OK;
+  FS2_REQUIRE(!lens || L > 0, "variance_embed_add: lens needs L > 0");
   int grid = (int)((rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA);
   if (C == 256) {
     FS2_CUDA_CHECK(launch_pdl(variance_embed_add_kernel<2>, dim3(grid), dim3(256), 0, st, hm, e_val, p_val, e_bins, p_bins, n_edges, e_tab, e_bias, p_tab,
-                              p_bias, rows, out, planes, planes_lo, e_ids, p_ids));
+                              p_bias, rows, out, planes, planes_lo, e_ids, p_ids, lens, L));
   } else if (C == 384) {
     FS2_CUDA_CHECK(launch_pdl(variance_embed_add_kernel<3>, dim3(grid), dim3(256), 0, st, hm, e_val, p_val, e_bins, p_bins, n_edges, e_tab, e_bias, p_tab,
-                              p_bias, rows, out, planes, planes_lo, e_ids, p_ids));
+                              p_bias, rows, out, planes, planes_lo, e_ids, p_ids, lens, L));
   }
   else { set_error("variance_embed_add: C=%d unsupported", C); return FS2_ERR_INVALID; }
   FS2_LAUNCH_CHECK();

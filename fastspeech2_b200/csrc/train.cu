@@ -674,7 +674,7 @@ int fs2_embed_backward(const int64_t* xs, const float* dy, const float* pe, int 
 int fs2_embed_posenc(const int64_t* xs, const float* table, int n_sym, const float* pe, const float* alpha, int B, int T, int C, float* out,
                      void* stream) {
   FS2_REQUIRE(xs && table && pe && alpha && out, "fs2_embed_posenc: null argument");
-  return embed_posenc(xs, table, n_sym, pe, alpha, B, T, C, out, nullptr, (cudaStream_t)stream);
+  return embed_posenc(xs, table, n_sym, pe, alpha, B, T, C, out, nullptr, nullptr, (cudaStream_t)stream);
 }
 int fs2_posenc_add(const float* x, const float* pe, const float* alpha, int B, int T, int C, float* y, void* stream) {
   FS2_REQUIRE(x && pe && alpha && y, "fs2_posenc_add: null argument");

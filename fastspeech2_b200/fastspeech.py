@@ -375,16 +375,27 @@ class FeedForwardTransformer(nn.Module):
     # -- the path ----------------------------------------------------------------------------
     def _forward(self, xs: torch.Tensor, ilens: torch.Tensor, olens: torch.Tensor = None, ds: torch.Tensor = None,
                  es: torch.Tensor = None, ps: torch.Tensor = None, is_inference: bool = False,
-                 _one_hot: bool = True, _defer_check: Optional[list] = None, _after_out: Optional[torch.Tensor] = None) -> Sequence[torch.Tensor]:
+                 _one_hot: bool = True, _defer_check: Optional[list] = None, _after_out: Optional[torch.Tensor] = None,
+                 per_utterance: bool = False, _olens_out: Optional[list] = None) -> Sequence[torch.Tensor]:
+        """The reference's `_forward` (fastspeech.py:169-243).  `per_utterance=True` (not in the reference) makes every
+        utterance's result independent of its batch mates: utterance b is bit-identical to the B = 1 call on
+        `xs[b:b+1, :ilens[b]]` (teacher-forced: with its es / ps sliced to olens[b]), in inference the decoder is masked by
+        the predicted lengths, every padded position of every returned tensor is exactly 0 (all-zero one-hot rows), and
+        row tiles wholly in padding are skipped.  It needs 1 <= ilens[b] <= Tmax, and in teacher-forced mode
+        olens[b] == sum(ds[b, :ilens[b]]).  `_olens_out` (list): receives the olens the decoder ran with."""
         # the handle-less ABI stages (LengthRegulator, losses, ...) run on the CURRENT device like any CUDA library call:
         # select the device the data lives on for the whole call, leave the caller's current device untouched
         if xs.is_cuda and torch.cuda.current_device() != (xs.device.index or 0):
             with torch.cuda.device(xs.device):
-                return self._forward(xs, ilens, olens, ds, es, ps, is_inference, _one_hot, _defer_check, _after_out)
+                return self._forward(xs, ilens, olens, ds, es, ps, is_inference, _one_hot, _defer_check, _after_out,
+                                     per_utterance, _olens_out)
+        if per_utterance:
+            self._check_ilens(xs, ilens)
         h = self._ready(xs)
         lib = _lib.load()
         dev, d = xs.device, self.dims
         st = _lib.stream_ptr(dev)
+        flags = _lib.FS2_PER_UTTERANCE if per_utterance else 0
         if xs.dim() != 2:
             raise ValueError("xs must be [B, Tmax]")
         B, T = xs.shape
@@ -411,23 +422,30 @@ class FeedForwardTransformer(nn.Module):
         hs = torch.empty((B, T, d.adim), **f32)
         d_log = None if is_inference else torch.empty((B, T), **f32)
         d_int = torch.empty((B, T), dtype=torch.int64, device=dev) if is_inference else None
-        _lib.check(lib.fs2_encode(h, _lib.ptr(xs), _lib.ptr(ilens), B, T, _lib.ptr(hs), _lib.ptr(d_log), _lib.ptr(d_int),
-                                  _lib.ptr(ws), ws.numel(), st), "fs2_encode")
+        _lib.check(lib.fs2_encode_ex(h, _lib.ptr(xs), _lib.ptr(ilens), B, T, _lib.ptr(hs), _lib.ptr(d_log), _lib.ptr(d_int),
+                                     _lib.ptr(ws), ws.numel(), flags, st), "fs2_encode_ex")
 
         # stage 2: length regulator
         cum, olens_lr, stats, _ = _lr.plan(hs, d_int if is_inference else ds, ilens, 1.0)
         if is_inference:
-            lmax, n_neg = stats.tolist()  # the single host sync of inference: sizes the mel buffers
+            if per_utterance:       # the ilens range rides along in the same transfer
+                lmax, n_neg, imin, imax = torch.cat([stats, torch.stack([ilens.min(), ilens.max()])]).tolist()
+                self._check_ilens_range(imin, imax, T)
+            else:
+                lmax, n_neg = stats.tolist()  # the single host sync of inference: sizes the mel buffers
             L = int(lmax)
             if L <= 0:
                 raise RuntimeError("inference produced zero frames")
             if L > self.decoder.embed[-1].pe.shape[1]:
                 self._extend_pe(self.decoder, L)
                 h = self._ready(xs)
-            olens_dec = None  # decoder unmasked, fastspeech.py:221-224
+            # reference semantics: decoder unmasked, fastspeech.py:221-224; per-utterance: masked by the planned lengths
+            olens_dec = olens_lr if per_utterance else None
         else:
             L = L_known
             olens_dec = olens.to(device=dev, dtype=torch.int64).contiguous()
+        if _olens_out is not None:
+            _olens_out.append(olens_lr if is_inference else olens_dec)
         hm = _lr.gather(hs, cum, ilens, L)
 
         # stage 3: variance adaptor + decoder + postnet
@@ -445,9 +463,9 @@ class FeedForwardTransformer(nn.Module):
         p_ids = torch.empty((B, L), dtype=torch.int64, device=dev) if want_ids else None
         es_c = None if is_inference else es.to(**f32).contiguous()
         ps_c = None if is_inference else ps.to(**f32).contiguous()
-        _lib.check(lib.fs2_decode(h, _lib.ptr(hm), _lib.ptr(olens_dec), _lib.ptr(es_c), _lib.ptr(ps_c), B, L, _lib.ptr(before),
-                                  _lib.ptr(after), _lib.ptr(e_out), _lib.ptr(p_out), _lib.ptr(e_ids), _lib.ptr(p_ids),
-                                  _lib.ptr(ws), ws.numel(), st), "fs2_decode")
+        _lib.check(lib.fs2_decode_ex(h, _lib.ptr(hm), _lib.ptr(olens_dec), _lib.ptr(es_c), _lib.ptr(ps_c), B, L, _lib.ptr(before),
+                                     _lib.ptr(after), _lib.ptr(e_out), _lib.ptr(p_out), _lib.ptr(e_ids), _lib.ptr(p_ids),
+                                     _lib.ptr(ws), ws.numel(), flags, st), "fs2_decode_ex")
 
         if is_inference:
             if not _one_hot:
@@ -464,8 +482,31 @@ class FeedForwardTransformer(nn.Module):
         if _defer_check is not None:          # CUDA-graph capture: no host read here, the caller validates after replay
             _defer_check.append((chk_dev, T, L))
             return before, after, d_log, e_out, p_out
-        self._validate_lengths(chk_dev.tolist(), T, L)
+        if per_utterance:   # + the ilens range and olens == sum(ds) (the zero rows of hm end at sum(ds)), same transfer
+            chk = torch.cat([chk_dev, torch.stack([ilens.min(), (olens_dec != olens_lr).sum()])]).tolist()
+            self._check_ilens_range(chk[4], chk[2], T)
+            if chk[5]:
+                raise ValueError(f"per_utterance: olens differs from sum(ds) in {chk[5]} utterance(s)")
+        else:
+            chk = chk_dev.tolist()
+        self._validate_lengths(chk[:4], T, L)
         return before, after, d_log, e_out, p_out
+
+    @staticmethod
+    def _check_ilens_range(imin: int, imax: int, T: int) -> None:
+        if imin < 1 or imax > T:
+            raise ValueError(f"per_utterance: every ilens[b] must lie in [1, Tmax={T}] (got min {imin}, max {imax})")
+
+    @classmethod
+    def _check_ilens(cls, xs: torch.Tensor, ilens: torch.Tensor) -> None:
+        """Argument checks of the per-utterance mode that need no device: shapes, and the ilens range when ilens is on
+        the host (lengths on the device are checked in the call's single host read)."""
+        if xs.dim() != 2:
+            raise ValueError("xs must be [B, Tmax]")
+        if not torch.is_tensor(ilens) or ilens.dim() != 1 or ilens.shape[0] != xs.shape[0] or xs.shape[0] == 0:
+            raise ValueError(f"ilens must be a non-empty [B] tensor matching xs {tuple(xs.shape)}")
+        if not ilens.is_cuda:
+            cls._check_ilens_range(int(ilens.min()), int(ilens.max()), int(xs.shape[1]))
 
     @staticmethod
     def _validate_lengths(chk, T: int, L: int) -> None:
@@ -524,6 +565,15 @@ class FeedForwardTransformer(nn.Module):
         ilens = torch.tensor([x.shape[0]], dtype=torch.long, device=x.device)
         _, outs, _, _, _ = self._forward(x.unsqueeze(0), ilens, is_inference=True, _one_hot=False)
         return outs[0]
+
+    def synthesize(self, xs: torch.Tensor, ilens: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Per-utterance batched inference (not in the reference): xs [B, Tmax] int64 (0 = pad), ilens [B] with
+        1 <= ilens[b] <= Tmax -> (mels [B, Lmax, odim], olens [B] int64, durations [B, Tmax] int64), all on the device.
+        durations[b], olens[b] and mels[b, :olens[b]] are bit-identical to what `inference(xs[b, :ilens[b]])` computes,
+        whatever else is in the batch; mels[b, olens[b]:] and durations[b, ilens[b]:] are 0.  One host read per call."""
+        got: list = []
+        _, after, dur, _, _ = self._forward(xs, ilens, is_inference=True, _one_hot=False, per_utterance=True, _olens_out=got)
+        return after, got[0], dur
 
 
 class GraphedForward:

@@ -10,6 +10,7 @@ buffer (+ their keys and shapes) and its `forward` is ONE call of the custom ope
     export_torchscript(model, "fs2.pt")                              # export_torchscript.py:46-48
     served = torch.jit.load("fs2.pt").cuda()                         # any process that imported this module
     mel = served(torch.tensor(ids).cuda())                           # [L, odim]; batched: served.batch(xs, ilens)
+    mels, olens = served.synthesize(xs, ilens)                       # batched, each utterance independent of its batch mates
 
 The operator is registered through `torch.library` (schema + CUDA implementation); there is no CPU implementation -- a
 CPU tensor fails loudly like the rest of the path.
@@ -27,6 +28,7 @@ from .hparams import load_hp
 _LIB = torch.library.Library("fs2_b200", "DEF")
 _LIB.define("inference(Tensor blob, str[] keys, int[] ranks, int[] dims, str precision, Tensor x) -> Tensor")
 _LIB.define("inference_batch(Tensor blob, str[] keys, int[] ranks, int[] dims, str precision, Tensor xs, Tensor ilens) -> (Tensor, Tensor)")
+_LIB.define("synthesize_batch(Tensor blob, str[] keys, int[] ranks, int[] dims, str precision, Tensor xs, Tensor ilens) -> (Tensor, Tensor)")
 
 # one packed model per (device, identity of the checkpoint blob): the op is functional from TorchScript's point of view,
 # the cache only avoids re-packing the checkpoint on every call
@@ -84,14 +86,22 @@ def _inference_batch(blob, keys, ranks, dims, precision, xs, ilens):
     return after, d.sum(dim=1)
 
 
+def _synthesize_batch(blob, keys, ranks, dims, precision, xs, ilens):
+    with torch.no_grad():
+        mels, olens, _ = _model_for(blob, keys, ranks, dims, precision).synthesize(xs, ilens)
+    return mels, olens
+
+
 def _no_cpu(*a, **k):
     raise RuntimeError("fs2_b200 operators run on CUDA tensors only (the H100 path has no CPU fallback)")
 
 
 _LIB.impl("inference", _inference, "CUDA")
 _LIB.impl("inference_batch", _inference_batch, "CUDA")
+_LIB.impl("synthesize_batch", _synthesize_batch, "CUDA")
 _LIB.impl("inference", _no_cpu, "CPU")
 _LIB.impl("inference_batch", _no_cpu, "CPU")
+_LIB.impl("synthesize_batch", _no_cpu, "CPU")
 
 
 class ScriptedFastSpeech2(torch.nn.Module):
@@ -114,6 +124,13 @@ class ScriptedFastSpeech2(torch.nn.Module):
     def batch(self, xs: torch.Tensor, ilens: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
         """xs [B,T] int64 (0 = pad), ilens [B] -> (mels [B,Lmax,odim], olens [B])."""
         return torch.ops.fs2_b200.inference_batch(self.blob, self.keys, self.ranks, self.dims, self.precision, xs, ilens)
+
+    @torch.jit.export
+    def synthesize(self, xs: torch.Tensor, ilens: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Per-utterance batch for dynamic batching: xs [B,T] int64 (0 = pad), ilens [B] -> (mels [B,Lmax,odim], olens [B]).
+        Each utterance's mels are bit-identical to forward() on it alone, whatever else is in the batch; padded frames
+        are 0 (FeedForwardTransformer.synthesize)."""
+        return torch.ops.fs2_b200.synthesize_batch(self.blob, self.keys, self.ranks, self.dims, self.precision, xs, ilens)
 
 
 def scripted(model: FeedForwardTransformer, precision: Optional[str] = None) -> torch.jit.ScriptModule:

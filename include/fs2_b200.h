@@ -128,6 +128,19 @@ int fs2_profile_read(fs2_handle* h, double* ms, int64_t* launches, double* flop,
 int fs2_encode(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B, int Tmax, float* hs, float* d_log,
                int64_t* d_int, void* ws, size_t ws_bytes, void* stream);
 
+/* Per-utterance batching (flags of fs2_encode_ex / fs2_decode_ex).  Without it a batch reproduces the reference's
+ * semantics, under which an utterance's result depends on its batch mates: the convolutions read the padded positions
+ * (non-zero after the first block) and inference runs the decoder unmasked.  With it, every tensor a convolution reads
+ * and every output holds exact zeros at rows t >= len_b (len = ilens in the encoder, olens in the decoder), so utterance b
+ * of a batch is bit-identical to the same utterance run alone (B = 1, Tmax = ilens[b], L = olens[b]) in every math mode,
+ * and row tiles wholly in padding are skipped. */
+#define FS2_PER_UTTERANCE 1
+
+/* fs2_encode with flags (0 or FS2_PER_UTTERANCE); fs2_encode is the flags = 0 case.  With FS2_PER_UTTERANCE,
+ * hs[b, t >= ilens[b], :] == 0 (d_log / d_int are 0 there in either mode). */
+int fs2_encode_ex(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B, int Tmax, float* hs, float* d_log,
+                  int64_t* d_int, void* ws, size_t ws_bytes, int flags, void* stream);
+
 /* ---- stage 2: LengthRegulator (needs no handle) ---------------------------------------- */
 /* core/duration_modeling/length_regulator.py:38-95 + utils/util.py:91-104.
  * Plan: per utterance, optionally scale by alpha (round half to even, :58-59), truncate to
@@ -155,6 +168,14 @@ int fs2_length_gather(const float* hs, const int32_t* cum, const int64_t* ilens,
 int fs2_decode(fs2_handle* h, const float* hm, const int64_t* olens, const float* es, const float* ps, int B, int L,
                float* before, float* after, float* e_out, float* p_out, int64_t* e_ids, int64_t* p_ids, void* ws,
                size_t ws_bytes, void* stream);
+
+/* fs2_decode with flags (0 or FS2_PER_UTTERANCE); fs2_decode is the flags = 0 case.  With FS2_PER_UTTERANCE, olens is
+ * required also when es / ps are NULL (predict-and-bucketize: pass the lengths of the length plan), hm must be zero at
+ * rows t >= olens[b] (fs2_length_gather writes it so), and at those rows before / after / e_out / p_out are 0 and
+ * e_ids / p_ids are -1 (an all-zero one-hot). */
+int fs2_decode_ex(fs2_handle* h, const float* hm, const int64_t* olens, const float* es, const float* ps, int B, int L,
+                  float* before, float* after, float* e_out, float* p_out, int64_t* e_ids, int64_t* p_ids, void* ws,
+                  size_t ws_bytes, int flags, void* stream);
 
 /* ---- stage 4: masked losses (fastspeech.py:277-333) ------------------------------------- */
 /* out7 (device, f32): l1, before, after, duration, energy, pitch, total -- the order of
