@@ -254,9 +254,11 @@ int run_blocks_planes(const std::vector<Block>& blocks, const BlockBufs& w, cons
 }
 
 // conv stack + scalar head (duration_predictor.py:64-86 / variance_predictor.py:39-60).  xp == nullptr: exact fp32 FMA on
-// the rows x; else error-compensated 3xF16 on the planes xp (the LayerNorms write the next layer's planes into t2p)
+// the rows x; else error-compensated 3xF16 on the planes xp (the LayerNorms write the next layer's planes into t2p).
+// head_scale (nullable, [B*L]): the head's value times a per-row factor, one fp32 rounding (prosody control)
 int run_predictor(const Predictor& p, const float* x, const __half* xp, int C, int B, int L, float* t1, float* t2, __half* t2p,
-                  const int64_t* lens, const int64_t* zlens, float* head_out, int64_t* dur_out, cudaStream_t st) {
+                  const int64_t* lens, const int64_t* zlens, float* head_out, int64_t* dur_out, const float* head_scale,
+                  cudaStream_t st) {
   const int64_t rows = (int64_t)B * L;
   const float* cur = x; const __half* cur_p = xp; int curC = C;
   for (int i = 0; i < p.layers; ++i) {
@@ -268,6 +270,7 @@ int run_predictor(const Predictor& p, const float* x, const __half* xp, int C, i
     RowNorm r = masked(make_norm(p.ln[i], t1, N, rows, N, xp ? nullptr : t2, N), zlens, L);
     if (i == p.layers - 1) {  // last layer: only the scalar head leaves the kernel
       r.out = nullptr; r.head_w = p.head_w; r.head_b = p.head_b; r.head_out = head_out; r.dur_out = dur_out;
+      r.head_scale = head_scale;
       r.lens = lens; r.L = L;
     } else if (xp) {
       r.split_out = t2p; r.split_lo = 1;
@@ -613,20 +616,30 @@ int fs2_encode_ex(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B,
   else { if ((rc = run_blocks(h->enc, p.w, ilens, zlens, B, Tmax, c.adim, c.aheads, FS2_MATH_FP32, false, st, &enc_out))) return rc; }
   FS2_CUDA_CHECK(cudaMemcpyAsync(hs, enc_out, (size_t)B * Tmax * c.adim * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (d_log || d_int)
-    if ((rc = run_predictor(h->dur, enc_out, planes ? p.w.xp : nullptr, c.adim, B, Tmax, p.t1, p.t2, p.t2p, ilens, zlens, d_log, d_int, st))) return rc;
+    if ((rc = run_predictor(h->dur, enc_out, planes ? p.w.xp : nullptr, c.adim, B, Tmax, p.t1, p.t2, p.t2p, ilens, zlens, d_log, d_int, nullptr, st))) return rc;
   return FS2_OK;
 }
 
 int fs2_length_plan(void* ds, int ds_dtype, const int64_t* ilens, float alpha, int B, int Tmax, int mutate_ds,
                     int32_t* cum, int64_t* olens, int64_t* stats, void* stream) {
+  return fs2_length_plan_ex(ds, ds_dtype, ilens, alpha, nullptr, B, Tmax, mutate_ds, cum, olens, stats, nullptr, stream);
+}
+
+int fs2_length_plan_ex(void* ds, int ds_dtype, const int64_t* ilens, float alpha, const float* alpha_v, int B, int Tmax,
+                       int mutate_ds, int32_t* cum, int64_t* olens, int64_t* stats, int64_t* d_used, void* stream) {
   FS2_REQUIRE(ds && ilens && cum && olens && stats, "fs2_length_plan: null argument");
-  return length_plan(ds, ds_dtype, ilens, alpha, B, Tmax, mutate_ds, cum, olens, stats, (cudaStream_t)stream);
+  return length_plan(ds, ds_dtype, ilens, alpha, alpha_v, B, Tmax, mutate_ds, cum, olens, stats, d_used, (cudaStream_t)stream);
 }
 
 int fs2_length_gather(const float* hs, const int32_t* cum, const int64_t* ilens, int B, int Tmax, int C, float* out,
                       int Lcap, void* stream) {
+  return fs2_length_gather_ex(hs, cum, ilens, B, Tmax, C, out, Lcap, nullptr, nullptr, stream);
+}
+
+int fs2_length_gather_ex(const float* hs, const int32_t* cum, const int64_t* ilens, int B, int Tmax, int C, float* out,
+                         int Lcap, const float* fac_in, float* fac_out, void* stream) {
   FS2_REQUIRE(hs && cum && ilens && (out || Lcap == 0), "fs2_length_gather: null argument");
-  return length_gather(hs, cum, ilens, B, Tmax, C, out, Lcap, (cudaStream_t)stream);
+  return length_gather(hs, cum, ilens, B, Tmax, C, out, Lcap, fac_in, fac_out, (cudaStream_t)stream);
 }
 
 int fs2_decode(fs2_handle* h, const float* hm, const int64_t* olens, const float* es, const float* ps, int B, int L,
@@ -638,8 +651,16 @@ int fs2_decode(fs2_handle* h, const float* hm, const int64_t* olens, const float
 int fs2_decode_ex(fs2_handle* h, const float* hm, const int64_t* olens, const float* es, const float* ps, int B, int L,
                   float* before, float* after, float* e_out, float* p_out, int64_t* e_ids, int64_t* p_ids, void* ws,
                   size_t ws_bytes, int flags, void* stream) {
+  return fs2_decode_ctl(h, hm, olens, es, ps, B, L, before, after, e_out, p_out, e_ids, p_ids, nullptr, nullptr, ws, ws_bytes,
+                        flags, stream);
+}
+
+int fs2_decode_ctl(fs2_handle* h, const float* hm, const int64_t* olens, const float* es, const float* ps, int B, int L,
+                   float* before, float* after, float* e_out, float* p_out, int64_t* e_ids, int64_t* p_ids,
+                   const float* e_scale, const float* p_scale, void* ws, size_t ws_bytes, int flags, void* stream) {
   FS2_REQUIRE(h && hm && before && after && e_out && p_out && ws, "fs2_decode: null argument");
   FS2_REQUIRE((es == nullptr) == (ps == nullptr), "fs2_decode: es and ps must both be given or both be NULL");
+  FS2_REQUIRE(!(e_scale || p_scale) || !es, "fs2_decode_ctl: e_scale / p_scale scale predicted values; with es / ps given there are none");
   FS2_REQUIRE((flags & ~FS2_PER_UTTERANCE) == 0, "fs2_decode_ex: unknown flags 0x%x", flags);
   FS2_REQUIRE(!(flags & FS2_PER_UTTERANCE) || olens, "fs2_decode_ex: FS2_PER_UTTERANCE needs olens");
   if (!h->loaded) { set_error("fs2_decode: weights not loaded"); return FS2_ERR_NOT_LOADED; }
@@ -664,8 +685,8 @@ int fs2_decode_ex(fs2_handle* h, const float* hm, const int64_t* olens, const fl
     ProfScope prof_scope(P_ROWNORM, 0, 8.0 * rows * c.adim, st);
     if ((rc = split_rows(hm, c.adim, rows, c.adim, p.hmp, st))) return rc;
   }
-  if ((rc = run_predictor(h->energy, hm, pred_planes ? p.hmp : nullptr, c.adim, B, L, p.t1, p.t2, p.t2p, olens, zlens, e_out, nullptr, st))) return rc;
-  if ((rc = run_predictor(h->pitch, hm, pred_planes ? p.hmp : nullptr, c.adim, B, L, p.t1, p.t2, p.t2p, olens, zlens, p_out, nullptr, st))) return rc;
+  if ((rc = run_predictor(h->energy, hm, pred_planes ? p.hmp : nullptr, c.adim, B, L, p.t1, p.t2, p.t2p, olens, zlens, e_out, nullptr, e_scale, st))) return rc;
+  if ((rc = run_predictor(h->pitch, hm, pred_planes ? p.hmp : nullptr, c.adim, B, L, p.t1, p.t2, p.t2p, olens, zlens, p_out, nullptr, p_scale, st))) return rc;
   // hs + pitch_embed(one_hot) + energy_embed(one_hot) (fastspeech.py:218-219); plane families: straight to the decoder
   // input Linear's operand planes
   { ProfScope prof_scope(P_VAR_EMBED, 0, 4.0 * rows * c.adim * 4, st);

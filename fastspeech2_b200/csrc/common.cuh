@@ -99,6 +99,7 @@ struct RowNorm {
   const float* pe; const float* alpha; int L;  // optional: y += alpha * pe[t], t = row % L
   // optional scalar head (predictors): s = y . head_w + head_b, 0 where t >= lens[b]
   const float* head_w; const float* head_b; float* head_out; int64_t* dur_out;
+  const float* head_scale;        // optional [rows]: head_out[row] = fp32(s * head_scale[row]), one rounding (prosody control)
   const int64_t* lens;            // optional mask (needs L > 0): rows t >= lens[b] write 0 to the head, out and split_out
   __half* split_out;              // optional operand planes of y (scaled by kPlaneScale): hi at [row][C], lo at [rows + row][C]
   int split_lo;                   // write the lo plane too (3xF16 consumer)
@@ -133,10 +134,12 @@ int qkv_to_planes(const float* qkv, int B, int L, int C, int heads, __half* qkp,
 // vt[(b*heads + h)*dk + d][t] = qkv[b, t, 2C + h*dk + d]   (test helper for the single-operator entry)
 int transpose_v(const float* qkv, int B, int L, int C, int heads, float* vt, int lpad, cudaStream_t st);
 
-int length_plan(void* ds, int ds_dtype, const int64_t* ilens, float alpha, int B, int T, int mutate, int32_t* cum,
-                int64_t* olens, int64_t* stats, cudaStream_t st);
+// alpha_v (nullable): per-phoneme factors [B, T] in place of the scalar alpha; d_used (nullable): [B, T] frame counts expanded
+int length_plan(void* ds, int ds_dtype, const int64_t* ilens, float alpha, const float* alpha_v, int B, int T, int mutate,
+                int32_t* cum, int64_t* olens, int64_t* stats, int64_t* d_used, cudaStream_t st);
+// fac_in [2][B, T] -> fac_out [2][B, Lcap] (both nullable): each frame takes the factors of its source phoneme, 1 past olens
 int length_gather(const float* hs, const int32_t* cum, const int64_t* ilens, int B, int T, int C, float* out, int Lcap,
-                  cudaStream_t st);
+                  const float* fac_in, float* fac_out, cudaStream_t st);
 
 int masked_losses(const float* before, const float* after, const float* ys, int ld_ys_time, const float* d_out,
                   const void* ds, int ds_dtype, const float* e_out, const float* p_out, const float* es, const float* ps,

@@ -19,20 +19,29 @@ namespace {
 
 constexpr int PLAN_THREADS = 256;
 
+// rint(fp32(d) * fp32(a)), half to even: torch.round(ds.float() * alpha).long() (:58-59).  Clamped to 2^31 so that a sum
+// of Tmax of them cannot wrap a long: any total past INT32_MAX reaches the caller through olens / stats[0] and is refused
+// there (cum is int32)
+__device__ __forceinline__ long scaled_duration(float d, float a) {
+  const float s = __fmul_rn(d, a);
+  return s >= 2147483648.0f ? 2147483648L : (long)rintf(s);
+}
+
 __device__ __forceinline__ long load_duration(const void* ds, int dtype, long idx, float alpha, bool scale) {
   if (dtype == FS2_DUR_F32) {
     float f = ((const float*)ds)[idx];
-    if (scale) return (long)rintf(f * alpha);  // torch.round(ds.float()*alpha).long()  (:58-59)
+    if (scale) return scaled_duration(f, alpha);
     return (long)truncf(f);                    // int(d_)                               (:93)
   }
   long d = dtype == FS2_DUR_I32 ? (long)((const int32_t*)ds)[idx] : (long)((const int64_t*)ds)[idx];
-  if (scale) return (long)rintf((float)d * alpha);
+  if (scale) return scaled_duration((float)d, alpha);
   return d;
 }
 
 __global__ void __launch_bounds__(PLAN_THREADS)
-length_plan_kernel(void* ds, int dtype, const int64_t* __restrict__ ilens, float alpha, int T, int mutate,
-                   int32_t* __restrict__ cum, int64_t* __restrict__ olens, unsigned long long* __restrict__ stats) {
+length_plan_kernel(void* ds, int dtype, const int64_t* __restrict__ ilens, float alpha, const float* __restrict__ alpha_v,
+                   int T, int mutate, int32_t* __restrict__ cum, int64_t* __restrict__ olens,
+                   unsigned long long* __restrict__ stats, int64_t* __restrict__ d_used) {
   __shared__ long warp_tot[PLAN_THREADS / 32];
   __shared__ long carry_s;
   __shared__ int any_nonzero, n_negative;
@@ -40,7 +49,7 @@ length_plan_kernel(void* ds, int dtype, const int64_t* __restrict__ ilens, float
   long ilen = ilens[b];
   if (ilen > T) ilen = T;
   if (ilen < 0) ilen = 0;
-  const bool scale = alpha != 1.0f;
+  const bool scale = alpha_v || alpha != 1.0f;   // alpha_v: one factor per phoneme [B, T], in place of the scalar
   const long base = (long)b * T;
   if (tid == 0) { carry_s = 0; any_nonzero = 0; n_negative = 0; }
   __syncthreads();
@@ -52,7 +61,7 @@ length_plan_kernel(void* ds, int dtype, const int64_t* __restrict__ ilens, float
     double part = 0.0;
     for (long t = tid; t < ilen; t += PLAN_THREADS) {
       if (dtype == FS2_DUR_F32 && !scale) part += (double)((const float*)ds)[base + t];
-      else part += (double)load_duration(ds, dtype, base + t, alpha, scale);
+      else part += (double)load_duration(ds, dtype, base + t, alpha_v ? alpha_v[base + t] : alpha, scale);
     }
     // any lane with a non-zero partial sum: exact for non-negative inputs (the only valid ones)
     if (part != 0.0) atomicOr(&any_nonzero, 1);
@@ -65,7 +74,7 @@ length_plan_kernel(void* ds, int dtype, const int64_t* __restrict__ ilens, float
     long t = t0 + tid;
     long d = 0;
     if (t < ilen) {
-      d = fill_one ? 1 : load_duration(ds, dtype, base + t, alpha, scale);
+      d = fill_one ? 1 : load_duration(ds, dtype, base + t, alpha_v ? alpha_v[base + t] : alpha, scale);
       if (d < 0) { atomicAdd(&n_negative, 1); d = 0; }
       if (fill_one && mutate) {  // d.fill_(1) on a view of the caller's tensor (:87)
         if (dtype == FS2_DUR_F32) ((float*)ds)[base + t] = 1.0f;
@@ -84,7 +93,10 @@ length_plan_kernel(void* ds, int dtype, const int64_t* __restrict__ ilens, float
     long prefix = carry_s;
     for (int w = 0; w < wid; ++w) prefix += warp_tot[w];
     v += prefix;
-    if (t < T) cum[base + t] = (int32_t)v;  // positions >= ilen repeat the total (d = 0 there)
+    if (t < T) {
+      cum[base + t] = (int32_t)v;  // positions >= ilen repeat the total (d = 0 there)
+      if (d_used) d_used[base + t] = d;   // the frame counts the gather expands: scaled, all-zero rule applied, 0 past ilen
+    }
     __syncthreads();
     if (tid == PLAN_THREADS - 1) carry_s = v;
     __syncthreads();
@@ -101,7 +113,8 @@ constexpr int FRAMES_PER_CTA = 32;
 template <int VEC_PER_ROW_MAX>
 __global__ void __launch_bounds__(256)
 length_gather_kernel(const float* __restrict__ hs, const int32_t* __restrict__ cum, const int64_t* __restrict__ ilens,
-                     int T, int C, float* __restrict__ out, int Lcap) {
+                     int T, int C, float* __restrict__ out, int Lcap, const float* __restrict__ fac_in,
+                     float* __restrict__ fac_out) {
   pdl_trigger(); pdl_wait();
   extern __shared__ int32_t scum[];  // [T]
   __shared__ int src_row[FRAMES_PER_CTA];
@@ -128,6 +141,11 @@ length_gather_kernel(const float* __restrict__ hs, const int32_t* __restrict__ c
       idx = lo;
     }
     src_row[tid] = idx;
+    if (fac_out && j < Lcap) {   // per-phoneme factors [2][B, T] -> per-frame [2][B, Lcap]; 1 where no phoneme is expanded
+      const long B = gridDim.y, o = (long)b * Lcap + j, i = (long)b * T + idx;
+      fac_out[o] = idx >= 0 ? fac_in[i] : 1.0f;
+      fac_out[B * Lcap + o] = idx >= 0 ? fac_in[B * T + i] : 1.0f;
+    }
   }
   __syncthreads();
   const int vec_per_row = C >> 2;
@@ -145,21 +163,23 @@ length_gather_kernel(const float* __restrict__ hs, const int32_t* __restrict__ c
 
 }  // namespace
 
-int length_plan(void* ds, int ds_dtype, const int64_t* ilens, float alpha, int B, int T, int mutate, int32_t* cum,
-                int64_t* olens, int64_t* stats, cudaStream_t st) {
+int length_plan(void* ds, int ds_dtype, const int64_t* ilens, float alpha, const float* alpha_v, int B, int T, int mutate,
+                int32_t* cum, int64_t* olens, int64_t* stats, int64_t* d_used, cudaStream_t st) {
   FS2_REQUIRE(alpha > 0.f, "length_plan: alpha must be > 0 (length_regulator.py:57)");
+  FS2_REQUIRE(!(alpha_v && mutate), "length_plan: per-phoneme factors scale a private copy, mutate_ds must be 0");
   FS2_REQUIRE(ds_dtype == FS2_DUR_I64 || ds_dtype == FS2_DUR_F32 || ds_dtype == FS2_DUR_I32, "length_plan: bad ds dtype %d", ds_dtype);
   FS2_CUDA_CHECK(cudaMemsetAsync(stats, 0, 2 * sizeof(int64_t), st));
   if (B == 0) return FS2_OK;
-  length_plan_kernel<<<B, PLAN_THREADS, 0, st>>>(ds, ds_dtype, ilens, alpha, T, mutate, cum, olens,
-                                                 reinterpret_cast<unsigned long long*>(stats));
+  length_plan_kernel<<<B, PLAN_THREADS, 0, st>>>(ds, ds_dtype, ilens, alpha, alpha_v, T, mutate, cum, olens,
+                                                 reinterpret_cast<unsigned long long*>(stats), d_used);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
 
 int length_gather(const float* hs, const int32_t* cum, const int64_t* ilens, int B, int T, int C, float* out, int Lcap,
-                  cudaStream_t st) {
+                  const float* fac_in, float* fac_out, cudaStream_t st) {
   FS2_REQUIRE(C % 4 == 0, "length_gather: C must be a multiple of 4");
+  FS2_REQUIRE((fac_in == nullptr) == (fac_out == nullptr), "length_gather: factors in and out must both be given or both be NULL");
   if (B == 0 || Lcap == 0) return FS2_OK;
   size_t smem = (size_t)T * sizeof(int32_t);
   FS2_REQUIRE(smem <= 200 * 1024, "length_gather: Tmax=%d too large for the shared cum row", T);
@@ -173,7 +193,7 @@ int length_gather(const float* hs, const int32_t* cum, const int64_t* ilens, int
     }
   }
   dim3 grid((Lcap + FRAMES_PER_CTA - 1) / FRAMES_PER_CTA, B);
-  FS2_CUDA_CHECK(launch_pdl(length_gather_kernel<0>, grid, dim3(256), smem, st, hs, cum, ilens, T, C, out, Lcap));
+  FS2_CUDA_CHECK(launch_pdl(length_gather_kernel<0>, grid, dim3(256), smem, st, hs, cum, ilens, T, C, out, Lcap, fac_in, fac_out));
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }

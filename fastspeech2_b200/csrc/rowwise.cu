@@ -108,7 +108,7 @@ __global__ void row_norm_kernel(RowNorm r) {
   if (r.head_w) {
     dot = warp_sum(dot) + __ldg(r.head_b);
     if (lane == 0) {
-      if (r.head_out) r.head_out[row] = padded ? 0.f : dot;
+      if (r.head_out) r.head_out[row] = padded ? 0.f : (r.head_scale ? __fmul_rn(dot, __ldg(r.head_scale + row)) : dot);
       if (r.dur_out) {
         // clamp(round(exp(x) - 1), min=0).long(), round = half to even (duration_predictor.py:77-81)
         float d = fmaxf(rintf(expf(dot) - 1.0f), 0.f);

@@ -203,6 +203,54 @@ def _init_like_reference(model: nn.Module, init_type: str) -> None:
             m.reset_parameters()
 
 
+_CONTROL_NAMES = ("speed", "pitch", "energy")
+
+
+def _controls_for(B: int, T: int, dev: torch.device, controls: Dict[str, Any], ilens: Any = None) -> Optional[Tuple]:
+    """Prosody controls -> (speed, pitch, energy), each None or a contiguous float32 [B, T] tensor on `dev`; None when
+    no control is given.  A control is a Python number, a [B] tensor (one factor per utterance) or a [B, T] tensor (one
+    factor per phoneme; entries at t >= ilens[b] are ignored).  Factors are rounded to fp32 first and must be finite
+    and > 0: values on the host are checked here (per-phoneme ones only when `ilens` is on the host too), the rest in
+    the caller's single host read (`_control_violations`)."""
+    if all(controls[k] is None for k in _CONTROL_NAMES):
+        return None
+    out = []
+    for name in _CONTROL_NAMES:
+        v = controls[name]
+        if v is None:
+            out.append(None)
+            continue
+        if not torch.is_tensor(v):
+            if isinstance(v, bool) or not isinstance(v, (int, float)):
+                raise ValueError(f"{name} must be a number or a tensor, got {type(v).__name__}")
+            v = torch.tensor(float(v), dtype=torch.float64)      # rounded to fp32 below (1e39 -> inf, 1e-50 -> 0)
+        v = v.detach().to(torch.float32)
+        used = None                       # host mask of the factors that matter; None: check on the device
+        if v.dim() == 0:
+            v = v.expand(B, T)
+            used = torch.ones((), dtype=torch.bool)
+        elif v.dim() == 1 and v.shape[0] == B:
+            v = v[:, None].expand(B, T)
+            used = torch.ones((), dtype=torch.bool)
+        elif tuple(v.shape) != (B, T):
+            raise ValueError(f"{name} must be a number, a [B={B}] or a [B={B}, Tmax={T}] tensor, got {tuple(v.shape)}")
+        elif torch.is_tensor(ilens) and not ilens.is_cuda and tuple(ilens.shape) == (B,):
+            used = torch.arange(T)[None, :] < ilens[:, None]
+        if not v.is_cuda and used is not None:
+            bad = ~(torch.isfinite(v) & (v > 0)) & used
+            if bool(bad.any()):
+                raise ValueError(f"{name}: every factor must be finite and > 0 in fp32 (got {float(v[bad][0])})")
+        out.append(v.to(dev).contiguous())
+    return tuple(out)
+
+
+def _control_violations(controls: Tuple, ilens: torch.Tensor, T: int) -> torch.Tensor:
+    """Device scalar: how many factors of the valid positions (t < ilens[b]) are non-finite or <= 0."""
+    valid = torch.arange(T, device=ilens.device)[None, :] < ilens[:, None]
+    bad = [(~(torch.isfinite(c) & (c > 0)) & valid).sum() for c in controls if c is not None]
+    return torch.stack(bad).sum()
+
+
 # ------------------------------------------------------------------------------------------------
 class FeedForwardTransformer(nn.Module):
     """Feed-forward Transformer TTS (FastSpeech2) on H100.  See module docstring."""
@@ -376,19 +424,29 @@ class FeedForwardTransformer(nn.Module):
     def _forward(self, xs: torch.Tensor, ilens: torch.Tensor, olens: torch.Tensor = None, ds: torch.Tensor = None,
                  es: torch.Tensor = None, ps: torch.Tensor = None, is_inference: bool = False,
                  _one_hot: bool = True, _defer_check: Optional[list] = None, _after_out: Optional[torch.Tensor] = None,
-                 per_utterance: bool = False, _olens_out: Optional[list] = None) -> Sequence[torch.Tensor]:
+                 per_utterance: bool = False, _olens_out: Optional[list] = None,
+                 _controls: Optional[Tuple] = None) -> Sequence[torch.Tensor]:
         """The reference's `_forward` (fastspeech.py:169-243).  `per_utterance=True` (not in the reference) makes every
         utterance's result independent of its batch mates: utterance b is bit-identical to the B = 1 call on
         `xs[b:b+1, :ilens[b]]` (teacher-forced: with its es / ps sliced to olens[b]), in inference the decoder is masked by
         the predicted lengths, every padded position of every returned tensor is exactly 0 (all-zero one-hot rows), and
         row tiles wholly in padding are skipped.  It needs 1 <= ilens[b] <= Tmax, and in teacher-forced mode
-        olens[b] == sum(ds[b, :ilens[b]]).  `_olens_out` (list): receives the olens the decoder ran with."""
+        olens[b] == sum(ds[b, :ilens[b]]).  `_olens_out` (list): receives the olens the decoder ran with.
+        `_controls` (from `_controls_for`): prosody factors (speed, pitch, energy) per phoneme, in inference only, and
+        only where an utterance's result does not depend on its batch mates (per_utterance, or B = 1); the returned
+        durations are then the frame counts actually expanded."""
         # the handle-less ABI stages (LengthRegulator, losses, ...) run on the CURRENT device like any CUDA library call:
         # select the device the data lives on for the whole call, leave the caller's current device untouched
         if xs.is_cuda and torch.cuda.current_device() != (xs.device.index or 0):
             with torch.cuda.device(xs.device):
                 return self._forward(xs, ilens, olens, ds, es, ps, is_inference, _one_hot, _defer_check, _after_out,
-                                     per_utterance, _olens_out)
+                                     per_utterance, _olens_out, _controls)
+        if _controls is not None:
+            if not is_inference:
+                raise ValueError("prosody controls apply to inference only (teacher-forced durations, energy and pitch are given)")
+            if not per_utterance and xs.shape[0] != 1:
+                raise ValueError("prosody controls on a batch need per_utterance=True (use synthesize): under the reference's "
+                                 "batch semantics an utterance's result depends on its batch mates")
         if per_utterance:
             self._check_ilens(xs, ilens)
         h = self._ready(xs)
@@ -426,16 +484,29 @@ class FeedForwardTransformer(nn.Module):
                                      _lib.ptr(ws), ws.numel(), flags, st), "fs2_encode_ex")
 
         # stage 2: length regulator
-        cum, olens_lr, stats, _ = _lr.plan(hs, d_int if is_inference else ds, ilens, 1.0)
+        speed, pitch, energy = _controls if _controls is not None else (None, None, None)
+        if speed is not None:       # scaled durations on a private copy; d_int then reports the frames actually expanded
+            d_used = torch.empty((B, T), dtype=torch.int64, device=dev)
+            cum, olens_lr, stats, _ = _lr.plan(hs, d_int, ilens, 1.0, alpha_v=speed, d_used=d_used)
+            d_int = d_used
+        else:
+            cum, olens_lr, stats, _ = _lr.plan(hs, d_int if is_inference else ds, ilens, 1.0)
         if is_inference:
+            words = [stats]
             if per_utterance:       # the ilens range rides along in the same transfer
-                lmax, n_neg, imin, imax = torch.cat([stats, torch.stack([ilens.min(), ilens.max()])]).tolist()
-                self._check_ilens_range(imin, imax, T)
-            else:
-                lmax, n_neg = stats.tolist()  # the single host sync of inference: sizes the mel buffers
-            L = int(lmax)
+                words.append(torch.stack([ilens.min(), ilens.max()]))
+            if _controls is not None:
+                words.append(_control_violations(_controls, ilens, T).view(1))
+            vals = torch.cat(words).tolist() if len(words) > 1 else stats.tolist()  # the single host sync of inference
+            if _controls is not None and vals[-1]:
+                raise ValueError(f"prosody controls: {vals[-1]} factor(s) are non-finite or <= 0 (each must be finite and > 0)")
+            if per_utterance:
+                self._check_ilens_range(vals[2], vals[3], T)
+            L = int(vals[0])
             if L <= 0:
                 raise RuntimeError("inference produced zero frames")
+            if L > _lr.INT32_MAX:
+                raise ValueError(f"an utterance expands to {L} frames, more than the length plan's int32 prefix sum holds")
             if L > self.decoder.embed[-1].pe.shape[1]:
                 self._extend_pe(self.decoder, L)
                 h = self._ready(xs)
@@ -446,7 +517,14 @@ class FeedForwardTransformer(nn.Module):
             olens_dec = olens.to(device=dev, dtype=torch.int64).contiguous()
         if _olens_out is not None:
             _olens_out.append(olens_lr if is_inference else olens_dec)
-        hm = _lr.gather(hs, cum, ilens, L)
+        fac = None
+        if pitch is not None or energy is not None:   # per-phoneme factors -> per-frame, in the gather's pass
+            ones = torch.ones((B, T), **f32)
+            fac = torch.empty((2, B, L), **f32)
+            hm = _lr.gather(hs, cum, ilens, L, torch.stack([energy if energy is not None else ones,
+                                                            pitch if pitch is not None else ones]), fac)
+        else:
+            hm = _lr.gather(hs, cum, ilens, L)
 
         # stage 3: variance adaptor + decoder + postnet
         ws = self._ws(B, T, L)
@@ -463,9 +541,11 @@ class FeedForwardTransformer(nn.Module):
         p_ids = torch.empty((B, L), dtype=torch.int64, device=dev) if want_ids else None
         es_c = None if is_inference else es.to(**f32).contiguous()
         ps_c = None if is_inference else ps.to(**f32).contiguous()
-        _lib.check(lib.fs2_decode_ex(h, _lib.ptr(hm), _lib.ptr(olens_dec), _lib.ptr(es_c), _lib.ptr(ps_c), B, L, _lib.ptr(before),
-                                     _lib.ptr(after), _lib.ptr(e_out), _lib.ptr(p_out), _lib.ptr(e_ids), _lib.ptr(p_ids),
-                                     _lib.ptr(ws), ws.numel(), flags, st), "fs2_decode_ex")
+        e_scale = fac[0] if energy is not None else None
+        p_scale = fac[1] if pitch is not None else None
+        _lib.check(lib.fs2_decode_ctl(h, _lib.ptr(hm), _lib.ptr(olens_dec), _lib.ptr(es_c), _lib.ptr(ps_c), B, L, _lib.ptr(before),
+                                      _lib.ptr(after), _lib.ptr(e_out), _lib.ptr(p_out), _lib.ptr(e_ids), _lib.ptr(p_ids),
+                                      _lib.ptr(e_scale), _lib.ptr(p_scale), _lib.ptr(ws), ws.numel(), flags, st), "fs2_decode_ctl")
 
         if is_inference:
             if not _one_hot:
@@ -566,13 +646,44 @@ class FeedForwardTransformer(nn.Module):
         _, outs, _, _, _ = self._forward(x.unsqueeze(0), ilens, is_inference=True, _one_hot=False)
         return outs[0]
 
-    def synthesize(self, xs: torch.Tensor, ilens: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    def inference_controlled(self, x: torch.Tensor, *, speed=None, pitch=None, energy=None) -> torch.Tensor:
+        """`inference` with prosody controls (not in the reference, whose `_forward` passes alpha = 1 to its
+        LengthRegulator and pitch / energy predictors; `inference` itself keeps the reference's signature).  Each control
+        is None, a number or a [T] tensor of per-phoneme factors, finite and > 0.  speed multiplies the predicted
+        durations (> 1 is slower): rint_half_even(fp32(d) * fp32(a)), then the all-zero rule on the scaled slice.  pitch
+        and energy multiply the predicted values before bucketize, one fp32 rounding, each frame by the factor of the
+        phoneme it was expanded from (pitch is in Hz: 2 ** (k / 12) shifts by k semitones).  With no control this is
+        `inference`."""
+        if x.dim() != 1:
+            raise ValueError("x must be [T]")
+        ctl = {"speed": speed, "pitch": pitch, "energy": energy}
+        for k, v in ctl.items():
+            if torch.is_tensor(v) and v.dim() != 0:
+                if v.dim() != 1 or v.shape[0] != x.shape[0]:
+                    raise ValueError(f"{k} must be a number or a [T={x.shape[0]}] tensor, got {tuple(v.shape)}")
+                ctl[k] = v[None, :]
+        controls = _controls_for(1, int(x.shape[0]), x.device, ctl)
+        ilens = torch.tensor([x.shape[0]], dtype=torch.long, device=x.device)
+        _, outs, _, _, _ = self._forward(x.unsqueeze(0), ilens, is_inference=True, _one_hot=False, _controls=controls)
+        return outs[0]
+
+    def synthesize(self, xs: torch.Tensor, ilens: torch.Tensor, *, speed=None, pitch=None,
+                   energy=None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Per-utterance batched inference (not in the reference): xs [B, Tmax] int64 (0 = pad), ilens [B] with
         1 <= ilens[b] <= Tmax -> (mels [B, Lmax, odim], olens [B] int64, durations [B, Tmax] int64), all on the device.
         durations[b], olens[b] and mels[b, :olens[b]] are bit-identical to what `inference(xs[b, :ilens[b]])` computes,
-        whatever else is in the batch; mels[b, olens[b]:] and durations[b, ilens[b]:] are 0.  One host read per call."""
+        whatever else is in the batch; mels[b, olens[b]:] and durations[b, ilens[b]:] are 0.  One host read per call.
+        speed / pitch / energy: prosody controls as in `inference_controlled`, each None, a number, a [B] tensor (per
+        utterance) or a [B, Tmax] tensor (per phoneme; entries past ilens[b] are ignored).  Utterance b is then
+        bit-identical to `inference_controlled` on it with its slice of the controls.  durations are the frame counts expanded (after speed and
+        the all-zero rule): durations.sum(1) == olens."""
+        if xs.dim() != 2:
+            raise ValueError("xs must be [B, Tmax]")
+        controls = _controls_for(int(xs.shape[0]), int(xs.shape[1]), xs.device,
+                                 {"speed": speed, "pitch": pitch, "energy": energy}, ilens)
         got: list = []
-        _, after, dur, _, _ = self._forward(xs, ilens, is_inference=True, _one_hot=False, per_utterance=True, _olens_out=got)
+        _, after, dur, _, _ = self._forward(xs, ilens, is_inference=True, _one_hot=False, per_utterance=True, _olens_out=got,
+                                            _controls=controls)
         return after, got[0], dur
 
 

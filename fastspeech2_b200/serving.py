@@ -11,6 +11,7 @@ buffer (+ their keys and shapes) and its `forward` is ONE call of the custom ope
     served = torch.jit.load("fs2.pt").cuda()                         # any process that imported this module
     mel = served(torch.tensor(ids).cuda())                           # [L, odim]; batched: served.batch(xs, ilens)
     mels, olens = served.synthesize(xs, ilens)                       # batched, each utterance independent of its batch mates
+    mels, olens, durations = served.synthesize_controlled(xs, ilens, speed, pitch, energy)   # + prosody controls
 
 The operator is registered through `torch.library` (schema + CUDA implementation); there is no CPU implementation -- a
 CPU tensor fails loudly like the rest of the path.
@@ -29,6 +30,8 @@ _LIB = torch.library.Library("fs2_b200", "DEF")
 _LIB.define("inference(Tensor blob, str[] keys, int[] ranks, int[] dims, str precision, Tensor x) -> Tensor")
 _LIB.define("inference_batch(Tensor blob, str[] keys, int[] ranks, int[] dims, str precision, Tensor xs, Tensor ilens) -> (Tensor, Tensor)")
 _LIB.define("synthesize_batch(Tensor blob, str[] keys, int[] ranks, int[] dims, str precision, Tensor xs, Tensor ilens) -> (Tensor, Tensor)")
+_LIB.define("synthesize_controlled(Tensor blob, str[] keys, int[] ranks, int[] dims, str precision, Tensor xs, Tensor ilens, "
+            "Tensor speed, Tensor pitch, Tensor energy) -> (Tensor, Tensor, Tensor)")
 
 # one packed model per (device, identity of the checkpoint blob): the op is functional from TorchScript's point of view,
 # the cache only avoids re-packing the checkpoint on every call
@@ -92,6 +95,11 @@ def _synthesize_batch(blob, keys, ranks, dims, precision, xs, ilens):
     return mels, olens
 
 
+def _synthesize_controlled(blob, keys, ranks, dims, precision, xs, ilens, speed, pitch, energy):
+    with torch.no_grad():
+        return _model_for(blob, keys, ranks, dims, precision).synthesize(xs, ilens, speed=speed, pitch=pitch, energy=energy)
+
+
 def _no_cpu(*a, **k):
     raise RuntimeError("fs2_b200 operators run on CUDA tensors only (the H100 path has no CPU fallback)")
 
@@ -99,9 +107,11 @@ def _no_cpu(*a, **k):
 _LIB.impl("inference", _inference, "CUDA")
 _LIB.impl("inference_batch", _inference_batch, "CUDA")
 _LIB.impl("synthesize_batch", _synthesize_batch, "CUDA")
+_LIB.impl("synthesize_controlled", _synthesize_controlled, "CUDA")
 _LIB.impl("inference", _no_cpu, "CPU")
 _LIB.impl("inference_batch", _no_cpu, "CPU")
 _LIB.impl("synthesize_batch", _no_cpu, "CPU")
+_LIB.impl("synthesize_controlled", _no_cpu, "CPU")
 
 
 class ScriptedFastSpeech2(torch.nn.Module):
@@ -131,6 +141,16 @@ class ScriptedFastSpeech2(torch.nn.Module):
         Each utterance's mels are bit-identical to forward() on it alone, whatever else is in the batch; padded frames
         are 0 (FeedForwardTransformer.synthesize)."""
         return torch.ops.fs2_b200.synthesize_batch(self.blob, self.keys, self.ranks, self.dims, self.precision, xs, ilens)
+
+    @torch.jit.export
+    def synthesize_controlled(self, xs: torch.Tensor, ilens: torch.Tensor, speed: torch.Tensor, pitch: torch.Tensor,
+                              energy: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """`synthesize` with prosody controls (e.g. SSML <prosody rate= pitch= volume=>): speed, pitch and energy are
+        0-d tensors (one factor for the batch), [B] (per utterance) or [B, T] (per phoneme) factors, finite and > 0;
+        pass torch.ones(()) for no change -> (mels [B,Lmax,odim], olens [B], durations [B,T] frame counts expanded).
+        Equal to FeedForwardTransformer.synthesize with the same controls."""
+        return torch.ops.fs2_b200.synthesize_controlled(self.blob, self.keys, self.ranks, self.dims, self.precision, xs,
+                                                        ilens, speed, pitch, energy)
 
 
 def scripted(model: FeedForwardTransformer, precision: Optional[str] = None) -> torch.jit.ScriptModule:

@@ -156,6 +156,24 @@ int fs2_length_plan(void* ds, int ds_dtype, const int64_t* ilens, float alpha, i
 int fs2_length_gather(const float* hs, const int32_t* cum, const int64_t* ilens, int B, int Tmax, int C, float* out,
                       int Lcap, void* stream);
 
+/* Prosody control (speed).  fs2_length_plan with one duration factor per phoneme; fs2_length_plan is the case
+ * alpha_v = d_used = NULL.  The reference scales by one scalar, torch.round(ds.float() * alpha).long()
+ * (length_regulator.py:57-59); here
+ *   alpha_v [B,Tmax] f32 or NULL: d'[b,t] = rint_half_even(fp32(d) * alpha_v[b,t]) (one fp32 rounding before the
+ *           rint), in place of the scalar alpha (which must then be 1).  The all-zero -> all-one rule (:86-88) is
+ *           evaluated on the scaled slice.  Requires mutate_ds == 0: the caller's ds are never written.
+ *   d_used  [B,Tmax] i64 out or NULL: the frame counts the gather expands (scaled, all-zero rule applied, 0 past ilens).
+ * A total frame count that does not fit the int32 prefix sum is reported, not wrapped: olens[b] and stats[0] hold the
+ * true total (at least 2^31), and the caller must refuse to gather from such a plan. */
+int fs2_length_plan_ex(void* ds, int ds_dtype, const int64_t* ilens, float alpha, const float* alpha_v, int B, int Tmax,
+                       int mutate_ds, int32_t* cum, int64_t* olens, int64_t* stats, int64_t* d_used, void* stream);
+/* fs2_length_gather with a side output for the pitch / energy controls; fs2_length_gather is fac_in = fac_out = NULL.
+ *   fac_in  [2][B,Tmax] f32: per-phoneme factors (plane 0 energy, plane 1 pitch, say; the kernel does not care)
+ *   fac_out [2][B,Lcap] f32 out: fac_out[k][b,j] = fac_in[k][b, min{i: cum[b,i] > j}] for j < olens[b], 1.0 for the rest
+ * Both or neither. */
+int fs2_length_gather_ex(const float* hs, const int32_t* cum, const int64_t* ilens, int B, int Tmax, int C, float* out,
+                         int Lcap, const float* fac_in, float* fac_out, void* stream);
+
 /* ---- stage 3: variance adaptor + mel decoder + Postnet --------------------------------- */
 /* fastspeech.py:195-238.
  *   hm [B,L,adim] f32: length-regulated encoder states (read only)
@@ -176,6 +194,17 @@ int fs2_decode(fs2_handle* h, const float* hm, const int64_t* olens, const float
 int fs2_decode_ex(fs2_handle* h, const float* hm, const int64_t* olens, const float* es, const float* ps, int B, int L,
                   float* before, float* after, float* e_out, float* p_out, int64_t* e_ids, int64_t* p_ids, void* ws,
                   size_t ws_bytes, int flags, void* stream);
+
+/* Prosody control (pitch, energy).  fs2_decode_ex with per-frame factors on the predicted values; fs2_decode_ex is the
+ * case e_scale = p_scale = NULL.  The reference's EnergyPredictor / PitchPredictor.inference(xs, alpha) return
+ * `xs * alpha` before bucketize (variance_predictor.py:58,140-152,213-225); here
+ *   e_scale, p_scale [B,L] f32 or NULL (each independently): e_out[b,t] = fp32(e[b,t] * e_scale[b,t]), one fp32
+ *           rounding, no FMA; likewise p_out.  e_ids / p_ids and the decoder input bucketize the scaled values.
+ * Predict mode only: a scale together with es / ps returns FS2_ERR_INVALID.  Valid with flags 0 and FS2_PER_UTTERANCE;
+ * fs2_length_gather_ex expands per-phoneme factors into this layout. */
+int fs2_decode_ctl(fs2_handle* h, const float* hm, const int64_t* olens, const float* es, const float* ps, int B, int L,
+                   float* before, float* after, float* e_out, float* p_out, int64_t* e_ids, int64_t* p_ids,
+                   const float* e_scale, const float* p_scale, void* ws, size_t ws_bytes, int flags, void* stream);
 
 /* ---- stage 4: masked losses (fastspeech.py:277-333) ------------------------------------- */
 /* out7 (device, f32): l1, before, after, duration, energy, pitch, total -- the order of

@@ -10,7 +10,11 @@ Workloads:
   c2             inference on bench.py's c2 batch (B=64, T=100): the predicted lengths are ragged;
   c2_teacher_forced
                  bench.py's c2 teacher-forced step (every utterance T x L): no padding at all, so the mode must cost
-                 nothing there.
+                 nothing there;
+  filelist64_controls
+                 `synthesize` on filelist64 with explicit all-1.0 per-phoneme speed / pitch / energy against no controls:
+                 the results are bit-identical, so the difference is the cost of the prosody-control path; plus a row
+                 at speed 1.25 (25 % more frames), as valid frames/s.
 Eager launches, one host read per inference call; the two semantics run in alternating windows of `--steps` calls,
 and each reports the median window of `--rounds`.  The card name and power limit are read in the same run.
 """
@@ -92,6 +96,24 @@ def teacher_forced_semantics(model, batch, steps: int, rounds: int) -> dict:
     return {"ms_per_step": med, "ms_windows": ms, "per_utterance_over_reference": med["per_utterance"] / med["reference"]}
 
 
+def controls_cost(model, xs, ilens, steps: int, rounds: int) -> dict:
+    ones = torch.ones(xs.shape, device=xs.device)
+    fns = {"none": lambda: model.synthesize(xs, ilens),
+           "neutral": lambda: model.synthesize(xs, ilens, speed=ones, pitch=ones, energy=ones),
+           "speed_1.25": lambda: model.synthesize(xs, ilens, speed=1.25 * ones, pitch=ones, energy=ones)}
+    with torch.no_grad():
+        outs = {name: fn() for name, fn in fns.items()}
+    assert all(torch.equal(a, b) for a, b in zip(outs["none"], outs["neutral"])), "all-1.0 controls changed the result"
+    ms = alternate(fns, steps, rounds)
+    out = {}
+    for name, (_, olens, _) in outs.items():
+        t, frames = median(ms[name]), int(olens.sum())
+        out[name] = {"value": frames / (t * 1e-3), "unit": "valid frames/s", "ms_per_step": t, "ms_windows": ms[name],
+                     "valid_frames": frames}
+    out["neutral_over_none"] = out["neutral"]["ms_per_step"] / out["none"]["ms_per_step"]
+    return out
+
+
 def card() -> dict:
     info = {"name": torch.cuda.get_device_name()}
     try:
@@ -122,11 +144,13 @@ def main():
     c2 = {k: v.to(dev) for k, v in make_batch(64, 100, 800, seed=1234).items()}
     fl = np.load(os.path.join(ROOT, "tests", "golden", "filelist64.npz"))
     line = {
-        "metric": "per-utterance vs reference-semantics batched synthesis", "precision": args.precision, "card": card(),
+        "metric": "per-utterance vs reference-semantics batched synthesis; cost of prosody controls", "precision": args.precision, "card": card(),
         "filelist64": inference_semantics(model, torch.from_numpy(fl["xs"]).to(dev), torch.from_numpy(fl["ilens"]).to(dev),
                                           args.steps, args.rounds),
         "c2": inference_semantics(model, c2["xs"], c2["ilens"], args.steps, args.rounds),
         "c2_teacher_forced": teacher_forced_semantics(model, c2, args.steps, args.rounds),
+        "filelist64_controls": controls_cost(model, torch.from_numpy(fl["xs"]).to(dev), torch.from_numpy(fl["ilens"]).to(dev),
+                                             args.steps, args.rounds),
         "timing": f"eager launches, alternating windows of {args.steps} calls, median of {args.rounds} windows per semantics",
     }
     print(json.dumps(line), flush=True)
