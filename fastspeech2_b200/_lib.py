@@ -37,6 +37,12 @@ class WeightDesc(C.Structure):
                 ("dtype", C.c_int32)]
 
 
+class VocoderConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("n_fft", "hop", "win_length", "n_mels", "math_mode")]
+
+
+FS2_VOC_BAD_LENGTH, FS2_VOC_RANGE = 1, 2     # bits of fs2_griffin_lim's / fs2_mel_magnitude's device status word
+
 _P, _I, _F, _L, _SZ = C.c_void_p, C.c_int, C.c_float, C.c_int64, C.c_size_t
 
 # name -> argtypes; every function returns int except the three noted below
@@ -92,6 +98,11 @@ SIGNATURES = {
     "fs2_stft_magphase": [_P, _I, _I, _I, _I, _P, _P, _P],
     "fs2_istft_recombine": [_P, _P, _I, _I, _I, _I, _P, _P],
     "fs2_istft_overlap_add": [_P, _I, _I, _I, _I, _P, _F, _P, _P],
+    "fs2_vocoder_create": [C.POINTER(_P), C.POINTER(VocoderConfig)],
+    "fs2_vocoder_load": [_P, _P, _P, _P, _P, _P],
+    "fs2_vocoder_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_mel_magnitude": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_griffin_lim": [_P, _P, _P, _I, _I, _I, _F, _P, _P, _P, _P, _P, _SZ, _P],
     "fs2_peer_alloc": [_SZ, C.POINTER(_P), _P],
     "fs2_peer_free": [_P],
     "fs2_peer_open": [_P, C.POINTER(_P)],
@@ -100,7 +111,7 @@ SIGNATURES = {
     "fs2_flag_signal": [_P, _L, _P],
     "fs2_flag_wait": [_P, _I, _I, _L, _P],
 }
-OTHER_SYMBOLS = ("fs2_last_error", "fs2_version", "fs2_destroy", "fs2_kernel_launches", "fs2_profile_label")
+OTHER_SYMBOLS = ("fs2_last_error", "fs2_version", "fs2_destroy", "fs2_kernel_launches", "fs2_profile_label", "fs2_vocoder_destroy")
 ALL_SYMBOLS = tuple(SIGNATURES) + OTHER_SYMBOLS
 
 _lib: Optional[C.CDLL] = None
@@ -130,6 +141,8 @@ def load() -> C.CDLL:
     lib.fs2_profile_label.argtypes = [_I]
     lib.fs2_destroy.restype = None
     lib.fs2_destroy.argtypes = [_P]
+    lib.fs2_vocoder_destroy.restype = None
+    lib.fs2_vocoder_destroy.argtypes = [_P]
     _lib = lib
     return lib
 

@@ -221,6 +221,18 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
+// Philox4x32-10 counter-based generator (dropout masks, Griffin-Lim initial phases): the output depends only on
+// (counter, key), so any element can be redrawn without stored state
+__device__ __forceinline__ uint4 philox4x32(uint4 ctr, uint2 key) {
+  const unsigned M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const unsigned hi0 = __umulhi(M0, ctr.x), lo0 = M0 * ctr.x, hi1 = __umulhi(M1, ctr.z), lo1 = M1 * ctr.z;
+    ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
+    key.x += W0; key.y += W1;
+  }
+  return ctr;
+}
 // torch.bucketize(right=False): first i with !(bins[i] < x) ... written as torch does so NaN -> n_edges
 __device__ __forceinline__ int bucket_of(float x, const float* __restrict__ bins, int n_edges) {
   int lo = 0, hi = n_edges;

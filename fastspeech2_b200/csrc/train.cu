@@ -14,18 +14,8 @@ inline int grid_for(long n, int block, int cap = 132 * 8) {
 }
 
 // ---- dropout (torch.nn.Dropout in train mode: keep with prob 1-p, scale by 1/(1-p)) ---------------------------------------
-// Philox4x32-10 counter-based generator: mask byte i depends only on (seed, i), so the same mask is reproduced in backward
-// without storing random state; tests inject masks instead (shared with the reference run).
-__device__ __forceinline__ uint4 philox4x32(uint4 ctr, uint2 key) {
-  const unsigned M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const unsigned hi0 = __umulhi(M0, ctr.x), lo0 = M0 * ctr.x, hi1 = __umulhi(M1, ctr.z), lo1 = M1 * ctr.z;
-    ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
-    key.x += W0; key.y += W1;
-  }
-  return ctr;
-}
+// Philox4x32-10 (common.cuh): mask byte i depends only on (seed, i), so the same mask is reproduced in backward without
+// storing random state; tests inject masks instead (shared with the reference run).
 __global__ void dropout_mask_kernel(uint8_t* __restrict__ mask, long n, float p, unsigned long long seed, unsigned long long offset) {
   const long quads = (n + 3) / 4;
   for (long q = (long)blockIdx.x * blockDim.x + threadIdx.x; q < quads; q += (long)gridDim.x * blockDim.x) {

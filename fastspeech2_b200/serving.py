@@ -12,6 +12,7 @@ buffer (+ their keys and shapes) and its `forward` is ONE call of the custom ope
     mel = served(torch.tensor(ids).cuda())                           # [L, odim]; batched: served.batch(xs, ilens)
     mels, olens = served.synthesize(xs, ilens)                       # batched, each utterance independent of its batch mates
     mels, olens, durations = served.synthesize_controlled(xs, ilens, speed, pitch, energy)   # + prosody controls
+    audio, alens = served.synthesize_audio(xs, ilens, speed, pitch, energy, 30, 0.0, 0)      # + Griffin-Lim vocoder
 
 The operator is registered through `torch.library` (schema + CUDA implementation); there is no CPU implementation -- a
 CPU tensor fails loudly like the rest of the path.
@@ -25,6 +26,7 @@ import torch
 
 from .fastspeech import FeedForwardTransformer
 from .hparams import load_hp
+from .vocoder import GriffinLimVocoder
 
 _LIB = torch.library.Library("fs2_b200", "DEF")
 _LIB.define("inference(Tensor blob, str[] keys, int[] ranks, int[] dims, str precision, Tensor x) -> Tensor")
@@ -32,10 +34,13 @@ _LIB.define("inference_batch(Tensor blob, str[] keys, int[] ranks, int[] dims, s
 _LIB.define("synthesize_batch(Tensor blob, str[] keys, int[] ranks, int[] dims, str precision, Tensor xs, Tensor ilens) -> (Tensor, Tensor)")
 _LIB.define("synthesize_controlled(Tensor blob, str[] keys, int[] ranks, int[] dims, str precision, Tensor xs, Tensor ilens, "
             "Tensor speed, Tensor pitch, Tensor energy) -> (Tensor, Tensor, Tensor)")
+_LIB.define("synthesize_audio(Tensor blob, str[] keys, int[] ranks, int[] dims, str precision, Tensor xs, Tensor ilens, "
+            "Tensor speed, Tensor pitch, Tensor energy, int n_iters, float momentum, int seed) -> (Tensor, Tensor)")
 
 # one packed model per (device, identity of the checkpoint blob): the op is functional from TorchScript's point of view,
 # the cache only avoids re-packing the checkpoint on every call
 _MODELS: Dict[Tuple, FeedForwardTransformer] = {}
+_VOCODERS: Dict[str, GriffinLimVocoder] = {}     # math mode -> vocoder with the default config's audio parameters
 
 
 def pack_state(state_dict: Dict[str, torch.Tensor]):
@@ -100,6 +105,16 @@ def _synthesize_controlled(blob, keys, ranks, dims, precision, xs, ilens, speed,
         return _model_for(blob, keys, ranks, dims, precision).synthesize(xs, ilens, speed=speed, pitch=pitch, energy=energy)
 
 
+def _synthesize_audio(blob, keys, ranks, dims, precision, xs, ilens, speed, pitch, energy, n_iters, momentum, seed):
+    m = _model_for(blob, keys, ranks, dims, precision)
+    voc = _VOCODERS.get(m.precision)
+    if voc is None:
+        voc = _VOCODERS[m.precision] = GriffinLimVocoder.from_hp(load_hp(), math_mode=m.precision)
+    with torch.no_grad():
+        mels, olens, _ = m.synthesize(xs, ilens, speed=speed, pitch=pitch, energy=energy)
+        return voc(mels, olens, n_iters=n_iters, momentum=momentum, seed=seed)
+
+
 def _no_cpu(*a, **k):
     raise RuntimeError("fs2_b200 operators run on CUDA tensors only (the H100 path has no CPU fallback)")
 
@@ -108,10 +123,12 @@ _LIB.impl("inference", _inference, "CUDA")
 _LIB.impl("inference_batch", _inference_batch, "CUDA")
 _LIB.impl("synthesize_batch", _synthesize_batch, "CUDA")
 _LIB.impl("synthesize_controlled", _synthesize_controlled, "CUDA")
+_LIB.impl("synthesize_audio", _synthesize_audio, "CUDA")
 _LIB.impl("inference", _no_cpu, "CPU")
 _LIB.impl("inference_batch", _no_cpu, "CPU")
 _LIB.impl("synthesize_batch", _no_cpu, "CPU")
 _LIB.impl("synthesize_controlled", _no_cpu, "CPU")
+_LIB.impl("synthesize_audio", _no_cpu, "CPU")
 
 
 class ScriptedFastSpeech2(torch.nn.Module):
@@ -151,6 +168,16 @@ class ScriptedFastSpeech2(torch.nn.Module):
         Equal to FeedForwardTransformer.synthesize with the same controls."""
         return torch.ops.fs2_b200.synthesize_controlled(self.blob, self.keys, self.ranks, self.dims, self.precision, xs,
                                                         ilens, speed, pitch, energy)
+
+    @torch.jit.export
+    def synthesize_audio(self, xs: torch.Tensor, ilens: torch.Tensor, speed: torch.Tensor, pitch: torch.Tensor,
+                         energy: torch.Tensor, n_iters: int = 30, momentum: float = 0.0,
+                         seed: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+        """`synthesize_controlled` followed by the Griffin-Lim vocoder (GriffinLimVocoder with the default config's audio
+        parameters, in this module's precision) -> (audio [B, (Lmax-1)*hop] fp32, alens [B] int64).  Each utterance's
+        audio is independent of its batch mates; audio past alens[b] is 0."""
+        return torch.ops.fs2_b200.synthesize_audio(self.blob, self.keys, self.ranks, self.dims, self.precision, xs, ilens,
+                                                   speed, pitch, energy, n_iters, momentum, seed)
 
 
 def scripted(model: FeedForwardTransformer, precision: Optional[str] = None) -> torch.jit.ScriptModule:

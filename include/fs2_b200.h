@@ -315,6 +315,41 @@ int fs2_stft_magphase(const float* spec, int ld, int B, int cutoff, int frames, 
 int fs2_istft_recombine(const float* mag, const float* phase, int B, int cutoff, int frames, int ld, float* rec, void* stream);
 int fs2_istft_overlap_add(const float* frames_out, int B, int n_fft, int hop, int frames, const float* window_sum, float tiny, float* y, void* stream);
 
+/* ---- batched waveform synthesis: mel inversion + per-utterance Griffin-Lim (DESIGN.md section 7) -------------------- */
+/* From the model's log-mels [B, Lmax, n_mels] with frame counts olens [B] to audio [B, (Lmax-1)*hop]:
+ *   M[b, f, :] = max(0, P . exp(mels[b, f, :])) for f < olens[b] (P = pinv(mel filterbank), [cutoff = n_fft/2+1, n_mels]);
+ *   y = ISTFT(M (.) u), then n_iters x { Z = STFT(y); Zh = Z - momentum/(1+momentum) Z_prev; u = Zh/|Zh| ((1,0) where
+ *   Zh == 0); Z_prev = Z; y = ISTFT(M (.) u) }, each utterance over its own olens[b] frames (reflect padding and window
+ *   sum at its own edges).  u at the start: the phasors of `angles` [B, cutoff, Lmax] (radians), or drawn from
+ *   Philox4x32-10 keyed by seeds[b] with counter f * cutoff + c.  audio[b, s] = 0 for s >= (olens[b]-1)*hop; utterance b
+ *   is bit-identical to a B = 1 call on its own frames.  No allocation, no synchronisation: calls can be graph-captured.
+ * Data-dependent checks run on the device and are reported in *status (device int, zeroed by the call):
+ *   FS2_VOC_BAD_LENGTH  some olens[b] outside [1, Lmax] or with (olens[b]-1)*hop <= n_fft/2 (too short for reflect
+ *                       padding); such an utterance's audio is 0;
+ *   FS2_VOC_RANGE       an fp16 operand plane (f16 / 3xF16 modes) would saturate: some exp(mel), |M (.) u| or |y| above
+ *                       65504 / kPlaneScale (4094).  Magnitudes of a signal within [-1, 1] are at most n_fft/2. */
+#define FS2_VOC_BAD_LENGTH 1
+#define FS2_VOC_RANGE 2
+typedef struct fs2_vocoder fs2_vocoder;
+typedef struct fs2_vocoder_config {
+  int32_t n_fft, hop, win_length, n_mels;
+  int32_t math_mode;   /* FS2_MATH_*: the three GEMMs (mel inversion, inverse and forward DFT) */
+} fs2_vocoder_config;
+/* on the current device */
+int fs2_vocoder_create(fs2_vocoder** out, const fs2_vocoder_config* cfg);
+void fs2_vocoder_destroy(fs2_vocoder* v);
+/* device fp32: w_forward / w_inverse [2*cutoff, n_fft] (windowed Fourier basis and its scaled pseudo-inverse, the
+ * reference STFT's forward_basis / inverse_basis), mel_inverse [cutoff, n_mels], window_sq [n_fft] (squared padded window) */
+int fs2_vocoder_load(fs2_vocoder* v, const float* w_forward, const float* w_inverse, const float* mel_inverse, const float* window_sq,
+                     void* stream);
+int fs2_vocoder_workspace_bytes(fs2_vocoder* v, int B, int Lmax, size_t* bytes);
+/* mag_out [B, cutoff, Lmax] = M (the reference's [B, freq, frames] layout), 0 at frames >= olens[b] */
+int fs2_mel_magnitude(fs2_vocoder* v, const float* mels, const int64_t* olens, int B, int Lmax, float* mag_out, int* status,
+                      void* ws, size_t ws_bytes, void* stream);
+/* seeds [B] (used when angles == NULL) or angles [B, cutoff, Lmax]; momentum in [0, 1); audio [B, (Lmax-1)*hop] */
+int fs2_griffin_lim(fs2_vocoder* v, const float* mels, const int64_t* olens, int B, int Lmax, int n_iters, float momentum,
+                    const int64_t* seeds, const float* angles, float* audio, int* status, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- multi-GPU exchange step: gather of the final mel shards on one rank over NVLink peer memory ----------------- */
 /* Replaces what a reference user would write as torch.distributed.gather / all_gather of `after_outs` (the reference has
  * no multi-GPU path; SURVEY.md section 8e defines the step).  The root rank owns one receive buffer and exports it with
