@@ -42,6 +42,7 @@ class VocoderConfig(C.Structure):
 
 
 FS2_VOC_BAD_LENGTH, FS2_VOC_RANGE = 1, 2     # bits of fs2_griffin_lim's / fs2_mel_magnitude's device status word
+FS2_MELGAN_BAD_LENGTH, FS2_MELGAN_RANGE = 1, 2   # bits of fs2_melgan's device status word
 
 _P, _I, _F, _L, _SZ = C.c_void_p, C.c_int, C.c_float, C.c_int64, C.c_size_t
 
@@ -103,6 +104,10 @@ SIGNATURES = {
     "fs2_vocoder_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
     "fs2_mel_magnitude": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
     "fs2_griffin_lim": [_P, _P, _P, _I, _I, _I, _F, _P, _P, _P, _P, _P, _SZ, _P],
+    "fs2_melgan_create": [C.POINTER(_P), _I],
+    "fs2_melgan_load": [_P, C.POINTER(_P), C.POINTER(_P), _P],
+    "fs2_melgan_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_melgan": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
     "fs2_peer_alloc": [_SZ, C.POINTER(_P), _P],
     "fs2_peer_free": [_P],
     "fs2_peer_open": [_P, C.POINTER(_P)],
@@ -111,7 +116,8 @@ SIGNATURES = {
     "fs2_flag_signal": [_P, _L, _P],
     "fs2_flag_wait": [_P, _I, _I, _L, _P],
 }
-OTHER_SYMBOLS = ("fs2_last_error", "fs2_version", "fs2_destroy", "fs2_kernel_launches", "fs2_profile_label", "fs2_vocoder_destroy")
+OTHER_SYMBOLS = ("fs2_last_error", "fs2_version", "fs2_destroy", "fs2_kernel_launches", "fs2_profile_label", "fs2_vocoder_destroy",
+                 "fs2_melgan_destroy")
 ALL_SYMBOLS = tuple(SIGNATURES) + OTHER_SYMBOLS
 
 _lib: Optional[C.CDLL] = None
@@ -143,6 +149,8 @@ def load() -> C.CDLL:
     lib.fs2_destroy.argtypes = [_P]
     lib.fs2_vocoder_destroy.restype = None
     lib.fs2_vocoder_destroy.argtypes = [_P]
+    lib.fs2_melgan_destroy.restype = None
+    lib.fs2_melgan_destroy.argtypes = [_P]
     _lib = lib
     return lib
 

@@ -22,17 +22,15 @@
 #include <math.h>
 #include <string.h>
 
-#include "common.cuh"
+#include "operand_planes.cuh"
 
 struct fs2_vocoder;
 
 namespace fs2 {
 namespace {
 
-constexpr float kPlaneMax = 65504.0f / kPlaneScale;   // largest |x| an operand plane holds without saturating
 constexpr int FPB = 8;                                 // output frames per ola_frame CTA
 
-enum OutKind { OUT_F32 = 0, OUT_HI = 1, OUT_HILO = 2 };   // GEMM operand as fp32 rows / hi plane / hi + lo planes
 
 inline int grid_for(long n, int block, int cap = 132 * 8) {
   long g = (n + block - 1) / block;
@@ -260,7 +258,6 @@ GlPlan plan(const fs2_vocoder* v, Bump& b, int B, int L, bool momentum_state) {
   return p;
 }
 
-int out_kind(int mode) { return mode == FS2_MATH_3XTF32 ? OUT_HILO : mode == FS2_MATH_F16 ? OUT_HI : OUT_F32; }
 
 // out [rows][w.N] = act(a [rows][w.K] . w^T), rows t >= lens[b] written as 0 (and skipped by the tensor-core kernel)
 int gemm(const fs2_vocoder* v, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens, float* out, cudaStream_t st) {
@@ -279,8 +276,6 @@ int gemm(const fs2_vocoder* v, const VWeight& w, const void* a, int B, int L, in
   return tap_gemm_planes(g, st);
 }
 
-template <typename K3, typename K2, typename K1>
-K1 pick(int kind, K3 k3, K2 k2, K1 k1) { return kind == OUT_HILO ? k3 : kind == OUT_HI ? k2 : k1; }
 
 int mel_stage(fs2_vocoder* v, const float* mels, const int64_t* olens, int B, int L, const GlPlan& p, int* status, cudaStream_t st) {
   const int kind = out_kind(v->cfg.math_mode), nm = v->cfg.n_mels;

@@ -7,6 +7,10 @@ Why a launcher: `python inference.py` puts the script's own directory first on `
 `fastspeech.py` (same directory) always wins over a `PYTHONPATH` entry.  This module puts `<repo>/dropin` (a module named
 `fastspeech` that re-exports our class) in front of the script directory and then executes the script as `__main__`.
 The other way to switch over is to copy `dropin/fastspeech.py` over the checkout's `fastspeech.py`.
+
+With FS2_MELGAN_CHECKPOINT=<file> (seungwonpark/melgan's checkpoint, or a bare generator state dict) the launcher also makes
+`torch.hub.load("seungwonpark/melgan", "melgan")` return `MelGANVocoder.from_checkpoint(<file>)`, so the reference's
+inference.py and train_fastspeech.py reach MelGAN audio without a network.  Every other `torch.hub.load` call is passed on.
 """
 from __future__ import annotations
 
@@ -15,6 +19,25 @@ import runpy
 import sys
 
 DROPIN_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "dropin")
+MELGAN_ENV = "FS2_MELGAN_CHECKPOINT"
+MELGAN_REPO, MELGAN_MODEL = "seungwonpark/melgan", "melgan"
+
+
+def install_melgan_hub(checkpoint: str) -> None:
+    """Route `torch.hub.load("seungwonpark/melgan", "melgan", ...)` (any branch suffix, e.g. ":master") to
+    `MelGANVocoder.from_checkpoint(checkpoint)`; every other call goes to the original `torch.hub.load`."""
+    import torch
+
+    original = getattr(torch.hub.load, "_fs2_original", torch.hub.load)
+
+    def load(repo_or_dir, model, *args, **kwargs):
+        if isinstance(repo_or_dir, str) and repo_or_dir.split(":")[0] == MELGAN_REPO and model == MELGAN_MODEL:
+            from fastspeech2_b200.melgan import MelGANVocoder
+            return MelGANVocoder.from_checkpoint(checkpoint)
+        return original(repo_or_dir, model, *args, **kwargs)
+
+    load._fs2_original = original
+    torch.hub.load = load
 
 
 def main(argv=None) -> None:
@@ -29,6 +52,8 @@ def main(argv=None) -> None:
     sys.path[:] = front + [p for p in sys.path if p not in front and p != ""]
     sys.modules.pop("fastspeech", None)
     sys.argv = [script] + argv[1:]
+    if os.environ.get(MELGAN_ENV):
+        install_melgan_hub(os.environ[MELGAN_ENV])
     runpy.run_path(script, run_name="__main__")
 
 

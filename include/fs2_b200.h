@@ -350,6 +350,32 @@ int fs2_mel_magnitude(fs2_vocoder* v, const float* mels, const int64_t* olens, i
 int fs2_griffin_lim(fs2_vocoder* v, const float* mels, const int64_t* olens, int B, int Lmax, int n_iters, float momentum,
                     const int64_t* seeds, const float* angles, float* audio, int* status, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- batched MelGAN vocoder (DESIGN.md section 8) ------------------------------------------------------------------- */
+/* seungwonpark/melgan's Generator(mel_channel = 80) on log-mels [B, Lmax, 80] with frame counts olens [B]: utterance b is
+ * the generator applied to its own frames mels[b, :olens[b]] followed by 10 frames of -11.5129, every reflection pad at its
+ * own edges, trimmed to olens[b] * 256 samples.  audio [B, Lmax * 256] fp32, 0 from olens[b] * 256 on; audio[b] is
+ * bit-identical to a B = 1 call on its own frames; mel frames past olens[b] are never read.  No allocation, no
+ * synchronisation: a call can be graph-captured.  It enqueues 60 kernels.
+ * Data-dependent checks run on the device and are reported in *status (device int, written by the call):
+ *   FS2_MELGAN_BAD_LENGTH  some olens[b] outside [1, Lmax]; that utterance's audio is 0;
+ *   FS2_MELGAN_RANGE       an fp16 operand plane (f16 / 3xF16 modes) would saturate: some GEMM input above 65504 /
+ *                          kPlaneScale (4094) in magnitude. */
+#define FS2_MELGAN_BAD_LENGTH 1
+#define FS2_MELGAN_RANGE 2
+typedef struct fs2_melgan_gen fs2_melgan_gen;
+/* on the current device; math_mode FS2_MATH_*: every GEMM of the generator (the last conv runs on CUDA cores in fp32) */
+int fs2_melgan_create(fs2_melgan_gen** out, int math_mode);
+void fs2_melgan_destroy(fs2_melgan_gen* m);
+/* weights[42], biases[42]: device fp32 tensors of the 42 convolutions in state_dict order (generator.1, generator.3,
+ * generator.4.blocks.{0,1,2}.{2,4}, generator.4.shortcuts.{0,1,2}, generator.6, ... generator.16), weight norm already
+ * folded (w = g * v / |v|), in torch's layouts: Conv1d [Cout, Cin, k], ConvTranspose1d [Cin, Cout, k].  Packed once into
+ * the GEMM layouts; the tensors may be freed afterwards (stream order). */
+int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float* const* biases, void* stream);
+/* fails (FS2_ERR_INVALID) when B * (Lmax + 10) * 256 reaches 2^31, or 65535 * 128 in FS2_MATH_FP32 */
+int fs2_melgan_workspace_bytes(fs2_melgan_gen* m, int B, int Lmax, size_t* bytes);
+int fs2_melgan(fs2_melgan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
+               size_t ws_bytes, void* stream);
+
 /* ---- multi-GPU exchange step: gather of the final mel shards on one rank over NVLink peer memory ----------------- */
 /* Replaces what a reference user would write as torch.distributed.gather / all_gather of `after_outs` (the reference has
  * no multi-GPU path; SURVEY.md section 8e defines the step).  The root rank owns one receive buffer and exports it with
