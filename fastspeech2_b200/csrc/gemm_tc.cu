@@ -22,10 +22,15 @@
 // 4 MMAs with K = 8 each (tf32; f16: ceil(K / 64) steps with K = 16 each: one 128-byte swizzle row either way).
 //
 // One persistent CTA per SM walks the 128 x BN output tiles (n fastest, so concurrently running CTAs share weight tiles
-// in L2).  Warp roles (3 warpgroups): warp 0 is the TMA producer; warpgroups 1 and 2 each own 64 rows of the tile, issue
-// their wgmma chain on every ring stage and release the stage as soon as the MMAs that read it have completed (one stage
-// stays in flight), then run the epilogue straight from the accumulator registers (bias / ReLU / tanh / residual, fp32
-// rows, operand planes, or the transposed V third) while the producer already fills the ring with the next tile.
+// in L2).  Warp roles (3 warpgroups): warp 0 is the TMA producer, filling one ordered ring of stages for the CTA's tiles
+// in turn; warpgroups 1 and 2 "ping-pong": the CTA's k-th tile belongs wholly to warpgroup k & 1, which issues the wgmma
+// chains of both 64-row halves on each of the tile's ring stages (BN accumulator registers per thread; setmaxnreg moves
+// registers from the producer warpgroup), releases a stage as soon as the MMAs that read it have completed (one stage
+// stays in flight), then runs the epilogue straight from the accumulator registers (bias / ReLU / tanh / residual, fp32
+// rows, operand planes, or the transposed V third) while the other warpgroup already issues the next tile's MMAs.  An
+// mbarrier pair makes the two main loops strictly alternate (see the consumer loop), so the tensor cores do not wait for
+// an epilogue.  A row's K loop (the MMAs that accumulate it, and their order) depends neither on its tile nor on the
+// warpgroup, so results do not depend on the schedule (per-utterance bit-identity, DESIGN.md §5).
 // Convolutions tile each utterance separately so the shifted boxes never cross an utterance boundary: floor(L/128) full
 // row tiles per utterance, and the tails (L % 128 rows, in 16-row granules loaded by separate small TMA boxes) of several
 // utterances packed into shared tiles, so no tensor-core rows are spent on padding.  Plain GEMMs (taps == 1) tile the flat
@@ -45,6 +50,7 @@ constexpr int BM = 128;
 constexpr int BK = 32;                 // fp32 elements per pipeline step = one 128-byte swizzle row (64 when the operands are fp16)
 constexpr int A_BYTES = BM * BK * 4;   // 16 KB
 constexpr int THREADS = 384;           // producer warpgroup + two consumer warpgroups
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;   // setmaxnreg: 128 * 40 + 256 * 232 <= 65536; a consumer holds BN accumulators
 constexpr int RING_BUDGET = 227 * 1024 - 1024 /*align slack*/ - 256 /*barriers*/;
 
 struct TcParams {
@@ -116,8 +122,11 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   const int steps = p.taps * kchunks;
   const int total_tiles = p.m_tiles * p.n_tiles;
 
+  uint64_t* order_bar = empty_bar + C::STAGES;             // [cg]: the other warpgroup has issued its previous tile's MMAs
+
   if (threadIdx.x == 0) {
-    for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }   // 8 consumer warps release
+    for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }   // the 4 warps of one consumer warpgroup release
+    mbar_init(&order_bar[0], 4); mbar_init(&order_bar[1], 4);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -135,7 +144,9 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     return packed < 0 && p.lens != nullptr && t0 >= p.lens[b];
   };
 
-  if (warp == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp != 0) { pdl_trigger(); return; }
     // ---- TMA producer: the whole warp runs the loop, one lane is elected inside each asm; everything a stage's loads need
     // is computed before the wait for its slot, and the tap / K-chunk indices are carried as counters
     const uint32_t tiles_addr = smem_u32(tiles), full_addr = smem_u32(full_bar);
@@ -169,23 +180,26 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         if (++kc == kchunks) { kc = 0; ++j; }
       }
     }
-  } else if (warp >= 4) {
-    // ---- consumers: warpgroup cg = 0 / 1 owns tile rows 64 cg .. 64 cg + 63 ----
+  } else {
+    // ---- consumers: warpgroup cg = 0 / 1 owns every other tile of the CTA (its k-th tile goes to k & 1), all 128 rows ----
+    setmaxnreg_inc<CONSUMER_REGS>();
     const int cg = (warp >> 2) - 1, wq = warp & 3;
-    const int r_lo = 64 * cg + 16 * wq + (lane >> 2);        // this thread's rows r_lo and r_lo + 8; columns 8 j + 2 (lane % 4)
+    const int r_lo = 16 * wq + (lane >> 2);      // rows 64 hf + r_lo + 8 h of the tile (hf, h = 0 / 1); columns 8 j + 2 (lane % 4)
     const int act = p.act, ldr = p.ldr, ldo = p.ldo;
     const float* __restrict__ resid = p.resid; float* __restrict__ out = p.out;
     const bool has_res = resid != nullptr;
     const float oscale = p.a_inv * (p.w_inv ? __ldg(p.w_inv) : 1.0f);   // exact power of two (1 in the tf32 family)
-    float d[BN / 2];
-    int n = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    float d[BN];                                  // [hf][BN / 2]: the accumulators of the tile's two 64-row halves
+    int n = 0;                                    // ring position: advanced past the other warpgroup's tiles as well
+    int k = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++k) {
       int n0, b, t0, packed;
       const int tile_steps = tile_coords(tile, n0, b, t0, packed) ? 0 : steps;
-      long m[2]; bool row_ok[2], row_zero[2];
+      if ((k & 1) != cg) { n += tile_steps; continue; }
+      long m[4]; bool row_ok[4], row_zero[4];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r_lo + 8 * h;
+      for (int i = 0; i < 4; ++i) {              // i = 2 hf + h
+        const int row = 64 * (i >> 1) + r_lo + 8 * (i & 1);
         int bb = b, t = t0 + row;
         bool ok = t < p.L;                       // flat mode: L == total rows
         if (packed >= 0) {                       // packed tail tile: 16-row granule g of the tile -> utterance b + g / gn
@@ -194,59 +208,90 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           t = t0 + gi * 16 + (row & 15);
           ok = u < p.upt && bb < p.B && t < p.L;
         }
-        m[h] = (long)bb * p.L + t; row_ok[h] = ok;
-        row_zero[h] = ok && p.lens != nullptr && t >= p.lens[bb];
-        if (has_res && ok) prefetch_l2(resid + m[h] * ldr + n0);   // residual rows -> L2 while the main loop runs
+        m[i] = (long)bb * p.L + t; row_ok[i] = ok;
+        row_zero[i] = ok && p.lens != nullptr && t >= p.lens[bb];
+        if (has_res && ok) prefetch_l2(resid + m[i] * ldr + n0);   // residual rows -> L2 while the main loop runs
       }
+      // Main loops alternate between the warpgroups: this tile's starts once the other warpgroup has issued the MMAs of the
+      // CTA's previous tile (it arrives even for a dead tile).  That keeps the tensor cores fed by one warpgroup while the
+      // other runs its epilogue, and it is what makes the parity waits below sound: every ring position before this tile
+      // has been filled, so the producer is never a whole ring round behind the position waited for.
+      if (k > 0) mbar_wait(&order_bar[cg], ((k - 1) >> 1) & 1);
       int prev = -1;
       for (int s = 0; s < tile_steps; ++s, ++n) {
         const int slot = n % C::STAGES, round = n / C::STAGES;
         const uint32_t base = smem_u32(tiles + (size_t)slot * C::STAGE_BYTES);
-        const uint64_t a_hi = make_sw128_kmajor_desc(base + cg * (A_BYTES / 2)), b_hi = make_sw128_kmajor_desc(base + C::B_HI);
-        const uint64_t a_lo = make_sw128_kmajor_desc(base + C::A_LO + cg * (A_BYTES / 2)), b_lo = make_sw128_kmajor_desc(base + C::B_LO);
+        const uint64_t a_hi = make_sw128_kmajor_desc(base), b_hi = make_sw128_kmajor_desc(base + C::B_HI);
+        const uint64_t a_lo = make_sw128_kmajor_desc(base + C::A_LO), b_lo = make_sw128_kmajor_desc(base + C::B_LO);
+        constexpr uint64_t HALF_A = (A_BYTES / 2) >> 4;   // second 64-row half of the A tile, in descriptor units
         mbar_wait(&full_bar[slot], round & 1);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {            // +32 bytes along K inside the swizzle row = +2 in descriptor units
-          if (PRECISE) {
-            mma_tile<BN, true>(d, a_lo + 2 * k, b_hi + 2 * k, (s | k) != 0);   // small terms first
-            mma_tile<BN, true>(d, a_hi + 2 * k, b_lo + 2 * k, 1);
-            mma_tile<BN, true>(d, a_hi + 2 * k, b_hi + 2 * k, 1);
-          } else {
-            mma_tile<BN, HALF>(d, a_hi + 2 * k, b_hi + 2 * k, (s | k) != 0);
+        for (int kk = 0; kk < 4; ++kk) {         // +32 bytes along K inside the swizzle row = +2 in descriptor units
+#pragma unroll
+          for (int hf = 0; hf < 2; ++hf) {
+            float* dh = d + hf * (BN / 2);
+            if (PRECISE) {
+              mma_tile<BN, true>(dh, a_lo + hf * HALF_A + 2 * kk, b_hi + 2 * kk, (s | kk) != 0);   // small terms first
+              mma_tile<BN, true>(dh, a_hi + hf * HALF_A + 2 * kk, b_lo + 2 * kk, 1);
+              mma_tile<BN, true>(dh, a_hi + hf * HALF_A + 2 * kk, b_hi + 2 * kk, 1);
+            } else {
+              mma_tile<BN, HALF>(dh, a_hi + hf * HALF_A + 2 * kk, b_hi + 2 * kk, (s | kk) != 0);
+            }
           }
         }
         wgmma_commit();
         wgmma_wait<1>();                         // the previous stage's MMAs are done: release its slot
-        pin_regs<BN / 2>(d);
+        pin_regs<BN>(d);
         if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
         prev = slot;
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&order_bar[cg ^ 1]);   // the other warpgroup's next main loop may start
       wgmma_wait<0>();
-      pin_regs<BN / 2>(d);
+      pin_regs<BN>(d);
       if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
       if (tile_steps == 0) {
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+        for (int i = 0; i < BN; ++i) d[i] = 0.f;
       }
 
       // ---- epilogue from registers: element pairs (row, columns c, c + 1) ----
+      // Row by row, every load of a row (bias, residual) is issued before its first store: as far as the compiler knows,
+      // the stores may alias the loads, so interleaving them would serialise one load latency per column pair.
       const bool to_vt = (p.vt_out != nullptr || p.vtp != nullptr) && n0 >= p.vt_col0;   // tile-uniform (tile widths divide the V third)
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (!row_ok[h] || (to_vt && row_zero[h])) continue;
-        const long mm = m[h];
+      for (int i = 0; i < 4; ++i) {
+        if (!row_ok[i] || (to_vt && row_zero[i])) continue;
+        const long mm = m[i];
+        float* dr = d + (i >> 1) * (BN / 2) + 2 * (i & 1);   // this row's pairs: dr[4 jj], dr[4 jj + 1]
 #pragma unroll
         for (int jj = 0; jj < BN / 8; ++jj) {
-          const int c = 8 * jj + 2 * (lane & 3), col = n0 + c;
-          float v0 = d[4 * jj + 2 * h], v1 = d[4 * jj + 2 * h + 1];
+          const int col = n0 + 8 * jj + 2 * (lane & 3);
+          float v0 = dr[4 * jj], v1 = dr[4 * jj + 1];
           const float b0 = p.bias ? __ldg(p.bias + col) : 0.f, b1 = p.bias ? __ldg(p.bias + col + 1) : 0.f;
           v0 = fmaf(v0, oscale, b0); v1 = fmaf(v1, oscale, b1);
-          if (to_vt) {
-            // transposed store: for a fixed column the 8 row groups of a warp hold consecutive time steps
-            const long ub = mm / p.vt_L; const int ut = (int)(mm - ub * p.vt_L);
-            const int rel = col - p.vt_col0, hh = rel / p.vt_dk, d0 = rel - hh * p.vt_dk;
-            const long o = ((ub * p.vt_heads + hh) * p.vt_dk + d0) * (long)p.vt_lpad + ut;
+          if (!to_vt) {
+            if (act == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            else if (act == ACT_TANH) { v0 = tanhf(v0); v1 = tanhf(v1); }
+            if (has_res) {
+              const float2 r = __ldg(reinterpret_cast<const float2*>(resid + mm * ldr + col));
+              v0 += r.x; v1 += r.y;
+            }
+            if (row_zero[i]) { v0 = 0.f; v1 = 0.f; }
+          }
+          dr[4 * jj] = v0; dr[4 * jj + 1] = v1;
+        }
+        if (to_vt) {
+          // transposed store: for a fixed column the 8 row groups of a warp hold consecutive time steps.
+          // vt[(ub * heads + h) * dk + d][ut] with h * dk + d = col - vt_col0
+          const long ub = mm / p.vt_L;
+          const long orow = ub * p.vt_heads * p.vt_dk * (long)p.vt_lpad + (mm - ub * p.vt_L);
+#pragma unroll
+          for (int jj = 0; jj < BN / 8; ++jj) {
+            const int col = n0 + 8 * jj + 2 * (lane & 3);
+            const float v0 = dr[4 * jj], v1 = dr[4 * jj + 1];
+            const long o = orow + (long)(col - p.vt_col0) * p.vt_lpad;
             if (p.vt_out != nullptr) {
               p.vt_out[o] = v0; p.vt_out[o + p.vt_lpad] = v1;
             } else {
@@ -256,15 +301,13 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
               p.vtp[o] = __low2half(h2); p.vtp[o + p.vt_lpad] = __high2half(h2);
               if (p.vtp_lo != nullptr) { p.vtp_lo[o] = __low2half(l2); p.vtp_lo[o + p.vt_lpad] = __high2half(l2); }
             }
-            continue;
           }
-          if (act == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-          else if (act == ACT_TANH) { v0 = tanhf(v0); v1 = tanhf(v1); }
-          if (has_res) {
-            const float2 r = __ldg(reinterpret_cast<const float2*>(resid + mm * ldr + col));
-            v0 += r.x; v1 += r.y;
-          }
-          if (row_zero[h]) { v0 = 0.f; v1 = 0.f; }
+          continue;
+        }
+#pragma unroll
+        for (int jj = 0; jj < BN / 8; ++jj) {
+          const int col = n0 + 8 * jj + 2 * (lane & 3);
+          const float v0 = dr[4 * jj], v1 = dr[4 * jj + 1];
           if (HALF && p.outp != nullptr) {       // operand planes of the next contraction
             const long off = mm * p.ldo_p + col;
             if (p.outp_lo != nullptr) {
