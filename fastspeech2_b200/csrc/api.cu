@@ -771,16 +771,40 @@ struct TempPlanes {
 
 int fs2_op_tap_gemm(int math_mode, const float* x, int B, int L, int K, const float* w, const float* bias, int N, int taps,
                     int act, const float* resid, float* out, void* stream) {
-  FS2_REQUIRE(x && w && out, "fs2_op_tap_gemm: null argument");
+  return fs2_op_tap_gemm_ex(math_mode, x, B, L, K, w, bias, N, taps, act, resid, nullptr, out, nullptr, 0, 0, nullptr, 0,
+                            stream);
+}
+int fs2_op_tap_gemm_ex(int math_mode, const float* x, int B, int L, int K, const float* w, const float* bias, int N,
+                       int taps, int act, const float* resid, const int64_t* lens, float* out, void* out_planes,
+                       int vt_col0, int vt_heads, void* vt, int vt_lpad, void* stream) {
+  const char* who = "fs2_op_tap_gemm";
+  FS2_REQUIRE(math_mode == FS2_MATH_FP32 || math_mode == FS2_MATH_TF32 || math_mode == FS2_MATH_F16 || math_mode == FS2_MATH_3XTF32,
+              "%s: unknown math mode %d", who, math_mode);
+  const bool planes = math_mode == FS2_MATH_F16 || math_mode == FS2_MATH_3XTF32;
+  FS2_REQUIRE(x && w && (out || (planes && (out_planes || vt))), "%s: null argument", who);
+  FS2_REQUIRE(B >= 0 && L >= 0 && K > 0 && N > 0 && taps > 0, "%s: bad shape B=%d L=%d K=%d N=%d taps=%d", who, B, L, K, N, taps);
+  FS2_REQUIRE(!out_planes || planes, "%s: out_planes needs FS2_MATH_F16 or FS2_MATH_3XTF32", who);
+  FS2_REQUIRE(!vt || math_mode != FS2_MATH_FP32, "%s: the fp32 family has no transposed V output", who);
+  FS2_REQUIRE(!vt || (vt_heads > 0 && vt_col0 >= 0 && vt_col0 < N && (N - vt_col0) % vt_heads == 0 && vt_lpad >= L),
+              "%s: transposed V needs 0 <= vt_col0 < N, heads dividing N - vt_col0 and vt_lpad >= L", who);
   Dense d; d.w = w; d.bias = bias; d.N = N; d.K = K; d.taps = taps;
   cudaStream_t st = (cudaStream_t)stream;
-  if (math_mode == FS2_MATH_FP32 || math_mode == FS2_MATH_TF32)
-    return dense(make_gemm(d, x, K, B, L, act, resid, N, out, N), math_mode, st, P_DEC_W1);
+  TapGemm g;
   TempPlanes t;
-  int rc = t.make(x, (long)B * L, K, w, (long)N * K * taps, st);
-  if (rc) return rc;
-  d.w_hi = t.w_hi; d.w_lo = t.w_lo; d.w_inv = t.sc + 1;
-  return dense(make_gemm_p(d, t.xp, B, L, math_mode == MATH_3XTF32, act, resid, N, out, N), math_mode, st, P_DEC_W1);
+  if (planes) {
+    int rc = t.make(x, (long)B * L, K, w, (long)N * K * taps, st);
+    if (rc) return rc;
+    d.w_hi = t.w_hi; d.w_lo = t.w_lo; d.w_inv = t.sc + 1;
+    g = make_gemm_p(d, t.xp, B, L, math_mode == MATH_3XTF32, act, resid, N, out, N);
+    planes_out(g, reinterpret_cast<__half*>(out_planes), N, math_mode == MATH_3XTF32);   // the lo flag covers vt's lo plane too
+  } else {
+    g = make_gemm(d, x, K, B, L, act, resid, N, out, N);
+  }
+  if (vt) {
+    g.vt_col0 = vt_col0; g.vt_heads = vt_heads; g.vt_dk = (N - vt_col0) / vt_heads; g.vt_lpad = vt_lpad;
+    if (planes) g.vtp = reinterpret_cast<__half*>(vt); else g.vt_out = reinterpret_cast<float*>(vt);
+  }
+  return dense(masked(g, lens), math_mode, st, P_DEC_W1);
 }
 int fs2_op_gemm_layernorm(int math_mode, const float* x, int64_t rows, int K, int N, const float* w, const float* bias, const float* resid,
                           const float* gamma, const float* beta, float eps, float* out, float* out_planes, void* stream) {

@@ -67,10 +67,10 @@ struct TcParams {
   // optional: columns >= vt_col0 are the V third of a q|k|v projection and are stored transposed,
   // vt[(b*heads + h)*dk + d][t] with row pitch vt_lpad, for the attention kernel's P.V operand
   float* vt_out; __half* vtp; __half* vtp_lo; int vt_col0, vt_dk, vt_heads, vt_lpad, vt_L;
-  // per-utterance mode (nullable; needs the per-utterance tiling): rows t >= lens[b] are written as exact zeros, and an
-  // ordinary tile with t0 >= lens[b] is dead -- no TMA loads, no MMAs, only the zero stores.  The V third and the q|k
-  // planes of those rows are not needed as zeros (the attention kernels read no key or query row past len), so dead
-  // tiles leave them unwritten and live tiles skip the transposed V stores for them.
+  // per-utterance mode (nullable; needs the per-utterance tiling): rows t >= lens[b] are written as exact zeros in every
+  // non-V column, fp32 rows and planes alike, and an ordinary tile with t0 >= lens[b] is dead -- no TMA loads, no MMAs,
+  // only those zero stores.  The transposed V third of those rows is not needed (the attention kernels read no key row
+  // past len), so dead and live tiles alike skip its stores there.
   const int64_t* lens;
 };
 
@@ -436,6 +436,7 @@ int check_common(const TapGemm& g, const char* who) {
 int tap_gemm_tf32(const TapGemm& g, cudaStream_t st) {
   int rc = check_common(g, "tap_gemm_tf32");
   if (rc) return rc;
+  FS2_REQUIRE(!g.vt_out || g.vt_col0 % tile_width(g.N) == 0, "tap_gemm_tf32: the transposed V third must start at a tile boundary");
   if ((long)g.B * g.L == 0) return FS2_OK;
   return launch_any<false, false>(g, st);
 }

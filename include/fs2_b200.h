@@ -227,6 +227,23 @@ int fs2_one_hot(const int64_t* ids, int64_t n, int n_bins, float* out, void* str
  * act: 0 none, 1 relu, 2 tanh */
 int fs2_op_tap_gemm(int math_mode, const float* x, int B, int L, int K, const float* w, const float* bias, int N, int taps,
                     int act, const float* resid, float* out, void* stream);
+/* fs2_op_tap_gemm with the rest of the kernel's epilogue; fs2_op_tap_gemm is this call with every new argument NULL / 0.
+ *   lens [B] i64 (device) or NULL: per-utterance mode, as in the FS2_PER_UTTERANCE stages.  Rows t >= lens[b] are written
+ *        as exact zeros (out and planes), and the tensor-core families skip the MMAs of 128-row tiles wholly past
+ *        lens[b].  Values lie in [0, L]; a convolution's (taps > 1) input must hold zeros at rows t >= lens[b].
+ *   out  may be NULL in FS2_MATH_F16 / FS2_MATH_3XTF32 when out_planes or vt is given.
+ *   out_planes (FS2_MATH_F16 / FS2_MATH_3XTF32 only) fp16 [P][B*L][N], P = 2 in FS2_MATH_3XTF32 (hi, lo) and 1 in
+ *        FS2_MATH_F16 (hi): the result as the operand planes of a next contraction, scaled by 16.
+ *   vt   (tensor-core families only) with vt_col0, vt_heads, vt_lpad: columns >= vt_col0 (the V third of a q|k|v
+ *        projection) get the bias only and are stored transposed, vt[(b*vt_heads + h)*dk + d][t] with
+ *        h*dk + d = n - vt_col0, dk = (N - vt_col0) / vt_heads and row pitch vt_lpad >= L, instead of in out /
+ *        out_planes; entries at t >= lens[b] and t >= L are not written.  FS2_MATH_TF32: fp32 [B*vt_heads][dk][vt_lpad];
+ *        the plane families: fp16 planes [P][B*vt_heads][dk][vt_lpad] scaled by 16 (vt_lpad % 8 == 0, dk % 32 == 0).
+ *        vt_col0 must be a multiple of the kernel's tile width (the largest of 128, 80, 64, 32, 16 dividing N).
+ * FS2_MATH_FP32 accepts lens and rejects out_planes and vt with FS2_ERR_INVALID. */
+int fs2_op_tap_gemm_ex(int math_mode, const float* x, int B, int L, int K, const float* w, const float* bias, int N,
+                       int taps, int act, const float* resid, const int64_t* lens, float* out, void* out_planes,
+                       int vt_col0, int vt_heads, void* vt, int vt_lpad, void* stream);
 /* out = LayerNorm_N(x . w^T + bias + resid) * gamma + beta as a tensor-core GEMM followed by the row LayerNorm kernel (x [rows,K], w [N,K]);
  * the form of core/encoder.py:60-62 / :67-69: FS2_MATH_TF32 (tf32 on the fp32 rows, N = 384),
  * FS2_MATH_F16 (f16) and FS2_MATH_3XTF32 (error-compensated 3xF16) on operand planes made on the fly here,
