@@ -70,6 +70,7 @@ SIGNATURES = {
     "fs2_op_tap_gemm": [_I, _P, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P],
     "fs2_op_tap_gemm_ex": [_I, _P, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P, _I, _P],
     "fs2_op_attention": [_I, _P, _P, _I, _I, _I, _I, _P, _P],
+    "fs2_op_attention_planes": [_I, _P, _P, _I, _P, _I, _I, _I, _I, _P, _P, _P],
     "fs2_op_gemm_layernorm": [_I, _P, _L, _I, _I, _P, _P, _P, _P, _P, _F, _P, _P, _P],
     "fs2_op_layernorm": [_P, _P, _P, _P, _F, _L, _I, _P, _P],
     "fs2_dropout_mask": [_P, _L, _F, C.c_uint64, C.c_uint64, _P],

@@ -196,9 +196,10 @@ int run_blocks(const std::vector<Block>& blocks, const BlockBufs& w, const int64
                                       : attention_fp32(w.qkv, lens, B, L, C, heads, w.ctx, st);
       if (rc) return rc;
     }
-    // x = LN(x + linear_out(ctx)) (attention.py:74, encoder.py:60-62).  Per-utterance mode: ctx rows past len are not
-    // guaranteed to be zero (the attention kernels scale whatever their query rows produced by 0, and those query rows
-    // may be unwritten); the out-projection reads each ctx row only for its own output row, which it writes as 0 there
+    // x = LN(x + linear_out(ctx)) (attention.py:74, encoder.py:60-62).  Per-utterance mode: ctx rows past len are the
+    // attention kernels' output of those query rows times 0 (the q|k|v projection writes them as zeros, DESIGN.md
+    // section 5, so they are zeros of either sign); the out-projection reads each ctx row only for its own output row,
+    // which it writes as 0 there
     if ((rc = dense(masked(make_gemm(k.out, w.ctx, C, B, L, ACT_NONE, x, C, y, C), zlens), math_mode, st, c_out))) return rc;
     if ((rc = norm_rows(masked(make_norm(k.ln1, y, C, rows, C, x, C), zlens, L), st))) return rc;
     // conv-FFN: hid = relu(conv_k(x)); x = LN(x + conv_1(hid))  (modules.py:247-248, encoder.py:64-69)
@@ -850,6 +851,8 @@ int fs2_op_gemm_layernorm(int math_mode, const float* x, int64_t rows, int K, in
 }
 int fs2_op_attention(int math_mode, const float* qkv, const int64_t* lens, int B, int L, int C, int heads, float* ctx,
                      void* stream) {
+  FS2_REQUIRE(math_mode == FS2_MATH_FP32 || math_mode == FS2_MATH_TF32 || math_mode == FS2_MATH_F16 || math_mode == FS2_MATH_3XTF32,
+              "fs2_op_attention: unknown math mode %d", math_mode);
   FS2_REQUIRE(qkv && ctx, "fs2_op_attention: null argument");
   FS2_REQUIRE(heads > 0 && C % heads == 0, "fs2_op_attention: C=%d not divisible by heads=%d", C, heads);
   cudaStream_t st = (cudaStream_t)stream;
@@ -874,6 +877,16 @@ int fs2_op_attention(int math_mode, const float* qkv, const int64_t* lens, int B
   if (!rc) { ProfScope prof_scope(P_DEC_ATTN, flop, bytes, st); rc = attention_planes(tmp, tmp + nqk, lpad, lens, B, L, C, heads, math_mode == MATH_3XTF32, ctx, nullptr, st); }
   cudaFreeAsync(tmp, st);
   return rc;
+}
+int fs2_op_attention_planes(int math_mode, const void* qkp, const void* vtp, int lpad, const int64_t* lens, int B, int L,
+                            int C, int heads, float* ctx, void* ctxp, void* stream) {
+  FS2_REQUIRE(math_mode == FS2_MATH_F16 || math_mode == FS2_MATH_3XTF32,
+              "fs2_op_attention_planes: unknown math mode %d (operand planes exist in FS2_MATH_F16 and FS2_MATH_3XTF32)", math_mode);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool x3 = math_mode == FS2_MATH_3XTF32;
+  ProfScope prof_scope(P_DEC_ATTN, 4.0 * B * (double)L * L * C, (x3 ? 4.0 : 2.0) * 4.0 * B * (double)L * C, st);
+  return attention_planes(reinterpret_cast<const __half*>(qkp), reinterpret_cast<const __half*>(vtp), lpad, lens, B, L, C,
+                          heads, x3, ctx, reinterpret_cast<__half*>(ctxp), st);
 }
 int fs2_op_layernorm(const float* x, const float* resid, const float* g, const float* b, float eps, int64_t rows, int C,
                      float* out, void* stream) {

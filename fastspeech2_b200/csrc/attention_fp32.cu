@@ -15,7 +15,7 @@
 // Used for the encoder in every mode and for the decoder in FS2_MATH_FP32.
 #include <math.h>
 
-#include "common.cuh"
+#include "tc_common.cuh"   // ensure_smem_attr
 
 namespace fs2 {
 namespace {
@@ -169,12 +169,9 @@ attention_fp32_kernel(const float* __restrict__ qkv, const int64_t* __restrict__
 
 template <int DK>
 int launch(const float* qkv, const int64_t* lens, int B, int L, int C, int heads, float* ctx, cudaStream_t st) {
-  static bool configured = false;
-  if (!configured) {
-    FS2_CUDA_CHECK(cudaFuncSetAttribute(attention_fp32_kernel<DK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)AttnSmem<DK>::bytes));
-    configured = true;
-  }
+  static unsigned long long configured = 0;   // per-device bit mask
+  int rc;
+  if ((rc = tc::ensure_smem_attr(attention_fp32_kernel<DK>, AttnSmem<DK>::bytes, &configured))) return rc;
   dim3 grid((L + BQ - 1) / BQ, heads, B);
   attention_fp32_kernel<DK><<<grid, 256, AttnSmem<DK>::bytes, st>>>(qkv, lens, L, C, ctx, 1.0f / sqrtf((float)DK));
   FS2_LAUNCH_CHECK();

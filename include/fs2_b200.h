@@ -257,6 +257,14 @@ int fs2_op_gemm_layernorm(int math_mode, const float* x, int64_t rows, int K, in
  * FS2_MATH_TF32: tensor-core tf32; FS2_MATH_F16 / FS2_MATH_3XTF32: tensor-core f16 / error-compensated 3xF16 on planes */
 int fs2_op_attention(int math_mode, const float* qkv, const int64_t* lens, int B, int L, int C, int heads, float* ctx,
                      void* stream);
+/* The operand-plane attention on the layouts the model's q|k|v projection writes, all fp16 scaled by 16:
+ *   qkp  q|k planes [P][B*L][2C] (16-byte aligned), P = 2 in FS2_MATH_3XTF32 (hi, lo) and 1 in FS2_MATH_F16 (hi);
+ *   vtp  V^T planes [P][B*heads][d_k][lpad], lpad >= L, lpad % 8 == 0 (16-byte aligned).
+ * Outputs (at least one): ctx fp32 [B,L,C] and/or ctxp, the context as operand planes [P][B*L][C] (32-byte aligned,
+ * B*L*C % 16 == 0).  lens as in fs2_op_attention; rows t >= lens[b] are written as +0.  Only q|k rows and V^T columns
+ * below lens[b] (below L when lens is NULL) are read for their values.  Other math modes are rejected. */
+int fs2_op_attention_planes(int math_mode, const void* qkp, const void* vtp, int lpad, const int64_t* lens, int B, int L,
+                            int C, int heads, float* ctx, void* ctxp, void* stream);
 /* y = LayerNorm_C(x (+resid)) * g + b over the last dim (C in {256,384}) */
 int fs2_op_layernorm(const float* x, const float* resid, const float* g, const float* b, float eps, int64_t rows, int C,
                      float* out, void* stream);

@@ -332,68 +332,6 @@ def test_attention_vs_torch(prec, C, L, masked):
     close(ctx, want, tol, f"attention C={C} L={L} masked={masked}")
 
 
-@pytest.mark.parametrize("prec", ["3xtf32", "f16"])
-def test_attention_persistent_ctas_many_work_items(prec):
-    """Many (batch, head, query tile) work items -- more CTAs than the H100 has SMs, so several waves --, ragged key lengths
-    incl. an utterance with no valid key at all (its rows must come out 0) and a length that ends inside a key tile."""
-    B, H, C, L = 14, 2, 384, 1000                                  # 14 * 2 * 16 = 448 CTAs of 64 queries > 132 SMs
-    g = torch.Generator().manual_seed(99)
-    qkv = torch.randn(B, L, 3 * C, generator=g)
-    lens = torch.tensor([1000, 0, 999, 130, 128, 1, 517, 1000, 64, 900, 0, 385, 1000, 257])
-    q, k, v = [t.view(B, L, H, C // H).transpose(1, 2).double() for t in qkv.split(C, dim=-1)]
-    s = q @ k.transpose(-1, -2) / (C // H) ** 0.5
-    valid = torch.arange(L)[None] < lens[:, None]
-    m = (valid[:, None, :] & valid[:, :, None])[:, None]
-    p = torch.nan_to_num(torch.softmax(s.masked_fill(~m, -float("inf")), -1)).masked_fill(~m, 0.0)
-    want = (p @ v).transpose(1, 2).reshape(B, L, C).float()
-    lib = _lib.load()
-    ctx = torch.full((B, L, C), float("nan"), device="cuda")
-    qkv_c, lens_c = qkv.cuda(), lens.cuda()
-    _lib.check(lib.fs2_op_attention(_lib.MATH_MODES[prec], _lib.ptr(qkv_c), _lib.ptr(lens_c), B, L, C, H, _lib.ptr(ctx), _lib.stream_ptr(ctx.device)),
-               "fs2_op_attention")
-    assert torch.isfinite(ctx).all()
-    tol = dict(max=5e-5, mean=5e-6) if prec == "3xtf32" else dict(max=1e-2, mean=1e-3)
-    close(ctx, want, tol, f"persistent attention {prec}")
-    assert float(ctx[1].abs().max()) == 0.0 and float(ctx[10].abs().max()) == 0.0
-
-
-@pytest.mark.parametrize("prec", ["3xtf32", "f16"])
-@pytest.mark.parametrize("C", [256, 384])
-def test_attention_partial_last_key_tile(prec, C):
-    """The last key tile of an utterance is trimmed to its valid keys rounded up to 16 (S product with N = n16, P.V over n16 / 16
-    K-steps, half / none of the softmax work): every residue class of len mod 128 around the 16 / 32 / 64 boundaries, plus an
-    unmasked call (lens = NULL) whose L itself ends inside a tile."""
-    H = 2
-    res = [1, 15, 16, 17, 31, 32, 33, 48, 63, 64, 65, 96, 112, 127, 128]
-    lens = torch.tensor([128 + r for r in res])
-    B, L = len(res), 256
-    g = torch.Generator().manual_seed(C)
-    qkv = torch.randn(B, L, 3 * C, generator=g)
-    q, k, v = [t.view(B, L, H, C // H).transpose(1, 2).double() for t in qkv.split(C, dim=-1)]
-    s = q @ k.transpose(-1, -2) / (C // H) ** 0.5
-    valid = torch.arange(L)[None] < lens[:, None]
-    m = (valid[:, None, :] & valid[:, :, None])[:, None]
-    want = (torch.softmax(s.masked_fill(~m, -float("inf")), -1).masked_fill(~m, 0.0) @ v).transpose(1, 2).reshape(B, L, C).float()
-    lib = _lib.load()
-    ctx = torch.full((B, L, C), float("nan"), device="cuda")
-    qkv_c, lens_c = qkv.cuda(), lens.cuda()
-    _lib.check(lib.fs2_op_attention(_lib.MATH_MODES[prec], _lib.ptr(qkv_c), _lib.ptr(lens_c), B, L, C, H, _lib.ptr(ctx), _lib.stream_ptr(ctx.device)),
-               "fs2_op_attention")
-    tol = dict(max=5e-5, mean=5e-6) if prec == "3xtf32" else dict(max=1e-2, mean=1e-3)
-    assert torch.isfinite(ctx).all()
-    for b in range(B):
-        close(ctx[b:b + 1], want[b:b + 1], tol, f"attention {prec} C={C} len={int(lens[b])}")
-    for Lu in (128 + 17, 128 + 40, 3 * 128 + 1):                   # unmasked, L not a multiple of the tile
-        qkv_u = torch.randn(2, Lu, 3 * C, generator=g)
-        qu, ku, vu = [t.view(2, Lu, H, C // H).transpose(1, 2).double() for t in qkv_u.split(C, dim=-1)]
-        want_u = (torch.softmax(qu @ ku.transpose(-1, -2) / (C // H) ** 0.5, -1) @ vu).transpose(1, 2).reshape(2, Lu, C).float()
-        ctx_u = torch.full((2, Lu, C), float("nan"), device="cuda")
-        qc = qkv_u.cuda()
-        _lib.check(lib.fs2_op_attention(_lib.MATH_MODES[prec], _lib.ptr(qc), None, 2, Lu, C, H, _lib.ptr(ctx_u), _lib.stream_ptr(ctx_u.device)),
-                   "fs2_op_attention")
-        close(ctx_u, want_u, tol, f"attention {prec} C={C} unmasked L={Lu}")
-
-
 @pytest.mark.parametrize("prec,N", [("tf32", 384), ("f16", 384), ("3xtf32", 384), ("f16", 256), ("3xtf32", 256)])
 @pytest.mark.parametrize("rows,K,with_resid", [(1000, 384, True), (51, 1024, True), (4097, 256, False), (40000, 384, True), (20000, 1024, True)])
 def test_fused_gemm_layernorm_vs_torch(prec, N, rows, K, with_resid):
