@@ -43,6 +43,7 @@ class VocoderConfig(C.Structure):
 
 FS2_VOC_BAD_LENGTH, FS2_VOC_RANGE = 1, 2     # bits of fs2_griffin_lim's / fs2_mel_magnitude's device status word
 FS2_MELGAN_BAD_LENGTH, FS2_MELGAN_RANGE = 1, 2   # bits of fs2_melgan's device status word
+FS2_WAVEGLOW_BAD_LENGTH, FS2_WAVEGLOW_RANGE = 1, 2   # bits of fs2_waveglow's device status word
 
 _P, _I, _F, _L, _SZ = C.c_void_p, C.c_int, C.c_float, C.c_int64, C.c_size_t
 
@@ -69,6 +70,7 @@ SIGNATURES = {
     "fs2_one_hot": [_P, _L, _I, _P, _P],
     "fs2_op_tap_gemm": [_I, _P, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P],
     "fs2_op_tap_gemm_ex": [_I, _P, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P, _I, _P],
+    "fs2_op_tap_gemm_dil": [_I, _P, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P, _I, _I, _P],
     "fs2_op_attention": [_I, _P, _P, _I, _I, _I, _I, _P, _P],
     "fs2_op_attention_planes": [_I, _P, _P, _I, _P, _I, _I, _I, _I, _P, _P, _P],
     "fs2_op_gemm_layernorm": [_I, _P, _L, _I, _I, _P, _P, _P, _P, _P, _F, _P, _P, _P],
@@ -110,6 +112,11 @@ SIGNATURES = {
     "fs2_melgan_load": [_P, C.POINTER(_P), C.POINTER(_P), _P],
     "fs2_melgan_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
     "fs2_melgan": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_waveglow_create": [C.POINTER(_P), _I, _I],
+    "fs2_waveglow_load": [_P, C.POINTER(_P), _I, _P],
+    "fs2_waveglow_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_waveglow": [_P, _P, _P, _I, _I, C.c_double, _P, _P, _P, _P, _P, _SZ, _P],
+    "fs2_waveglow_noise": [_P, _P, _I, _I, _P, _P],
     "fs2_peer_alloc": [_SZ, C.POINTER(_P), _P],
     "fs2_peer_free": [_P],
     "fs2_peer_open": [_P, C.POINTER(_P)],
@@ -119,7 +126,7 @@ SIGNATURES = {
     "fs2_flag_wait": [_P, _I, _I, _L, _P],
 }
 OTHER_SYMBOLS = ("fs2_last_error", "fs2_version", "fs2_destroy", "fs2_kernel_launches", "fs2_profile_label", "fs2_vocoder_destroy",
-                 "fs2_melgan_destroy")
+                 "fs2_melgan_destroy", "fs2_waveglow_destroy")
 ALL_SYMBOLS = tuple(SIGNATURES) + OTHER_SYMBOLS
 
 _lib: Optional[C.CDLL] = None
@@ -153,6 +160,8 @@ def load() -> C.CDLL:
     lib.fs2_vocoder_destroy.argtypes = [_P]
     lib.fs2_melgan_destroy.restype = None
     lib.fs2_melgan_destroy.argtypes = [_P]
+    lib.fs2_waveglow_destroy.restype = None
+    lib.fs2_waveglow_destroy.argtypes = [_P]
     _lib = lib
     return lib
 

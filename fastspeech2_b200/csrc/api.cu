@@ -778,12 +778,21 @@ int fs2_op_tap_gemm(int math_mode, const float* x, int B, int L, int K, const fl
 int fs2_op_tap_gemm_ex(int math_mode, const float* x, int B, int L, int K, const float* w, const float* bias, int N,
                        int taps, int act, const float* resid, const int64_t* lens, float* out, void* out_planes,
                        int vt_col0, int vt_heads, void* vt, int vt_lpad, void* stream) {
+  return fs2_op_tap_gemm_dil(math_mode, x, B, L, K, w, bias, N, taps, act, resid, lens, out, out_planes, vt_col0, vt_heads, vt,
+                             vt_lpad, 1, stream);
+}
+int fs2_op_tap_gemm_dil(int math_mode, const float* x, int B, int L, int K, const float* w, const float* bias, int N,
+                        int taps, int act, const float* resid, const int64_t* lens, float* out, void* out_planes,
+                        int vt_col0, int vt_heads, void* vt, int vt_lpad, int dil, void* stream) {
   const char* who = "fs2_op_tap_gemm";
   FS2_REQUIRE(math_mode == FS2_MATH_FP32 || math_mode == FS2_MATH_TF32 || math_mode == FS2_MATH_F16 || math_mode == FS2_MATH_3XTF32,
               "%s: unknown math mode %d", who, math_mode);
   const bool planes = math_mode == FS2_MATH_F16 || math_mode == FS2_MATH_3XTF32;
   FS2_REQUIRE(x && w && (out || (planes && (out_planes || vt))), "%s: null argument", who);
   FS2_REQUIRE(B >= 0 && L >= 0 && K > 0 && N > 0 && taps > 0, "%s: bad shape B=%d L=%d K=%d N=%d taps=%d", who, B, L, K, N, taps);
+  // tap rows t + (j - pad) * dil are int32 row coordinates: keep them in range (dil = 1 is the undilated call, as before)
+  FS2_REQUIRE(dil == 1 || (dil > 1 && (long)dil * ((taps - 1) / 2) + L < (1L << 30)),
+              "%s: need dil >= 1 and dil * (taps - 1) / 2 + L < 2^30 (got dil=%d taps=%d L=%d)", who, dil, taps, L);
   FS2_REQUIRE(!out_planes || planes, "%s: out_planes needs FS2_MATH_F16 or FS2_MATH_3XTF32", who);
   FS2_REQUIRE(!vt || math_mode != FS2_MATH_FP32, "%s: the fp32 family has no transposed V output", who);
   FS2_REQUIRE(!vt || (vt_heads > 0 && vt_col0 >= 0 && vt_col0 < N && (N - vt_col0) % vt_heads == 0 && vt_lpad >= L),
@@ -805,6 +814,7 @@ int fs2_op_tap_gemm_ex(int math_mode, const float* x, int B, int L, int K, const
     g.vt_col0 = vt_col0; g.vt_heads = vt_heads; g.vt_dk = (N - vt_col0) / vt_heads; g.vt_lpad = vt_lpad;
     if (planes) g.vtp = reinterpret_cast<__half*>(vt); else g.vt_out = reinterpret_cast<float*>(vt);
   }
+  g.dil = dil;
   return dense(masked(g, lens), math_mode, st, P_DEC_W1);
 }
 int fs2_op_gemm_layernorm(int math_mode, const float* x, int64_t rows, int K, int N, const float* w, const float* bias, const float* resid,

@@ -51,7 +51,7 @@ enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_TANH = 2 };
 constexpr float kPlaneScale = 16.0f;
 constexpr float kPlaneInv = 1.0f / 16.0f;
 
-// out[m, n] = act( sum_{j<taps} sum_{k<K} x[b, t+j-pad, k] * w[j][n][k] + bias[n] ) (+ resid[m, n])
+// out[m, n] = act( sum_{j<taps} sum_{k<K} x[b, t+(j-pad)*dil, k] * w[j][n][k] + bias[n] ) (+ resid[m, n])
 // x rows have stride ldx floats, time extent L per utterance (zero outside [0,L)); m = b*L + t.
 struct TapGemm {
   const float* x; int ldx;      // fp32 activations (fp32 FMA and tf32 families)
@@ -76,6 +76,7 @@ struct TapGemm {
   // per-utterance mode (FS2_PER_UTTERANCE): rows t >= lens[b] are written as exact zeros (fp32 rows and planes; the
   // transposed V third is left unwritten there), and the tensor-core kernel skips row tiles that lie wholly past lens[b]
   const int64_t* lens = nullptr;
+  int dil = 1;                  // tap spacing in rows (dilated convolution); 0 (a memset TapGemm) counts as 1
 };
 int tap_gemm_fp32(const TapGemm& g, cudaStream_t st);
 int tap_gemm_tf32(const TapGemm& g, cudaStream_t st);   // wgmma + TMA, tf32 on fp32 data (gemm_tc.cu)

@@ -1,6 +1,6 @@
 // fp32 "tap GEMM": every Linear / Conv1d of the path as one shared-memory-staged kernel.
 //
-//   out[b,t,n] = act( sum_{j<taps} sum_{k<K} x[b, t+j-pad, k] * w[j][n][k] + bias[n] ) (+ resid[b,t,n])
+//   out[b,t,n] = act( sum_{j<taps} sum_{k<K} x[b, t+(j-pad)*dil, k] * w[j][n][k] + bias[n] ) (+ resid[b,t,n])
 //
 // Replaces nn.Linear (attention.py:48-50,74; encoder.py:119; fastspeech.py:153) and nn.Conv1d
 // (modules.py:225-234, duration_predictor.py:48-55, variance_predictor.py:24-33,
@@ -35,7 +35,7 @@ tap_gemm_fp32_kernel(TapGemm g) {
   const int tid = threadIdx.x;
   const int M = g.B * g.L;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-  const int pad = (g.taps - 1) / 2;
+  const int pad = (g.taps - 1) / 2, dil = g.dil > 1 ? g.dil : 1;
 
   // loader mapping: 4 threads cover one 16-float row chunk; rows lr and lr+64
   const int lr = tid >> 2, lk = (tid & 3) * 4;
@@ -60,7 +60,7 @@ tap_gemm_fp32_kernel(TapGemm g) {
     int j = s / kchunks, k0 = (s - j * kchunks) * BK;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      int ts = a_t[i] + j - pad;
+      int ts = a_t[i] + (j - pad) * dil;
       if (a_ok[i] && ts >= 0 && ts < g.L)
         ra[i] = __ldg(reinterpret_cast<const float4*>(g.x + (a_base[i] + ts) * g.ldx + k0 + lk));
       else

@@ -1,7 +1,7 @@
 // Tensor-core "tap GEMM" for sm_90a: wgmma (warpgroup MMA, tf32 or f16 operands, fp32 accumulators in registers),
 // operands staged in shared memory by TMA (cp.async.bulk.tensor, 128-byte swizzle), mbarrier pipelines, persistent CTAs.
 //
-//   out[b,t,n] = act( sum_{j<taps} sum_{k<K} x[b, t+j-pad, k] * w[j][n][k] + bias[n] ) (+ resid[b,t,n])
+//   out[b,t,n] = act( sum_{j<taps} sum_{k<K} x[b, t+(j-pad)*dil, k] * w[j][n][k] + bias[n] ) (+ resid[b,t,n])
 //
 // Same contract as gemm_fp32.cu (the CUDA-core family).  Three instantiation families:
 //   <BN, false, false>  plain tf32 (one MMA per product) on the fp32 activations themselves: the decoder side in
@@ -16,8 +16,9 @@
 // fp32 rows and / or as the operand planes of the next contraction (no separate split / conversion pass).
 //
 // Why no im2col: activations are [B, time, channel] with channels innermost, which *is* the K-major A operand of a GEMM.
-// Tap j of a 1-D convolution is the same matrix shifted by (j - pad) rows, so the producer just issues the TMA box at row
-// coordinate t0 + j - pad of a 3-D tensor map {channel, time, utterance}; rows outside [0, L) of the utterance are
+// Tap j of a 1-D convolution is the same matrix shifted by (j - pad) * dil rows (dil = 1 except in dilated convolutions), so
+// the producer just issues the TMA box at row coordinate t0 + (j - pad) * dil of a 3-D tensor map {channel, time,
+// utterance}; rows outside [0, L) of the utterance are
 // zero-filled by the TMA unit (that is exactly Conv1d's "same" padding).  K loop = taps x ceil(K / 32) pipeline steps of
 // 4 MMAs with K = 8 each (tf32; f16: ceil(K / 64) steps with K = 16 each: one 128-byte swizzle row either way).
 //
@@ -59,7 +60,7 @@ struct TcParams {
   // convolutions (tiles_per_utt > 0): every utterance has `full` 128-row tiles; its tail (L % 128 rows, `gn` granules
   // of 16 rows) shares a packed tile with the tails of upt - 1 other utterances, so no MMA rows are wasted on padding
   int B, full, gn, upt, full_tiles;
-  int K, taps, pad;
+  int K, taps, pad, dil;         // tap j reads rows t + (j - pad) * dil
   const float* bias; const float* resid; int ldr; int act;
   float* out; int ldo;
   float a_inv; const float* w_inv;   // accumulator scale = a_inv * (w_inv ? *w_inv : 1): undoes the operand planes' pre-scaling
@@ -157,7 +158,7 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       int j = 0, kc = 0;                        // tap, K chunk of step s
       for (int s = 0; s < steps; ++s, ++n) {
         const int slot = n % C::STAGES, round = n / C::STAGES;
-        const int k0 = kc * C::BKE, row = t0 + j - p.pad;
+        const int k0 = kc * C::BKE, row = t0 + (j - p.pad) * p.dil;
         const uint32_t st = tiles_addr + (uint32_t)slot * C::STAGE_BYTES, fb = full_addr + (uint32_t)slot * 8u;
         pin_before(st, fb, k0, row);
         mbar_wait(&empty_bar[slot], (round & 1) ^ 1);
@@ -355,7 +356,7 @@ int launch(const TapGemm& g, cudaStream_t st) {
   int rc;
   if ((rc = ensure_smem_attr(tap_gemm_tc_kernel<BN, PRECISE, HALF>, C::SMEM, &configured))) return rc;
   TcParams p;
-  p.K = g.K; p.taps = g.taps; p.pad = (g.taps - 1) / 2;
+  p.K = g.K; p.taps = g.taps; p.pad = (g.taps - 1) / 2; p.dil = g.dil > 1 ? g.dil : 1;
   p.bias = g.bias; p.resid = g.resid; p.ldr = g.ldr; p.act = g.act; p.out = g.out; p.ldo = g.ldo;
   const long rows = (long)g.B * g.L;
   p.a_inv = HALF ? g.a_inv : 1.0f; p.w_inv = HALF ? g.w_inv : nullptr;

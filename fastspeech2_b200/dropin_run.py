@@ -10,7 +10,9 @@ The other way to switch over is to copy `dropin/fastspeech.py` over the checkout
 
 With FS2_MELGAN_CHECKPOINT=<file> (seungwonpark/melgan's checkpoint, or a bare generator state dict) the launcher also makes
 `torch.hub.load("seungwonpark/melgan", "melgan")` return `MelGANVocoder.from_checkpoint(<file>)`, so the reference's
-inference.py and train_fastspeech.py reach MelGAN audio without a network.  Every other `torch.hub.load` call is passed on.
+inference.py and train_fastspeech.py reach MelGAN audio without a network.  With FS2_WAVEGLOW_CHECKPOINT=<file>
+(DeepLearningExamples' WaveGlow checkpoint) `torch.hub.load("nvidia/DeepLearningExamples:torchhub", "nvidia_waveglow",
+...)` returns `WaveGlowVocoder.from_checkpoint(<file>)` in the same way.  Every other `torch.hub.load` call is passed on.
 """
 from __future__ import annotations
 
@@ -21,6 +23,8 @@ import sys
 DROPIN_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "dropin")
 MELGAN_ENV = "FS2_MELGAN_CHECKPOINT"
 MELGAN_REPO, MELGAN_MODEL = "seungwonpark/melgan", "melgan"
+WAVEGLOW_ENV = "FS2_WAVEGLOW_CHECKPOINT"
+WAVEGLOW_REPO, WAVEGLOW_MODEL = "nvidia/deeplearningexamples", "nvidia_waveglow"
 
 
 def install_melgan_hub(checkpoint: str) -> None:
@@ -40,6 +44,30 @@ def install_melgan_hub(checkpoint: str) -> None:
     torch.hub.load = load
 
 
+def install_waveglow_hub(checkpoint: str) -> None:
+    """Route `torch.hub.load("nvidia/DeepLearningExamples", "nvidia_waveglow", ...)` (any branch suffix, e.g. ":torchhub";
+    GitHub names are case-insensitive) to `WaveGlowVocoder.from_checkpoint(checkpoint)`: the hub entry's
+    `model_math="fp16"` selects math_mode "f16", anything else the default "3xf16", and `pretrained=False` (an untrained
+    model) is refused.  Every other call goes to the `torch.hub.load` this wraps (a MelGAN hook installed before stays)."""
+    import torch
+
+    inner = getattr(torch.hub.load, "_fs2_waveglow_inner", torch.hub.load)
+
+    def load(repo_or_dir, model, *args, **kwargs):
+        if isinstance(repo_or_dir, str) and repo_or_dir.split(":")[0].lower() == WAVEGLOW_REPO and model == WAVEGLOW_MODEL:
+            from fastspeech2_b200.waveglow import WaveGlowVocoder
+            if not kwargs.get("pretrained", True):
+                raise ValueError(f"{WAVEGLOW_ENV} serves the pretrained checkpoint only (pretrained=False was asked)")
+            mode = "f16" if kwargs.get("model_math", "fp32") == "fp16" else "3xf16"
+            return WaveGlowVocoder.from_checkpoint(checkpoint, math_mode=mode)
+        return inner(repo_or_dir, model, *args, **kwargs)
+
+    # no `_fs2_original` here: a MelGAN hook installed after this one then chains to this hook, not past it, so the two
+    # hooks compose in either order
+    load._fs2_waveglow_inner = inner
+    torch.hub.load = load
+
+
 def main(argv=None) -> None:
     argv = list(sys.argv[1:] if argv is None else argv)
     if not argv:
@@ -54,6 +82,8 @@ def main(argv=None) -> None:
     sys.argv = [script] + argv[1:]
     if os.environ.get(MELGAN_ENV):
         install_melgan_hub(os.environ[MELGAN_ENV])
+    if os.environ.get(WAVEGLOW_ENV):
+        install_waveglow_hub(os.environ[WAVEGLOW_ENV])
     runpy.run_path(script, run_name="__main__")
 
 

@@ -244,6 +244,12 @@ int fs2_op_tap_gemm(int math_mode, const float* x, int B, int L, int K, const fl
 int fs2_op_tap_gemm_ex(int math_mode, const float* x, int B, int L, int K, const float* w, const float* bias, int N,
                        int taps, int act, const float* resid, const int64_t* lens, float* out, void* out_planes,
                        int vt_col0, int vt_heads, void* vt, int vt_lpad, void* stream);
+/* fs2_op_tap_gemm_ex with dilated taps: tap j reads row t + (j - pad) * dil of the same utterance (zero outside [0, L)),
+ * the layout of nn.Conv1d(dilation = dil, padding = pad * dil).  dil >= 1, and dil * pad + L < 2^30 when dil > 1
+ * (FS2_ERR_INVALID otherwise); fs2_op_tap_gemm_ex is the case dil = 1. */
+int fs2_op_tap_gemm_dil(int math_mode, const float* x, int B, int L, int K, const float* w, const float* bias, int N,
+                        int taps, int act, const float* resid, const int64_t* lens, float* out, void* out_planes,
+                        int vt_col0, int vt_heads, void* vt, int vt_lpad, int dil, void* stream);
 /* out = LayerNorm_N(x . w^T + bias + resid) * gamma + beta as a tensor-core GEMM followed by the row LayerNorm kernel (x [rows,K], w [N,K]);
  * the form of core/encoder.py:60-62 / :67-69: FS2_MATH_TF32 (tf32 on the fp32 rows, N = 384),
  * FS2_MATH_F16 (f16) and FS2_MATH_3XTF32 (error-compensated 3xF16) on operand planes made on the fly here,
@@ -400,6 +406,43 @@ int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float*
 int fs2_melgan_workspace_bytes(fs2_melgan_gen* m, int B, int Lmax, size_t* bytes);
 int fs2_melgan(fs2_melgan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
                size_t ws_bytes, void* stream);
+
+/* ---- batched WaveGlow vocoder (DESIGN.md section 9) ----------------------------------------------------------------- */
+/* DeepLearningExamples' WaveGlow (n_mel_channels 80, n_flows 12, n_group 8, n_early_every 4, n_early_size 2, WN: 8 layers,
+ * kernel 3, n_channels C) in its inverse direction, `infer`, on log-mels [B, Lmax, 80] with frame counts olens [B]:
+ * utterance b is infer(mels[b, :olens[b]]) alone -- the upsampling sees only its frames below olens[b] and every dilated
+ * convolution zero-pads at its own edges.  audio [B, Lmax * 256] fp32, 0 from olens[b] * 256 on; audio[b] is bit-identical
+ * to a B = 1 call with the same noise; mel frames past olens[b] and z steps past olens[b] * 32 are never read.
+ * Noise: z [B, 8, Lmax * 32] (device fp32, the layout WaveGlow.forward returns: channels 0-1 the early output of flow 4,
+ * 2-3 that of flow 8, 4-7 the last four) or, when z is NULL, drawn per utterance from Philox4x32-10 keyed by seeds[b]
+ * (fs2_waveglow_noise writes the same draw).  The flows receive fp32(sigma * z), the product taken in double and rounded
+ * once.  No allocation, no synchronisation: a call
+ * can be graph-captured.  It enqueues 496 kernels (497 in FS2_MATH_F16 / FS2_MATH_3XTF32).
+ * Data-dependent checks run on the device and are reported in *status (device int, written by the call):
+ *   FS2_WAVEGLOW_BAD_LENGTH  some olens[b] outside [1, Lmax]; that utterance's audio is 0;
+ *   FS2_WAVEGLOW_RANGE       an fp16 operand plane (f16 / 3xF16 modes) would saturate: some GEMM input above 65504 /
+ *                            kPlaneScale (4094) in magnitude. */
+#define FS2_WAVEGLOW_BAD_LENGTH 1
+#define FS2_WAVEGLOW_RANGE 2
+typedef struct fs2_waveglow_net fs2_waveglow_net;
+/* on the current device; math_mode FS2_MATH_*: every GEMM (start, end, coupling and the 1x1 inverses run on CUDA cores in
+ * fp32); n_channels C: a multiple of 64 in [64, 1024] (the published models use 256 or 512) */
+int fs2_waveglow_create(fs2_waveglow_net** out, int math_mode, int n_channels);
+void fs2_waveglow_destroy(fs2_waveglow_net* m);
+/* tensors[638]: device fp32, weight norm folded, torch layouts: upsample.weight [80, 80, 1024], upsample.bias [80], then per
+ * flow k = 0 .. 11 (c = 8, 8, 8, 8, 6, 6, 6, 6, 4, 4, 4, 4 channels, h = c / 2): start.weight [C, h, 1], start.bias [C],
+ * in_layers.{0..7}.(weight [2C, C, 3], bias [2C]), cond_layers.{0..7}.(weight [2C, 640, 1], bias [2C]),
+ * res_skip_layers.{0..7}.(weight [2C or C (i = 7), C, 1], bias), end.weight [2h, C, 1], end.bias [2h], and the inverse of
+ * convinv.k's weight [c, c].  Packed once; the tensors may be freed afterwards (stream order). */
+int fs2_waveglow_load(fs2_waveglow_net* m, const float* const* tensors, int n, void* stream);
+/* fails (FS2_ERR_INVALID) when B * Lmax * 32 reaches 2^31, or exceeds 65535 * 128 in FS2_MATH_FP32 */
+int fs2_waveglow_workspace_bytes(fs2_waveglow_net* m, int B, int Lmax, size_t* bytes);
+/* sigma finite and >= 0; seeds [B] i64 (device, used when z is NULL) or z [B, 8, Lmax * 32] */
+int fs2_waveglow(fs2_waveglow_net* m, const float* mels, const int64_t* olens, int B, int Lmax, double sigma, const int64_t* seeds,
+                 const float* z, float* audio, int* status, void* ws, size_t ws_bytes, void* stream);
+/* the standard-normal draw a seeded fs2_waveglow call uses: z [B, 8, Lmax * 32], 0 at steps t >= olens[b] * 32.  Element
+ * (b, ch, t) is Box-Muller on Philox4x32-10(counter (t, ch / 4, 0, 0), key (seeds[b] mod 2^32, seeds[b] / 2^32)). */
+int fs2_waveglow_noise(const int64_t* seeds, const int64_t* olens, int B, int Lmax, float* z, void* stream);
 
 /* ---- multi-GPU exchange step: gather of the final mel shards on one rank over NVLink peer memory ----------------- */
 /* Replaces what a reference user would write as torch.distributed.gather / all_gather of `after_outs` (the reference has
