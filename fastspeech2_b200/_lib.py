@@ -84,6 +84,10 @@ SIGNATURES = {
     "fs2_conv_forward": [_P, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P],
     "fs2_conv_dgrad": [_P, _I, _I, _I, _P, _I, _I, _P, _P, _P],
     "fs2_conv_wgrad": [_P, _P, _I, _I, _I, _I, _I, _P, _P, _P],
+    "fs2_conv_forward_ex": [_P, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P, _I, _P],
+    "fs2_conv_dgrad_ex": [_P, _I, _I, _I, _P, _I, _I, _P, _P, _I, _P],
+    "fs2_conv_wgrad_tc_ws_bytes": [_I, _I, _I, _I, _I, C.POINTER(_SZ)],
+    "fs2_conv_wgrad_tc": [_P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _SZ, _P],
     "fs2_layernorm_backward": [_P, _P, _P, _F, _L, _I, _P, _P, _P, _P],
     "fs2_batchnorm_train": [_P, _L, _I, _P, _P, _F, _F, _I, _P, _P, _P, _P, _P, _P],
     "fs2_batchnorm_backward": [_P, _P, _P, _P, _F, _L, _I, _P, _P, _P, _P, _P],

@@ -571,6 +571,34 @@ int fs2_conv_dgrad(const float* dy, int B, int L, int N, const float* w, int K, 
   g.resid = nullptr; g.ldr = 0; g.out = dx; g.ldo = K;
   return tap_gemm_fp32(g, st);
 }
+/* the same with a math mode: FS2_MATH_FP32 is exactly the calls above; FS2_MATH_TF32 runs the packed weights through the
+ * tap GEMM's tf32 family (gemm_tc.cu) */
+int fs2_conv_forward_ex(const float* x, int B, int L, int K, const float* w, const float* bias, int N, int taps, int act, const float* resid,
+                        float* out, float* scratch, int math_mode, void* stream) {
+  if (math_mode == FS2_MATH_FP32) return fs2_conv_forward(x, B, L, K, w, bias, N, taps, act, resid, out, scratch, stream);
+  FS2_REQUIRE(math_mode == FS2_MATH_TF32, "fs2_conv_forward_ex: math_mode must be FS2_MATH_FP32 or FS2_MATH_TF32");
+  FS2_REQUIRE(x && w && out && scratch, "fs2_conv_forward_ex: null argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = pack_conv_weight(w, N, K, taps, nullptr, scratch, st);
+  if (rc) return rc;
+  TapGemm g;
+  g.x = x; g.ldx = K; g.B = B; g.L = L; g.K = K; g.w = scratch; g.bias = bias; g.N = N; g.taps = taps; g.act = act;
+  g.resid = resid; g.ldr = N; g.out = out; g.ldo = N;
+  return tap_gemm_tf32(g, st);
+}
+int fs2_conv_dgrad_ex(const float* dy, int B, int L, int N, const float* w, int K, int taps, float* dx, float* scratch, int math_mode,
+                      void* stream) {
+  if (math_mode == FS2_MATH_FP32) return fs2_conv_dgrad(dy, B, L, N, w, K, taps, dx, scratch, stream);
+  FS2_REQUIRE(math_mode == FS2_MATH_TF32, "fs2_conv_dgrad_ex: math_mode must be FS2_MATH_FP32 or FS2_MATH_TF32");
+  FS2_REQUIRE(dy && w && dx && scratch, "fs2_conv_dgrad_ex: null argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  pack_dgrad_weight_kernel<<<grid_for((long)N * K * taps, 256), 256, 0, st>>>(w, N, K, taps, scratch);
+  FS2_LAUNCH_CHECK();
+  TapGemm g;
+  g.x = dy; g.ldx = N; g.B = B; g.L = L; g.K = N; g.w = scratch; g.bias = nullptr; g.N = K; g.taps = taps; g.act = ACT_NONE;
+  g.resid = nullptr; g.ldr = 0; g.out = dx; g.ldo = K;
+  return tap_gemm_tf32(g, st);
+}
 int fs2_conv_wgrad(const float* dy, const float* x, int B, int L, int N, int K, int taps, float* dw, float* dbias, void* stream) {
   FS2_REQUIRE(dy && x && dw, "fs2_conv_wgrad: null argument");
   cudaStream_t st = (cudaStream_t)stream;

@@ -21,7 +21,12 @@ mode raise (the reference's scripts call those under `model.eval()`).
 Precision (`precision=` / FS2_PRECISION): "3xf16" (default; alias "3xtf32") is the reference-precision
 mode -- every contraction, attention included, error-compensated on the tensor cores, fp32-class
 results; "f16" and "tf32" are the 10-bit-mantissa fast modes for the decoder side; "fp32" is exact
-fp32 FMA on CUDA cores (include/fs2_b200.h, FS2_MATH_*).
+fp32 FMA on CUDA cores (include/fs2_b200.h, FS2_MATH_*).  `precision` governs eval only.
+
+Train precision (`train_precision=` / FS2_TRAIN_PRECISION): "fp32" (default) trains in fp32 on CUDA cores; "tf32" runs
+every convolution and projection of the train step (forward, input and weight gradient) on the tensor cores in tf32
+with fp32 accumulation, as cuDNN does for a reference user's Conv1d by default.  Attention, the norms and the rest of
+the step stay fp32 (DESIGN.md §10).
 """
 from __future__ import annotations
 
@@ -37,6 +42,19 @@ from . import length_regulator as _lr
 from .weights import ModelDims, positional_table, variance_bins
 
 DEFAULT_PRECISION = os.environ.get("FS2_PRECISION", "3xf16")
+TRAIN_PRECISIONS = ("fp32", "tf32")
+
+
+def resolve_train_precision(train_precision: Optional[str] = None) -> str:
+    """The train path's math mode: the argument, else FS2_TRAIN_PRECISION, else "fp32".  "fp32" is fp32 on CUDA cores;
+    "tf32" runs every convolution and projection of the train step on the tensor cores (DESIGN.md §10)."""
+    mode = train_precision or os.environ.get("FS2_TRAIN_PRECISION") or "fp32"
+    if mode in ("f16", "3xf16", "3xtf32"):
+        raise ValueError(f"train_precision={mode!r} is not supported: the {mode} kernels read fixed-scale fp16 operand planes, "
+                         "which cannot hold gradients without underflow; use 'fp32' or 'tf32'")
+    if mode not in TRAIN_PRECISIONS:
+        raise ValueError(f"train_precision must be one of {list(TRAIN_PRECISIONS)}, got {mode!r}")
+    return mode
 
 
 def _get(node: Any, key: str, default: Any = None) -> Any:
@@ -256,7 +274,7 @@ class FeedForwardTransformer(nn.Module):
     """Feed-forward Transformer TTS (FastSpeech2) on H100.  See module docstring."""
 
     @classmethod
-    def from_checkpoint(cls, checkpoint, hp=None, precision: Optional[str] = None, device=None):
+    def from_checkpoint(cls, checkpoint, hp=None, precision: Optional[str] = None, device=None, train_precision: Optional[str] = None):
         """Build the model from a reference checkpoint: a path or the loaded dict `{"model": state_dict, "optim": ..,
         "step": .., "hp_str": .., "githash": ..}` that train_fastspeech.py:235-244 writes (or a bare state_dict, the
         `--old_model` case of inference.py:161-163).  `hp` defaults to the checkpoint's own `hp_str` like
@@ -271,12 +289,12 @@ class FeedForwardTransformer(nn.Module):
             hp = load_hp_str(checkpoint["hp_str"])
         idim = int(sd["encoder.embed.0.weight"].shape[0])
         odim = int(_get(_get(hp, "audio"), "num_mels"))
-        model = cls(idim, odim, hp, precision=precision)
+        model = cls(idim, odim, hp, precision=precision, train_precision=train_precision)
         model.load_state_dict(sd, strict="model" in checkpoint)
         model.eval()
         return model.to(device) if device is not None else model
 
-    def __init__(self, idim: int, odim: int, hp: Dict, precision: Optional[str] = None):
+    def __init__(self, idim: int, odim: int, hp: Dict, precision: Optional[str] = None, train_precision: Optional[str] = None):
         super().__init__()
         dims = dims_from_hp(idim, odim, hp)
         self.dims = dims
@@ -290,6 +308,7 @@ class FeedForwardTransformer(nn.Module):
         self.precision = precision or DEFAULT_PRECISION
         if self.precision not in _lib.MATH_MODES:
             raise ValueError(f"precision must be one of {sorted(_lib.MATH_MODES)}")
+        self.train_precision = resolve_train_precision(train_precision)
 
         A, D = dims.adim, dims.ddim
         self.encoder = _FFTStack(nn.Sequential(nn.Embedding(idim, A, padding_idx=0), _ScaledPosEnc(A, dims.pe_len)),

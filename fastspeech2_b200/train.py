@@ -3,8 +3,11 @@
 
 Every number is produced by kernels of libfs2b200.so (csrc/train.cu + the fp32 forward kernels); torch.autograd is used only
 as the graph that chains them: each stage below is a `torch.autograd.Function` whose forward / backward are C-ABI calls.
-Arithmetic is fp32 on CUDA cores (the reference trains in fp32); the stage order, dropout sites and BatchNorm batch
-statistics follow the reference modules line by line (cited at each step of `train_forward`).
+Arithmetic is fp32 on CUDA cores by default (the reference trains in fp32); with `train_precision="tf32"` every
+convolution and projection (`ConvFn`: forward, input and weight gradient) runs on the tensor cores in tf32 instead, the
+way a reference user on an H100 gets TF32 for every Conv1d from cuDNN's defaults (DESIGN.md §10).  The stage order,
+dropout sites and BatchNorm batch statistics follow the reference modules line by line (cited at each step of
+`train_forward`).
 
 Dropout masks come from `MaskSource`: the library's Philox kernel in production, or masks injected by a test so that the
 reference (with `torch.nn.functional.dropout` patched to consume the same list) and this path drop the same elements.
@@ -67,23 +70,32 @@ class MaskSource:
 
 # ------------------------------------------------------------------------------------------------------------------------
 class ConvFn(torch.autograd.Function):
-    """out = act(conv1d_same(x, w) + bias) (+ resid); x [B,L,K], w [N,K,taps] (nn.Conv1d) or [N,K] (nn.Linear)."""
+    """out = act(conv1d_same(x, w) + bias) (+ resid); x [B,L,K], w [N,K,taps] (nn.Conv1d) or [N,K] (nn.Linear).
+    `math`: _lib.MATH_FP32 (CUDA cores) or _lib.MATH_TF32 (forward and input gradient on the tap GEMM's tf32 family,
+    weight gradient on the tensor-core wgrad kernel; the bias gradient is the same column sum in both)."""
 
     @staticmethod
-    def forward(ctx, x, w, bias, act, resid):
+    def forward(ctx, x, w, bias, act, resid, math=_lib.MATH_FP32):
         lib = _lib.load()
         x = _c(x)
         B, L, K = x.shape
         N = w.shape[0]
         taps = w.shape[2] if w.dim() == 3 else 1
         assert not (act != ACT_NONE and resid is not None)
+        if math not in (_lib.MATH_FP32, _lib.MATH_TF32):
+            raise ValueError(f"ConvFn: math mode {math} is neither MATH_FP32 nor MATH_TF32")
         out = torch.empty((B, L, N), dtype=torch.float32, device=x.device)
         scratch = torch.empty((N * K * taps,), dtype=torch.float32, device=x.device)
         wc = _c(w.detach())
-        _chk(lib.fs2_conv_forward(x.data_ptr(), B, L, K, wc.data_ptr(), _p(None if bias is None else _c(bias.detach())), N, taps, int(act),
-                                  _p(None if resid is None else _c(resid)), out.data_ptr(), scratch.data_ptr(), _st(x)), "fs2_conv_forward")
+        args = (x.data_ptr(), B, L, K, wc.data_ptr(), _p(None if bias is None else _c(bias.detach())), N, taps, int(act),
+                _p(None if resid is None else _c(resid)), out.data_ptr(), scratch.data_ptr())
+        if math == _lib.MATH_FP32:
+            _chk(lib.fs2_conv_forward(*args, _st(x)), "fs2_conv_forward")
+        else:
+            _chk(lib.fs2_conv_forward_ex(*args, math, _st(x)), "fs2_conv_forward_ex")
         ctx.save_for_backward(x, wc, out if act != ACT_NONE else None)
         ctx.meta = (B, L, K, N, taps, int(act), bias is not None, resid is not None, w.shape)
+        ctx.math = math
         return out
 
     @staticmethod
@@ -97,15 +109,33 @@ class ConvFn(torch.autograd.Function):
             g = torch.empty_like(dy)
             _chk(lib.fs2_act_backward(dy.data_ptr(), out.data_ptr(), act, g.data_ptr(), dy.numel(), _st(dy)), "fs2_act_backward")
         dx = dw = db = None
+        tf32 = ctx.math == _lib.MATH_TF32
         if ctx.needs_input_grad[0]:
             dx = torch.empty((B, L, K), dtype=torch.float32, device=dy.device)
             scratch = torch.empty((N * K * taps,), dtype=torch.float32, device=dy.device)
-            _chk(lib.fs2_conv_dgrad(g.data_ptr(), B, L, N, w.data_ptr(), K, taps, dx.data_ptr(), scratch.data_ptr(), _st(dy)), "fs2_conv_dgrad")
+            args = (g.data_ptr(), B, L, N, w.data_ptr(), K, taps, dx.data_ptr(), scratch.data_ptr())
+            if tf32:
+                _chk(lib.fs2_conv_dgrad_ex(*args, ctx.math, _st(dy)), "fs2_conv_dgrad_ex")
+            else:
+                _chk(lib.fs2_conv_dgrad(*args, _st(dy)), "fs2_conv_dgrad")
         if ctx.needs_input_grad[1]:
             dw = torch.zeros(wshape, dtype=torch.float32, device=dy.device)
             db = torch.zeros((N,), dtype=torch.float32, device=dy.device) if has_bias else None
-            _chk(lib.fs2_conv_wgrad(g.data_ptr(), x.data_ptr(), B, L, N, K, taps, dw.data_ptr(), _p(db), _st(dy)), "fs2_conv_wgrad")
-        return dx, dw, db, None, (dy if has_resid else None)
+            if tf32:
+                nbytes = wgrad_tc_ws_bytes(B, L, N, K, taps)
+                ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=dy.device)
+                _chk(lib.fs2_conv_wgrad_tc(g.data_ptr(), x.data_ptr(), B, L, N, K, taps, dw.data_ptr(), _p(db), ws.data_ptr(), nbytes, _st(dy)),
+                     "fs2_conv_wgrad_tc")
+            else:
+                _chk(lib.fs2_conv_wgrad(g.data_ptr(), x.data_ptr(), B, L, N, K, taps, dw.data_ptr(), _p(db), _st(dy)), "fs2_conv_wgrad")
+        return dx, dw, db, None, (dy if has_resid else None), None
+
+
+def wgrad_tc_ws_bytes(B: int, L: int, N: int, K: int, taps: int) -> int:
+    """Workspace bytes of fs2_conv_wgrad_tc for this shape (raises on a size the library rejects)."""
+    n = C.c_size_t(0)
+    _chk(_lib.load().fs2_conv_wgrad_tc_ws_bytes(int(B), int(L), int(N), int(K), int(taps), C.byref(n)), "fs2_conv_wgrad_tc_ws_bytes")
+    return int(n.value)
 
 
 class LayerNormFn(torch.autograd.Function):
@@ -448,33 +478,33 @@ def _drop(x: torch.Tensor, p: float, masks: MaskSource, channel_first: bool = Fa
     return DropoutFn.apply(x, masks.next(tuple(x.shape), p, x.device), p)
 
 
-def _fft_blocks(stack, x, lens, heads: int, rate: float, masks: MaskSource):
+def _fft_blocks(stack, x, lens, heads: int, rate: float, masks: MaskSource, math: int = _lib.MATH_FP32):
     """core/encoder.py:46-71 (post-LN, concat_after=False) x num_blocks."""
     B, L, C_ = x.shape
     for blk in stack.encoders_:
         a = blk.self_attn
-        q = ConvFn.apply(x, a.linear_q.weight, a.linear_q.bias, ACT_NONE, None)              # attention.py:48-50
-        k = ConvFn.apply(x, a.linear_k.weight, a.linear_k.bias, ACT_NONE, None)
-        v = ConvFn.apply(x, a.linear_v.weight, a.linear_v.bias, ACT_NONE, None)
+        q = ConvFn.apply(x, a.linear_q.weight, a.linear_q.bias, ACT_NONE, None, math)        # attention.py:48-50
+        k = ConvFn.apply(x, a.linear_k.weight, a.linear_k.bias, ACT_NONE, None, math)
+        v = ConvFn.apply(x, a.linear_v.weight, a.linear_v.bias, ACT_NONE, None, math)
         dmask = masks.next((B, heads, L, L), rate, x.device) if rate > 0 else None           # attention.py:69
         ctx = AttentionFn.apply(q, k, v, lens, heads, rate, dmask)
-        att = ConvFn.apply(ctx, a.linear_out.weight, a.linear_out.bias, ACT_NONE, None)       # attention.py:74
+        att = ConvFn.apply(ctx, a.linear_out.weight, a.linear_out.bias, ACT_NONE, None, math)  # attention.py:74
         x = AddFn.apply(x, _drop(att, rate, masks))                                           # encoder.py:60
         x = LayerNormFn.apply(x, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)             # encoder.py:62
         f = blk.feed_forward
-        h = ConvFn.apply(x, f.w_1.weight, f.w_1.bias, ACT_RELU, None)                         # modules.py:247
+        h = ConvFn.apply(x, f.w_1.weight, f.w_1.bias, ACT_RELU, None, math)                   # modules.py:247
         h = _drop(h, rate, masks)                                                             # modules.py:248
-        y = ConvFn.apply(h, f.w_2.weight, f.w_2.bias, ACT_NONE, None)
+        y = ConvFn.apply(h, f.w_2.weight, f.w_2.bias, ACT_NONE, None, math)
         x = AddFn.apply(x, _drop(y, rate, masks))                                             # encoder.py:67
         x = LayerNormFn.apply(x, blk.norm2.weight, blk.norm2.bias, blk.norm2.eps)             # encoder.py:69
     return x
 
 
-def _predictor(pred, x, lens, rate: float, masks: MaskSource):
+def _predictor(pred, x, lens, rate: float, masks: MaskSource, math: int = _lib.MATH_FP32):
     """duration_predictor.py:64-86 / variance_predictor.py:39-78: [conv -> ReLU -> LayerNorm(channels) -> Dropout] x n, Linear -> 1, mask."""
     for layer in pred.conv:
         conv, ln = layer[0], layer[2].layer_norm
-        x = ConvFn.apply(x, conv.weight, conv.bias, ACT_RELU, None)
+        x = ConvFn.apply(x, conv.weight, conv.bias, ACT_RELU, None, math)
         x = LayerNormFn.apply(x, ln.weight, ln.bias, ln.eps)
         x = _drop(x, rate, masks, channel_first=True)
     return RowDotFn.apply(x, pred.linear.weight, pred.linear.bias, lens)
@@ -488,6 +518,7 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
     if dev.type != "cuda":
         raise _lib.Fs2Error("train-mode forward needs CUDA tensors (no CPU fallback)")
     masks = masks or MaskSource(seed=int(torch.initial_seed()) & 0xFFFFFFFF)
+    math = _lib.MATH_TF32 if model.train_precision == "tf32" else _lib.MATH_FP32
     d = model.dims
     ilens = ilens.to(device=dev, dtype=torch.int64).contiguous()
     olens = olens.to(device=dev, dtype=torch.int64).contiguous()
@@ -507,12 +538,12 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
     enc_pos = model.encoder.embed[-1]
     x = EmbedFn.apply(xs, model.encoder.embed[0].weight, enc_pos.alpha, enc_pos.pe)
     x = _drop(x, ER, masks)                                                                   # embedding.py:120
-    hs = _fft_blocks(model.encoder, x, ilens, d.aheads, ER, masks)
+    hs = _fft_blocks(model.encoder, x, ilens, d.aheads, ER, masks, math)
     # duration predictor on the encoder states, then LengthRegulator with the ground-truth durations (:209-211)
-    d_outs = _predictor(model.duration_predictor, hs, ilens, model.duration_dropout_rate, masks)
+    d_outs = _predictor(model.duration_predictor, hs, ilens, model.duration_dropout_rate, masks, math)
     hm = LengthRegulatorFn.apply(hs, ds, ilens, L)
-    e_outs = _predictor(model.energy_predictor.predictor, hm, olens, PR, masks)               # :212-215
-    p_outs = _predictor(model.pitch_predictor.predictor, hm, olens, PR, masks)
+    e_outs = _predictor(model.energy_predictor.predictor, hm, olens, PR, masks, math)               # :212-215
+    p_outs = _predictor(model.pitch_predictor.predictor, hm, olens, PR, masks, math)
     # hs + pitch_embed(one_hot(ps)) + energy_embed(one_hot(es)) (:200-206,218-219); bucket ids from the library's bucketize
     e_ids = torch.empty((B, L), dtype=torch.int64, device=dev)
     p_ids = torch.empty((B, L), dtype=torch.int64, device=dev)
@@ -523,21 +554,21 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
     hm = OneHotLinearAddFn.apply(hm, e_ids, model.energy_embed.weight, model.energy_embed.bias)
     # decoder input layer (core/encoder.py:118-125): Linear -> LayerNorm -> Dropout -> ReLU -> scaled positional encoding (+ dropout)
     emb = model.decoder.embed
-    z = ConvFn.apply(hm, emb[0].weight, emb[0].bias, ACT_NONE, None)
+    z = ConvFn.apply(hm, emb[0].weight, emb[0].bias, ACT_NONE, None, math)
     z = LayerNormFn.apply(z, emb[1].weight, emb[1].bias, emb[1].eps)
     z = _drop(z, DR, masks)
     z = ReluFn.apply(z)
     z = PosEncFn.apply(z, emb[4].alpha, emb[4].pe)
     z = _drop(z, DR, masks)
-    z = _fft_blocks(model.decoder, z, olens, d.aheads, DR, masks)
-    before = ConvFn.apply(z, model.feat_out.weight, model.feat_out.bias, ACT_NONE, None)      # :228-230
+    z = _fft_blocks(model.decoder, z, olens, d.aheads, DR, masks, math)
+    before = ConvFn.apply(z, model.feat_out.weight, model.feat_out.bias, ACT_NONE, None, math)  # :228-230
     # Postnet (modules.py:283-359): [conv(no bias) -> BatchNorm1d(batch statistics) -> tanh -> dropout] x 4, conv -> BN -> dropout; + residual
     y = before
     n_post = len(model.postnet.postnet)
     for i, layer in enumerate(model.postnet.postnet):
         conv, bn = layer[0], layer[1]
         last = i == n_post - 1
-        y = ConvFn.apply(y, conv.weight, None, ACT_NONE, None)
+        y = ConvFn.apply(y, conv.weight, None, ACT_NONE, None, math)
         y = BatchNormFn.apply(y, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, bn.momentum if bn.momentum is not None else 0.1,
                               ACT_NONE if last else ACT_TANH)
         with torch.no_grad():

@@ -294,6 +294,24 @@ int fs2_conv_forward(const float* x, int B, int L, int K, const float* w, const 
                      float* out, float* scratch, void* stream);
 int fs2_conv_dgrad(const float* dy, int B, int L, int N, const float* w, int K, int taps, float* dx, float* scratch, void* stream);
 int fs2_conv_wgrad(const float* dy, const float* x, int B, int L, int N, int K, int taps, float* dw /* += */, float* dbias /* += or NULL */, void* stream);
+/* The tf32 train mode (DESIGN.md §10).  math_mode FS2_MATH_FP32 is exactly fs2_conv_forward / fs2_conv_dgrad; FS2_MATH_TF32
+ * runs the same packed weights through the tensor-core tap GEMM's tf32 family (operands truncated to tf32 by the MMA, fp32
+ * accumulation), which needs K % 4 == 0, N % 16 == 0 (forward; dgrad: the reverse) and 16-byte aligned rows.  Other modes:
+ * FS2_ERR_INVALID. */
+int fs2_conv_forward_ex(const float* x, int B, int L, int K, const float* w, const float* bias, int N, int taps, int act, const float* resid,
+                        float* out, float* scratch, int math_mode, void* stream);
+int fs2_conv_dgrad_ex(const float* dy, int B, int L, int N, const float* w, int K, int taps, float* dx, float* scratch, int math_mode,
+                      void* stream);
+/* Weight gradient on the tensor cores: dw[n][k][j] += sum_{b, t < L} dy[b,t,n] * x[b, t+j-pad, k] (x zero outside [0, L) of
+ * each utterance; pad = (taps - 1) / 2, taps odd), dw in the reference layout [N][K][taps]; dy [B,L,N], x [B,L,K] fp32.
+ * Operands are rounded to tf32 (round to nearest) and multiplied by tf32 wgmma with fp32 accumulation; split-K partial
+ * sums are added into dw in a fixed order, without atomics, so the same inputs always give the same bits, on any H100.
+ * dbias (+=, optional) is the column sum of dy (fs2_colsum, atomics).  ws: caller-owned device workspace of at least
+ * fs2_conv_wgrad_tc_ws_bytes(...) bytes, 16-byte aligned; its contents on entry do not matter.  Any N, K >= 1; sizes whose
+ * workspace or tensor strides would overflow, and a short workspace, are FS2_ERR_INVALID.  B * L == 0 adds nothing. */
+int fs2_conv_wgrad_tc_ws_bytes(int B, int L, int N, int K, int taps, size_t* bytes);
+int fs2_conv_wgrad_tc(const float* dy, const float* x, int B, int L, int N, int K, int taps, float* dw /* += */, float* dbias /* += or NULL */,
+                      void* ws, size_t ws_bytes, void* stream);
 /* nn.LayerNorm backward from the saved input rows (C in {256, 384}) */
 int fs2_layernorm_backward(const float* x, const float* dy, const float* gamma, float eps, int64_t rows, int C, float* dx, float* dgamma /* += */,
                            float* dbeta /* += */, void* stream);
