@@ -563,6 +563,7 @@ int fs2_conv_forward(const float* x, int B, int L, int K, const float* w, const 
 }
 int fs2_conv_dgrad(const float* dy, int B, int L, int N, const float* w, int K, int taps, float* dx, float* scratch, void* stream) {
   FS2_REQUIRE(dy && w && dx && scratch, "fs2_conv_dgrad: null argument");
+  FS2_REQUIRE(taps > 0 && (taps & 1) == 1, "fs2_conv_dgrad: taps must be odd (got %d)", taps);
   cudaStream_t st = (cudaStream_t)stream;
   pack_dgrad_weight_kernel<<<grid_for((long)N * K * taps, 256), 256, 0, st>>>(w, N, K, taps, scratch);
   FS2_LAUNCH_CHECK();
@@ -591,6 +592,7 @@ int fs2_conv_dgrad_ex(const float* dy, int B, int L, int N, const float* w, int 
   if (math_mode == FS2_MATH_FP32) return fs2_conv_dgrad(dy, B, L, N, w, K, taps, dx, scratch, stream);
   FS2_REQUIRE(math_mode == FS2_MATH_TF32, "fs2_conv_dgrad_ex: math_mode must be FS2_MATH_FP32 or FS2_MATH_TF32");
   FS2_REQUIRE(dy && w && dx && scratch, "fs2_conv_dgrad_ex: null argument");
+  FS2_REQUIRE(taps > 0 && (taps & 1) == 1, "fs2_conv_dgrad_ex: taps must be odd (got %d)", taps);
   cudaStream_t st = (cudaStream_t)stream;
   pack_dgrad_weight_kernel<<<grid_for((long)N * K * taps, 256), 256, 0, st>>>(w, N, K, taps, scratch);
   FS2_LAUNCH_CHECK();
@@ -601,6 +603,7 @@ int fs2_conv_dgrad_ex(const float* dy, int B, int L, int N, const float* w, int 
 }
 int fs2_conv_wgrad(const float* dy, const float* x, int B, int L, int N, int K, int taps, float* dw, float* dbias, void* stream) {
   FS2_REQUIRE(dy && x && dw, "fs2_conv_wgrad: null argument");
+  FS2_REQUIRE(B >= 0 && L >= 0 && N > 0 && K > 0 && taps > 0 && (taps & 1) == 1, "fs2_conv_wgrad: need B, L >= 0, N, K > 0 and odd taps");
   cudaStream_t st = (cudaStream_t)stream;
   const long M = (long)B * L;
   if (M == 0) return FS2_OK;

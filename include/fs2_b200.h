@@ -289,7 +289,8 @@ int fs2_relu(const float* x, float* y, int64_t n, void* stream);
 int fs2_add(const float* a, const float* b, float* y, int64_t n, void* stream);
 int fs2_colsum(const float* x, int64_t rows, int C, float* out /* += */, void* stream);
 /* Conv1d("same") / Linear: forward (core/modules.py:247-248, attention.py:48-50,74, ...), input gradient, weight + bias
- * gradient.  scratch: N*K*taps floats */
+ * gradient.  scratch: N*K*taps floats.  taps must be odd: fs2_conv_dgrad and fs2_conv_wgrad return FS2_ERR_INVALID
+ * for even or non-positive taps (and wgrad for N, K < 1 or B, L < 0) before launching anything */
 int fs2_conv_forward(const float* x, int B, int L, int K, const float* w, const float* bias, int N, int taps, int act, const float* resid,
                      float* out, float* scratch, void* stream);
 int fs2_conv_dgrad(const float* dy, int B, int L, int N, const float* w, int K, int taps, float* dx, float* scratch, void* stream);
