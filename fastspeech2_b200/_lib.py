@@ -116,6 +116,8 @@ SIGNATURES = {
     "fs2_melgan_load": [_P, C.POINTER(_P), C.POINTER(_P), _P],
     "fs2_melgan_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
     "fs2_melgan": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_op_melgan_block": [_I, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P],
+    "fs2_op_melgan_upsample": [_I, _I, _I, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P],
     "fs2_waveglow_create": [C.POINTER(_P), _I, _I],
     "fs2_waveglow_load": [_P, C.POINTER(_P), _I, _P],
     "fs2_waveglow_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],

@@ -428,18 +428,38 @@ MgPlan plan(Bump& b, int B, int L, bool fused) {
 
 
 
+// one GEMM weight from its torch-layout tensors (melgan_pack_kernel's kind, Cin, Cout, taps, s): the packed fp32 [N][K],
+// the bias [N], the power-of-two scale and the fp16 planes; w->N, w->K and the buffers are set by the caller
+int pack_weight(MWeight* w, int kind, const float* wt, const float* wt2, const float* b, const float* b2, int Cin, int Cout, int taps,
+                int s, cudaStream_t st) {
+  const long n = (long)w->N * w->K;
+  melgan_pack_kernel<<<grid_for(n, 256), 256, 0, st>>>(kind, wt, wt2, w->N, w->K, Cin, Cout, taps, s, w->w);
+  FS2_LAUNCH_CHECK();
+  melgan_bias_kernel<<<grid_for(w->N, 256), 256, 0, st>>>(b, b2, w->N, Cout, w->bias);
+  FS2_LAUNCH_CHECK();
+  int rc = weight_scale(w->w, n, w->sc, w->sc + 1, st); if (rc) return rc;
+  return split_f16(w->w, w->hi, w->lo, n, w->sc, st);
+}
+
+// carves one MWeight of N x K out of a Bump
+void carve(Bump& b, MWeight* w, int N, int K) {
+  w->N = N; w->K = K;
+  const size_t n = (size_t)N * K;
+  w->w = b.floats(n); w->hi = (__half*)b.bytes(n * 2); w->lo = (__half*)b.bytes(n * 2); w->sc = b.floats(2); w->bias = b.floats(N);
+}
+
 // out [B * Lp][w.N] = a [B * Lp][w.K] . w^T + bias, rows t >= lens[b] written as 0 (and skipped by the tensor-core kernel)
-int gemm(const fs2_melgan_gen* m, const MWeight& w, const void* a, int B, int Lp, const int64_t* lens, float* out, cudaStream_t st) {
+int gemm(int mode, const MWeight& w, const void* a, int B, int Lp, const int64_t* lens, float* out, cudaStream_t st) {
   TapGemm g;
   memset(&g, 0, sizeof(g));
   g.B = B; g.L = Lp; g.K = w.K; g.N = w.N; g.taps = 1; g.act = ACT_NONE; g.out = out; g.ldo = w.N; g.lens = lens;
   g.w = w.w; g.bias = w.bias; g.a_inv = 1.0f; g.ldx = w.K;
-  if (m->math_mode == FS2_MATH_FP32 || m->math_mode == FS2_MATH_TF32) {
+  if (mode == FS2_MATH_FP32 || mode == FS2_MATH_TF32) {
     g.x = (const float*)a;
-    return m->math_mode == FS2_MATH_FP32 ? tap_gemm_fp32(g, st) : tap_gemm_tf32(g, st);
+    return mode == FS2_MATH_FP32 ? tap_gemm_fp32(g, st) : tap_gemm_tf32(g, st);
   }
   g.xp = (const __half*)a; g.w_hi = w.hi; g.w_lo = w.lo; g.w_inv = w.sc + 1; g.a_inv = kPlaneInv;
-  g.precise = m->math_mode == FS2_MATH_3XTF32;
+  g.precise = mode == FS2_MATH_3XTF32;
   return tap_gemm_planes(g, st);
 }
 
@@ -456,20 +476,48 @@ int run_taps(int kind, bool reflect_edges, const float* x, const int64_t* lens, 
 // mma.sync kernel where it measured faster than producers + the wgmma tap-GEMM (H100, filelist64, DESIGN.md section 8):
 // C <= 128 in f16, C <= 64 in 3xF16.  At C = 256 (and 128 in 3xF16) the fused kernel's per-warp weight fragments cost
 // more than the unfused route's HBM round trips.
-bool fused_blocks(const fs2_melgan_gen* m, int C) {
-  return (m->math_mode == FS2_MATH_F16 && C <= 128) || (m->math_mode == FS2_MATH_3XTF32 && C <= 64);
+bool fused_blocks(int mode, int C) {
+  return (mode == FS2_MATH_F16 && C <= 128) || (mode == FS2_MATH_3XTF32 && C <= 64);
 }
 
 template <int C>
-int run_block(const fs2_melgan_gen* m, const MWeight& w1, const MWeight& w2, const float* x, const int64_t* lens, int B, int Lp, int d,
-              float* out, int* status, cudaStream_t st) {
+int run_block(int mode, const MWeight& w1, const MWeight& w2, const float* x, const int64_t* lens, int B, int Lp, int d, float* out,
+              int* status, cudaStream_t st) {
   constexpr int warps = C == 256 ? 2 : 4;          // as in melgan_block_kernel: 16 rows per warp
   const long rows = (long)B * Lp, ctas = (rows + 16 * warps - 1) / (16 * warps);
   FS2_REQUIRE(ctas < (1L << 31), "fs2_melgan: too many rows (%ld)", rows);
-  auto k = m->math_mode == FS2_MATH_3XTF32 ? melgan_block_kernel<C, true> : melgan_block_kernel<C, false>;
+  auto k = mode == FS2_MATH_3XTF32 ? melgan_block_kernel<C, true> : melgan_block_kernel<C, false>;
   k<<<(unsigned)ctas, 32 * warps, 0, st>>>(x, lens, B, Lp, d, w1.hi, w1.lo, w1.sc + 1, w1.bias, w2.hi, w2.lo, w2.sc + 1, w2.bias, out, status);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
+}
+
+// One residual block x -> out on [B * Lp][C] rows (dilation d, w1 = the dilated conv, w2 = [W2 | Ws]): the fused kernel
+// (f16 / 3xF16, C in {32, 64, 128, 256}), or producers + tap-GEMMs through the scratch operand a (rows * 3C floats) and h
+// (rows * C floats).
+int res_block(int mode, bool fused, const MWeight& w1, const MWeight& w2, const float* x, const int64_t* lens, int B, int Lp, int C, int d,
+              void* a, float* h, float* out, int* status, cudaStream_t st) {
+  if (fused) {
+    return C == 256 ? run_block<256>(mode, w1, w2, x, lens, B, Lp, d, out, status, st)
+         : C == 128 ? run_block<128>(mode, w1, w2, x, lens, B, Lp, d, out, status, st)
+         : C == 64  ? run_block<64>(mode, w1, w2, x, lens, B, Lp, d, out, status, st)
+                    : run_block<32>(mode, w1, w2, x, lens, B, Lp, d, out, status, st);
+  }
+  const int kind = out_kind(mode);
+  int rc = run_taps(kind, true, x, lens, B, Lp, C, d, a, status, st);
+  if (rc || (rc = gemm(mode, w1, a, B, Lp, lens, h, st))) return rc;
+  auto concat = pick(kind, melgan_concat_kernel<OUT_HILO>, melgan_concat_kernel<OUT_HI>, melgan_concat_kernel<OUT_F32>);
+  concat<<<grid_for((long)B * Lp * (2 * C / 4), 256), 256, 0, st>>>(h, x, lens, B, Lp, C, (float*)a, (__half*)a, status);
+  FS2_LAUNCH_CHECK();
+  return gemm(mode, w2, a, B, Lp, lens, out, st);
+}
+
+// lrelu + ConvTranspose1d (k = 2s, stride s, pad s/2) x [B * Lin][Cin] -> out [B * Lin][s Cout] = [B * Lin * s][Cout], through
+// the scratch operand a (rows * 3 Cin floats): rows t < lens[b] of x in, rows >= lens[b] * s of out written as 0
+int upsample(int mode, const MWeight& w, const float* x, const int64_t* lens, int B, int Lin, int Cin, void* a, float* out, int* status,
+             cudaStream_t st) {
+  int rc = run_taps(out_kind(mode), false, x, lens, B, Lin, Cin, 1, a, status, st);
+  return rc ? rc : gemm(mode, w, a, B, Lin, lens, out, st);
 }
 
 int check_size(const fs2_melgan_gen* m, int B, int L) {
@@ -525,12 +573,7 @@ int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float*
   }
   for (int pass = 0; pass < 2; ++pass) {       // pass 0 sizes the arena, pass 1 carves it
     Bump b(pass ? m->arena : nullptr, pass ? (size_t)-1 : 0);
-    for (int j = 0; j < nj; ++j) {
-      MWeight* w = jobs[j].w;
-      w->N = jobs[j].N; w->K = jobs[j].K;
-      const size_t n = (size_t)w->N * w->K;
-      w->w = b.floats(n); w->hi = (__half*)b.bytes(n * 2); w->lo = (__half*)b.bytes(n * 2); w->sc = b.floats(2); w->bias = b.floats(w->N);
-    }
+    for (int j = 0; j < nj; ++j) carve(b, jobs[j].w, jobs[j].N, jobs[j].K);
     m->post_w = b.floats(kPostTaps * kPostC);
     m->post_b = b.floats(1);
     if (pass == 0) {
@@ -541,15 +584,9 @@ int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float*
   }
   for (int j = 0; j < nj; ++j) {
     const Job& q = jobs[j];
-    MWeight* w = q.w;
-    const long n = (long)w->N * w->K;
-    melgan_pack_kernel<<<grid_for(n, 256), 256, 0, st>>>(q.kind, weights[q.l], q.l2 >= 0 ? weights[q.l2] : nullptr, w->N, w->K, q.Cin,
-                                                         q.Cout, q.taps, q.s, w->w);
-    FS2_LAUNCH_CHECK();
-    melgan_bias_kernel<<<grid_for(w->N, 256), 256, 0, st>>>(biases[q.l], q.l2 >= 0 ? biases[q.l2] : nullptr, w->N, q.Cout, w->bias);
-    FS2_LAUNCH_CHECK();
-    int rc = weight_scale(w->w, n, w->sc, w->sc + 1, st); if (rc) return rc;
-    rc = split_f16(w->w, w->hi, w->lo, n, w->sc, st); if (rc) return rc;
+    const int rc = pack_weight(q.w, q.kind, weights[q.l], q.l2 >= 0 ? weights[q.l2] : nullptr, biases[q.l], q.l2 >= 0 ? biases[q.l2] : nullptr,
+                               q.Cin, q.Cout, q.taps, q.s, st);
+    if (rc) return rc;
   }
   melgan_pack_kernel<<<1, 256, 0, st>>>(0, weights[kLayers - 1], nullptr, 1, kPostTaps * kPostC, kPostC, 1, kPostTaps, 0, m->post_w);
   FS2_LAUNCH_CHECK();
@@ -589,34 +626,20 @@ int fs2_melgan(fs2_melgan_gen* m, const float* mels, const int64_t* olens, int B
     k<<<grid_for((long)B * Lp0 * (kMels * kPreTaps / 4), 256), 256, 0, st>>>(mels, p.lens, B, Lmax, Lp0, (float*)p.a, (__half*)p.a, status);
     FS2_LAUNCH_CHECK();
   }
-  if ((rc = gemm(m, m->pre, p.a, B, Lp0, p.lens, p.x[0], st))) return rc;
+  const int mode = m->math_mode;
+  if ((rc = gemm(mode, m->pre, p.a, B, Lp0, p.lens, p.x[0], st))) return rc;
   int cur = 0;
-  auto concat = pick(kind, melgan_concat_kernel<OUT_HILO>, melgan_concat_kernel<OUT_HI>, melgan_concat_kernel<OUT_F32>);
   for (int s = 0; s < kStages; ++s) {
     const int Lin = Lp0 * upsampling(s), Lout = Lp0 * upsampling(s + 1), C = kCout[s];
     const int64_t* lin = p.lens + (long)s * B;
     const int64_t* lout = p.lens + (long)(s + 1) * B;
     // lrelu, ConvTranspose1d: [B * Lin][s Cout] row-major is [B * Lout][Cout]
-    if ((rc = run_taps(kind, false, p.x[cur], lin, B, Lin, kCin[s], 1, p.a, status, st))) return rc;
-    if ((rc = gemm(m, m->up[s], p.a, B, Lin, lin, p.x[cur ^ 1], st))) return rc;
+    if ((rc = upsample(mode, m->up[s], p.x[cur], lin, B, Lin, kCin[s], p.a, p.x[cur ^ 1], status, st))) return rc;
     cur ^= 1;
     for (int i = 0, d = 1; i < 3; ++i, d *= 3) {
-      if (fused_blocks(m, C)) {
-        const MWeight &w1 = m->dil[s][i], &w2 = m->pair[s][i];
-        float *xi = p.x[cur], *xo = p.x[cur ^ 1];
-        rc = C == 256 ? run_block<256>(m, w1, w2, xi, lout, B, Lout, d, xo, status, st)
-           : C == 128 ? run_block<128>(m, w1, w2, xi, lout, B, Lout, d, xo, status, st)
-           : C == 64  ? run_block<64>(m, w1, w2, xi, lout, B, Lout, d, xo, status, st)
-                      : run_block<32>(m, w1, w2, xi, lout, B, Lout, d, xo, status, st);
-        if (rc) return rc;
-        cur ^= 1;
-        continue;
-      }
-      if ((rc = run_taps(kind, true, p.x[cur], lout, B, Lout, C, d, p.a, status, st))) return rc;
-      if ((rc = gemm(m, m->dil[s][i], p.a, B, Lout, lout, p.h, st))) return rc;
-      concat<<<grid_for((long)B * Lout * (2 * C / 4), 256), 256, 0, st>>>(p.h, p.x[cur], lout, B, Lout, C, (float*)p.a, (__half*)p.a, status);
-      FS2_LAUNCH_CHECK();
-      if ((rc = gemm(m, m->pair[s][i], p.a, B, Lout, lout, p.x[cur ^ 1], st))) return rc;
+      if ((rc = res_block(mode, fused_blocks(mode, C), m->dil[s][i], m->pair[s][i], p.x[cur], lout, B, Lout, C, d, p.a, p.h, p.x[cur ^ 1],
+                          status, st)))
+        return rc;
       cur ^= 1;
     }
   }
@@ -625,6 +648,77 @@ int fs2_melgan(fs2_melgan_gen* m, const float* mels, const int64_t* olens, int B
                                                                    audio);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
+}
+
+// ---- single layers on the vocoder's own code paths (tests) ----------------------------------------------------------
+// Both pack the caller's torch-layout weights into a stream-ordered temporary with the calls fs2_melgan_load makes, then
+// run what fs2_melgan runs for that layer.
+int fs2_op_melgan_block(int math_mode, int route, int C, const float* x, const int64_t* lens, int B, int Lp, int d, const float* w1,
+                        const float* b1, const float* w2, const float* b2, const float* ws, const float* bs, float* out, int* status,
+                        void* stream) {
+  const char* who = "fs2_op_melgan_block";
+  FS2_REQUIRE(math_mode >= FS2_MATH_FP32 && math_mode <= FS2_MATH_F16, "%s: bad math_mode %d", who, math_mode);
+  FS2_REQUIRE(route >= 0 && route <= 2, "%s: route must be 0 (the vocoder's), 1 (unfused) or 2 (fused), got %d", who, route);
+  FS2_REQUIRE(C == 32 || C == 64 || C == 128 || C == 256, "%s: C must be 32, 64, 128 or 256 (got %d)", who, C);
+  const bool planes = math_mode == FS2_MATH_F16 || math_mode == FS2_MATH_3XTF32;
+  FS2_REQUIRE(route != 2 || planes, "%s: the fused route runs in FS2_MATH_F16 / FS2_MATH_3XTF32 only", who);
+  FS2_REQUIRE(x && lens && w1 && b1 && w2 && b2 && ws && bs && out && status, "%s: null argument", who);
+  FS2_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 31) == 0,
+              "%s: x must be 16-byte and out 32-byte aligned", who);
+  FS2_REQUIRE(B >= 1 && Lp >= 1 && d >= 1 && (long)Lp + d < (1L << 30), "%s: bad shape B=%d Lp=%d d=%d", who, B, Lp, d);
+  const long rows = (long)B * Lp;
+  FS2_REQUIRE(rows * 3 * C < (1L << 31) && (math_mode != FS2_MATH_FP32 || rows <= 65535L * 128), "%s: too many rows (%ld)", who, rows);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool fused = route == 0 ? fused_blocks(math_mode, C) : route == 2;
+  MWeight wd, wp;
+  void* a = nullptr;
+  float* h = nullptr;
+  void* base = nullptr;
+  for (int pass = 0; pass < 2; ++pass) {       // pass 0 sizes the temporary, pass 1 carves it
+    Bump b(base, (size_t)-1);
+    carve(b, &wd, C, 3 * C);
+    carve(b, &wp, C, 2 * C);
+    a = b.floats((size_t)rows * 3 * C);
+    h = b.floats((size_t)rows * C);
+    if (pass == 0) FS2_CUDA_CHECK(cudaMallocAsync(&base, b.off + 256, st));
+  }
+  FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
+  int rc = pack_weight(&wd, 0, w1, nullptr, b1, nullptr, C, C, 3, 0, st);
+  if (!rc) rc = pack_weight(&wp, 2, w2, ws, b2, bs, C, C, 1, 0, st);
+  if (!rc) rc = res_block(math_mode, fused, wd, wp, x, lens, B, Lp, C, d, a, h, out, status, st);
+  cudaFreeAsync(base, st);
+  return rc;
+}
+
+int fs2_op_melgan_upsample(int math_mode, int Cin, int Cout, int s, const float* x, const int64_t* lens, int B, int Lin, const float* w,
+                           const float* b, float* out, int* status, void* stream) {
+  const char* who = "fs2_op_melgan_upsample";
+  FS2_REQUIRE(math_mode >= FS2_MATH_FP32 && math_mode <= FS2_MATH_F16, "%s: bad math_mode %d", who, math_mode);
+  FS2_REQUIRE(s >= 2 && s % 2 == 0, "%s: the stride s must be even and >= 2 (got %d)", who, s);
+  FS2_REQUIRE(Cin >= 16 && Cin % 16 == 0 && Cout >= 16 && Cout % 16 == 0, "%s: Cin and Cout must be multiples of 16 (got %d, %d)", who,
+              Cin, Cout);
+  FS2_REQUIRE(x && lens && w && b && out && status, "%s: null argument", who);
+  FS2_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 31) == 0,
+              "%s: x must be 16-byte and out 32-byte aligned", who);
+  FS2_REQUIRE(B >= 1 && Lin >= 1, "%s: bad shape B=%d Lin=%d", who, B, Lin);
+  const long rows = (long)B * Lin;
+  FS2_REQUIRE(rows * s * Cout < (1L << 31) && rows * 3 * Cin < (1L << 31) && (math_mode != FS2_MATH_FP32 || rows <= 65535L * 128),
+              "%s: too many rows (%ld)", who, rows);
+  cudaStream_t st = (cudaStream_t)stream;
+  MWeight wu;
+  void* a = nullptr;
+  void* base = nullptr;
+  for (int pass = 0; pass < 2; ++pass) {
+    Bump bb(base, (size_t)-1);
+    carve(bb, &wu, s * Cout, 3 * Cin);
+    a = bb.floats((size_t)rows * 3 * Cin);
+    if (pass == 0) FS2_CUDA_CHECK(cudaMallocAsync(&base, bb.off + 256, st));
+  }
+  FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
+  int rc = pack_weight(&wu, 1, w, nullptr, b, nullptr, Cin, Cout, 0, s, st);
+  if (!rc) rc = upsample(math_mode, wu, x, lens, B, Lin, Cin, a, out, status, st);
+  cudaFreeAsync(base, st);
+  return rc;
 }
 
 }  // extern "C"

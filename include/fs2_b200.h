@@ -425,6 +425,23 @@ int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float*
 int fs2_melgan_workspace_bytes(fs2_melgan_gen* m, int B, int Lmax, size_t* bytes);
 int fs2_melgan(fs2_melgan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
                size_t ws_bytes, void* stream);
+/* Single MelGAN layers on fs2_melgan's code paths (used by the per-layer tests).  Weights come in torch's layouts and are
+ * packed into a stream-ordered temporary as fs2_melgan_load packs them.  status (device int) is set to 0 or
+ * FS2_MELGAN_RANGE.  x 16-byte and out 32-byte aligned.
+ * fs2_op_melgan_block: one residual block on rows [B*Lp][C], utterance b at rows t < lens[b]:
+ *   out = Ws . x + bs + W2 . lrelu(W1 (*)_d reflect_d(lrelu(x)) + b1) + b2, rows t >= lens[b] written as +0;
+ *   w1 [C][C][3] (dilation d), w2 and ws [C][C][1].  Every lens[b] must be 0 or lie in [d + 1, Lp], so that one
+ *   reflection reaches every tap (fs2_melgan's stages always meet this); rows t >= lens[b] of x are never read.
+ *   route 0 = the route fs2_melgan takes at this C and math mode, 1 = producers + tap-GEMMs, 2 = the fused kernel
+ *   (FS2_MATH_F16 / FS2_MATH_3XTF32 only).  C in {32, 64, 128, 256}.
+ * fs2_op_melgan_upsample: lrelu + ConvTranspose1d(Cin -> Cout, k = 2s, stride s, padding s/2) on x [B*Lin][Cin], each
+ *   utterance over its rows t < lens[b] (lens[b] in [0, Lin]) with zeros outside them; w [Cin][Cout][2s], b [Cout];
+ *   out [B*Lin*s][Cout], rows at or past lens[b]*s written as +0.  s even, Cin and Cout multiples of 16. */
+int fs2_op_melgan_block(int math_mode, int route, int C, const float* x, const int64_t* lens, int B, int Lp, int d, const float* w1,
+                        const float* b1, const float* w2, const float* b2, const float* ws, const float* bs, float* out, int* status,
+                        void* stream);
+int fs2_op_melgan_upsample(int math_mode, int Cin, int Cout, int s, const float* x, const int64_t* lens, int B, int Lin, const float* w,
+                           const float* b, float* out, int* status, void* stream);
 
 /* ---- batched WaveGlow vocoder (DESIGN.md section 9) ----------------------------------------------------------------- */
 /* DeepLearningExamples' WaveGlow (n_mel_channels 80, n_flows 12, n_group 8, n_early_every 4, n_early_size 2, WN: 8 layers,

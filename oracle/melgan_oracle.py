@@ -81,9 +81,9 @@ def batched(gen: Generator, mels: torch.Tensor, olens) -> torch.Tensor:
     """The batched contract, one utterance at a time: mels [B, Lmax, 80], olens [B] -> fp32 audio [B, Lmax * 256], each
     utterance the generator on its own frames plus the tail frames, trimmed to olens[b] * 256, zero past it."""
     B, L, _ = mels.shape
-    out = torch.zeros(B, L * HOP, dtype=mels.dtype)
+    out = torch.zeros(B, L * HOP, dtype=mels.dtype, device=mels.device)
     for b, n in enumerate(int(v) for v in olens):
         m = mels[b, :n].T[None]
-        m = torch.cat((m, torch.full((1, m.shape[1], TAIL_FRAMES), TAIL_VALUE, dtype=m.dtype)), dim=2)
+        m = torch.cat((m, torch.full((1, m.shape[1], TAIL_FRAMES), TAIL_VALUE, dtype=m.dtype, device=m.device)), dim=2)
         out[b, : n * HOP] = gen(m)[0, 0, : n * HOP]
     return out

@@ -201,10 +201,60 @@ def test_bad_math_mode_and_inference_shape_raise(voc):
 def test_library_exports_melgan_entry_points():
     lib = _lib.load()
     header = open(os.path.join(REPO, "include", "fs2_b200.h")).read()
-    for name in ("fs2_melgan_create", "fs2_melgan_load", "fs2_melgan_workspace_bytes", "fs2_melgan"):
+    for name in ("fs2_melgan_create", "fs2_melgan_load", "fs2_melgan_workspace_bytes", "fs2_melgan", "fs2_op_melgan_block",
+                 "fs2_op_melgan_upsample"):
         assert hasattr(lib, name) and name in _lib.SIGNATURES, name
         assert f"int {name}(" in header, name
     assert hasattr(lib, "fs2_melgan_destroy") and "void fs2_melgan_destroy(" in header
+
+
+def test_single_layer_entries_reject_bad_arguments_on_the_host():
+    """fs2_op_melgan_block and fs2_op_melgan_upsample refuse these before they touch memory (the pointers are never
+    dereferenced)."""
+    lib = _lib.load()
+    p = 256     # a stand-in non-null, aligned pointer
+
+    def block(mode=_lib.MATH_3XTF32, route=0, C=64, x=p, out=p, B=2, Lp=40, d=3):
+        return lib.fs2_op_melgan_block(mode, route, C, x, p, B, Lp, d, p, p, p, p, p, p, out, p, None)
+
+    def upsample(mode=_lib.MATH_3XTF32, Cin=64, Cout=32, s=2, x=p, B=2, Lin=40):
+        return lib.fs2_op_melgan_upsample(mode, Cin, Cout, s, x, p, B, Lin, p, p, p, p, None)
+
+    for mode in (-1, 4, 7):
+        assert block(mode=mode) == -1 and b"math_mode" in lib.fs2_last_error()
+        assert upsample(mode=mode) == -1 and b"math_mode" in lib.fs2_last_error()
+    for route in (-1, 3):
+        assert block(route=route) == -1 and b"route" in lib.fs2_last_error()
+    for mode in (_lib.MATH_FP32, _lib.MATH_TF32):
+        assert block(mode=mode, route=2) == -1 and b"fused route" in lib.fs2_last_error()
+    for C in (0, 16, 48, 96, 512):
+        assert block(C=C) == -1 and b"C must be" in lib.fs2_last_error()
+    assert block(x=None) == -1 and b"null" in lib.fs2_last_error()
+    assert block(x=p + 8) == -1 and b"aligned" in lib.fs2_last_error()
+    assert block(out=p + 16) == -1 and b"aligned" in lib.fs2_last_error()
+    assert block(d=0) == -1 and b"shape" in lib.fs2_last_error()
+    assert block(B=0) == -1 and b"shape" in lib.fs2_last_error()
+    assert block(mode=_lib.MATH_FP32, route=1, B=65535, Lp=129) == -1 and b"too many rows" in lib.fs2_last_error()
+    for s in (0, 1, 3, 7):
+        assert upsample(s=s) == -1 and b"stride" in lib.fs2_last_error()
+    for Cin, Cout in ((40, 32), (64, 24), (0, 32)):
+        assert upsample(Cin=Cin, Cout=Cout) == -1 and b"multiples of 16" in lib.fs2_last_error()
+    assert upsample(x=None) == -1 and b"null" in lib.fs2_last_error()
+    assert upsample(x=p + 4) == -1 and b"aligned" in lib.fs2_last_error()
+    assert upsample(Lin=0) == -1 and b"shape" in lib.fs2_last_error()
+
+
+def test_case_table_covers_the_block_instantiations():
+    """The per-layer GPU cases (tests/test_gpu_melgan_kernels.py) reach every (C, precision) instantiation of the fused
+    block on both routes, every dilation, and the geometry edges: empty, d + 1 and Lp utterances, a warp spanning two live
+    utterances, a last CTA with a partial warp and an idle one; the upsampling lengths include 0, 1 and a tile tail."""
+    import test_gpu_melgan_kernels as K
+    assert K.check_coverage() == []
+    assert sorted({(c.C, c.d) for c in K.BLOCK_CASES}) == [(C, d) for C in (32, 64, 128, 256) for d in (1, 3, 9)]
+    assert [K.fused_blocks(m, C) for m in ("f16", "3xf16") for C in (32, 64, 128, 256)] == [True] * 3 + [False] + [True] * 2 + [False] * 2
+    # 100 rows: only the warp at row 16 holds live rows of two utterances (0 and 1); the last CTA has 36 rows, 1 idle warp
+    c = K.BlockCase(64, 1, 20, (20, 2, 0, 7, 20))
+    assert K.straddles(c) == [16] and K.last_cta(c) == (36, 1)
 
 
 def test_melgan_kernels_do_not_spill():
