@@ -43,6 +43,7 @@ class VocoderConfig(C.Structure):
 
 FS2_VOC_BAD_LENGTH, FS2_VOC_RANGE = 1, 2     # bits of fs2_griffin_lim's / fs2_mel_magnitude's device status word
 FS2_MELGAN_BAD_LENGTH, FS2_MELGAN_RANGE = 1, 2   # bits of fs2_melgan's device status word
+FS2_MELGAN_BAD_START = 4                          # and of fs2_melgan_window's
 FS2_WAVEGLOW_BAD_LENGTH, FS2_WAVEGLOW_RANGE = 1, 2   # bits of fs2_waveglow's device status word
 
 _P, _I, _F, _L, _SZ = C.c_void_p, C.c_int, C.c_float, C.c_int64, C.c_size_t
@@ -116,6 +117,8 @@ SIGNATURES = {
     "fs2_melgan_load": [_P, C.POINTER(_P), C.POINTER(_P), _P],
     "fs2_melgan_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
     "fs2_melgan": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_melgan_window_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_melgan_window": [_P, _P, _P, _P, _I, _I, _I, _P, _L, _P, _P, _SZ, _P],
     "fs2_op_melgan_block": [_I, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P],
     "fs2_op_melgan_upsample": [_I, _I, _I, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P],
     "fs2_waveglow_create": [C.POINTER(_P), _I, _I],

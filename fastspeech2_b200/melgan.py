@@ -81,6 +81,7 @@ class MelGANVocoder(nn.Module):
         self._layers = [m for m in self.modules() if isinstance(m, _WNConv)]      # state_dict order, 42 convolutions
         self._handles = {}       # device index -> (fs2_melgan_gen*, parameter fingerprint it was loaded from)
         self._ws = {}            # device index -> workspace tensor
+        self._wws = {}           # device index -> window workspace tensor (fs2_melgan_window)
         self._epoch = 0
 
     def __del__(self):
@@ -184,7 +185,7 @@ class MelGANVocoder(nn.Module):
             self._ws[device.index] = ws
         return ws
 
-    def _inputs(self, mels, olens):
+    def _inputs(self, mels, olens, check_size=None):
         if not torch.is_tensor(mels) or mels.dim() != 3 or mels.shape[2] != N_MELS or mels.shape[0] == 0 or mels.shape[1] == 0:
             raise ValueError(f"mels must be a non-empty [B, Lmax, {N_MELS}] tensor")
         if not torch.is_tensor(olens) or olens.dim() != 1 or olens.shape[0] != mels.shape[0]:
@@ -194,7 +195,7 @@ class MelGANVocoder(nn.Module):
         if not mels.is_cuda or not olens.is_cuda:
             raise ValueError("mels and olens must be CUDA tensors (the H100 path has no CPU fallback)")
         B, L, _ = mels.shape
-        self._check_size(B, L)
+        (check_size or self._check_size)(B, L)
         return mels.to(torch.float32).contiguous(), olens.to(device=mels.device, dtype=torch.int64).contiguous(), B, L
 
     def _check_size(self, B: int, L: int) -> None:
@@ -207,17 +208,80 @@ class MelGANVocoder(nn.Module):
             raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 sample rows, B * (Lmax + 10) * {HOP} = {rows} "
                              f"(B={B}, Lmax={L}); split the batch or use another math mode")
 
+    def _window_workspace(self, h, B: int, n_frames: int, device: torch.device) -> torch.Tensor:
+        n = C.c_size_t()
+        _lib.check(_lib.load().fs2_melgan_window_workspace_bytes(h, B, n_frames, C.byref(n)), "fs2_melgan_window_workspace_bytes")
+        ws = self._wws.get(device.index)
+        if ws is None or ws.numel() < n.value:
+            self._wws.pop(device.index, None)
+            ws = torch.empty(n.value, dtype=torch.uint8, device=device)
+            self._wws[device.index] = ws
+        return ws
+
+    @staticmethod
+    def _check_frames(n_frames) -> None:
+        if isinstance(n_frames, bool) or not isinstance(n_frames, int) or n_frames < 1:
+            raise ValueError(f"n_frames / chunk_frames must be an int >= 1 (got {n_frames!r})")
+
+    def _check_window_size(self, B: int, n_frames: int) -> None:
+        """fs2_melgan_window's limits on the window's B * (256 * n_frames + 36) rows, raised here as ValueError."""
+        self._check_frames(n_frames)
+        rows = B * (n_frames * HOP + 36)
+        if rows >= 1 << 31:
+            raise ValueError(f"B * (256 * n_frames + 36) must stay below 2^31 window rows (B={B}, n_frames={n_frames})")
+        if self.math_mode == "fp32" and rows > 65535 * 128:
+            raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 window rows, B * (256 * n_frames + 36) = {rows} "
+                             f"(B={B}, n_frames={n_frames}); use fewer frames per window")
+
+    def _starts(self, starts, B: int, device: torch.device) -> torch.Tensor:
+        """starts as an int, a host list or tensor (checked >= 0 here) or a device tensor (checked on the device) -> [B]
+        int64 on `device`."""
+        if isinstance(starts, bool):
+            raise ValueError("starts must be an int, a list or an integer tensor")
+        if isinstance(starts, int):
+            starts = [starts] * B
+        if not torch.is_tensor(starts):
+            try:
+                starts = torch.tensor(starts)
+            except (TypeError, ValueError, RuntimeError):
+                raise ValueError("starts must be an int, a list or an integer tensor") from None
+        if starts.dim() != 1 or starts.shape[0] != B:
+            raise ValueError(f"starts must hold B={B} frame offsets")
+        if starts.dtype.is_floating_point or starts.dtype == torch.bool or starts.is_complex():
+            raise ValueError("starts must be an integer tensor")
+        if not starts.is_cuda:
+            if bool((starts < 0).any()):
+                raise ValueError("every starts[b] must be >= 0")
+        elif starts.device != device:
+            raise ValueError("starts must be on the same device as mels")
+        return starts.to(device=device, dtype=torch.int64).contiguous()
+
+    def _window_call(self, h, mels, olens, starts, B: int, L: int, n_frames: int, audio: torch.Tensor, ld: int, status: torch.Tensor,
+                     ws: torch.Tensor) -> None:
+        dev = mels.device
+        with torch.cuda.device(dev):
+            _lib.check(_lib.load().fs2_melgan_window(h, _lib.ptr(mels), _lib.ptr(olens), _lib.ptr(starts), B, L, n_frames, audio.data_ptr(), ld,
+                                                     _lib.ptr(status), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)), "fs2_melgan_window")
+
     def _check_status(self, status: torch.Tensor) -> None:
         s = int(status.item())                                                   # the call's one host read
         if s & _lib.FS2_MELGAN_BAD_LENGTH:
             raise ValueError("every olens[b] must lie in [1, Lmax]")
+        if s & _lib.FS2_MELGAN_BAD_START:
+            raise ValueError("every starts[b] must be >= 0")
         if s & _lib.FS2_MELGAN_RANGE:
             raise ValueError(f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
                              f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'")
 
     # ---- synthesis ------------------------------------------------------------------------------------------------
-    def forward(self, mels: torch.Tensor, olens: torch.Tensor):
-        """-> (audio [B, Lmax * 256] fp32, alens [B] int64 = olens * 256)."""
+    def forward(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int | None = None):
+        """-> (audio [B, Lmax * 256] fp32, alens [B] int64 = olens * 256).
+
+        chunk_frames=k: the same bits, computed as windows of k frames written straight into the output, with the
+        workspace of one window (fs2_melgan_window): in fp32 mode this vocodes batches the whole call refuses.  Still one
+        host read per call: the windows' status words are ORed on the device."""
+        if chunk_frames is not None:
+            return self._chunked(mels, olens, chunk_frames)
         mels, olens, B, L = self._inputs(mels, olens)
         dev = mels.device
         h = self._handle(dev)
@@ -228,6 +292,57 @@ class MelGANVocoder(nn.Module):
             _lib.check(_lib.load().fs2_melgan(h, _lib.ptr(mels), _lib.ptr(olens), B, L, _lib.ptr(audio), _lib.ptr(status), _lib.ptr(ws),
                                               ws.numel(), _lib.stream_ptr(dev)), "fs2_melgan")
         self._check_status(status)
+        return audio, olens * HOP
+
+    def _window_inputs(self, mels, olens, n_frames):
+        """_inputs with the window's limits in place of the whole call's (Lmax bounds only the per-utterance rows)."""
+        self._check_frames(n_frames)
+        def check(B, L):
+            self._check_window_size(B, n_frames)
+            if (L + 10) * HOP >= 1 << 31:
+                raise ValueError(f"(Lmax + 10) * {HOP} must stay below 2^31 samples (Lmax={L})")
+        return self._inputs(mels, olens, check)
+
+    def window(self, mels: torch.Tensor, olens: torch.Tensor, starts, n_frames: int):
+        """One window of the audio (DESIGN.md section 11): -> (audio [B, n_frames * 256] fp32, alens [B] int64 =
+        clamp(olens - starts, 0, n_frames) * 256).  audio[b, :alens[b]] are samples [starts[b] * 256, ...) of
+        `forward(mels, olens)[0][b]`, bit for bit; the rest is 0.  starts: an int (every utterance), a host list or tensor,
+        or a device tensor.  Only mel frames [starts[b] - 6, starts[b] + n_frames + 6) below olens[b] are read; the
+        workspace depends on B and n_frames only.  One host read per call."""
+        mels, olens, B, L = self._window_inputs(mels, olens, n_frames)
+        dev = mels.device
+        starts = self._starts(starts, B, dev)
+        h = self._handle(dev)
+        ws = self._window_workspace(h, B, n_frames, dev)
+        audio = torch.empty((B, n_frames * HOP), dtype=torch.float32, device=dev)
+        status = torch.empty((1,), dtype=torch.int32, device=dev)
+        self._window_call(h, mels, olens, starts, B, L, n_frames, audio, n_frames * HOP, status, ws)
+        self._check_status(status)
+        return audio, (olens - starts).clamp(0, n_frames) * HOP
+
+    def stream(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int = 32):
+        """Lockstep windows: yields (audio, alens) of `window(mels, olens, k * chunk_frames, chunk_frames)` for k = 0 ..
+        ceil(Lmax / chunk_frames) - 1, the last one cut at Lmax, so that the chunks concatenated along time are
+        `forward(mels, olens)`.  Utterances that have ended give rows of 0 (alens 0)."""
+        self._check_frames(chunk_frames)
+        L = mels.shape[1]
+        for c0 in range(0, L, chunk_frames):
+            yield self.window(mels, olens, c0, min(chunk_frames, L - c0))
+
+    def _chunked(self, mels, olens, k: int):
+        mels, olens, B, L = self._window_inputs(mels, olens, k)
+        dev = mels.device
+        h = self._handle(dev)
+        ws = self._window_workspace(h, B, min(k, L), dev)
+        audio = torch.empty((B, L * HOP), dtype=torch.float32, device=dev)
+        c0s = list(range(0, L, k))
+        starts = torch.tensor(c0s, dtype=torch.int64).repeat_interleave(B).reshape(len(c0s), B).to(dev)
+        status = torch.empty((len(c0s),), dtype=torch.int32, device=dev)
+        for i, c0 in enumerate(c0s):
+            n = min(k, L - c0)
+            self._window_call(h, mels, olens, starts[i], B, L, n, audio[:, c0 * HOP:], L * HOP, status[i: i + 1], ws)
+        bits = torch.tensor([_lib.FS2_MELGAN_BAD_LENGTH, _lib.FS2_MELGAN_RANGE, _lib.FS2_MELGAN_BAD_START], dtype=torch.int32, device=dev)
+        self._check_status(((status[:, None] & bits) != 0).any(0).int().mul(bits).sum().reshape(1))
         return audio, olens * HOP
 
     @staticmethod

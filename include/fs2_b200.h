@@ -425,6 +425,20 @@ int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float*
 int fs2_melgan_workspace_bytes(fs2_melgan_gen* m, int B, int Lmax, size_t* bytes);
 int fs2_melgan(fs2_melgan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
                size_t ws_bytes, void* stream);
+/* A window of the same audio (DESIGN.md section 11): for every utterance b, audio row b (audio_ld >= n_frames * 256
+ * samples apart, n_frames * 256 written) holds samples [starts[b] * 256, min(starts[b] + n_frames, olens[b]) * 256) of
+ * utterance b, bit-identical to the same samples of fs2_melgan on the whole batch in every math mode, then +0.  A row
+ * with starts[b] >= olens[b] is all +0.  starts [B] is a device array, so one captured call serves every step of a stream.
+ * Only mel frames [starts[b] - 6, starts[b] + n_frames + 6) below olens[b] are read.  The workspace depends on B and
+ * n_frames only; the limits apply to the window's B * (256 * n_frames + 36) rows (below 2^31, at most 65535 * 128 in
+ * FS2_MATH_FP32), and (Lmax + 10) * 256 must stay below 2^31.  No allocation, no synchronisation; it enqueues the same
+ * kernels as fs2_melgan.  *status: the bits of fs2_melgan (FS2_MELGAN_RANGE only for rows whose values equal the whole
+ * call's) and
+ *   FS2_MELGAN_BAD_START   some starts[b] < 0; that row is +0. */
+#define FS2_MELGAN_BAD_START 4
+int fs2_melgan_window_workspace_bytes(fs2_melgan_gen* m, int B, int n_frames, size_t* bytes);
+int fs2_melgan_window(fs2_melgan_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax,
+                      int n_frames, float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream);
 /* Single MelGAN layers on fs2_melgan's code paths (used by the per-layer tests).  Weights come in torch's layouts and are
  * packed into a stream-ordered temporary as fs2_melgan_load packs them.  status (device int) is set to 0 or
  * FS2_MELGAN_RANGE.  x 16-byte and out 32-byte aligned.
