@@ -27,8 +27,10 @@
 // in turn; warpgroups 1 and 2 "ping-pong": the CTA's k-th tile belongs wholly to warpgroup k & 1, which issues the wgmma
 // chains of both 64-row halves on each of the tile's ring stages (BN accumulator registers per thread; setmaxnreg moves
 // registers from the producer warpgroup), releases a stage as soon as the MMAs that read it have completed (one stage
-// stays in flight), then runs the epilogue straight from the accumulator registers (bias / ReLU / tanh / residual, fp32
-// rows, operand planes, or the transposed V third) while the other warpgroup already issues the next tile's MMAs.  An
+// stays in flight), then runs the epilogue (bias / ReLU / tanh / residual, fp32 rows, operand planes, or the transposed
+// V third) while the other warpgroup already issues the next tile's MMAs.  The epilogue goes through a small staging area
+// in shared memory, 16 columns at a time (Cfg::SW), so that one rolled loop with tile-uniform choices stores whole row
+// segments and V runs of up to 128 time steps; where the ring leaves no room for it, it runs from the registers.  An
 // mbarrier pair makes the two main loops strictly alternate (see the consumer loop), so the tensor cores do not wait for
 // an epilogue.  A row's K loop (the MMAs that accumulate it, and their order) depends neither on its tile nor on the
 // warpgroup, so results do not depend on the schedule (per-utterance bit-identity, DESIGN.md §5).
@@ -75,13 +77,26 @@ struct TcParams {
   const int64_t* lens;
 };
 
+// Epilogue staging (per consumer warpgroup): one slice of SW columns of its 128-row tile, either row-major (SW floats per
+// row, 16-byte chunks XOR-swizzled by row) or, for the transposed V third, column-major (VT_PITCH floats per column,
+// rows XOR-swizzled in 4-row groups by row / 32).  Both patterns make the fragment writes and the read-back free of
+// bank conflicts.
+constexpr int VT_PITCH = BM + 4;
+constexpr int stage_area(int sw) { return 2 * 4 * sw * VT_PITCH; }   // two warpgroups; the column-major form is the larger
+
 template <int BN, bool PRECISE, bool HALF = false>
 struct Cfg {
   static constexpr int B_BYTES = BN * BK * 4;
   static constexpr int STAGE_BYTES = (PRECISE ? 2 : 1) * (A_BYTES + B_BYTES);   // [A hi][A lo][B hi][B lo]
   static_assert(!PRECISE || HALF, "the error-compensated family is 3xF16");
   static constexpr int STAGES = (RING_BUDGET / STAGE_BYTES) > 8 ? 8 : (RING_BUDGET / STAGE_BYTES);
-  static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 + 256;
+  static constexpr int RING = STAGES * STAGE_BYTES;
+  // staging slice width in the shared memory the ring leaves over; 0: no room (f16 / tf32 at BN = 128), the epilogue
+  // then runs straight from the accumulator registers
+  static constexpr int SW = RING + stage_area(16) <= RING_BUDGET ? 16 : RING + stage_area(8) <= RING_BUDGET ? 8 : 0;
+  static constexpr int STG_BYTES = SW ? stage_area(SW) : 0;
+  static constexpr size_t SMEM = (size_t)RING + STG_BYTES + 1024 + 256;
+  static_assert(SMEM <= 227 * 1024 && BN % (SW ? SW : 16) == 0, "staging must fit beside the ring and divide the tile");
   static constexpr int BKE = HALF ? 2 * BK : BK;           // K elements per pipeline step
   static constexpr int A_LO = A_BYTES;                      // offsets inside a stage
   static constexpr int B_HI = PRECISE ? 2 * A_BYTES : A_BYTES;
@@ -105,6 +120,39 @@ __device__ __forceinline__ void mma_tile(float* d, uint64_t a, uint64_t b, uint3
   } else if constexpr (BN - C0 >= 16) {
     if constexpr (HALF) wgmma_f16_n16(d + C0 / 2, a, b + (C0 * 128 >> 4), acc); else wgmma_tf32_n16(d + C0 / 2, a, b + (C0 * 128 >> 4), acc);
     mma_tile<BN, HALF, C0 + 16>(d, a, b, acc);
+  }
+}
+
+__device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+// row-major staging: physical 16-byte chunk of logical chunk c in row r is c ^ row_swz(r); column-major: row r sits at
+// r ^ col_swz(r)
+template <int SW>
+__device__ __forceinline__ int row_swz(int r) { return SW == 16 ? 3 * ((r >> 1) & 1) : (r >> 2) & 1; }
+__device__ __forceinline__ int col_swz(int r) { return r ^ ((r >> 5) << 2); }
+
+// Writes slice s (columns SW s .. SW s + SW - 1 of the warpgroup's 128 x BN accumulators) to its staging area.  The
+// accumulators need constant register indices: one branch per slice.
+template <int BN, int SW, int S = 0>
+__device__ __forceinline__ void stage_slice(const float* d, int s, float* stg, bool col_major, int wq, int lane) {
+  if constexpr (S < BN / SW) {
+    if (s != S) { stage_slice<BN, SW, S + 1>(d, s, stg, col_major, wq, lane); return; }
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) {
+#pragma unroll
+      for (int jj = 0; jj < SW / 8; ++jj) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float* v = d + hf * (BN / 2) + 4 * (S * (SW / 8) + jj) + 2 * h;
+          const int row = 64 * hf + 16 * wq + (lane >> 2) + 8 * h, col = 8 * jj + 2 * (lane & 3);
+          if (col_major) {
+            stg[col * VT_PITCH + col_swz(row)] = v[0];
+            stg[(col + 1) * VT_PITCH + col_swz(row)] = v[1];
+          } else {
+            *reinterpret_cast<float2*>(stg + row * SW + 4 * ((col >> 2) ^ row_swz<SW>(row)) + (col & 3)) = make_float2(v[0], v[1]);
+          }
+        }
+      }
+    }
   }
 }
 
@@ -191,27 +239,45 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     const bool has_res = resid != nullptr;
     const float oscale = p.a_inv * (p.w_inv ? __ldg(p.w_inv) : 1.0f);   // exact power of two (1 in the tf32 family)
     float d[BN];                                  // [hf][BN / 2]: the accumulators of the tile's two 64-row halves
+    constexpr int SW = C::SW, LPR = SW / 8;       // staged epilogue: slice width, threads per row (8 columns each)
+    float* stg = reinterpret_cast<float*>(tiles + (size_t)C::RING + 256) + cg * (C::STG_BYTES / 8);
+    const int tid = threadIdx.x - 128 * (cg + 1);
     int n = 0;                                    // ring position: advanced past the other warpgroup's tiles as well
     int k = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++k) {
       int n0, b, t0, packed;
       const int tile_steps = tile_coords(tile, n0, b, t0, packed) ? 0 : steps;
       if ((k & 1) != cg) { n += tile_steps; continue; }
-      long m[4]; bool row_ok[4], row_zero[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {              // i = 2 hf + h
-        const int row = 64 * (i >> 1) + r_lo + 8 * (i & 1);
+      // row of the tile -> global row mm; ok: the row exists; zero: per-utterance mode, the row lies past lens;
+      // *left: rows of the utterance from this one on that exist and lie before lens
+      auto row_at = [&](int row, long& mm, bool& ok, bool& zero, int* left = nullptr) {
         int bb = b, t = t0 + row;
-        bool ok = t < p.L;                       // flat mode: L == total rows
+        ok = t < p.L;                            // flat mode: L == total rows
         if (packed >= 0) {                       // packed tail tile: 16-row granule g of the tile -> utterance b + g / gn
           const int g = row >> 4, u = g / p.gn, gi = g - u * p.gn;
           bb += u;
           t = t0 + gi * 16 + (row & 15);
           ok = u < p.upt && bb < p.B && t < p.L;
         }
-        m[i] = (long)bb * p.L + t; row_ok[i] = ok;
-        row_zero[i] = ok && p.lens != nullptr && t >= p.lens[bb];
-        if (has_res && ok) prefetch_l2(resid + m[i] * ldr + n0);   // residual rows -> L2 while the main loop runs
+        mm = (long)bb * p.L + t;
+        zero = ok && p.lens != nullptr && t >= p.lens[bb];
+        if (left) *left = ok && !zero ? (p.lens != nullptr && p.lens[bb] < p.L ? (int)p.lens[bb] : p.L) - t : 0;
+      };
+      const bool to_vt = (p.vt_out != nullptr || p.vtp != nullptr) && n0 >= p.vt_col0;   // tile-uniform (tile widths divide the V third)
+      long m[4]; bool row_ok[4], row_zero[4];    // direct epilogue: the thread's accumulator rows 64 hf + r_lo + 8 h
+      if constexpr (SW == 0) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {            // i = 2 hf + h
+          row_at(64 * (i >> 1) + r_lo + 8 * (i & 1), m[i], row_ok[i], row_zero[i]);
+          if (has_res && row_ok[i]) prefetch_l2(resid + m[i] * ldr + n0);   // residual rows -> L2 while the main loop runs
+        }
+      } else if (has_res) {
+#pragma unroll
+        for (int i = 0; i < LPR; ++i) {
+          long mm; bool ok, zero;
+          row_at(tid / LPR + (BM / LPR) * i, mm, ok, zero);
+          if (ok) prefetch_l2(resid + mm * ldr + n0);   // residual rows -> L2 while the main loop runs
+        }
       }
       // Main loops alternate between the warpgroups: this tile's starts once the other warpgroup has issued the MMAs of the
       // CTA's previous tile (it arrives even for a dead tile).  That keeps the tensor cores fed by one warpgroup while the
@@ -257,10 +323,124 @@ tap_gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         for (int i = 0; i < BN; ++i) d[i] = 0.f;
       }
 
+      if constexpr (SW > 0) {
+        // ---- staged epilogue: per slice, the accumulators go to shared memory and come back as whole row segments
+        // (8 columns per thread, LPR threads per row) or, for the V third, as column runs of 8 consecutive rows ----
+        const bool res16 = (reinterpret_cast<uintptr_t>(resid) & 15) == 0;
+        // V tiles: this thread's rows r8 .. r8 + 7 lie in one 16-row granule, so the rows to store (ok, not past lens) are
+        // its first nv, with global rows mm0 + i; vrun: they form one aligned 16-byte run of a vt row
+        const int r8 = 8 * (tid & 15);
+        auto vt_row = [&](int mm) {              // vt[(ub * heads + h) * dk + d][ut] for h * dk + d = 0 (B * L < 2^31 rows)
+          const int ub = mm / p.vt_L;
+          return (long)ub * p.vt_heads * p.vt_dk * p.vt_lpad + (mm - ub * p.vt_L);
+        };
+        long mm0 = 0, vo = 0; int nv = 0; bool vrun = false;
+        if (to_vt) {
+          bool ok, zero;
+          row_at(r8, mm0, ok, zero, &nv);
+          nv = nv < 8 ? nv : 8;
+          vo = vt_row(mm0);
+          vrun = nv == 8 && (int)mm0 % p.vt_L + 8 <= p.vt_L && (vo & 7) == 0 && p.vtp != nullptr &&
+                 (reinterpret_cast<uintptr_t>(p.vtp) & 15) == 0;
+        }
+#pragma unroll 1
+        for (int s = 0; s < BN / SW; ++s) {
+          named_bar_sync(1 + cg, 128);           // the warpgroup has read the previous slice
+          stage_slice<BN, SW>(d, s, stg, to_vt, wq, lane);
+          named_bar_sync(1 + cg, 128);
+          if (to_vt) {
+#pragma unroll
+            for (int pass = 0; pass < SW / 8; ++pass) {
+              const int cl = (tid >> 4) + 8 * pass, col = n0 + s * SW + cl;
+              const float bias = p.bias ? __ldg(p.bias + col) : 0.f;
+              const float4 x0 = *reinterpret_cast<const float4*>(stg + cl * VT_PITCH + col_swz(r8));
+              const float4 x1 = *reinterpret_cast<const float4*>(stg + cl * VT_PITCH + col_swz(r8 + 4));
+              float v[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+#pragma unroll
+              for (int e = 0; e < 8; ++e) v[e] = fmaf(v[e], oscale, bias);
+              const long oc = (long)(col - p.vt_col0) * p.vt_lpad;
+              if (vrun) {                        // 16 consecutive threads: 128 time steps of one vt row
+                uint4 hi, lo;
+                split_pair(v[0], v[1], hi.x, lo.x); split_pair(v[2], v[3], hi.y, lo.y);
+                split_pair(v[4], v[5], hi.z, lo.z); split_pair(v[6], v[7], hi.w, lo.w);
+                *reinterpret_cast<uint4*>(p.vtp + vo + oc) = hi;
+                if (p.vtp_lo != nullptr) *reinterpret_cast<uint4*>(p.vtp_lo + vo + oc) = lo;
+                continue;
+              }
+#pragma unroll 1
+              for (int i = 0; i < nv; ++i) {     // rows that cross an utterance or are not 16-byte aligned in vt
+                const float x = fmaf(stg[cl * VT_PITCH + col_swz(r8 + i)], oscale, bias);
+                const long o = vt_row(mm0 + i) + oc;
+                if (p.vt_out != nullptr) { p.vt_out[o] = x; continue; }
+                uint32_t hi, lo;
+                split_pair(x, x, hi, lo);
+                p.vtp[o] = __ushort_as_half((unsigned short)hi);
+                if (p.vtp_lo != nullptr) p.vtp_lo[o] = __ushort_as_half((unsigned short)lo);
+              }
+            }
+            continue;
+          }
+          const int h = tid % LPR, col = n0 + s * SW + 8 * h;
+          float bv[8];
+#pragma unroll
+          for (int e = 0; e < 8; ++e) bv[e] = p.bias ? __ldg(p.bias + col + e) : 0.f;
+#pragma unroll 1
+          for (int i = 0; i < LPR; ++i) {
+            const int row = tid / LPR + (BM / LPR) * i;
+            long mm; bool ok, zero;
+            row_at(row, mm, ok, zero);
+            if (!ok) continue;
+            // every load of the row (residual) is issued before its stores: a caller's residual may be the output
+            float rv[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+            if (has_res) {
+              const float* rp = resid + mm * ldr + col;
+              if (res16) {
+                const float4 a = __ldg(reinterpret_cast<const float4*>(rp)), c = __ldg(reinterpret_cast<const float4*>(rp + 4));
+                rv[0] = a.x; rv[1] = a.y; rv[2] = a.z; rv[3] = a.w; rv[4] = c.x; rv[5] = c.y; rv[6] = c.z; rv[7] = c.w;
+              } else {
+#pragma unroll
+                for (int e = 0; e < 8; e += 2) {
+                  const float2 a = __ldg(reinterpret_cast<const float2*>(rp + e));
+                  rv[e] = a.x; rv[e + 1] = a.y;
+                }
+              }
+            }
+            const float* sr = stg + row * SW;
+            const float4 x0 = *reinterpret_cast<const float4*>(sr + 4 * ((2 * h) ^ row_swz<SW>(row)));
+            const float4 x1 = *reinterpret_cast<const float4*>(sr + 4 * ((2 * h + 1) ^ row_swz<SW>(row)));
+            float v[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              v[e] = fmaf(v[e], oscale, bv[e]);
+              if (act == ACT_RELU) v[e] = fmaxf(v[e], 0.f);
+              else if (act == ACT_TANH) v[e] = tanhf(v[e]);
+              if (has_res) v[e] += rv[e];
+              if (zero) v[e] = 0.f;
+            }
+            if (HALF && p.outp != nullptr) {     // operand planes of the next contraction
+              const long off = mm * p.ldo_p + col;
+              if (p.outp_lo != nullptr) {
+                uint4 hi, lo;
+                split_pair(v[0], v[1], hi.x, lo.x); split_pair(v[2], v[3], hi.y, lo.y);
+                split_pair(v[4], v[5], hi.z, lo.z); split_pair(v[6], v[7], hi.w, lo.w);
+                *reinterpret_cast<uint4*>(p.outp + off) = hi;
+                *reinterpret_cast<uint4*>(p.outp_lo + off) = lo;
+              } else {
+                *reinterpret_cast<uint4*>(p.outp + off) = make_uint4(hi_pair(v[0], v[1]), hi_pair(v[2], v[3]), hi_pair(v[4], v[5]), hi_pair(v[6], v[7]));
+              }
+            }
+            if (out != nullptr) {
+              *reinterpret_cast<float4*>(out + mm * ldo + col) = make_float4(v[0], v[1], v[2], v[3]);
+              *reinterpret_cast<float4*>(out + mm * ldo + col + 4) = make_float4(v[4], v[5], v[6], v[7]);
+            }
+          }
+        }
+        continue;
+      }
+
       // ---- epilogue from registers: element pairs (row, columns c, c + 1) ----
       // Row by row, every load of a row (bias, residual) is issued before its first store: as far as the compiler knows,
       // the stores may alias the loads, so interleaving them would serialise one load latency per column pair.
-      const bool to_vt = (p.vt_out != nullptr || p.vtp != nullptr) && n0 >= p.vt_col0;   // tile-uniform (tile widths divide the V third)
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         if (!row_ok[i] || (to_vt && row_zero[i])) continue;
