@@ -45,6 +45,7 @@ FS2_VOC_BAD_LENGTH, FS2_VOC_RANGE = 1, 2     # bits of fs2_griffin_lim's / fs2_m
 FS2_MELGAN_BAD_LENGTH, FS2_MELGAN_RANGE = 1, 2   # bits of fs2_melgan's device status word
 FS2_MELGAN_BAD_START = 4                          # and of fs2_melgan_window's
 FS2_WAVEGLOW_BAD_LENGTH, FS2_WAVEGLOW_RANGE = 1, 2   # bits of fs2_waveglow's device status word
+FS2_WAVEGLOW_BAD_START = 4                           # and of fs2_waveglow_window's
 
 _P, _I, _F, _L, _SZ = C.c_void_p, C.c_int, C.c_float, C.c_int64, C.c_size_t
 
@@ -126,6 +127,8 @@ SIGNATURES = {
     "fs2_waveglow_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
     "fs2_waveglow": [_P, _P, _P, _I, _I, C.c_double, _P, _P, _P, _P, _P, _SZ, _P],
     "fs2_waveglow_noise": [_P, _P, _I, _I, _P, _P],
+    "fs2_waveglow_window_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_waveglow_window": [_P, _P, _P, _P, _I, _I, _I, C.c_double, _P, _P, _P, _L, _P, _P, _SZ, _P],
     "fs2_peer_alloc": [_SZ, C.POINTER(_P), _P],
     "fs2_peer_free": [_P],
     "fs2_peer_open": [_P, C.POINTER(_P)],

@@ -22,10 +22,18 @@
 // The flow state [B * Ls][8] holds the audio channels in columns 8 - c .. 7, and starts as fp32(sigma * z) in all eight:
 // z's channels 0-1 and 2-3 are exactly the early noise prepended after flows 4 and 8, so the concatenation costs nothing.
 // After flow 0 the state is the audio itself ([B, Ls, 8] row-major = [B, Lmax * 256]), so the last flow writes `audio`.
-// Launches per call: 4 + 12 * 41 = 496, plus 1 (the cond planes) in f16 / 3xF16.
+// Launches per call: 4 + 12 * 41 = 496, plus 1 (the cond planes) in f16 / 3xF16; a window adds 1 (its audio copy).
 //
 // A GEMM row depends only on its own input rows (the in-layer GEMM: rows t, t +- 2^i of its own utterance, zero outside
 // [0, olens * 32)), in a fixed K order, so per-utterance results do not depend on the batch.
+//
+// Windows (fs2_waveglow_window, DESIGN.md section 12): the same kernels and GEMMs on one buffer per utterance that holds
+// global frames [f0, f1) = [max(0, s - H), min(olens, s + n + H)) around the core [s, s + n), H = 96 frames, every buffer
+// (n + 2H) * 32 step rows long (window descriptors [kWinRows][B] in the workspace; nullptr = the whole call).  A flow
+// reaches 255 step rows on each side, so halo rows at a side that is not an utterance edge (f0 > 0, f1 < olens) differ
+// from the whole call's by at most 255 more rows per flow, and the core is exact after all 12.  The noise, the upsampling
+// operand and the cond planes are keyed by global frames and steps, so they are exact everywhere in the buffer; start and
+// gate range-check only rows whose values equal the whole call's (exact_row).
 #include <math.h>
 #include <string.h>
 
@@ -39,6 +47,13 @@ constexpr int kCond = kMels * kGroup;          // 640 cond channels per step
 constexpr int kUpTaps = 4, kUpK = kUpTaps * kMels, kUpN = kMels * kHop, kUpKernel = kUpTaps * kHop;
 constexpr int kPerFlow = 2 + 6 * kLayers + 3;  // tensors per flow in fs2_waveglow_load
 constexpr int kTensors = 2 + kFlows * kPerFlow;
+// ---- window plan (DESIGN.md section 12) ----
+constexpr int kFlowReach = (1 << kLayers) - 1;                              // 8 k = 3 layers at dilation 2^i: 255 step rows
+constexpr int kHalo = (kFlows * kFlowReach + kSteps - 1) / kSteps;          // 96 frames on each side of a window's core
+static_assert(kHalo * kSteps >= kFlows * kFlowReach, "the halo must cover the 12 flows' reach");
+// window descriptors, one [B] row each: frames and step rows of the buffer (the GEMMs' lens), its first global frame, the
+// utterance's frame count (0 when invalid), the core's first frame in the buffer and its frame count (0: an empty window)
+enum { kWinF, kWinS, kWinF0, kWinN, kWinCore0, kWinCoreN, kWinRows };
 
 __host__ __device__ inline int flow_channels(int k) { return k < 4 ? 8 : k < 8 ? 6 : 4; }
 
@@ -47,7 +62,15 @@ inline int grid_for(long n, int block, int cap = 132 * 8) {
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
-// four GEMM-operand values at element offset off (a multiple of 4) of a [rows][K] operand; plane = rows * K
+// local step row t of utterance b's window buffer holds the whole call's values: not within `margin` rows of a side that
+// is not an utterance edge
+__device__ __forceinline__ bool exact_row(const int64_t* __restrict__ win, int B, int b, int t, int margin) {
+  const int64_t f0 = win[kWinF0 * B + b], nf = win[kWinF * B + b], ns = win[kWinS * B + b];
+  return (f0 == 0 || t >= margin) && (f0 + nf == win[kWinN * B + b] || t < ns - margin);
+}
+
+// four GEMM-operand values at element offset off (a multiple of 4) of a [rows][K] operand; plane = rows * K; status ==
+// nullptr: a halo row, not range-checked
 template <int OUT>
 __device__ __forceinline__ void put_quad(float4 v, long off, float* __restrict__ out32, __half* __restrict__ outp, long plane,
                                          int* __restrict__ status) {
@@ -55,7 +78,7 @@ __device__ __forceinline__ void put_quad(float4 v, long off, float* __restrict__
     *reinterpret_cast<float4*>(out32 + off) = v;
     return;
   }
-  if (!(fabsf(v.x) <= kPlaneMax && fabsf(v.y) <= kPlaneMax && fabsf(v.z) <= kPlaneMax && fabsf(v.w) <= kPlaneMax))
+  if (status && !(fabsf(v.x) <= kPlaneMax && fabsf(v.y) <= kPlaneMax && fabsf(v.z) <= kPlaneMax && fabsf(v.w) <= kPlaneMax))
     atomicOr(status, FS2_WAVEGLOW_RANGE);               // saturation is reported, not hidden
   if (OUT == OUT_HILO) {
     uint2 hi, lo;
@@ -86,6 +109,32 @@ __global__ void wg_prep_kernel(const int64_t* __restrict__ olens, int B, int L, 
   if (threadIdx.x == 0) *status = bad ? FS2_WAVEGLOW_BAD_LENGTH : 0;
 }
 
+// one CTA, a window of nf frames from starts[b]: the kWinRows descriptors (see the top of the file) of the core
+// [starts[b], min(starts[b] + nf, olens[b])), all 0 when that is empty or olens[b] is invalid; *status = 0 or
+// FS2_WAVEGLOW_BAD_LENGTH | FS2_WAVEGLOW_BAD_START (some starts[b] < 0).  Runs first, as wg_prep_kernel does.
+__global__ void wg_win_desc_kernel(const int64_t* __restrict__ olens, const int64_t* __restrict__ starts, int B, int L, int nf,
+                                   int64_t* __restrict__ win, int* __restrict__ status) {
+  __shared__ int bad;
+  if (threadIdx.x == 0) bad = 0;
+  __syncthreads();
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    const int64_t n = olens[b], s = starts[b];
+    const bool ok = n >= 1 && n <= L;
+    if (!ok) atomicOr(&bad, FS2_WAVEGLOW_BAD_LENGTH);
+    if (s < 0) atomicOr(&bad, FS2_WAVEGLOW_BAD_START);
+    const bool live = ok && s >= 0 && s < n;
+    const int64_t c1 = live ? min(s + nf, n) : 0, f0 = live ? max(s - kHalo, (int64_t)0) : 0, f1 = live ? min(c1 + kHalo, n) : 0;
+    win[kWinF * B + b] = f1 - f0;
+    win[kWinS * B + b] = (f1 - f0) * kSteps;
+    win[kWinF0 * B + b] = f0;
+    win[kWinN * B + b] = ok ? n : 0;
+    win[kWinCore0 * B + b] = live ? s - f0 : 0;
+    win[kWinCoreN * B + b] = live ? c1 - s : 0;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) *status = bad;
+}
+
 // Four standard normals for channels 4q .. 4q + 3 of step t of the utterance with seed s: Philox4x32-10 with key
 // (s mod 2^32, s / 2^32) and counter (t, q, 0, 0), Box-Muller on two pairs of 23-bit uniforms in (0, 1).
 __device__ __forceinline__ float4 normal4(uint64_t seed, uint32_t t, uint32_t q) {
@@ -99,11 +148,13 @@ __device__ __forceinline__ float4 normal4(uint64_t seed, uint32_t t, uint32_t q)
   return make_float4(r0 * c0, r0 * s0, r1 * c1, r1 * s1);
 }
 
-// The standard-normal draw z [B, 8, Ls] for the steps t < n_b = min(lens[b] * mult, Ls): from zin (same layout) or from
+// The standard-normal draw z [B, 8, Ls] for the steps t < n_b = min(lens[b] * mult, Ls): from zin ([B, 8, ldz]) or from
 // Philox keyed by seeds[b].  state [B * Ls][8] (nullable) = fp32(sigma * z), the product in double and rounded once;
-// zout [B, 8, Ls] (nullable) = z; both 0 for t >= n_b.  zin is never read there.
-__global__ void wg_noise_kernel(const float* __restrict__ zin, const int64_t* __restrict__ seeds, const int64_t* __restrict__ lens,
-                                int mult, int B, int Ls, double sigma, float* __restrict__ state, float* __restrict__ zout) {
+// zout [B, 8, Ls] (nullable) = z; both 0 for t >= n_b.  zin is never read there.  win (a window): local step t is global
+// step f0 * 32 + t, in zin and in the Philox counter alike.
+__global__ void wg_noise_kernel(const float* __restrict__ zin, int ldz, const int64_t* __restrict__ seeds, const int64_t* __restrict__ lens,
+                                const int64_t* __restrict__ win, int mult, int B, int Ls, double sigma, float* __restrict__ state,
+                                float* __restrict__ zout) {
   const long total = (long)B * Ls * 2;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const long row = i >> 1;
@@ -112,11 +163,12 @@ __global__ void wg_noise_kernel(const float* __restrict__ zin, const int64_t* __
     n = n < 0 ? 0 : (n > Ls ? Ls : n);
     float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
     if (t < n) {
+      const long tg = win ? win[kWinF0 * B + b] * kSteps + t : t;
       if (zin) {
-        const float* zb = zin + ((long)b * kGroup + 4 * q) * Ls + t;
-        z = make_float4(zb[0], zb[Ls], zb[2L * Ls], zb[3L * Ls]);
+        const float* zb = zin + ((long)b * kGroup + 4 * q) * ldz + tg;
+        z = make_float4(zb[0], zb[ldz], zb[2L * ldz], zb[3L * ldz]);
       } else {
-        z = normal4((uint64_t)seeds[b], (uint32_t)t, (uint32_t)q);
+        z = normal4((uint64_t)seeds[b], (uint32_t)tg, (uint32_t)q);
       }
     }
     if (state)
@@ -130,10 +182,12 @@ __global__ void wg_noise_kernel(const float* __restrict__ zin, const int64_t* __
 }
 
 // upsampling operand [B * L][4 * 80]: tap j of frame row t = mel frame t - 3 + j of its utterance, 0 outside [0, n).
-// Rows t >= n are not written (the GEMM writes 0 there); frames past olens[b] are never read.
+// Rows t >= n are not written (the GEMM writes 0 there); frames past olens[b] are never read.  mels has Lm frames per
+// utterance.  win (a window, n = the buffer's frames): row t is global frame f0 + t, and the source is 0 outside
+// [0, olens[b]), so every row equals the whole call's.
 template <int OUT>
-__global__ void wg_up_operand_kernel(const float* __restrict__ mels, const int64_t* __restrict__ lensF, int B, int L,
-                                     float* __restrict__ out32, __half* __restrict__ outp, int* __restrict__ status) {
+__global__ void wg_up_operand_kernel(const float* __restrict__ mels, const int64_t* __restrict__ lensF, const int64_t* __restrict__ win,
+                                     int B, int L, int Lm, float* __restrict__ out32, __half* __restrict__ outp, int* __restrict__ status) {
   constexpr int Q = kUpK / 4;
   const long rows = (long)B * L, total = rows * Q, plane = rows * kUpK;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -141,9 +195,9 @@ __global__ void wg_up_operand_kernel(const float* __restrict__ mels, const int64
     const int k = (int)(i - row * Q) * 4, j = k / kMels, c = k - j * kMels;
     const int b = (int)(row / L), t = (int)(row - (long)b * L), n = (int)lensF[b];
     if (t >= n) continue;
-    const int src = t - (kUpTaps - 1) + j;
+    const int src = t - (kUpTaps - 1) + j + (win ? (int)win[kWinF0 * B + b] : 0), lim = win ? (int)win[kWinN * B + b] : n;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (src >= 0 && src < n) v = *reinterpret_cast<const float4*>(mels + ((long)b * L + src) * kMels + c);
+    if (src >= 0 && src < lim) v = *reinterpret_cast<const float4*>(mels + ((long)b * Lm + src) * kMels + c);
     put_quad<OUT>(v, row * kUpK + k, out32, outp, plane, status);
   }
 }
@@ -165,10 +219,11 @@ __global__ void wg_planes_kernel(const float* __restrict__ x, const int64_t* __r
 
 // WN start: x[r][n] = bias[n] + sum_{q < h} w[n][q] * state[r][o + q] for t < lens[b], else 0 -- fp32 rows (the residual
 // stream) and, in the plane modes, the in-layer GEMM's operand planes.  Padded rows are written: the dilated taps read them.
+// win / margin (a window): only exact rows are range-checked.
 template <int OUT>
-__global__ void wg_start_kernel(const float* __restrict__ state, const int64_t* __restrict__ lens, int B, int Ls, int C, int o, int h,
-                                const float* __restrict__ w, const float* __restrict__ bias, float* __restrict__ x,
-                                __half* __restrict__ xp, int* __restrict__ status) {
+__global__ void wg_start_kernel(const float* __restrict__ state, const int64_t* __restrict__ lens, const int64_t* __restrict__ win,
+                                int margin, int B, int Ls, int C, int o, int h, const float* __restrict__ w, const float* __restrict__ bias,
+                                float* __restrict__ x, __half* __restrict__ xp, int* __restrict__ status) {
   const int Q = C / 4;
   const long rows = (long)B * Ls, total = rows * Q, plane = rows * C;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -188,16 +243,18 @@ __global__ void wg_start_kernel(const float* __restrict__ state, const int64_t* 
       }
     }
     *reinterpret_cast<float4*>(x + row * C + n) = v;
-    if (OUT != OUT_F32) put_quad<OUT>(v, row * C + n, nullptr, xp, plane, status);
+    if (OUT != OUT_F32)
+      put_quad<OUT>(v, row * C + n, nullptr, xp, plane, !win || exact_row(win, B, b, t, margin) ? status : nullptr);
   }
 }
 
 // gate: acts[r][c] = tanh(ia[r][c]) * sigmoid(ia[r][C + c]) as the res / skip GEMMs' operand (rows t >= lens[b] are not
 // written).  xchk (nullable, plane modes): the layer's input rows x, written as planes by the previous res GEMM's
-// epilogue, are range-checked here.
+// epilogue, are range-checked here.  win (a window): acts only at rows exact at `margin`, x at `xmargin`.
 template <int OUT>
-__global__ void wg_gate_kernel(const float* __restrict__ ia, const float* __restrict__ xchk, const int64_t* __restrict__ lens, int B,
-                               int Ls, int C, float* __restrict__ out32, __half* __restrict__ outp, int* __restrict__ status) {
+__global__ void wg_gate_kernel(const float* __restrict__ ia, const float* __restrict__ xchk, const int64_t* __restrict__ lens,
+                               const int64_t* __restrict__ win, int margin, int xmargin, int B, int Ls, int C, float* __restrict__ out32,
+                               __half* __restrict__ outp, int* __restrict__ status) {
   const int Q = C / 4;
   const long rows = (long)B * Ls, total = rows * Q, plane = rows * C;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -209,8 +266,8 @@ __global__ void wg_gate_kernel(const float* __restrict__ ia, const float* __rest
     const float4 g = *reinterpret_cast<const float4*>(ia + row * 2 * C + C + c);
     const float4 v = make_float4(tanhf(a.x) * (1.f / (1.f + expf(-g.x))), tanhf(a.y) * (1.f / (1.f + expf(-g.y))),
                                  tanhf(a.z) * (1.f / (1.f + expf(-g.z))), tanhf(a.w) * (1.f / (1.f + expf(-g.w))));
-    put_quad<OUT>(v, row * C + c, out32, outp, plane, status);
-    if (xchk) {
+    put_quad<OUT>(v, row * C + c, out32, outp, plane, !win || exact_row(win, B, b, t, margin) ? status : nullptr);
+    if (xchk && (!win || exact_row(win, B, b, t, xmargin))) {
       const float4 x = *reinterpret_cast<const float4*>(xchk + row * C + c);
       if (!(fabsf(x.x) <= kPlaneMax && fabsf(x.y) <= kPlaneMax && fabsf(x.z) <= kPlaneMax && fabsf(x.w) <= kPlaneMax))
         atomicOr(status, FS2_WAVEGLOW_RANGE);
@@ -272,6 +329,20 @@ __global__ void __launch_bounds__(256) wg_flow_kernel(const float* __restrict__ 
       for (int q = 0; q < c; ++q) y = fmaf(swi[lane * c + q], v[q], y);
       dst[lane] = y;
     }
+  }
+}
+
+// a window's audio: row b (ld samples apart) = the core's samples of the final state [B * Ls][8] (utterance b's samples
+// are contiguous there), then +0 up to nf * 256
+__global__ void wg_win_audio_kernel(const float* __restrict__ state, const int64_t* __restrict__ win, int B, int Ls, int nf,
+                                    float* __restrict__ audio, long ld) {
+  const int n = nf * kHop;
+  const long total = (long)B * n;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int b = (int)(i / n), t = (int)(i - (long)b * n);
+    float v = 0.f;
+    if (t < win[kWinCoreN * B + b] * kHop) v = state[(long)b * Ls * kGroup + win[kWinCore0 * B + b] * kHop + t];
+    audio[(long)b * ld + t] = v;
   }
 }
 
@@ -338,6 +409,7 @@ namespace fs2 {
 namespace {
 
 struct WgPlan {
+  int64_t* win;        // a window call: the kWinRows descriptors [kWinRows][B] (lensF and lensS are its first two rows)
   int64_t* lensF;      // [B] frame lengths (0 for a bad olens[b])
   int64_t* lensS;      // [B] step lengths = lensF * 32
   void* up_a;          // upsampling operand [B * L][320]
@@ -356,12 +428,20 @@ struct WgPlan {
 
 bool plane_mode(int mode) { return mode == FS2_MATH_F16 || mode == FS2_MATH_3XTF32; }
 
-WgPlan plan(Bump& b, int mode, int C, int B, int L) {
+// buffers of L frames per utterance: the whole call's (L = Lmax) or a window's (window, L = n_frames + 2H)
+WgPlan plan(Bump& b, int mode, int C, int B, int L, bool window = false) {
   const size_t frames = (size_t)B * L, rows = frames * kSteps;
   const bool planes = plane_mode(mode);
   WgPlan p;
-  p.lensF = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
-  p.lensS = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
+  if (window) {
+    p.win = (int64_t*)b.bytes((size_t)kWinRows * B * sizeof(int64_t));
+    p.lensF = p.win ? p.win + kWinF * B : nullptr;
+    p.lensS = p.win ? p.win + kWinS * B : nullptr;
+  } else {
+    p.win = nullptr;
+    p.lensF = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
+    p.lensS = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
+  }
   p.up_a = b.floats(frames * kUpK);                   // fp32 rows, or hi + lo planes: the same bytes
   p.state = b.floats(rows * kGroup);
   p.x[0] = b.floats(rows * C);
@@ -405,12 +485,92 @@ int check_size(const fs2_waveglow_net* m, int B, int L) {
   return FS2_OK;
 }
 
+// a window's limits apply to its rows: B buffers of (n_frames + 2H) * 32 step rows
+int check_window(const fs2_waveglow_net* m, int B, int nf) {
+  FS2_REQUIRE(B >= 1 && nf >= 1, "fs2_waveglow_window: need B >= 1 and n_frames >= 1 (got %d, %d)", B, nf);
+  const long rows = (long)B * ((long)nf + 2 * kHalo) * kSteps;
+  FS2_REQUIRE(rows < (1L << 31), "fs2_waveglow_window: B * (n_frames + 192) * 32 = %ld window rows exceed the int32 row index", rows);
+  FS2_REQUIRE(m->math_mode != FS2_MATH_FP32 || rows <= 65535L * 128,
+              "fs2_waveglow_window: B * (n_frames + 192) * 32 = %ld window rows exceed fp32 mode's limit of %ld", rows, 65535L * 128);
+  return FS2_OK;
+}
+
 template <typename K>
 int launch_flow(K kernel, int c, int C, const float* skip, const float* in, float* out, const int64_t* lens, int B, int Ls, int o,
                 const WFlow& f, cudaStream_t st) {
   const size_t smem = (size_t)(c * C + c * c + c) * sizeof(float);
   kernel<<<grid_for((long)B * Ls, 8), 256, smem, st>>>(skip, C, in, out, lens, B, Ls, o, f.end_w, f.end_b, f.winv);
   FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+// The inverse flow on the plan p: whole utterances (starts == nullptr; buffers of Lmax frames, audio written by the last
+// flow) or a window of nf frames from starts[b] (buffers of nf + 2H frames, the window descriptors p.win, the core copied
+// out by wg_win_audio_kernel).  audio rows ld samples apart.  Both enqueue the same kernels but the first and the last.
+int run(const fs2_waveglow_net* m, const WgPlan& p, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax,
+        int nf, double sigma, const int64_t* seeds, const float* z, float* audio, long ld, int* status, cudaStream_t st) {
+  const bool window = starts != nullptr;
+  const int L = window ? nf + 2 * kHalo : Lmax;
+  const int kind = out_kind(m->math_mode), C = m->C, Ls = L * kSteps;
+  const bool planes = plane_mode(m->math_mode);
+  const long rows = (long)B * Ls;
+  const int64_t* win = p.win;
+  int rc;
+
+  if (window)
+    wg_win_desc_kernel<<<1, 256, 0, st>>>(olens, starts, B, Lmax, nf, p.win, status);
+  else
+    wg_prep_kernel<<<1, 256, 0, st>>>(olens, B, Lmax, p.lensF, p.lensS, status);
+  FS2_LAUNCH_CHECK();
+  wg_noise_kernel<<<grid_for(rows * 2, 256), 256, 0, st>>>(z, Lmax * kSteps, seeds, p.lensS, win, 1, B, Ls, sigma, p.state, nullptr);
+  FS2_LAUNCH_CHECK();
+  {
+    auto k = pick(kind, wg_up_operand_kernel<OUT_HILO>, wg_up_operand_kernel<OUT_HI>, wg_up_operand_kernel<OUT_F32>);
+    k<<<grid_for((long)B * L * (kUpK / 4), 256), 256, 0, st>>>(mels, p.lensF, win, B, L, Lmax, (float*)p.up_a, (__half*)p.up_a, status);
+    FS2_LAUNCH_CHECK();
+  }
+  if ((rc = gemm(m, m->up, p.up_a, B, L, p.lensF, 1, nullptr, p.cond, nullptr, st))) return rc;
+  if (planes) {
+    auto k = kind == OUT_HILO ? wg_planes_kernel<OUT_HILO> : wg_planes_kernel<OUT_HI>;
+    k<<<grid_for(rows * (kCond / 4), 256), 256, 0, st>>>(p.cond, p.lensS, B, Ls, kCond, p.condp, status);
+    FS2_LAUNCH_CHECK();
+  }
+  const void* cond_a = planes ? (const void*)p.condp : (const void*)p.cond;
+  auto start = pick(kind, wg_start_kernel<OUT_HILO>, wg_start_kernel<OUT_HI>, wg_start_kernel<OUT_F32>);
+  auto gate = pick(kind, wg_gate_kernel<OUT_HILO>, wg_gate_kernel<OUT_HI>, wg_gate_kernel<OUT_F32>);
+  for (int k = kFlows - 1; k >= 0; --k) {
+    const WFlow& f = m->flows[k];
+    const int c = flow_channels(k), h = c / 2, o = kGroup - c;
+    const int exact = (kFlows - 1 - k) * kFlowReach;          // a window's rows are exact this far from an interior side
+    start<<<grid_for(rows * (C / 4), 256), 256, 0, st>>>(p.state, p.lensS, win, exact, B, Ls, C, o, h, f.start_w, f.start_b, p.x[0], p.xp,
+                                                         status);
+    FS2_LAUNCH_CHECK();
+    int cur = 0, sk = 0;
+    for (int i = 0; i < kLayers; ++i) {
+      if ((rc = gemm(m, f.cond[i], cond_a, B, Ls, p.lensS, 1, nullptr, p.cd, nullptr, st))) return rc;
+      const void* xa = planes ? (const void*)p.xp : (const void*)p.x[cur];
+      if ((rc = gemm(m, f.in[i], xa, B, Ls, p.lensS, 1 << i, p.cd, p.ia, nullptr, st))) return rc;
+      // layer i's input x is exact at exact + 2^i - 1, its in-layer output (and so acts and the next x) at exact + 2^(i+1) - 1
+      gate<<<grid_for(rows * (C / 4), 256), 256, 0, st>>>(p.ia, planes && i > 0 ? p.x[cur] : nullptr, p.lensS, win, exact + (2 << i) - 1,
+                                                           exact + (1 << i) - 1, B, Ls, C, (float*)p.acts, (__half*)p.acts, status);
+      FS2_LAUNCH_CHECK();
+      if (i < kLayers - 1) {
+        if ((rc = gemm(m, f.res[i], p.acts, B, Ls, p.lensS, 1, p.x[cur], p.x[cur ^ 1], p.xp, st))) return rc;
+        cur ^= 1;
+      }
+      if ((rc = gemm(m, f.skip[i], p.acts, B, Ls, p.lensS, 1, i ? p.skip[sk] : nullptr, p.skip[sk ^ 1], nullptr, st))) return rc;
+      sk ^= 1;
+    }
+    float* dst = k == 0 && !window ? audio : p.state;
+    rc = h == 4 ? launch_flow(wg_flow_kernel<4>, c, C, p.skip[sk], p.state, dst, p.lensS, B, Ls, o, f, st)
+       : h == 3 ? launch_flow(wg_flow_kernel<3>, c, C, p.skip[sk], p.state, dst, p.lensS, B, Ls, o, f, st)
+                : launch_flow(wg_flow_kernel<2>, c, C, p.skip[sk], p.state, dst, p.lensS, B, Ls, o, f, st);
+    if (rc) return rc;
+  }
+  if (window) {
+    wg_win_audio_kernel<<<grid_for((long)B * nf * kHop, 256), 256, 0, st>>>(p.state, p.win, B, Ls, nf, audio, ld);
+    FS2_LAUNCH_CHECK();
+  }
   return FS2_OK;
 }
 
@@ -540,7 +700,8 @@ int fs2_waveglow_noise(const int64_t* seeds, const int64_t* olens, int B, int Lm
   FS2_REQUIRE(seeds && olens && z, "fs2_waveglow_noise: null argument");
   FS2_REQUIRE(B >= 1 && Lmax >= 1 && (long)B * Lmax * kSteps < (1L << 31), "fs2_waveglow_noise: bad shape B=%d Lmax=%d", B, Lmax);
   const int Ls = Lmax * kSteps;
-  wg_noise_kernel<<<grid_for((long)B * Ls * 2, 256), 256, 0, (cudaStream_t)stream>>>(nullptr, seeds, olens, kSteps, B, Ls, 1.0, nullptr, z);
+  wg_noise_kernel<<<grid_for((long)B * Ls * 2, 256), 256, 0, (cudaStream_t)stream>>>(nullptr, Ls, seeds, olens, nullptr, kSteps, B, Ls, 1.0,
+                                                                                   nullptr, z);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
@@ -553,59 +714,39 @@ int fs2_waveglow(fs2_waveglow_net* m, const float* mels, const int64_t* olens, i
   FS2_REQUIRE(isfinite(sigma) && sigma >= 0.0, "fs2_waveglow: sigma must be finite and >= 0");
   int rc = check_size(m, B, Lmax);
   if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
   Bump b(ws, ws_bytes);
   WgPlan p = plan(b, m->math_mode, m->C, B, Lmax);
   if (!b.ok()) { set_error("fs2_waveglow: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
-  const int kind = out_kind(m->math_mode), C = m->C, Ls = Lmax * kSteps;
-  const bool planes = plane_mode(m->math_mode);
-  const long rows = (long)B * Ls;
+  return run(m, p, mels, olens, nullptr, B, Lmax, 0, sigma, seeds, z, audio, (long)Lmax * kHop, status, (cudaStream_t)stream);
+}
 
-  wg_prep_kernel<<<1, 256, 0, st>>>(olens, B, Lmax, p.lensF, p.lensS, status);
-  FS2_LAUNCH_CHECK();
-  wg_noise_kernel<<<grid_for(rows * 2, 256), 256, 0, st>>>(z, seeds, p.lensS, 1, B, Ls, sigma, p.state, nullptr);
-  FS2_LAUNCH_CHECK();
-  {
-    auto k = pick(kind, wg_up_operand_kernel<OUT_HILO>, wg_up_operand_kernel<OUT_HI>, wg_up_operand_kernel<OUT_F32>);
-    k<<<grid_for((long)B * Lmax * (kUpK / 4), 256), 256, 0, st>>>(mels, p.lensF, B, Lmax, (float*)p.up_a, (__half*)p.up_a, status);
-    FS2_LAUNCH_CHECK();
-  }
-  if ((rc = gemm(m, m->up, p.up_a, B, Lmax, p.lensF, 1, nullptr, p.cond, nullptr, st))) return rc;
-  if (planes) {
-    auto k = kind == OUT_HILO ? wg_planes_kernel<OUT_HILO> : wg_planes_kernel<OUT_HI>;
-    k<<<grid_for(rows * (kCond / 4), 256), 256, 0, st>>>(p.cond, p.lensS, B, Ls, kCond, p.condp, status);
-    FS2_LAUNCH_CHECK();
-  }
-  const void* cond_a = planes ? (const void*)p.condp : (const void*)p.cond;
-  auto start = pick(kind, wg_start_kernel<OUT_HILO>, wg_start_kernel<OUT_HI>, wg_start_kernel<OUT_F32>);
-  auto gate = pick(kind, wg_gate_kernel<OUT_HILO>, wg_gate_kernel<OUT_HI>, wg_gate_kernel<OUT_F32>);
-  for (int k = kFlows - 1; k >= 0; --k) {
-    const WFlow& f = m->flows[k];
-    const int c = flow_channels(k), h = c / 2, o = kGroup - c;
-    start<<<grid_for(rows * (C / 4), 256), 256, 0, st>>>(p.state, p.lensS, B, Ls, C, o, h, f.start_w, f.start_b, p.x[0], p.xp, status);
-    FS2_LAUNCH_CHECK();
-    int cur = 0, sk = 0;
-    for (int i = 0; i < kLayers; ++i) {
-      if ((rc = gemm(m, f.cond[i], cond_a, B, Ls, p.lensS, 1, nullptr, p.cd, nullptr, st))) return rc;
-      const void* xa = planes ? (const void*)p.xp : (const void*)p.x[cur];
-      if ((rc = gemm(m, f.in[i], xa, B, Ls, p.lensS, 1 << i, p.cd, p.ia, nullptr, st))) return rc;
-      gate<<<grid_for(rows * (C / 4), 256), 256, 0, st>>>(p.ia, planes && i > 0 ? p.x[cur] : nullptr, p.lensS, B, Ls, C, (float*)p.acts,
-                                                           (__half*)p.acts, status);
-      FS2_LAUNCH_CHECK();
-      if (i < kLayers - 1) {
-        if ((rc = gemm(m, f.res[i], p.acts, B, Ls, p.lensS, 1, p.x[cur], p.x[cur ^ 1], p.xp, st))) return rc;
-        cur ^= 1;
-      }
-      if ((rc = gemm(m, f.skip[i], p.acts, B, Ls, p.lensS, 1, i ? p.skip[sk] : nullptr, p.skip[sk ^ 1], nullptr, st))) return rc;
-      sk ^= 1;
-    }
-    float* dst = k == 0 ? audio : p.state;
-    rc = h == 4 ? launch_flow(wg_flow_kernel<4>, c, C, p.skip[sk], p.state, dst, p.lensS, B, Ls, o, f, st)
-       : h == 3 ? launch_flow(wg_flow_kernel<3>, c, C, p.skip[sk], p.state, dst, p.lensS, B, Ls, o, f, st)
-                : launch_flow(wg_flow_kernel<2>, c, C, p.skip[sk], p.state, dst, p.lensS, B, Ls, o, f, st);
-    if (rc) return rc;
-  }
+int fs2_waveglow_window_workspace_bytes(fs2_waveglow_net* m, int B, int n_frames, size_t* bytes) {
+  FS2_REQUIRE(m && bytes, "fs2_waveglow_window_workspace_bytes: null argument");
+  int rc = check_window(m, B, n_frames);
+  if (rc) return rc;
+  Bump b(nullptr, 0);
+  plan(b, m->math_mode, m->C, B, n_frames + 2 * kHalo, true);
+  *bytes = b.off + 256;
   return FS2_OK;
+}
+
+int fs2_waveglow_window(fs2_waveglow_net* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax,
+                        int n_frames, double sigma, const int64_t* seeds, const float* z, float* audio, int64_t audio_ld,
+                        int* status, void* ws, size_t ws_bytes, void* stream) {
+  FS2_REQUIRE(m && mels && olens && starts && audio && status && ws && (seeds || z), "fs2_waveglow_window: null argument");
+  FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "fs2_waveglow_window: mels must be 16-byte aligned");
+  FS2_REQUIRE(isfinite(sigma) && sigma >= 0.0, "fs2_waveglow_window: sigma must be finite and >= 0");
+  int rc = check_window(m, B, n_frames);
+  if (rc) return rc;
+  FS2_REQUIRE(Lmax >= 1 && (long)Lmax * kSteps < (1L << 31), "fs2_waveglow_window: need 1 <= Lmax and Lmax * 32 below 2^31 (got Lmax = %d)",
+              Lmax);
+  FS2_REQUIRE(audio_ld >= (int64_t)n_frames * kHop, "fs2_waveglow_window: audio_ld = %lld below n_frames * 256 = %ld",
+              (long long)audio_ld, (long)n_frames * kHop);
+  Bump b(ws, ws_bytes);
+  WgPlan p = plan(b, m->math_mode, m->C, B, n_frames + 2 * kHalo, true);
+  if (!b.ok()) { set_error("fs2_waveglow_window: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
+  FS2_REQUIRE(m->loaded, "fs2_waveglow_window: weights not loaded (fs2_waveglow_load)");
+  return run(m, p, mels, olens, starts, B, Lmax, n_frames, sigma, seeds, z, audio, (long)audio_ld, status, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -29,6 +29,7 @@ N_MELS = 80
 N_GROUP = 8
 STEPS = HOP // N_GROUP              # step rows (groups of 8 samples) per mel frame
 N_FLOWS, N_LAYERS = 12, 8
+HALO = 96                           # frames a window's buffer holds on each side of its core: ceil(12 * 255 / 32)
 
 
 def flow_channels(k: int) -> int:
@@ -84,7 +85,12 @@ class WaveGlowVocoder(nn.Module):
     The flows receive fp32(sigma * z).
 
     math_mode: "3xf16" (default, fp32-class), "f16", "tf32" or "fp32" for the GEMMs.  One host read per call (the
-    device-side length and range checks)."""
+    device-side length and range checks).
+
+    Streaming (DESIGN.md section 12): `window(mels, olens, starts, n_frames, seed=...)` computes n_frames frames of audio
+    per utterance from starts[b], bit-identical to the same samples of `forward` with the same noise; `stream(...)` yields
+    lockstep windows whose concatenation is `forward`, and `forward(..., chunk_frames=k)` computes the whole call's bits
+    window by window.  A window's workspace depends on B and n_frames only."""
 
     def __init__(self, n_channels: int = 512, math_mode: str = "3xf16"):
         super().__init__()
@@ -105,6 +111,7 @@ class WaveGlowVocoder(nn.Module):
         self.convinv = nn.ModuleList([_Inv(flow_channels(k)) for k in range(N_FLOWS)])
         self._handles = {}       # device index -> (fs2_waveglow_net*, parameter fingerprint it was loaded from)
         self._ws = {}            # device index -> workspace tensor
+        self._wws = {}           # device index -> window workspace tensor
         self._epoch = 0
 
     def __del__(self):
@@ -236,9 +243,10 @@ class WaveGlowVocoder(nn.Module):
             self._ws[device.index] = ws
         return ws
 
-    def _inputs(self, mels, olens, sigma, seed, z):
+    def _inputs(self, mels, olens, sigma, seed, z, check_size=None):
         """Validated (mels fp32, olens int64, B, Lmax, sigma, seeds or None, z fp32 or None); every check that needs no
-        device runs before the one that asks for CUDA tensors."""
+        device runs before the one that asks for CUDA tensors.  check_size(B, Lmax): the limits (default: the whole
+        call's)."""
         if not torch.is_tensor(mels) or mels.dim() != 3 or mels.shape[2] != N_MELS or mels.shape[0] == 0 or mels.shape[1] == 0:
             raise ValueError(f"mels must be a non-empty [B, Lmax, {N_MELS}] tensor")
         if not mels.dtype.is_floating_point:
@@ -259,7 +267,7 @@ class WaveGlowVocoder(nn.Module):
             seeds = self._seeds(seed, B, mels.device)
         if not mels.is_cuda or not olens.is_cuda or (z is not None and z.device != mels.device):
             raise ValueError("mels, olens and z must be CUDA tensors on one device (the H100 path has no CPU fallback)")
-        self._check_size(B, L)
+        (check_size or self._check_size)(B, L)
         if z is not None:
             z = z.to(torch.float32).contiguous()
         return mels.to(torch.float32).contiguous(), olens.to(device=mels.device, dtype=torch.int64).contiguous(), B, L, sigma, seeds, z
@@ -298,6 +306,8 @@ class WaveGlowVocoder(nn.Module):
         s = int(status.item())                                                   # the call's one host read
         if s & _lib.FS2_WAVEGLOW_BAD_LENGTH:
             raise ValueError("every olens[b] must lie in [1, Lmax]")
+        if s & _lib.FS2_WAVEGLOW_BAD_START:
+            raise ValueError("every starts[b] must be >= 0")
         if s & _lib.FS2_WAVEGLOW_RANGE:
             raise ValueError(f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
                              f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'")
@@ -322,8 +332,15 @@ class WaveGlowVocoder(nn.Module):
                        "fs2_waveglow_noise")
         return z
 
-    def forward(self, mels: torch.Tensor, olens: torch.Tensor, *, sigma: float = 1.0, seed=None, z=None):
-        """-> (audio [B, Lmax * 256] fp32, alens [B] int64 = olens * 256)."""
+    def forward(self, mels: torch.Tensor, olens: torch.Tensor, *, sigma: float = 1.0, seed=None, z=None, chunk_frames: int | None = None):
+        """-> (audio [B, Lmax * 256] fp32, alens [B] int64 = olens * 256).
+
+        chunk_frames=k: the same bits, computed as windows of k frames written straight into the output, with the
+        workspace of one window (fs2_waveglow_window): in fp32 mode this vocodes batches the whole call refuses.  seed=None
+        draws the same one int64 as the whole call.  Still one host read per call: the windows' status words are ORed on
+        the device."""
+        if chunk_frames is not None:
+            return self._chunked(mels, olens, chunk_frames, sigma, seed, z)
         mels, olens, B, L, sigma, seeds, z = self._inputs(mels, olens, sigma, seed, z)
         dev = mels.device
         h = self._handle(dev)
@@ -335,6 +352,134 @@ class WaveGlowVocoder(nn.Module):
                                                 _lib.ptr(audio), _lib.ptr(status), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)),
                        "fs2_waveglow")
         self._check_status(status)
+        return audio, olens * HOP
+
+    # ---- windows (DESIGN.md section 12) ----------------------------------------------------------------------------
+    @staticmethod
+    def _check_frames(n_frames) -> None:
+        if isinstance(n_frames, bool) or not isinstance(n_frames, int) or n_frames < 1:
+            raise ValueError(f"n_frames / chunk_frames must be an int >= 1 (got {n_frames!r})")
+
+    def _check_window_size(self, B: int, n_frames: int) -> None:
+        """fs2_waveglow_window's limits on the window's B * (n_frames + 192) * 32 step rows, raised here as ValueError."""
+        self._check_frames(n_frames)
+        rows = B * (n_frames + 2 * HALO) * STEPS
+        if rows >= 1 << 31:
+            raise ValueError(f"B * (n_frames + {2 * HALO}) * {STEPS} must stay below 2^31 window rows (B={B}, n_frames={n_frames})")
+        if self.math_mode == "fp32" and rows > 65535 * 128:
+            raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 window rows, B * (n_frames + {2 * HALO}) * {STEPS} = {rows} "
+                             f"(B={B}, n_frames={n_frames}); use fewer frames per window")
+
+    def _window_inputs(self, mels, olens, n_frames, sigma, seed, z):
+        """_inputs with the window's limits in place of the whole call's (Lmax bounds only z's and mels' layout)."""
+        self._check_frames(n_frames)
+
+        def check(B, L):
+            self._check_window_size(B, n_frames)
+            if L * STEPS >= 1 << 31:
+                raise ValueError(f"Lmax * {STEPS} must stay below 2^31 steps (Lmax={L})")
+        return self._inputs(mels, olens, sigma, seed, z, check)
+
+    def _window_workspace(self, h, B: int, n_frames: int, device: torch.device) -> torch.Tensor:
+        n = C.c_size_t()
+        _lib.check(_lib.load().fs2_waveglow_window_workspace_bytes(h, B, n_frames, C.byref(n)), "fs2_waveglow_window_workspace_bytes")
+        ws = self._wws.get(device.index)
+        if ws is None or ws.numel() < n.value:
+            self._wws.pop(device.index, None)
+            ws = torch.empty(n.value, dtype=torch.uint8, device=device)
+            self._wws[device.index] = ws
+        return ws
+
+    @staticmethod
+    def _starts(starts, B: int, device: torch.device) -> torch.Tensor:
+        """starts as an int, a host list or tensor (checked >= 0 here) or a device tensor (checked on the device) -> [B]
+        int64 on `device`."""
+        if isinstance(starts, bool):
+            raise ValueError("starts must be an int, a list or an integer tensor")
+        if isinstance(starts, int):
+            starts = [starts] * B
+        if not torch.is_tensor(starts):
+            try:
+                starts = torch.tensor(starts)
+            except (TypeError, ValueError, RuntimeError):
+                raise ValueError("starts must be an int, a list or an integer tensor") from None
+        if starts.dim() != 1 or starts.shape[0] != B:
+            raise ValueError(f"starts must hold B={B} frame offsets")
+        if starts.dtype.is_floating_point or starts.dtype == torch.bool or starts.is_complex():
+            raise ValueError("starts must be an integer tensor")
+        if not starts.is_cuda:
+            if bool((starts < 0).any()):
+                raise ValueError("every starts[b] must be >= 0")
+        elif starts.device != device:
+            raise ValueError("starts must be on the same device as mels")
+        return starts.to(device=device, dtype=torch.int64).contiguous()
+
+    def _window_call(self, h, mels, olens, starts, B: int, L: int, n_frames: int, sigma: float, seeds, z, audio: torch.Tensor, ld: int,
+                     status: torch.Tensor, ws: torch.Tensor) -> None:
+        dev = mels.device
+        with torch.cuda.device(dev):
+            _lib.check(_lib.load().fs2_waveglow_window(h, _lib.ptr(mels), _lib.ptr(olens), _lib.ptr(starts), B, L, n_frames, sigma,
+                                                       _lib.ptr(seeds), _lib.ptr(z), audio.data_ptr(), ld, _lib.ptr(status), _lib.ptr(ws),
+                                                       ws.numel(), _lib.stream_ptr(dev)), "fs2_waveglow_window")
+
+    def window(self, mels: torch.Tensor, olens: torch.Tensor, starts, n_frames: int, *, sigma: float = 1.0, seed=None, z=None):
+        """One window of the audio (DESIGN.md section 12): -> (audio [B, n_frames * 256] fp32, alens [B] int64 =
+        clamp(olens - starts, 0, n_frames) * 256).  audio[b, :alens[b]] are samples [starts[b] * 256, ...) of
+        `forward(mels, olens, sigma=sigma, seed=seed / z=z)[0][b]`, bit for bit; the rest is 0.  starts: an int (every
+        utterance), a host list or tensor, or a device tensor.  The noise must be given (seed or z [B, 8, Lmax * 32]): a
+        window is only meaningful against a whole call with the same draw.  Only mel frames [starts[b] - 99, starts[b] +
+        n_frames + 96) below olens[b] and the z steps 32 times those frames are read; the workspace depends on B and
+        n_frames only.  One host read per call."""
+        if seed is None and z is None:
+            raise ValueError("window needs the noise: pass seed (an int or a [B] tensor) or z, as the whole call it continues")
+        mels, olens, B, L, sigma, seeds, z = self._window_inputs(mels, olens, n_frames, sigma, seed, z)
+        dev = mels.device
+        starts = self._starts(starts, B, dev)
+        h = self._handle(dev)
+        ws = self._window_workspace(h, B, n_frames, dev)
+        audio = torch.empty((B, n_frames * HOP), dtype=torch.float32, device=dev)
+        status = torch.empty((1,), dtype=torch.int32, device=dev)
+        self._window_call(h, mels, olens, starts, B, L, n_frames, sigma, seeds, z, audio, n_frames * HOP, status, ws)
+        self._check_status(status)
+        return audio, (olens - starts).clamp(0, n_frames) * HOP
+
+    @staticmethod
+    def _resolve_seed(seed, z):
+        """seed=None without z: the one int64 the whole call would draw, drawn once for every window of a stream."""
+        if seed is None and z is None:
+            return int(torch.randint(-2 ** 63, 2 ** 63 - 1, (), dtype=torch.int64))
+        return seed
+
+    def stream(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int = 32, *, sigma: float = 1.0, seed=None, z=None):
+        """Lockstep windows: yields (audio, alens) of `window(mels, olens, k * chunk_frames, chunk_frames, ...)` for k = 0 ..
+        ceil(Lmax / chunk_frames) - 1, the last one cut at Lmax, so that the chunks concatenated along time are
+        `forward(mels, olens, sigma=sigma, seed=seed, z=z)`; seed=None draws the whole call's one int64, once.  Utterances
+        that have ended give rows of 0 (alens 0)."""
+        self._check_frames(chunk_frames)
+        seed = self._resolve_seed(seed, z)
+        if torch.is_tensor(mels) and mels.dim() == 3 and seed is not None:
+            seed = self._seeds(seed, mels.shape[0], mels.device)          # validated and moved once
+        L = mels.shape[1]
+        for c0 in range(0, L, chunk_frames):
+            yield self.window(mels, olens, c0, min(chunk_frames, L - c0), sigma=sigma, seed=seed, z=z)
+
+    def _chunked(self, mels, olens, k: int, sigma, seed, z):
+        self._check_frames(k)
+        seed = self._resolve_seed(seed, z)
+        mels, olens, B, L, sigma, seeds, z = self._window_inputs(mels, olens, k, sigma, seed, z)
+        dev = mels.device
+        h = self._handle(dev)
+        ws = self._window_workspace(h, B, min(k, L), dev)
+        audio = torch.empty((B, L * HOP), dtype=torch.float32, device=dev)
+        c0s = list(range(0, L, k))
+        starts = torch.tensor(c0s, dtype=torch.int64).repeat_interleave(B).reshape(len(c0s), B).to(dev)
+        status = torch.empty((len(c0s),), dtype=torch.int32, device=dev)
+        for i, c0 in enumerate(c0s):
+            n = min(k, L - c0)
+            self._window_call(h, mels, olens, starts[i], B, L, n, sigma, seeds, z, audio[:, c0 * HOP:], L * HOP, status[i: i + 1], ws)
+        bits = torch.tensor([_lib.FS2_WAVEGLOW_BAD_LENGTH, _lib.FS2_WAVEGLOW_RANGE, _lib.FS2_WAVEGLOW_BAD_START], dtype=torch.int32,
+                            device=dev)
+        self._check_status(((status[:, None] & bits) != 0).any(0).int().mul(bits).sum().reshape(1))
         return audio, olens * HOP
 
     def infer(self, spect: torch.Tensor, sigma: float = 1.0) -> torch.Tensor:

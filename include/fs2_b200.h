@@ -490,6 +490,23 @@ int fs2_waveglow_workspace_bytes(fs2_waveglow_net* m, int B, int Lmax, size_t* b
 /* sigma finite and >= 0; seeds [B] i64 (device, used when z is NULL) or z [B, 8, Lmax * 32] */
 int fs2_waveglow(fs2_waveglow_net* m, const float* mels, const int64_t* olens, int B, int Lmax, double sigma, const int64_t* seeds,
                  const float* z, float* audio, int* status, void* ws, size_t ws_bytes, void* stream);
+/* A window of the same audio (DESIGN.md section 12): for every utterance b, audio row b (audio_ld >= n_frames * 256
+ * samples apart, n_frames * 256 written) holds samples [starts[b] * 256, min(starts[b] + n_frames, olens[b]) * 256) of
+ * utterance b, bit-identical to the same samples of fs2_waveglow on the whole batch with the same sigma and seeds / z in
+ * every math mode, then +0.  A row with starts[b] >= olens[b] is all +0.  starts, olens and seeds [B] are device arrays,
+ * so one captured call serves every step of a stream.  z keeps the whole call's layout [B, 8, Lmax * 32].  Only mel frames
+ * [starts[b] - 99, starts[b] + n_frames + 96) below olens[b] and z steps [(starts[b] - 96) * 32, (starts[b] + n_frames +
+ * 96) * 32) below olens[b] * 32 are read.  The workspace depends on B and n_frames only; the limits apply to the window's
+ * B * (n_frames + 192) * 32 step rows (below 2^31, at most 65535 * 128 in FS2_MATH_FP32), and Lmax * 32 must stay below
+ * 2^31.  No allocation, no synchronisation.  It enqueues 497 kernels (498 in FS2_MATH_F16 / FS2_MATH_3XTF32): those of
+ * fs2_waveglow and a copy of the window's audio.  *status: the bits of fs2_waveglow (FS2_WAVEGLOW_RANGE only for values
+ * the whole call also checks) and
+ *   FS2_WAVEGLOW_BAD_START   some starts[b] < 0; that row is +0. */
+#define FS2_WAVEGLOW_BAD_START 4
+int fs2_waveglow_window_workspace_bytes(fs2_waveglow_net* m, int B, int n_frames, size_t* bytes);
+int fs2_waveglow_window(fs2_waveglow_net* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax,
+                        int n_frames, double sigma, const int64_t* seeds, const float* z, float* audio, int64_t audio_ld,
+                        int* status, void* ws, size_t ws_bytes, void* stream);
 /* the standard-normal draw a seeded fs2_waveglow call uses: z [B, 8, Lmax * 32], 0 at steps t >= olens[b] * 32.  Element
  * (b, ch, t) is Box-Muller on Philox4x32-10(counter (t, ch / 4, 0, 0), key (seeds[b] mod 2^32, seeds[b] / 2^32)). */
 int fs2_waveglow_noise(const int64_t* seeds, const int64_t* olens, int B, int Lmax, float* z, void* stream);
