@@ -96,6 +96,9 @@ SIGNATURES = {
     "fs2_bgemm": [_P, _L, _L, _L, _L, _P, _L, _L, _L, _L, _P, _L, _L, _L, _L, _I, _I, _I, _I, _I, _F, _P],
     "fs2_attn_softmax": [_P, _P, _P, _F, _I, _I, _I, _P, _P, _P],
     "fs2_attn_softmax_backward": [_P, _P, _P, _F, _I, _I, _I, _P, _P],
+    "fs2_attn_train_ws_bytes": [_I, _I, _I, _I, C.POINTER(_SZ)],
+    "fs2_attn_train_forward": [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P, C.c_uint64, C.c_uint64, _P, _P, _P, _SZ, _P],
+    "fs2_attn_train_backward": [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P, C.c_uint64, C.c_uint64, _P, _P, _P, _P, _SZ, _P],
     "fs2_embed_posenc": [_P, _P, _I, _P, _P, _I, _I, _I, _P, _P],
     "fs2_embed_backward": [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P],
     "fs2_posenc_add": [_P, _P, _P, _I, _I, _I, _P, _P],

@@ -27,6 +27,10 @@ Train precision (`train_precision=` / FS2_TRAIN_PRECISION): "fp32" (default) tra
 every convolution and projection of the train step (forward, input and weight gradient) on the tensor cores in tf32
 with fp32 accumulation, as cuDNN does for a reference user's Conv1d by default.  Attention, the norms and the rest of
 the step stay fp32 (DESIGN.md §10).
+
+Train attention (`train_attention=` / FS2_TRAIN_ATTENTION): "materialized" (default) runs the train step's attention as
+fp32 batched products over a stored [B, heads, L, L] score tensor; "flash" (needs train_precision="tf32") runs it on
+fused tf32 tensor-core kernels that store only the row log-sum-exp (DESIGN.md §13).
 """
 from __future__ import annotations
 
@@ -43,6 +47,8 @@ from .weights import ModelDims, positional_table, variance_bins
 
 DEFAULT_PRECISION = os.environ.get("FS2_PRECISION", "3xf16")
 TRAIN_PRECISIONS = ("fp32", "tf32")
+TRAIN_ATTENTIONS = ("materialized", "flash")
+FLASH_HEAD_WIDTHS = (128, 192)
 
 
 def resolve_train_precision(train_precision: Optional[str] = None) -> str:
@@ -54,6 +60,18 @@ def resolve_train_precision(train_precision: Optional[str] = None) -> str:
                          "which cannot hold gradients without underflow; use 'fp32' or 'tf32'")
     if mode not in TRAIN_PRECISIONS:
         raise ValueError(f"train_precision must be one of {list(TRAIN_PRECISIONS)}, got {mode!r}")
+    return mode
+
+
+def resolve_train_attention(train_attention: Optional[str] = None, train_precision: str = "fp32") -> str:
+    """The train step's attention: the argument, else FS2_TRAIN_ATTENTION, else "materialized".  "flash" runs on the fused
+    tf32 kernels (DESIGN.md §13), so it needs train_precision="tf32"."""
+    mode = train_attention or os.environ.get("FS2_TRAIN_ATTENTION") or "materialized"
+    if mode not in TRAIN_ATTENTIONS:
+        raise ValueError(f"train_attention must be one of {list(TRAIN_ATTENTIONS)}, got {mode!r}")
+    if mode == "flash" and train_precision != "tf32":
+        raise ValueError(f"train_attention='flash' needs train_precision='tf32', got {train_precision!r}: the fused attention's products "
+                         "are 1xTF32 on the tensor cores, which the fp32 train mode does not allow (it has no fp32-class flash kernel)")
     return mode
 
 
@@ -274,7 +292,8 @@ class FeedForwardTransformer(nn.Module):
     """Feed-forward Transformer TTS (FastSpeech2) on H100.  See module docstring."""
 
     @classmethod
-    def from_checkpoint(cls, checkpoint, hp=None, precision: Optional[str] = None, device=None, train_precision: Optional[str] = None):
+    def from_checkpoint(cls, checkpoint, hp=None, precision: Optional[str] = None, device=None, train_precision: Optional[str] = None,
+                        train_attention: Optional[str] = None):
         """Build the model from a reference checkpoint: a path or the loaded dict `{"model": state_dict, "optim": ..,
         "step": .., "hp_str": .., "githash": ..}` that train_fastspeech.py:235-244 writes (or a bare state_dict, the
         `--old_model` case of inference.py:161-163).  `hp` defaults to the checkpoint's own `hp_str` like
@@ -289,12 +308,13 @@ class FeedForwardTransformer(nn.Module):
             hp = load_hp_str(checkpoint["hp_str"])
         idim = int(sd["encoder.embed.0.weight"].shape[0])
         odim = int(_get(_get(hp, "audio"), "num_mels"))
-        model = cls(idim, odim, hp, precision=precision, train_precision=train_precision)
+        model = cls(idim, odim, hp, precision=precision, train_precision=train_precision, train_attention=train_attention)
         model.load_state_dict(sd, strict="model" in checkpoint)
         model.eval()
         return model.to(device) if device is not None else model
 
-    def __init__(self, idim: int, odim: int, hp: Dict, precision: Optional[str] = None, train_precision: Optional[str] = None):
+    def __init__(self, idim: int, odim: int, hp: Dict, precision: Optional[str] = None, train_precision: Optional[str] = None,
+                 train_attention: Optional[str] = None):
         super().__init__()
         dims = dims_from_hp(idim, odim, hp)
         self.dims = dims
@@ -309,6 +329,12 @@ class FeedForwardTransformer(nn.Module):
         if self.precision not in _lib.MATH_MODES:
             raise ValueError(f"precision must be one of {sorted(_lib.MATH_MODES)}")
         self.train_precision = resolve_train_precision(train_precision)
+        self.train_attention = resolve_train_attention(train_attention, self.train_precision)
+        if self.train_attention == "flash":
+            for name, width in (("adim", dims.adim), ("ddim", dims.ddim)):
+                if width % dims.aheads or width // dims.aheads not in FLASH_HEAD_WIDTHS:
+                    raise ValueError(f"train_attention='flash' supports head widths {list(FLASH_HEAD_WIDTHS)}; {name} = {width} with "
+                                     f"aheads = {dims.aheads} gives {width / dims.aheads:g}")
 
         A, D = dims.adim, dims.ddim
         self.encoder = _FFTStack(nn.Sequential(nn.Embedding(idim, A, padding_idx=0), _ScaledPosEnc(A, dims.pe_len)),

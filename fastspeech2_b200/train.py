@@ -7,7 +7,8 @@ Arithmetic is fp32 on CUDA cores by default (the reference trains in fp32); with
 convolution and projection (`ConvFn`: forward, input and weight gradient) runs on the tensor cores in tf32 instead, the
 way a reference user on an H100 gets TF32 for every Conv1d from cuDNN's defaults (DESIGN.md §10).  The stage order,
 dropout sites and BatchNorm batch statistics follow the reference modules line by line (cited at each step of
-`train_forward`).
+`train_forward`).  With `train_attention="flash"` (tf32 only) self-attention runs on the fused tensor-core kernels of
+csrc/attention_train_tc.cu (`FlashAttentionFn`, DESIGN.md §13) instead of the materialized `AttentionFn`.
 
 Dropout masks come from `MaskSource`: the library's Philox kernel in production, or masks injected by a test so that the
 reference (with `torch.nn.functional.dropout` patched to consume the same list) and this path drop the same elements.
@@ -66,6 +67,20 @@ class MaskSource:
         _chk(_lib.load().fs2_dropout_mask(m.data_ptr(), n, float(p), self.seed, self.offset, _lib.stream_ptr(device)), "fs2_dropout_mask")
         self.offset += (n + 3) // 4
         return m
+
+    def attention(self, shape, p: float, device):
+        """The mask source of a fused attention site: (injected mask, 0, 0), or (None, seed, offset) for the kernels to
+        regenerate the Philox mask `next` would have drawn.  `offset` advances exactly as in `next`, so every later mask of
+        the step is unchanged and both attention paths drop the same elements; nothing [B, h, L, L] is allocated."""
+        if self.injected is not None:
+            return self.next(shape, p, device), 0, 0
+        self.calls += 1
+        n = 1
+        for s in shape:
+            n *= int(s)
+        off = self.offset
+        self.offset += (n + 3) // 4
+        return None, self.seed, off
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -269,6 +284,47 @@ class AttentionFn(torch.autograd.Function):
         _bgemm(ds.data_ptr(), ss, k.data_ptr(), qs, dq.data_ptr(), qs, B, heads, L, dk, L, scale, st)            # dQ = dS K / sqrt(dk)
         _bgemm(ds.data_ptr(), st_t, q.data_ptr(), qs, dkk.data_ptr(), qs, B, heads, L, dk, L, scale, st)         # dK = dS^T Q / sqrt(dk)
         return dq, dkk, dv, None, None, None, None
+
+
+def attn_train_ws_bytes(B: int, L: int, C_: int, heads: int) -> int:
+    """Workspace bytes of fs2_attn_train_forward / _backward for this shape (raises on a shape the library rejects)."""
+    n = C.c_size_t(0)
+    _chk(_lib.load().fs2_attn_train_ws_bytes(int(B), int(L), int(C_), int(heads), C.byref(n)), "fs2_attn_train_ws_bytes")
+    return int(n.value)
+
+
+class FlashAttentionFn(torch.autograd.Function):
+    """AttentionFn's contract on the fused tf32 kernels (DESIGN.md §13): saves q, k, v, O and the row log-sum-exp only;
+    the dropout mask is `dmask` (injected) or regenerated from (seed, offset)."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, lens, heads, p_drop, dmask, seed, offset):
+        q, k, v = _c(q), _c(k), _c(v)
+        B, L, C_ = q.shape
+        nbytes = attn_train_ws_bytes(B, L, C_, heads)
+        ws = torch.empty((nbytes,), dtype=torch.uint8, device=q.device)
+        out = torch.empty((B, L, C_), dtype=torch.float32, device=q.device)
+        lse = torch.empty((B * heads, L), dtype=torch.float32, device=q.device)
+        _chk(_lib.load().fs2_attn_train_forward(q.data_ptr(), k.data_ptr(), v.data_ptr(), lens.data_ptr(), B, L, C_, heads, float(p_drop), _p(dmask),
+                                                int(seed), int(offset), out.data_ptr(), lse.data_ptr(), ws.data_ptr(), nbytes, _st(q)),
+             "fs2_attn_train_forward")
+        ctx.save_for_backward(q, k, v, out, lse, lens, dmask)
+        ctx.meta = (heads, float(p_drop), int(seed), int(offset))
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        q, k, v, out, lse, lens, dmask = ctx.saved_tensors
+        heads, p_drop, seed, offset = ctx.meta
+        dout = _c(dout)
+        B, L, C_ = q.shape
+        nbytes = attn_train_ws_bytes(B, L, C_, heads)
+        ws = torch.empty((nbytes,), dtype=torch.uint8, device=q.device)
+        dq, dkk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        _chk(_lib.load().fs2_attn_train_backward(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr(), dout.data_ptr(),
+                                                 lens.data_ptr(), B, L, C_, heads, p_drop, _p(dmask), seed, offset, dq.data_ptr(), dkk.data_ptr(),
+                                                 dv.data_ptr(), ws.data_ptr(), nbytes, _st(dout)), "fs2_attn_train_backward")
+        return dq, dkk, dv, None, None, None, None, None, None
 
 
 class EmbedFn(torch.autograd.Function):
@@ -478,16 +534,21 @@ def _drop(x: torch.Tensor, p: float, masks: MaskSource, channel_first: bool = Fa
     return DropoutFn.apply(x, masks.next(tuple(x.shape), p, x.device), p)
 
 
-def _fft_blocks(stack, x, lens, heads: int, rate: float, masks: MaskSource, math: int = _lib.MATH_FP32):
-    """core/encoder.py:46-71 (post-LN, concat_after=False) x num_blocks."""
+def _fft_blocks(stack, x, lens, heads: int, rate: float, masks: MaskSource, math: int = _lib.MATH_FP32, flash: bool = False):
+    """core/encoder.py:46-71 (post-LN, concat_after=False) x num_blocks.  `flash`: attention on the fused tf32 kernels
+    (FlashAttentionFn) instead of the materialized AttentionFn."""
     B, L, C_ = x.shape
     for blk in stack.encoders_:
         a = blk.self_attn
         q = ConvFn.apply(x, a.linear_q.weight, a.linear_q.bias, ACT_NONE, None, math)        # attention.py:48-50
         k = ConvFn.apply(x, a.linear_k.weight, a.linear_k.bias, ACT_NONE, None, math)
         v = ConvFn.apply(x, a.linear_v.weight, a.linear_v.bias, ACT_NONE, None, math)
-        dmask = masks.next((B, heads, L, L), rate, x.device) if rate > 0 else None           # attention.py:69
-        ctx = AttentionFn.apply(q, k, v, lens, heads, rate, dmask)
+        if flash:
+            dmask, seed, off = masks.attention((B, heads, L, L), rate, x.device) if rate > 0 else (None, 0, 0)   # attention.py:69
+            ctx = FlashAttentionFn.apply(q, k, v, lens, heads, rate, dmask, seed, off)
+        else:
+            dmask = masks.next((B, heads, L, L), rate, x.device) if rate > 0 else None       # attention.py:69
+            ctx = AttentionFn.apply(q, k, v, lens, heads, rate, dmask)
         att = ConvFn.apply(ctx, a.linear_out.weight, a.linear_out.bias, ACT_NONE, None, math)  # attention.py:74
         x = AddFn.apply(x, _drop(att, rate, masks))                                           # encoder.py:60
         x = LayerNormFn.apply(x, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)             # encoder.py:62
@@ -519,6 +580,7 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
         raise _lib.Fs2Error("train-mode forward needs CUDA tensors (no CPU fallback)")
     masks = masks or MaskSource(seed=int(torch.initial_seed()) & 0xFFFFFFFF)
     math = _lib.MATH_TF32 if model.train_precision == "tf32" else _lib.MATH_FP32
+    flash = model.train_attention == "flash"
     d = model.dims
     ilens = ilens.to(device=dev, dtype=torch.int64).contiguous()
     olens = olens.to(device=dev, dtype=torch.int64).contiguous()
@@ -538,7 +600,7 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
     enc_pos = model.encoder.embed[-1]
     x = EmbedFn.apply(xs, model.encoder.embed[0].weight, enc_pos.alpha, enc_pos.pe)
     x = _drop(x, ER, masks)                                                                   # embedding.py:120
-    hs = _fft_blocks(model.encoder, x, ilens, d.aheads, ER, masks, math)
+    hs = _fft_blocks(model.encoder, x, ilens, d.aheads, ER, masks, math, flash)
     # duration predictor on the encoder states, then LengthRegulator with the ground-truth durations (:209-211)
     d_outs = _predictor(model.duration_predictor, hs, ilens, model.duration_dropout_rate, masks, math)
     hm = LengthRegulatorFn.apply(hs, ds, ilens, L)
@@ -560,7 +622,7 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
     z = ReluFn.apply(z)
     z = PosEncFn.apply(z, emb[4].alpha, emb[4].pe)
     z = _drop(z, DR, masks)
-    z = _fft_blocks(model.decoder, z, olens, d.aheads, DR, masks, math)
+    z = _fft_blocks(model.decoder, z, olens, d.aheads, DR, masks, math, flash)
     before = ConvFn.apply(z, model.feat_out.weight, model.feat_out.bias, ACT_NONE, None, math)  # :228-230
     # Postnet (modules.py:283-359): [conv(no bias) -> BatchNorm1d(batch statistics) -> tanh -> dropout] x 4, conv -> BN -> dropout; + residual
     y = before

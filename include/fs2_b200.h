@@ -329,6 +329,26 @@ int fs2_bgemm(const float* a, int64_t abs_, int64_t ahs, int64_t ars, int64_t ac
 /* core/attention.py:58-69 on materialised scores [B*heads, L, L]: mask, softmax, masked_fill(0) -> p; dropout -> pd; and its backward */
 int fs2_attn_softmax(const float* s, const int64_t* lens, const uint8_t* dmask, float p_drop, int B, int heads, int L, float* p, float* pd, void* stream);
 int fs2_attn_softmax_backward(const float* p, const float* dpd, const uint8_t* dmask, float p_drop, int B, int heads, int L, float* ds, void* stream);
+/* Fused attention of the tf32 train mode (DESIGN.md §13, csrc/attention_train_tc.cu): the forward and backward of
+ * fs2_bgemm + fs2_attn_softmax[_backward] above (train.py's AttentionFn) on q, k, v [B, L, C] (heads contiguous, head width
+ * C / heads = 128 or 192), without any [B, heads, L, L] tensor.  Products are 1xTF32 on the tensor cores (operands rounded
+ * to tf32 with round-to-nearest, fp32 accumulation); no atomics, so the same inputs give the same bits.  A score is valid
+ * where query and key are below lens[b] (clamped to [0, L]); rows of out / dq and of dk / dv past lens[b] are written as 0,
+ * and nothing past lens[b] is read.  Dropout after the softmax (scale 1 / (1 - p_drop)): dmask [B, heads, L, L] uint8
+ * (1 = keep) when non-NULL, else element e = ((b heads + h) L + i) L + j is kept where byte e of
+ * fs2_dropout_mask(mask, B heads L L, p_drop, seed, offset) is 1 (regenerated, never stored).  lse [B * heads, L] is the row
+ * log-sum-exp of the valid scores (0 for rows past lens[b]); the backward takes it and the forward's out.
+ * ws: caller-owned device workspace, 16-byte aligned, of at least fs2_attn_train_ws_bytes(...) =
+ *   4 * align256(B L C 4) + align256(B heads L 4) bytes;
+ * its contents on entry do not matter.  B, L >= 1; a null pointer, another head width, C not divisible by heads, p_drop
+ * outside [0, 1), a short or misaligned workspace and sizes that would overflow are FS2_ERR_INVALID. */
+int fs2_attn_train_ws_bytes(int B, int L, int C, int heads, size_t* bytes);
+int fs2_attn_train_forward(const float* q, const float* k, const float* v, const int64_t* lens, int B, int L, int C, int heads, float p_drop,
+                           const uint8_t* dmask, uint64_t seed, uint64_t offset, float* out, float* lse, void* ws, size_t ws_bytes,
+                           void* stream);
+int fs2_attn_train_backward(const float* q, const float* k, const float* v, const float* out, const float* lse, const float* dout,
+                            const int64_t* lens, int B, int L, int C, int heads, float p_drop, const uint8_t* dmask, uint64_t seed,
+                            uint64_t offset, float* dq, float* dk, float* dv, void* ws, size_t ws_bytes, void* stream);
 /* encoder input (fastspeech.py:65-67 + embedding.py:105-120 before its dropout) and its backward; decoder-side x + alpha*pe */
 int fs2_embed_posenc(const int64_t* xs, const float* table, int n_sym, const float* pe, const float* alpha, int B, int T, int C, float* out,
                      void* stream);
