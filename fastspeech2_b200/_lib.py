@@ -41,6 +41,12 @@ class VocoderConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("n_fft", "hop", "win_length", "n_mels", "math_mode")]
 
 
+class FeaturesConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("sample_rate", "n_fft", "hop", "win_length", "n_mels", "math_mode")] + \
+               [(n, C.c_double) for n in ("f0_floor", "f0_ceil", "channels_in_octave", "allowed_range")]
+
+
+FS2_FEAT_BAD_LENGTH, FS2_FEAT_RANGE = 1, 2   # bits of fs2_mel_energy's / fs2_dio's device status word
 FS2_VOC_BAD_LENGTH, FS2_VOC_RANGE = 1, 2     # bits of fs2_griffin_lim's / fs2_mel_magnitude's device status word
 FS2_MELGAN_BAD_LENGTH, FS2_MELGAN_RANGE = 1, 2   # bits of fs2_melgan's device status word
 FS2_MELGAN_BAD_START = 4                          # and of fs2_melgan_window's
@@ -117,6 +123,11 @@ SIGNATURES = {
     "fs2_vocoder_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
     "fs2_mel_magnitude": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
     "fs2_griffin_lim": [_P, _P, _P, _I, _I, _I, _F, _P, _P, _P, _P, _P, _SZ, _P],
+    "fs2_features_create": [C.POINTER(_P), C.POINTER(FeaturesConfig)],
+    "fs2_features_load": [_P, _P, _P, _P],
+    "fs2_features_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_mel_energy": [_P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _P],
+    "fs2_dio": [_P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _P],
     "fs2_melgan_create": [C.POINTER(_P), _I],
     "fs2_melgan_load": [_P, C.POINTER(_P), C.POINTER(_P), _P],
     "fs2_melgan_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
@@ -141,7 +152,7 @@ SIGNATURES = {
     "fs2_flag_wait": [_P, _I, _I, _L, _P],
 }
 OTHER_SYMBOLS = ("fs2_last_error", "fs2_version", "fs2_destroy", "fs2_kernel_launches", "fs2_profile_label", "fs2_vocoder_destroy",
-                 "fs2_melgan_destroy", "fs2_waveglow_destroy")
+                 "fs2_melgan_destroy", "fs2_waveglow_destroy", "fs2_features_destroy")
 ALL_SYMBOLS = tuple(SIGNATURES) + OTHER_SYMBOLS
 
 _lib: Optional[C.CDLL] = None
@@ -177,6 +188,8 @@ def load() -> C.CDLL:
     lib.fs2_melgan_destroy.argtypes = [_P]
     lib.fs2_waveglow_destroy.restype = None
     lib.fs2_waveglow_destroy.argtypes = [_P]
+    lib.fs2_features_destroy.restype = None
+    lib.fs2_features_destroy.argtypes = [_P]
     _lib = lib
     return lib
 

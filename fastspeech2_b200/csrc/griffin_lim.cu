@@ -22,7 +22,7 @@
 #include <math.h>
 #include <string.h>
 
-#include "operand_planes.cuh"
+#include "vocoder_weights.cuh"
 
 struct fs2_vocoder;
 
@@ -208,11 +208,6 @@ __global__ void pad_pack_kernel(const float* __restrict__ src, int SR, int SC, i
   }
 }
 
-struct VWeight {               // one GEMM weight [N][K]: fp32 (fp32 / tf32 families) and scaled fp16 planes
-  float* w = nullptr; __half* hi = nullptr; __half* lo = nullptr; float* sc = nullptr;   // sc = [scale, 1 / scale]
-  int N = 0, K = 0;
-};
-
 struct Bump {
   char* base; size_t off = 0, cap;
   Bump(void* b, size_t c) : base((char*)b), cap(c) {}
@@ -222,6 +217,31 @@ struct Bump {
 };
 
 }  // namespace
+
+int vweight_pack(VWeight& w, const float* src, int SR, int SC, int transpose, cudaStream_t st) {
+  const long n = (long)w.N * w.K;
+  pad_pack_kernel<<<grid_for(n, 256), 256, 0, st>>>(src, SR, SC, transpose, w.w, w.N, w.K);
+  FS2_LAUNCH_CHECK();
+  int rc = weight_scale(w.w, n, w.sc, w.sc + 1, st); if (rc) return rc;
+  return split_f16(w.w, w.hi, w.lo, n, w.sc, st);
+}
+
+int vweight_gemm(int math_mode, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens, float* out,
+                 cudaStream_t st) {
+  TapGemm g;
+  memset(&g, 0, sizeof(g));
+  g.B = B; g.L = L; g.K = w.K; g.N = w.N; g.taps = 1; g.act = act; g.out = out; g.ldo = w.N; g.lens = lens;
+  g.w = w.w; g.a_inv = 1.0f;
+  if (math_mode == FS2_MATH_FP32 || math_mode == FS2_MATH_TF32) {
+    g.x = (const float*)a; g.ldx = w.K;
+    return math_mode == FS2_MATH_FP32 ? tap_gemm_fp32(g, st) : tap_gemm_tf32(g, st);
+  }
+  g.ldx = w.K;
+  g.xp = (const __half*)a; g.w_hi = w.hi; g.w_lo = w.lo; g.w_inv = w.sc + 1; g.a_inv = kPlaneInv;
+  g.precise = math_mode == FS2_MATH_3XTF32;
+  return tap_gemm_planes(g, st);
+}
+
 }  // namespace fs2
 
 struct fs2_vocoder {
@@ -261,19 +281,7 @@ GlPlan plan(const fs2_vocoder* v, Bump& b, int B, int L, bool momentum_state) {
 
 // out [rows][w.N] = act(a [rows][w.K] . w^T), rows t >= lens[b] written as 0 (and skipped by the tensor-core kernel)
 int gemm(const fs2_vocoder* v, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens, float* out, cudaStream_t st) {
-  TapGemm g;
-  memset(&g, 0, sizeof(g));
-  g.B = B; g.L = L; g.K = w.K; g.N = w.N; g.taps = 1; g.act = act; g.out = out; g.ldo = w.N; g.lens = lens;
-  g.w = w.w; g.a_inv = 1.0f;
-  const int mode = v->cfg.math_mode;
-  if (mode == FS2_MATH_FP32 || mode == FS2_MATH_TF32) {
-    g.x = (const float*)a; g.ldx = w.K;
-    return mode == FS2_MATH_FP32 ? tap_gemm_fp32(g, st) : tap_gemm_tf32(g, st);
-  }
-  g.ldx = w.K;
-  g.xp = (const __half*)a; g.w_hi = w.hi; g.w_lo = w.lo; g.w_inv = w.sc + 1; g.a_inv = kPlaneInv;
-  g.precise = mode == FS2_MATH_3XTF32;
-  return tap_gemm_planes(g, st);
+  return vweight_gemm(v->cfg.math_mode, w, a, B, L, act, lens, out, st);
 }
 
 
@@ -349,11 +357,8 @@ int fs2_vocoder_load(fs2_vocoder* v, const float* w_forward, const float* w_inve
   struct { const float* src; int sr, sc, tr; VWeight* w; } packs[3] = {
       {w_forward, c2, nf, 0, &v->fwd}, {w_inverse, c2, nf, 1, &v->inv}, {mel_inverse, v->cutoff, v->cfg.n_mels, 0, &v->mel}};
   for (auto& p : packs) {
-    const long n = (long)p.w->N * p.w->K;
-    pad_pack_kernel<<<grid_for(n, 256), 256, 0, st>>>(p.src, p.sr, p.sc, p.tr, p.w->w, p.w->N, p.w->K);
-    FS2_LAUNCH_CHECK();
-    int rc = weight_scale(p.w->w, n, p.w->sc, p.w->sc + 1, st); if (rc) return rc;
-    rc = split_f16(p.w->w, p.w->hi, p.w->lo, n, p.w->sc, st); if (rc) return rc;
+    const int rc = vweight_pack(*p.w, p.src, p.sr, p.sc, p.tr, st);
+    if (rc) return rc;
   }
   FS2_CUDA_CHECK(cudaMemcpyAsync(v->win_sq, window_sq, nf * sizeof(float), cudaMemcpyDeviceToDevice, st));
   v->loaded = true;

@@ -420,6 +420,49 @@ int fs2_mel_magnitude(fs2_vocoder* v, const float* mels, const int64_t* olens, i
 int fs2_griffin_lim(fs2_vocoder* v, const float* mels, const int64_t* olens, int B, int Lmax, int n_iters, float momentum,
                     const int64_t* seeds, const float* angles, float* audio, int* status, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- training features: mel, energy and DIO pitch per utterance (DESIGN.md section 14) ----------------------------- */
+/* What the reference's nvidia_preprocessing.py computes per wav file, for a ragged batch: wav [B, Nmax] fp32 with lens [B]
+ * (int64); utterance b is x_b = wav[b, :lens[b]] and samples past lens[b] are never read.  T_b = lens[b] / hop + 1,
+ * Tmax = Nmax / hop + 1.
+ *   fs2_mel_energy  mel [B, Tmax, n_mels] = log(max(mel_basis . |STFT(x_b)|, 1e-5)) (the layout synthesis returns) and
+ *                   energy [B, Tmax] = sqrt(sum_c |STFT(x_b)|[c]^2); the STFT is the reference's (periodic Hann window,
+ *                   reflect padding of n_fft/2 at the utterance's own edges, stride hop), on the tap GEMM in math_mode.
+ *   fs2_dio         f0 [B, Tmax] float64 and plens [B] int64: WORLD's DIO (pyworld.dio with f0_floor, f0_ceil,
+ *                   channels_in_octave, frame_period = hop / sample_rate * 1000, speed 1, allowed_range) truncated to
+ *                   plens[b] = min(f0_length_b, T_b), f0_length = int(1000.0 * lens[b] / sample_rate / frame_period) + 1.
+ *                   Float64 throughout; the filters run as direct-form circular FIRs.
+ * Frames past T_b / plens[b] are +0.  Utterance b is bit-identical to a B = 1 call on x_b.  No allocation, no
+ * synchronisation: calls can be graph-captured.  Data-dependent checks are reported in *status (device int, zeroed by the call):
+ *   FS2_FEAT_BAD_LENGTH  some lens[b] outside (n_fft/2, Nmax] (reflect padding needs more than n_fft/2 samples); that
+ *                        utterance's outputs are 0 and its plens 0;
+ *   FS2_FEAT_RANGE       some |x| > 1 (or NaN) within lens (the reference asserts |y| <= 1; it also bounds the fp16
+ *                        operand planes, |STFT| <= n_fft/2).
+ * Workspace (one buffer serves both entries), with cutoff = n_fft/2 + 1, cpad = ceil(2 cutoff / 64) * 64,
+ * mpad = ceil(cutoff / 64) * 64, Tp = Tmax + 1, P = 2 round(sample_rate / (f0_floor * 2^(1/channels_in_octave)) / 2),
+ * every term rounded up to 256 bytes; the total is the larger sum plus 256:
+ *   mel  = B Tmax (n_fft + cpad + mpad + n_mels) * 4 + B * 8
+ *   dio  = B * 24 + B (Nmax + 1 + 2P) * 8 + B (Nmax + 2) * 8 + 4 B (Nmax / 2 + 2) * 8 + 4 B * 4 + (n_bands + 4) B Tp * 8
+ *   that is at most 48 B Nmax + 16 KiB * B + 4 KiB at the default 22.05 kHz,
+ *   n_fft 1024, hop 256, 80 mels. */
+#define FS2_FEAT_BAD_LENGTH 1
+#define FS2_FEAT_RANGE 2
+typedef struct fs2_features fs2_features;
+typedef struct fs2_features_config {
+  int32_t sample_rate, n_fft, hop, win_length, n_mels;
+  int32_t math_mode;    /* FS2_MATH_*: the two GEMMs (forward DFT, mel filterbank) */
+  double f0_floor, f0_ceil, channels_in_octave, allowed_range;   /* DIO: 71, 800, 2, 0.1 in the reference */
+} fs2_features_config;
+/* create touches no device; load allocates the weights on the current device, and calls run on that device */
+int fs2_features_create(fs2_features** out, const fs2_features_config* cfg);
+void fs2_features_destroy(fs2_features* f);
+/* device fp32: w_forward [2*cutoff, n_fft] (the reference STFT's windowed forward_basis), mel_basis [n_mels, cutoff] */
+int fs2_features_load(fs2_features* f, const float* w_forward, const float* mel_basis, void* stream);
+int fs2_features_workspace_bytes(fs2_features* f, int B, int Nmax, size_t* bytes);
+int fs2_mel_energy(fs2_features* f, const float* wav, const int64_t* lens, int B, int Nmax, float* mel, float* energy, int* status,
+                   void* ws, size_t ws_bytes, void* stream);
+int fs2_dio(fs2_features* f, const float* wav, const int64_t* lens, int B, int Nmax, double* f0, int64_t* plens, int* status,
+            void* ws, size_t ws_bytes, void* stream);
+
 /* ---- batched MelGAN vocoder (DESIGN.md section 8) ------------------------------------------------------------------- */
 /* seungwonpark/melgan's Generator(mel_channel = 80) on log-mels [B, Lmax, 80] with frame counts olens [B]: utterance b is
  * the generator applied to its own frames mels[b, :olens[b]] followed by 10 frames of -11.5129, every reflection pad at its
