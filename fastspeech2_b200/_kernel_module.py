@@ -1,0 +1,253 @@
+"""Host-side layer the signal modules share (MelGAN, WaveGlow, Griffin-Lim, feature extraction): the per-device handle
+and workspace caches, the status-word check, weight-norm checkpoint normalisation, and the window layer of the two neural
+vocoders (DESIGN.md sections 11-12)."""
+from __future__ import annotations
+
+import ctypes as C
+
+import torch
+import torch.nn as nn
+
+from . import _lib
+
+
+class Handles:
+    """One library handle per device with the key it was loaded from; a call with another key reloads it in place."""
+
+    def __init__(self, destroy: str):
+        self._destroy = destroy  # the C entry that frees a handle
+        self._ents = {}          # device index -> (handle, key)
+
+    def get(self, device: torch.device, key, create, load):
+        """The handle of `device`: create() -> handle on first use, then load(handle, device) whenever key changes."""
+        ent = self._ents.get(device.index)
+        if ent is not None and ent[1] == key:
+            return ent[0]
+        with torch.cuda.device(device):
+            h = ent[0] if ent is not None else create()
+            load(h, device)
+        self._ents[device.index] = (h, key)
+        return h
+
+    def destroy_all(self) -> None:
+        lib = _lib._lib
+        for h, _ in self._ents.values():
+            if lib is not None and h:
+                getattr(lib, self._destroy)(h)
+
+
+def query_bytes(entry: str, *args) -> int:
+    """What a `*_workspace_bytes(..., size_t* bytes)` C entry answers for args."""
+    n = C.c_size_t()
+    _lib.check(getattr(_lib.load(), entry)(*args, C.byref(n)), entry)
+    return n.value
+
+
+def workspace(cache: dict, device: torch.device, nbytes: int) -> torch.Tensor:
+    """cache[device.index]: a uint8 buffer of at least nbytes on `device`, grown on demand.  The smaller buffer goes back
+    to the allocator before the larger one is taken, so growing never holds both."""
+    ws = cache.get(device.index)
+    if ws is not None and ws.numel() >= nbytes:
+        return ws
+    cache.pop(device.index, None)
+    del ws
+    ws = cache[device.index] = torch.empty(nbytes, dtype=torch.uint8, device=device)
+    return ws
+
+
+def check_status(status: torch.Tensor, table) -> None:
+    """Raises ValueError(message) for the first (bit, message) of table whose bit is set in the device status word."""
+    s = int(status.item())                                                   # the call's one host read
+    for bit, message in table:
+        if s & bit:
+            raise ValueError(message)
+
+
+# ---- weight-norm checkpoints --------------------------------------------------------------------------------------
+
+class _WNConv(nn.Module):
+    """The parameters of one weight-normalised convolution, registered in `torch.nn.utils.weight_norm`'s order (bias,
+    weight_g, weight_v).  weight = weight_g * weight_v / |weight_v|, the norm taken per index of dim 0: output channels of
+    a Conv1d [Cout, Cin, k], *input* channels of a ConvTranspose1d [Cin, Cout, k]."""
+
+    def __init__(self, cin: int, cout: int, k: int, transposed: bool = False):
+        super().__init__()
+        proto = nn.ConvTranspose1d(cin, cout, k) if transposed else nn.Conv1d(cin, cout, k)   # torch's default init
+        v = proto.weight.detach()
+        self.transposed = transposed
+        self.bias = nn.Parameter(proto.bias.detach().clone())
+        self.weight_g = nn.Parameter(torch.norm_except_dim(v, 2, 0).clone())
+        self.weight_v = nn.Parameter(v.clone())
+
+    def folded(self) -> torch.Tensor:
+        """fp32 weight, computed on the CPU exactly as torch's weight_norm computes it there (`torch._weight_norm`)."""
+        return torch._weight_norm(self.weight_v.detach().float().cpu(), self.weight_g.detach().float().cpu(), 0)
+
+
+def _take(sd: dict, keys, shapes) -> dict:
+    """Pops keys from sd as fp32 CPU tensors: a missing key, then a wrongly shaped one, raises ValueError naming it."""
+    for k in keys:
+        if k not in sd:
+            raise ValueError(f"missing key {k}")
+    t = {}
+    for k in keys:
+        v = sd.pop(k)
+        if not torch.is_tensor(v) or tuple(v.shape) != tuple(shapes[k]):
+            got = tuple(v.shape) if torch.is_tensor(v) else type(v).__name__
+            raise ValueError(f"key {k} has shape {got}, expected {tuple(shapes[k])}")
+        t[k] = v.detach().float().cpu()
+    return t
+
+
+def normalise_checkpoint(module: nn.Module, sd) -> dict:
+    """Checkpoint dict -> module's state dict, validated key by key.  A weight-normalised convolution (_WNConv) takes
+    `weight_g` / `weight_v` keys or a plain `weight` (after `remove_weight_norm`), stored as v = w, g = |w|, which folds
+    back to w bit for bit; every other key of the state dict is taken as it is.  A missing, unexpected or wrongly shaped
+    key raises ValueError naming it."""
+    sd = dict(sd)
+    out = {}
+    for p, m in module.named_modules():
+        if not isinstance(m, _WNConv):
+            continue
+        if f"{p}.weight" in sd and (f"{p}.weight_g" in sd or f"{p}.weight_v" in sd):
+            raise ValueError(f"unexpected key {p}.weight alongside {p}.weight_g / weight_v")
+        wanted = [f"{p}.bias"] + ([f"{p}.weight"] if f"{p}.weight" in sd else [f"{p}.weight_g", f"{p}.weight_v"])
+        shapes = {f"{p}.bias": m.bias.shape, f"{p}.weight": m.weight_v.shape, f"{p}.weight_g": m.weight_g.shape,
+                  f"{p}.weight_v": m.weight_v.shape}
+        t = _take(sd, wanted, shapes)
+        out[f"{p}.bias"] = t[f"{p}.bias"]
+        if f"{p}.weight" in t:
+            w = t[f"{p}.weight"].contiguous()
+            _, norms = torch._weight_norm_interface(w, torch.ones_like(m.weight_g, device="cpu"), 0)
+            out[f"{p}.weight_g"] = norms.reshape(m.weight_g.shape)
+            out[f"{p}.weight_v"] = w
+        else:
+            out[f"{p}.weight_g"] = t[f"{p}.weight_g"]
+            out[f"{p}.weight_v"] = t[f"{p}.weight_v"]
+    own = module.state_dict()
+    for k in own:
+        if k not in out:
+            out.update(_take(sd, [k], {k: own[k].shape}))
+    if sd:
+        raise ValueError(f"unexpected key {sorted(sd)[0]}")
+    return out
+
+
+# ---- the neural vocoders' windows -----------------------------------------------------------------------------------
+
+class WindowedVocoder(nn.Module):
+    """What MelGANVocoder and WaveGlowVocoder share around their C entries: the handle, reloaded when a parameter
+    changes; the whole call's and the window's workspaces; the status check; and the window layer (`window`'s inputs,
+    `stream`'s loop, `forward(chunk_frames=)`).
+
+    A subclass names its C entries (_DESTROY, _WORKSPACE_BYTES, _WINDOW_BYTES) and provides _create() -> handle,
+    _load(handle, device), _status_table() -> [(bit, message)] and _window_rows(B, n_frames) -> (rows, their formula).
+    A window call is call(h, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws)."""
+
+    HOP = 256                    # audio samples per mel frame
+
+    def __init__(self):
+        super().__init__()
+        self._handles = Handles(self._DESTROY)
+        self._ws = {}            # device index -> workspace tensor
+        self._wws = {}           # device index -> window workspace tensor
+        self._epoch = 0
+
+    def __del__(self):
+        if getattr(self, "_handles", None) is not None:
+            self._handles.destroy_all()
+
+    def invalidate(self) -> None:
+        """Force a weight reload on the next call (after in-place writes through `.data`, which torch does not version)."""
+        self._epoch += 1
+
+    def _fingerprint(self):
+        return (self._epoch,) + tuple((p.data_ptr(), p._version) for p in self.parameters())
+
+    def _handle(self, device: torch.device):
+        return self._handles.get(device, self._fingerprint(), self._create, self._load)
+
+    def _workspace(self, h, B: int, L: int, device: torch.device) -> torch.Tensor:
+        return workspace(self._ws, device, query_bytes(self._WORKSPACE_BYTES, h, B, L))
+
+    def _window_workspace(self, h, B: int, n_frames: int, device: torch.device) -> torch.Tensor:
+        return workspace(self._wws, device, query_bytes(self._WINDOW_BYTES, h, B, n_frames))
+
+    def _check_status(self, status: torch.Tensor) -> None:
+        check_status(status, self._status_table())
+
+    @staticmethod
+    def _check_frames(n_frames) -> None:
+        if isinstance(n_frames, bool) or not isinstance(n_frames, int) or n_frames < 1:
+            raise ValueError(f"n_frames / chunk_frames must be an int >= 1 (got {n_frames!r})")
+
+    def _check_window_size(self, B: int, n_frames: int) -> None:
+        """The window entry's limits on its rows, raised here as ValueError: below 2^31, and at most 65535 * 128 in fp32
+        mode (its CUDA-core GEMMs put 128-row tiles on grid.y)."""
+        self._check_frames(n_frames)
+        rows, formula = self._window_rows(B, n_frames)
+        if rows >= 1 << 31:
+            raise ValueError(f"{formula} must stay below 2^31 window rows (B={B}, n_frames={n_frames})")
+        if self.math_mode == "fp32" and rows > 65535 * 128:
+            raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 window rows, {formula} = {rows} "
+                             f"(B={B}, n_frames={n_frames}); use fewer frames per window")
+
+    @staticmethod
+    def _starts(starts, B: int, device: torch.device) -> torch.Tensor:
+        """starts as an int, a host list or tensor (checked >= 0 here) or a device tensor (checked on the device) -> [B]
+        int64 on `device`."""
+        if isinstance(starts, bool):
+            raise ValueError("starts must be an int, a list or an integer tensor")
+        if isinstance(starts, int):
+            starts = [starts] * B
+        if not torch.is_tensor(starts):
+            try:
+                starts = torch.tensor(starts)
+            except (TypeError, ValueError, RuntimeError):
+                raise ValueError("starts must be an int, a list or an integer tensor") from None
+        if starts.dim() != 1 or starts.shape[0] != B:
+            raise ValueError(f"starts must hold B={B} frame offsets")
+        if starts.dtype.is_floating_point or starts.dtype == torch.bool or starts.is_complex():
+            raise ValueError("starts must be an integer tensor")
+        if not starts.is_cuda:
+            if bool((starts < 0).any()):
+                raise ValueError("every starts[b] must be >= 0")
+        elif starts.device != device:
+            raise ValueError("starts must be on the same device as mels")
+        return starts.to(device=device, dtype=torch.int64).contiguous()
+
+    def _window(self, call, mels, olens, starts, B: int, L: int, n_frames: int):
+        """One window on validated mels / olens: -> (audio [B, n_frames * HOP], alens)."""
+        dev = mels.device
+        starts = self._starts(starts, B, dev)
+        h = self._handle(dev)
+        ws = self._window_workspace(h, B, n_frames, dev)
+        audio = torch.empty((B, n_frames * self.HOP), dtype=torch.float32, device=dev)
+        status = torch.empty((1,), dtype=torch.int32, device=dev)
+        call(h, mels, olens, starts, B, L, n_frames, audio, n_frames * self.HOP, status, ws)
+        self._check_status(status)
+        return audio, (olens - starts).clamp(0, n_frames) * self.HOP
+
+    @staticmethod
+    def _stream(mels, chunk_frames: int, window):
+        """window(c0, n) for the lockstep windows c0 = 0, chunk_frames, ... of mels' Lmax frames, the last one cut at Lmax."""
+        L = mels.shape[1]
+        for c0 in range(0, L, chunk_frames):
+            yield window(c0, min(chunk_frames, L - c0))
+
+    def _chunked(self, call, mels, olens, B: int, L: int, k: int):
+        """forward(chunk_frames=k) on validated mels / olens: windows of k frames written straight into the output, one
+        host read for all of them (their status words are ORed on the device)."""
+        dev = mels.device
+        h = self._handle(dev)
+        ws = self._window_workspace(h, B, min(k, L), dev)
+        audio = torch.empty((B, L * self.HOP), dtype=torch.float32, device=dev)
+        c0s = list(range(0, L, k))
+        starts = torch.tensor(c0s, dtype=torch.int64).repeat_interleave(B).reshape(len(c0s), B).to(dev)
+        status = torch.empty((len(c0s),), dtype=torch.int32, device=dev)
+        for i, c0 in enumerate(c0s):
+            n = min(k, L - c0)
+            call(h, mels, olens, starts[i], B, L, n, audio[:, c0 * self.HOP:], L * self.HOP, status[i: i + 1], ws)
+        bits = torch.tensor([bit for bit, _ in self._status_table()], dtype=torch.int32, device=dev)
+        self._check_status(((status[:, None] & bits) != 0).any(0).int().mul(bits).sum().reshape(1))
+        return audio, olens * self.HOP

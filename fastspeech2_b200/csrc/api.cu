@@ -91,18 +91,6 @@ struct fs2_handle {
 namespace fs2 {
 namespace {
 
-struct Bump {  // bump allocator over a caller-provided (or null = counting) buffer
-  char* base; size_t off = 0, cap;
-  Bump(void* b, size_t c) : base((char*)b), cap(c) {}
-  float* floats(size_t n) { return (float*)bytes(n * sizeof(float)); }
-  void* bytes(size_t n) {
-    size_t a = (off + 255) & ~(size_t)255;
-    off = a + n;
-    return base ? base + a : nullptr;
-  }
-  bool ok() const { return base == nullptr || off <= cap; }
-};
-
 using Map = std::unordered_map<std::string, const fs2_weight_desc*>;
 
 // selects the handle's device for the duration of an ABI call and restores the caller's (torch's) current device

@@ -89,6 +89,16 @@ int planes_to_rows(const __half* planes, long n, float* out, cudaStream_t st);  
 int weight_scale(const float* w, long n, float* scale, float* inv, cudaStream_t st);
 constexpr int MATH_3XTF32 = FS2_MATH_3XTF32;            // also what the other tensor-core modes use for the encoder + predictors
 
+// bump allocator over a caller-provided buffer (null: counting only, the size needed is `off`), 256-byte aligned carves
+struct Bump {
+  char* base; size_t off = 0, cap;
+  Bump(void* b, size_t c) : base((char*)b), cap(c) {}
+  void* bytes(size_t n) { size_t a = (off + 255) & ~(size_t)255; off = a + n; return base ? base + a : nullptr; }
+  float* floats(size_t n) { return (float*)bytes(n * sizeof(float)); }
+  double* doubles(size_t n) { return (double*)bytes(n * sizeof(double)); }
+  bool ok() const { return base == nullptr || off <= cap; }
+};
+
 // Row LayerNorm with the fusions the path needs.
 struct RowNorm {
   const float* x; int ldx;        // [rows, C]

@@ -22,7 +22,6 @@
 //   dio_fix          FixF0Contour, one warp per utterance: steps 1-2 across the lanes, steps 3-4 as sequential walks
 // Every sum has a fixed order and nothing depends on the batch, so utterance b is bit-identical to a B = 1 call.
 #include <math.h>
-#include <string.h>
 
 #include <vector>
 
@@ -45,15 +44,6 @@ inline int grid_for(long n, int block, int cap = 132 * 8) {
 }
 
 inline int matlab_round(double x) { return x > 0 ? (int)(x + 0.5) : (int)(x - 0.5); }
-
-struct Bump {
-  char* base; size_t off = 0, cap;
-  Bump(void* b, size_t c) : base((char*)b), cap(c) {}
-  void* bytes(size_t n) { size_t a = (off + 255) & ~(size_t)255; off = a + n; return base ? base + a : nullptr; }
-  float* floats(size_t n) { return (float*)bytes(n * sizeof(float)); }
-  double* doubles(size_t n) { return (double*)bytes(n * sizeof(double)); }
-  bool ok() const { return base == nullptr || off <= cap; }
-};
 
 // ---- mel and energy ------------------------------------------------------------------------------------------------
 
@@ -583,21 +573,14 @@ int fs2_features_load(fs2_features* f, const float* w_forward, const float* mel_
   const int nf = f->cfg.n_fft;
   f->fwd.N = f->cpad; f->fwd.K = nf;
   f->mel.N = f->cfg.n_mels; f->mel.K = f->mpad;
-  VWeight* ws[2] = {&f->fwd, &f->mel};
-  for (int pass = 0; pass < 2; ++pass) {       // pass 0 sizes the arena, pass 1 carves it
-    Bump b(pass ? f->arena : nullptr, pass ? (size_t)-1 : 0);
-    for (VWeight* w : ws) {
-      const size_t n = (size_t)w->N * w->K;
-      w->w = b.floats(n); w->hi = (__half*)b.bytes(n * 2); w->lo = (__half*)b.bytes(n * 2); w->sc = b.floats(2);
-    }
+  int rc = arena_carve(&f->arena, st, [&](Bump& b) {
+    vweight_carve(b, f->fwd, false);
+    vweight_carve(b, f->mel, false);
     f->taps = b.doubles(f->taps_host.size());
-    if (pass == 0) {
-      if (f->arena) { FS2_CUDA_CHECK(cudaStreamSynchronize(st)); FS2_CUDA_CHECK(cudaFree(f->arena)); f->arena = nullptr; }
-      FS2_CUDA_CHECK(cudaMalloc(&f->arena, b.off + 256));
-    }
-  }
+  });
+  if (rc) return rc;
   FS2_CUDA_CHECK(cudaGetDevice(&f->device));
-  int rc = vweight_pack(f->fwd, w_forward, 2 * f->cutoff, nf, 0, st); if (rc) return rc;
+  rc = vweight_pack(f->fwd, w_forward, 2 * f->cutoff, nf, 0, st); if (rc) return rc;
   rc = vweight_pack(f->mel, mel_basis, f->cfg.n_mels, f->cutoff, 0, st); if (rc) return rc;
   FS2_CUDA_CHECK(cudaMemcpyAsync(f->taps, f->taps_host.data(), f->taps_host.size() * sizeof(double), cudaMemcpyHostToDevice, st));
   FS2_CUDA_CHECK(cudaStreamSynchronize(st));   // the host taps must outlive the copy; loading is not on the hot path

@@ -20,7 +20,6 @@
 // the batch: the same rows see the same K loop, the same element-wise maps and the same overlap-add order.
 #include <float.h>
 #include <math.h>
-#include <string.h>
 
 #include "vocoder_weights.cuh"
 
@@ -198,50 +197,7 @@ __global__ void mag_transpose_kernel(const float* __restrict__ m, int ldm, int B
   }
 }
 
-// dst [DR][DC] = src [SR][SC] (or its transpose), zero-padded
-__global__ void pad_pack_kernel(const float* __restrict__ src, int SR, int SC, int transpose, float* __restrict__ dst, int DR, int DC) {
-  const long total = (long)DR * DC;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const int r = (int)(i / DC), c = (int)(i % DC);
-    const int sr = transpose ? c : r, sc = transpose ? r : c;
-    dst[i] = sr < SR && sc < SC ? src[(long)sr * SC + sc] : 0.f;
-  }
-}
-
-struct Bump {
-  char* base; size_t off = 0, cap;
-  Bump(void* b, size_t c) : base((char*)b), cap(c) {}
-  void* bytes(size_t n) { size_t a = (off + 255) & ~(size_t)255; off = a + n; return base ? base + a : nullptr; }
-  float* floats(size_t n) { return (float*)bytes(n * sizeof(float)); }
-  bool ok() const { return base == nullptr || off <= cap; }
-};
-
 }  // namespace
-
-int vweight_pack(VWeight& w, const float* src, int SR, int SC, int transpose, cudaStream_t st) {
-  const long n = (long)w.N * w.K;
-  pad_pack_kernel<<<grid_for(n, 256), 256, 0, st>>>(src, SR, SC, transpose, w.w, w.N, w.K);
-  FS2_LAUNCH_CHECK();
-  int rc = weight_scale(w.w, n, w.sc, w.sc + 1, st); if (rc) return rc;
-  return split_f16(w.w, w.hi, w.lo, n, w.sc, st);
-}
-
-int vweight_gemm(int math_mode, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens, float* out,
-                 cudaStream_t st) {
-  TapGemm g;
-  memset(&g, 0, sizeof(g));
-  g.B = B; g.L = L; g.K = w.K; g.N = w.N; g.taps = 1; g.act = act; g.out = out; g.ldo = w.N; g.lens = lens;
-  g.w = w.w; g.a_inv = 1.0f;
-  if (math_mode == FS2_MATH_FP32 || math_mode == FS2_MATH_TF32) {
-    g.x = (const float*)a; g.ldx = w.K;
-    return math_mode == FS2_MATH_FP32 ? tap_gemm_fp32(g, st) : tap_gemm_tf32(g, st);
-  }
-  g.ldx = w.K;
-  g.xp = (const __half*)a; g.w_hi = w.hi; g.w_lo = w.lo; g.w_inv = w.sc + 1; g.a_inv = kPlaneInv;
-  g.precise = math_mode == FS2_MATH_3XTF32;
-  return tap_gemm_planes(g, st);
-}
-
 }  // namespace fs2
 
 struct fs2_vocoder {
@@ -278,20 +234,13 @@ GlPlan plan(const fs2_vocoder* v, Bump& b, int B, int L, bool momentum_state) {
   return p;
 }
 
-
-// out [rows][w.N] = act(a [rows][w.K] . w^T), rows t >= lens[b] written as 0 (and skipped by the tensor-core kernel)
-int gemm(const fs2_vocoder* v, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens, float* out, cudaStream_t st) {
-  return vweight_gemm(v->cfg.math_mode, w, a, B, L, act, lens, out, st);
-}
-
-
 int mel_stage(fs2_vocoder* v, const float* mels, const int64_t* olens, int B, int L, const GlPlan& p, int* status, cudaStream_t st) {
   const int kind = out_kind(v->cfg.math_mode), nm = v->cfg.n_mels;
   auto k = pick(kind, mel_expand_kernel<OUT_HILO>, mel_expand_kernel<OUT_HI>, mel_expand_kernel<OUT_F32>);
   const long total = (long)B * L * (nm / 2);
   k<<<grid_for(total, 256), 256, 0, st>>>(mels, olens, B, L, nm, v->cfg.hop, v->cfg.n_fft / 2, (float*)p.melx, (__half*)p.melx, status);
   FS2_LAUNCH_CHECK();
-  return gemm(v, v->mel, p.melx, B, L, ACT_RELU, olens, p.mag, st);
+  return vweight_gemm(v->cfg.math_mode, v->mel, p.melx, B, L, ACT_RELU, olens, p.mag, st);
 }
 
 int check_call(fs2_vocoder* v, const float* mels, const int64_t* olens, int B, int L, const int* status, void* ws) {
@@ -341,25 +290,15 @@ int fs2_vocoder_load(fs2_vocoder* v, const float* w_forward, const float* w_inve
   v->fwd.N = v->cpad; v->fwd.K = nf;
   v->inv.N = nf; v->inv.K = v->cpad;
   v->mel.N = v->mpad; v->mel.K = v->cfg.n_mels;
-  VWeight* ws[3] = {&v->fwd, &v->inv, &v->mel};
-  for (int pass = 0; pass < 2; ++pass) {       // pass 0 sizes the arena, pass 1 carves it
-    Bump b(pass ? v->arena : nullptr, pass ? (size_t)-1 : 0);
-    for (VWeight* w : ws) {
-      const size_t n = (size_t)w->N * w->K;
-      w->w = b.floats(n); w->hi = (__half*)b.bytes(n * 2); w->lo = (__half*)b.bytes(n * 2); w->sc = b.floats(2);
-    }
+  int rc = arena_carve(&v->arena, st, [&](Bump& b) {
+    for (VWeight* w : {&v->fwd, &v->inv, &v->mel}) vweight_carve(b, *w, false);
     v->win_sq = b.floats(nf);
-    if (pass == 0) {
-      if (v->arena) { FS2_CUDA_CHECK(cudaStreamSynchronize(st)); FS2_CUDA_CHECK(cudaFree(v->arena)); v->arena = nullptr; }
-      FS2_CUDA_CHECK(cudaMalloc(&v->arena, b.off + 256));
-    }
-  }
+  });
+  if (rc) return rc;
   struct { const float* src; int sr, sc, tr; VWeight* w; } packs[3] = {
       {w_forward, c2, nf, 0, &v->fwd}, {w_inverse, c2, nf, 1, &v->inv}, {mel_inverse, v->cutoff, v->cfg.n_mels, 0, &v->mel}};
-  for (auto& p : packs) {
-    const int rc = vweight_pack(*p.w, p.src, p.sr, p.sc, p.tr, st);
-    if (rc) return rc;
-  }
+  for (auto& p : packs)
+    if ((rc = vweight_pack(*p.w, p.src, p.sr, p.sc, p.tr, st))) return rc;
   FS2_CUDA_CHECK(cudaMemcpyAsync(v->win_sq, window_sq, nf * sizeof(float), cudaMemcpyDeviceToDevice, st));
   v->loaded = true;
   return FS2_OK;
@@ -421,7 +360,7 @@ int fs2_griffin_lim(fs2_vocoder* v, const float* mels, const int64_t* olens, int
                                  rec32, recp, status);
     FS2_LAUNCH_CHECK();
   }
-  if ((rc = gemm(v, v->inv, p.rec, B, Lmax, ACT_NONE, olens, p.fr, st))) return rc;
+  if ((rc = vweight_gemm(v->cfg.math_mode, v->inv, p.rec, B, Lmax, ACT_NONE, olens, p.fr, st))) return rc;
   const dim3 ola_grid((Lmax + FPB - 1) / FPB, B);
   const size_t ola_smem = (size_t)((FPB - 1) * hop + nf) * sizeof(float);
   auto ola = pick(kind, ola_frame_kernel<OUT_HILO>, ola_frame_kernel<OUT_HI>, ola_frame_kernel<OUT_F32>);
@@ -432,13 +371,13 @@ int fs2_griffin_lim(fs2_vocoder* v, const float* mels, const int64_t* olens, int
     ola<<<ola_grid, 256, ola_smem, st>>>(p.fr, v->win_sq, olens, Lmax, nf, hop, scale, frm32, frmp, rows * nf, status);
     FS2_LAUNCH_CHECK();
     float* z = p.z[it & 1];
-    if ((rc = gemm(v, v->fwd, p.frames, B, Lmax, ACT_NONE, olens, z, st))) return rc;
+    if ((rc = vweight_gemm(v->cfg.math_mode, v->fwd, p.frames, B, Lmax, ACT_NONE, olens, z, st))) return rc;
     // Z_prev starts at 0: the first pass has no momentum term
     auto k = it == 0 ? proj0 : proj;
     k<<<proj_grid, 256, 0, st>>>(p.mag, v->mpad, z, p.z[(it + 1) & 1], mom_k, seeds, angles, olens, B, Lmax, v->cutoff, v->cpad, hop,
                                  half, rec32, recp, status);
     FS2_LAUNCH_CHECK();
-    if ((rc = gemm(v, v->inv, p.rec, B, Lmax, ACT_NONE, olens, p.fr, st))) return rc;
+    if ((rc = vweight_gemm(v->cfg.math_mode, v->inv, p.rec, B, Lmax, ACT_NONE, olens, p.fr, st))) return rc;
   }
   const long n_audio = (long)B * (Lmax - 1) * hop;
   ola_audio_kernel<<<grid_for(n_audio, 256), 256, 0, st>>>(p.fr, v->win_sq, olens, B, Lmax, nf, hop, scale, audio);

@@ -32,11 +32,10 @@
 // outside the window as 0: such rows lie in the halo and are discarded.  Only rows whose values equal the whole call's
 // (all but `margin` rows at a window side that is not an utterance edge) are range-checked.
 #include <math.h>
-#include <string.h>
 
 #include <algorithm>
 
-#include "operand_planes.cuh"
+#include "vocoder_weights.cuh"
 
 namespace fs2 {
 namespace {
@@ -484,19 +483,6 @@ __global__ void melgan_bias_kernel(const float* __restrict__ b, const float* __r
     dst[n] = b2 ? b[n] + b2[n] : b[n % Cout];
 }
 
-struct MWeight {               // one GEMM weight [N][K]: fp32 (fp32 / tf32 families) and scaled fp16 planes, bias [N]
-  float* w = nullptr; __half* hi = nullptr; __half* lo = nullptr; float* sc = nullptr; float* bias = nullptr;   // sc = [scale, 1 / scale]
-  int N = 0, K = 0;
-};
-
-struct Bump {
-  char* base; size_t off = 0, cap;
-  Bump(void* b, size_t c) : base((char*)b), cap(c) {}
-  void* bytes(size_t n) { size_t a = (off + 255) & ~(size_t)255; off = a + n; return base ? base + a : nullptr; }
-  float* floats(size_t n) { return (float*)bytes(n * sizeof(float)); }
-  bool ok() const { return base == nullptr || off <= cap; }
-};
-
 }  // namespace
 }  // namespace fs2
 
@@ -504,7 +490,7 @@ struct fs2_melgan_gen {
   int device = 0, math_mode = 0;
   bool loaded = false;
   void* arena = nullptr;
-  fs2::MWeight pre, up[fs2::kStages], dil[fs2::kStages][3], pair[fs2::kStages][3];
+  fs2::VWeight pre, up[fs2::kStages], dil[fs2::kStages][3], pair[fs2::kStages][3];
   float* post_w = nullptr;     // [7][32]
   float* post_b = nullptr;
 };
@@ -554,37 +540,13 @@ MgPlan plan(Bump& b, int B, int L, bool fused) {
 
 // one GEMM weight from its torch-layout tensors (melgan_pack_kernel's kind, Cin, Cout, taps, s): the packed fp32 [N][K],
 // the bias [N], the power-of-two scale and the fp16 planes; w->N, w->K and the buffers are set by the caller
-int pack_weight(MWeight* w, int kind, const float* wt, const float* wt2, const float* b, const float* b2, int Cin, int Cout, int taps,
+int pack_weight(const VWeight& w, int kind, const float* wt, const float* wt2, const float* b, const float* b2, int Cin, int Cout, int taps,
                 int s, cudaStream_t st) {
-  const long n = (long)w->N * w->K;
-  melgan_pack_kernel<<<grid_for(n, 256), 256, 0, st>>>(kind, wt, wt2, w->N, w->K, Cin, Cout, taps, s, w->w);
+  melgan_pack_kernel<<<grid_for((long)w.N * w.K, 256), 256, 0, st>>>(kind, wt, wt2, w.N, w.K, Cin, Cout, taps, s, w.w);
   FS2_LAUNCH_CHECK();
-  melgan_bias_kernel<<<grid_for(w->N, 256), 256, 0, st>>>(b, b2, w->N, Cout, w->bias);
+  melgan_bias_kernel<<<grid_for(w.N, 256), 256, 0, st>>>(b, b2, w.N, Cout, w.bias);
   FS2_LAUNCH_CHECK();
-  int rc = weight_scale(w->w, n, w->sc, w->sc + 1, st); if (rc) return rc;
-  return split_f16(w->w, w->hi, w->lo, n, w->sc, st);
-}
-
-// carves one MWeight of N x K out of a Bump
-void carve(Bump& b, MWeight* w, int N, int K) {
-  w->N = N; w->K = K;
-  const size_t n = (size_t)N * K;
-  w->w = b.floats(n); w->hi = (__half*)b.bytes(n * 2); w->lo = (__half*)b.bytes(n * 2); w->sc = b.floats(2); w->bias = b.floats(N);
-}
-
-// out [B * Lp][w.N] = a [B * Lp][w.K] . w^T + bias, rows t >= lens[b] written as 0 (and skipped by the tensor-core kernel)
-int gemm(int mode, const MWeight& w, const void* a, int B, int Lp, const int64_t* lens, float* out, cudaStream_t st) {
-  TapGemm g;
-  memset(&g, 0, sizeof(g));
-  g.B = B; g.L = Lp; g.K = w.K; g.N = w.N; g.taps = 1; g.act = ACT_NONE; g.out = out; g.ldo = w.N; g.lens = lens;
-  g.w = w.w; g.bias = w.bias; g.a_inv = 1.0f; g.ldx = w.K;
-  if (mode == FS2_MATH_FP32 || mode == FS2_MATH_TF32) {
-    g.x = (const float*)a;
-    return mode == FS2_MATH_FP32 ? tap_gemm_fp32(g, st) : tap_gemm_tf32(g, st);
-  }
-  g.xp = (const __half*)a; g.w_hi = w.hi; g.w_lo = w.lo; g.w_inv = w.sc + 1; g.a_inv = kPlaneInv;
-  g.precise = mode == FS2_MATH_3XTF32;
-  return tap_gemm_planes(g, st);
+  return vweight_planes(w, st);
 }
 
 // the taps producer: operand rows [B * Lp] (window win, lens) from x, ldx rows per utterance in window xwin (nullptr: the
@@ -607,7 +569,7 @@ bool fused_blocks(int mode, int C) {
 }
 
 template <int C>
-int run_block(int mode, const MWeight& w1, const MWeight& w2, const float* x, const int64_t* lens, const int64_t* win, int B, int Lp, int d,
+int run_block(int mode, const VWeight& w1, const VWeight& w2, const float* x, const int64_t* lens, const int64_t* win, int B, int Lp, int d,
               int margin, float* out, int* status, cudaStream_t st) {
   constexpr int warps = C == 256 ? 2 : 4;          // as in melgan_block_kernel: 16 rows per warp
   const long rows = (long)B * Lp, ctas = (rows + 16 * warps - 1) / (16 * warps);
@@ -621,7 +583,7 @@ int run_block(int mode, const MWeight& w1, const MWeight& w2, const float* x, co
 // One residual block x -> out on [B * Lp][C] rows (dilation d, w1 = the dilated conv, w2 = [W2 | Ws]): the fused kernel
 // (f16 / 3xF16, C in {32, 64, 128, 256}), or producers + tap-GEMMs through the scratch operand a (rows * 3C floats) and h
 // (rows * C floats).  win, margin: the rows' window and its halo rows after this block (see exact_row).
-int res_block(int mode, bool fused, const MWeight& w1, const MWeight& w2, const float* x, const int64_t* lens, const int64_t* win, int B,
+int res_block(int mode, bool fused, const VWeight& w1, const VWeight& w2, const float* x, const int64_t* lens, const int64_t* win, int B,
               int Lp, int C, int d, int margin, void* a, float* h, float* out, int* status, cudaStream_t st) {
   if (fused) {
     return C == 256 ? run_block<256>(mode, w1, w2, x, lens, win, B, Lp, d, margin, out, status, st)
@@ -631,20 +593,20 @@ int res_block(int mode, bool fused, const MWeight& w1, const MWeight& w2, const 
   }
   const int kind = out_kind(mode);
   int rc = run_taps(kind, true, x, nullptr, Lp, lens, win, B, Lp, C, d, margin, a, status, st);
-  if (rc || (rc = gemm(mode, w1, a, B, Lp, lens, h, st))) return rc;
+  if (rc || (rc = vweight_gemm(mode, w1, a, B, Lp, ACT_NONE, lens, h, st))) return rc;
   auto concat = pick(kind, melgan_concat_kernel<OUT_HILO>, melgan_concat_kernel<OUT_HI>, melgan_concat_kernel<OUT_F32>);
   concat<<<grid_for((long)B * Lp * (2 * C / 4), 256), 256, 0, st>>>(h, x, lens, win, B, Lp, C, margin, (float*)a, (__half*)a, status);
   FS2_LAUNCH_CHECK();
-  return gemm(mode, w2, a, B, Lp, lens, out, st);
+  return vweight_gemm(mode, w2, a, B, Lp, ACT_NONE, lens, out, st);
 }
 
 // lrelu + ConvTranspose1d (k = 2s, stride s, pad s/2) x [B * Lin][Cin] -> out [B * Lin][s Cout] = [B * Lin * s][Cout], through
 // the scratch operand a (rows * 3 Cin floats): rows t < lens[b] of x in, rows >= lens[b] * s of out written as 0.  A window:
 // the input window (win, lens; Lin rows per utterance) is read from x's own window xwin of ldx rows per utterance.
-int upsample(int mode, const MWeight& w, const float* x, const int64_t* xwin, int ldx, const int64_t* lens, const int64_t* win, int B, int Lin,
+int upsample(int mode, const VWeight& w, const float* x, const int64_t* xwin, int ldx, const int64_t* lens, const int64_t* win, int B, int Lin,
              int Cin, void* a, float* out, int* status, cudaStream_t st) {
   int rc = run_taps(out_kind(mode), false, x, xwin, ldx, lens, win, B, Lin, Cin, 1, 1, a, status, st);
-  return rc ? rc : gemm(mode, w, a, B, Lin, lens, out, st);
+  return rc ? rc : vweight_gemm(mode, w, a, B, Lin, ACT_NONE, lens, out, st);
 }
 
 // The generator on the plan p: whole utterances (starts == nullptr; every buffer (Lmax + 10) * up_s rows per utterance,
@@ -666,7 +628,7 @@ int generate(const fs2_melgan_gen* m, const MgPlan& p, const float* mels, const 
                                                                                 (__half*)p.a, status);
     FS2_LAUNCH_CHECK();
   }
-  if ((rc = gemm(mode, m->pre, p.a, B, rows(0), lens(0, 0), p.x[0], st))) return rc;
+  if ((rc = vweight_gemm(mode, m->pre, p.a, B, rows(0), ACT_NONE, lens(0, 0), p.x[0], st))) return rc;
   int cur = 0;
   for (int s = 0; s < kStages; ++s) {
     const int C = kCout[s], cw = convt_win(s), Lin = w ? (int)convt_rows(s, nf) : rows(s);
@@ -739,7 +701,7 @@ int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float*
   cudaStream_t st = (cudaStream_t)stream;
   // layer index of the state_dict order: 0 = generator.1; stage s: 1 + 10 s = its ConvTranspose1d, then the ResStack's
   // blocks.i.2 (2 + 10 s + 2 i), blocks.i.4 (3 + 10 s + 2 i), shortcuts.i (8 + 10 s + i); 41 = generator.16
-  struct Job { MWeight* w; int kind, N, K, Cin, Cout, taps, s; int l, l2; };
+  struct Job { VWeight* w; int kind, N, K, Cin, Cout, taps, s; int l, l2; };
   Job jobs[1 + kStages * 7];
   int nj = 0;
   jobs[nj++] = {&m->pre, 0, 512, kMels * kPreTaps, kMels, 512, kPreTaps, 0, 0, -1};
@@ -751,21 +713,18 @@ int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float*
       jobs[nj++] = {&m->pair[s][i], 2, co, 2 * co, co, co, 1, 0, base + 2 + 2 * i, base + 7 + i};
     }
   }
-  for (int pass = 0; pass < 2; ++pass) {       // pass 0 sizes the arena, pass 1 carves it
-    Bump b(pass ? m->arena : nullptr, pass ? (size_t)-1 : 0);
-    for (int j = 0; j < nj; ++j) carve(b, jobs[j].w, jobs[j].N, jobs[j].K);
+  for (int j = 0; j < nj; ++j) { jobs[j].w->N = jobs[j].N; jobs[j].w->K = jobs[j].K; }
+  m->loaded = false;
+  int rc = arena_carve(&m->arena, st, [&](Bump& b) {
+    for (int j = 0; j < nj; ++j) vweight_carve(b, *jobs[j].w, true);
     m->post_w = b.floats(kPostTaps * kPostC);
     m->post_b = b.floats(1);
-    if (pass == 0) {
-      if (m->arena) { FS2_CUDA_CHECK(cudaStreamSynchronize(st)); FS2_CUDA_CHECK(cudaFree(m->arena)); m->arena = nullptr; }
-      m->loaded = false;
-      FS2_CUDA_CHECK(cudaMalloc(&m->arena, b.off + 256));
-    }
-  }
+  });
+  if (rc) return rc;
   for (int j = 0; j < nj; ++j) {
     const Job& q = jobs[j];
-    const int rc = pack_weight(q.w, q.kind, weights[q.l], q.l2 >= 0 ? weights[q.l2] : nullptr, biases[q.l], q.l2 >= 0 ? biases[q.l2] : nullptr,
-                               q.Cin, q.Cout, q.taps, q.s, st);
+    rc = pack_weight(*q.w, q.kind, weights[q.l], q.l2 >= 0 ? weights[q.l2] : nullptr, biases[q.l], q.l2 >= 0 ? biases[q.l2] : nullptr,
+                     q.Cin, q.Cout, q.taps, q.s, st);
     if (rc) return rc;
   }
   melgan_pack_kernel<<<1, 256, 0, st>>>(0, weights[kLayers - 1], nullptr, 1, kPostTaps * kPostC, kPostC, 1, kPostTaps, 0, m->post_w);
@@ -846,21 +805,23 @@ int fs2_op_melgan_block(int math_mode, int route, int C, const float* x, const i
   FS2_REQUIRE(rows * 3 * C < (1L << 31) && (math_mode != FS2_MATH_FP32 || rows <= 65535L * 128), "%s: too many rows (%ld)", who, rows);
   cudaStream_t st = (cudaStream_t)stream;
   const bool fused = route == 0 ? fused_blocks(math_mode, C) : route == 2;
-  MWeight wd, wp;
+  VWeight wd, wp;
+  wd.N = C; wd.K = 3 * C;
+  wp.N = C; wp.K = 2 * C;
   void* a = nullptr;
   float* h = nullptr;
   void* base = nullptr;
   for (int pass = 0; pass < 2; ++pass) {       // pass 0 sizes the temporary, pass 1 carves it
     Bump b(base, (size_t)-1);
-    carve(b, &wd, C, 3 * C);
-    carve(b, &wp, C, 2 * C);
+    vweight_carve(b, wd, true);
+    vweight_carve(b, wp, true);
     a = b.floats((size_t)rows * 3 * C);
     h = b.floats((size_t)rows * C);
     if (pass == 0) FS2_CUDA_CHECK(cudaMallocAsync(&base, b.off + 256, st));
   }
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
-  int rc = pack_weight(&wd, 0, w1, nullptr, b1, nullptr, C, C, 3, 0, st);
-  if (!rc) rc = pack_weight(&wp, 2, w2, ws, b2, bs, C, C, 1, 0, st);
+  int rc = pack_weight(wd, 0, w1, nullptr, b1, nullptr, C, C, 3, 0, st);
+  if (!rc) rc = pack_weight(wp, 2, w2, ws, b2, bs, C, C, 1, 0, st);
   if (!rc) rc = res_block(math_mode, fused, wd, wp, x, lens, nullptr, B, Lp, C, d, 0, a, h, out, status, st);
   cudaFreeAsync(base, st);
   return rc;
@@ -881,17 +842,18 @@ int fs2_op_melgan_upsample(int math_mode, int Cin, int Cout, int s, const float*
   FS2_REQUIRE(rows * s * Cout < (1L << 31) && rows * 3 * Cin < (1L << 31) && (math_mode != FS2_MATH_FP32 || rows <= 65535L * 128),
               "%s: too many rows (%ld)", who, rows);
   cudaStream_t st = (cudaStream_t)stream;
-  MWeight wu;
+  VWeight wu;
+  wu.N = s * Cout; wu.K = 3 * Cin;
   void* a = nullptr;
   void* base = nullptr;
   for (int pass = 0; pass < 2; ++pass) {
     Bump bb(base, (size_t)-1);
-    carve(bb, &wu, s * Cout, 3 * Cin);
+    vweight_carve(bb, wu, true);
     a = bb.floats((size_t)rows * 3 * Cin);
     if (pass == 0) FS2_CUDA_CHECK(cudaMallocAsync(&base, bb.off + 256, st));
   }
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
-  int rc = pack_weight(&wu, 1, w, nullptr, b, nullptr, Cin, Cout, 0, s, st);
+  int rc = pack_weight(wu, 1, w, nullptr, b, nullptr, Cin, Cout, 0, s, st);
   if (!rc) rc = upsample(math_mode, wu, x, nullptr, Lin, lens, nullptr, B, Lin, Cin, a, out, status, st);
   cudaFreeAsync(base, st);
   return rc;

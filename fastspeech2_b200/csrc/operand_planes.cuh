@@ -1,5 +1,5 @@
-// Helpers of the kernels that write tap-GEMM operands directly (griffin_lim.cu, melgan.cu): the operand's form by math
-// mode, and the range an fp16 operand plane holds.
+// Helpers of the kernels that write tap-GEMM operands directly (griffin_lim.cu, melgan.cu, waveglow.cu, features.cu, through
+// vocoder_weights.cuh): the operand's form by math mode, and the range an fp16 operand plane holds.
 #pragma once
 #include "common.cuh"
 

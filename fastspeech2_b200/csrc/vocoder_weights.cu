@@ -1,0 +1,61 @@
+// The signal modules' GEMM weights (vocoder_weights.cuh).
+#include <string.h>
+
+#include "vocoder_weights.cuh"
+
+namespace fs2 {
+namespace {
+
+inline int grid_for(long n, int block, int cap = 132 * 8) {
+  long g = (n + block - 1) / block;
+  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+}
+
+// dst [DR][DC] = src [SR][SC] (or its transpose), zero-padded
+__global__ void pad_pack_kernel(const float* __restrict__ src, int SR, int SC, int transpose, float* __restrict__ dst, int DR, int DC) {
+  const long total = (long)DR * DC;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int r = (int)(i / DC), c = (int)(i % DC);
+    const int sr = transpose ? c : r, sc = transpose ? r : c;
+    dst[i] = sr < SR && sc < SC ? src[(long)sr * SC + sc] : 0.f;
+  }
+}
+
+}  // namespace
+
+void vweight_carve(Bump& b, VWeight& w, bool bias) {
+  const size_t n = (size_t)w.taps * w.N * w.K;
+  w.w = b.floats(n); w.hi = (__half*)b.bytes(n * 2); w.lo = (__half*)b.bytes(n * 2); w.sc = b.floats(2);
+  w.bias = bias ? b.floats(w.N) : nullptr;
+}
+
+int vweight_planes(const VWeight& w, cudaStream_t st) {
+  const long n = (long)w.taps * w.N * w.K;
+  int rc = weight_scale(w.w, n, w.sc, w.sc + 1, st); if (rc) return rc;
+  return split_f16(w.w, w.hi, w.lo, n, w.sc, st);
+}
+
+int vweight_pack(VWeight& w, const float* src, int SR, int SC, int transpose, cudaStream_t st) {
+  const long n = (long)w.N * w.K;
+  pad_pack_kernel<<<grid_for(n, 256), 256, 0, st>>>(src, SR, SC, transpose, w.w, w.N, w.K);
+  FS2_LAUNCH_CHECK();
+  return vweight_planes(w, st);
+}
+
+int vweight_gemm(int math_mode, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens, float* out,
+                 cudaStream_t st, const float* resid, int dil, __half* outp) {
+  TapGemm g;
+  memset(&g, 0, sizeof(g));
+  g.B = B; g.L = L; g.K = w.K; g.N = w.N; g.taps = w.taps; g.dil = dil; g.act = act; g.out = out; g.ldo = w.N; g.lens = lens;
+  g.w = w.w; g.bias = w.bias; g.resid = resid; g.ldr = w.N; g.a_inv = 1.0f; g.ldx = w.K;
+  if (math_mode == FS2_MATH_FP32 || math_mode == FS2_MATH_TF32) {
+    g.x = (const float*)a;
+    return math_mode == FS2_MATH_FP32 ? tap_gemm_fp32(g, st) : tap_gemm_tf32(g, st);
+  }
+  g.xp = (const __half*)a; g.w_hi = w.hi; g.w_lo = w.lo; g.w_inv = w.sc + 1; g.a_inv = kPlaneInv;
+  g.precise = math_mode == FS2_MATH_3XTF32;
+  if (outp) { g.outp = outp; g.ldo_p = w.N; g.outp_lo = g.precise; }
+  return tap_gemm_planes(g, st);
+}
+
+}  // namespace fs2

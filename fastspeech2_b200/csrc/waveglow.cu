@@ -35,9 +35,8 @@
 // operand and the cond planes are keyed by global frames and steps, so they are exact everywhere in the buffer; start and
 // gate range-check only rows whose values equal the whole call's (exact_row).
 #include <math.h>
-#include <string.h>
 
-#include "operand_planes.cuh"
+#include "vocoder_weights.cuh"
 
 namespace fs2 {
 namespace {
@@ -374,24 +373,11 @@ __global__ void wg_add_kernel(const float* __restrict__ a, const float* __restri
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dst[i] = a[i] + b[i];
 }
 
-struct WWeight {               // one GEMM weight [taps][N][K]: fp32 (fp32 / tf32 families) and scaled fp16 planes, bias [N]
-  float* w = nullptr; __half* hi = nullptr; __half* lo = nullptr; float* sc = nullptr; float* bias = nullptr;   // sc = [scale, 1 / scale]
-  int N = 0, K = 0, taps = 1;
-};
-
 struct WFlow {
   float *start_w = nullptr, *start_b = nullptr;   // [C][h], [C]
-  WWeight cond[kLayers], in[kLayers], res[kLayers - 1], skip[kLayers];
+  VWeight cond[kLayers], in[kLayers], res[kLayers - 1], skip[kLayers];
   float *end_w = nullptr, *end_b = nullptr;       // [2h][C], [2h]
   float* winv = nullptr;                          // [c][c]
-};
-
-struct Bump {
-  char* base; size_t off = 0, cap;
-  Bump(void* b, size_t c) : base((char*)b), cap(c) {}
-  void* bytes(size_t n) { size_t a = (off + 255) & ~(size_t)255; off = a + n; return base ? base + a : nullptr; }
-  float* floats(size_t n) { return (float*)bytes(n * sizeof(float)); }
-  bool ok() const { return base == nullptr || off <= cap; }
 };
 
 }  // namespace
@@ -401,7 +387,7 @@ struct fs2_waveglow_net {
   int device = 0, math_mode = 0, C = 0;
   bool loaded = false;
   void* arena = nullptr;
-  fs2::WWeight up;
+  fs2::VWeight up;
   fs2::WFlow flows[fs2::kFlows];
 };
 
@@ -455,24 +441,6 @@ WgPlan plan(Bump& b, int mode, int C, int B, int L, bool window = false) {
   p.condp = planes ? (__half*)b.floats(rows * kCond) : nullptr;
   p.cond = planes && 2 * C >= kCond ? p.ia : b.floats(rows * kCond);    // ia holds rows * 2C floats
   return p;
-}
-
-// out [B * L][w.N] = a [B * L][w.K] (taps at dilation dil) . w^T + bias (+ resid), rows t >= lens[b] written as 0 (and
-// skipped by the tensor-core kernel); outp (plane modes, nullable): the result's operand planes as well
-int gemm(const fs2_waveglow_net* m, const WWeight& w, const void* a, int B, int L, const int64_t* lens, int dil, const float* resid,
-         float* out, __half* outp, cudaStream_t st) {
-  TapGemm g;
-  memset(&g, 0, sizeof(g));
-  g.B = B; g.L = L; g.K = w.K; g.N = w.N; g.taps = w.taps; g.dil = dil; g.act = ACT_NONE; g.out = out; g.ldo = w.N; g.lens = lens;
-  g.w = w.w; g.bias = w.bias; g.resid = resid; g.ldr = w.N; g.a_inv = 1.0f; g.ldx = w.K;
-  if (!plane_mode(m->math_mode)) {
-    g.x = (const float*)a;
-    return m->math_mode == FS2_MATH_FP32 ? tap_gemm_fp32(g, st) : tap_gemm_tf32(g, st);
-  }
-  g.xp = (const __half*)a; g.w_hi = w.hi; g.w_lo = w.lo; g.w_inv = w.sc + 1; g.a_inv = kPlaneInv;
-  g.precise = m->math_mode == FS2_MATH_3XTF32;
-  if (outp) { g.outp = outp; g.ldo_p = w.N; g.outp_lo = g.precise; }
-  return tap_gemm_planes(g, st);
 }
 
 int check_size(const fs2_waveglow_net* m, int B, int L) {
@@ -529,7 +497,7 @@ int run(const fs2_waveglow_net* m, const WgPlan& p, const float* mels, const int
     k<<<grid_for((long)B * L * (kUpK / 4), 256), 256, 0, st>>>(mels, p.lensF, win, B, L, Lmax, (float*)p.up_a, (__half*)p.up_a, status);
     FS2_LAUNCH_CHECK();
   }
-  if ((rc = gemm(m, m->up, p.up_a, B, L, p.lensF, 1, nullptr, p.cond, nullptr, st))) return rc;
+  if ((rc = vweight_gemm(m->math_mode, m->up, p.up_a, B, L, ACT_NONE, p.lensF, p.cond, st))) return rc;
   if (planes) {
     auto k = kind == OUT_HILO ? wg_planes_kernel<OUT_HILO> : wg_planes_kernel<OUT_HI>;
     k<<<grid_for(rows * (kCond / 4), 256), 256, 0, st>>>(p.cond, p.lensS, B, Ls, kCond, p.condp, status);
@@ -547,18 +515,18 @@ int run(const fs2_waveglow_net* m, const WgPlan& p, const float* mels, const int
     FS2_LAUNCH_CHECK();
     int cur = 0, sk = 0;
     for (int i = 0; i < kLayers; ++i) {
-      if ((rc = gemm(m, f.cond[i], cond_a, B, Ls, p.lensS, 1, nullptr, p.cd, nullptr, st))) return rc;
+      if ((rc = vweight_gemm(m->math_mode, f.cond[i], cond_a, B, Ls, ACT_NONE, p.lensS, p.cd, st))) return rc;
       const void* xa = planes ? (const void*)p.xp : (const void*)p.x[cur];
-      if ((rc = gemm(m, f.in[i], xa, B, Ls, p.lensS, 1 << i, p.cd, p.ia, nullptr, st))) return rc;
+      if ((rc = vweight_gemm(m->math_mode, f.in[i], xa, B, Ls, ACT_NONE, p.lensS, p.ia, st, p.cd, 1 << i))) return rc;
       // layer i's input x is exact at exact + 2^i - 1, its in-layer output (and so acts and the next x) at exact + 2^(i+1) - 1
       gate<<<grid_for(rows * (C / 4), 256), 256, 0, st>>>(p.ia, planes && i > 0 ? p.x[cur] : nullptr, p.lensS, win, exact + (2 << i) - 1,
                                                            exact + (1 << i) - 1, B, Ls, C, (float*)p.acts, (__half*)p.acts, status);
       FS2_LAUNCH_CHECK();
       if (i < kLayers - 1) {
-        if ((rc = gemm(m, f.res[i], p.acts, B, Ls, p.lensS, 1, p.x[cur], p.x[cur ^ 1], p.xp, st))) return rc;
+        if ((rc = vweight_gemm(m->math_mode, f.res[i], p.acts, B, Ls, ACT_NONE, p.lensS, p.x[cur ^ 1], st, p.x[cur], 1, p.xp))) return rc;
         cur ^= 1;
       }
-      if ((rc = gemm(m, f.skip[i], p.acts, B, Ls, p.lensS, 1, i ? p.skip[sk] : nullptr, p.skip[sk ^ 1], nullptr, st))) return rc;
+      if ((rc = vweight_gemm(m->math_mode, f.skip[i], p.acts, B, Ls, ACT_NONE, p.lensS, p.skip[sk ^ 1], st, i ? p.skip[sk] : nullptr))) return rc;
       sk ^= 1;
     }
     float* dst = k == 0 && !window ? audio : p.state;
@@ -607,7 +575,7 @@ int fs2_waveglow_load(fs2_waveglow_net* m, const float* const* t, int n, void* s
   cudaStream_t st = (cudaStream_t)stream;
   const int C = m->C;
   // GEMM weights in the order they are carved and packed: (weight, source tensor index, N row offset in it)
-  struct Job { WWeight* w; int src, bsrc, bsrc2, row0; };
+  struct Job { VWeight* w; int src, bsrc, bsrc2, row0; };
   Job jobs[1 + kFlows * (4 * kLayers - 1)];
   int nj = 0;
   m->up.N = kUpN; m->up.K = kUpK;
@@ -629,29 +597,20 @@ int fs2_waveglow_load(fs2_waveglow_net* m, const float* const* t, int n, void* s
       jobs[nj++] = {&f.skip[i], rs_w, rs_w + 1, -1, i < kLayers - 1 ? C : 0};
     }
   }
-  for (int pass = 0; pass < 2; ++pass) {       // pass 0 sizes the arena, pass 1 carves it
-    Bump b(pass ? m->arena : nullptr, pass ? (size_t)-1 : 0);
-    for (int j = 0; j < nj; ++j) {
-      WWeight* w = jobs[j].w;
-      const size_t e = (size_t)w->taps * w->N * w->K;
-      w->w = b.floats(e); w->hi = (__half*)b.bytes(e * 2); w->lo = (__half*)b.bytes(e * 2); w->sc = b.floats(2);
-      w->bias = jobs[j].bsrc >= 0 ? b.floats(w->N) : nullptr;
-    }
+  m->loaded = false;
+  int rc = arena_carve(&m->arena, st, [&](Bump& b) {
+    for (int j = 0; j < nj; ++j) vweight_carve(b, *jobs[j].w, jobs[j].bsrc >= 0);
     for (int k = 0; k < kFlows; ++k) {
       WFlow& f = m->flows[k];
       const int c = flow_channels(k), h = c / 2;
       f.start_w = b.floats((size_t)C * h); f.start_b = b.floats(C);
       f.end_w = b.floats((size_t)c * C); f.end_b = b.floats(c); f.winv = b.floats((size_t)c * c);
     }
-    if (pass == 0) {
-      if (m->arena) { FS2_CUDA_CHECK(cudaStreamSynchronize(st)); FS2_CUDA_CHECK(cudaFree(m->arena)); m->arena = nullptr; }
-      m->loaded = false;
-      FS2_CUDA_CHECK(cudaMalloc(&m->arena, b.off + 256));
-    }
-  }
+  });
+  if (rc) return rc;
   for (int j = 0; j < nj; ++j) {
     const Job& q = jobs[j];
-    WWeight* w = q.w;
+    VWeight* w = q.w;
     const long e = (long)w->taps * w->N * w->K;
     if (j == 0) {
       wg_pack_up_kernel<<<grid_for(e, 256), 256, 0, st>>>(t[0], t[1], w->w, w->bias);
@@ -670,8 +629,7 @@ int fs2_waveglow_load(fs2_waveglow_net* m, const float* const* t, int n, void* s
         FS2_CUDA_CHECK(cudaMemcpyAsync(w->bias, t[q.bsrc] + q.row0, w->N * sizeof(float), cudaMemcpyDeviceToDevice, st));
       }
     }
-    int rc = weight_scale(w->w, e, w->sc, w->sc + 1, st); if (rc) return rc;
-    rc = split_f16(w->w, w->hi, w->lo, e, w->sc, st); if (rc) return rc;
+    if ((rc = vweight_planes(*w, st))) return rc;
   }
   for (int k = 0; k < kFlows; ++k) {
     WFlow& f = m->flows[k];

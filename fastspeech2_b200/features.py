@@ -21,6 +21,7 @@ import ctypes as C
 import torch
 
 from . import _lib
+from ._kernel_module import Handles, check_status, query_bytes, workspace
 from .vocoder import STFT, mel_filterbank
 
 
@@ -40,7 +41,7 @@ class FeatureExtractor(torch.nn.Module):
         self.stft = STFT(self.n_fft, self.hop_length, self.win_length, math_mode=math_mode)   # the windowed Fourier basis
         self.register_buffer("mel_basis", torch.from_numpy(mel_filterbank(self.sample_rate, self.n_fft, self.n_mels, self.fmin, fmax)))
         self._sizer = None          # an fs2_features* that is never loaded: answers workspace queries without a device
-        self._handles = {}          # device index -> (fs2_features*, data pointers the weights were loaded from)
+        self._handles = Handles("fs2_features_destroy")   # keyed by the data pointers the weights were loaded from
         self._ws = {}               # device index -> workspace tensor
 
     @classmethod
@@ -52,11 +53,11 @@ class FeatureExtractor(torch.nn.Module):
         return cls(a["sample_rate"], a["n_fft"], a["hop_length"], a["win_length"], n_mels, a["fmin"], a["fmax"], math_mode=math_mode)
 
     def __del__(self):
+        if getattr(self, "_handles", None) is not None:
+            self._handles.destroy_all()
         lib = _lib._lib
-        hs = [h for h, _ in getattr(self, "_handles", {}).values()] + [getattr(self, "_sizer", None)]
-        for h in hs:
-            if lib is not None and h:
-                lib.fs2_features_destroy(h)
+        if lib is not None and getattr(self, "_sizer", None):
+            lib.fs2_features_destroy(self._sizer)
 
     def _config(self) -> _lib.FeaturesConfig:
         return _lib.FeaturesConfig(self.sample_rate, self.n_fft, self.hop_length, self.win_length, self.n_mels,
@@ -72,31 +73,17 @@ class FeatureExtractor(torch.nn.Module):
         """Bytes of device workspace a call on [B, n_max] samples needs (either entry)."""
         if self._sizer is None:
             self._sizer = self._create()
-        n = C.c_size_t()
-        _lib.check(_lib.load().fs2_features_workspace_bytes(self._sizer, int(B), int(n_max), C.byref(n)),
-                   "fs2_features_workspace_bytes")
-        return n.value
+        return query_bytes("fs2_features_workspace_bytes", self._sizer, int(B), int(n_max))
 
     def _handle(self, device: torch.device):
-        srcs = (self.stft.forward_basis, self.mel_basis)
-        key = tuple(t.data_ptr() for t in srcs)
-        ent = self._handles.get(device.index)
-        if ent is not None and ent[1] == key:
-            return ent[0]
-        h = ent[0] if ent is not None else self._create()
-        w = [t.to(device=device, dtype=torch.float32).contiguous() for t in srcs]
-        with torch.cuda.device(device):
-            _lib.check(_lib.load().fs2_features_load(h, _lib.ptr(w[0]), _lib.ptr(w[1]), _lib.stream_ptr(device)), "fs2_features_load")
-        self._handles[device.index] = (h, key)
-        return h
+        return self._handles.get(device, tuple(t.data_ptr() for t in (self.stft.forward_basis, self.mel_basis)), self._create, self._load)
+
+    def _load(self, h, device: torch.device) -> None:
+        w = [t.to(device=device, dtype=torch.float32).contiguous() for t in (self.stft.forward_basis, self.mel_basis)]
+        _lib.check(_lib.load().fs2_features_load(h, _lib.ptr(w[0]), _lib.ptr(w[1]), _lib.stream_ptr(device)), "fs2_features_load")
 
     def _workspace(self, B: int, n_max: int, device: torch.device) -> torch.Tensor:
-        n = self.workspace_bytes(B, n_max)
-        ws = self._ws.get(device.index)
-        if ws is None or ws.numel() < n:
-            ws = torch.empty(n, dtype=torch.uint8, device=device)
-            self._ws[device.index] = ws
-        return ws
+        return workspace(self._ws, device, self.workspace_bytes(B, n_max))
 
     def _inputs(self, wavs: torch.Tensor, lens: torch.Tensor):
         if not torch.is_tensor(wavs) or wavs.dim() != 2 or wavs.shape[0] == 0:
@@ -115,12 +102,10 @@ class FeatureExtractor(torch.nn.Module):
         return wavs.contiguous(), lens.to(device=wavs.device, dtype=torch.int64).contiguous(), B, n_max
 
     def _check_status(self, status: torch.Tensor) -> None:
-        s = int(status.item())                                                   # the call's one host read
-        if s & _lib.FS2_FEAT_BAD_LENGTH:
-            raise ValueError(f"every lens[b] must lie in (n_fft/2, Nmax] = ({self.n_fft // 2}, Nmax] (reflect padding at the "
-                             f"utterance's edges)")
-        if s & _lib.FS2_FEAT_RANGE:
-            raise ValueError("samples must lie in [-1, 1] (the reference asserts it before its STFT)")
+        check_status(status, [
+            (_lib.FS2_FEAT_BAD_LENGTH, f"every lens[b] must lie in (n_fft/2, Nmax] = ({self.n_fft // 2}, Nmax] (reflect padding at "
+                                       f"the utterance's edges)"),
+            (_lib.FS2_FEAT_RANGE, "samples must lie in [-1, 1] (the reference asserts it before its STFT)")])
 
     def _call(self, entry: str, wavs, lens, outs):
         dev = wavs.device

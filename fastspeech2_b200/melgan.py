@@ -18,30 +18,12 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from ._kernel_module import WindowedVocoder, _WNConv, normalise_checkpoint
 
 HOP = 256
 N_MELS = 80
 MAX_WAV_VALUE = 32768.0
 _STAGES = ((512, 256, 8), (256, 128, 8), (128, 64, 2), (64, 32, 2))    # ConvTranspose1d (Cin, Cout, stride), k = 2 * stride
-
-
-class _WNConv(nn.Module):
-    """The parameters of one weight-normalised convolution, registered in `torch.nn.utils.weight_norm`'s order (bias,
-    weight_g, weight_v).  weight = weight_g * weight_v / |weight_v|, the norm taken per index of dim 0: output channels of
-    a Conv1d [Cout, Cin, k], *input* channels of a ConvTranspose1d [Cin, Cout, k]."""
-
-    def __init__(self, cin: int, cout: int, k: int, transposed: bool = False):
-        super().__init__()
-        proto = nn.ConvTranspose1d(cin, cout, k) if transposed else nn.Conv1d(cin, cout, k)   # torch's default init
-        v = proto.weight.detach()
-        self.transposed = transposed
-        self.bias = nn.Parameter(proto.bias.detach().clone())
-        self.weight_g = nn.Parameter(torch.norm_except_dim(v, 2, 0).clone())
-        self.weight_v = nn.Parameter(v.clone())
-
-    def folded(self) -> torch.Tensor:
-        """fp32 weight, computed on the CPU exactly as torch's weight_norm computes it there (`torch._weight_norm`)."""
-        return torch._weight_norm(self.weight_v.detach().float().cpu(), self.weight_g.detach().float().cpu(), 0)
 
 
 class _ResStack(nn.Module):
@@ -61,7 +43,7 @@ def _generator() -> nn.Sequential:
     return nn.Sequential(*mods)
 
 
-class MelGANVocoder(nn.Module):
+class MelGANVocoder(WindowedVocoder):
     """seungwonpark/melgan's `Generator(mel_channel=80)` on the H100 kernels.
 
     `forward(mels [B, Lmax, 80], olens [B])` -> (audio [B, Lmax * 256] fp32, alens = olens * 256).  Utterance b is the
@@ -71,6 +53,8 @@ class MelGANVocoder(nn.Module):
     is the hub object's method.  math_mode: "3xf16" (default, fp32-class), "f16", "tf32" or "fp32" for the GEMMs.  One
     host read per call (the device-side length and range checks)."""
 
+    _DESTROY, _WORKSPACE_BYTES, _WINDOW_BYTES = "fs2_melgan_destroy", "fs2_melgan_workspace_bytes", "fs2_melgan_window_workspace_bytes"
+
     def __init__(self, math_mode: str = "3xf16"):
         super().__init__()
         if math_mode not in _lib.MATH_MODES:
@@ -79,16 +63,6 @@ class MelGANVocoder(nn.Module):
         self.mel_channel = N_MELS
         self.generator = _generator()
         self._layers = [m for m in self.modules() if isinstance(m, _WNConv)]      # state_dict order, 42 convolutions
-        self._handles = {}       # device index -> (fs2_melgan_gen*, parameter fingerprint it was loaded from)
-        self._ws = {}            # device index -> workspace tensor
-        self._wws = {}           # device index -> window workspace tensor (fs2_melgan_window)
-        self._epoch = 0
-
-    def __del__(self):
-        lib = _lib._lib
-        for h, _ in getattr(self, "_handles", {}).values():
-            if lib is not None and h:
-                lib.fs2_melgan_destroy(h)
 
     # ---- checkpoints ----------------------------------------------------------------------------------------------
     @classmethod
@@ -105,40 +79,8 @@ class MelGANVocoder(nn.Module):
         if "model_g" in sd:
             sd = sd["model_g"]
         voc = cls(math_mode=math_mode)
-        voc.load_state_dict(voc._normalise(sd))
+        voc.load_state_dict(normalise_checkpoint(voc, sd))
         return voc
-
-    def _normalise(self, sd) -> dict:
-        """Checkpoint dict -> this module's weight_g / weight_v state dict, validated key by key."""
-        sd = dict(sd)
-        prefixes = {name: m for name, m in self.named_modules() if isinstance(m, _WNConv)}
-        out = {}
-        for p, m in prefixes.items():
-            if f"{p}.weight" in sd and (f"{p}.weight_g" in sd or f"{p}.weight_v" in sd):
-                raise ValueError(f"unexpected key {p}.weight alongside {p}.weight_g / weight_v")
-            wanted = [f"{p}.bias"] + ([f"{p}.weight"] if f"{p}.weight" in sd else [f"{p}.weight_g", f"{p}.weight_v"])
-            for k in wanted:
-                if k not in sd:
-                    raise ValueError(f"missing key {k}")
-            t = {k: sd.pop(k) for k in wanted}
-            shapes = {f"{p}.bias": m.bias.shape, f"{p}.weight": m.weight_v.shape, f"{p}.weight_g": m.weight_g.shape,
-                      f"{p}.weight_v": m.weight_v.shape}
-            for k, v in t.items():
-                if not torch.is_tensor(v) or tuple(v.shape) != tuple(shapes[k]):
-                    got = tuple(v.shape) if torch.is_tensor(v) else type(v).__name__
-                    raise ValueError(f"key {k} has shape {got}, expected {tuple(shapes[k])}")
-            out[f"{p}.bias"] = t[f"{p}.bias"].float()
-            if f"{p}.weight" in t:
-                w = t[f"{p}.weight"].detach().float().cpu().contiguous()
-                _, norms = torch._weight_norm_interface(w, torch.ones_like(m.weight_g, device="cpu"), 0)
-                out[f"{p}.weight_g"] = norms.reshape(m.weight_g.shape)
-                out[f"{p}.weight_v"] = w
-            else:
-                out[f"{p}.weight_g"] = t[f"{p}.weight_g"].float()
-                out[f"{p}.weight_v"] = t[f"{p}.weight_v"].float()
-        if sd:
-            raise ValueError(f"unexpected key {sorted(sd)[0]}")
-        return out
 
     def eval(self, inference: bool = False):
         """The hub object's signature.  inference=True removes weight norm there; here the folded weights are what the
@@ -146,44 +88,18 @@ class MelGANVocoder(nn.Module):
         super().eval()
         return self
 
-    def invalidate(self) -> None:
-        """Force a weight reload on the next call (after in-place writes through `.data`, which torch does not version)."""
-        self._epoch += 1
-
     # ---- device state ---------------------------------------------------------------------------------------------
-    def _fingerprint(self):
-        return (self._epoch,) + tuple((p.data_ptr(), p._version) for p in self.parameters())
+    def _create(self):
+        h = C.c_void_p()
+        _lib.check(_lib.load().fs2_melgan_create(C.byref(h), _lib.MATH_MODES[self.math_mode]), "fs2_melgan_create")
+        return h.value
 
-    def _handle(self, device: torch.device):
-        lib = _lib.load()
-        key = self._fingerprint()
-        ent = self._handles.get(device.index)
-        if ent is not None and ent[1] == key:
-            return ent[0]
-        with torch.cuda.device(device):
-            if ent is None:
-                h = C.c_void_p()
-                _lib.check(lib.fs2_melgan_create(C.byref(h), _lib.MATH_MODES[self.math_mode]), "fs2_melgan_create")
-                h = h.value
-            else:
-                h = ent[0]
-            ws = [m.folded().to(device).contiguous() for m in self._layers]
-            bs = [m.bias.detach().float().to(device).contiguous() for m in self._layers]
-            wp = (C.c_void_p * len(ws))(*[t.data_ptr() for t in ws])
-            bp = (C.c_void_p * len(bs))(*[t.data_ptr() for t in bs])
-            _lib.check(lib.fs2_melgan_load(h, wp, bp, _lib.stream_ptr(device)), "fs2_melgan_load")
-        self._handles[device.index] = (h, key)
-        return h
-
-    def _workspace(self, h, B: int, L: int, device: torch.device) -> torch.Tensor:
-        n = C.c_size_t()
-        _lib.check(_lib.load().fs2_melgan_workspace_bytes(h, B, L, C.byref(n)), "fs2_melgan_workspace_bytes")
-        ws = self._ws.get(device.index)
-        if ws is None or ws.numel() < n.value:
-            self._ws.pop(device.index, None)
-            ws = torch.empty(n.value, dtype=torch.uint8, device=device)
-            self._ws[device.index] = ws
-        return ws
+    def _load(self, h, device: torch.device) -> None:
+        ws = [m.folded().to(device).contiguous() for m in self._layers]
+        bs = [m.bias.detach().float().to(device).contiguous() for m in self._layers]
+        wp = (C.c_void_p * len(ws))(*[t.data_ptr() for t in ws])
+        bp = (C.c_void_p * len(bs))(*[t.data_ptr() for t in bs])
+        _lib.check(_lib.load().fs2_melgan_load(h, wp, bp, _lib.stream_ptr(device)), "fs2_melgan_load")
 
     def _inputs(self, mels, olens, check_size=None):
         if not torch.is_tensor(mels) or mels.dim() != 3 or mels.shape[2] != N_MELS or mels.shape[0] == 0 or mels.shape[1] == 0:
@@ -208,53 +124,9 @@ class MelGANVocoder(nn.Module):
             raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 sample rows, B * (Lmax + 10) * {HOP} = {rows} "
                              f"(B={B}, Lmax={L}); split the batch or use another math mode")
 
-    def _window_workspace(self, h, B: int, n_frames: int, device: torch.device) -> torch.Tensor:
-        n = C.c_size_t()
-        _lib.check(_lib.load().fs2_melgan_window_workspace_bytes(h, B, n_frames, C.byref(n)), "fs2_melgan_window_workspace_bytes")
-        ws = self._wws.get(device.index)
-        if ws is None or ws.numel() < n.value:
-            self._wws.pop(device.index, None)
-            ws = torch.empty(n.value, dtype=torch.uint8, device=device)
-            self._wws[device.index] = ws
-        return ws
-
-    @staticmethod
-    def _check_frames(n_frames) -> None:
-        if isinstance(n_frames, bool) or not isinstance(n_frames, int) or n_frames < 1:
-            raise ValueError(f"n_frames / chunk_frames must be an int >= 1 (got {n_frames!r})")
-
-    def _check_window_size(self, B: int, n_frames: int) -> None:
-        """fs2_melgan_window's limits on the window's B * (256 * n_frames + 36) rows, raised here as ValueError."""
-        self._check_frames(n_frames)
-        rows = B * (n_frames * HOP + 36)
-        if rows >= 1 << 31:
-            raise ValueError(f"B * (256 * n_frames + 36) must stay below 2^31 window rows (B={B}, n_frames={n_frames})")
-        if self.math_mode == "fp32" and rows > 65535 * 128:
-            raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 window rows, B * (256 * n_frames + 36) = {rows} "
-                             f"(B={B}, n_frames={n_frames}); use fewer frames per window")
-
-    def _starts(self, starts, B: int, device: torch.device) -> torch.Tensor:
-        """starts as an int, a host list or tensor (checked >= 0 here) or a device tensor (checked on the device) -> [B]
-        int64 on `device`."""
-        if isinstance(starts, bool):
-            raise ValueError("starts must be an int, a list or an integer tensor")
-        if isinstance(starts, int):
-            starts = [starts] * B
-        if not torch.is_tensor(starts):
-            try:
-                starts = torch.tensor(starts)
-            except (TypeError, ValueError, RuntimeError):
-                raise ValueError("starts must be an int, a list or an integer tensor") from None
-        if starts.dim() != 1 or starts.shape[0] != B:
-            raise ValueError(f"starts must hold B={B} frame offsets")
-        if starts.dtype.is_floating_point or starts.dtype == torch.bool or starts.is_complex():
-            raise ValueError("starts must be an integer tensor")
-        if not starts.is_cuda:
-            if bool((starts < 0).any()):
-                raise ValueError("every starts[b] must be >= 0")
-        elif starts.device != device:
-            raise ValueError("starts must be on the same device as mels")
-        return starts.to(device=device, dtype=torch.int64).contiguous()
+    def _window_rows(self, B: int, n_frames: int):
+        """fs2_melgan_window's largest buffer: B * (256 * n_frames + 36) rows."""
+        return B * (n_frames * HOP + 36), "B * (256 * n_frames + 36)"
 
     def _window_call(self, h, mels, olens, starts, B: int, L: int, n_frames: int, audio: torch.Tensor, ld: int, status: torch.Tensor,
                      ws: torch.Tensor) -> None:
@@ -263,15 +135,11 @@ class MelGANVocoder(nn.Module):
             _lib.check(_lib.load().fs2_melgan_window(h, _lib.ptr(mels), _lib.ptr(olens), _lib.ptr(starts), B, L, n_frames, audio.data_ptr(), ld,
                                                      _lib.ptr(status), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)), "fs2_melgan_window")
 
-    def _check_status(self, status: torch.Tensor) -> None:
-        s = int(status.item())                                                   # the call's one host read
-        if s & _lib.FS2_MELGAN_BAD_LENGTH:
-            raise ValueError("every olens[b] must lie in [1, Lmax]")
-        if s & _lib.FS2_MELGAN_BAD_START:
-            raise ValueError("every starts[b] must be >= 0")
-        if s & _lib.FS2_MELGAN_RANGE:
-            raise ValueError(f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
-                             f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'")
+    def _status_table(self):
+        return [(_lib.FS2_MELGAN_BAD_LENGTH, "every olens[b] must lie in [1, Lmax]"),
+                (_lib.FS2_MELGAN_BAD_START, "every starts[b] must be >= 0"),
+                (_lib.FS2_MELGAN_RANGE, f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
+                                        f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'")]
 
     # ---- synthesis ------------------------------------------------------------------------------------------------
     def forward(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int | None = None):
@@ -281,7 +149,8 @@ class MelGANVocoder(nn.Module):
         workspace of one window (fs2_melgan_window): in fp32 mode this vocodes batches the whole call refuses.  Still one
         host read per call: the windows' status words are ORed on the device."""
         if chunk_frames is not None:
-            return self._chunked(mels, olens, chunk_frames)
+            mels, olens, B, L = self._window_inputs(mels, olens, chunk_frames)
+            return self._chunked(self._window_call, mels, olens, B, L, chunk_frames)
         mels, olens, B, L = self._inputs(mels, olens)
         dev = mels.device
         h = self._handle(dev)
@@ -310,40 +179,14 @@ class MelGANVocoder(nn.Module):
         or a device tensor.  Only mel frames [starts[b] - 6, starts[b] + n_frames + 6) below olens[b] are read; the
         workspace depends on B and n_frames only.  One host read per call."""
         mels, olens, B, L = self._window_inputs(mels, olens, n_frames)
-        dev = mels.device
-        starts = self._starts(starts, B, dev)
-        h = self._handle(dev)
-        ws = self._window_workspace(h, B, n_frames, dev)
-        audio = torch.empty((B, n_frames * HOP), dtype=torch.float32, device=dev)
-        status = torch.empty((1,), dtype=torch.int32, device=dev)
-        self._window_call(h, mels, olens, starts, B, L, n_frames, audio, n_frames * HOP, status, ws)
-        self._check_status(status)
-        return audio, (olens - starts).clamp(0, n_frames) * HOP
+        return self._window(self._window_call, mels, olens, starts, B, L, n_frames)
 
     def stream(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int = 32):
         """Lockstep windows: yields (audio, alens) of `window(mels, olens, k * chunk_frames, chunk_frames)` for k = 0 ..
         ceil(Lmax / chunk_frames) - 1, the last one cut at Lmax, so that the chunks concatenated along time are
         `forward(mels, olens)`.  Utterances that have ended give rows of 0 (alens 0)."""
         self._check_frames(chunk_frames)
-        L = mels.shape[1]
-        for c0 in range(0, L, chunk_frames):
-            yield self.window(mels, olens, c0, min(chunk_frames, L - c0))
-
-    def _chunked(self, mels, olens, k: int):
-        mels, olens, B, L = self._window_inputs(mels, olens, k)
-        dev = mels.device
-        h = self._handle(dev)
-        ws = self._window_workspace(h, B, min(k, L), dev)
-        audio = torch.empty((B, L * HOP), dtype=torch.float32, device=dev)
-        c0s = list(range(0, L, k))
-        starts = torch.tensor(c0s, dtype=torch.int64).repeat_interleave(B).reshape(len(c0s), B).to(dev)
-        status = torch.empty((len(c0s),), dtype=torch.int32, device=dev)
-        for i, c0 in enumerate(c0s):
-            n = min(k, L - c0)
-            self._window_call(h, mels, olens, starts[i], B, L, n, audio[:, c0 * HOP:], L * HOP, status[i: i + 1], ws)
-        bits = torch.tensor([_lib.FS2_MELGAN_BAD_LENGTH, _lib.FS2_MELGAN_RANGE, _lib.FS2_MELGAN_BAD_START], dtype=torch.int32, device=dev)
-        self._check_status(((status[:, None] & bits) != 0).any(0).int().mul(bits).sum().reshape(1))
-        return audio, olens * HOP
+        yield from self._stream(mels, chunk_frames, lambda c0, n: self.window(mels, olens, c0, n))
 
     @staticmethod
     def quantize(audio: torch.Tensor) -> torch.Tensor:

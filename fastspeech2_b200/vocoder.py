@@ -18,6 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._kernel_module import Handles, check_status, query_bytes, workspace
 
 
 def _hann(win_length: int, n_fft: int) -> np.ndarray:
@@ -200,7 +201,7 @@ class GriffinLimVocoder(torch.nn.Module):
         self.register_buffer("mel_basis", torch.from_numpy(basis))                                  # [n_mels, cutoff]
         self.register_buffer("mel_inverse", torch.from_numpy(mel_inverse(basis)))                   # [cutoff, n_mels]
         self.register_buffer("_window_sq", torch.from_numpy(_hann(self.win_length, self.n_fft) ** 2).float(), persistent=False)
-        self._handles = {}       # device index -> (fs2_vocoder*, data pointers the bases were loaded from)
+        self._handles = Handles("fs2_vocoder_destroy")   # keyed by the data pointers the bases were loaded from
         self._ws = {}            # device index -> workspace tensor
 
     @classmethod
@@ -212,41 +213,27 @@ class GriffinLimVocoder(torch.nn.Module):
         return cls(a["sample_rate"], a["n_fft"], a["hop_length"], a["win_length"], n_mels, a["fmin"], a["fmax"], math_mode=math_mode)
 
     def __del__(self):
-        lib = _lib._lib
-        for h, _ in getattr(self, "_handles", {}).values():
-            if lib is not None and h:
-                lib.fs2_vocoder_destroy(h)
+        if getattr(self, "_handles", None) is not None:
+            self._handles.destroy_all()
 
     def _bases(self):
         return (self.stft.forward_basis, self.stft.inverse_basis, self.mel_inverse, self._window_sq)
 
     def _handle(self, device: torch.device):
-        lib = _lib.load()
+        return self._handles.get(device, tuple(t.data_ptr() for t in self._bases()), self._create, self._load)
+
+    def _create(self):
+        h = C.c_void_p()
+        cfg = _lib.VocoderConfig(self.n_fft, self.hop_length, self.win_length, self.n_mels, _lib.MATH_MODES[self.math_mode])
+        _lib.check(_lib.load().fs2_vocoder_create(C.byref(h), C.byref(cfg)), "fs2_vocoder_create")
+        return h.value
+
+    def _load(self, h, device: torch.device) -> None:
         bases = [t.to(device=device, dtype=torch.float32).contiguous() for t in self._bases()]
-        key = tuple(t.data_ptr() for t in self._bases())
-        ent = self._handles.get(device.index)
-        if ent is not None and ent[1] == key:
-            return ent[0]
-        with torch.cuda.device(device):
-            if ent is None:
-                h = C.c_void_p()
-                cfg = _lib.VocoderConfig(self.n_fft, self.hop_length, self.win_length, self.n_mels, _lib.MATH_MODES[self.math_mode])
-                _lib.check(lib.fs2_vocoder_create(C.byref(h), C.byref(cfg)), "fs2_vocoder_create")
-                h = h.value
-            else:
-                h = ent[0]
-            _lib.check(lib.fs2_vocoder_load(h, *[_lib.ptr(t) for t in bases], _lib.stream_ptr(device)), "fs2_vocoder_load")
-        self._handles[device.index] = (h, key)
-        return h
+        _lib.check(_lib.load().fs2_vocoder_load(h, *[_lib.ptr(t) for t in bases], _lib.stream_ptr(device)), "fs2_vocoder_load")
 
     def _workspace(self, h, B: int, L: int, device: torch.device) -> torch.Tensor:
-        n = C.c_size_t()
-        _lib.check(_lib.load().fs2_vocoder_workspace_bytes(h, B, L, C.byref(n)), "fs2_vocoder_workspace_bytes")
-        ws = self._ws.get(device.index)
-        if ws is None or ws.numel() < n.value:
-            ws = torch.empty(n.value, dtype=torch.uint8, device=device)
-            self._ws[device.index] = ws
-        return ws
+        return workspace(self._ws, device, query_bytes("fs2_vocoder_workspace_bytes", h, B, L))
 
     def _inputs(self, mels: torch.Tensor, olens: torch.Tensor, check_device: bool = True):
         if not torch.is_tensor(mels) or mels.dim() != 3 or mels.shape[2] != self.n_mels:
@@ -268,13 +255,11 @@ class GriffinLimVocoder(torch.nn.Module):
             raise ValueError("mels and olens must be CUDA tensors (the H100 path has no CPU fallback)")
 
     def _check_status(self, status: torch.Tensor) -> None:
-        s = int(status.item())                                                   # the call's one host read
-        if s & _lib.FS2_VOC_BAD_LENGTH:
-            raise ValueError(f"every olens[b] must lie in [1, Lmax] with (olens[b]-1)*hop > n_fft/2 = {self.n_fft // 2} "
-                             f"(reflect padding at the utterance's edges)")
-        if s & _lib.FS2_VOC_RANGE:
-            raise ValueError(f"magnitudes exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
-                             f"(|exp(mel)|, |M| or |signal| above {65504 / 16:g}); use math_mode='fp32' or 'tf32'")
+        check_status(status, [
+            (_lib.FS2_VOC_BAD_LENGTH, f"every olens[b] must lie in [1, Lmax] with (olens[b]-1)*hop > n_fft/2 = {self.n_fft // 2} "
+                                      f"(reflect padding at the utterance's edges)"),
+            (_lib.FS2_VOC_RANGE, f"magnitudes exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
+                                 f"(|exp(mel)|, |M| or |signal| above {65504 / 16:g}); use math_mode='fp32' or 'tf32'")])
 
     def mel_to_magnitude(self, mels: torch.Tensor, olens: torch.Tensor) -> torch.Tensor:
         """[B, Lmax, n_mels] log-mels -> linear magnitudes [B, n_fft/2+1, Lmax] (0 past olens[b]): the input `griffin_lim`

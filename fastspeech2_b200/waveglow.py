@@ -22,7 +22,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .melgan import _WNConv
+from ._kernel_module import WindowedVocoder, _WNConv, normalise_checkpoint
 
 HOP = 256
 N_MELS = 80
@@ -69,7 +69,7 @@ class _WN(nn.Module):
         self.end = _Conv((2 * n_half, c, 1), 2 * n_half)           # zero-initialised, as in the published model
 
 
-class WaveGlowVocoder(nn.Module):
+class WaveGlowVocoder(WindowedVocoder):
     """DeepLearningExamples' `WaveGlow` (n_mel_channels 80, n_flows 12, n_group 8, n_early_every 4, n_early_size 2, WN 8
     layers of kernel 3, n_channels C) on the H100 kernels.
 
@@ -92,6 +92,9 @@ class WaveGlowVocoder(nn.Module):
     lockstep windows whose concatenation is `forward`, and `forward(..., chunk_frames=k)` computes the whole call's bits
     window by window.  A window's workspace depends on B and n_frames only."""
 
+    _DESTROY = "fs2_waveglow_destroy"
+    _WORKSPACE_BYTES, _WINDOW_BYTES = "fs2_waveglow_workspace_bytes", "fs2_waveglow_window_workspace_bytes"
+
     def __init__(self, n_channels: int = 512, math_mode: str = "3xf16"):
         super().__init__()
         if math_mode not in _lib.MATH_MODES:
@@ -109,16 +112,6 @@ class WaveGlowVocoder(nn.Module):
             self.upsample.bias.uniform_(-bound, bound)
         self.WN = nn.ModuleList([_WN(flow_channels(k) // 2, n_channels) for k in range(N_FLOWS)])
         self.convinv = nn.ModuleList([_Inv(flow_channels(k)) for k in range(N_FLOWS)])
-        self._handles = {}       # device index -> (fs2_waveglow_net*, parameter fingerprint it was loaded from)
-        self._ws = {}            # device index -> workspace tensor
-        self._wws = {}           # device index -> window workspace tensor
-        self._epoch = 0
-
-    def __del__(self):
-        lib = _lib._lib
-        for h, _ in getattr(self, "_handles", {}).values():
-            if lib is not None and h:
-                lib.fs2_waveglow_destroy(h)
 
     # ---- checkpoints ----------------------------------------------------------------------------------------------
     @classmethod
@@ -141,49 +134,8 @@ class WaveGlowVocoder(nn.Module):
         if not torch.is_tensor(b) or b.dim() != 1:
             raise ValueError("missing key WN.0.start.bias (n_channels is read from it)")
         voc = cls(n_channels=int(b.shape[0]), math_mode=math_mode)
-        voc.load_state_dict(voc._normalise(sd))
+        voc.load_state_dict(normalise_checkpoint(voc, sd))
         return voc
-
-    def _normalise(self, sd) -> dict:
-        """Checkpoint dict -> this module's state dict, validated key by key."""
-        sd = dict(sd)
-        out = {}
-        wn = {name: m for name, m in self.named_modules() if isinstance(m, _WNConv)}
-        for p, m in wn.items():
-            if f"{p}.weight" in sd and (f"{p}.weight_g" in sd or f"{p}.weight_v" in sd):
-                raise ValueError(f"unexpected key {p}.weight alongside {p}.weight_g / weight_v")
-            wanted = [f"{p}.bias"] + ([f"{p}.weight"] if f"{p}.weight" in sd else [f"{p}.weight_g", f"{p}.weight_v"])
-            shapes = {f"{p}.bias": m.bias.shape, f"{p}.weight": m.weight_v.shape, f"{p}.weight_g": m.weight_g.shape,
-                      f"{p}.weight_v": m.weight_v.shape}
-            t = self._take(sd, wanted, shapes)
-            out[f"{p}.bias"] = t[f"{p}.bias"]
-            if f"{p}.weight" in t:
-                w = t[f"{p}.weight"].contiguous()
-                _, norms = torch._weight_norm_interface(w, torch.ones_like(m.weight_g, device="cpu"), 0)
-                out[f"{p}.weight_g"] = norms.reshape(m.weight_g.shape)
-                out[f"{p}.weight_v"] = w
-            else:
-                out[f"{p}.weight_g"] = t[f"{p}.weight_g"]
-                out[f"{p}.weight_v"] = t[f"{p}.weight_v"]
-        own = self.state_dict()
-        plain = [k for k in own if k not in out]
-        out.update(self._take(sd, plain, {k: own[k].shape for k in plain}))
-        if sd:
-            raise ValueError(f"unexpected key {sorted(sd)[0]}")
-        return out
-
-    @staticmethod
-    def _take(sd: dict, keys, shapes) -> dict:
-        t = {}
-        for k in keys:
-            if k not in sd:
-                raise ValueError(f"missing key {k}")
-            v = sd.pop(k)
-            if not torch.is_tensor(v) or tuple(v.shape) != tuple(shapes[k]):
-                got = tuple(v.shape) if torch.is_tensor(v) else type(v).__name__
-                raise ValueError(f"key {k} has shape {got}, expected {tuple(shapes[k])}")
-            t[k] = v.detach().float().cpu()
-        return t
 
     @staticmethod
     def remove_weightnorm(model):
@@ -191,14 +143,7 @@ class WaveGlowVocoder(nn.Module):
         weights either way, so the parameters keep their weight_g / weight_v form and the audio is the same."""
         return model
 
-    def invalidate(self) -> None:
-        """Force a weight reload on the next call (after in-place writes through `.data`, which torch does not version)."""
-        self._epoch += 1
-
     # ---- device state ---------------------------------------------------------------------------------------------
-    def _fingerprint(self):
-        return (self._epoch,) + tuple((p.data_ptr(), p._version) for p in self.parameters())
-
     def _tensors(self):
         """The 638 fp32 CPU tensors of fs2_waveglow_load, in its order (weight norm folded, W_inverse in float64)."""
         plain = lambda t: t.detach().float().cpu().contiguous()
@@ -213,35 +158,16 @@ class WaveGlowVocoder(nn.Module):
             ts += [plain(wn.end.weight), plain(wn.end.bias), torch.linalg.inv(W).float().contiguous()]
         return ts
 
-    def _handle(self, device: torch.device):
-        lib = _lib.load()
-        key = self._fingerprint()
-        ent = self._handles.get(device.index)
-        if ent is not None and ent[1] == key:
-            return ent[0]
-        with torch.cuda.device(device):
-            if ent is None:
-                h = C.c_void_p()
-                _lib.check(lib.fs2_waveglow_create(C.byref(h), _lib.MATH_MODES[self.math_mode], self.n_channels), "fs2_waveglow_create")
-                h = h.value
-            else:
-                h = ent[0]
-            ts = [t.to(device) for t in self._tensors()]
-            tp = (C.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
-            _lib.check(lib.fs2_waveglow_load(h, tp, len(ts), _lib.stream_ptr(device)), "fs2_waveglow_load")
-            torch.cuda.current_stream(device).synchronize()       # the staging tensors are freed on return
-        self._handles[device.index] = (h, key)
-        return h
+    def _create(self):
+        h = C.c_void_p()
+        _lib.check(_lib.load().fs2_waveglow_create(C.byref(h), _lib.MATH_MODES[self.math_mode], self.n_channels), "fs2_waveglow_create")
+        return h.value
 
-    def _workspace(self, h, B: int, L: int, device: torch.device) -> torch.Tensor:
-        n = C.c_size_t()
-        _lib.check(_lib.load().fs2_waveglow_workspace_bytes(h, B, L, C.byref(n)), "fs2_waveglow_workspace_bytes")
-        ws = self._ws.get(device.index)
-        if ws is None or ws.numel() < n.value:
-            self._ws.pop(device.index, None)
-            ws = torch.empty(n.value, dtype=torch.uint8, device=device)
-            self._ws[device.index] = ws
-        return ws
+    def _load(self, h, device: torch.device) -> None:
+        ts = [t.to(device) for t in self._tensors()]
+        tp = (C.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+        _lib.check(_lib.load().fs2_waveglow_load(h, tp, len(ts), _lib.stream_ptr(device)), "fs2_waveglow_load")
+        torch.cuda.current_stream(device).synchronize()       # the staging tensors are freed on return
 
     def _inputs(self, mels, olens, sigma, seed, z, check_size=None):
         """Validated (mels fp32, olens int64, B, Lmax, sigma, seeds or None, z fp32 or None); every check that needs no
@@ -302,15 +228,11 @@ class WaveGlowVocoder(nn.Module):
             raise ValueError(f"sigma must be a finite number >= 0, got {sigma!r}")
         return float(sigma)
 
-    def _check_status(self, status: torch.Tensor) -> None:
-        s = int(status.item())                                                   # the call's one host read
-        if s & _lib.FS2_WAVEGLOW_BAD_LENGTH:
-            raise ValueError("every olens[b] must lie in [1, Lmax]")
-        if s & _lib.FS2_WAVEGLOW_BAD_START:
-            raise ValueError("every starts[b] must be >= 0")
-        if s & _lib.FS2_WAVEGLOW_RANGE:
-            raise ValueError(f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
-                             f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'")
+    def _status_table(self):
+        return [(_lib.FS2_WAVEGLOW_BAD_LENGTH, "every olens[b] must lie in [1, Lmax]"),
+                (_lib.FS2_WAVEGLOW_BAD_START, "every starts[b] must be >= 0"),
+                (_lib.FS2_WAVEGLOW_RANGE, f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
+                                          f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'")]
 
     # ---- synthesis ------------------------------------------------------------------------------------------------
     @classmethod
@@ -340,7 +262,10 @@ class WaveGlowVocoder(nn.Module):
         draws the same one int64 as the whole call.  Still one host read per call: the windows' status words are ORed on
         the device."""
         if chunk_frames is not None:
-            return self._chunked(mels, olens, chunk_frames, sigma, seed, z)
+            self._check_frames(chunk_frames)
+            seed = self._resolve_seed(seed, z)
+            mels, olens, B, L, sigma, seeds, z = self._window_inputs(mels, olens, chunk_frames, sigma, seed, z)
+            return self._chunked(self._window_call(sigma, seeds, z), mels, olens, B, L, chunk_frames)
         mels, olens, B, L, sigma, seeds, z = self._inputs(mels, olens, sigma, seed, z)
         dev = mels.device
         h = self._handle(dev)
@@ -355,20 +280,9 @@ class WaveGlowVocoder(nn.Module):
         return audio, olens * HOP
 
     # ---- windows (DESIGN.md section 12) ----------------------------------------------------------------------------
-    @staticmethod
-    def _check_frames(n_frames) -> None:
-        if isinstance(n_frames, bool) or not isinstance(n_frames, int) or n_frames < 1:
-            raise ValueError(f"n_frames / chunk_frames must be an int >= 1 (got {n_frames!r})")
-
-    def _check_window_size(self, B: int, n_frames: int) -> None:
-        """fs2_waveglow_window's limits on the window's B * (n_frames + 192) * 32 step rows, raised here as ValueError."""
-        self._check_frames(n_frames)
-        rows = B * (n_frames + 2 * HALO) * STEPS
-        if rows >= 1 << 31:
-            raise ValueError(f"B * (n_frames + {2 * HALO}) * {STEPS} must stay below 2^31 window rows (B={B}, n_frames={n_frames})")
-        if self.math_mode == "fp32" and rows > 65535 * 128:
-            raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 window rows, B * (n_frames + {2 * HALO}) * {STEPS} = {rows} "
-                             f"(B={B}, n_frames={n_frames}); use fewer frames per window")
+    def _window_rows(self, B: int, n_frames: int):
+        """fs2_waveglow_window's buffers: B * (n_frames + 192) * 32 step rows."""
+        return B * (n_frames + 2 * HALO) * STEPS, f"B * (n_frames + {2 * HALO}) * {STEPS}"
 
     def _window_inputs(self, mels, olens, n_frames, sigma, seed, z):
         """_inputs with the window's limits in place of the whole call's (Lmax bounds only z's and mels' layout)."""
@@ -380,47 +294,17 @@ class WaveGlowVocoder(nn.Module):
                 raise ValueError(f"Lmax * {STEPS} must stay below 2^31 steps (Lmax={L})")
         return self._inputs(mels, olens, sigma, seed, z, check)
 
-    def _window_workspace(self, h, B: int, n_frames: int, device: torch.device) -> torch.Tensor:
-        n = C.c_size_t()
-        _lib.check(_lib.load().fs2_waveglow_window_workspace_bytes(h, B, n_frames, C.byref(n)), "fs2_waveglow_window_workspace_bytes")
-        ws = self._wws.get(device.index)
-        if ws is None or ws.numel() < n.value:
-            self._wws.pop(device.index, None)
-            ws = torch.empty(n.value, dtype=torch.uint8, device=device)
-            self._wws[device.index] = ws
-        return ws
-
     @staticmethod
-    def _starts(starts, B: int, device: torch.device) -> torch.Tensor:
-        """starts as an int, a host list or tensor (checked >= 0 here) or a device tensor (checked on the device) -> [B]
-        int64 on `device`."""
-        if isinstance(starts, bool):
-            raise ValueError("starts must be an int, a list or an integer tensor")
-        if isinstance(starts, int):
-            starts = [starts] * B
-        if not torch.is_tensor(starts):
-            try:
-                starts = torch.tensor(starts)
-            except (TypeError, ValueError, RuntimeError):
-                raise ValueError("starts must be an int, a list or an integer tensor") from None
-        if starts.dim() != 1 or starts.shape[0] != B:
-            raise ValueError(f"starts must hold B={B} frame offsets")
-        if starts.dtype.is_floating_point or starts.dtype == torch.bool or starts.is_complex():
-            raise ValueError("starts must be an integer tensor")
-        if not starts.is_cuda:
-            if bool((starts < 0).any()):
-                raise ValueError("every starts[b] must be >= 0")
-        elif starts.device != device:
-            raise ValueError("starts must be on the same device as mels")
-        return starts.to(device=device, dtype=torch.int64).contiguous()
-
-    def _window_call(self, h, mels, olens, starts, B: int, L: int, n_frames: int, sigma: float, seeds, z, audio: torch.Tensor, ld: int,
-                     status: torch.Tensor, ws: torch.Tensor) -> None:
-        dev = mels.device
-        with torch.cuda.device(dev):
-            _lib.check(_lib.load().fs2_waveglow_window(h, _lib.ptr(mels), _lib.ptr(olens), _lib.ptr(starts), B, L, n_frames, sigma,
-                                                       _lib.ptr(seeds), _lib.ptr(z), audio.data_ptr(), ld, _lib.ptr(status), _lib.ptr(ws),
-                                                       ws.numel(), _lib.stream_ptr(dev)), "fs2_waveglow_window")
+    def _window_call(sigma: float, seeds, z):
+        """The window call with this noise (seeds or z): call(h, mels, olens, starts, B, Lmax, n_frames, audio, ld, status, ws)."""
+        def call(h, mels, olens, starts, B: int, L: int, n_frames: int, audio: torch.Tensor, ld: int, status: torch.Tensor,
+                 ws: torch.Tensor) -> None:
+            dev = mels.device
+            with torch.cuda.device(dev):
+                _lib.check(_lib.load().fs2_waveglow_window(h, _lib.ptr(mels), _lib.ptr(olens), _lib.ptr(starts), B, L, n_frames, sigma,
+                                                           _lib.ptr(seeds), _lib.ptr(z), audio.data_ptr(), ld, _lib.ptr(status),
+                                                           _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)), "fs2_waveglow_window")
+        return call
 
     def window(self, mels: torch.Tensor, olens: torch.Tensor, starts, n_frames: int, *, sigma: float = 1.0, seed=None, z=None):
         """One window of the audio (DESIGN.md section 12): -> (audio [B, n_frames * 256] fp32, alens [B] int64 =
@@ -433,15 +317,7 @@ class WaveGlowVocoder(nn.Module):
         if seed is None and z is None:
             raise ValueError("window needs the noise: pass seed (an int or a [B] tensor) or z, as the whole call it continues")
         mels, olens, B, L, sigma, seeds, z = self._window_inputs(mels, olens, n_frames, sigma, seed, z)
-        dev = mels.device
-        starts = self._starts(starts, B, dev)
-        h = self._handle(dev)
-        ws = self._window_workspace(h, B, n_frames, dev)
-        audio = torch.empty((B, n_frames * HOP), dtype=torch.float32, device=dev)
-        status = torch.empty((1,), dtype=torch.int32, device=dev)
-        self._window_call(h, mels, olens, starts, B, L, n_frames, sigma, seeds, z, audio, n_frames * HOP, status, ws)
-        self._check_status(status)
-        return audio, (olens - starts).clamp(0, n_frames) * HOP
+        return self._window(self._window_call(sigma, seeds, z), mels, olens, starts, B, L, n_frames)
 
     @staticmethod
     def _resolve_seed(seed, z):
@@ -459,28 +335,7 @@ class WaveGlowVocoder(nn.Module):
         seed = self._resolve_seed(seed, z)
         if torch.is_tensor(mels) and mels.dim() == 3 and seed is not None:
             seed = self._seeds(seed, mels.shape[0], mels.device)          # validated and moved once
-        L = mels.shape[1]
-        for c0 in range(0, L, chunk_frames):
-            yield self.window(mels, olens, c0, min(chunk_frames, L - c0), sigma=sigma, seed=seed, z=z)
-
-    def _chunked(self, mels, olens, k: int, sigma, seed, z):
-        self._check_frames(k)
-        seed = self._resolve_seed(seed, z)
-        mels, olens, B, L, sigma, seeds, z = self._window_inputs(mels, olens, k, sigma, seed, z)
-        dev = mels.device
-        h = self._handle(dev)
-        ws = self._window_workspace(h, B, min(k, L), dev)
-        audio = torch.empty((B, L * HOP), dtype=torch.float32, device=dev)
-        c0s = list(range(0, L, k))
-        starts = torch.tensor(c0s, dtype=torch.int64).repeat_interleave(B).reshape(len(c0s), B).to(dev)
-        status = torch.empty((len(c0s),), dtype=torch.int32, device=dev)
-        for i, c0 in enumerate(c0s):
-            n = min(k, L - c0)
-            self._window_call(h, mels, olens, starts[i], B, L, n, sigma, seeds, z, audio[:, c0 * HOP:], L * HOP, status[i: i + 1], ws)
-        bits = torch.tensor([_lib.FS2_WAVEGLOW_BAD_LENGTH, _lib.FS2_WAVEGLOW_RANGE, _lib.FS2_WAVEGLOW_BAD_START], dtype=torch.int32,
-                            device=dev)
-        self._check_status(((status[:, None] & bits) != 0).any(0).int().mul(bits).sum().reshape(1))
-        return audio, olens * HOP
+        yield from self._stream(mels, chunk_frames, lambda c0, n: self.window(mels, olens, c0, n, sigma=sigma, seed=seed, z=z))
 
     def infer(self, spect: torch.Tensor, sigma: float = 1.0) -> torch.Tensor:
         """DeepLearningExamples' `infer`: spect [B, 80, T] -> audio [B, T * 256] fp32, fresh noise per call."""

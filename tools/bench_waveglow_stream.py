@@ -49,20 +49,21 @@ class Stream:
     """Preallocated lockstep windows of one batch: starts for every step on the device, one output row block per step."""
 
     def __init__(self, voc, mels, olens, n, seeds):
-        self.voc, self.mels, self.olens, self.n, self.seeds = voc, mels.contiguous(), olens.contiguous(), n, seeds
+        self.mels, self.olens, self.n = mels.contiguous(), olens.contiguous(), n
         B, L = mels.shape[:2]
         self.B, self.L = B, L
         dev = mels.device
         self.h = voc._handle(dev)
         self.ws = voc._window_workspace(self.h, B, n, dev)
+        self.call = voc._window_call(SIGMA, seeds, None)
         self.steps = -(-L // n)
         self.starts = (torch.arange(self.steps, device=dev, dtype=torch.int64) * n)[:, None].expand(self.steps, B).contiguous()
         self.audio = torch.empty(B, self.steps * n * HOP, device=dev)
         self.status = torch.zeros(self.steps, dtype=torch.int32, device=dev)
 
     def window(self, k):
-        self.voc._window_call(self.h, self.mels, self.olens, self.starts[k], self.B, self.L, self.n, SIGMA, self.seeds, None,
-                              self.audio[:, k * self.n * HOP:], self.steps * self.n * HOP, self.status[k: k + 1], self.ws)
+        self.call(self.h, self.mels, self.olens, self.starts[k], self.B, self.L, self.n, self.audio[:, k * self.n * HOP:],
+                  self.steps * self.n * HOP, self.status[k: k + 1], self.ws)
 
     def run(self):
         for k in range(self.steps):
