@@ -10,7 +10,7 @@
 #include <unordered_map>
 #include <vector>
 
-#include "common.cuh"
+#include "vocoder_weights.cuh"
 
 namespace fs2 {
 
@@ -23,17 +23,10 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-struct Dense {           // one Linear / Conv1d in kernel layout
-  const float* w = nullptr;     // [taps][N][K] fp32 (fp32 FMA and tf32 families)
-  const __half* w_hi = nullptr; // fp16 hi / lo planes of (scale * w): f16 reads hi, 3xF16 reads both
-  const __half* w_lo = nullptr;
-  const float* w_inv = nullptr; // device scalar 1 / scale (a power of two chosen per layer at load time)
-  const float* bias = nullptr;  // [N] or nullptr
-  int N = 0, K = 0, taps = 1;
-};
+// every Linear / Conv1d is a VWeight (vocoder_weights.cuh) with a per-layer power-of-two scale chosen at load time
 struct Norm { const float* g = nullptr; const float* b = nullptr; float eps = 1e-5f; };
-struct Block { Dense qkv, out, w1, w2; Norm ln1, ln2; };
-struct Predictor { Dense conv[4]; Norm ln[4]; const float* head_w = nullptr; const float* head_b = nullptr; int layers = 0; };
+struct Block { VWeight qkv, out, w1, w2; Norm ln1, ln2; };
+struct Predictor { VWeight conv[4]; Norm ln[4]; const float* head_w = nullptr; const float* head_b = nullptr; int layers = 0; };
 
 
 // ---- per-kernel-class CUDA-event profiler (bench.py roofline; off by default) -------------
@@ -73,8 +66,8 @@ struct fs2_handle {
   fs2_config cfg;
   int device = 0;
   bool loaded = false;
-  float* arena = nullptr;     // packed weights (owned)
-  size_t arena_floats = 0;
+  void* arena = nullptr;      // packed weights (owned)
+  size_t arena_bytes = 0;
   // encoder side
   const float* emb = nullptr; const float* enc_pe = nullptr; const float* enc_alpha = nullptr;
   std::vector<fs2::Block> enc, dec;
@@ -83,9 +76,9 @@ struct fs2_handle {
   const float* e_tab = nullptr; const float* e_tab_bias = nullptr;
   const float* p_tab = nullptr; const float* p_tab_bias = nullptr;
   // decoder side
-  fs2::Dense dec_in; fs2::Norm dec_in_ln; const float* dec_pe = nullptr; const float* dec_alpha = nullptr;
-  fs2::Dense feat_out;
-  std::vector<fs2::Dense> postnet;
+  fs2::VWeight dec_in; fs2::Norm dec_in_ln; const float* dec_pe = nullptr; const float* dec_alpha = nullptr;
+  fs2::VWeight feat_out;
+  std::vector<fs2::VWeight> postnet;
 };
 
 namespace fs2 {
@@ -114,8 +107,7 @@ int dense(const TapGemm& g, int math_mode, cudaStream_t st, int cls) {
   const double e_out = (g.out ? 4.0 : 0.0) + ((g.outp || g.vtp) ? (g.outp_lo ? 4.0 : 2.0) : 0.0);
   ProfScope prof_scope(cls, 2.0 * M * g.N * g.K * g.taps,
                e_in * (M * g.K + (double)g.taps * g.N * g.K) + M * g.N * (e_out + (g.resid ? 4.0 : 0.0)), st);
-  if (g.xp) return tap_gemm_planes(g, st);
-  return math_mode == FS2_MATH_TF32 ? tap_gemm_tf32(g, st) : tap_gemm_fp32(g, st);
+  return tap_gemm(g, math_mode, st);
 }
 int norm_rows(const RowNorm& r, cudaStream_t st) {
   ProfScope prof_scope(P_ROWNORM, 8.0 * r.rows * r.C,
@@ -125,21 +117,8 @@ int norm_rows(const RowNorm& r, cudaStream_t st) {
 inline int round4(int x) { return (x + 3) & ~3; }
 inline int round8(int x) { return (x + 7) & ~7; }
 
-TapGemm make_gemm(const Dense& d, const float* x, int ldx, int B, int L, int act, const float* resid, int ldr, float* out,
-                  int ldo) {
-  TapGemm g;
-  g.x = x; g.ldx = ldx; g.B = B; g.L = L; g.K = d.K; g.w = d.w; g.bias = d.bias; g.N = d.N; g.taps = d.taps;
-  g.act = act; g.resid = resid; g.ldr = ldr; g.out = out; g.ldo = ldo;
-  return g;
-}
-// contraction on operand planes written by this library (kPlaneScale): f16 on the hi planes, or 3xF16 (x3)
-TapGemm make_gemm_p(const Dense& d, const __half* xp, int B, int L, bool x3, int act, const float* resid, int ldr, float* out,
-                    int ldo) {
-  TapGemm g = make_gemm(d, nullptr, d.K, B, L, act, resid, ldr, out, ldo);
-  g.xp = xp; g.w_hi = d.w_hi; g.w_lo = d.w_lo; g.w_inv = d.w_inv; g.a_inv = kPlaneInv; g.precise = x3;
-  return g;
-}
-void planes_out(TapGemm& g, __half* outp, int ldo_p, bool lo) { g.outp = outp; g.ldo_p = ldo_p; g.outp_lo = lo; }
+// a GEMM's A operand in math_mode: the fp32 rows x, or the operand planes xp of the same tensor in the plane modes
+inline const void* operand(int math_mode, const float* x, const __half* xp) { return plane_mode(math_mode) ? (const void*)xp : x; }
 
 RowNorm make_norm(const Norm& n, const float* x, int ldx, int64_t rows, int C, float* out, int ldo) {
   RowNorm r;
@@ -151,7 +130,6 @@ RowNorm make_norm(const Norm& n, const float* x, int ldx, int64_t rows, int C, f
 // Per-utterance mode (FS2_PER_UTTERANCE): zlens != nullptr.  Every tensor a convolution reads or the caller receives then
 // holds exact zeros at rows t >= zlens[b], so each convolution's "same" padding falls at the utterance's own length, as in
 // a B = 1 run.  zlens == nullptr leaves the kernels exactly as in the reference-semantics path.
-TapGemm masked(TapGemm g, const int64_t* zlens) { g.lens = zlens; return g; }
 RowNorm masked(RowNorm r, const int64_t* zlens, int L) {
   if (zlens) { r.lens = zlens; r.L = L; }
   return r;
@@ -163,79 +141,54 @@ struct BlockBufs {
   __half *xp, *qkp, *vtp, *ctxp, *hidp;   // plane families: the same tensors as operand planes (qkp..hidp alias the fp32 ones)
 };
 
-// FFT blocks of the fp32-FMA and tf32 families (fp32 rows everywhere); the result lands in *result
+// FFT blocks in math mode `mode`; the result lands in *result.  fp32 / tf32: fp32 rows everywhere.  f16 / 3xF16: every
+// contraction reads fp16 operand planes written by its producer and writes the planes its consumer reads; fp32 rows exist
+// only for the residual stream (x, y), and residual + LayerNorm run as a row kernel after each projection.  On entry w.xp
+// holds the planes of w.x; on exit it holds the planes of *result.
 int run_blocks(const std::vector<Block>& blocks, const BlockBufs& w, const int64_t* lens, const int64_t* zlens, int B, int L,
-               int C, int heads, int math_mode, bool is_dec, cudaStream_t st, float** result) {
+               int C, int heads, int mode, bool is_dec, cudaStream_t st, float** result) {
   const int64_t rows = (int64_t)B * L;
   const int c_qkv = is_dec ? P_DEC_QKV : P_ENC_QKV, c_att = is_dec ? P_DEC_ATTN : P_ENC_ATTN;
   const int c_out = is_dec ? P_DEC_OUT : P_ENC_OUT, c_w1 = is_dec ? P_DEC_W1 : P_ENC_W1, c_w2 = is_dec ? P_DEC_W2 : P_ENC_W2;
+  const bool planes = plane_mode(mode), x3 = mode == FS2_MATH_3XTF32;
+  const int lpad = planes ? round8(L) : round4(L);
   float *x = w.x, *y = w.y;
   for (const Block& k : blocks) {
     int rc;
-    // q | k | v projection (attention.py:48-50), one GEMM with N = 3C
-    TapGemm gq = masked(make_gemm(k.qkv, x, C, B, L, ACT_NONE, nullptr, 0, w.qkv, 3 * C), zlens);
-    if (math_mode == FS2_MATH_TF32) {  // V third stored transposed for the tensor-core attention (gemm_tc.cu epilogue)
-      gq.vt_out = w.vt; gq.vt_col0 = 2 * C; gq.vt_dk = C / heads; gq.vt_heads = heads; gq.vt_lpad = round4(L);
-    }
-    if ((rc = dense(gq, math_mode, st, c_qkv))) return rc;
+    // q | k | v projection (attention.py:48-50), one GEMM with N = 3C.  tf32: the V third is also stored transposed for the
+    // tensor-core attention (gemm_tc.cu epilogue).  Plane modes: q | k leave as planes [P][rows][2C], the V third as
+    // transposed planes [P][B*heads][dk][lpad]; no fp32 copy exists
+    TapGemm gq = vweight_gemm_args(mode, k.qkv, operand(mode, x, w.xp), B, L, ACT_NONE, zlens, planes ? nullptr : w.qkv,
+                                   nullptr, 1, w.qkp);
+    if (planes) { gq.ldo_p = 2 * C; gq.vtp = w.vtp; }
+    else if (mode == FS2_MATH_TF32) gq.vt_out = w.vt;
+    if (gq.vtp || gq.vt_out) { gq.vt_col0 = 2 * C; gq.vt_dk = C / heads; gq.vt_heads = heads; gq.vt_lpad = lpad; }
+    if ((rc = dense(gq, mode, st, c_qkv))) return rc;
     {
-      ProfScope prof_scope(c_att, 4.0 * B * (double)L * L * C, 4.0 * 4.0 * B * (double)L * C, st);
-      rc = math_mode == FS2_MATH_TF32 ? attention_tf32(w.qkv, w.vt, round4(L), lens, B, L, C, heads, w.ctx, st)
-                                      : attention_fp32(w.qkv, lens, B, L, C, heads, w.ctx, st);
+      ProfScope prof_scope(c_att, 4.0 * B * (double)L * L * C, (planes && !x3 ? 2.0 : 4.0) * 4.0 * B * (double)L * C, st);
+      rc = planes ? attention_planes(w.qkp, w.vtp, lpad, lens, B, L, C, heads, x3, nullptr, w.ctxp, st)
+         : mode == FS2_MATH_TF32 ? attention_tf32(w.qkv, w.vt, lpad, lens, B, L, C, heads, w.ctx, st)
+                                 : attention_fp32(w.qkv, lens, B, L, C, heads, w.ctx, st);
       if (rc) return rc;
     }
-    // x = LN(x + linear_out(ctx)) (attention.py:74, encoder.py:60-62).  Per-utterance mode: ctx rows past len are the
-    // attention kernels' output of those query rows times 0 (the q|k|v projection writes them as zeros, DESIGN.md
-    // section 5, so they are zeros of either sign); the out-projection reads each ctx row only for its own output row,
-    // which it writes as 0 there
-    if ((rc = dense(masked(make_gemm(k.out, w.ctx, C, B, L, ACT_NONE, x, C, y, C), zlens), math_mode, st, c_out))) return rc;
-    if ((rc = norm_rows(masked(make_norm(k.ln1, y, C, rows, C, x, C), zlens, L), st))) return rc;
-    // conv-FFN: hid = relu(conv_k(x)); x = LN(x + conv_1(hid))  (modules.py:247-248, encoder.py:64-69)
-    if ((rc = dense(masked(make_gemm(k.w1, x, C, B, L, ACT_RELU, nullptr, 0, w.hid, k.w1.N), zlens), math_mode, st, c_w1))) return rc;
-    if ((rc = dense(masked(make_gemm(k.w2, w.hid, k.w1.N, B, L, ACT_NONE, x, C, y, C), zlens), math_mode, st, c_w2))) return rc;
-    if ((rc = norm_rows(masked(make_norm(k.ln2, y, C, rows, C, x, C), zlens, L), st))) return rc;
-  }
-  *result = x;
-  return FS2_OK;
-}
-
-// FFT blocks of the plane families: every contraction reads fp16 operand planes written by its producer and writes the
-// planes its consumer reads; fp32 rows exist only for the residual stream (x, y).  x3: error-compensated (hi + lo planes,
-// fp32-class); else f16 on the hi planes; residual + LayerNorm run as a row kernel after each projection.
-// On entry w.xp holds the planes of w.x; on exit it holds the planes of *result.
-int run_blocks_planes(const std::vector<Block>& blocks, const BlockBufs& w, const int64_t* lens, const int64_t* zlens, int B,
-                      int L, int C, int heads, bool x3, bool is_dec, cudaStream_t st, float** result) {
-  const int64_t rows = (int64_t)B * L;
-  const int c_qkv = is_dec ? P_DEC_QKV : P_ENC_QKV, c_att = is_dec ? P_DEC_ATTN : P_ENC_ATTN;
-  const int c_out = is_dec ? P_DEC_OUT : P_ENC_OUT, c_w1 = is_dec ? P_DEC_W1 : P_ENC_W1, c_w2 = is_dec ? P_DEC_W2 : P_ENC_W2;
-  const int lpad = round8(L);
-  float *x = w.x, *y = w.y;
-  for (const Block& k : blocks) {
-    int rc;
-    // q | k | v projection (attention.py:48-50), one GEMM with N = 3C: q | k leave as planes [P][rows][2C], the V third
-    // as transposed planes [P][B*heads][dk][lpad]; no fp32 copy exists
-    TapGemm gq = masked(make_gemm_p(k.qkv, w.xp, B, L, x3, ACT_NONE, nullptr, 0, nullptr, 0), zlens);
-    planes_out(gq, w.qkp, 2 * C, x3);
-    gq.vtp = w.vtp; gq.vt_col0 = 2 * C; gq.vt_dk = C / heads; gq.vt_heads = heads; gq.vt_lpad = lpad;
-    if ((rc = dense(gq, FS2_MATH_F16, st, c_qkv))) return rc;
-    {
-      ProfScope prof_scope(c_att, 4.0 * B * (double)L * L * C, (x3 ? 4.0 : 2.0) * 4.0 * B * (double)L * C, st);
-      if ((rc = attention_planes(w.qkp, w.vtp, lpad, lens, B, L, C, heads, x3, nullptr, w.ctxp, st))) return rc;
-    }
-    // x = LN(x + linear_out(ctx)) (attention.py:74, encoder.py:60-62); the LayerNorm also writes the conv-FFN's operand planes
-    // (per-utterance mode: see run_blocks on the ctx rows past len)
-    if ((rc = dense(masked(make_gemm_p(k.out, w.ctxp, B, L, x3, ACT_NONE, x, C, y, C), zlens), FS2_MATH_F16, st, c_out))) return rc;
+    // x = LN(x + linear_out(ctx)) (attention.py:74, encoder.py:60-62); plane modes: the LayerNorm also writes the conv-FFN's
+    // operand planes.  Per-utterance mode: ctx rows past len are the attention kernels' output of those query rows times 0
+    // (the q|k|v projection writes them as zeros, DESIGN.md section 5, so they are zeros of either sign); the out-projection
+    // reads each ctx row only for its own output row, which it writes as 0 there
+    if ((rc = dense(vweight_gemm_args(mode, k.out, operand(mode, w.ctx, w.ctxp), B, L, ACT_NONE, zlens, y, x), mode, st, c_out)))
+      return rc;
     RowNorm r1 = masked(make_norm(k.ln1, y, C, rows, C, x, C), zlens, L);
-    r1.split_out = w.xp; r1.split_lo = x3;
+    if (planes) { r1.split_out = w.xp; r1.split_lo = x3; }
     if ((rc = norm_rows(r1, st))) return rc;
-    // conv-FFN: hid = relu(conv_k(x)); x = LN(x + conv_1(hid))  (modules.py:247-248, encoder.py:64-69); the hidden
-    // activations exist only as planes
-    TapGemm g1 = masked(make_gemm_p(k.w1, w.xp, B, L, x3, ACT_RELU, nullptr, 0, nullptr, 0), zlens);
-    planes_out(g1, w.hidp, k.w1.N, x3);
-    if ((rc = dense(g1, FS2_MATH_F16, st, c_w1))) return rc;
-    if ((rc = dense(masked(make_gemm_p(k.w2, w.hidp, B, L, x3, ACT_NONE, x, C, y, C), zlens), FS2_MATH_F16, st, c_w2))) return rc;
+    // conv-FFN: hid = relu(conv_k(x)); x = LN(x + conv_1(hid))  (modules.py:247-248, encoder.py:64-69); plane modes: the
+    // hidden activations exist only as planes
+    TapGemm g1 = vweight_gemm_args(mode, k.w1, operand(mode, x, w.xp), B, L, ACT_RELU, zlens, planes ? nullptr : w.hid, nullptr,
+                                   1, w.hidp);
+    if ((rc = dense(g1, mode, st, c_w1))) return rc;
+    if ((rc = dense(vweight_gemm_args(mode, k.w2, operand(mode, w.hid, w.hidp), B, L, ACT_NONE, zlens, y, x), mode, st, c_w2)))
+      return rc;
     RowNorm r2 = masked(make_norm(k.ln2, y, C, rows, C, x, C), zlens, L);
-    r2.split_out = w.xp; r2.split_lo = x3;                 // planes of the block output: A operand of the next q|k|v / mel projection
+    if (planes) { r2.split_out = w.xp; r2.split_lo = x3; }   // planes of the block output: A operand of the next q|k|v / mel projection
     if ((rc = norm_rows(r2, st))) return rc;
   }
   *result = x;
@@ -249,13 +202,13 @@ int run_predictor(const Predictor& p, const float* x, const __half* xp, int C, i
                   const int64_t* lens, const int64_t* zlens, float* head_out, int64_t* dur_out, const float* head_scale,
                   cudaStream_t st) {
   const int64_t rows = (int64_t)B * L;
-  const float* cur = x; const __half* cur_p = xp; int curC = C;
+  const int mode = xp ? MATH_3XTF32 : FS2_MATH_FP32;
+  const float* cur = x; const __half* cur_p = xp;
   for (int i = 0; i < p.layers; ++i) {
     int rc;
     const int N = p.conv[i].N;
-    TapGemm g = xp ? make_gemm_p(p.conv[i], cur_p, B, L, true, ACT_RELU, nullptr, 0, t1, N)
-                   : make_gemm(p.conv[i], cur, curC, B, L, ACT_RELU, nullptr, 0, t1, N);
-    if ((rc = dense(masked(g, zlens), FS2_MATH_FP32, st, P_PRED_GEMM))) return rc;
+    if ((rc = dense(vweight_gemm_args(mode, p.conv[i], operand(mode, cur, cur_p), B, L, ACT_RELU, zlens, t1), mode, st, P_PRED_GEMM)))
+      return rc;
     RowNorm r = masked(make_norm(p.ln[i], t1, N, rows, N, xp ? nullptr : t2, N), zlens, L);
     if (i == p.layers - 1) {  // last layer: only the scalar head leaves the kernel
       r.out = nullptr; r.head_w = p.head_w; r.head_b = p.head_b; r.head_out = head_out; r.dur_out = dur_out;
@@ -265,7 +218,7 @@ int run_predictor(const Predictor& p, const float* x, const __half* xp, int C, i
       r.split_out = t2p; r.split_lo = 1;
     }
     if ((rc = norm_rows(r, st))) return rc;
-    cur = t2; cur_p = t2p; curC = N;
+    cur = t2; cur_p = t2p;
   }
   return FS2_OK;
 }
@@ -279,45 +232,42 @@ const fs2_weight_desc* find(const Map& m, const std::string& k) {
   const fs2_weight_desc* var = find(m, key);                                  \
   if (!var) { set_error("fs2_load_weights: missing key '%s'", std::string(key).c_str()); return FS2_ERR_MISSING_WEIGHT; }
 
+// One pass over the checkpoint: on a counting Bump it checks every tensor and sizes the arena, on the arena it fills it
 struct Packer {
-  fs2_handle* h; const Map& m; cudaStream_t st; Bump bump; bool counting;
-  Packer(fs2_handle* h_, const Map& m_, cudaStream_t s, float* base, size_t cap)
-      : h(h_), m(m_), st(s), bump(base, cap), counting(base == nullptr) {}
+  fs2_handle* h; const Map& m; cudaStream_t st; Bump& bump; bool counting;
+  Packer(fs2_handle* h_, const Map& m_, cudaStream_t s, Bump& b) : h(h_), m(m_), st(s), bump(b), counting(b.base == nullptr) {}
 
-  int copy(const std::string& key, int64_t n, const float** out) {
+  int copy_into(const std::string& key, int64_t n, float* dst) {
     NEED(d, key);
     int64_t have = 1; for (int i = 0; i < d->ndim; ++i) have *= d->shape[i];
     if (have != n) { set_error("fs2_load_weights: '%s' has %lld elements, expected %lld", key.c_str(), (long long)have, (long long)n); return FS2_ERR_INVALID; }
-    float* dst = bump.floats(n);
     if (!counting) FS2_CUDA_CHECK(cudaMemcpyAsync(dst, d->data, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return FS2_OK;
+  }
+  int copy(const std::string& key, int64_t n, const float** out) {
+    float* dst = bump.floats(n);
     *out = dst;
-    return FS2_OK;
+    return copy_into(key, n, dst);
   }
-  // Linear [N,K] (taps=1) or Conv1d [N,K,taps] -> [taps][N][K]
-  int dense(const std::string& wkey, const std::string& bkey, int N, int K, int taps, Dense* out, const float* scale = nullptr,
-            const float* shift = nullptr) {
-    NEED(w, wkey);
-    int64_t have = 1; for (int i = 0; i < w->ndim; ++i) have *= w->shape[i];
-    if (have != (int64_t)N * K * taps) { set_error("fs2_load_weights: '%s' has %lld elements, expected %dx%dx%d", wkey.c_str(), (long long)have, N, K, taps); return FS2_ERR_INVALID; }
-    float* dst = bump.floats((size_t)N * K * taps);
-    if (!counting) { int rc = pack_conv_weight((const float*)w->data, N, K, taps, scale, dst, st); if (rc) return rc; }
-    out->w = dst; out->N = N; out->K = K; out->taps = taps; out->bias = shift;
-    if (!bkey.empty()) { int rc = copy(bkey, N, &out->bias); if (rc) return rc; }
-    return FS2_OK;
+  // a [taps][N][K] weight with a bias [N], carved from the arena
+  VWeight carve(int N, int K, int taps) {
+    VWeight w; w.N = N; w.K = K; w.taps = taps;
+    vweight_carve(bump, w, true);
+    return w;
   }
-  // fp16 hi / lo planes of (s * w) with the layer's power-of-two scale s (gemm_tc.cu): f16 reads the hi plane,
-  // 3xF16 reads both; the consuming epilogue multiplies by 1 / s (d->w_inv, a device scalar)
-  int split(Dense* d) {
-    const size_t n = (size_t)d->N * d->K * d->taps;
-    __half* hh = (__half*)bump.bytes(n * sizeof(__half));
-    __half* lh = (__half*)bump.bytes(n * sizeof(__half));
-    float* sc = bump.floats(2);       // [scale, 1 / scale]
-    if (!counting) {
-      int rc = weight_scale(d->w, (long)n, sc, sc + 1, st); if (rc) return rc;
-      rc = split_f16(d->w, hh, lh, (long)n, sc, st); if (rc) return rc;
-    }
-    d->w_hi = hh; d->w_lo = lh; d->w_inv = sc + 1;
-    return FS2_OK;
+  // w's rows from the Linear [N,K] (taps=1) or Conv1d [N,K,taps] wkey, times scale[n] when given, and its planes
+  int fill(const std::string& wkey, VWeight& w, const float* scale = nullptr) {
+    NEED(d, wkey);
+    int64_t have = 1; for (int i = 0; i < d->ndim; ++i) have *= d->shape[i];
+    if (have != (int64_t)w.N * w.K * w.taps) { set_error("fs2_load_weights: '%s' has %lld elements, expected %dx%dx%d", wkey.c_str(), (long long)have, w.N, w.K, w.taps); return FS2_ERR_INVALID; }
+    if (counting) return FS2_OK;
+    int rc = pack_conv_weight((const float*)d->data, w.N, w.K, w.taps, scale, w.w, st);
+    return rc ? rc : vweight_planes(w, st);
+  }
+  int dense(const std::string& wkey, const std::string& bkey, int N, int K, int taps, VWeight* out) {
+    *out = carve(N, K, taps);
+    int rc = fill(wkey, *out);
+    return rc ? rc : copy_into(bkey, N, out->bias);
   }
   // positional table [1, rows, C]: as many rows as the checkpoint tensor holds (the reference regenerates a longer table
   // on demand, core/embedding.py:48-66; the Python class does the same and the repack picks the new length up here)
@@ -341,23 +291,21 @@ struct Packer {
       std::string p = prefix + ".encoders_." + std::to_string(i) + ".";
       Block& b = (*out)[i];
       // fused q|k|v: three [C,C] Linear weights stacked along N
-      float* wq = bump.floats((size_t)3 * C * C);
-      float* bq = bump.floats((size_t)3 * C);
+      b.qkv = carve(3 * C, C, 1);
       const char* nm[3] = {"q", "k", "v"};
       for (int j = 0; j < 3; ++j) {
         NEED(w, p + "self_attn.linear_" + nm[j] + ".weight");
         NEED(bb, p + "self_attn.linear_" + nm[j] + ".bias");
         if (!counting) {
-          FS2_CUDA_CHECK(cudaMemcpyAsync(wq + (size_t)j * C * C, w->data, (size_t)C * C * sizeof(float), cudaMemcpyDeviceToDevice, st));
-          FS2_CUDA_CHECK(cudaMemcpyAsync(bq + (size_t)j * C, bb->data, (size_t)C * sizeof(float), cudaMemcpyDeviceToDevice, st));
+          FS2_CUDA_CHECK(cudaMemcpyAsync(b.qkv.w + (size_t)j * C * C, w->data, (size_t)C * C * sizeof(float), cudaMemcpyDeviceToDevice, st));
+          FS2_CUDA_CHECK(cudaMemcpyAsync(b.qkv.bias + (size_t)j * C, bb->data, (size_t)C * sizeof(float), cudaMemcpyDeviceToDevice, st));
         }
       }
-      b.qkv.w = wq; b.qkv.bias = bq; b.qkv.N = 3 * C; b.qkv.K = C; b.qkv.taps = 1;
       int rc;
+      if (!counting && (rc = vweight_planes(b.qkv, st))) return rc;
       if ((rc = dense(p + "self_attn.linear_out.weight", p + "self_attn.linear_out.bias", C, C, 1, &b.out))) return rc;
       if ((rc = dense(p + "feed_forward.w_1.weight", p + "feed_forward.w_1.bias", H, C, kffn, &b.w1))) return rc;
       if ((rc = dense(p + "feed_forward.w_2.weight", p + "feed_forward.w_2.bias", C, H, 1, &b.w2))) return rc;
-      for (Dense* d : {&b.qkv, &b.out, &b.w1, &b.w2}) if ((rc = split(d))) return rc;
       if ((rc = norm(p + "norm1.", C, 1e-5f, &b.ln1))) return rc;   // encoder.py:37-38
       if ((rc = norm(p + "norm2.", C, 1e-5f, &b.ln2))) return rc;
     }
@@ -370,7 +318,6 @@ struct Packer {
       std::string p = prefix + "conv." + std::to_string(i) + ".";
       int rc;
       if ((rc = dense(p + "0.weight", p + "0.bias", c.pred_chans, i == 0 ? c.adim : c.pred_chans, c.pred_kernel, &out->conv[i]))) return rc;
-      if ((rc = split(&out->conv[i]))) return rc;
       if ((rc = norm(p + "2.layer_norm.", c.pred_chans, 1e-12f, &out->ln[i]))) return rc;  // modules.py:115
     }
     int rc;
@@ -407,26 +354,24 @@ struct Packer {
     }
     // decoder (fastspeech.py:119-136; input layer core/encoder.py:118-125)
     if ((rc = dense("decoder.embed.0.weight", "decoder.embed.0.bias", c.ddim, c.adim, 1, &h->dec_in))) return rc;
-    if ((rc = split(&h->dec_in))) return rc;                                   // hi/lo copies serve FS2_MATH_3XTF32
     if ((rc = norm("decoder.embed.1.", c.ddim, 1e-5f, &h->dec_in_ln))) return rc;
     if ((rc = copy("decoder.embed.4.alpha", 1, &h->dec_alpha))) return rc;
     if ((rc = pos_table("decoder.embed.4.pe", c.ddim, &h->dec_pe, &h->dec_pe_len))) return rc;
     if ((rc = blocks("decoder", c.dlayers, c.ddim, c.dunits, c.ffn_kernel, &h->dec))) return rc;
     if ((rc = dense("feat_out.weight", "feat_out.bias", c.odim, c.ddim, 1, &h->feat_out))) return rc;
-    if ((rc = split(&h->feat_out))) return rc;
     // Postnet: Conv1d(no bias) + BatchNorm1d(eval) folded into weight scale + bias (modules.py:283-348)
-    h->postnet.assign(c.postnet_layers, Dense());
+    h->postnet.assign(c.postnet_layers, VWeight());
     for (int i = 0; i < c.postnet_layers; ++i) {
       std::string p = "postnet.postnet." + std::to_string(i) + ".";
       int cin = i == 0 ? c.odim : c.postnet_chans;
       int cout = i == c.postnet_layers - 1 ? c.odim : c.postnet_chans;
+      VWeight& w = h->postnet[i];
+      w = carve(cout, cin, c.postnet_filts);
       float* scale = bump.floats(cout);
-      float* shift = bump.floats(cout);
       NEED(g, p + "1.weight"); NEED(b, p + "1.bias"); NEED(mu, p + "1.running_mean"); NEED(var, p + "1.running_var");
       if (!counting && (rc = fold_batchnorm((const float*)g->data, (const float*)b->data, (const float*)mu->data,
-                                            (const float*)var->data, 1e-5f, cout, scale, shift, st))) return rc;
-      if ((rc = dense(p + "0.weight", "", cout, cin, c.postnet_filts, &h->postnet[i], scale, shift))) return rc;
-      if ((rc = split(&h->postnet[i]))) return rc;
+                                            (const float*)var->data, 1e-5f, cout, scale, w.bias, st))) return rc;
+      if ((rc = fill(p + "0.weight", w, scale))) return rc;
     }
     return FS2_OK;
   }
@@ -547,20 +492,7 @@ int fs2_load_weights(fs2_handle* h, const fs2_weight_desc* w, int n, void* strea
     m[w[i].name] = &w[i];
   }
   h->loaded = false;
-  size_t need;
-  {
-    Packer count(h, m, st, nullptr, 0);
-    int rc = count.run();
-    if (rc) return rc;
-    need = count.bump.off + 256;
-  }
-  if (need > h->arena_floats * sizeof(float)) {
-    if (h->arena) { FS2_CUDA_CHECK(cudaStreamSynchronize(st)); FS2_CUDA_CHECK(cudaFree(h->arena)); h->arena = nullptr; }
-    FS2_CUDA_CHECK(cudaMalloc(&h->arena, need));
-    h->arena_floats = need / sizeof(float);
-  }
-  Packer pack(h, m, st, h->arena, need);
-  int rc = pack.run();
+  int rc = arena_carve(&h->arena, &h->arena_bytes, st, [&](Bump& b) { return Packer(h, m, st, b).run(); });
   if (rc) return rc;
   h->loaded = true;
   return FS2_OK;
@@ -601,8 +533,8 @@ int fs2_encode_ex(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B,
   { ProfScope prof_scope(P_EMBED, 0, (planes ? 12.0 : 8.0) * B * Tmax * c.adim, st);
     if ((rc = embed_posenc(xs, h->emb, c.idim, h->enc_pe, h->enc_alpha, B, Tmax, c.adim, p.w.x, planes ? p.w.xp : nullptr, zlens, st))) return rc; }
   float* enc_out = nullptr;
-  if (planes) { if ((rc = run_blocks_planes(h->enc, p.w, ilens, zlens, B, Tmax, c.adim, c.aheads, true, false, st, &enc_out))) return rc; }
-  else { if ((rc = run_blocks(h->enc, p.w, ilens, zlens, B, Tmax, c.adim, c.aheads, FS2_MATH_FP32, false, st, &enc_out))) return rc; }
+  if ((rc = run_blocks(h->enc, p.w, ilens, zlens, B, Tmax, c.adim, c.aheads, planes ? MATH_3XTF32 : FS2_MATH_FP32, false, st,
+                       &enc_out))) return rc;
   FS2_CUDA_CHECK(cudaMemcpyAsync(hs, enc_out, (size_t)B * Tmax * c.adim * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (d_log || d_int)
     if ((rc = run_predictor(h->dur, enc_out, planes ? p.w.xp : nullptr, c.adim, B, Tmax, p.t1, p.t2, p.t2p, ilens, zlens, d_log, d_int, nullptr, st))) return rc;
@@ -664,7 +596,7 @@ int fs2_decode_ctl(fs2_handle* h, const float* hm, const int64_t* olens, const f
   if (!b.ok()) { set_error("fs2_decode: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
   const int mode = c.math_mode;
   const bool pred_planes = mode != FS2_MATH_FP32;                              // predictors: 3xF16 in every tensor-core mode
-  const bool dec_planes = mode == FS2_MATH_3XTF32 || mode == FS2_MATH_F16;     // decoder side on operand planes
+  const bool dec_planes = plane_mode(mode);                                    // decoder side on operand planes
   const bool x3 = mode == FS2_MATH_3XTF32;
   const int64_t* zlens = (flags & FS2_PER_UTTERANCE) ? olens : nullptr;   // hm rows past olens are zero (length_gather)
   int rc;
@@ -684,38 +616,32 @@ int fs2_decode_ctl(fs2_handle* h, const float* hm, const int64_t* olens, const f
                                dec_planes ? p.hm2p : nullptr, x3, e_ids, p_ids, zlens, L, st))) return rc; }
   // decoder input layer: Linear -> LayerNorm -> ReLU -> x + alpha*pe (core/encoder.py:118-125)
   {
-    TapGemm g = dec_planes ? make_gemm_p(h->dec_in, p.hm2p, B, L, x3, ACT_NONE, nullptr, 0, p.w.y, c.ddim)
-                           : make_gemm(h->dec_in, p.hm2, c.adim, B, L, ACT_NONE, nullptr, 0, p.w.y, c.ddim);
-    if ((rc = dense(masked(g, zlens), mode, st, P_DEC_IN))) return rc;
+    if ((rc = dense(vweight_gemm_args(mode, h->dec_in, operand(mode, p.hm2, p.hm2p), B, L, ACT_NONE, zlens, p.w.y), mode, st,
+                    P_DEC_IN))) return rc;
     RowNorm r = masked(make_norm(h->dec_in_ln, p.w.y, c.ddim, rows, c.ddim, p.w.x, c.ddim), zlens, L);
     r.relu_after = 1; r.pe = h->dec_pe; r.alpha = h->dec_alpha; r.L = L;
     if (dec_planes) { r.split_out = p.w.xp; r.split_lo = x3; }    // first block's q|k|v reads the planes
     if ((rc = norm_rows(r, st))) return rc;
   }
   float* dec_out = nullptr;
-  if (dec_planes) { if ((rc = run_blocks_planes(h->dec, p.w, olens, zlens, B, L, c.ddim, c.aheads, x3, true, st, &dec_out))) return rc; }
-  else { if ((rc = run_blocks(h->dec, p.w, olens, zlens, B, L, c.ddim, c.aheads, mode, true, st, &dec_out))) return rc; }
+  if ((rc = run_blocks(h->dec, p.w, olens, zlens, B, L, c.ddim, c.aheads, mode, true, st, &dec_out))) return rc;
   // mel linear (fastspeech.py:228-230); plane families: from the planes of the last block's output, and the Postnet
   // chain stays in planes until the final residual layer
-  {
-    TapGemm g = masked(dec_planes ? make_gemm_p(h->feat_out, p.w.xp, B, L, x3, ACT_NONE, nullptr, 0, before, c.odim)
-                                  : make_gemm(h->feat_out, dec_out, c.ddim, B, L, ACT_NONE, nullptr, 0, before, c.odim), zlens);
-    if (dec_planes) planes_out(g, p.beforep, c.odim, x3);
-    if ((rc = dense(g, mode, st, P_FEAT_OUT))) return rc;
-  }
+  if ((rc = dense(vweight_gemm_args(mode, h->feat_out, operand(mode, dec_out, p.w.xp), B, L, ACT_NONE, zlens, before, nullptr, 1,
+                                    p.beforep), mode, st, P_FEAT_OUT))) return rc;
   // Postnet + residual (fastspeech.py:236-238, modules.py:350-359)
-  const float* cur = before; int curC = c.odim;
+  const float* cur = before;
   const __half* cur_p = p.beforep;
   float* pp[2] = {p.q1, p.q2};
   for (int i = 0; i < c.postnet_layers; ++i) {
     const bool last = i == c.postnet_layers - 1;
     float* dst = last ? after : pp[i & 1];
-    const int N = h->postnet[i].N;
-    TapGemm g = dec_planes ? make_gemm_p(h->postnet[i], cur_p, B, L, x3, last ? ACT_NONE : ACT_TANH, last ? before : nullptr, c.odim, last ? dst : nullptr, N)
-                           : make_gemm(h->postnet[i], cur, curC, B, L, last ? ACT_NONE : ACT_TANH, last ? before : nullptr, c.odim, dst, N);
-    if (dec_planes && !last) planes_out(g, reinterpret_cast<__half*>(dst), N, x3);
-    if ((rc = dense(masked(g, zlens), mode, st, P_POSTNET))) return rc;
-    cur = dst; cur_p = reinterpret_cast<const __half*>(dst); curC = N;
+    // plane families: the inner layers write only the planes the next one reads
+    TapGemm g = vweight_gemm_args(mode, h->postnet[i], operand(mode, cur, cur_p), B, L, last ? ACT_NONE : ACT_TANH, zlens,
+                                  dec_planes && !last ? nullptr : dst, last ? before : nullptr, 1,
+                                  last ? nullptr : reinterpret_cast<__half*>(dst));
+    if ((rc = dense(g, mode, st, P_POSTNET))) return rc;
+    cur = dst; cur_p = reinterpret_cast<const __half*>(dst);
   }
   return FS2_OK;
 }
@@ -740,19 +666,22 @@ int fs2_one_hot(const int64_t* ids, int64_t n, int n_bins, float* out, void* str
 }
 
 namespace {
-// single-operator entries of the plane families (tests): operand planes of x and w are made on the fly in a
-// stream-ordered temporary; layout [x planes 2*nx][w hi nw][w lo nw][scale, inv]
+// single-operator entries (tests): the weight [taps][N][K] at the caller's pointer; in the plane families the operand planes
+// of x and the weight's scale and planes are made on the fly in a stream-ordered temporary, layout
+// [x planes 2*nx][w hi nw][w lo nw][scale, inv]
 struct TempPlanes {
-  __half* base = nullptr; __half *xp, *w_hi, *w_lo; float* sc; cudaStream_t st;
-  int make(const float* x, long rows, int K, const float* w, long nw, cudaStream_t s) {
+  __half* base = nullptr; __half* xp = nullptr; VWeight w; cudaStream_t st;
+  TempPlanes(const float* w_, const float* bias, int N, int K, int taps) {
+    w.w = const_cast<float*>(w_); w.bias = const_cast<float*>(bias); w.N = N; w.K = K; w.taps = taps;
+  }
+  int make(const float* x, long rows, cudaStream_t s) {
     st = s;
-    const size_t nx = (size_t)rows * K, nx8 = (2 * nx + 15) & ~(size_t)15, nw8 = ((size_t)nw + 15) & ~(size_t)15;
+    const size_t nx = (size_t)rows * w.K, nw = (size_t)w.taps * w.N * w.K;
+    const size_t nx8 = (2 * nx + 15) & ~(size_t)15, nw8 = (nw + 15) & ~(size_t)15;
     FS2_CUDA_CHECK(cudaMallocAsync(&base, (nx8 + 2 * nw8) * sizeof(__half) + 64, st));
-    xp = base; w_hi = base + nx8; w_lo = w_hi + nw8; sc = reinterpret_cast<float*>(w_lo + nw8);
-    int rc = split_rows(x, K, rows, K, xp, st);
-    if (!rc) rc = weight_scale(w, nw, sc, sc + 1, st);
-    if (!rc) rc = split_f16(w, w_hi, w_lo, nw, sc, st);
-    return rc;
+    xp = base; w.hi = base + nx8; w.lo = w.hi + nw8; w.sc = reinterpret_cast<float*>(w.lo + nw8);
+    int rc = split_rows(x, w.K, rows, w.K, xp, st);
+    return rc ? rc : vweight_planes(w, st);
   }
   ~TempPlanes() { if (base) cudaFreeAsync(base, st); }
 };
@@ -775,7 +704,7 @@ int fs2_op_tap_gemm_dil(int math_mode, const float* x, int B, int L, int K, cons
   const char* who = "fs2_op_tap_gemm";
   FS2_REQUIRE(math_mode == FS2_MATH_FP32 || math_mode == FS2_MATH_TF32 || math_mode == FS2_MATH_F16 || math_mode == FS2_MATH_3XTF32,
               "%s: unknown math mode %d", who, math_mode);
-  const bool planes = math_mode == FS2_MATH_F16 || math_mode == FS2_MATH_3XTF32;
+  const bool planes = plane_mode(math_mode);
   FS2_REQUIRE(x && w && (out || (planes && (out_planes || vt))), "%s: null argument", who);
   FS2_REQUIRE(B >= 0 && L >= 0 && K > 0 && N > 0 && taps > 0, "%s: bad shape B=%d L=%d K=%d N=%d taps=%d", who, B, L, K, N, taps);
   // tap rows t + (j - pad) * dil are int32 row coordinates: keep them in range (dil = 1 is the undilated call, as before)
@@ -785,25 +714,17 @@ int fs2_op_tap_gemm_dil(int math_mode, const float* x, int B, int L, int K, cons
   FS2_REQUIRE(!vt || math_mode != FS2_MATH_FP32, "%s: the fp32 family has no transposed V output", who);
   FS2_REQUIRE(!vt || (vt_heads > 0 && vt_col0 >= 0 && vt_col0 < N && (N - vt_col0) % vt_heads == 0 && vt_lpad >= L),
               "%s: transposed V needs 0 <= vt_col0 < N, heads dividing N - vt_col0 and vt_lpad >= L", who);
-  Dense d; d.w = w; d.bias = bias; d.N = N; d.K = K; d.taps = taps;
   cudaStream_t st = (cudaStream_t)stream;
-  TapGemm g;
-  TempPlanes t;
-  if (planes) {
-    int rc = t.make(x, (long)B * L, K, w, (long)N * K * taps, st);
-    if (rc) return rc;
-    d.w_hi = t.w_hi; d.w_lo = t.w_lo; d.w_inv = t.sc + 1;
-    g = make_gemm_p(d, t.xp, B, L, math_mode == MATH_3XTF32, act, resid, N, out, N);
-    planes_out(g, reinterpret_cast<__half*>(out_planes), N, math_mode == MATH_3XTF32);   // the lo flag covers vt's lo plane too
-  } else {
-    g = make_gemm(d, x, K, B, L, act, resid, N, out, N);
-  }
+  TempPlanes t(w, bias, N, K, taps);
+  if (planes) { int rc = t.make(x, (long)B * L, st); if (rc) return rc; }
+  TapGemm g = vweight_gemm_args(math_mode, t.w, operand(math_mode, x, t.xp), B, L, act, lens, out, resid, dil,
+                                reinterpret_cast<__half*>(out_planes));
   if (vt) {
     g.vt_col0 = vt_col0; g.vt_heads = vt_heads; g.vt_dk = (N - vt_col0) / vt_heads; g.vt_lpad = vt_lpad;
     if (planes) g.vtp = reinterpret_cast<__half*>(vt); else g.vt_out = reinterpret_cast<float*>(vt);
+    g.outp_lo = g.precise;   // the lo flag covers vt's lo plane too
   }
-  g.dil = dil;
-  return dense(masked(g, lens), math_mode, st, P_DEC_W1);
+  return dense(g, math_mode, st, P_DEC_W1);
 }
 int fs2_op_gemm_layernorm(int math_mode, const float* x, int64_t rows, int K, int N, const float* w, const float* bias, const float* resid,
                           const float* gamma, const float* beta, float eps, float* out, float* out_planes, void* stream) {
@@ -813,23 +734,16 @@ int fs2_op_gemm_layernorm(int math_mode, const float* x, int64_t rows, int K, in
               "fs2_op_gemm_layernorm: tensor-core modes only (FS2_MATH_TF32, FS2_MATH_F16, FS2_MATH_3XTF32)");
   FS2_REQUIRE(N == 384 || (N == 256 && math_mode != FS2_MATH_TF32), "fs2_op_gemm_layernorm: N must be 384 (or 256 in the plane families)");
   cudaStream_t st = (cudaStream_t)stream;
-  Dense d; d.w = w; d.bias = bias; d.N = N; d.K = K; d.taps = 1;
   FS2_REQUIRE(!out_planes || math_mode != FS2_MATH_TF32, "fs2_op_gemm_layernorm: the tf32 variant has no plane output in this entry");
   // y = x w^T + bias + resid on the tensor cores, then the row LayerNorm (which also writes the operand planes)
   float* y = nullptr;
   __half* op = nullptr;
   FS2_CUDA_CHECK(cudaMallocAsync(&y, (size_t)rows * N * sizeof(float) + 64, st));
-  int rc = FS2_OK;
-  if (math_mode == FS2_MATH_TF32) {
-    rc = dense(make_gemm(d, x, K, 1, (int)rows, ACT_NONE, resid, N, y, N), FS2_MATH_TF32, st, P_DEC_OUT);
-  } else {
-    TempPlanes t;
-    rc = t.make(x, (long)rows, K, w, (long)N * K, st);
-    if (!rc) {
-      d.w_hi = t.w_hi; d.w_lo = t.w_lo; d.w_inv = t.sc + 1;
-      rc = dense(make_gemm_p(d, t.xp, 1, (int)rows, math_mode == MATH_3XTF32, ACT_NONE, resid, N, y, N), FS2_MATH_F16, st, P_DEC_OUT);
-    }
-  }
+  TempPlanes t(w, bias, N, K, 1);
+  int rc = plane_mode(math_mode) ? t.make(x, (long)rows, st) : FS2_OK;
+  if (!rc)
+    rc = dense(vweight_gemm_args(math_mode, t.w, operand(math_mode, x, t.xp), 1, (int)rows, ACT_NONE, nullptr, y, resid), math_mode,
+               st, P_DEC_OUT);
   Norm n; n.g = gamma; n.b = beta; n.eps = eps;
   RowNorm r = make_norm(n, y, N, rows, N, out, N);
   // optional: the result's operand planes (what the next contraction would read), returned as fp32 = (hi + lo) / kPlaneScale

@@ -430,7 +430,7 @@ struct fs2_features {
   std::vector<double> taps_host;   // low-cut taps (2 M + 1), then each band's Nuttall window (4 h)
   bool loaded = false;
   int device = -1;
-  void* arena = nullptr;
+  void* arena = nullptr; size_t arena_bytes = 0;
   fs2::VWeight fwd, mel;           // forward DFT [cpad][n_fft], mel filterbank [n_mels][mpad]
   double* taps = nullptr;
 };
@@ -573,10 +573,11 @@ int fs2_features_load(fs2_features* f, const float* w_forward, const float* mel_
   const int nf = f->cfg.n_fft;
   f->fwd.N = f->cpad; f->fwd.K = nf;
   f->mel.N = f->cfg.n_mels; f->mel.K = f->mpad;
-  int rc = arena_carve(&f->arena, st, [&](Bump& b) {
+  int rc = arena_carve(&f->arena, &f->arena_bytes, st, [&](Bump& b) {
     vweight_carve(b, f->fwd, false);
     vweight_carve(b, f->mel, false);
     f->taps = b.doubles(f->taps_host.size());
+    return FS2_OK;
   });
   if (rc) return rc;
   FS2_CUDA_CHECK(cudaGetDevice(&f->device));

@@ -204,7 +204,7 @@ struct fs2_vocoder {
   fs2_vocoder_config cfg;
   int device = 0, cutoff = 0, cpad = 0, mpad = 0;
   bool loaded = false;
-  void* arena = nullptr;
+  void* arena = nullptr; size_t arena_bytes = 0;
   fs2::VWeight fwd, inv, mel;   // forward DFT [cpad][n_fft], inverse DFT [n_fft][cpad], mel pseudo-inverse [mpad][n_mels]
   float* win_sq = nullptr;
 };
@@ -290,9 +290,10 @@ int fs2_vocoder_load(fs2_vocoder* v, const float* w_forward, const float* w_inve
   v->fwd.N = v->cpad; v->fwd.K = nf;
   v->inv.N = nf; v->inv.K = v->cpad;
   v->mel.N = v->mpad; v->mel.K = v->cfg.n_mels;
-  int rc = arena_carve(&v->arena, st, [&](Bump& b) {
+  int rc = arena_carve(&v->arena, &v->arena_bytes, st, [&](Bump& b) {
     for (VWeight* w : {&v->fwd, &v->inv, &v->mel}) vweight_carve(b, *w, false);
     v->win_sq = b.floats(nf);
+    return FS2_OK;
   });
   if (rc) return rc;
   struct { const float* src; int sr, sc, tr; VWeight* w; } packs[3] = {

@@ -489,7 +489,7 @@ __global__ void melgan_bias_kernel(const float* __restrict__ b, const float* __r
 struct fs2_melgan_gen {
   int device = 0, math_mode = 0;
   bool loaded = false;
-  void* arena = nullptr;
+  void* arena = nullptr; size_t arena_bytes = 0;
   fs2::VWeight pre, up[fs2::kStages], dil[fs2::kStages][3], pair[fs2::kStages][3];
   float* post_w = nullptr;     // [7][32]
   float* post_b = nullptr;
@@ -715,10 +715,11 @@ int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float*
   }
   for (int j = 0; j < nj; ++j) { jobs[j].w->N = jobs[j].N; jobs[j].w->K = jobs[j].K; }
   m->loaded = false;
-  int rc = arena_carve(&m->arena, st, [&](Bump& b) {
+  int rc = arena_carve(&m->arena, &m->arena_bytes, st, [&](Bump& b) {
     for (int j = 0; j < nj; ++j) vweight_carve(b, *jobs[j].w, true);
     m->post_w = b.floats(kPostTaps * kPostC);
     m->post_b = b.floats(1);
+    return FS2_OK;
   });
   if (rc) return rc;
   for (int j = 0; j < nj; ++j) {

@@ -3,7 +3,7 @@
 // stage.  fp32 on CUDA cores, correctness first (the reference's training arithmetic is fp32): simple tiled kernels, each
 // citing the reference op whose autograd formula it implements.  The Python side (fastspeech2_b200/train.py) chains them
 // with torch.autograd.Function objects -- autograd is used for graph plumbing only, every number is produced here.
-#include "common.cuh"
+#include "vocoder_weights.cuh"
 
 namespace fs2 {
 namespace {
@@ -495,6 +495,27 @@ __global__ void loss_backward_kernel(const float* __restrict__ before, const flo
   }
 }
 
+// the bodies of fs2_conv_forward(_ex) and fs2_conv_dgrad(_ex) (see there); `who` names the entry in error messages
+int conv_forward(const char* who, int math_mode, const float* x, int B, int L, int K, const float* w, const float* bias, int N,
+                 int taps, int act, const float* resid, float* out, float* scratch, void* stream) {
+  FS2_REQUIRE(x && w && out && scratch, "%s: null argument", who);
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = pack_conv_weight(w, N, K, taps, nullptr, scratch, st);
+  if (rc) return rc;
+  VWeight pw; pw.w = scratch; pw.bias = const_cast<float*>(bias); pw.N = N; pw.K = K; pw.taps = taps;
+  return vweight_gemm(math_mode, pw, x, B, L, act, nullptr, out, st, resid);
+}
+int conv_dgrad(const char* who, int math_mode, const float* dy, int B, int L, int N, const float* w, int K, int taps, float* dx,
+               float* scratch, void* stream) {
+  FS2_REQUIRE(dy && w && dx && scratch, "%s: null argument", who);
+  FS2_REQUIRE(taps > 0 && (taps & 1) == 1, "%s: taps must be odd (got %d)", who, taps);
+  cudaStream_t st = (cudaStream_t)stream;
+  pack_dgrad_weight_kernel<<<grid_for((long)N * K * taps, 256), 256, 0, st>>>(w, N, K, taps, scratch);
+  FS2_LAUNCH_CHECK();
+  VWeight pw; pw.w = scratch; pw.N = K; pw.K = N; pw.taps = taps;   // dx = conv(dy, w flipped / transposed): K outputs from N inputs
+  return vweight_gemm(math_mode, pw, dy, B, L, ACT_NONE, nullptr, dx, st);
+}
+
 }  // namespace
 }  // namespace fs2
 
@@ -552,25 +573,10 @@ int fs2_colsum(const float* x, int64_t rows, int C, float* out, void* stream) {
  * scratch: >= N*K*taps floats */
 int fs2_conv_forward(const float* x, int B, int L, int K, const float* w, const float* bias, int N, int taps, int act, const float* resid,
                      float* out, float* scratch, void* stream) {
-  FS2_REQUIRE(x && w && out && scratch, "fs2_conv_forward: null argument");
-  cudaStream_t st = (cudaStream_t)stream;
-  int rc = pack_conv_weight(w, N, K, taps, nullptr, scratch, st);
-  if (rc) return rc;
-  TapGemm g;
-  g.x = x; g.ldx = K; g.B = B; g.L = L; g.K = K; g.w = scratch; g.bias = bias; g.N = N; g.taps = taps; g.act = act;
-  g.resid = resid; g.ldr = N; g.out = out; g.ldo = N;
-  return tap_gemm_fp32(g, st);
+  return conv_forward("fs2_conv_forward", FS2_MATH_FP32, x, B, L, K, w, bias, N, taps, act, resid, out, scratch, stream);
 }
 int fs2_conv_dgrad(const float* dy, int B, int L, int N, const float* w, int K, int taps, float* dx, float* scratch, void* stream) {
-  FS2_REQUIRE(dy && w && dx && scratch, "fs2_conv_dgrad: null argument");
-  FS2_REQUIRE(taps > 0 && (taps & 1) == 1, "fs2_conv_dgrad: taps must be odd (got %d)", taps);
-  cudaStream_t st = (cudaStream_t)stream;
-  pack_dgrad_weight_kernel<<<grid_for((long)N * K * taps, 256), 256, 0, st>>>(w, N, K, taps, scratch);
-  FS2_LAUNCH_CHECK();
-  TapGemm g;
-  g.x = dy; g.ldx = N; g.B = B; g.L = L; g.K = N; g.w = scratch; g.bias = nullptr; g.N = K; g.taps = taps; g.act = ACT_NONE;
-  g.resid = nullptr; g.ldr = 0; g.out = dx; g.ldo = K;
-  return tap_gemm_fp32(g, st);
+  return conv_dgrad("fs2_conv_dgrad", FS2_MATH_FP32, dy, B, L, N, w, K, taps, dx, scratch, stream);
 }
 /* the same with a math mode: FS2_MATH_FP32 is exactly the calls above; FS2_MATH_TF32 runs the packed weights through the
  * tap GEMM's tf32 family (gemm_tc.cu) */
@@ -578,28 +584,13 @@ int fs2_conv_forward_ex(const float* x, int B, int L, int K, const float* w, con
                         float* out, float* scratch, int math_mode, void* stream) {
   if (math_mode == FS2_MATH_FP32) return fs2_conv_forward(x, B, L, K, w, bias, N, taps, act, resid, out, scratch, stream);
   FS2_REQUIRE(math_mode == FS2_MATH_TF32, "fs2_conv_forward_ex: math_mode must be FS2_MATH_FP32 or FS2_MATH_TF32");
-  FS2_REQUIRE(x && w && out && scratch, "fs2_conv_forward_ex: null argument");
-  cudaStream_t st = (cudaStream_t)stream;
-  int rc = pack_conv_weight(w, N, K, taps, nullptr, scratch, st);
-  if (rc) return rc;
-  TapGemm g;
-  g.x = x; g.ldx = K; g.B = B; g.L = L; g.K = K; g.w = scratch; g.bias = bias; g.N = N; g.taps = taps; g.act = act;
-  g.resid = resid; g.ldr = N; g.out = out; g.ldo = N;
-  return tap_gemm_tf32(g, st);
+  return conv_forward("fs2_conv_forward_ex", math_mode, x, B, L, K, w, bias, N, taps, act, resid, out, scratch, stream);
 }
 int fs2_conv_dgrad_ex(const float* dy, int B, int L, int N, const float* w, int K, int taps, float* dx, float* scratch, int math_mode,
                       void* stream) {
   if (math_mode == FS2_MATH_FP32) return fs2_conv_dgrad(dy, B, L, N, w, K, taps, dx, scratch, stream);
   FS2_REQUIRE(math_mode == FS2_MATH_TF32, "fs2_conv_dgrad_ex: math_mode must be FS2_MATH_FP32 or FS2_MATH_TF32");
-  FS2_REQUIRE(dy && w && dx && scratch, "fs2_conv_dgrad_ex: null argument");
-  FS2_REQUIRE(taps > 0 && (taps & 1) == 1, "fs2_conv_dgrad_ex: taps must be odd (got %d)", taps);
-  cudaStream_t st = (cudaStream_t)stream;
-  pack_dgrad_weight_kernel<<<grid_for((long)N * K * taps, 256), 256, 0, st>>>(w, N, K, taps, scratch);
-  FS2_LAUNCH_CHECK();
-  TapGemm g;
-  g.x = dy; g.ldx = N; g.B = B; g.L = L; g.K = N; g.w = scratch; g.bias = nullptr; g.N = K; g.taps = taps; g.act = ACT_NONE;
-  g.resid = nullptr; g.ldr = 0; g.out = dx; g.ldo = K;
-  return tap_gemm_tf32(g, st);
+  return conv_dgrad("fs2_conv_dgrad_ex", math_mode, dy, B, L, N, w, K, taps, dx, scratch, stream);
 }
 int fs2_conv_wgrad(const float* dy, const float* x, int B, int L, int N, int K, int taps, float* dw, float* dbias, void* stream) {
   FS2_REQUIRE(dy && x && dw, "fs2_conv_wgrad: null argument");

@@ -1,4 +1,4 @@
-// The signal modules' GEMM weights (vocoder_weights.cuh).
+// The library's GEMM weights and tap-GEMM call (vocoder_weights.cuh).
 #include <string.h>
 
 #include "vocoder_weights.cuh"
@@ -42,20 +42,31 @@ int vweight_pack(VWeight& w, const float* src, int SR, int SC, int transpose, cu
   return vweight_planes(w, st);
 }
 
-int vweight_gemm(int math_mode, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens, float* out,
-                 cudaStream_t st, const float* resid, int dil, __half* outp) {
+TapGemm vweight_gemm_args(int math_mode, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens,
+                          float* out, const float* resid, int dil, __half* outp) {
   TapGemm g;
   memset(&g, 0, sizeof(g));
   g.B = B; g.L = L; g.K = w.K; g.N = w.N; g.taps = w.taps; g.dil = dil; g.act = act; g.out = out; g.ldo = w.N; g.lens = lens;
   g.w = w.w; g.bias = w.bias; g.resid = resid; g.ldr = w.N; g.a_inv = 1.0f; g.ldx = w.K;
   if (math_mode == FS2_MATH_FP32 || math_mode == FS2_MATH_TF32) {
     g.x = (const float*)a;
-    return math_mode == FS2_MATH_FP32 ? tap_gemm_fp32(g, st) : tap_gemm_tf32(g, st);
+    return g;
   }
   g.xp = (const __half*)a; g.w_hi = w.hi; g.w_lo = w.lo; g.w_inv = w.sc + 1; g.a_inv = kPlaneInv;
   g.precise = math_mode == FS2_MATH_3XTF32;
   if (outp) { g.outp = outp; g.ldo_p = w.N; g.outp_lo = g.precise; }
+  return g;
+}
+
+int tap_gemm(const TapGemm& g, int math_mode, cudaStream_t st) {
+  if (math_mode == FS2_MATH_FP32) return tap_gemm_fp32(g, st);
+  if (math_mode == FS2_MATH_TF32) return tap_gemm_tf32(g, st);
   return tap_gemm_planes(g, st);
+}
+
+int vweight_gemm(int math_mode, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens, float* out,
+                 cudaStream_t st, const float* resid, int dil, __half* outp) {
+  return tap_gemm(vweight_gemm_args(math_mode, w, a, B, L, act, lens, out, resid, dil, outp), math_mode, st);
 }
 
 }  // namespace fs2

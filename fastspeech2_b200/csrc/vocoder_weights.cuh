@@ -1,6 +1,7 @@
-// GEMM weights of the signal modules (melgan.cu, waveglow.cu, griffin_lim.cu, features.cu): one [taps][N][K] matrix held
-// as fp32 rows (fp32 / tf32 math modes) and as power-of-two-scaled fp16 hi / lo planes (f16 / 3xF16), with an optional
-// bias [N]; the tap-GEMM call over it; and the device arena a module's weights are carved from.
+// The library's GEMM weights (the acoustic model in api.cu, the train convolutions in train.cu and the signal modules
+// melgan.cu, waveglow.cu, griffin_lim.cu, features.cu): one [taps][N][K] matrix held as fp32 rows (fp32 / tf32 math modes)
+// and as power-of-two-scaled fp16 hi / lo planes (f16 / 3xF16), with an optional bias [N]; the tap-GEMM call over it, the
+// one place that maps a math mode to a tap-GEMM family; and the device arena a module's weights are carved from.
 #pragma once
 #include "operand_planes.cuh"
 
@@ -20,23 +21,37 @@ int vweight_planes(const VWeight& w, cudaStream_t st);
 // fill w's buffers from src [SR][SC] (its transpose when `transpose`), zero-padded to [N][K]: fp32 rows, scale, planes
 int vweight_pack(VWeight& w, const float* src, int SR, int SC, int transpose, cudaStream_t st);
 
-// out [B*L][w.N] = act(a [B*L][w.K] (w.taps taps at dilation dil) . w^T + w.bias) (+ resid [B*L][w.N]), a as fp32 rows
-// (fp32 / tf32) or as hi (+ lo) planes (f16 / 3xF16); rows t >= lens[b] are written as 0 (and skipped by the tensor-core
-// kernel).  outp (plane modes, nullable): the result's operand planes as well, with the lo plane in 3xF16
+// The TapGemm of out [B*L][w.N] = act(a [B*L][w.K] (w.taps taps at dilation dil) . w^T + w.bias) (+ resid [B*L][w.N]), a as
+// fp32 rows (fp32 / tf32) or as hi (+ lo) planes (f16 / 3xF16); rows t >= lens[b] are written as 0 (and skipped by the
+// tensor-core kernel).  outp (plane modes, nullable; ignored in the others): the result's operand planes as well, with the
+// lo plane in 3xF16
+TapGemm vweight_gemm_args(int math_mode, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens,
+                          float* out, const float* resid = nullptr, int dil = 1, __half* outp = nullptr);
+
+// runs g on the tap-GEMM family of math_mode
+int tap_gemm(const TapGemm& g, int math_mode, cudaStream_t st);
+
+// tap_gemm(vweight_gemm_args(...))
 int vweight_gemm(int math_mode, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens, float* out,
                  cudaStream_t st, const float* resid = nullptr, int dil = 1, __half* outp = nullptr);
 
-// (Re)allocates *arena for what carve(Bump&) places in it: carve runs on a counting Bump, the old arena is freed once the
-// stream has drained, and carve runs again on the new arena to set the pointers
+// (Re)allocates *arena (*cap bytes) for what carve(Bump&) places in it.  carve returns FS2_OK or an error code; it runs on a
+// counting Bump first, and an error there returns before anything is freed.  An arena already large enough is reused;
+// otherwise the old one is freed once the stream has drained and a new one allocated.  carve then runs again on the arena
+// to set the pointers.
 template <typename Carve>
-int arena_carve(void** arena, cudaStream_t st, Carve carve) {
+int arena_carve(void** arena, size_t* cap, cudaStream_t st, Carve carve) {
   Bump count(nullptr, 0);
-  carve(count);
-  if (*arena) { FS2_CUDA_CHECK(cudaStreamSynchronize(st)); FS2_CUDA_CHECK(cudaFree(*arena)); *arena = nullptr; }
-  FS2_CUDA_CHECK(cudaMalloc(arena, count.off + 256));
-  Bump b(*arena, (size_t)-1);
-  carve(b);
-  return FS2_OK;
+  int rc = carve(count);
+  if (rc) return rc;
+  const size_t need = count.off + 256;
+  if (need > *cap) {
+    if (*arena) { FS2_CUDA_CHECK(cudaStreamSynchronize(st)); FS2_CUDA_CHECK(cudaFree(*arena)); *arena = nullptr; *cap = 0; }
+    FS2_CUDA_CHECK(cudaMalloc(arena, need));
+    *cap = need;
+  }
+  Bump b(*arena, *cap);
+  return carve(b);
 }
 
 }  // namespace fs2

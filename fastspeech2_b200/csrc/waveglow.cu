@@ -386,7 +386,7 @@ struct WFlow {
 struct fs2_waveglow_net {
   int device = 0, math_mode = 0, C = 0;
   bool loaded = false;
-  void* arena = nullptr;
+  void* arena = nullptr; size_t arena_bytes = 0;
   fs2::VWeight up;
   fs2::WFlow flows[fs2::kFlows];
 };
@@ -411,8 +411,6 @@ struct WgPlan {
   void* acts;          // gate output [B * Ls][C] (fp32 rows or planes)
   float* skip[2];      // skip accumulator [B * Ls][C], ping-pong
 };
-
-bool plane_mode(int mode) { return mode == FS2_MATH_F16 || mode == FS2_MATH_3XTF32; }
 
 // buffers of L frames per utterance: the whole call's (L = Lmax) or a window's (window, L = n_frames + 2H)
 WgPlan plan(Bump& b, int mode, int C, int B, int L, bool window = false) {
@@ -598,7 +596,7 @@ int fs2_waveglow_load(fs2_waveglow_net* m, const float* const* t, int n, void* s
     }
   }
   m->loaded = false;
-  int rc = arena_carve(&m->arena, st, [&](Bump& b) {
+  int rc = arena_carve(&m->arena, &m->arena_bytes, st, [&](Bump& b) {
     for (int j = 0; j < nj; ++j) vweight_carve(b, *jobs[j].w, jobs[j].bsrc >= 0);
     for (int k = 0; k < kFlows; ++k) {
       WFlow& f = m->flows[k];
@@ -606,6 +604,7 @@ int fs2_waveglow_load(fs2_waveglow_net* m, const float* const* t, int n, void* s
       f.start_w = b.floats((size_t)C * h); f.start_b = b.floats(C);
       f.end_w = b.floats((size_t)c * C); f.end_b = b.floats(c); f.winv = b.floats((size_t)c * c);
     }
+    return FS2_OK;
   });
   if (rc) return rc;
   for (int j = 0; j < nj; ++j) {
