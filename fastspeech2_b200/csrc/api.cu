@@ -524,8 +524,8 @@ int fs2_encode_ex(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B,
   t_prof = &h->prof;
   Bump b(ws, ws_bytes);
   EncodePlan p = plan_encode(c, b, B, Tmax);
-  if (!b.ok()) { set_error("fs2_encode: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
-  int rc;
+  int rc = b.check("fs2_encode");
+  if (rc) return rc;
   // the encoder's output feeds round() in the duration predictor: exact fp32 FMA in FS2_MATH_FP32,
   // error-compensated 3xF16 on the tensor cores in every other mode (never a plain 10-bit-mantissa product)
   const bool planes = c.math_mode != FS2_MATH_FP32;
@@ -593,13 +593,13 @@ int fs2_decode_ctl(fs2_handle* h, const float* hm, const int64_t* olens, const f
   t_prof = &h->prof;
   Bump b(ws, ws_bytes);
   DecodePlan p = plan_decode(c, b, B, L);
-  if (!b.ok()) { set_error("fs2_decode: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
+  int rc = b.check("fs2_decode");
+  if (rc) return rc;
   const int mode = c.math_mode;
   const bool pred_planes = mode != FS2_MATH_FP32;                              // predictors: 3xF16 in every tensor-core mode
   const bool dec_planes = plane_mode(mode);                                    // decoder side on operand planes
   const bool x3 = mode == FS2_MATH_3XTF32;
   const int64_t* zlens = (flags & FS2_PER_UTTERANCE) ? olens : nullptr;   // hm rows past olens are zero (length_gather)
-  int rc;
   // energy / pitch predictors on the length-regulated states (fastspeech.py:195-196,214-216); fp32-class.  hm enters the
   // library as fp32 rows (the LengthRegulator is its own ABI stage), so this is the one operand pre-pass left in a step
   if (pred_planes) {

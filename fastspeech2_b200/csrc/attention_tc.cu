@@ -65,16 +65,6 @@ struct ACfg {
   static constexpr size_t SMEM = (Q_ELEMS + K_ELEMS + V_ELEMS) * sizeof(float);
 };
 
-__device__ __forceinline__ uint32_t to_tf32(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return r;
-}
-__device__ __forceinline__ void mma_tf32(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
 // rows [r0, r0 + nrows) x cols [0, ncols) of a global matrix (row pitch ld elements) -> shared (pitch lds); rows >= valid
 // and columns >= cvalid are zero (cvalid is a multiple of the vector width except at the very end of a row)
 template <int NCOLS>
@@ -149,7 +139,7 @@ attention_tc_kernel(AParams p) {
 #pragma unroll
       for (int n = 0; n < BKV / 8; ++n) {
         const float2 kb = *reinterpret_cast<const float2*>(Ks + (n * 8 + g) * LDQ + kk + 2 * tq);
-        mma_tf32(s[n], a, to_tf32(kb.x), to_tf32(kb.y));
+        mma_tf32(s[n], a[0], a[1], a[2], a[3], to_tf32(kb.x), to_tf32(kb.y));
       }
     }
 
@@ -191,7 +181,7 @@ attention_tc_kernel(AParams p) {
 #pragma unroll
       for (int j = 0; j < DK / 8; ++j) {
         const float2 vb = *reinterpret_cast<const float2*>(Vs + (j * 8 + g) * LDV + n * 8 + 2 * tq);
-        mma_tf32(o[j], a, to_tf32(vb.x), to_tf32(vb.y));
+        mma_tf32(o[j], a[0], a[1], a[2], a[3], to_tf32(vb.x), to_tf32(vb.y));
       }
     }
   }

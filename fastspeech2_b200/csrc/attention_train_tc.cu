@@ -39,6 +39,7 @@
 
 namespace fs2 {
 namespace {
+using namespace tc;
 
 constexpr int AT_TILE = 64;      // queries per forward / dQ CTA, keys per dK/dV CTA, keys per forward / dQ step
 constexpr int AT_QSTEP = 32;     // queries per dK/dV step
@@ -64,16 +65,7 @@ struct AttnParams {
   float *out, *lse_out, *dq, *dk, *dv;
 };
 
-__device__ __forceinline__ float rna(float v) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-  return __uint_as_float(r);
-}
 __device__ __forceinline__ uint32_t u(float v) { return __float_as_uint(v); }
-__device__ __forceinline__ void mma(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ void cp_async16(float* smem, const float* gmem, bool valid) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem), "r"(valid ? 16 : 0)
                : "memory");
@@ -160,13 +152,13 @@ __device__ __forceinline__ unsigned keep_frag_t(const Drop& d, unsigned long lon
   return bits;
 }
 
-// ---- prep: out = rna(in) on rows t < len of every utterance ----------------------------------------------------------------
+// ---- prep: out = in rounded to tf32 on rows t < len of every utterance ----------------------------------------------------
 __global__ void __launch_bounds__(256) attn_round_kernel(const float* __restrict__ in, const int64_t* __restrict__ lens, int L, int C, long n,
                                                          float* __restrict__ out) {
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
     const long row = i / C;
     const int b = (int)(row / L), t = (int)(row - (long)b * L);
-    if (t < clamp_len(lens, b, L)) out[i] = rna(in[i]);
+    if (t < clamp_len(lens, b, L)) out[i] = __uint_as_float(to_tf32(in[i]));
   }
 }
 
@@ -219,7 +211,7 @@ __global__ void __launch_bounds__(128, 1) attn_fwd_kernel(const AttnParams a) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const float* kb = sK + (8 * j + g) * SS + 8 * kk + t;
-        mma(s[j], a0, a1, a2, a3, u(kb[0]), u(kb[4]));
+        mma_tf32(s[j], a0, a1, a2, a3, u(kb[0]), u(kb[4]));
       }
     }
     __syncthreads();                                    // every warp is done with sK: prefetch the next K tile
@@ -258,7 +250,7 @@ __global__ void __launch_bounds__(128, 1) attn_fwd_kernel(const AttnParams a) {
         const float p = exp2f(s[j][e] - mu[e >> 1]);
         l[e >> 1] += p;
         const int bit = (e >> 1) * 2 + (e & 1);
-        s[j][e] = rna(a.drop.on ? (((kb >> bit) & 1) ? p * a.drop.keep_scale : 0.f) : p);
+        s[j][e] = __uint_as_float(to_tf32(a.drop.on ? (((kb >> bit) & 1) ? p * a.drop.keep_scale : 0.f) : p));
       }
     }
     cp_async_wait<1>();                                 // V(k0) landed; K(k0 + 64) may still be in flight
@@ -269,7 +261,7 @@ __global__ void __launch_bounds__(128, 1) attn_fwd_kernel(const AttnParams a) {
       const uint32_t a0 = u(s[j][0]), a1 = u(s[j][2]), a2 = u(s[j][1]), a3 = u(s[j][3]);
       const float* vb = sV + (8 * j + 2 * t) * SS + g;
 #pragma unroll
-      for (int n = 0; n < NT; ++n) mma(o[n], a0, a1, a2, a3, u(vb[8 * n]), u(vb[SS + 8 * n]));
+      for (int n = 0; n < NT; ++n) mma_tf32(o[n], a0, a1, a2, a3, u(vb[8 * n]), u(vb[SS + 8 * n]));
     }
     __syncthreads();                                    // every warp is done with sV: prefetch the next V tile
     if (k0 + AT_TILE < len) load_rows<DK>(sV, a.vr + ubase, C, k0 + AT_TILE, AT_TILE, len, threadIdx.x, 128);
@@ -378,8 +370,8 @@ __global__ void __launch_bounds__(256, 1) attn_dkdv_kernel(const AttnParams a) {
       for (int j = 0; j < 2; ++j) {
         const float* qb = sQ + (16 * qh + 8 * j + g) * SS + 8 * kk + t;
         const float* ob = sO + (16 * qh + 8 * j + g) * SS + 8 * kk + t;
-        mma(st[j], k_0, k_1, k_2, k_3, u(qb[0]), u(qb[4]));
-        mma(dp[j], v_0, v_1, v_2, v_3, u(ob[0]), u(ob[4]));
+        mma_tf32(st[j], k_0, k_1, k_2, k_3, u(qb[0]), u(qb[4]));
+        mma_tf32(dp[j], v_0, v_1, v_2, v_3, u(ob[0]), u(ob[4]));
       }
     }
 #pragma unroll
@@ -398,8 +390,8 @@ __global__ void __launch_bounds__(256, 1) attn_dkdv_kernel(const AttnParams a) {
           g_ = keep ? g_ * a.drop.keep_scale : 0.f;
         }
         const int at = (16 * kg + g + 8 * (e >> 1)) * AT_PS + ql;
-        sP[at] = rna(pd);
-        sS[at] = rna(p * (g_ - sD[ql]));
+        sP[at] = __uint_as_float(to_tf32(pd));
+        sS[at] = __uint_as_float(to_tf32(p * (g_ - sD[ql])));
       }
     }
     __syncthreads();
@@ -411,7 +403,7 @@ __global__ void __launch_bounds__(256, 1) attn_dkdv_kernel(const AttnParams a) {
       const uint32_t a0 = u(A[8 * kq]), a1 = u(A[8 * AT_PS + 8 * kq]), a2 = u(A[8 * kq + 4]), a3 = u(A[8 * AT_PS + 8 * kq + 4]);
       const float* bb = Bm + 8 * kq * SS;
 #pragma unroll
-      for (int n = 0; n < NT; ++n) mma(acc[n], a0, a1, a2, a3, u(bb[8 * n]), u(bb[4 * SS + 8 * n]));
+      for (int n = 0; n < NT; ++n) mma_tf32(acc[n], a0, a1, a2, a3, u(bb[8 * n]), u(bb[4 * SS + 8 * n]));
     }
   }
   const float mult = qh ? a.scale : 1.f;
@@ -484,7 +476,7 @@ __global__ void __launch_bounds__(128, 1) attn_dq_kernel(const AttnParams a) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const float* vb = sV + (8 * j + g) * SS + 8 * kk + t;
-        mma(dp[j], o_0, o_1, o_2, o_3, u(vb[0]), u(vb[4]));
+        mma_tf32(dp[j], o_0, o_1, o_2, o_3, u(vb[0]), u(vb[4]));
       }
     }
     __syncthreads();                                    // every warp is done with sV: prefetch the next V tile
@@ -499,7 +491,7 @@ __global__ void __launch_bounds__(128, 1) attn_dq_kernel(const AttnParams a) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const float* kb = sK + (8 * j + g) * SS + 8 * kk + t;
-        mma(s[j], q_0, q_1, q_2, q_3, u(kb[0]), u(kb[4]));
+        mma_tf32(s[j], q_0, q_1, q_2, q_3, u(kb[0]), u(kb[4]));
       }
     }
 #pragma unroll
@@ -513,7 +505,7 @@ __global__ void __launch_bounds__(128, 1) attn_dq_kernel(const AttnParams a) {
         const float p = valid ? exp2f(s[j][e] * a.sl2 - lse2[h]) : 0.f;
         float g_ = dp[j][e];
         if (a.drop.on) g_ = ((kb >> (2 * h + (e & 1))) & 1) ? g_ * a.drop.keep_scale : 0.f;
-        s[j][e] = rna(p * (g_ - dr[h]));
+        s[j][e] = __uint_as_float(to_tf32(p * (g_ - dr[h])));
       }
     }
     // dQ += dS . K, A column t <-> key 2t, t + 4 <-> key 2t + 1
@@ -522,7 +514,7 @@ __global__ void __launch_bounds__(128, 1) attn_dq_kernel(const AttnParams a) {
       const uint32_t a0 = u(s[j][0]), a1 = u(s[j][2]), a2 = u(s[j][1]), a3 = u(s[j][3]);
       const float* kb = sK + (8 * j + 2 * t) * SS + g;
 #pragma unroll
-      for (int n = 0; n < NT; ++n) mma(acc[n], a0, a1, a2, a3, u(kb[8 * n]), u(kb[SS + 8 * n]));
+      for (int n = 0; n < NT; ++n) mma_tf32(acc[n], a0, a1, a2, a3, u(kb[8 * n]), u(kb[SS + 8 * n]));
     }
     __syncthreads();                                    // every warp is done with sK: prefetch the next K tile
     if (k0 + AT_TILE < len) load_rows<DK>(sK, a.kr + ubase, C, k0 + AT_TILE, AT_TILE, len, threadIdx.x, 128);
@@ -553,8 +545,6 @@ struct AttnPlan {
   int dk, tiles;
   size_t plane, dvec_off, bytes;   // rounded copies at k * plane (k = 0..3: q, k, v, dO), D at dvec_off
 };
-
-uint64_t align256(uint64_t v) { return (v + 255) & ~(uint64_t)255; }
 
 int attn_plan(int B, int L, int C, int heads, AttnPlan* pl, const char* who) {
   FS2_REQUIRE(B >= 1 && L >= 1 && C >= 1 && heads >= 1, "%s: need B, L, C, heads >= 1", who);
@@ -602,8 +592,7 @@ AttnParams make_params(const AttnPlan& pl, const int64_t* lens, int L, int C, in
 
 int round_rows(const float* in, const int64_t* lens, int B, int L, int C, float* out, cudaStream_t st) {
   const long n = (long)B * L * C;
-  const long blocks = (n + 255) / 256;
-  attn_round_kernel<<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, st>>>(in, lens, L, C, n, out);
+  attn_round_kernel<<<grid_for(n, 256, 132 * 16), 256, 0, st>>>(in, lens, L, C, n, out);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }

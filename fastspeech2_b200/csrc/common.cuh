@@ -79,6 +79,7 @@ struct TapGemm {
   int dil = 1;                  // tap spacing in rows (dilated convolution); 0 (a memset TapGemm) counts as 1
 };
 int tap_gemm_fp32(const TapGemm& g, cudaStream_t st);
+constexpr long kTapGemmFp32MaxRows = 65535L * 128;     // tap_gemm_fp32 puts row tiles of 128 on grid.y (at most 65535)
 int tap_gemm_tf32(const TapGemm& g, cudaStream_t st);   // wgmma + TMA, tf32 on fp32 data (gemm_tc.cu)
 int tap_gemm_planes(const TapGemm& g, cudaStream_t st); // same kernel on fp16 operand planes: f16 or 3xF16 (g.precise)
 int split_f16(const float* src, __half* hi, __half* lo, long n, const float* scale /*device scalar or null*/, cudaStream_t st);
@@ -89,15 +90,28 @@ int planes_to_rows(const __half* planes, long n, float* out, cudaStream_t st);  
 int weight_scale(const float* w, long n, float* scale, float* inv, cudaStream_t st);
 constexpr int MATH_3XTF32 = FS2_MATH_3XTF32;            // also what the other tensor-core modes use for the encoder + predictors
 
+constexpr size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+
 // bump allocator over a caller-provided buffer (null: counting only, the size needed is `off`), 256-byte aligned carves
 struct Bump {
   char* base; size_t off = 0, cap;
   Bump(void* b, size_t c) : base((char*)b), cap(c) {}
-  void* bytes(size_t n) { size_t a = (off + 255) & ~(size_t)255; off = a + n; return base ? base + a : nullptr; }
+  void* bytes(size_t n) { size_t a = align256(off); off = a + n; return base ? base + a : nullptr; }
   float* floats(size_t n) { return (float*)bytes(n * sizeof(float)); }
   double* doubles(size_t n) { return (double*)bytes(n * sizeof(double)); }
-  bool ok() const { return base == nullptr || off <= cap; }
+  // FS2_ERR_WORKSPACE (error "<who>: workspace too small") when the carves overran the buffer
+  int check(const char* who) const {
+    if (base == nullptr || off <= cap) return FS2_OK;
+    set_error("%s: workspace too small (%zu < %zu)", who, cap, off);
+    return FS2_ERR_WORKSPACE;
+  }
 };
+
+// blocks of a grid-stride launch over n items: ceil(n / block), at least 1 and at most cap
+inline int grid_for(long n, int block, int cap = 132 * 8) {
+  long g = (n + block - 1) / block;
+  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+}
 
 // Row LayerNorm with the fusions the path needs.
 struct RowNorm {

@@ -38,11 +38,6 @@ constexpr double kLog2 = 0.69314718055994529;
 constexpr double kMaxValue = 100000.0;
 constexpr double kSafeGuard = 1e-12;
 
-inline int grid_for(long n, int block, int cap = 132 * 8) {
-  long g = (n + block - 1) / block;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 inline int matlab_round(double x) { return x > 0 ? (int)(x + 0.5) : (int)(x - 0.5); }
 
 // ---- mel and energy ------------------------------------------------------------------------------------------------
@@ -51,21 +46,6 @@ inline int matlab_round(double x) { return x > 0 ? (int)(x + 0.5) : (int)(x - 0.
 __device__ __forceinline__ int frames_of(const int64_t* __restrict__ lens, int b, int Nmax, int hop, int half) {
   const int64_t n = lens[b];
   return (n > half && n <= Nmax) ? (int)(n / hop) + 1 : 0;
-}
-
-// one pair of GEMM-operand values at element offset off (even) of a [rows][K] operand; plane = rows * K
-template <int OUT>
-__device__ __forceinline__ void store_operand(float v0, float v1, long off, float* __restrict__ out32, __half* __restrict__ outp, long plane) {
-  if (OUT == OUT_F32) {
-    *reinterpret_cast<float2*>(out32 + off) = make_float2(v0, v1);
-  } else if (OUT == OUT_HILO) {
-    uint32_t hi, lo;
-    split_pair(v0, v1, hi, lo);
-    *reinterpret_cast<uint32_t*>(outp + off) = hi;
-    *reinterpret_cast<uint32_t*>(outp + plane + off) = lo;
-  } else {
-    *reinterpret_cast<uint32_t*>(outp + off) = hi_pair(v0, v1);
-  }
 }
 
 // frames[row, k] = reflect_pad(x_b, n_fft/2)[t * hop + k] for t < T_b (rows past T_b are not written); flens[b] = T_b
@@ -94,7 +74,7 @@ __global__ void feat_frames_kernel(const float* __restrict__ wav, const int64_t*
       v[e] = wav[(long)b * Nmax + s];
     }
     if (!(fabsf(v[0]) <= 1.f && fabsf(v[1]) <= 1.f)) atomicOr(status, FS2_FEAT_RANGE);   // NaN included
-    store_operand<OUT>(v[0], v[1], row * n_fft + k, out32, outp, plane);
+    store_pair<OUT, RANGE_NEVER>(v[0], v[1], row * n_fft + k, out32, outp, plane, nullptr, 0);
   }
 }
 
@@ -124,7 +104,7 @@ __global__ void feat_magnitude_kernel(const float* __restrict__ z, int cpad, int
           acc += m[e] * m[e];
         }
       }
-      store_operand<OUT>(m[0], m[1], row * mpad + c, out32, outp, plane);
+      store_pair<OUT, RANGE_NEVER>(m[0], m[1], row * mpad + c, out32, outp, plane, nullptr, 0);
     }
     acc = warp_sum(acc);
     if (lane == 0) energy[row] = sqrtf(acc);
@@ -594,7 +574,7 @@ int fs2_features_workspace_bytes(fs2_features* f, int B, int Nmax, size_t* bytes
   Bump a(nullptr, 0), b(nullptr, 0);
   mel_plan(f, a, B, Nmax / f->cfg.hop + 1);
   dio_plan(f, b, B, Nmax);
-  *bytes = (((a.off > b.off ? a.off : b.off) + 255) & ~(size_t)255) + 256;
+  *bytes = align256(a.off > b.off ? a.off : b.off) + 256;
   return FS2_OK;
 }
 
@@ -607,7 +587,7 @@ int fs2_mel_energy(fs2_features* f, const float* wav, const int64_t* lens, int B
   const int T = Nmax / f->cfg.hop + 1, nf = f->cfg.n_fft, nm = f->cfg.n_mels, kind = out_kind(f->cfg.math_mode);
   Bump b(ws, ws_bytes);
   MelPlan p = mel_plan(f, b, B, T);
-  if (!b.ok()) { set_error("fs2_mel_energy: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
+  if ((rc = b.check("fs2_mel_energy"))) return rc;
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
   {
     auto k = pick(kind, feat_frames_kernel<OUT_HILO>, feat_frames_kernel<OUT_HI>, feat_frames_kernel<OUT_F32>);
@@ -637,7 +617,7 @@ int fs2_dio(fs2_features* f, const float* wav, const int64_t* lens, int B, int N
   const double fs = (double)f->cfg.sample_rate;
   Bump b(ws, ws_bytes);
   DioPlan p = dio_plan(f, b, B, Nmax);
-  if (!b.ok()) { set_error("fs2_dio: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
+  if ((rc = b.check("fs2_dio"))) return rc;
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
   dio_prepare_kernel<<<B, 256, 0, st>>>(wav, lens, Nmax, f->cfg.n_fft / 2, f->cfg.hop, f->cfg.sample_rate, f->frame_period, f->fft_extra,
                                         p.Tp, p.meta, plens, status);

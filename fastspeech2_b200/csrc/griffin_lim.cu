@@ -30,35 +30,10 @@ namespace {
 
 constexpr int FPB = 8;                                 // output frames per ola_frame CTA
 
-
-inline int grid_for(long n, int block, int cap = 132 * 8) {
-  long g = (n + block - 1) / block;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 // frames of utterance b that are processed; 0 for a length that fails the contract (reported by mel_expand)
 __device__ __forceinline__ int valid_len(const int64_t* __restrict__ olens, int b, int L, int hop, int half) {
   const int64_t n = olens[b];
   return (n >= 1 && n <= L && (n - 1) * hop > half) ? (int)n : 0;
-}
-
-// one pair of GEMM-operand values at element offset off (even) of a [rows][K] operand; plane_stride = rows * K
-template <int OUT>
-__device__ __forceinline__ void store_pair(float v0, float v1, long off, float* __restrict__ out32, __half* __restrict__ outp,
-                                           long plane_stride, int* __restrict__ status) {
-  if (OUT == OUT_F32) {
-    *reinterpret_cast<float2*>(out32 + off) = make_float2(v0, v1);
-    return;
-  }
-  if (!(fabsf(v0) <= kPlaneMax && fabsf(v1) <= kPlaneMax)) atomicOr(status, FS2_VOC_RANGE);   // saturation is reported, not hidden
-  if (OUT == OUT_HILO) {
-    uint32_t hi, lo;
-    split_pair(v0, v1, hi, lo);
-    *reinterpret_cast<uint32_t*>(outp + off) = hi;
-    *reinterpret_cast<uint32_t*>(outp + plane_stride + off) = lo;
-  } else {
-    *reinterpret_cast<uint32_t*>(outp + off) = hi_pair(v0, v1);
-  }
 }
 
 // exp(mels) as the mel GEMM's operand (K = n_mels); zero rows past the utterance.  Also checks olens.
@@ -77,7 +52,7 @@ __global__ void mel_expand_kernel(const float* __restrict__ mels, const int64_t*
       const float2 m = *reinterpret_cast<const float2*>(mels + row * n_mels + k);
       v0 = expf(m.x); v1 = expf(m.y);
     }
-    store_pair<OUT>(v0, v1, row * n_mels + k, out32, outp, plane, status);
+    store_pair<OUT, RANGE_ALWAYS>(v0, v1, row * n_mels + k, out32, outp, plane, status, FS2_VOC_RANGE);
   }
 }
 
@@ -127,7 +102,7 @@ __global__ void gl_project_kernel(const float* __restrict__ mag, int ldm, const 
         v[e] = mag[row * ldm + c] * (col < cutoff ? u.x : u.y);
       }
     }
-    store_pair<OUT>(v[0], v[1], row * cpad + j, out32, outp, plane, status);
+    store_pair<OUT, RANGE_ALWAYS>(v[0], v[1], row * cpad + j, out32, outp, plane, status, FS2_VOC_RANGE);
   }
 }
 
@@ -172,7 +147,8 @@ __global__ void __launch_bounds__(256) ola_frame_kernel(const float* __restrict_
   const int hp = n_fft / 2;
   for (int i = threadIdx.x; i < nf * hp; i += blockDim.x) {
     const int f = i / hp, k = (i - f * hp) * 2;
-    store_pair<OUT>(seg[f * hop + k], seg[f * hop + k + 1], (row0 + f0 + f) * n_fft + k, out32, outp, plane, status);
+    store_pair<OUT, RANGE_ALWAYS>(seg[f * hop + k], seg[f * hop + k + 1], (row0 + f0 + f) * n_fft + k, out32, outp, plane, status,
+                                  FS2_VOC_RANGE);
   }
 }
 
@@ -321,7 +297,7 @@ int fs2_mel_magnitude(fs2_vocoder* v, const float* mels, const int64_t* olens, i
   cudaStream_t st = (cudaStream_t)stream;
   Bump b(ws, ws_bytes);
   GlPlan p = plan(v, b, B, Lmax, false);
-  if (!b.ok()) { set_error("fs2_mel_magnitude: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
+  if ((rc = b.check("fs2_mel_magnitude"))) return rc;
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
   if ((rc = mel_stage(v, mels, olens, B, Lmax, p, status, st))) return rc;
   const long total = (long)B * v->cutoff * Lmax;
@@ -341,7 +317,7 @@ int fs2_griffin_lim(fs2_vocoder* v, const float* mels, const int64_t* olens, int
   const bool mom = momentum > 0.f;
   Bump b(ws, ws_bytes);
   GlPlan p = plan(v, b, B, Lmax, mom);
-  if (!b.ok()) { set_error("fs2_griffin_lim: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
+  if ((rc = b.check("fs2_griffin_lim"))) return rc;
   const int nf = v->cfg.n_fft, hop = v->cfg.hop, half = nf / 2, kind = out_kind(v->cfg.math_mode);
   const float mom_k = (float)((double)momentum / (1.0 + (double)momentum));
   const float scale = (float)nf / (float)hop;

@@ -45,12 +45,6 @@ constexpr int kLayers = 42;                          // convolutions, in state_d
 constexpr float kPadMel = -11.5129f;                 // value of the tail frames (seungwonpark/melgan `inference`)
 constexpr int kCin[kStages] = {512, 256, 128, 64}, kCout[kStages] = {256, 128, 64, 32}, kStride[kStages] = {8, 8, 2, 2};
 
-
-inline int grid_for(long n, int block, int cap = 132 * 8) {
-  long g = (n + block - 1) / block;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 __host__ __device__ constexpr int upsampling(int s) { return s == 0 ? 1 : s == 1 ? 8 : s == 2 ? 64 : s == 3 ? 128 : 256; }
 // ReflectionPad1d index map on [0, n) (edge sample not repeated); n exceeds every pad used here
 __device__ __forceinline__ int reflect(int i, int n) {
@@ -100,28 +94,6 @@ __device__ __forceinline__ Rows rows_of(const int64_t* __restrict__ win, const i
 // local row t holds the whole call's values: not within `margin` rows of a window side that is not an utterance edge
 __device__ __forceinline__ bool exact_row(const Rows& r, int t, int margin) {
   return (r.start == 0 || t >= margin) && (r.start + r.len == r.n || t < r.len - margin);
-}
-
-// four GEMM-operand values at element offset off (a multiple of 4) of a [rows][K] operand; plane = rows * K; status ==
-// nullptr: a halo row, not range-checked
-template <int OUT>
-__device__ __forceinline__ void store_quad(float4 v, long off, float* __restrict__ out32, __half* __restrict__ outp, long plane,
-                                           int* __restrict__ status) {
-  if (OUT == OUT_F32) {
-    *reinterpret_cast<float4*>(out32 + off) = v;
-    return;
-  }
-  if (status && !(fabsf(v.x) <= kPlaneMax && fabsf(v.y) <= kPlaneMax && fabsf(v.z) <= kPlaneMax && fabsf(v.w) <= kPlaneMax))
-    atomicOr(status, FS2_MELGAN_RANGE);                 // saturation is reported, not hidden
-  if (OUT == OUT_HILO) {
-    uint2 hi, lo;
-    split_pair(v.x, v.y, hi.x, lo.x);
-    split_pair(v.z, v.w, hi.y, lo.y);
-    *reinterpret_cast<uint2*>(outp + off) = hi;
-    *reinterpret_cast<uint2*>(outp + plane + off) = lo;
-  } else {
-    *reinterpret_cast<uint2*>(outp + off) = make_uint2(hi_pair(v.x, v.y), hi_pair(v.z, v.w));
-  }
 }
 
 // one CTA: lens[s][b] = (olens[b] + 10) * up_s for 1 <= olens[b] <= L, else 0 (the utterance is skipped); *status = 0 or
@@ -182,7 +154,7 @@ __global__ void melgan_pre_operand_kernel(const float* __restrict__ mels, const 
     float4 v = make_float4(kPadMel, kPadMel, kPadMel, kPadMel);
     if (src < r.n - kTail) v = *reinterpret_cast<const float4*>(mels + ((long)b * L + src) * kMels + c);
     v = make_float4((v.x + 5.f) / 5.f, (v.y + 5.f) / 5.f, (v.z + 5.f) / 5.f, (v.w + 5.f) / 5.f);
-    store_quad<OUT>(v, row * K + k, out32, outp, plane, status);
+    store_quad<OUT, RANGE_IF_STATUS>(v, row * K + k, out32, outp, plane, status, FS2_MELGAN_RANGE);
   }
 }
 
@@ -212,7 +184,8 @@ __device__ __forceinline__ void taps_loop(const float* __restrict__ x, const int
     }
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (in) v = lrelu4(*reinterpret_cast<const float4*>(x + ((long)b * ldx + src) * C + c));
-    store_quad<OUT>(v, row * K + k, out32, outp, plane, !WINDOW || exact_row(r, t, margin) ? status : nullptr);
+    store_quad<OUT, RANGE_IF_STATUS>(v, row * K + k, out32, outp, plane, !WINDOW || exact_row(r, t, margin) ? status : nullptr,
+                                     FS2_MELGAN_RANGE);
   }
 }
 
@@ -238,7 +211,7 @@ __global__ void melgan_concat_kernel(const float* __restrict__ h, const float* _
     const Rows r = rows_of(win, lens, B, b);
     if (t >= r.len) continue;
     const float4 v = k < C ? lrelu4(*reinterpret_cast<const float4*>(h + row * C + k)) : *reinterpret_cast<const float4*>(x + row * C + k - C);
-    store_quad<OUT>(v, row * K + k, out32, outp, plane, exact_row(r, t, margin) ? status : nullptr);
+    store_quad<OUT, RANGE_IF_STATUS>(v, row * K + k, out32, outp, plane, exact_row(r, t, margin) ? status : nullptr, FS2_MELGAN_RANGE);
   }
 }
 
@@ -654,22 +627,13 @@ int generate(const fs2_melgan_gen* m, const MgPlan& p, const float* mels, const 
 
 int check_size(const fs2_melgan_gen* m, int B, int L) {
   FS2_REQUIRE(B >= 1 && L >= 1, "fs2_melgan: need B >= 1 and Lmax >= 1 (got %d, %d)", B, L);
-  const long samples = (long)B * (L + kTail) * upsampling(kStages);
-  FS2_REQUIRE(samples < (1L << 31), "fs2_melgan: B * (Lmax + 10) * 256 = %ld sample rows exceed the int32 row index", samples);
-  // the CUDA-core GEMM puts row tiles of 128 on grid.y (at most 65535)
-  FS2_REQUIRE(m->math_mode != FS2_MATH_FP32 || samples <= 65535L * 128,
-              "fs2_melgan: B * (Lmax + 10) * 256 = %ld sample rows exceed fp32 mode's limit of %ld", samples, 65535L * 128);
-  return FS2_OK;
+  return check_rows("fs2_melgan", "B * (Lmax + 10) * 256", "sample", (long)B * (L + kTail) * upsampling(kStages), m->math_mode);
 }
 
 // a window's limits apply to its rows: the largest buffer, level 4, has B * level_rows(4, nf) rows
 int check_window(const fs2_melgan_gen* m, int B, int nf) {
   FS2_REQUIRE(B >= 1 && nf >= 1, "fs2_melgan_window: need B >= 1 and n_frames >= 1 (got %d, %d)", B, nf);
-  const long rows = (long)B * level_rows(kStages, nf);
-  FS2_REQUIRE(rows < (1L << 31), "fs2_melgan_window: B * (256 * n_frames + 36) = %ld window rows exceed the int32 row index", rows);
-  FS2_REQUIRE(m->math_mode != FS2_MATH_FP32 || rows <= 65535L * 128,
-              "fs2_melgan_window: B * (256 * n_frames + 36) = %ld window rows exceed fp32 mode's limit of %ld", rows, 65535L * 128);
-  return FS2_OK;
+  return check_rows("fs2_melgan_window", "B * (256 * n_frames + 36)", "window", (long)B * level_rows(kStages, nf), m->math_mode);
 }
 
 }  // namespace
@@ -755,7 +719,7 @@ int fs2_melgan(fs2_melgan_gen* m, const float* mels, const int64_t* olens, int B
   cudaStream_t st = (cudaStream_t)stream;
   Bump b(ws, ws_bytes);
   MgPlan p = plan(b, B, Lmax, false);
-  if (!b.ok()) { set_error("fs2_melgan: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
+  if ((rc = b.check("fs2_melgan"))) return rc;
   return generate(m, p, mels, olens, nullptr, B, Lmax, 0, audio, (long)Lmax * upsampling(kStages), status, st);
 }
 
@@ -781,7 +745,7 @@ int fs2_melgan_window(fs2_melgan_gen* m, const float* mels, const int64_t* olens
               (long long)audio_ld, (long)n_frames * upsampling(kStages));
   Bump b(ws, ws_bytes);
   MgPlan p = window_plan(b, B, n_frames);
-  if (!b.ok()) { set_error("fs2_melgan_window: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
+  if ((rc = b.check("fs2_melgan_window"))) return rc;
   FS2_REQUIRE(m->loaded, "fs2_melgan_window: weights not loaded (fs2_melgan_load)");
   return generate(m, p, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, (cudaStream_t)stream);
 }
@@ -803,7 +767,7 @@ int fs2_op_melgan_block(int math_mode, int route, int C, const float* x, const i
               "%s: x must be 16-byte and out 32-byte aligned", who);
   FS2_REQUIRE(B >= 1 && Lp >= 1 && d >= 1 && (long)Lp + d < (1L << 30), "%s: bad shape B=%d Lp=%d d=%d", who, B, Lp, d);
   const long rows = (long)B * Lp;
-  FS2_REQUIRE(rows * 3 * C < (1L << 31) && (math_mode != FS2_MATH_FP32 || rows <= 65535L * 128), "%s: too many rows (%ld)", who, rows);
+  FS2_REQUIRE(rows * 3 * C < (1L << 31) && (math_mode != FS2_MATH_FP32 || rows <= kTapGemmFp32MaxRows), "%s: too many rows (%ld)", who, rows);
   cudaStream_t st = (cudaStream_t)stream;
   const bool fused = route == 0 ? fused_blocks(math_mode, C) : route == 2;
   VWeight wd, wp;
@@ -840,7 +804,7 @@ int fs2_op_melgan_upsample(int math_mode, int Cin, int Cout, int s, const float*
               "%s: x must be 16-byte and out 32-byte aligned", who);
   FS2_REQUIRE(B >= 1 && Lin >= 1, "%s: bad shape B=%d Lin=%d", who, B, Lin);
   const long rows = (long)B * Lin;
-  FS2_REQUIRE(rows * s * Cout < (1L << 31) && rows * 3 * Cin < (1L << 31) && (math_mode != FS2_MATH_FP32 || rows <= 65535L * 128),
+  FS2_REQUIRE(rows * s * Cout < (1L << 31) && rows * 3 * Cin < (1L << 31) && (math_mode != FS2_MATH_FP32 || rows <= kTapGemmFp32MaxRows),
               "%s: too many rows (%ld)", who, rows);
   cudaStream_t st = (cudaStream_t)stream;
   VWeight wu;

@@ -278,11 +278,6 @@ __global__ void fold_batchnorm_kernel(const float* gamma, const float* beta, con
   shift[n] = beta[n] - mean[n] * s;
 }
 
-inline int grid_for(long n, int block, int cap = 132 * 8) {
-  long g = (n + block - 1) / block;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 }  // namespace
 
 int embed_posenc(const int64_t* xs, const float* table, int n_sym, const float* pe, const float* alpha, int B, int T,

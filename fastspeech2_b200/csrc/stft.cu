@@ -14,11 +14,6 @@
 namespace fs2 {
 namespace {
 
-inline int grid_for(long n, int block, int cap = 132 * 8) {
-  long g = (n + block - 1) / block;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 // frames[b, f, k] = xpad[b, f*hop + k], xpad = reflect-pad(x, n_fft/2) (utils/stft.py:89-95: F.pad(..., mode="reflect"))
 __global__ void stft_frames_kernel(const float* __restrict__ x, int n, int n_fft, int hop, int frames, long total, float* __restrict__ out) {
   const int half = n_fft / 2;

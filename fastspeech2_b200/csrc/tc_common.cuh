@@ -1,6 +1,6 @@
-// Inline-PTX building blocks shared by the Hopper tensor-core kernels (gemm_tc.cu, attention_tc.cu): mbarrier, TMA
-// (cp.async.bulk.tensor), wgmma (warpgroup MMA with both operands in shared memory), GMMA shared-memory
-// descriptors, and the host-side tensor-map encoder.  sm_90a.
+// Inline-PTX building blocks shared by the Hopper tensor-core kernels (gemm_tc.cu, attention_tc.cu, attention_train_tc.cu,
+// wgrad_tc.cu): mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with both operands in shared memory), GMMA
+// shared-memory descriptors, tf32 rounding and the warp-level tf32 mma.sync, and the host-side tensor-map encoder.  sm_90a.
 #pragma once
 #include <cuda.h>
 
@@ -140,6 +140,19 @@ __device__ __forceinline__ void wgmma_f16_rs_n128(float* d, const uint32_t* a, u
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
+}
+
+// ---- warp-level tf32 mma.sync ---------------------------------------------------------------------------------
+// x rounded to tf32 (nearest, ties away from zero), as the bits of an mma operand
+__device__ __forceinline__ uint32_t to_tf32(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return r;
+}
+// c[0..3] += A (16 x 8, row) . B (8 x 8, col), m16n8k8 with tf32 operands and fp32 accumulators
+__device__ __forceinline__ void mma_tf32(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
 // warp-specialised kernels: the producer warpgroup hands registers to the consumers (all warps of a warpgroup execute it)

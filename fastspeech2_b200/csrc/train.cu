@@ -8,11 +8,6 @@
 namespace fs2 {
 namespace {
 
-inline int grid_for(long n, int block, int cap = 132 * 8) {
-  long g = (n + block - 1) / block;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 // ---- dropout (torch.nn.Dropout in train mode: keep with prob 1-p, scale by 1/(1-p)) ---------------------------------------
 // Philox4x32-10 (common.cuh): mask byte i depends only on (seed, i), so the same mask is reproduced in backward without
 // storing random state; tests inject masks instead (shared with the reference run).

@@ -6,11 +6,6 @@
 namespace fs2 {
 namespace {
 
-inline int grid_for(long n, int block, int cap = 132 * 8) {
-  long g = (n + block - 1) / block;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 // dst [DR][DC] = src [SR][SC] (or its transpose), zero-padded
 __global__ void pad_pack_kernel(const float* __restrict__ src, int SR, int SC, int transpose, float* __restrict__ dst, int DR, int DC) {
   const long total = (long)DR * DC;
@@ -62,6 +57,13 @@ int tap_gemm(const TapGemm& g, int math_mode, cudaStream_t st) {
   if (math_mode == FS2_MATH_FP32) return tap_gemm_fp32(g, st);
   if (math_mode == FS2_MATH_TF32) return tap_gemm_tf32(g, st);
   return tap_gemm_planes(g, st);
+}
+
+int check_rows(const char* who, const char* formula, const char* noun, long rows, int math_mode) {
+  FS2_REQUIRE(rows < (1L << 31), "%s: %s = %ld %s rows exceed the int32 row index", who, formula, rows, noun);
+  FS2_REQUIRE(math_mode != FS2_MATH_FP32 || rows <= kTapGemmFp32MaxRows, "%s: %s = %ld %s rows exceed fp32 mode's limit of %ld", who,
+              formula, rows, noun, kTapGemmFp32MaxRows);
+  return FS2_OK;
 }
 
 int vweight_gemm(int math_mode, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens, float* out,

@@ -31,6 +31,10 @@ TapGemm vweight_gemm_args(int math_mode, const VWeight& w, const void* a, int B,
 // runs g on the tap-GEMM family of math_mode
 int tap_gemm(const TapGemm& g, int math_mode, cudaStream_t st);
 
+// The row limits of a call whose GEMMs have up to `rows` rows: below 2^31 (int32 row indices) and, in fp32, at most
+// kTapGemmFp32MaxRows.  The error reads "<who>: <formula> = <rows> <noun> rows exceed ...".
+int check_rows(const char* who, const char* formula, const char* noun, long rows, int math_mode);
+
 // tap_gemm(vweight_gemm_args(...))
 int vweight_gemm(int math_mode, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens, float* out,
                  cudaStream_t st, const float* resid = nullptr, int dil = 1, __half* outp = nullptr);

@@ -56,38 +56,11 @@ enum { kWinF, kWinS, kWinF0, kWinN, kWinCore0, kWinCoreN, kWinRows };
 
 __host__ __device__ inline int flow_channels(int k) { return k < 4 ? 8 : k < 8 ? 6 : 4; }
 
-inline int grid_for(long n, int block, int cap = 132 * 8) {
-  long g = (n + block - 1) / block;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 // local step row t of utterance b's window buffer holds the whole call's values: not within `margin` rows of a side that
 // is not an utterance edge
 __device__ __forceinline__ bool exact_row(const int64_t* __restrict__ win, int B, int b, int t, int margin) {
   const int64_t f0 = win[kWinF0 * B + b], nf = win[kWinF * B + b], ns = win[kWinS * B + b];
   return (f0 == 0 || t >= margin) && (f0 + nf == win[kWinN * B + b] || t < ns - margin);
-}
-
-// four GEMM-operand values at element offset off (a multiple of 4) of a [rows][K] operand; plane = rows * K; status ==
-// nullptr: a halo row, not range-checked
-template <int OUT>
-__device__ __forceinline__ void put_quad(float4 v, long off, float* __restrict__ out32, __half* __restrict__ outp, long plane,
-                                         int* __restrict__ status) {
-  if (OUT == OUT_F32) {
-    *reinterpret_cast<float4*>(out32 + off) = v;
-    return;
-  }
-  if (status && !(fabsf(v.x) <= kPlaneMax && fabsf(v.y) <= kPlaneMax && fabsf(v.z) <= kPlaneMax && fabsf(v.w) <= kPlaneMax))
-    atomicOr(status, FS2_WAVEGLOW_RANGE);               // saturation is reported, not hidden
-  if (OUT == OUT_HILO) {
-    uint2 hi, lo;
-    split_pair(v.x, v.y, hi.x, lo.x);
-    split_pair(v.z, v.w, hi.y, lo.y);
-    *reinterpret_cast<uint2*>(outp + off) = hi;
-    *reinterpret_cast<uint2*>(outp + plane + off) = lo;
-  } else {
-    *reinterpret_cast<uint2*>(outp + off) = make_uint2(hi_pair(v.x, v.y), hi_pair(v.z, v.w));
-  }
 }
 
 // one CTA: lensF[b] = olens[b], lensS[b] = olens[b] * 32 for 1 <= olens[b] <= L, else 0 (the utterance is skipped);
@@ -197,7 +170,7 @@ __global__ void wg_up_operand_kernel(const float* __restrict__ mels, const int64
     const int src = t - (kUpTaps - 1) + j + (win ? (int)win[kWinF0 * B + b] : 0), lim = win ? (int)win[kWinN * B + b] : n;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (src >= 0 && src < lim) v = *reinterpret_cast<const float4*>(mels + ((long)b * Lm + src) * kMels + c);
-    put_quad<OUT>(v, row * kUpK + k, out32, outp, plane, status);
+    store_quad<OUT, RANGE_IF_STATUS>(v, row * kUpK + k, out32, outp, plane, status, FS2_WAVEGLOW_RANGE);
   }
 }
 
@@ -212,7 +185,7 @@ __global__ void wg_planes_kernel(const float* __restrict__ x, const int64_t* __r
     const int b = (int)(row / Ls), t = (int)(row - (long)b * Ls);
     if (t >= (int)lens[b]) continue;
     const long off = row * K + (i - row * Q) * 4;
-    put_quad<OUT>(*reinterpret_cast<const float4*>(x + off), off, nullptr, outp, plane, status);
+    store_quad<OUT, RANGE_IF_STATUS>(*reinterpret_cast<const float4*>(x + off), off, nullptr, outp, plane, status, FS2_WAVEGLOW_RANGE);
   }
 }
 
@@ -243,7 +216,8 @@ __global__ void wg_start_kernel(const float* __restrict__ state, const int64_t* 
     }
     *reinterpret_cast<float4*>(x + row * C + n) = v;
     if (OUT != OUT_F32)
-      put_quad<OUT>(v, row * C + n, nullptr, xp, plane, !win || exact_row(win, B, b, t, margin) ? status : nullptr);
+      store_quad<OUT, RANGE_IF_STATUS>(v, row * C + n, nullptr, xp, plane, !win || exact_row(win, B, b, t, margin) ? status : nullptr,
+                                       FS2_WAVEGLOW_RANGE);
   }
 }
 
@@ -265,7 +239,8 @@ __global__ void wg_gate_kernel(const float* __restrict__ ia, const float* __rest
     const float4 g = *reinterpret_cast<const float4*>(ia + row * 2 * C + C + c);
     const float4 v = make_float4(tanhf(a.x) * (1.f / (1.f + expf(-g.x))), tanhf(a.y) * (1.f / (1.f + expf(-g.y))),
                                  tanhf(a.z) * (1.f / (1.f + expf(-g.z))), tanhf(a.w) * (1.f / (1.f + expf(-g.w))));
-    put_quad<OUT>(v, row * C + c, out32, outp, plane, !win || exact_row(win, B, b, t, margin) ? status : nullptr);
+    store_quad<OUT, RANGE_IF_STATUS>(v, row * C + c, out32, outp, plane, !win || exact_row(win, B, b, t, margin) ? status : nullptr,
+                                     FS2_WAVEGLOW_RANGE);
     if (xchk && (!win || exact_row(win, B, b, t, xmargin))) {
       const float4 x = *reinterpret_cast<const float4*>(xchk + row * C + c);
       if (!(fabsf(x.x) <= kPlaneMax && fabsf(x.y) <= kPlaneMax && fabsf(x.z) <= kPlaneMax && fabsf(x.w) <= kPlaneMax))
@@ -443,22 +418,14 @@ WgPlan plan(Bump& b, int mode, int C, int B, int L, bool window = false) {
 
 int check_size(const fs2_waveglow_net* m, int B, int L) {
   FS2_REQUIRE(B >= 1 && L >= 1, "fs2_waveglow: need B >= 1 and Lmax >= 1 (got %d, %d)", B, L);
-  const long rows = (long)B * L * kSteps;
-  FS2_REQUIRE(rows < (1L << 31), "fs2_waveglow: B * Lmax * 32 = %ld step rows exceed the int32 row index", rows);
-  // the CUDA-core GEMM puts row tiles of 128 on grid.y (at most 65535)
-  FS2_REQUIRE(m->math_mode != FS2_MATH_FP32 || rows <= 65535L * 128,
-              "fs2_waveglow: B * Lmax * 32 = %ld step rows exceed fp32 mode's limit of %ld", rows, 65535L * 128);
-  return FS2_OK;
+  return check_rows("fs2_waveglow", "B * Lmax * 32", "step", (long)B * L * kSteps, m->math_mode);
 }
 
 // a window's limits apply to its rows: B buffers of (n_frames + 2H) * 32 step rows
 int check_window(const fs2_waveglow_net* m, int B, int nf) {
   FS2_REQUIRE(B >= 1 && nf >= 1, "fs2_waveglow_window: need B >= 1 and n_frames >= 1 (got %d, %d)", B, nf);
-  const long rows = (long)B * ((long)nf + 2 * kHalo) * kSteps;
-  FS2_REQUIRE(rows < (1L << 31), "fs2_waveglow_window: B * (n_frames + 192) * 32 = %ld window rows exceed the int32 row index", rows);
-  FS2_REQUIRE(m->math_mode != FS2_MATH_FP32 || rows <= 65535L * 128,
-              "fs2_waveglow_window: B * (n_frames + 192) * 32 = %ld window rows exceed fp32 mode's limit of %ld", rows, 65535L * 128);
-  return FS2_OK;
+  return check_rows("fs2_waveglow_window", "B * (n_frames + 192) * 32", "window", (long)B * ((long)nf + 2 * kHalo) * kSteps,
+                    m->math_mode);
 }
 
 template <typename K>
@@ -673,7 +640,7 @@ int fs2_waveglow(fs2_waveglow_net* m, const float* mels, const int64_t* olens, i
   if (rc) return rc;
   Bump b(ws, ws_bytes);
   WgPlan p = plan(b, m->math_mode, m->C, B, Lmax);
-  if (!b.ok()) { set_error("fs2_waveglow: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
+  if ((rc = b.check("fs2_waveglow"))) return rc;
   return run(m, p, mels, olens, nullptr, B, Lmax, 0, sigma, seeds, z, audio, (long)Lmax * kHop, status, (cudaStream_t)stream);
 }
 
@@ -701,7 +668,7 @@ int fs2_waveglow_window(fs2_waveglow_net* m, const float* mels, const int64_t* o
               (long long)audio_ld, (long)n_frames * kHop);
   Bump b(ws, ws_bytes);
   WgPlan p = plan(b, m->math_mode, m->C, B, n_frames + 2 * kHalo, true);
-  if (!b.ok()) { set_error("fs2_waveglow_window: workspace too small (%zu < %zu)", ws_bytes, b.off); return FS2_ERR_WORKSPACE; }
+  if ((rc = b.check("fs2_waveglow_window"))) return rc;
   FS2_REQUIRE(m->loaded, "fs2_waveglow_window: weights not loaded (fs2_waveglow_load)");
   return run(m, p, mels, olens, starts, B, Lmax, n_frames, sigma, seeds, z, audio, (long)audio_ld, status, (cudaStream_t)stream);
 }

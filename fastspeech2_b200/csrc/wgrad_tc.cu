@@ -56,12 +56,6 @@ struct WgradParams {
   float* part;               // [splits][taps][N][K]
 };
 
-__device__ __forceinline__ float tf32_rna(float v) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-  return __uint_as_float(r);
-}
-
 // in [B][L][C] -> `copies` outputs [B][C][pitch] (copy stride cstride floats), rounded to tf32: copy r holds time t at
 // column t + shift + r, and zeros in columns [0, shift + r); columns past L + shift + r are not written.
 // One 32 x 32 tile per step.
@@ -78,7 +72,7 @@ __global__ void __launch_bounds__(256) transpose_tf32_kernel(const float* __rest
     const float* src = in + (long)b * L * C;
     for (int y = ty; y < 32; y += 8) {
       const int t = t0 + y, c = c0 + tx;
-      if (t < L && c < C) tile[y][tx] = tf32_rna(src[(long)t * C + c]);
+      if (t < L && c < C) tile[y][tx] = __uint_as_float(to_tf32(src[(long)t * C + c]));
     }
     __syncthreads();
     for (int r = 0; r < copies; ++r) {
@@ -217,7 +211,6 @@ struct WgradPlan {
 };
 
 bool mul_ok(uint64_t a, uint64_t b, uint64_t* r) { return !__builtin_mul_overflow(a, b, r); }
-uint64_t align256(uint64_t v) { return (v + 255) & ~(uint64_t)255; }
 
 // Shape -> decomposition and workspace layout; FS2_ERR_INVALID for a bad or overflowing size.  B * L == 0 plans nothing.
 int wgrad_plan(int B, int L, int N, int K, int taps, WgradPlan* pl, const char* who) {
@@ -291,8 +284,8 @@ int fs2_conv_wgrad_tc(const float* dy, const float* x, int B, int L, int N, int 
   float* xT = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ws) + pl.xT_off);
   const long xstride = (long)B * K * pl.Lx;      // floats between x^T phase copies
   auto transpose = [&](const float* in, int C_, int shift, int copies, long pitch, float* out) -> int {
-    const long tiles = (long)B * pl.cpu * ((C_ + 31) / 32);
-    transpose_tf32_kernel<<<(unsigned)(tiles < 132 * 16 ? tiles : 132 * 16), 256, 0, st>>>(in, B, L, C_, shift, copies, pitch, xstride, out);
+    const long tiles = (long)B * pl.cpu * ((C_ + 31) / 32);   // one 32 x 32 tile per block step
+    transpose_tf32_kernel<<<grid_for(tiles, 1, 132 * 16), 256, 0, st>>>(in, B, L, C_, shift, copies, pitch, xstride, out);
     FS2_LAUNCH_CHECK();
     return FS2_OK;
   };
@@ -310,9 +303,7 @@ int fs2_conv_wgrad_tc(const float* dy, const float* x, int B, int L, int N, int 
   const int grid = pl.units < sm_count_current() ? pl.units : sm_count_current();
   wgrad_tc_kernel<<<grid, WT_THREADS, WT_SMEM, st>>>(mdy, mx[0], mx[1], mx[2], mx[3], p);
   FS2_LAUNCH_CHECK();
-  const long tnk = (long)taps * N * K;
-  const long blocks = (tnk + 255) / 256;
-  wgrad_reduce_kernel<<<(unsigned)(blocks < 132 * 8 ? blocks : 132 * 8), 256, 0, st>>>(part, pl.splits, taps, N, K, dw);
+  wgrad_reduce_kernel<<<grid_for((long)taps * N * K, 256), 256, 0, st>>>(part, pl.splits, taps, N, K, dw);
   FS2_LAUNCH_CHECK();
   if (dbias) return fs2_colsum(dy, (int64_t)B * L, N, dbias, stream);
   return FS2_OK;
