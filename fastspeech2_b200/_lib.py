@@ -53,6 +53,11 @@ FS2_MELGAN_BAD_START = 4                          # and of fs2_melgan_window's
 FS2_WAVEGLOW_BAD_LENGTH, FS2_WAVEGLOW_RANGE = 1, 2   # bits of fs2_waveglow's device status word
 FS2_WAVEGLOW_BAD_START = 4                           # and of fs2_waveglow_window's
 
+class NoamAdamHp(C.Structure):
+    _fields_ = [(n, C.c_double) for n in ("rate_scale", "warmup_pow", "beta1", "beta2", "eps")]
+
+
+FS2_OPTIM_CHUNK = 65536                           # elements per chunk of the optimizer's parameter table
 _P, _I, _F, _L, _SZ = C.c_void_p, C.c_int, C.c_float, C.c_int64, C.c_size_t
 
 # name -> argtypes; every function returns int except the three noted below
@@ -150,6 +155,10 @@ SIGNATURES = {
     "fs2_peer_copy": [_P, _P, _SZ, _P],
     "fs2_flag_signal": [_P, _L, _P],
     "fs2_flag_wait": [_P, _I, _I, _L, _P],
+    "fs2_optim_ws_bytes": [_P, _I, C.POINTER(_SZ)],
+    "fs2_optim_noam_adam": [_P, _P, _I, C.POINTER(NoamAdamHp), _P, _P, _P, _SZ, _P],
+    "fs2_optim_clip_noam_adam": [_P, _P, _I, C.POINTER(NoamAdamHp), _F, _P, _P, _P, _P, _SZ, _P],
+    "fs2_optim_noam_scalars": [_L, _I, C.POINTER(NoamAdamHp), _P, _P, _P, _P],
 }
 OTHER_SYMBOLS = ("fs2_last_error", "fs2_version", "fs2_destroy", "fs2_kernel_launches", "fs2_profile_label", "fs2_vocoder_destroy",
                  "fs2_melgan_destroy", "fs2_waveglow_destroy", "fs2_features_destroy")

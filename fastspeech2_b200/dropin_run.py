@@ -13,6 +13,8 @@ With FS2_MELGAN_CHECKPOINT=<file> (seungwonpark/melgan's checkpoint, or a bare g
 inference.py and train_fastspeech.py reach MelGAN audio without a network.  With FS2_WAVEGLOW_CHECKPOINT=<file>
 (DeepLearningExamples' WaveGlow checkpoint) `torch.hub.load("nvidia/DeepLearningExamples:torchhub", "nvidia_waveglow",
 ...)` returns `WaveGlowVocoder.from_checkpoint(<file>)` in the same way.  Every other `torch.hub.load` call is passed on.
+With FS2_OPTIMIZER=fused, the checkout's `core.optimizer.get_std_opt` is replaced by `fastspeech2_b200.optim.get_std_opt`
+before the script runs, so train_fastspeech.py's optimizer step runs on the library's kernels.
 """
 from __future__ import annotations
 
@@ -25,6 +27,15 @@ MELGAN_ENV = "FS2_MELGAN_CHECKPOINT"
 MELGAN_REPO, MELGAN_MODEL = "seungwonpark/melgan", "melgan"
 WAVEGLOW_ENV = "FS2_WAVEGLOW_CHECKPOINT"
 WAVEGLOW_REPO, WAVEGLOW_MODEL = "nvidia/deeplearningexamples", "nvidia_waveglow"
+OPTIMIZER_ENV = "FS2_OPTIMIZER"
+
+
+def install_fused_optimizer() -> None:
+    """Serve `core.optimizer.get_std_opt` (imported from the script's checkout, first on sys.path) from
+    fastspeech2_b200.optim: same signature, NoamOpt's surface, the update on the library's kernels."""
+    import core.optimizer
+    from fastspeech2_b200 import optim
+    core.optimizer.get_std_opt = optim.get_std_opt
 
 
 def install_melgan_hub(checkpoint: str) -> None:
@@ -84,6 +95,11 @@ def main(argv=None) -> None:
         install_melgan_hub(os.environ[MELGAN_ENV])
     if os.environ.get(WAVEGLOW_ENV):
         install_waveglow_hub(os.environ[WAVEGLOW_ENV])
+    mode = os.environ.get(OPTIMIZER_ENV, "")
+    if mode == "fused":
+        install_fused_optimizer()
+    elif mode not in ("", "torch"):
+        raise SystemExit(f"{OPTIMIZER_ENV}={mode!r}: expected 'fused' or 'torch'")
     runpy.run_path(script, run_name="__main__")
 
 

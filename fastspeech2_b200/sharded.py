@@ -248,6 +248,8 @@ class GradientSync:
         loss.backward()
         sync.all_reduce()                   # ONE collective over the whole bucket (NCCL ring / NVLS over NVLink), mean over ranks
         clip_grad_norm_(...); optimizer.step(); sync.zero_grad()
+        # or, with fastspeech2_b200.optim.NoamAdam (the grads stay views of the bucket):
+        norm = optimizer.clip_and_step(grad_clip); sync.zero_grad()
 
     The whole model is 35 M parameters = 141 MB of fp32 gradients: one bucket, one launch -- with NVSwitch the cost is
     launch latency plus bytes, so splitting into DDP-style 25 MB buckets buys nothing once backward has finished, and

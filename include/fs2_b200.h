@@ -593,6 +593,47 @@ int fs2_peer_copy(void* dst, const void* src, size_t bytes, void* stream);
 int fs2_flag_signal(int64_t* flag, int64_t value, void* stream);
 int fs2_flag_wait(const int64_t* flags, int n, int skip, int64_t value, void* stream);
 
+/* ---- optimizer step: Noam-scheduled Adam, gradient-norm clipping and the NaN guard (DESIGN.md section 15) --------- */
+/* Replaces the reference loop's `clip_grad_norm_(model.parameters(), grad_clip); if isnan(norm): skip; NoamOpt.step()`
+ * (train_fastspeech.py:117-124, core/optimizer.py) with Adam(betas, eps, weight_decay=0) arithmetic bit-identical to
+ * torch's foreach Adam.  fastspeech2_b200/optim.py::NoamAdam drives these.
+ *
+ * The parameter table is an array of entries in DEVICE memory, built by the caller: one per parameter that has a
+ * gradient.  Entry t covers chunks [chunk0, chunk0 + ceil(numel / FS2_OPTIM_CHUNK)) with chunk0 the running sum of the
+ * chunk counts of the entries before it; `numel` (HOST, n entries) repeats the sizes so that the call can check them and
+ * size its grid.  Any numel >= 1 and any 4-byte aligned pointer are valid (16-byte vectors where the four arrays of an
+ * entry share their alignment).  `step` is the entry's Adam step count (fp32, as torch keeps it).
+ *
+ * Workspace (caller-owned, 256-byte aligned, size from fs2_optim_ws_bytes):
+ *   align256(8 n_chunks) + align256(8 n) + align256(16)  bytes  (fp64 chunk sums of squares; per-entry step size and
+ *   bias-correction root; norm, coefficient, skip flag).
+ * Device state (caller-owned): noam_step (int64, NoamOpt._step), lr (double, the lr of the last step that ran).
+ *   fs2_optim_noam_adam       noam_step += 1, lr = rate(noam_step), every entry's step += 1, one Adam update
+ *   fs2_optim_clip_noam_adam  total norm of the grads (fp64 chunk sums, fixed-order reduction, one rounding to fp32) into
+ *                             *norm, coefficient min(max_norm * (1 / (norm + 1e-6)), 1); NaN norm: nothing else changes;
+ *                             otherwise the update above on grad * coefficient (the grads themselves are not written)
+ *   fs2_optim_noam_scalars    test entry: lr, fp32 step size and fp32 bias-correction root for steps step0 .. step0+count-1
+ * Three (clip) or two kernels, no allocation, no synchronisation: graph-capturable.  An empty table, numel < 1, a
+ * chunk count past 2^31 - 1, a null pointer or a short / misaligned workspace are FS2_ERR_INVALID. */
+#define FS2_OPTIM_CHUNK 65536
+typedef struct fs2_optim_entry {
+  float* param; const float* grad; float* exp_avg; float* exp_avg_sq; float* step;
+  int64_t numel; int64_t chunk0;
+} fs2_optim_entry;
+typedef struct fs2_noam_adam_hp {
+  double rate_scale;   /* factor * model_size ** -0.5, computed by the caller as NoamOpt.rate groups it */
+  double warmup_pow;   /* warmup ** -1.5 */
+  double beta1, beta2, eps;
+} fs2_noam_adam_hp;
+int fs2_optim_ws_bytes(const int64_t* numel, int n, size_t* bytes);
+int fs2_optim_noam_adam(const fs2_optim_entry* table, const int64_t* numel, int n, const fs2_noam_adam_hp* hp,
+                        int64_t* noam_step, double* lr, void* ws, size_t ws_bytes, void* stream);
+int fs2_optim_clip_noam_adam(const fs2_optim_entry* table, const int64_t* numel, int n, const fs2_noam_adam_hp* hp,
+                             float max_norm, int64_t* noam_step, double* lr, float* norm, void* ws, size_t ws_bytes,
+                             void* stream);
+int fs2_optim_noam_scalars(int64_t step0, int count, const fs2_noam_adam_hp* hp, double* lr, float* step_size,
+                           float* bc2_sqrt, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
