@@ -52,6 +52,18 @@ FS2_MELGAN_BAD_LENGTH, FS2_MELGAN_RANGE = 1, 2   # bits of fs2_melgan's device s
 FS2_MELGAN_BAD_START = 4                          # and of fs2_melgan_window's
 FS2_WAVEGLOW_BAD_LENGTH, FS2_WAVEGLOW_RANGE = 1, 2   # bits of fs2_waveglow's device status word
 FS2_WAVEGLOW_BAD_START = 4                           # and of fs2_waveglow_window's
+FS2_HIFIGAN_BAD_LENGTH, FS2_HIFIGAN_RANGE = 1, 2     # bits of fs2_hifigan's device status word
+FS2_HIFIGAN_MAX_UPSAMPLES, FS2_HIFIGAN_MAX_KERNELS = 8, 8
+
+
+class HiFiGANConfig(C.Structure):
+    _fields_ = [("resblock", C.c_int32), ("num_upsamples", C.c_int32),
+                ("upsample_rates", C.c_int32 * FS2_HIFIGAN_MAX_UPSAMPLES),
+                ("upsample_kernel_sizes", C.c_int32 * FS2_HIFIGAN_MAX_UPSAMPLES),
+                ("upsample_initial_channel", C.c_int32), ("num_kernels", C.c_int32),
+                ("resblock_kernel_sizes", C.c_int32 * FS2_HIFIGAN_MAX_KERNELS), ("num_dilations", C.c_int32),
+                ("resblock_dilation_sizes", (C.c_int32 * 4) * FS2_HIFIGAN_MAX_KERNELS)]
+
 
 class NoamAdamHp(C.Structure):
     _fields_ = [(n, C.c_double) for n in ("rate_scale", "warmup_pow", "beta1", "beta2", "eps")]
@@ -141,6 +153,12 @@ SIGNATURES = {
     "fs2_melgan_window": [_P, _P, _P, _P, _I, _I, _I, _P, _L, _P, _P, _SZ, _P],
     "fs2_op_melgan_block": [_I, _I, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P],
     "fs2_op_melgan_upsample": [_I, _I, _I, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P],
+    "fs2_hifigan_create": [C.POINTER(_P), _I, C.POINTER(HiFiGANConfig)],
+    "fs2_hifigan_load": [_P, C.POINTER(_P), C.POINTER(_P), _P],
+    "fs2_hifigan_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_hifigan": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_op_hifigan_resblock": [_I, _I, _I, _I, _I, C.POINTER(_I), _P, _P, _I, _I, C.POINTER(_P), C.POINTER(_P), _P, _P, _P],
+    "fs2_op_hifigan_upsample": [_I, _I, _I, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P],
     "fs2_waveglow_create": [C.POINTER(_P), _I, _I],
     "fs2_waveglow_load": [_P, C.POINTER(_P), _I, _P],
     "fs2_waveglow_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
@@ -161,7 +179,7 @@ SIGNATURES = {
     "fs2_optim_noam_scalars": [_L, _I, C.POINTER(NoamAdamHp), _P, _P, _P, _P],
 }
 OTHER_SYMBOLS = ("fs2_last_error", "fs2_version", "fs2_destroy", "fs2_kernel_launches", "fs2_profile_label", "fs2_vocoder_destroy",
-                 "fs2_melgan_destroy", "fs2_waveglow_destroy", "fs2_features_destroy")
+                 "fs2_melgan_destroy", "fs2_waveglow_destroy", "fs2_features_destroy", "fs2_hifigan_destroy")
 ALL_SYMBOLS = tuple(SIGNATURES) + OTHER_SYMBOLS
 
 _lib: Optional[C.CDLL] = None
@@ -199,6 +217,8 @@ def load() -> C.CDLL:
     lib.fs2_waveglow_destroy.argtypes = [_P]
     lib.fs2_features_destroy.restype = None
     lib.fs2_features_destroy.argtypes = [_P]
+    lib.fs2_hifigan_destroy.restype = None
+    lib.fs2_hifigan_destroy.argtypes = [_P]
     _lib = lib
     return lib
 

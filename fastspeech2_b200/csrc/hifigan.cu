@@ -1,0 +1,551 @@
+// Batched HiFi-GAN vocoder (DESIGN.md section 16): log-mels [B, Lmax, 80] -> audio [B, Lmax * 256], each utterance
+// jik876/hifi-gan's Generator over its own olens[b] frames, on the library's tap-GEMM.
+//
+// Stage s (s = 0 .. U, U = num_upsamples) has Lp_s = Lmax * up_s rows per utterance (up_0 = 1, up_{s+1} = up_s * u_s) of
+// C_s = C0 / 2^s channels, and every GEMM of the stage runs with TapGemm::lens = lens_s = olens * up_s: row tiles wholly past
+// an utterance are skipped and padded rows come out as exact zeros.  Every convolution is "same" with zero padding at the
+// utterance's own edges, which is exactly what the tap GEMM's native taps give when the operand's rows past lens_s are
+// zeros: the TMA unit zero-fills rows outside [0, Lp_s), and the producers below write every row, +0 past lens_s.
+//
+//   mel operand   mel rows (0 past olens)                                       -> GEMM 7 taps, 80 -> C0    = conv_pre
+//   per stage s:
+//     act         lrelu(x, 0.1), x = the previous MRF's ((r0 + r1) + ...) / nk   -> GEMM 3 taps, C_s -> u C_{s+1}: the
+//                 ConvTranspose1d(k = 2u, stride u, pad u / 2) as a polyphase GEMM.  Output row t's u phases, written
+//                 row-major, are rows u t .. u t + u - 1 of the next stage; phase r < u/2 reads input rows {t-1, t}, r >= u/2
+//                 reads {t, t+1}, and the third tap of each phase has zero weights.  Native taps rather than MelGAN's
+//                 producer-stacked K = 3 Cin operand: the producer writes Cin values per row instead of 3 Cin, and the
+//                 operand is the same lrelu rows every block convolution reads.
+//     per resblock j of the MRF, per conv step m (ResBlock1: x = c2(lrelu(c1(lrelu(x)))) + x; ResBlock2: x = c(lrelu(x)) + x):
+//                 act lrelu(x) -> GEMM k taps at dilation d_m (-> act -> GEMM k taps, dilation 1), the residual add in the
+//                 last GEMM's epilogue (TapGemm::resid)
+//     add         S += r_j for the middle resblocks (1 .. nk - 2): the MRF sum in hifi-gan's order
+//   post          lrelu((S + r_last) / nk, 0.01), conv C -> 1 (k = 7, zero padding), tanh, on CUDA cores, +0 past olens * 256
+//
+// Launches per call: 4 + U * (2 + nk * G + max(nk - 2, 0)), G = 12 (ResBlock1: 3 steps of 2 producers + 2 GEMMs) or 4
+// (ResBlock2: 2 steps of 1 + 1), in every math mode: 160 for V1, 49 for V3.
+//
+// Buffers, each [B * Lp_s][C_s] at the current stage, so A floats per frame with A = max_s up_s * C_s (8192 for V1 and V3):
+// xu (the upsampling output every resblock of the MRF reads), S (r0, then the running sum), two chain buffers T0 / T1 (a
+// resblock's intermediate x and h; the last resblock ends in one of them, which the next producer combines with S), and the
+// GEMM operand (fp32 rows, or hi + lo fp16 planes: the same bytes).  5 * 4 * A bytes per frame of B * Lmax: 163,840 for V1
+// and V3.
+//
+// A GEMM row depends only on its own utterance's input rows, in a fixed K order, and every producer reads rows of its own
+// utterance below lens_s only, so per-utterance results do not depend on the batch.
+#include <math.h>
+
+#include <algorithm>
+#include <vector>
+
+#include "vocoder_weights.cuh"
+
+namespace fs2 {
+namespace {
+
+constexpr int kMels = 80, kHop = 256, kPreTaps = 7, kPostTaps = 7, kMaxUps = FS2_HIFIGAN_MAX_UPSAMPLES;
+constexpr float kSlope = 0.1f, kPostSlope = 0.01f;   // hifi-gan's LRELU_SLOPE, and F.leaky_relu's default before conv_post
+
+__device__ __forceinline__ float lrelu(float v, float s) { return v > 0.f ? v : v * s; }
+
+struct Ups { int n; int up[kMaxUps + 1]; };   // cumulative upsampling of stages 0 .. n
+
+// one CTA: lens[s][b] = olens[b] * up_s for 1 <= olens[b] <= L, else 0 (the utterance is skipped); *status = 0 or
+// FS2_HIFIGAN_BAD_LENGTH.  Runs first, so the producers' range bits land on a cleared word.
+__global__ void hifigan_prep_kernel(const int64_t* __restrict__ olens, int B, int L, Ups ups, int64_t* __restrict__ lens,
+                                    int* __restrict__ status) {
+  __shared__ int bad;
+  if (threadIdx.x == 0) bad = 0;
+  __syncthreads();
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    const int64_t n = olens[b];
+    const bool ok = n >= 1 && n <= L;
+    if (!ok) atomicOr(&bad, FS2_HIFIGAN_BAD_LENGTH);
+    for (int s = 0; s <= ups.n; ++s) lens[(long)s * B + b] = ok ? n * ups.up[s] : 0;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) *status = bad;
+}
+
+// conv_pre's operand [B * L][80]: mel frame t of utterance b for t < lens[b], +0 past it (frames past olens[b] are never read)
+template <int OUT>
+__global__ void hifigan_mel_operand_kernel(const float* __restrict__ mels, const int64_t* __restrict__ lens, int B, int L,
+                                           float* __restrict__ out32, __half* __restrict__ outp, int* __restrict__ status) {
+  constexpr int Q = kMels / 4;
+  const long rows = (long)B * L, total = rows * Q, plane = rows * kMels;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const long row = i / Q;
+    const int b = (int)(row / L), t = (int)(row - (long)b * L);
+    const long off = row * kMels + (i - row * Q) * 4;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (t < lens[b]) v = *reinterpret_cast<const float4*>(mels + off);
+    store_quad<OUT, RANGE_IF_STATUS>(v, off, out32, outp, plane, status, FS2_HIFIGAN_RANGE);
+  }
+}
+
+// a GEMM operand [B * Lp][C] = lrelu(v, 0.1) with v = x, or the MRF combine v = (x + r) / nk (r nullable: x / nk), for
+// t < lens[b]; +0 past it.  Every row is written: the next GEMM's taps read rows past lens[b] as its zero padding.
+template <int OUT>
+__global__ void hifigan_act_kernel(const float* __restrict__ x, const float* __restrict__ r, int nk, const int64_t* __restrict__ lens,
+                                   int B, int Lp, int C, float* __restrict__ out32, __half* __restrict__ outp, int* __restrict__ status) {
+  const int Q = C / 4;
+  const long rows = (long)B * Lp, total = rows * Q, plane = rows * C;
+  const float fk = (float)nk;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const long row = i / Q;
+    const int b = (int)(row / Lp), t = (int)(row - (long)b * Lp);
+    const long off = row * C + (i - row * Q) * 4;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (t < lens[b]) {
+      v = *reinterpret_cast<const float4*>(x + off);
+      if (r) {
+        const float4 w = *reinterpret_cast<const float4*>(r + off);
+        v = make_float4(v.x + w.x, v.y + w.y, v.z + w.z, v.w + w.w);
+      }
+      if (nk != 1) v = make_float4(v.x / fk, v.y / fk, v.z / fk, v.w / fk);
+      v = make_float4(lrelu(v.x, kSlope), lrelu(v.y, kSlope), lrelu(v.z, kSlope), lrelu(v.w, kSlope));
+    }
+    store_quad<OUT, RANGE_IF_STATUS>(v, off, out32, outp, plane, status, FS2_HIFIGAN_RANGE);
+  }
+}
+
+// s[i] += r[i] over n floats (n a multiple of 4): the MRF's running sum; rows past lens are +0 in both
+__global__ void hifigan_add_kernel(float* __restrict__ s, const float* __restrict__ r, long n) {
+  for (long i = ((long)blockIdx.x * blockDim.x + threadIdx.x) * 4; i < n; i += (long)gridDim.x * blockDim.x * 4) {
+    float4 a = *reinterpret_cast<const float4*>(s + i);
+    const float4 b = *reinterpret_cast<const float4*>(r + i);
+    *reinterpret_cast<float4*>(s + i) = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+  }
+}
+
+// audio[b, t] = tanh(bias + sum_j sum_c w[j][c] lrelu(x[t + j - 3][c], 0.01)) for t < lens[b], else +0, where x = (S + R) / nk
+// (R nullable) is the last MRF's output, 0 outside [0, lens[b]).  w: [7][C] in dynamic shared memory.
+__global__ void __launch_bounds__(256) hifigan_post_kernel(const float* __restrict__ S, const float* __restrict__ R, int nk,
+                                                           const int64_t* __restrict__ lens, int B, int Lp, int C,
+                                                           const float* __restrict__ w, const float* __restrict__ bias,
+                                                           float* __restrict__ audio) {
+  extern __shared__ __align__(16) float ws[];
+  for (int i = threadIdx.x; i < kPostTaps * C; i += blockDim.x) ws[i] = w[i];
+  __syncthreads();
+  const float b0 = __ldg(bias), fk = (float)nk;
+  const long total = (long)B * Lp;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int b = (int)(i / Lp), t = (int)(i - (long)b * Lp), n = (int)lens[b];
+    float y = 0.f;
+    if (t < n) {
+      float acc = b0;
+#pragma unroll 1
+      for (int j = 0; j < kPostTaps; ++j) {
+        const int src = t + j - kPostTaps / 2;
+        if (src < 0 || src >= n) continue;
+        const long row = ((long)b * Lp + src) * C;
+        for (int q = 0; q < C / 4; ++q) {
+          float4 v = __ldg(reinterpret_cast<const float4*>(S + row) + q);
+          if (R) {
+            const float4 r = __ldg(reinterpret_cast<const float4*>(R + row) + q);
+            v = make_float4(v.x + r.x, v.y + r.y, v.z + r.z, v.w + r.w);
+          }
+          if (nk != 1) v = make_float4(v.x / fk, v.y / fk, v.z / fk, v.w / fk);
+          const float4 wv = *reinterpret_cast<const float4*>(ws + j * C + 4 * q);
+          acc = fmaf(wv.x, lrelu(v.x, kPostSlope), acc);
+          acc = fmaf(wv.y, lrelu(v.y, kPostSlope), acc);
+          acc = fmaf(wv.z, lrelu(v.z, kPostSlope), acc);
+          acc = fmaf(wv.w, lrelu(v.w, kPostSlope), acc);
+        }
+      }
+      y = tanhf(acc);
+    }
+    audio[i] = y;
+  }
+}
+
+// GEMM weight [taps][N][K] from a folded torch-layout weight:
+//   kind 0  Conv1d w [N][K][taps]               -> dst[j][n][c] = w[n][c][j]
+//   kind 1  ConvTranspose1d w [K][Cout][2u]     -> dst[j][r Cout + co][ci] = w[ci][co][k(r, j)], taps = 3, tap j reading input
+//           row t + j - 1 (0 where phase r does not read it): k = r + u/2 + u (j = 0), r + u/2 (j = 1) for r < u/2;
+//           r + u/2 (j = 1), r + u/2 - u (j = 2) for r >= u/2
+__global__ void hifigan_pack_kernel(int kind, const float* __restrict__ w, int N, int K, int taps, int Cout, int u, float* __restrict__ dst) {
+  const long nk = (long)N * K, total = nk * taps;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int j = (int)(i / nk);
+    const long rem = i - (long)j * nk;
+    const int n = (int)(rem / K), c = (int)(rem - (long)n * K);
+    float v;
+    if (kind == 0) {
+      v = w[((long)n * K + c) * taps + j];
+    } else {
+      const int r = n / Cout, co = n - r * Cout, p = u / 2;
+      const int kk = r < p ? (j == 1 ? r + p : j == 0 ? r + p + u : -1) : (j == 2 ? r + p - u : j == 1 ? r + p : -1);
+      v = kk >= 0 ? w[((long)c * Cout + co) * (2 * u) + kk] : 0.f;
+    }
+    dst[i] = v;
+  }
+}
+
+// dst[n] = b[n % Cout]
+__global__ void hifigan_bias_kernel(const float* __restrict__ b, int N, int Cout, float* __restrict__ dst) {
+  for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < N; n += gridDim.x * blockDim.x) dst[n] = b[n % Cout];
+}
+
+// ---- host side ------------------------------------------------------------------------------------------------------
+
+// what a config implies: widths, cumulative upsampling, convolutions per resblock and in all
+struct Shape {
+  int U, nk, type, steps, per;        // upsamplings, resblocks per MRF, resblock type, conv steps and convolutions per resblock
+  int C[kMaxUps + 1];                  // stage widths C0 / 2^s
+  Ups ups;
+  int layers;                          // convolutions in state_dict order
+  long act;                            // floats per frame of the largest stage buffer, max_s up_s * C_s
+};
+
+Shape shape_of(const fs2_hifigan_config& c) {
+  Shape s;
+  s.U = c.num_upsamples; s.nk = c.num_kernels; s.type = c.resblock;
+  s.steps = s.type == 1 ? 3 : 2; s.per = s.type == 1 ? 6 : 2;
+  s.ups.n = s.U; s.ups.up[0] = 1;
+  s.C[0] = c.upsample_initial_channel;
+  s.act = s.C[0];
+  for (int i = 0; i < s.U; ++i) {
+    s.C[i + 1] = s.C[i] / 2;
+    s.ups.up[i + 1] = s.ups.up[i] * c.upsample_rates[i];
+    s.act = std::max(s.act, (long)s.ups.up[i + 1] * s.C[i + 1]);
+  }
+  s.layers = 2 + s.U + s.U * s.nk * s.per;
+  return s;
+}
+
+int validate(const fs2_hifigan_config* c) {
+  const char* who = "fs2_hifigan_create";
+  FS2_REQUIRE(c->resblock == 1 || c->resblock == 2, "%s: resblock must be 1 or 2 (got %d)", who, c->resblock);
+  FS2_REQUIRE(c->num_upsamples >= 1 && c->num_upsamples <= kMaxUps, "%s: num_upsamples must lie in [1, %d] (got %d)", who, kMaxUps,
+              c->num_upsamples);
+  long prod = 1;
+  for (int i = 0; i < c->num_upsamples; ++i) {
+    const int u = c->upsample_rates[i];
+    FS2_REQUIRE(u >= 2 && u % 2 == 0 && u <= kHop, "%s: upsample_rates[%d] = %d must be even, in [2, 256]", who, i, u);
+    FS2_REQUIRE(c->upsample_kernel_sizes[i] == 2 * u, "%s: upsample_kernel_sizes[%d] = %d must be twice the rate %d", who, i,
+                c->upsample_kernel_sizes[i], u);
+    prod *= u;
+  }
+  FS2_REQUIRE(prod == kHop, "%s: the product of upsample_rates is %ld, not the hop 256", who, prod);
+  const int C0 = c->upsample_initial_channel;
+  FS2_REQUIRE(C0 >= 32 && C0 <= 2048 && C0 % (32 << c->num_upsamples) == 0,
+              "%s: upsample_initial_channel = %d must lie in [32, 2048] with every width C0 / 2^i a multiple of 32", who, C0);
+  FS2_REQUIRE(c->num_kernels >= 1 && c->num_kernels <= FS2_HIFIGAN_MAX_KERNELS, "%s: num_kernels must lie in [1, %d] (got %d)", who,
+              FS2_HIFIGAN_MAX_KERNELS, c->num_kernels);
+  FS2_REQUIRE(c->num_dilations == (c->resblock == 1 ? 3 : 2), "%s: num_dilations must be %d for resblock %d (got %d)", who,
+              c->resblock == 1 ? 3 : 2, c->resblock, c->num_dilations);
+  for (int j = 0; j < c->num_kernels; ++j) {
+    const int k = c->resblock_kernel_sizes[j];
+    FS2_REQUIRE(k >= 1 && k <= 31 && k % 2 == 1, "%s: resblock_kernel_sizes[%d] = %d must be odd, in [1, 31]", who, j, k);
+    for (int m = 0; m < c->num_dilations; ++m) {
+      const int d = c->resblock_dilation_sizes[j][m];
+      FS2_REQUIRE(d >= 1 && d <= 1024, "%s: resblock_dilation_sizes[%d][%d] = %d must lie in [1, 1024]", who, j, m, d);
+    }
+  }
+  return FS2_OK;
+}
+
+// the act producer (x, r, nk as in hifigan_act_kernel) into the operand a
+int act(int kind, const float* x, const float* r, int nk, const int64_t* lens, int B, int Lp, int C, void* a, int* status, cudaStream_t st) {
+  auto k = pick(kind, hifigan_act_kernel<OUT_HILO>, hifigan_act_kernel<OUT_HI>, hifigan_act_kernel<OUT_F32>);
+  k<<<grid_for((long)B * Lp * (C / 4), 256), 256, 0, st>>>(x, r, nk, lens, B, Lp, C, (float*)a, (__half*)a, status);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+// lrelu + ConvTranspose1d: x [B * Lin][Cin] (combined with r / nk) -> out [B * Lin][u Cout] = [B * Lin * u][Cout] through the
+// operand a; rows >= lens[b] * u of out written as +0
+int upsample(int mode, const VWeight& w, const float* x, const float* r, int nk, const int64_t* lens, int B, int Lin, int Cin, void* a,
+             float* out, int* status, cudaStream_t st) {
+  int rc = act(out_kind(mode), x, r, nk, lens, B, Lin, Cin, a, status, st);
+  return rc ? rc : vweight_gemm(mode, w, a, B, Lin, ACT_NONE, lens, out, st);
+}
+
+// One residual block x -> dest on rows [B * Lp][C]: w = its convolutions in state_dict order, dil its dilations.  Step m
+// writes t[m & 1], the last one dest; dest must differ from x and from the buffer the last step reads (t[(steps - 2) & 1]).
+int resblock(int mode, int type, const VWeight* w, const int* dil, const float* x, const int64_t* lens, int B, int Lp, int C, void* a,
+             float* const* t, float* dest, int* status, cudaStream_t st) {
+  const int steps = type == 1 ? 3 : 2, kind = out_kind(mode);
+  const float* X = x;
+  int rc;
+  for (int m = 0; m < steps; ++m) {
+    float* out = m == steps - 1 ? dest : t[m & 1];
+    if ((rc = act(kind, X, nullptr, 1, lens, B, Lp, C, a, status, st))) return rc;
+    if (type == 1) {
+      if ((rc = vweight_gemm(mode, w[m], a, B, Lp, ACT_NONE, lens, out, st, nullptr, dil[m]))) return rc;   // h = c1(lrelu(x))
+      if ((rc = act(kind, out, nullptr, 1, lens, B, Lp, C, a, status, st))) return rc;
+      if ((rc = vweight_gemm(mode, w[3 + m], a, B, Lp, ACT_NONE, lens, out, st, X, 1))) return rc;        // c2(lrelu(h)) + x
+    } else {
+      if ((rc = vweight_gemm(mode, w[m], a, B, Lp, ACT_NONE, lens, out, st, X, dil[m]))) return rc;       // c(lrelu(x)) + x
+    }
+    X = out;
+  }
+  return FS2_OK;
+}
+
+struct HgPlan {
+  int64_t* lens;      // [U + 1][B]
+  void* a;            // GEMM operand
+  float* xu;          // the upsampling output of the current stage
+  float* s;           // MRF sum
+  float* t[2];        // chain buffers
+};
+
+HgPlan plan(Bump& b, const Shape& sh, int B, int L) {
+  const size_t n = (size_t)B * L * sh.act;
+  HgPlan p;
+  p.lens = (int64_t*)b.bytes((size_t)(sh.U + 1) * B * sizeof(int64_t));
+  p.a = b.floats(n);
+  p.xu = b.floats(n);
+  p.s = b.floats(n);
+  p.t[0] = b.floats(n);
+  p.t[1] = b.floats(n);
+  return p;
+}
+
+// GEMM weight from its torch-layout tensors: packed fp32 [taps][N][K], bias [N], scale and fp16 planes
+int pack_weight(const VWeight& w, int kind, const float* wt, const float* b, int Cout, int u, cudaStream_t st) {
+  hifigan_pack_kernel<<<grid_for((long)w.taps * w.N * w.K, 256), 256, 0, st>>>(kind, wt, w.N, w.K, w.taps, Cout, u, w.w);
+  FS2_LAUNCH_CHECK();
+  hifigan_bias_kernel<<<grid_for(w.N, 256), 256, 0, st>>>(b, w.N, Cout, w.bias);
+  FS2_LAUNCH_CHECK();
+  return vweight_planes(w, st);
+}
+
+void set_conv(VWeight& w, int N, int K, int taps) { w.N = N; w.K = K; w.taps = taps; }
+
+int check_size(int math_mode, int B, int L) {
+  FS2_REQUIRE(B >= 1 && L >= 1, "fs2_hifigan: need B >= 1 and Lmax >= 1 (got %d, %d)", B, L);
+  return check_rows("fs2_hifigan", "B * Lmax * 256", "sample", (long)B * L * kHop, math_mode);
+}
+
+}  // namespace
+}  // namespace fs2
+
+struct fs2_hifigan_gen {
+  int device = 0, math_mode = 0;
+  fs2_hifigan_config cfg;
+  fs2::Shape sh;
+  bool loaded = false;
+  void* arena = nullptr; size_t arena_bytes = 0;
+  fs2::VWeight pre, up[fs2::kMaxUps];
+  std::vector<fs2::VWeight> blk;   // [U * nk][per]: the resblocks' convolutions in state_dict order
+  float* post_w = nullptr;         // [7][C_U]
+  float* post_b = nullptr;
+};
+
+namespace fs2 {
+namespace {
+
+int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const int64_t* olens, int B, int L, float* audio, int* status,
+             cudaStream_t st) {
+  const Shape& sh = m->sh;
+  const int mode = m->math_mode, kind = out_kind(mode);
+  auto lens = [&](int s) -> const int64_t* { return p.lens + (long)s * B; };
+  int rc;
+  hifigan_prep_kernel<<<1, 256, 0, st>>>(olens, B, L, sh.ups, p.lens, status);
+  FS2_LAUNCH_CHECK();
+  {
+    auto k = pick(kind, hifigan_mel_operand_kernel<OUT_HILO>, hifigan_mel_operand_kernel<OUT_HI>, hifigan_mel_operand_kernel<OUT_F32>);
+    k<<<grid_for((long)B * L * (kMels / 4), 256), 256, 0, st>>>(mels, lens(0), B, L, (float*)p.a, (__half*)p.a, status);
+    FS2_LAUNCH_CHECK();
+  }
+  if ((rc = vweight_gemm(mode, m->pre, p.a, B, L, ACT_NONE, lens(0), p.t[0], st))) return rc;
+  // the stage input: conv_pre's output, then each MRF's (S + r) / nk
+  const float* x = p.t[0];
+  const float* r = nullptr;
+  int nk_in = 1;
+  for (int s = 0; s < sh.U; ++s) {
+    const int Lin = L * sh.ups.up[s], Lp = L * sh.ups.up[s + 1], C = sh.C[s + 1];
+    if ((rc = upsample(mode, m->up[s], x, r, nk_in, lens(s), B, Lin, sh.C[s], p.a, p.xu, status, st))) return rc;
+    float* last = p.s;
+    for (int j = 0; j < sh.nk; ++j) {
+      const int g = s * sh.nk + j;
+      last = j == 0 ? p.s : p.t[(sh.steps - 1) & 1];
+      if ((rc = resblock(mode, sh.type, &m->blk[(size_t)g * sh.per], m->cfg.resblock_dilation_sizes[j], p.xu, lens(s + 1), B, Lp, C, p.a,
+                         p.t, last, status, st)))
+        return rc;
+      if (j >= 1 && j < sh.nk - 1) {
+        hifigan_add_kernel<<<grid_for((long)B * Lp * C / 4, 256), 256, 0, st>>>(p.s, last, (long)B * Lp * C);
+        FS2_LAUNCH_CHECK();
+      }
+    }
+    x = p.s;
+    r = sh.nk > 1 ? last : nullptr;
+    nk_in = sh.nk;
+  }
+  const int Lout = L * kHop, C = sh.C[sh.U];
+  hifigan_post_kernel<<<grid_for((long)B * Lout, 256), 256, kPostTaps * C * sizeof(float), st>>>(x, r, nk_in, lens(sh.U), B, Lout, C,
+                                                                                                  m->post_w, m->post_b, audio);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+// a stream-ordered temporary for the single-layer entries: carve(Bump&) on a counting pass, then on the allocation
+template <typename Carve>
+int temp_carve(void** base, cudaStream_t st, Carve carve) {
+  Bump count(nullptr, 0);
+  carve(count);
+  FS2_CUDA_CHECK(cudaMallocAsync(base, count.off + 256, st));
+  Bump b(*base, count.off + 256);
+  carve(b);
+  return FS2_OK;
+}
+
+}  // namespace
+}  // namespace fs2
+
+using namespace fs2;
+
+extern "C" {
+
+int fs2_hifigan_create(fs2_hifigan_gen** out, int math_mode, const fs2_hifigan_config* cfg) {
+  FS2_REQUIRE(out && cfg, "fs2_hifigan_create: null argument");
+  FS2_REQUIRE(math_mode >= FS2_MATH_FP32 && math_mode <= FS2_MATH_F16, "fs2_hifigan_create: bad math_mode %d", math_mode);
+  int rc = validate(cfg);
+  if (rc) return rc;
+  int dev = 0;
+  FS2_CUDA_CHECK(cudaGetDevice(&dev));
+  fs2_hifigan_gen* m = new fs2_hifigan_gen();
+  m->math_mode = math_mode;
+  m->device = dev;
+  m->cfg = *cfg;
+  m->sh = shape_of(*cfg);
+  const Shape& sh = m->sh;
+  set_conv(m->pre, sh.C[0], kMels, kPreTaps);
+  for (int s = 0; s < sh.U; ++s) set_conv(m->up[s], cfg->upsample_rates[s] * sh.C[s + 1], sh.C[s], 3);
+  m->blk.resize((size_t)sh.U * sh.nk * sh.per);
+  for (int s = 0; s < sh.U; ++s)
+    for (int j = 0; j < sh.nk; ++j)
+      for (int i = 0; i < sh.per; ++i) set_conv(m->blk[((size_t)s * sh.nk + j) * sh.per + i], sh.C[s + 1], sh.C[s + 1], cfg->resblock_kernel_sizes[j]);
+  *out = m;
+  return FS2_OK;
+}
+
+void fs2_hifigan_destroy(fs2_hifigan_gen* m) {
+  if (!m) return;
+  if (m->arena) cudaFree(m->arena);
+  delete m;
+}
+
+int fs2_hifigan_load(fs2_hifigan_gen* m, const float* const* weights, const float* const* biases, void* stream) {
+  FS2_REQUIRE(m && weights && biases, "fs2_hifigan_load: null argument");
+  const Shape& sh = m->sh;
+  for (int i = 0; i < sh.layers; ++i) FS2_REQUIRE(weights[i] && biases[i], "fs2_hifigan_load: layer %d: null tensor", i);
+  cudaStream_t st = (cudaStream_t)stream;
+  m->loaded = false;
+  int rc = arena_carve(&m->arena, &m->arena_bytes, st, [&](Bump& b) {
+    vweight_carve(b, m->pre, true);
+    for (int s = 0; s < sh.U; ++s) vweight_carve(b, m->up[s], true);
+    for (auto& w : m->blk) vweight_carve(b, w, true);
+    m->post_w = b.floats((size_t)kPostTaps * sh.C[sh.U]);
+    m->post_b = b.floats(1);
+    return FS2_OK;
+  });
+  if (rc) return rc;
+  if ((rc = pack_weight(m->pre, 0, weights[0], biases[0], sh.C[0], 0, st))) return rc;
+  for (int s = 0; s < sh.U; ++s)
+    if ((rc = pack_weight(m->up[s], 1, weights[1 + s], biases[1 + s], sh.C[s + 1], m->cfg.upsample_rates[s], st))) return rc;
+  for (size_t i = 0; i < m->blk.size(); ++i)
+    if ((rc = pack_weight(m->blk[i], 0, weights[1 + sh.U + i], biases[1 + sh.U + i], m->blk[i].N, 0, st))) return rc;
+  const int C = sh.C[sh.U], last = sh.layers - 1;
+  hifigan_pack_kernel<<<grid_for((long)kPostTaps * C, 256), 256, 0, st>>>(0, weights[last], 1, C, kPostTaps, 1, 0, m->post_w);
+  FS2_LAUNCH_CHECK();
+  FS2_CUDA_CHECK(cudaMemcpyAsync(m->post_b, biases[last], sizeof(float), cudaMemcpyDeviceToDevice, st));
+  m->loaded = true;
+  return FS2_OK;
+}
+
+int fs2_hifigan_workspace_bytes(fs2_hifigan_gen* m, int B, int Lmax, size_t* bytes) {
+  FS2_REQUIRE(m && bytes, "fs2_hifigan_workspace_bytes: null argument");
+  int rc = check_size(m->math_mode, B, Lmax);
+  if (rc) return rc;
+  Bump b(nullptr, 0);
+  plan(b, m->sh, B, Lmax);
+  *bytes = b.off + 256;
+  return FS2_OK;
+}
+
+int fs2_hifigan(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
+                size_t ws_bytes, void* stream) {
+  FS2_REQUIRE(m && mels && olens && audio && status && ws, "fs2_hifigan: null argument");
+  FS2_REQUIRE(m->loaded, "fs2_hifigan: weights not loaded (fs2_hifigan_load)");
+  FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "fs2_hifigan: mels must be 16-byte aligned");
+  int rc = check_size(m->math_mode, B, Lmax);
+  if (rc) return rc;
+  Bump b(ws, ws_bytes);
+  HgPlan p = plan(b, m->sh, B, Lmax);
+  if ((rc = b.check("fs2_hifigan"))) return rc;
+  return generate(m, p, mels, olens, B, Lmax, audio, status, (cudaStream_t)stream);
+}
+
+// ---- single layers on the vocoder's own code paths (tests) ----------------------------------------------------------
+int fs2_op_hifigan_resblock(int math_mode, int type, int C, int k, int nd, const int* dils, const float* x, const int64_t* lens, int B,
+                            int Lp, const float* const* weights, const float* const* biases, float* out, int* status, void* stream) {
+  const char* who = "fs2_op_hifigan_resblock";
+  FS2_REQUIRE(math_mode >= FS2_MATH_FP32 && math_mode <= FS2_MATH_F16, "%s: bad math_mode %d", who, math_mode);
+  FS2_REQUIRE(type == 1 || type == 2, "%s: type must be 1 or 2 (got %d)", who, type);
+  FS2_REQUIRE(C >= 32 && C % 32 == 0, "%s: C must be a multiple of 32 (got %d)", who, C);
+  FS2_REQUIRE(k >= 1 && k <= 31 && k % 2 == 1, "%s: k must be odd, in [1, 31] (got %d)", who, k);
+  FS2_REQUIRE(nd == (type == 1 ? 3 : 2), "%s: nd must be %d for type %d (got %d)", who, type == 1 ? 3 : 2, type, nd);
+  FS2_REQUIRE(dils && x && lens && weights && biases && out && status, "%s: null argument", who);
+  for (int i = 0; i < nd; ++i) FS2_REQUIRE(dils[i] >= 1 && dils[i] <= 1024, "%s: dilation %d out of [1, 1024]", who, dils[i]);
+  const int per = type == 1 ? 6 : 2;
+  for (int i = 0; i < per; ++i) FS2_REQUIRE(weights[i] && biases[i], "%s: null argument", who);
+  FS2_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 31) == 0,
+              "%s: x must be 16-byte and out 32-byte aligned", who);
+  FS2_REQUIRE(B >= 1 && Lp >= 1, "%s: bad shape B=%d Lp=%d", who, B, Lp);
+  const long rows = (long)B * Lp;
+  FS2_REQUIRE(rows * C < (1L << 31) && (math_mode != FS2_MATH_FP32 || rows <= kTapGemmFp32MaxRows), "%s: too many rows (%ld)", who, rows);
+  cudaStream_t st = (cudaStream_t)stream;
+  VWeight w[6];
+  for (int i = 0; i < per; ++i) set_conv(w[i], C, C, k);
+  void* a = nullptr;
+  float* t[2] = {nullptr, nullptr};
+  void* base = nullptr;
+  int rc = temp_carve(&base, st, [&](Bump& b) {
+    for (int i = 0; i < per; ++i) vweight_carve(b, w[i], true);
+    a = b.floats((size_t)rows * C);
+    t[0] = b.floats((size_t)rows * C);
+    t[1] = b.floats((size_t)rows * C);
+  });
+  if (rc) return rc;
+  FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
+  for (int i = 0; i < per && !rc; ++i) rc = pack_weight(w[i], 0, weights[i], biases[i], C, 0, st);
+  if (!rc) rc = resblock(math_mode, type, w, dils, x, lens, B, Lp, C, a, t, out, status, st);
+  cudaFreeAsync(base, st);
+  return rc;
+}
+
+int fs2_op_hifigan_upsample(int math_mode, int Cin, int Cout, int u, const float* x, const int64_t* lens, int B, int Lin, const float* w,
+                            const float* b, float* out, int* status, void* stream) {
+  const char* who = "fs2_op_hifigan_upsample";
+  FS2_REQUIRE(math_mode >= FS2_MATH_FP32 && math_mode <= FS2_MATH_F16, "%s: bad math_mode %d", who, math_mode);
+  FS2_REQUIRE(u >= 2 && u % 2 == 0 && u <= kHop, "%s: the rate u must be even, in [2, 256] (got %d)", who, u);
+  FS2_REQUIRE(Cin >= 32 && Cin % 32 == 0 && Cout >= 32 && Cout % 32 == 0, "%s: Cin and Cout must be multiples of 32 (got %d, %d)", who,
+              Cin, Cout);
+  FS2_REQUIRE(x && lens && w && b && out && status, "%s: null argument", who);
+  FS2_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 31) == 0,
+              "%s: x must be 16-byte and out 32-byte aligned", who);
+  FS2_REQUIRE(B >= 1 && Lin >= 1, "%s: bad shape B=%d Lin=%d", who, B, Lin);
+  const long rows = (long)B * Lin;
+  FS2_REQUIRE(rows * u * Cout < (1L << 31) && rows * Cin < (1L << 31) && (math_mode != FS2_MATH_FP32 || rows <= kTapGemmFp32MaxRows),
+              "%s: too many rows (%ld)", who, rows);
+  cudaStream_t st = (cudaStream_t)stream;
+  VWeight wu;
+  set_conv(wu, u * Cout, Cin, 3);
+  void* a = nullptr;
+  void* base = nullptr;
+  int rc = temp_carve(&base, st, [&](Bump& bb) {
+    vweight_carve(bb, wu, true);
+    a = bb.floats((size_t)rows * Cin);
+  });
+  if (rc) return rc;
+  FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
+  rc = pack_weight(wu, 1, w, b, Cout, u, st);
+  if (!rc) rc = upsample(math_mode, wu, x, nullptr, 1, lens, B, Lin, Cin, a, out, status, st);
+  cudaFreeAsync(base, st);
+  return rc;
+}
+
+}  // extern "C"

@@ -1,0 +1,278 @@
+"""Batched HiFi-GAN vocoder on the library's kernels (DESIGN.md section 16).
+
+jik876/hifi-gan's generators read this project's mels as they are: 22,050 Hz, n_fft 1024, hop 256, 80 bands from 0 to
+8,000 Hz, natural log clamped at 1e-5.  `HiFiGANVocoder` runs the `Generator` of a hifi-gan config batched and per utterance
+on libfs2b200.so (csrc/hifigan.cu) and loads its `g_XXXXXXXX` checkpoints from a local file.
+
+The module's parameters carry the checkpoint's keys (`conv_pre.{bias,weight_g,weight_v}`, `ups.{i}.*`,
+`resblocks.{j}.convs1.{m}.*` / `convs2.{m}.*` or `resblocks.{j}.convs.{m}.*`, `conv_post.*`; the lists with shapes for V1,
+V2 and V3 are tests/golden/hifigan_state_dict_keys.json).  They are written from the published code, not checked against a
+real checkpoint file.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import json
+import math
+import os
+
+import torch
+import torch.nn as nn
+
+from . import _lib
+from ._kernel_module import WindowedVocoder, _WNConv, normalise_checkpoint
+
+HOP = 256
+N_MELS = 80
+MAX_WAV_VALUE = 32768.0
+
+# hifi-gan's published config_v1.json, config_v2.json and config_v3.json (the fields the generator uses).  V2's widths
+# (128 ... 8) are refused by HiFiGANVocoder; the entry is here for its key list.
+CONFIGS = {
+    "v1": {"resblock": "1", "upsample_rates": [8, 8, 2, 2], "upsample_kernel_sizes": [16, 16, 4, 4], "upsample_initial_channel": 512,
+           "resblock_kernel_sizes": [3, 7, 11], "resblock_dilation_sizes": [[1, 3, 5], [1, 3, 5], [1, 3, 5]], "num_mels": 80},
+    "v2": {"resblock": "1", "upsample_rates": [8, 8, 2, 2], "upsample_kernel_sizes": [16, 16, 4, 4], "upsample_initial_channel": 128,
+           "resblock_kernel_sizes": [3, 7, 11], "resblock_dilation_sizes": [[1, 3, 5], [1, 3, 5], [1, 3, 5]], "num_mels": 80},
+    "v3": {"resblock": "2", "upsample_rates": [8, 8, 4], "upsample_kernel_sizes": [16, 16, 8], "upsample_initial_channel": 256,
+           "resblock_kernel_sizes": [3, 5, 7], "resblock_dilation_sizes": [[1, 2], [2, 6], [3, 12]], "num_mels": 80},
+}
+_FIELDS = ("resblock", "upsample_rates", "upsample_kernel_sizes", "upsample_initial_channel", "resblock_kernel_sizes",
+           "resblock_dilation_sizes")
+
+
+def load_config(config) -> dict:
+    """A hifi-gan config as a dict of the fields the generator uses: from "v1" / "v2" / "v3", a dict (e.g. a loaded
+    config.json) or the path of a config.json.  Only its form is checked here; `check_config` checks what this library
+    runs."""
+    if isinstance(config, str) and config.lower() in CONFIGS:
+        config = CONFIGS[config.lower()]
+    elif isinstance(config, (str, os.PathLike)):
+        with open(config) as f:
+            config = json.load(f)
+    if not isinstance(config, dict):
+        raise ValueError("config must be 'v1', 'v2', 'v3', a dict or the path of a hifi-gan config.json")
+    for k in _FIELDS:
+        if k not in config:
+            raise ValueError(f"config: missing field {k}")
+    out = {"resblock": str(config["resblock"]), "upsample_initial_channel": config["upsample_initial_channel"]}
+    for k in ("upsample_rates", "upsample_kernel_sizes", "resblock_kernel_sizes"):
+        out[k] = [v for v in config[k]]
+    out["resblock_dilation_sizes"] = [list(d) for d in config["resblock_dilation_sizes"]]
+    if "num_mels" in config:
+        out["num_mels"] = config["num_mels"]
+    return out
+
+
+def _ints(name, values):
+    if not all(isinstance(v, int) and not isinstance(v, bool) for v in values):
+        raise ValueError(f"config: {name} must hold integers")
+
+
+def check_config(cfg: dict) -> None:
+    """Raises ValueError naming the field for a config the kernels do not run: num_mels other than 80; a resblock type
+    other than "1" or "2"; upsample rates that are odd, whose product is not the hop 256, or whose kernel sizes are not
+    twice the rate; a convolution width (upsample_initial_channel / 2^i) that is not a multiple of 32 (this refuses V2) or
+    above 2048; even resblock kernel sizes; too few dilations per resblock."""
+    if cfg.get("num_mels", N_MELS) != N_MELS:
+        raise ValueError(f"config: num_mels must be {N_MELS} (got {cfg['num_mels']})")
+    if cfg["resblock"] not in ("1", "2"):
+        raise ValueError(f"config: resblock must be \"1\" or \"2\" (got {cfg['resblock']!r})")
+    rates, ks = cfg["upsample_rates"], cfg["upsample_kernel_sizes"]
+    _ints("upsample_rates", rates)
+    _ints("upsample_kernel_sizes", ks)
+    if not 1 <= len(rates) <= _lib.FS2_HIFIGAN_MAX_UPSAMPLES:
+        raise ValueError(f"config: upsample_rates must hold 1 to {_lib.FS2_HIFIGAN_MAX_UPSAMPLES} rates")
+    if any(u < 2 or u % 2 for u in rates):
+        raise ValueError(f"config: upsample_rates must be even (got {rates})")
+    if math.prod(rates) != HOP:
+        raise ValueError(f"config: the product of upsample_rates must be the hop {HOP} (got {math.prod(rates)})")
+    if len(ks) != len(rates) or any(k != 2 * u for k, u in zip(ks, rates)):
+        raise ValueError(f"config: upsample_kernel_sizes must be twice the upsample_rates (got {ks} for {rates})")
+    c0 = cfg["upsample_initial_channel"]
+    _ints("upsample_initial_channel", [c0])
+    widths = [c0 // 2 ** i for i in range(len(rates) + 1)]
+    if c0 > 2048 or c0 % 2 ** len(rates) or any(w % 32 or w < 32 for w in widths):
+        raise ValueError(f"config: upsample_initial_channel = {c0} gives convolution widths {widths}; every one must be a "
+                         f"multiple of 32 (and at most 2048)")
+    kers, dils = cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"]
+    _ints("resblock_kernel_sizes", kers)
+    if not 1 <= len(kers) <= _lib.FS2_HIFIGAN_MAX_KERNELS or any(k < 1 or k > 31 or k % 2 == 0 for k in kers):
+        raise ValueError(f"config: resblock_kernel_sizes must be 1 to {_lib.FS2_HIFIGAN_MAX_KERNELS} odd sizes in [1, 31] (got {kers})")
+    need = 3 if cfg["resblock"] == "1" else 2
+    if len(dils) != len(kers) or any(len(d) < need for d in dils):
+        raise ValueError(f"config: resblock_dilation_sizes must hold {need} dilations for each of the {len(kers)} kernel sizes")
+    for d in dils:
+        _ints("resblock_dilation_sizes", d)
+        if any(v < 1 or v > 1024 for v in d[:need]):
+            raise ValueError(f"config: resblock_dilation_sizes must lie in [1, 1024] (got {dils})")
+
+
+class _ResBlock1(nn.Module):
+    def __init__(self, c: int, k: int):
+        super().__init__()
+        self.convs1 = nn.ModuleList([_WNConv(c, c, k) for _ in range(3)])
+        self.convs2 = nn.ModuleList([_WNConv(c, c, k) for _ in range(3)])
+
+
+class _ResBlock2(nn.Module):
+    def __init__(self, c: int, k: int):
+        super().__init__()
+        self.convs = nn.ModuleList([_WNConv(c, c, k) for _ in range(2)])
+
+
+def add_layers(module: nn.Module, cfg: dict) -> nn.Module:
+    """Registers the generator's parameter holders on module, in hifi-gan's order, so that its state_dict keys are the
+    checkpoint's: conv_pre, ups, resblocks, conv_post.  No check of the config beyond its shapes (the key lists of
+    configs the kernels refuse, such as V2, come from here too)."""
+    rates, ks, c0 = cfg["upsample_rates"], cfg["upsample_kernel_sizes"], cfg["upsample_initial_channel"]
+    block = _ResBlock1 if str(cfg["resblock"]) == "1" else _ResBlock2
+    module.conv_pre = _WNConv(N_MELS, c0, 7)
+    module.ups = nn.ModuleList([_WNConv(c0 // 2 ** i, c0 // 2 ** (i + 1), k, transposed=True) for i, k in enumerate(ks)])
+    module.resblocks = nn.ModuleList([block(c0 // 2 ** (i + 1), k) for i in range(len(rates)) for k in cfg["resblock_kernel_sizes"]])
+    module.conv_post = _WNConv(c0 // 2 ** len(rates), 1, 7)
+    return module
+
+
+class HiFiGANVocoder(WindowedVocoder):
+    """jik876/hifi-gan's `Generator(h)` on the H100 kernels.
+
+    `forward(mels [B, Lmax, 80], olens [B])` -> (audio [B, Lmax * 256] fp32, alens = olens * 256).  Utterance b is the
+    generator applied to mels[b, :olens[b]] alone: every convolution zero-pads at its own edges, no tail frames, no mel
+    normalisation.  It is bit-identical to a B = 1 call on its own frames whatever else is in the batch, audio past
+    alens[b] is +0, and mel frames past olens[b] are never read.  config: "v1", "v3", a dict or a config.json path
+    (`check_config` lists what is refused).  math_mode: "3xf16" (default, fp32-class), "f16", "tf32" or "fp32" for the
+    GEMMs.  One host read per call (the device-side length and range checks)."""
+
+    _DESTROY, _WORKSPACE_BYTES, _WINDOW_BYTES = "fs2_hifigan_destroy", "fs2_hifigan_workspace_bytes", None
+
+    def __init__(self, config="v1", math_mode: str = "3xf16"):
+        super().__init__()
+        if math_mode not in _lib.MATH_MODES:
+            raise ValueError(f"math_mode must be one of {sorted(_lib.MATH_MODES)}")
+        cfg = load_config(config)
+        check_config(cfg)
+        self.config = cfg
+        self.math_mode = math_mode
+        add_layers(self, cfg)
+        self._layers = [m for m in self.modules() if isinstance(m, _WNConv)]      # state_dict order
+
+    def launches(self) -> int:
+        """Kernels one call enqueues: 4 + U * (2 + K * G + max(K - 2, 0)), G = 12 (resblock "1") or 4 (resblock "2")."""
+        U, K = len(self.config["upsample_rates"]), len(self.config["resblock_kernel_sizes"])
+        G = 12 if self.config["resblock"] == "1" else 4
+        return 4 + U * (2 + K * G + max(K - 2, 0))
+
+    def flops_per_frame(self) -> int:
+        """Multiply-adds x 2 per mel frame of the generator's convolutions (the transposed ones counted as torch runs them:
+        Cin * Cout * k per input row)."""
+        cfg = self.config
+        c0, f = cfg["upsample_initial_channel"], 0
+        f += N_MELS * c0 * 7
+        up = 1
+        convs = 6 if cfg["resblock"] == "1" else 2
+        for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
+            cin, cout = c0 // 2 ** i, c0 // 2 ** (i + 1)
+            f += up * cin * cout * k
+            up *= u
+            f += up * sum(convs * cout * cout * kk for kk in cfg["resblock_kernel_sizes"])
+        f += up * (c0 // 2 ** len(cfg["upsample_rates"])) * 7
+        return 2 * f
+
+    # ---- checkpoints ----------------------------------------------------------------------------------------------
+    @classmethod
+    def from_checkpoint(cls, path_or_dict, config=None, math_mode: str = "3xf16") -> "HiFiGANVocoder":
+        """A hifi-gan generator checkpoint (`g_XXXXXXXX`: a dict with "generator") or a bare generator state dict, given as
+        a file path or as the loaded dict.  Either may hold `weight_g` / `weight_v` keys or plain `weight` keys (after
+        `remove_weight_norm`).  config: as in the constructor; None reads config.json beside a checkpoint path, as
+        hifi-gan's inference.py does (the dilations cannot be read from the weights).  A missing, unexpected or wrongly
+        shaped key raises ValueError naming it."""
+        sd = path_or_dict
+        if config is None:
+            if not isinstance(sd, (str, os.PathLike)):
+                raise ValueError("config is required when the checkpoint is given as a dict")
+            path = os.path.join(os.path.dirname(os.path.abspath(sd)), "config.json")
+            if not os.path.exists(path):
+                raise ValueError(f"config is required: no config.json beside {sd}")
+            config = path
+        voc = cls(config, math_mode=math_mode)
+        if isinstance(sd, (str, os.PathLike)):
+            sd = torch.load(sd, map_location="cpu", weights_only=True)
+        if not isinstance(sd, dict):
+            raise ValueError("expected a checkpoint dict (with 'generator') or a generator state dict")
+        if "generator" in sd:
+            sd = sd["generator"]
+        voc.load_state_dict(normalise_checkpoint(voc, sd))
+        return voc
+
+    # ---- device state ---------------------------------------------------------------------------------------------
+    def _c_config(self) -> _lib.HiFiGANConfig:
+        cfg = self.config
+        c = _lib.HiFiGANConfig()
+        c.resblock = int(cfg["resblock"])
+        c.num_upsamples = len(cfg["upsample_rates"])
+        for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
+            c.upsample_rates[i], c.upsample_kernel_sizes[i] = u, k
+        c.upsample_initial_channel = cfg["upsample_initial_channel"]
+        c.num_kernels = len(cfg["resblock_kernel_sizes"])
+        c.num_dilations = 3 if c.resblock == 1 else 2
+        for j, (k, d) in enumerate(zip(cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"])):
+            c.resblock_kernel_sizes[j] = k
+            for m in range(c.num_dilations):
+                c.resblock_dilation_sizes[j][m] = d[m]
+        return c
+
+    def _create(self):
+        h = C.c_void_p()
+        cfg = self._c_config()
+        _lib.check(_lib.load().fs2_hifigan_create(C.byref(h), _lib.MATH_MODES[self.math_mode], C.byref(cfg)), "fs2_hifigan_create")
+        return h.value
+
+    def _load(self, h, device: torch.device) -> None:
+        ws = [m.folded().to(device).contiguous() for m in self._layers]
+        bs = [m.bias.detach().float().to(device).contiguous() for m in self._layers]
+        wp = (C.c_void_p * len(ws))(*[t.data_ptr() for t in ws])
+        bp = (C.c_void_p * len(bs))(*[t.data_ptr() for t in bs])
+        _lib.check(_lib.load().fs2_hifigan_load(h, wp, bp, _lib.stream_ptr(device)), "fs2_hifigan_load")
+
+    def _inputs(self, mels, olens):
+        if not torch.is_tensor(mels) or mels.dim() != 3 or mels.shape[2] != N_MELS or mels.shape[0] == 0 or mels.shape[1] == 0:
+            raise ValueError(f"mels must be a non-empty [B, Lmax, {N_MELS}] tensor")
+        if not torch.is_tensor(olens) or olens.dim() != 1 or olens.shape[0] != mels.shape[0]:
+            raise ValueError(f"olens must be a [B={mels.shape[0]}] tensor")
+        if olens.dtype.is_floating_point or olens.dtype == torch.bool:
+            raise ValueError("olens must be an integer tensor")
+        if not mels.is_cuda or not olens.is_cuda:
+            raise ValueError("mels and olens must be CUDA tensors (the H100 path has no CPU fallback)")
+        B, L, _ = mels.shape
+        self._check_size(B, L)
+        return mels.to(torch.float32).contiguous(), olens.to(device=mels.device, dtype=torch.int64).contiguous(), B, L
+
+    def _check_size(self, B: int, L: int) -> None:
+        """The limits fs2_hifigan checks, raised here as ValueError: B * Lmax * 256 sample rows below 2^31, and at most
+        65535 * 128 in fp32 mode (its CUDA-core GEMMs put 128-row tiles on grid.y)."""
+        rows = B * L * HOP
+        if rows >= 1 << 31:
+            raise ValueError(f"B * Lmax * {HOP} must stay below 2^31 sample rows (B={B}, Lmax={L})")
+        if self.math_mode == "fp32" and rows > 65535 * 128:
+            raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 sample rows, B * Lmax * {HOP} = {rows} "
+                             f"(B={B}, Lmax={L}); split the batch or use another math mode")
+
+    def _status_table(self):
+        return [(_lib.FS2_HIFIGAN_BAD_LENGTH, "every olens[b] must lie in [1, Lmax]"),
+                (_lib.FS2_HIFIGAN_RANGE, f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
+                                         f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'")]
+
+    # ---- synthesis ------------------------------------------------------------------------------------------------
+    def forward(self, mels: torch.Tensor, olens: torch.Tensor):
+        """-> (audio [B, Lmax * 256] fp32, alens [B] int64 = olens * 256)."""
+        mels, olens, B, L = self._inputs(mels, olens)
+        dev = mels.device
+        h = self._handle(dev)
+        ws = self._workspace(h, B, L, dev)
+        audio = torch.empty((B, L * HOP), dtype=torch.float32, device=dev)
+        status = torch.empty((1,), dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.load().fs2_hifigan(h, _lib.ptr(mels), _lib.ptr(olens), B, L, _lib.ptr(audio), _lib.ptr(status), _lib.ptr(ws),
+                                               ws.numel(), _lib.stream_ptr(dev)), "fs2_hifigan")
+        self._check_status(status)
+        return audio, olens * HOP

@@ -520,6 +520,63 @@ int fs2_op_melgan_block(int math_mode, int route, int C, const float* x, const i
 int fs2_op_melgan_upsample(int math_mode, int Cin, int Cout, int s, const float* x, const int64_t* lens, int B, int Lin, const float* w,
                            const float* b, float* out, int* status, void* stream);
 
+/* ---- batched HiFi-GAN vocoder (DESIGN.md section 16) ---------------------------------------------------------------- */
+/* jik876/hifi-gan's Generator on log-mels [B, Lmax, 80] with frame counts olens [B]: utterance b is the generator applied
+ * to mels[b, :olens[b]] alone (every convolution zero-pads at its own edges; no tail frames, no normalisation), olens[b] *
+ * 256 samples.  audio [B, Lmax * 256] fp32, +0 from olens[b] * 256 on; audio[b] is bit-identical to a B = 1 call on its
+ * own frames; mel frames past olens[b] are never read.  No allocation, no synchronisation: a call can be graph-captured.
+ * It enqueues 4 + U * (2 + K * G + max(K - 2, 0)) kernels, U = num_upsamples, K = num_kernels, G = 12 (resblock 1) or 4
+ * (resblock 2): 160 for V1, 49 for V3, in every math mode.
+ * Data-dependent checks run on the device and are reported in *status (device int, written by the call):
+ *   FS2_HIFIGAN_BAD_LENGTH  some olens[b] outside [1, Lmax]; that utterance's audio is 0;
+ *   FS2_HIFIGAN_RANGE       an fp16 operand plane (f16 / 3xF16 modes) would saturate: some GEMM input above 65504 /
+ *                           kPlaneScale (4094) in magnitude. */
+#define FS2_HIFIGAN_BAD_LENGTH 1
+#define FS2_HIFIGAN_RANGE 2
+#define FS2_HIFIGAN_MAX_UPSAMPLES 8
+#define FS2_HIFIGAN_MAX_KERNELS 8
+/* hifi-gan's config.json fields.  Accepted: resblock 1 or 2; the upsample rates even, their product 256, every kernel size
+ * twice its rate; every width upsample_initial_channel / 2^i (i = 0 .. num_upsamples) a multiple of 32, at most 2048;
+ * resblock kernel sizes odd in [1, 31]; num_dilations 3 (resblock 1) or 2 (resblock 2), dilations in [1, 1024]. */
+typedef struct fs2_hifigan_config {
+  int resblock;
+  int num_upsamples;
+  int upsample_rates[FS2_HIFIGAN_MAX_UPSAMPLES];
+  int upsample_kernel_sizes[FS2_HIFIGAN_MAX_UPSAMPLES];
+  int upsample_initial_channel;
+  int num_kernels;
+  int resblock_kernel_sizes[FS2_HIFIGAN_MAX_KERNELS];
+  int num_dilations;
+  int resblock_dilation_sizes[FS2_HIFIGAN_MAX_KERNELS][4];
+} fs2_hifigan_config;
+typedef struct fs2_hifigan_gen fs2_hifigan_gen;
+/* on the current device; math_mode FS2_MATH_*: every GEMM of the generator (conv_post runs on CUDA cores in fp32).
+ * FS2_ERR_INVALID for a config outside the accepted set. */
+int fs2_hifigan_create(fs2_hifigan_gen** out, int math_mode, const fs2_hifigan_config* cfg);
+void fs2_hifigan_destroy(fs2_hifigan_gen* m);
+/* weights[n], biases[n]: device fp32 tensors of the n convolutions in state_dict order (conv_pre, ups.{0..U-1},
+ * resblocks.{0..U*K-1} with convs1.{0,1,2} then convs2.{0,1,2} (resblock 1) or convs.{0,1} (resblock 2), conv_post), weight
+ * norm already folded, in torch's layouts: Conv1d [Cout, Cin, k], ConvTranspose1d [Cin, Cout, k].  Packed once; the tensors
+ * may be freed afterwards (stream order). */
+int fs2_hifigan_load(fs2_hifigan_gen* m, const float* const* weights, const float* const* biases, void* stream);
+/* fails (FS2_ERR_INVALID) when B * Lmax * 256 reaches 2^31, or exceeds 65535 * 128 in FS2_MATH_FP32 */
+int fs2_hifigan_workspace_bytes(fs2_hifigan_gen* m, int B, int Lmax, size_t* bytes);
+int fs2_hifigan(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
+                size_t ws_bytes, void* stream);
+/* Single HiFi-GAN layers on fs2_hifigan's code paths (used by the per-layer tests).  Weights come in torch's layouts and are
+ * packed into a stream-ordered temporary as fs2_hifigan_load packs them.  status (device int) is set to 0 or
+ * FS2_HIFIGAN_RANGE.  x 16-byte and out 32-byte aligned; utterance b is rows t < lens[b] (lens[b] in [0, Lp]), zero outside
+ * them; rows t >= lens[b] of x are never read and those of out are written as +0.
+ * fs2_op_hifigan_resblock: one residual block (type 1 or 2) on rows [B*Lp][C], kernel size k, dilations dils[nd] (host;
+ *   nd = 3 for type 1, 2 for type 2); weights / biases (host arrays of device pointers): the block's convolutions in
+ *   state_dict order, each [C][C][k] / [C].  C a multiple of 32.
+ * fs2_op_hifigan_upsample: lrelu(x, 0.1) then ConvTranspose1d(Cin -> Cout, k = 2u, stride u, padding u/2) on x [B*Lin][Cin];
+ *   w [Cin][Cout][2u], b [Cout]; out [B*Lin*u][Cout].  u even, Cin and Cout multiples of 32. */
+int fs2_op_hifigan_resblock(int math_mode, int type, int C, int k, int nd, const int* dils, const float* x, const int64_t* lens, int B,
+                            int Lp, const float* const* weights, const float* const* biases, float* out, int* status, void* stream);
+int fs2_op_hifigan_upsample(int math_mode, int Cin, int Cout, int u, const float* x, const int64_t* lens, int B, int Lin, const float* w,
+                            const float* b, float* out, int* status, void* stream);
+
 /* ---- batched WaveGlow vocoder (DESIGN.md section 9) ----------------------------------------------------------------- */
 /* DeepLearningExamples' WaveGlow (n_mel_channels 80, n_flows 12, n_group 8, n_early_every 4, n_early_size 2, WN: 8 layers,
  * kernel 3, n_channels C) in its inverse direction, `infer`, on log-mels [B, Lmax, 80] with frame counts olens [B]:
