@@ -1,14 +1,20 @@
-"""Host-side layer the signal modules share (MelGAN, WaveGlow, Griffin-Lim, feature extraction): the per-device handle
-and workspace caches, the status-word check, weight-norm checkpoint normalisation, and the window layer of the two neural
-vocoders (DESIGN.md sections 11-12)."""
+"""Host-side layer the signal modules share (MelGAN, HiFi-GAN, WaveGlow, Griffin-Lim, feature extraction): the per-device
+handle and workspace caches, the status-word check, checkpoint reading and weight-norm normalisation, and the call surface
+of the three neural vocoders: input and size checks, the whole call, and the windows of MelGAN and WaveGlow (DESIGN.md
+sections 11-12)."""
 from __future__ import annotations
 
 import ctypes as C
+import os
 
 import torch
 import torch.nn as nn
 
 from . import _lib
+
+HOP = 256                        # audio samples per mel frame
+N_MELS = 80
+MAX_WAV_VALUE = 32768.0
 
 
 class Handles:
@@ -63,7 +69,19 @@ def check_status(status: torch.Tensor, table) -> None:
             raise ValueError(message)
 
 
-# ---- weight-norm checkpoints --------------------------------------------------------------------------------------
+# ---- checkpoints --------------------------------------------------------------------------------------------------
+
+def read_checkpoint(path_or_dict, wrapper_key: str, what: str) -> dict:
+    """A checkpoint given as a file path or as the loaded dict -> its state dict: what is under wrapper_key when the
+    dict has that key, else the dict itself.  `what` names the bare state dict in the error."""
+    sd = path_or_dict
+    if isinstance(sd, (str, os.PathLike)):
+        sd = torch.load(sd, map_location="cpu", weights_only=True)
+    if not isinstance(sd, dict):
+        raise ValueError(f"expected a checkpoint dict (with '{wrapper_key}') or {what}")
+    return sd[wrapper_key] if wrapper_key in sd else sd
+
+
 
 class _WNConv(nn.Module):
     """The parameters of one weight-normalised convolution, registered in `torch.nn.utils.weight_norm`'s order (bias,
@@ -133,21 +151,28 @@ def normalise_checkpoint(module: nn.Module, sd) -> dict:
     return out
 
 
-# ---- the neural vocoders' windows -----------------------------------------------------------------------------------
+# ---- the neural vocoders --------------------------------------------------------------------------------------------
 
-class WindowedVocoder(nn.Module):
-    """What MelGANVocoder and WaveGlowVocoder share around their C entries: the handle, reloaded when a parameter
-    changes; the whole call's and the window's workspaces; the status check; and the window layer (`window`'s inputs,
-    `stream`'s loop, `forward(chunk_frames=)`).
+class NeuralVocoder(nn.Module):
+    """What MelGANVocoder, HiFiGANVocoder and WaveGlowVocoder share around their C entries: the math mode; the handle,
+    reloaded when a parameter changes; the mels / olens and size checks; the whole call with its workspace and status
+    check; and, for MelGAN and WaveGlow, the window layer (`window`'s inputs, `stream`'s loop, `forward(chunk_frames=)`).
 
-    A subclass names its C entries (_DESTROY, _WORKSPACE_BYTES, _WINDOW_BYTES) and provides _create() -> handle,
-    _load(handle, device), _status_table() -> [(bit, message)] and _window_rows(B, n_frames) -> (rows, their formula).
-    A window call is call(h, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws)."""
+    A subclass names its C entries (_DESTROY, _WORKSPACE_BYTES, _WINDOW_BYTES) and the prefix of its status bits (_STATUS,
+    e.g. "FS2_MELGAN"), and provides _create() -> handle, _load(handle, device) and _rows(B, Lmax) -> (rows, their
+    formula, their noun).  A whole call is call(h, mels, olens, B, Lmax, audio, status, ws).
 
-    HOP = 256                    # audio samples per mel frame
+    A vocoder without a window entry sets _WINDOW_BYTES = None: it has no `window`, `stream` or `chunk_frames`, and nothing
+    below the windows' heading applies to it.  One with windows also provides _window_rows(B, n_frames) -> (rows, their
+    formula); a window call is call(h, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws)."""
 
-    def __init__(self):
+    HOP = HOP
+
+    def __init__(self, math_mode: str):
         super().__init__()
+        if math_mode not in _lib.MATH_MODES:
+            raise ValueError(f"math_mode must be one of {sorted(_lib.MATH_MODES)}")
+        self.math_mode = math_mode
         self._handles = Handles(self._DESTROY)
         self._ws = {}            # device index -> workspace tensor
         self._wws = {}           # device index -> window workspace tensor
@@ -167,14 +192,78 @@ class WindowedVocoder(nn.Module):
     def _handle(self, device: torch.device):
         return self._handles.get(device, self._fingerprint(), self._create, self._load)
 
+    def _load_layers(self, entry: str, h, device: torch.device) -> None:
+        """entry(h, weights, biases, stream) on the folded weights and the biases of self._layers (a GAN vocoder's
+        weight-normalised convolutions in state_dict order)."""
+        ws = [m.folded().to(device).contiguous() for m in self._layers]
+        bs = [m.bias.detach().float().to(device).contiguous() for m in self._layers]
+        wp = (C.c_void_p * len(ws))(*[t.data_ptr() for t in ws])
+        bp = (C.c_void_p * len(bs))(*[t.data_ptr() for t in bs])
+        _lib.check(getattr(_lib.load(), entry)(h, wp, bp, _lib.stream_ptr(device)), entry)
+
     def _workspace(self, h, B: int, L: int, device: torch.device) -> torch.Tensor:
         return workspace(self._ws, device, query_bytes(self._WORKSPACE_BYTES, h, B, L))
 
-    def _window_workspace(self, h, B: int, n_frames: int, device: torch.device) -> torch.Tensor:
-        return workspace(self._wws, device, query_bytes(self._WINDOW_BYTES, h, B, n_frames))
+    def _status_table(self):
+        """[(bit, message)] of the status word: <_STATUS>_BAD_LENGTH, _BAD_START where the vocoder has windows, _RANGE."""
+        table = [(getattr(_lib, self._STATUS + "_BAD_LENGTH"), "every olens[b] must lie in [1, Lmax]")]
+        if hasattr(_lib, self._STATUS + "_BAD_START"):
+            table.append((getattr(_lib, self._STATUS + "_BAD_START"), "every starts[b] must be >= 0"))
+        table.append((getattr(_lib, self._STATUS + "_RANGE"),
+                      f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
+                      f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'"))
+        return table
 
     def _check_status(self, status: torch.Tensor) -> None:
         check_status(status, self._status_table())
+
+    @staticmethod
+    def _check_mels_olens(mels, olens) -> None:
+        """The checks of mels [B, Lmax, 80] and olens [B] that need no device."""
+        if not torch.is_tensor(mels) or mels.dim() != 3 or mels.shape[2] != N_MELS or mels.shape[0] == 0 or mels.shape[1] == 0:
+            raise ValueError(f"mels must be a non-empty [B, Lmax, {N_MELS}] tensor")
+        if not torch.is_tensor(olens) or olens.dim() != 1 or olens.shape[0] != mels.shape[0]:
+            raise ValueError(f"olens must be a [B={mels.shape[0]}] tensor")
+        if olens.dtype.is_floating_point or olens.dtype == torch.bool:
+            raise ValueError("olens must be an integer tensor")
+
+    def _mels_olens(self, mels, olens, check_size=None):
+        """Validated (mels fp32, olens int64, B, Lmax) of a call whose only inputs they are.  check_size(B, Lmax): the
+        limits (default: the whole call's)."""
+        self._check_mels_olens(mels, olens)
+        if not mels.is_cuda or not olens.is_cuda:
+            raise ValueError("mels and olens must be CUDA tensors (the H100 path has no CPU fallback)")
+        B, L, _ = mels.shape
+        (check_size or self._check_size)(B, L)
+        return mels.to(torch.float32).contiguous(), olens.to(device=mels.device, dtype=torch.int64).contiguous(), B, L
+
+    def _check_rows(self, rows: int, formula: str, noun: str, where: str, advice: str) -> None:
+        """The limits the C entries put on the rows of their largest buffer, raised here as ValueError: below 2^31, and at
+        most 65535 * 128 in fp32 mode (its CUDA-core GEMMs put 128-row tiles on grid.y)."""
+        if rows >= 1 << 31:
+            raise ValueError(f"{formula} must stay below 2^31 {noun} rows ({where})")
+        if self.math_mode == "fp32" and rows > 65535 * 128:
+            raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 {noun} rows, {formula} = {rows} ({where}); {advice}")
+
+    def _check_size(self, B: int, L: int) -> None:
+        """_check_rows on the whole call's rows."""
+        self._check_rows(*self._rows(B, L), f"B={B}, Lmax={L}", "split the batch or use another math mode")
+
+    def _whole(self, call, mels, olens, B: int, L: int):
+        """The whole call on validated mels / olens: -> (audio [B, Lmax * HOP], alens = olens * HOP)."""
+        dev = mels.device
+        h = self._handle(dev)
+        ws = self._workspace(h, B, L, dev)
+        audio = torch.empty((B, L * self.HOP), dtype=torch.float32, device=dev)
+        status = torch.empty((1,), dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            call(h, mels, olens, B, L, audio, status, ws)
+        self._check_status(status)
+        return audio, olens * self.HOP
+
+    # ---- windows (MelGAN and WaveGlow) ----------------------------------------------------------------------------
+    def _window_workspace(self, h, B: int, n_frames: int, device: torch.device) -> torch.Tensor:
+        return workspace(self._wws, device, query_bytes(self._WINDOW_BYTES, h, B, n_frames))
 
     @staticmethod
     def _check_frames(n_frames) -> None:
@@ -182,15 +271,9 @@ class WindowedVocoder(nn.Module):
             raise ValueError(f"n_frames / chunk_frames must be an int >= 1 (got {n_frames!r})")
 
     def _check_window_size(self, B: int, n_frames: int) -> None:
-        """The window entry's limits on its rows, raised here as ValueError: below 2^31, and at most 65535 * 128 in fp32
-        mode (its CUDA-core GEMMs put 128-row tiles on grid.y)."""
+        """_check_rows on a window's rows."""
         self._check_frames(n_frames)
-        rows, formula = self._window_rows(B, n_frames)
-        if rows >= 1 << 31:
-            raise ValueError(f"{formula} must stay below 2^31 window rows (B={B}, n_frames={n_frames})")
-        if self.math_mode == "fp32" and rows > 65535 * 128:
-            raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 window rows, {formula} = {rows} "
-                             f"(B={B}, n_frames={n_frames}); use fewer frames per window")
+        self._check_rows(*self._window_rows(B, n_frames), "window", f"B={B}, n_frames={n_frames}", "use fewer frames per window")
 
     @staticmethod
     def _starts(starts, B: int, device: torch.device) -> torch.Tensor:

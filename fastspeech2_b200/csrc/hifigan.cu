@@ -158,34 +158,6 @@ __global__ void __launch_bounds__(256) hifigan_post_kernel(const float* __restri
   }
 }
 
-// GEMM weight [taps][N][K] from a folded torch-layout weight:
-//   kind 0  Conv1d w [N][K][taps]               -> dst[j][n][c] = w[n][c][j]
-//   kind 1  ConvTranspose1d w [K][Cout][2u]     -> dst[j][r Cout + co][ci] = w[ci][co][k(r, j)], taps = 3, tap j reading input
-//           row t + j - 1 (0 where phase r does not read it): k = r + u/2 + u (j = 0), r + u/2 (j = 1) for r < u/2;
-//           r + u/2 (j = 1), r + u/2 - u (j = 2) for r >= u/2
-__global__ void hifigan_pack_kernel(int kind, const float* __restrict__ w, int N, int K, int taps, int Cout, int u, float* __restrict__ dst) {
-  const long nk = (long)N * K, total = nk * taps;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const int j = (int)(i / nk);
-    const long rem = i - (long)j * nk;
-    const int n = (int)(rem / K), c = (int)(rem - (long)n * K);
-    float v;
-    if (kind == 0) {
-      v = w[((long)n * K + c) * taps + j];
-    } else {
-      const int r = n / Cout, co = n - r * Cout, p = u / 2;
-      const int kk = r < p ? (j == 1 ? r + p : j == 0 ? r + p + u : -1) : (j == 2 ? r + p - u : j == 1 ? r + p : -1);
-      v = kk >= 0 ? w[((long)c * Cout + co) * (2 * u) + kk] : 0.f;
-    }
-    dst[i] = v;
-  }
-}
-
-// dst[n] = b[n % Cout]
-__global__ void hifigan_bias_kernel(const float* __restrict__ b, int N, int Cout, float* __restrict__ dst) {
-  for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < N; n += gridDim.x * blockDim.x) dst[n] = b[n % Cout];
-}
-
 // ---- host side ------------------------------------------------------------------------------------------------------
 
 // what a config implies: widths, cumulative upsampling, convolutions per resblock and in all
@@ -303,15 +275,7 @@ HgPlan plan(Bump& b, const Shape& sh, int B, int L) {
   return p;
 }
 
-// GEMM weight from its torch-layout tensors: packed fp32 [taps][N][K], bias [N], scale and fp16 planes
-int pack_weight(const VWeight& w, int kind, const float* wt, const float* b, int Cout, int u, cudaStream_t st) {
-  hifigan_pack_kernel<<<grid_for((long)w.taps * w.N * w.K, 256), 256, 0, st>>>(kind, wt, w.N, w.K, w.taps, Cout, u, w.w);
-  FS2_LAUNCH_CHECK();
-  hifigan_bias_kernel<<<grid_for(w.N, 256), 256, 0, st>>>(b, w.N, Cout, w.bias);
-  FS2_LAUNCH_CHECK();
-  return vweight_planes(w, st);
-}
-
+// a GEMM weight here is [taps][N][K] tap matrices with K = Cin, so vweight_pack_conv packs it at tap_stride = N K
 void set_conv(VWeight& w, int N, int K, int taps) { w.N = N; w.K = K; w.taps = taps; }
 
 int check_size(int math_mode, int B, int L) {
@@ -381,17 +345,6 @@ int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const
   return FS2_OK;
 }
 
-// a stream-ordered temporary for the single-layer entries: carve(Bump&) on a counting pass, then on the allocation
-template <typename Carve>
-int temp_carve(void** base, cudaStream_t st, Carve carve) {
-  Bump count(nullptr, 0);
-  carve(count);
-  FS2_CUDA_CHECK(cudaMallocAsync(base, count.off + 256, st));
-  Bump b(*base, count.off + 256);
-  carve(b);
-  return FS2_OK;
-}
-
 }  // namespace
 }  // namespace fs2
 
@@ -443,14 +396,17 @@ int fs2_hifigan_load(fs2_hifigan_gen* m, const float* const* weights, const floa
     return FS2_OK;
   });
   if (rc) return rc;
-  if ((rc = pack_weight(m->pre, 0, weights[0], biases[0], sh.C[0], 0, st))) return rc;
-  for (int s = 0; s < sh.U; ++s)
-    if ((rc = pack_weight(m->up[s], 1, weights[1 + s], biases[1 + s], sh.C[s + 1], m->cfg.upsample_rates[s], st))) return rc;
-  for (size_t i = 0; i < m->blk.size(); ++i)
-    if ((rc = pack_weight(m->blk[i], 0, weights[1 + sh.U + i], biases[1 + sh.U + i], m->blk[i].N, 0, st))) return rc;
+  if ((rc = vweight_pack_conv(m->pre, weights[0], biases[0], kMels, sh.C[0], kPreTaps, 0, (long)sh.C[0] * kMels, st))) return rc;
+  for (int s = 0; s < sh.U; ++s) {
+    const VWeight& w = m->up[s];
+    if ((rc = vweight_pack_conv(w, weights[1 + s], biases[1 + s], w.K, sh.C[s + 1], 3, m->cfg.upsample_rates[s], (long)w.N * w.K, st))) return rc;
+  }
+  for (size_t i = 0; i < m->blk.size(); ++i) {
+    const VWeight& w = m->blk[i];
+    if ((rc = vweight_pack_conv(w, weights[1 + sh.U + i], biases[1 + sh.U + i], w.K, w.N, w.taps, 0, (long)w.N * w.K, st))) return rc;
+  }
   const int C = sh.C[sh.U], last = sh.layers - 1;
-  hifigan_pack_kernel<<<grid_for((long)kPostTaps * C, 256), 256, 0, st>>>(0, weights[last], 1, C, kPostTaps, 1, 0, m->post_w);
-  FS2_LAUNCH_CHECK();
+  if ((rc = conv_pack(weights[last], 1, C, kPostTaps, 1, 0, C, C, m->post_w, st))) return rc;
   FS2_CUDA_CHECK(cudaMemcpyAsync(m->post_b, biases[last], sizeof(float), cudaMemcpyDeviceToDevice, st));
   m->loaded = true;
   return FS2_OK;
@@ -511,7 +467,7 @@ int fs2_op_hifigan_resblock(int math_mode, int type, int C, int k, int nd, const
   });
   if (rc) return rc;
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
-  for (int i = 0; i < per && !rc; ++i) rc = pack_weight(w[i], 0, weights[i], biases[i], C, 0, st);
+  for (int i = 0; i < per && !rc; ++i) rc = vweight_pack_conv(w[i], weights[i], biases[i], C, C, k, 0, (long)C * C, st);
   if (!rc) rc = resblock(math_mode, type, w, dils, x, lens, B, Lp, C, a, t, out, status, st);
   cudaFreeAsync(base, st);
   return rc;
@@ -542,7 +498,7 @@ int fs2_op_hifigan_upsample(int math_mode, int Cin, int Cout, int u, const float
   });
   if (rc) return rc;
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
-  rc = pack_weight(wu, 1, w, b, Cout, u, st);
+  rc = vweight_pack_conv(wu, w, b, Cin, Cout, 3, u, (long)wu.N * Cin, st);
   if (!rc) rc = upsample(math_mode, wu, x, nullptr, 1, lens, B, Lin, Cin, a, out, status, st);
   cudaFreeAsync(base, st);
   return rc;

@@ -424,38 +424,6 @@ __global__ void __launch_bounds__(256) melgan_post_kernel(const float* __restric
   }
 }
 
-// GEMM weight [N][K] from a folded torch-layout weight:
-//   kind 0  Conv1d w [N][Cin][taps]              -> dst[n][j Cin + c] = w[n][c][j]
-//   kind 1  ConvTranspose1d w [Cin][Cout][2s]    -> dst[r Cout + co][j Cin + ci] = w[ci][co][k(r, j)] (0 where phase r
-//           does not read input row t + j - 1): k = r + s/2 + s for j = 0, r + s/2 for j = 1 (r < s/2); r + s/2 - s for
-//           j = 2, r + s/2 for j = 1 (r >= s/2)
-//   kind 2  [W2 | Ws], both [N][Cin][1]           -> dst[n][c] = W2[n][c], dst[n][Cin + c] = Ws[n][c]
-__global__ void melgan_pack_kernel(int kind, const float* __restrict__ w, const float* __restrict__ w2, int N, int K, int Cin, int Cout,
-                                   int taps, int s, float* __restrict__ dst) {
-  const long total = (long)N * K;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const int n = (int)(i / K), k = (int)(i - (long)n * K);
-    float v;
-    if (kind == 0) {
-      const int j = k / Cin, c = k - j * Cin;
-      v = w[((long)n * Cin + c) * taps + j];
-    } else if (kind == 1) {
-      const int r = n / Cout, co = n - r * Cout, j = k / Cin, ci = k - j * Cin, p = s / 2;
-      const int kk = r < p ? (j == 1 ? r + p : j == 0 ? r + p + s : -1) : (j == 2 ? r + p - s : j == 1 ? r + p : -1);
-      v = kk >= 0 ? w[((long)ci * Cout + co) * (2 * s) + kk] : 0.f;
-    } else {
-      v = k < Cin ? w[(long)n * Cin + k] : w2[(long)n * Cin + k - Cin];
-    }
-    dst[i] = v;
-  }
-}
-
-// dst[n] = b[n % Cout] (+ b2[n])
-__global__ void melgan_bias_kernel(const float* __restrict__ b, const float* __restrict__ b2, int N, int Cout, float* __restrict__ dst) {
-  for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < N; n += gridDim.x * blockDim.x)
-    dst[n] = b2 ? b[n] + b2[n] : b[n % Cout];
-}
-
 }  // namespace
 }  // namespace fs2
 
@@ -507,19 +475,6 @@ MgPlan plan(Bump& b, int B, int L, bool fused) {
   p.x[1] = b.floats(frames * kActPerFrame);
   p.h = fused ? nullptr : b.floats(frames * kActPerFrame);
   return p;
-}
-
-
-
-// one GEMM weight from its torch-layout tensors (melgan_pack_kernel's kind, Cin, Cout, taps, s): the packed fp32 [N][K],
-// the bias [N], the power-of-two scale and the fp16 planes; w->N, w->K and the buffers are set by the caller
-int pack_weight(const VWeight& w, int kind, const float* wt, const float* wt2, const float* b, const float* b2, int Cin, int Cout, int taps,
-                int s, cudaStream_t st) {
-  melgan_pack_kernel<<<grid_for((long)w.N * w.K, 256), 256, 0, st>>>(kind, wt, wt2, w.N, w.K, Cin, Cout, taps, s, w.w);
-  FS2_LAUNCH_CHECK();
-  melgan_bias_kernel<<<grid_for(w.N, 256), 256, 0, st>>>(b, b2, w.N, Cout, w.bias);
-  FS2_LAUNCH_CHECK();
-  return vweight_planes(w, st);
 }
 
 // the taps producer: operand rows [B * Lp] (window win, lens) from x, ldx rows per utterance in window xwin (nullptr: the
@@ -665,16 +620,18 @@ int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float*
   cudaStream_t st = (cudaStream_t)stream;
   // layer index of the state_dict order: 0 = generator.1; stage s: 1 + 10 s = its ConvTranspose1d, then the ResStack's
   // blocks.i.2 (2 + 10 s + 2 i), blocks.i.4 (3 + 10 s + 2 i), shortcuts.i (8 + 10 s + i); 41 = generator.16
-  struct Job { VWeight* w; int kind, N, K, Cin, Cout, taps, s; int l, l2; };
+  // A GEMM weight here is [N][K] with a convolution's taps side by side along K (vweight_pack_conv at tap_stride = Cin); a
+  // residual block's 1x1 convolution and its shortcut (l2) share one weight [W2 | Ws] over the operand [h | x]
+  struct Job { VWeight* w; int N, K, Cin, Cout, taps, s; int l, l2; };
   Job jobs[1 + kStages * 7];
   int nj = 0;
-  jobs[nj++] = {&m->pre, 0, 512, kMels * kPreTaps, kMels, 512, kPreTaps, 0, 0, -1};
+  jobs[nj++] = {&m->pre, 512, kMels * kPreTaps, kMels, 512, kPreTaps, 0, 0, -1};
   for (int s = 0; s < kStages; ++s) {
     const int ci = kCin[s], co = kCout[s], sd = kStride[s], base = 1 + 10 * s;
-    jobs[nj++] = {&m->up[s], 1, sd * co, 3 * ci, ci, co, 0, sd, base, -1};
+    jobs[nj++] = {&m->up[s], sd * co, 3 * ci, ci, co, 3, sd, base, -1};
     for (int i = 0; i < 3; ++i) {
-      jobs[nj++] = {&m->dil[s][i], 0, co, 3 * co, co, co, 3, 0, base + 1 + 2 * i, -1};
-      jobs[nj++] = {&m->pair[s][i], 2, co, 2 * co, co, co, 1, 0, base + 2 + 2 * i, base + 7 + i};
+      jobs[nj++] = {&m->dil[s][i], co, 3 * co, co, co, 3, 0, base + 1 + 2 * i, -1};
+      jobs[nj++] = {&m->pair[s][i], co, 2 * co, co, co, 1, 0, base + 2 + 2 * i, base + 7 + i};
     }
   }
   for (int j = 0; j < nj; ++j) { jobs[j].w->N = jobs[j].N; jobs[j].w->K = jobs[j].K; }
@@ -688,12 +645,11 @@ int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float*
   if (rc) return rc;
   for (int j = 0; j < nj; ++j) {
     const Job& q = jobs[j];
-    rc = pack_weight(*q.w, q.kind, weights[q.l], q.l2 >= 0 ? weights[q.l2] : nullptr, biases[q.l], q.l2 >= 0 ? biases[q.l2] : nullptr,
-                     q.Cin, q.Cout, q.taps, q.s, st);
+    rc = vweight_pack_conv(*q.w, weights[q.l], biases[q.l], q.Cin, q.Cout, q.taps, q.s, q.Cin, st, q.l2 >= 0 ? weights[q.l2] : nullptr,
+                           q.l2 >= 0 ? biases[q.l2] : nullptr);
     if (rc) return rc;
   }
-  melgan_pack_kernel<<<1, 256, 0, st>>>(0, weights[kLayers - 1], nullptr, 1, kPostTaps * kPostC, kPostC, 1, kPostTaps, 0, m->post_w);
-  FS2_LAUNCH_CHECK();
+  if ((rc = conv_pack(weights[kLayers - 1], 1, kPostC, kPostTaps, 1, 0, kPostC, kPostTaps * kPostC, m->post_w, st))) return rc;
   FS2_CUDA_CHECK(cudaMemcpyAsync(m->post_b, biases[kLayers - 1], sizeof(float), cudaMemcpyDeviceToDevice, st));
   m->loaded = true;
   return FS2_OK;
@@ -776,17 +732,16 @@ int fs2_op_melgan_block(int math_mode, int route, int C, const float* x, const i
   void* a = nullptr;
   float* h = nullptr;
   void* base = nullptr;
-  for (int pass = 0; pass < 2; ++pass) {       // pass 0 sizes the temporary, pass 1 carves it
-    Bump b(base, (size_t)-1);
+  int rc = temp_carve(&base, st, [&](Bump& b) {
     vweight_carve(b, wd, true);
     vweight_carve(b, wp, true);
     a = b.floats((size_t)rows * 3 * C);
     h = b.floats((size_t)rows * C);
-    if (pass == 0) FS2_CUDA_CHECK(cudaMallocAsync(&base, b.off + 256, st));
-  }
+  });
+  if (rc) return rc;
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
-  int rc = pack_weight(wd, 0, w1, nullptr, b1, nullptr, C, C, 3, 0, st);
-  if (!rc) rc = pack_weight(wp, 2, w2, ws, b2, bs, C, C, 1, 0, st);
+  rc = vweight_pack_conv(wd, w1, b1, C, C, 3, 0, C, st);
+  if (!rc) rc = vweight_pack_conv(wp, w2, b2, C, C, 1, 0, C, st, ws, bs);
   if (!rc) rc = res_block(math_mode, fused, wd, wp, x, lens, nullptr, B, Lp, C, d, 0, a, h, out, status, st);
   cudaFreeAsync(base, st);
   return rc;
@@ -811,14 +766,13 @@ int fs2_op_melgan_upsample(int math_mode, int Cin, int Cout, int s, const float*
   wu.N = s * Cout; wu.K = 3 * Cin;
   void* a = nullptr;
   void* base = nullptr;
-  for (int pass = 0; pass < 2; ++pass) {
-    Bump bb(base, (size_t)-1);
+  int rc = temp_carve(&base, st, [&](Bump& bb) {
     vweight_carve(bb, wu, true);
     a = bb.floats((size_t)rows * 3 * Cin);
-    if (pass == 0) FS2_CUDA_CHECK(cudaMallocAsync(&base, bb.off + 256, st));
-  }
+  });
+  if (rc) return rc;
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
-  int rc = pack_weight(wu, 1, w, nullptr, b, nullptr, Cin, Cout, 0, s, st);
+  rc = vweight_pack_conv(wu, w, b, Cin, Cout, 3, s, Cin, st);
   if (!rc) rc = upsample(math_mode, wu, x, nullptr, Lin, lens, nullptr, B, Lin, Cin, a, out, status, st);
   cudaFreeAsync(base, st);
   return rc;

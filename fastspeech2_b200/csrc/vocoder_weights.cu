@@ -16,6 +16,36 @@ __global__ void pad_pack_kernel(const float* __restrict__ src, int SR, int SC, i
   }
 }
 
+// Element (tap j, row n, column c) of a convolution's GEMM weight, at dst[j * tap_stride + n * row_stride + c], from the
+// folded torch-layout weight:
+//   u == 0  Conv1d w [N][Cin][taps]            -> w[n][c][j]
+//   u >= 2  ConvTranspose1d w [Cin][Cout][2u]  -> row n = r Cout + co is output phase r, taps = 3, tap j reading input row
+//           t + j - 1: w[c][co][k(r, j)] (0 where phase r does not read that row), k = r + u/2 + u (j = 0), r + u/2 (j = 1)
+//           for r < u/2; r + u/2 (j = 1), r + u/2 - u (j = 2) for r >= u/2
+__global__ void conv_pack_kernel(const float* __restrict__ w, int N, int Cin, int taps, int Cout, int u, long tap_stride, long row_stride,
+                                 float* __restrict__ dst) {
+  const long nc = (long)N * Cin, total = nc * taps;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int j = (int)(i / nc);
+    const long rem = i - (long)j * nc;
+    const int n = (int)(rem / Cin), c = (int)(rem - (long)n * Cin);
+    float v;
+    if (u == 0) {
+      v = w[((long)n * Cin + c) * taps + j];
+    } else {
+      const int r = n / Cout, co = n - r * Cout, p = u / 2;
+      const int kk = r < p ? (j == 1 ? r + p : j == 0 ? r + p + u : -1) : (j == 2 ? r + p - u : j == 1 ? r + p : -1);
+      v = kk >= 0 ? w[((long)c * Cout + co) * (2 * u) + kk] : 0.f;
+    }
+    dst[j * tap_stride + n * row_stride + c] = v;
+  }
+}
+
+// dst[n] = b[n % Cout] (+ b2[n])
+__global__ void conv_bias_kernel(const float* __restrict__ b, const float* __restrict__ b2, int N, int Cout, float* __restrict__ dst) {
+  for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < N; n += gridDim.x * blockDim.x) dst[n] = b2 ? b[n % Cout] + b2[n] : b[n % Cout];
+}
+
 }  // namespace
 
 void vweight_carve(Bump& b, VWeight& w, bool bias) {
@@ -33,6 +63,22 @@ int vweight_planes(const VWeight& w, cudaStream_t st) {
 int vweight_pack(VWeight& w, const float* src, int SR, int SC, int transpose, cudaStream_t st) {
   const long n = (long)w.N * w.K;
   pad_pack_kernel<<<grid_for(n, 256), 256, 0, st>>>(src, SR, SC, transpose, w.w, w.N, w.K);
+  FS2_LAUNCH_CHECK();
+  return vweight_planes(w, st);
+}
+
+int conv_pack(const float* wt, int N, int Cin, int taps, int Cout, int u, long tap_stride, long row_stride, float* dst, cudaStream_t st) {
+  conv_pack_kernel<<<grid_for((long)taps * N * Cin, 256), 256, 0, st>>>(wt, N, Cin, taps, Cout, u, tap_stride, row_stride, dst);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+int vweight_pack_conv(const VWeight& w, const float* wt, const float* b, int Cin, int Cout, int taps, int u, long tap_stride, cudaStream_t st,
+                      const float* wt2, const float* b2) {
+  int rc = conv_pack(wt, w.N, Cin, taps, Cout, u, tap_stride, w.K, w.w, st);
+  if (!rc && wt2) rc = conv_pack(wt2, w.N, Cin, taps, Cout, u, tap_stride, w.K, w.w + Cin, st);
+  if (rc) return rc;
+  conv_bias_kernel<<<grid_for(w.N, 256), 256, 0, st>>>(b, b2, w.N, Cout, w.bias);
   FS2_LAUNCH_CHECK();
   return vweight_planes(w, st);
 }

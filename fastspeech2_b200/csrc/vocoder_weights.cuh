@@ -1,5 +1,5 @@
 // The library's GEMM weights (the acoustic model in api.cu, the train convolutions in train.cu and the signal modules
-// melgan.cu, waveglow.cu, griffin_lim.cu, features.cu): one [taps][N][K] matrix held as fp32 rows (fp32 / tf32 math modes)
+// melgan.cu, hifigan.cu, waveglow.cu, griffin_lim.cu, features.cu): one [taps][N][K] matrix held as fp32 rows (fp32 / tf32 math modes)
 // and as power-of-two-scaled fp16 hi / lo planes (f16 / 3xF16), with an optional bias [N]; the tap-GEMM call over it, the
 // one place that maps a math mode to a tap-GEMM family; and the device arena a module's weights are carved from.
 #pragma once
@@ -20,6 +20,19 @@ int vweight_planes(const VWeight& w, cudaStream_t st);
 
 // fill w's buffers from src [SR][SC] (its transpose when `transpose`), zero-padded to [N][K]: fp32 rows, scale, planes
 int vweight_pack(VWeight& w, const float* src, int SR, int SC, int transpose, cudaStream_t st);
+
+// A convolution's GEMM rows from its folded torch-layout weight wt, element (tap j, row n, column c) at
+// dst[j * tap_stride + n * row_stride + c] for j < taps, n < N, c < Cin.  u == 0: Conv1d wt [N][Cin][taps].  u >= 2:
+// ConvTranspose1d wt [Cin][Cout][2u] (stride u, padding u / 2) as a polyphase matrix of taps = 3 and N = u Cout rows, row
+// r Cout + co being output phase r and tap j reading input row t + j - 1 (zeros where the phase does not read it).
+int conv_pack(const float* wt, int N, int Cin, int taps, int Cout, int u, long tap_stride, long row_stride, float* dst, cudaStream_t st);
+
+// w (its N, K and buffers set) from a convolution's torch-layout tensors: conv_pack into w.w at row stride w.K, taps side
+// by side along K (tap_stride = Cin, w.taps = 1) or as tap matrices (tap_stride = N K, w.taps = taps); bias [N] =
+// b[n % Cout]; scale and planes.  wt2, b2 (nullable): a second 1-tap convolution of the same rows, packed in columns
+// [Cin, 2 Cin) and its bias added, so that one GEMM over [x | y] computes wt . x + wt2 . y.
+int vweight_pack_conv(const VWeight& w, const float* wt, const float* b, int Cin, int Cout, int taps, int u, long tap_stride, cudaStream_t st,
+                      const float* wt2 = nullptr, const float* b2 = nullptr);
 
 // The TapGemm of out [B*L][w.N] = act(a [B*L][w.K] (w.taps taps at dilation dil) . w^T + w.bias) (+ resid [B*L][w.N]), a as
 // fp32 rows (fp32 / tf32) or as hi (+ lo) planes (f16 / 3xF16); rows t >= lens[b] are written as 0 (and skipped by the
@@ -56,6 +69,18 @@ int arena_carve(void** arena, size_t* cap, cudaStream_t st, Carve carve) {
   }
   Bump b(*arena, *cap);
   return carve(b);
+}
+
+// a stream-ordered temporary for the single-layer entries: carve(Bump&) on a counting pass, then on the allocation; the
+// caller releases *base with cudaFreeAsync on the same stream
+template <typename Carve>
+int temp_carve(void** base, cudaStream_t st, Carve carve) {
+  Bump count(nullptr, 0);
+  carve(count);
+  FS2_CUDA_CHECK(cudaMallocAsync(base, count.off + 256, st));
+  Bump b(*base, count.off + 256);
+  carve(b);
+  return FS2_OK;
 }
 
 }  // namespace fs2

@@ -20,11 +20,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._kernel_module import WindowedVocoder, _WNConv, normalise_checkpoint
-
-HOP = 256
-N_MELS = 80
-MAX_WAV_VALUE = 32768.0
+from ._kernel_module import HOP, MAX_WAV_VALUE, N_MELS, NeuralVocoder, _WNConv, normalise_checkpoint, read_checkpoint  # noqa: F401
 
 # hifi-gan's published config_v1.json, config_v2.json and config_v3.json (the fields the generator uses).  V2's widths
 # (128 ... 8) are refused by HiFiGANVocoder; the entry is here for its key list.
@@ -133,7 +129,7 @@ def add_layers(module: nn.Module, cfg: dict) -> nn.Module:
     return module
 
 
-class HiFiGANVocoder(WindowedVocoder):
+class HiFiGANVocoder(NeuralVocoder):
     """jik876/hifi-gan's `Generator(h)` on the H100 kernels.
 
     `forward(mels [B, Lmax, 80], olens [B])` -> (audio [B, Lmax * 256] fp32, alens = olens * 256).  Utterance b is the
@@ -144,15 +140,13 @@ class HiFiGANVocoder(WindowedVocoder):
     GEMMs.  One host read per call (the device-side length and range checks)."""
 
     _DESTROY, _WORKSPACE_BYTES, _WINDOW_BYTES = "fs2_hifigan_destroy", "fs2_hifigan_workspace_bytes", None
+    _STATUS = "FS2_HIFIGAN"
 
     def __init__(self, config="v1", math_mode: str = "3xf16"):
-        super().__init__()
-        if math_mode not in _lib.MATH_MODES:
-            raise ValueError(f"math_mode must be one of {sorted(_lib.MATH_MODES)}")
+        super().__init__(math_mode)
         cfg = load_config(config)
         check_config(cfg)
         self.config = cfg
-        self.math_mode = math_mode
         add_layers(self, cfg)
         self._layers = [m for m in self.modules() if isinstance(m, _WNConv)]      # state_dict order
 
@@ -195,13 +189,7 @@ class HiFiGANVocoder(WindowedVocoder):
                 raise ValueError(f"config is required: no config.json beside {sd}")
             config = path
         voc = cls(config, math_mode=math_mode)
-        if isinstance(sd, (str, os.PathLike)):
-            sd = torch.load(sd, map_location="cpu", weights_only=True)
-        if not isinstance(sd, dict):
-            raise ValueError("expected a checkpoint dict (with 'generator') or a generator state dict")
-        if "generator" in sd:
-            sd = sd["generator"]
-        voc.load_state_dict(normalise_checkpoint(voc, sd))
+        voc.load_state_dict(normalise_checkpoint(voc, read_checkpoint(sd, "generator", "a generator state dict")))
         return voc
 
     # ---- device state ---------------------------------------------------------------------------------------------
@@ -228,51 +216,19 @@ class HiFiGANVocoder(WindowedVocoder):
         return h.value
 
     def _load(self, h, device: torch.device) -> None:
-        ws = [m.folded().to(device).contiguous() for m in self._layers]
-        bs = [m.bias.detach().float().to(device).contiguous() for m in self._layers]
-        wp = (C.c_void_p * len(ws))(*[t.data_ptr() for t in ws])
-        bp = (C.c_void_p * len(bs))(*[t.data_ptr() for t in bs])
-        _lib.check(_lib.load().fs2_hifigan_load(h, wp, bp, _lib.stream_ptr(device)), "fs2_hifigan_load")
+        self._load_layers("fs2_hifigan_load", h, device)
 
-    def _inputs(self, mels, olens):
-        if not torch.is_tensor(mels) or mels.dim() != 3 or mels.shape[2] != N_MELS or mels.shape[0] == 0 or mels.shape[1] == 0:
-            raise ValueError(f"mels must be a non-empty [B, Lmax, {N_MELS}] tensor")
-        if not torch.is_tensor(olens) or olens.dim() != 1 or olens.shape[0] != mels.shape[0]:
-            raise ValueError(f"olens must be a [B={mels.shape[0]}] tensor")
-        if olens.dtype.is_floating_point or olens.dtype == torch.bool:
-            raise ValueError("olens must be an integer tensor")
-        if not mels.is_cuda or not olens.is_cuda:
-            raise ValueError("mels and olens must be CUDA tensors (the H100 path has no CPU fallback)")
-        B, L, _ = mels.shape
-        self._check_size(B, L)
-        return mels.to(torch.float32).contiguous(), olens.to(device=mels.device, dtype=torch.int64).contiguous(), B, L
+    def _rows(self, B: int, L: int):
+        """fs2_hifigan's largest buffer: B * Lmax * 256 sample rows."""
+        return B * L * HOP, f"B * Lmax * {HOP}", "sample"
 
-    def _check_size(self, B: int, L: int) -> None:
-        """The limits fs2_hifigan checks, raised here as ValueError: B * Lmax * 256 sample rows below 2^31, and at most
-        65535 * 128 in fp32 mode (its CUDA-core GEMMs put 128-row tiles on grid.y)."""
-        rows = B * L * HOP
-        if rows >= 1 << 31:
-            raise ValueError(f"B * Lmax * {HOP} must stay below 2^31 sample rows (B={B}, Lmax={L})")
-        if self.math_mode == "fp32" and rows > 65535 * 128:
-            raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 sample rows, B * Lmax * {HOP} = {rows} "
-                             f"(B={B}, Lmax={L}); split the batch or use another math mode")
-
-    def _status_table(self):
-        return [(_lib.FS2_HIFIGAN_BAD_LENGTH, "every olens[b] must lie in [1, Lmax]"),
-                (_lib.FS2_HIFIGAN_RANGE, f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
-                                         f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'")]
+    @staticmethod
+    def _call(h, mels, olens, B: int, L: int, audio: torch.Tensor, status: torch.Tensor, ws: torch.Tensor) -> None:
+        _lib.check(_lib.load().fs2_hifigan(h, _lib.ptr(mels), _lib.ptr(olens), B, L, _lib.ptr(audio), _lib.ptr(status), _lib.ptr(ws),
+                                           ws.numel(), _lib.stream_ptr(mels.device)), "fs2_hifigan")
 
     # ---- synthesis ------------------------------------------------------------------------------------------------
     def forward(self, mels: torch.Tensor, olens: torch.Tensor):
         """-> (audio [B, Lmax * 256] fp32, alens [B] int64 = olens * 256)."""
-        mels, olens, B, L = self._inputs(mels, olens)
-        dev = mels.device
-        h = self._handle(dev)
-        ws = self._workspace(h, B, L, dev)
-        audio = torch.empty((B, L * HOP), dtype=torch.float32, device=dev)
-        status = torch.empty((1,), dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.load().fs2_hifigan(h, _lib.ptr(mels), _lib.ptr(olens), B, L, _lib.ptr(audio), _lib.ptr(status), _lib.ptr(ws),
-                                               ws.numel(), _lib.stream_ptr(dev)), "fs2_hifigan")
-        self._check_status(status)
-        return audio, olens * HOP
+        mels, olens, B, L = self._mels_olens(mels, olens)
+        return self._whole(self._call, mels, olens, B, L)

@@ -12,17 +12,13 @@ against a real checkpoint file.
 from __future__ import annotations
 
 import ctypes as C
-import os
 
 import torch
 import torch.nn as nn
 
 from . import _lib
-from ._kernel_module import WindowedVocoder, _WNConv, normalise_checkpoint
+from ._kernel_module import HOP, MAX_WAV_VALUE, N_MELS, NeuralVocoder, _WNConv, normalise_checkpoint, read_checkpoint
 
-HOP = 256
-N_MELS = 80
-MAX_WAV_VALUE = 32768.0
 _STAGES = ((512, 256, 8), (256, 128, 8), (128, 64, 2), (64, 32, 2))    # ConvTranspose1d (Cin, Cout, stride), k = 2 * stride
 
 
@@ -43,7 +39,7 @@ def _generator() -> nn.Sequential:
     return nn.Sequential(*mods)
 
 
-class MelGANVocoder(WindowedVocoder):
+class MelGANVocoder(NeuralVocoder):
     """seungwonpark/melgan's `Generator(mel_channel=80)` on the H100 kernels.
 
     `forward(mels [B, Lmax, 80], olens [B])` -> (audio [B, Lmax * 256] fp32, alens = olens * 256).  Utterance b is the
@@ -54,12 +50,10 @@ class MelGANVocoder(WindowedVocoder):
     host read per call (the device-side length and range checks)."""
 
     _DESTROY, _WORKSPACE_BYTES, _WINDOW_BYTES = "fs2_melgan_destroy", "fs2_melgan_workspace_bytes", "fs2_melgan_window_workspace_bytes"
+    _STATUS = "FS2_MELGAN"
 
     def __init__(self, math_mode: str = "3xf16"):
-        super().__init__()
-        if math_mode not in _lib.MATH_MODES:
-            raise ValueError(f"math_mode must be one of {sorted(_lib.MATH_MODES)}")
-        self.math_mode = math_mode
+        super().__init__(math_mode)
         self.mel_channel = N_MELS
         self.generator = _generator()
         self._layers = [m for m in self.modules() if isinstance(m, _WNConv)]      # state_dict order, 42 convolutions
@@ -71,13 +65,7 @@ class MelGANVocoder(WindowedVocoder):
         or as the loaded dict.  Either may hold `weight_g` / `weight_v` keys or plain `weight` keys (after
         `remove_weight_norm`, what the hub object holds); a plain weight w is stored as v = w, g = |w|, which folds back to
         w bit for bit.  A missing, unexpected or wrongly shaped key raises ValueError naming it."""
-        sd = path_or_dict
-        if isinstance(sd, (str, os.PathLike)):
-            sd = torch.load(sd, map_location="cpu", weights_only=True)
-        if not isinstance(sd, dict):
-            raise ValueError("expected a checkpoint dict (with 'model_g') or a generator state dict")
-        if "model_g" in sd:
-            sd = sd["model_g"]
+        sd = read_checkpoint(path_or_dict, "model_g", "a generator state dict")
         voc = cls(math_mode=math_mode)
         voc.load_state_dict(normalise_checkpoint(voc, sd))
         return voc
@@ -95,34 +83,11 @@ class MelGANVocoder(WindowedVocoder):
         return h.value
 
     def _load(self, h, device: torch.device) -> None:
-        ws = [m.folded().to(device).contiguous() for m in self._layers]
-        bs = [m.bias.detach().float().to(device).contiguous() for m in self._layers]
-        wp = (C.c_void_p * len(ws))(*[t.data_ptr() for t in ws])
-        bp = (C.c_void_p * len(bs))(*[t.data_ptr() for t in bs])
-        _lib.check(_lib.load().fs2_melgan_load(h, wp, bp, _lib.stream_ptr(device)), "fs2_melgan_load")
+        self._load_layers("fs2_melgan_load", h, device)
 
-    def _inputs(self, mels, olens, check_size=None):
-        if not torch.is_tensor(mels) or mels.dim() != 3 or mels.shape[2] != N_MELS or mels.shape[0] == 0 or mels.shape[1] == 0:
-            raise ValueError(f"mels must be a non-empty [B, Lmax, {N_MELS}] tensor")
-        if not torch.is_tensor(olens) or olens.dim() != 1 or olens.shape[0] != mels.shape[0]:
-            raise ValueError(f"olens must be a [B={mels.shape[0]}] tensor")
-        if olens.dtype.is_floating_point or olens.dtype == torch.bool:
-            raise ValueError("olens must be an integer tensor")
-        if not mels.is_cuda or not olens.is_cuda:
-            raise ValueError("mels and olens must be CUDA tensors (the H100 path has no CPU fallback)")
-        B, L, _ = mels.shape
-        (check_size or self._check_size)(B, L)
-        return mels.to(torch.float32).contiguous(), olens.to(device=mels.device, dtype=torch.int64).contiguous(), B, L
-
-    def _check_size(self, B: int, L: int) -> None:
-        """The limits fs2_melgan checks, raised here as ValueError: B * (Lmax + 10) * 256 sample rows below 2^31, and at
-        most 65535 * 128 in fp32 mode (its CUDA-core GEMMs put 128-row tiles on grid.y)."""
-        rows = B * (L + 10) * HOP
-        if rows >= 1 << 31:
-            raise ValueError(f"B * (Lmax + 10) * {HOP} must stay below 2^31 sample rows (B={B}, Lmax={L})")
-        if self.math_mode == "fp32" and rows > 65535 * 128:
-            raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 sample rows, B * (Lmax + 10) * {HOP} = {rows} "
-                             f"(B={B}, Lmax={L}); split the batch or use another math mode")
+    def _rows(self, B: int, L: int):
+        """fs2_melgan's largest buffer: B * (Lmax + 10) * 256 sample rows."""
+        return B * (L + 10) * HOP, f"B * (Lmax + 10) * {HOP}", "sample"
 
     def _window_rows(self, B: int, n_frames: int):
         """fs2_melgan_window's largest buffer: B * (256 * n_frames + 36) rows."""
@@ -135,11 +100,10 @@ class MelGANVocoder(WindowedVocoder):
             _lib.check(_lib.load().fs2_melgan_window(h, _lib.ptr(mels), _lib.ptr(olens), _lib.ptr(starts), B, L, n_frames, audio.data_ptr(), ld,
                                                      _lib.ptr(status), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)), "fs2_melgan_window")
 
-    def _status_table(self):
-        return [(_lib.FS2_MELGAN_BAD_LENGTH, "every olens[b] must lie in [1, Lmax]"),
-                (_lib.FS2_MELGAN_BAD_START, "every starts[b] must be >= 0"),
-                (_lib.FS2_MELGAN_RANGE, f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
-                                        f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'")]
+    @staticmethod
+    def _call(h, mels, olens, B: int, L: int, audio: torch.Tensor, status: torch.Tensor, ws: torch.Tensor) -> None:
+        _lib.check(_lib.load().fs2_melgan(h, _lib.ptr(mels), _lib.ptr(olens), B, L, _lib.ptr(audio), _lib.ptr(status), _lib.ptr(ws),
+                                          ws.numel(), _lib.stream_ptr(mels.device)), "fs2_melgan")
 
     # ---- synthesis ------------------------------------------------------------------------------------------------
     def forward(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int | None = None):
@@ -151,26 +115,17 @@ class MelGANVocoder(WindowedVocoder):
         if chunk_frames is not None:
             mels, olens, B, L = self._window_inputs(mels, olens, chunk_frames)
             return self._chunked(self._window_call, mels, olens, B, L, chunk_frames)
-        mels, olens, B, L = self._inputs(mels, olens)
-        dev = mels.device
-        h = self._handle(dev)
-        ws = self._workspace(h, B, L, dev)
-        audio = torch.empty((B, L * HOP), dtype=torch.float32, device=dev)
-        status = torch.empty((1,), dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.load().fs2_melgan(h, _lib.ptr(mels), _lib.ptr(olens), B, L, _lib.ptr(audio), _lib.ptr(status), _lib.ptr(ws),
-                                              ws.numel(), _lib.stream_ptr(dev)), "fs2_melgan")
-        self._check_status(status)
-        return audio, olens * HOP
+        mels, olens, B, L = self._mels_olens(mels, olens)
+        return self._whole(self._call, mels, olens, B, L)
 
     def _window_inputs(self, mels, olens, n_frames):
-        """_inputs with the window's limits in place of the whole call's (Lmax bounds only the per-utterance rows)."""
+        """_mels_olens with the window's limits in place of the whole call's (Lmax bounds only the per-utterance rows)."""
         self._check_frames(n_frames)
         def check(B, L):
             self._check_window_size(B, n_frames)
             if (L + 10) * HOP >= 1 << 31:
                 raise ValueError(f"(Lmax + 10) * {HOP} must stay below 2^31 samples (Lmax={L})")
-        return self._inputs(mels, olens, check)
+        return self._mels_olens(mels, olens, check)
 
     def window(self, mels: torch.Tensor, olens: torch.Tensor, starts, n_frames: int):
         """One window of the audio (DESIGN.md section 11): -> (audio [B, n_frames * 256] fp32, alens [B] int64 =

@@ -16,16 +16,13 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
 
 import torch
 import torch.nn as nn
 
 from . import _lib
-from ._kernel_module import WindowedVocoder, _WNConv, normalise_checkpoint
+from ._kernel_module import HOP, N_MELS, NeuralVocoder, _WNConv, normalise_checkpoint, read_checkpoint
 
-HOP = 256
-N_MELS = 80
 N_GROUP = 8
 STEPS = HOP // N_GROUP              # step rows (groups of 8 samples) per mel frame
 N_FLOWS, N_LAYERS = 12, 8
@@ -69,7 +66,7 @@ class _WN(nn.Module):
         self.end = _Conv((2 * n_half, c, 1), 2 * n_half)           # zero-initialised, as in the published model
 
 
-class WaveGlowVocoder(WindowedVocoder):
+class WaveGlowVocoder(NeuralVocoder):
     """DeepLearningExamples' `WaveGlow` (n_mel_channels 80, n_flows 12, n_group 8, n_early_every 4, n_early_size 2, WN 8
     layers of kernel 3, n_channels C) on the H100 kernels.
 
@@ -94,15 +91,13 @@ class WaveGlowVocoder(WindowedVocoder):
 
     _DESTROY = "fs2_waveglow_destroy"
     _WORKSPACE_BYTES, _WINDOW_BYTES = "fs2_waveglow_workspace_bytes", "fs2_waveglow_window_workspace_bytes"
+    _STATUS = "FS2_WAVEGLOW"
 
     def __init__(self, n_channels: int = 512, math_mode: str = "3xf16"):
-        super().__init__()
-        if math_mode not in _lib.MATH_MODES:
-            raise ValueError(f"math_mode must be one of {sorted(_lib.MATH_MODES)}")
+        super().__init__(math_mode)
         if not isinstance(n_channels, int) or n_channels < 64 or n_channels > 1024 or n_channels % 64:
             raise ValueError(f"n_channels must be a multiple of 64 in [64, 1024] (the published models use 256 or 512), "
                              f"got {n_channels}")
-        self.math_mode = math_mode
         self.n_channels = n_channels
         self.n_mel_channels, self.n_flows, self.n_group = N_MELS, N_FLOWS, N_GROUP
         self.upsample = _Conv((N_MELS, N_MELS, 1024), N_MELS)
@@ -121,13 +116,7 @@ class WaveGlowVocoder(WindowedVocoder):
         `weight_g` / `weight_v` or plain `weight` keys (after `remove_weightnorm`); a plain weight w is stored as v = w,
         g = |w|, which folds back to w.  n_channels is read from WN.0.start's bias and checked against every other key: a
         missing, unexpected or wrongly shaped key raises ValueError naming it."""
-        sd = path_or_dict
-        if isinstance(sd, (str, os.PathLike)):
-            sd = torch.load(sd, map_location="cpu", weights_only=True)
-        if not isinstance(sd, dict):
-            raise ValueError("expected a checkpoint dict (with 'state_dict') or a WaveGlow state dict")
-        if "state_dict" in sd:
-            sd = sd["state_dict"]
+        sd = read_checkpoint(path_or_dict, "state_dict", "a WaveGlow state dict")
         if sd and all(isinstance(k, str) and k.startswith("module.") for k in sd):
             sd = {k[len("module."):]: v for k, v in sd.items()}
         b = sd.get("WN.0.start.bias")
@@ -173,13 +162,10 @@ class WaveGlowVocoder(WindowedVocoder):
         """Validated (mels fp32, olens int64, B, Lmax, sigma, seeds or None, z fp32 or None); every check that needs no
         device runs before the one that asks for CUDA tensors.  check_size(B, Lmax): the limits (default: the whole
         call's)."""
-        if not torch.is_tensor(mels) or mels.dim() != 3 or mels.shape[2] != N_MELS or mels.shape[0] == 0 or mels.shape[1] == 0:
-            raise ValueError(f"mels must be a non-empty [B, Lmax, {N_MELS}] tensor")
+        self._check_mels_olens(mels, olens)
         if not mels.dtype.is_floating_point:
             raise ValueError("mels must be a floating-point tensor")
-        if not torch.is_tensor(olens) or olens.dim() != 1 or olens.shape[0] != mels.shape[0]:
-            raise ValueError(f"olens must be a [B={mels.shape[0]}] tensor")
-        if olens.dtype.is_floating_point or olens.dtype.is_complex or olens.dtype == torch.bool:
+        if olens.dtype.is_complex:
             raise ValueError("olens must be an integer tensor")
         B, L, _ = mels.shape
         sigma = self._sigma(sigma)
@@ -198,15 +184,9 @@ class WaveGlowVocoder(WindowedVocoder):
             z = z.to(torch.float32).contiguous()
         return mels.to(torch.float32).contiguous(), olens.to(device=mels.device, dtype=torch.int64).contiguous(), B, L, sigma, seeds, z
 
-    def _check_size(self, B: int, L: int) -> None:
-        """The limits fs2_waveglow checks, raised here as ValueError: B * Lmax * 32 step rows below 2^31, and at most
-        65535 * 128 in fp32 mode (its CUDA-core GEMMs put 128-row tiles on grid.y)."""
-        rows = B * L * STEPS
-        if rows >= 1 << 31:
-            raise ValueError(f"B * Lmax * {STEPS} must stay below 2^31 step rows (B={B}, Lmax={L})")
-        if self.math_mode == "fp32" and rows > 65535 * 128:
-            raise ValueError(f"math_mode='fp32' takes at most 65535 * 128 step rows, B * Lmax * {STEPS} = {rows} "
-                             f"(B={B}, Lmax={L}); split the batch or use another math mode")
+    def _rows(self, B: int, L: int):
+        """fs2_waveglow's buffers: B * Lmax * 32 step rows."""
+        return B * L * STEPS, f"B * Lmax * {STEPS}", "step"
 
     @staticmethod
     def _seeds(seed, B: int, device) -> torch.Tensor:
@@ -227,12 +207,6 @@ class WaveGlowVocoder(WindowedVocoder):
         if isinstance(sigma, bool) or not isinstance(sigma, (int, float)) or not math.isfinite(sigma) or sigma < 0:
             raise ValueError(f"sigma must be a finite number >= 0, got {sigma!r}")
         return float(sigma)
-
-    def _status_table(self):
-        return [(_lib.FS2_WAVEGLOW_BAD_LENGTH, "every olens[b] must lie in [1, Lmax]"),
-                (_lib.FS2_WAVEGLOW_BAD_START, "every starts[b] must be >= 0"),
-                (_lib.FS2_WAVEGLOW_RANGE, f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
-                                          f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'")]
 
     # ---- synthesis ------------------------------------------------------------------------------------------------
     @classmethod
@@ -267,17 +241,11 @@ class WaveGlowVocoder(WindowedVocoder):
             mels, olens, B, L, sigma, seeds, z = self._window_inputs(mels, olens, chunk_frames, sigma, seed, z)
             return self._chunked(self._window_call(sigma, seeds, z), mels, olens, B, L, chunk_frames)
         mels, olens, B, L, sigma, seeds, z = self._inputs(mels, olens, sigma, seed, z)
-        dev = mels.device
-        h = self._handle(dev)
-        ws = self._workspace(h, B, L, dev)
-        audio = torch.empty((B, L * HOP), dtype=torch.float32, device=dev)
-        status = torch.empty((1,), dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(_lib.load().fs2_waveglow(h, _lib.ptr(mels), _lib.ptr(olens), B, L, sigma, _lib.ptr(seeds), _lib.ptr(z),
-                                                _lib.ptr(audio), _lib.ptr(status), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)),
-                       "fs2_waveglow")
-        self._check_status(status)
-        return audio, olens * HOP
+
+        def call(h, mels, olens, B: int, L: int, audio: torch.Tensor, status: torch.Tensor, ws: torch.Tensor) -> None:
+            _lib.check(_lib.load().fs2_waveglow(h, _lib.ptr(mels), _lib.ptr(olens), B, L, sigma, _lib.ptr(seeds), _lib.ptr(z), _lib.ptr(audio),
+                                                _lib.ptr(status), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(mels.device)), "fs2_waveglow")
+        return self._whole(call, mels, olens, B, L)
 
     # ---- windows (DESIGN.md section 12) ----------------------------------------------------------------------------
     def _window_rows(self, B: int, n_frames: int):

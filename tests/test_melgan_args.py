@@ -262,12 +262,23 @@ def test_melgan_kernels_do_not_spill():
     if not reports:
         pytest.skip("no ptxas reports (library built elsewhere)")
     text = open(reports[0]).read()
-    # instantiations: prep, post, pack, bias (1 each), pre_operand and concat (3 operand kinds), taps (3 x 2), the fused
-    # residual block (4 channel counts x f16 / 3xF16)
-    expected = {"melgan_prep_kernel": 1, "melgan_post_kernel": 1, "melgan_pack_kernel": 1, "melgan_bias_kernel": 1,
-                "melgan_pre_operand_kernel": 3, "melgan_concat_kernel": 3, "melgan_taps_kernel": 6, "melgan_block_kernel": 8}
+    # instantiations: prep, post (1 each), pre_operand and concat (3 operand kinds), taps (3 x 2), the fused residual block
+    # (4 channel counts x f16 / 3xF16)
+    expected = {"melgan_prep_kernel": 1, "melgan_post_kernel": 1, "melgan_pre_operand_kernel": 3, "melgan_concat_kernel": 3, "melgan_taps_kernel": 6, "melgan_block_kernel": 8}
     for kernel, n in expected.items():
         props = re.findall(r"Function properties for \S*%s\S*\n(.*)" % kernel, text)
         assert len(props) == n, (kernel, len(props))
         for line in props:
             assert "0 bytes spill stores, 0 bytes spill loads" in line, (kernel, line)
+
+
+def test_shared_weight_pack_kernels_do_not_spill():
+    """The convolution weight pack and bias kernels MelGAN and HiFi-GAN load their checkpoints through (csrc/vocoder_weights.cu)."""
+    reports = glob.glob(os.path.join(REPO, "fastspeech2_b200", "build", "vocoder_weights.ptxas.txt"))
+    if not reports:
+        pytest.skip("no ptxas reports (library built elsewhere)")
+    text = open(reports[0]).read()
+    for kernel in ("conv_pack_kernel", "conv_bias_kernel"):
+        props = re.findall(r"Function properties for \S*%s\S*\n(.*)" % kernel, text)
+        assert len(props) == 1, (kernel, len(props))
+        assert "0 bytes spill stores, 0 bytes spill loads" in props[0], (kernel, props[0])

@@ -290,6 +290,6 @@ def test_window_support_adds_no_instantiation_and_no_spill():
         pytest.skip("no ptxas reports (library built elsewhere)")
     text = open(reports[0]).read()
     props = re.findall(r"Function properties for (\S*melgan\S*)\n(.*)", text)
-    assert len(props) == 1 + 1 + 1 + 1 + 3 + 3 + 6 + 8                    # as before windows: runtime arguments only
+    assert len(props) == 1 + 1 + 3 + 3 + 6 + 8                            # as before windows: runtime arguments only
     for name, line in props:
         assert "0 bytes spill stores, 0 bytes spill loads" in line, (name, line)
