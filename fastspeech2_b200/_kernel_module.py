@@ -1,7 +1,7 @@
 """Host-side layer the signal modules share (MelGAN, HiFi-GAN, WaveGlow, Griffin-Lim, feature extraction): the per-device
 handle and workspace caches, the status-word check, checkpoint reading and weight-norm normalisation, and the call surface
-of the three neural vocoders: input and size checks, the whole call, and the windows of MelGAN and WaveGlow (DESIGN.md
-sections 11-12)."""
+of the three neural vocoders: input and size checks, the whole call, and the windows (DESIGN.md sections 11, 12 and
+17)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -156,15 +156,14 @@ def normalise_checkpoint(module: nn.Module, sd) -> dict:
 class NeuralVocoder(nn.Module):
     """What MelGANVocoder, HiFiGANVocoder and WaveGlowVocoder share around their C entries: the math mode; the handle,
     reloaded when a parameter changes; the mels / olens and size checks; the whole call with its workspace and status
-    check; and, for MelGAN and WaveGlow, the window layer (`window`'s inputs, `stream`'s loop, `forward(chunk_frames=)`).
+    check; and the window layer (`window`'s inputs, `stream`'s loop, `forward(chunk_frames=)`).
 
     A subclass names its C entries (_DESTROY, _WORKSPACE_BYTES, _WINDOW_BYTES) and the prefix of its status bits (_STATUS,
     e.g. "FS2_MELGAN"), and provides _create() -> handle, _load(handle, device) and _rows(B, Lmax) -> (rows, their
     formula, their noun).  A whole call is call(h, mels, olens, B, Lmax, audio, status, ws).
 
-    A vocoder without a window entry sets _WINDOW_BYTES = None: it has no `window`, `stream` or `chunk_frames`, and nothing
-    below the windows' heading applies to it.  One with windows also provides _window_rows(B, n_frames) -> (rows, their
-    formula); a window call is call(h, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws)."""
+    Every one has windows: it also provides _window_rows(B, n_frames) -> (rows, their formula); a window call is
+    call(h, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws)."""
 
     HOP = HOP
 
@@ -261,7 +260,7 @@ class NeuralVocoder(nn.Module):
         self._check_status(status)
         return audio, olens * self.HOP
 
-    # ---- windows (MelGAN and WaveGlow) ----------------------------------------------------------------------------
+    # ---- windows (MelGAN, HiFi-GAN and WaveGlow) ------------------------------------------------------------------
     def _window_workspace(self, h, B: int, n_frames: int, device: torch.device) -> torch.Tensor:
         return workspace(self._wws, device, query_bytes(self._WINDOW_BYTES, h, B, n_frames))
 

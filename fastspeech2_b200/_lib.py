@@ -53,6 +53,7 @@ FS2_MELGAN_BAD_START = 4                          # and of fs2_melgan_window's
 FS2_WAVEGLOW_BAD_LENGTH, FS2_WAVEGLOW_RANGE = 1, 2   # bits of fs2_waveglow's device status word
 FS2_WAVEGLOW_BAD_START = 4                           # and of fs2_waveglow_window's
 FS2_HIFIGAN_BAD_LENGTH, FS2_HIFIGAN_RANGE = 1, 2     # bits of fs2_hifigan's device status word
+FS2_HIFIGAN_BAD_START = 4                            # and of fs2_hifigan_window's
 FS2_HIFIGAN_MAX_UPSAMPLES, FS2_HIFIGAN_MAX_KERNELS = 8, 8
 
 
@@ -157,6 +158,8 @@ SIGNATURES = {
     "fs2_hifigan_load": [_P, C.POINTER(_P), C.POINTER(_P), _P],
     "fs2_hifigan_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
     "fs2_hifigan": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_hifigan_window_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_hifigan_window": [_P, _P, _P, _P, _I, _I, _I, _P, _L, _P, _P, _SZ, _P],
     "fs2_op_hifigan_resblock": [_I, _I, _I, _I, _I, C.POINTER(_I), _P, _P, _I, _I, C.POINTER(_P), C.POINTER(_P), _P, _P, _P],
     "fs2_op_hifigan_upsample": [_I, _I, _I, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P],
     "fs2_waveglow_create": [C.POINTER(_P), _I, _I],

@@ -32,6 +32,19 @@
 //
 // A GEMM row depends only on its own utterance's input rows, in a fixed K order, and every producer reads rows of its own
 // utterance below lens_s only, so per-utterance results do not depend on the batch.
+//
+// Windows (fs2_hifigan_window, DESIGN.md section 17): the same kernels and GEMMs on a window of each utterance's rows.
+// Walking back from the audio, conv_post reads 3 rows on each side, each MRF R = the largest resblock reach, and
+// upsampling s reads r_s input rows around its core (the polyphase rule above); conv_pre reads 3 frames more.  For the core
+// frames [c0, c1), level s (0 = conv_pre's output, s >= 1 = upsampling s-1's output) holds global rows
+// [c0 up_s - h_s, c1 up_s + h_s) clipped to [0, olens up_s), h_0 = r_0 + 3 and h_{s+1} = u_s r_s, in a buffer of
+// n up_s + 2 h_s rows per utterance; upsampling s reads its input window [c0 up_s - r_s, c1 up_s + r_s) (clipped) out of
+// level s.  Every GEMM runs with lens = the clipped length, so the rows-past-lens and zero-fill rules above give each
+// convolution its padding wherever a buffer side is an utterance edge.  At a side that is not one, level 0 is wrong in its
+// outer 3 rows, level s+1 enters wrong in u_s / 2 rows (the edge phases read outside the operand) and each MRF widens that
+// by R; since u_s r_s >= (what the next layer reads) + u_s / 2, the wrong rows never reach the core.  A window descriptor
+// [start | len | n] x B per buffer (nullptr = the whole utterance: start 0, len = n = lens[b]) maps local rows to global
+// ones, and producers range-check only rows whose values equal the whole call's (exact_row).
 #include <math.h>
 
 #include <algorithm>
@@ -47,12 +60,37 @@ constexpr float kSlope = 0.1f, kPostSlope = 0.01f;   // hifi-gan's LRELU_SLOPE, 
 
 __device__ __forceinline__ float lrelu(float v, float s) { return v > 0.f ? v : v * s; }
 
-struct Ups { int n; int up[kMaxUps + 1]; };   // cumulative upsampling of stages 0 .. n
+// cumulative upsampling of stages 0 .. n, and the window plan (see the top of the file): the upsamplings' input reaches
+// r_s and the level halos h_s
+struct Ups { int n; int up[kMaxUps + 1]; int reach[kMaxUps]; int halo[kMaxUps + 1]; };
+
+// window descriptors of a window call: levels 0 .. U, the upsamplings' input windows, and the audio samples
+__host__ __device__ constexpr int win_level(int s) { return s; }
+__host__ __device__ constexpr int win_ups(int U, int s) { return U + 1 + s; }
+__host__ __device__ constexpr int win_audio(int U) { return 2 * U + 1; }
+__host__ __device__ constexpr int n_wins(int U) { return 2 * U + 2; }
+
+// rows of utterance b in a buffer: global rows [start, start + len) of the utterance's n rows at its rate
+struct Rows { int start, len, n; };
+__device__ __forceinline__ Rows rows_of(const int64_t* __restrict__ win, const int64_t* __restrict__ lens, int B, int b) {
+  if (!win) {
+    const int n = (int)lens[b];
+    return {0, n, n};
+  }
+  return {(int)win[b], (int)win[B + b], (int)win[2 * B + b]};
+}
+// local row t holds the whole call's values: not within `margin` rows of a window side that is not an utterance edge
+__device__ __forceinline__ bool exact_row(const Rows& r, int t, int margin) {
+  return (r.start == 0 || t >= margin) && (r.start + r.len == r.n || t < r.len - margin);
+}
 
 // one CTA: lens[s][b] = olens[b] * up_s for 1 <= olens[b] <= L, else 0 (the utterance is skipped); *status = 0 or
 // FS2_HIFIGAN_BAD_LENGTH.  Runs first, so the producers' range bits land on a cleared word.
-__global__ void hifigan_prep_kernel(const int64_t* __restrict__ olens, int B, int L, Ups ups, int64_t* __restrict__ lens,
-                                    int* __restrict__ status) {
+// starts != nullptr (a window of nf frames from starts[b]): lens = the n_wins(U) window descriptors instead, for the core
+// frames [c0, c1) = [starts[b], min(starts[b] + nf, olens[b])); empty (len 0) when that is empty or the utterance is
+// invalid, and FS2_HIFIGAN_BAD_START for starts[b] < 0.
+__global__ void hifigan_prep_kernel(const int64_t* __restrict__ olens, const int64_t* __restrict__ starts, int B, int L, int nf, Ups ups,
+                                    int64_t* __restrict__ lens, int* __restrict__ status) {
   __shared__ int bad;
   if (threadIdx.x == 0) bad = 0;
   __syncthreads();
@@ -60,52 +98,89 @@ __global__ void hifigan_prep_kernel(const int64_t* __restrict__ olens, int B, in
     const int64_t n = olens[b];
     const bool ok = n >= 1 && n <= L;
     if (!ok) atomicOr(&bad, FS2_HIFIGAN_BAD_LENGTH);
-    for (int s = 0; s <= ups.n; ++s) lens[(long)s * B + b] = ok ? n * ups.up[s] : 0;
+    if (!starts) {
+      for (int s = 0; s <= ups.n; ++s) lens[(long)s * B + b] = ok ? n * ups.up[s] : 0;
+      continue;
+    }
+    const int64_t c0 = starts[b];
+    if (c0 < 0) atomicOr(&bad, FS2_HIFIGAN_BAD_START);
+    const bool live = ok && c0 >= 0 && c0 < n;
+    const int64_t c1 = live ? min(c0 + nf, n) : 0;
+    auto put = [&](int w, int64_t lo, int64_t hi, int64_t total) {
+      int64_t* d = lens + 3L * w * B + b;
+      d[0] = live ? lo : 0;
+      d[B] = live ? hi - lo : 0;
+      d[2 * B] = live ? total : 0;
+    };
+    for (int s = 0; s <= ups.n; ++s) {
+      const int64_t up = ups.up[s], total = n * up;
+      put(win_level(s), max(c0 * up - ups.halo[s], (int64_t)0), min(c1 * up + ups.halo[s], total), total);
+      if (s < ups.n) put(win_ups(ups.n, s), max(c0 * up - ups.reach[s], (int64_t)0), min(c1 * up + ups.reach[s], total), total);
+    }
+    put(win_audio(ups.n), c0 * kHop, c1 * kHop, n * kHop);
   }
   __syncthreads();
   if (threadIdx.x == 0) *status = bad;
 }
 
-// conv_pre's operand [B * L][80]: mel frame t of utterance b for t < lens[b], +0 past it (frames past olens[b] are never read)
+// conv_pre's operand [B * Lp][80]: mel frame start + t of utterance b for t < len (the rows of window win, nullptr: the
+// whole utterance, Lp = L), +0 past it (frames past olens[b] are never read).  Mel rows are L frames apart.
 template <int OUT>
-__global__ void hifigan_mel_operand_kernel(const float* __restrict__ mels, const int64_t* __restrict__ lens, int B, int L,
-                                           float* __restrict__ out32, __half* __restrict__ outp, int* __restrict__ status) {
+__global__ void hifigan_mel_operand_kernel(const float* __restrict__ mels, const int64_t* __restrict__ lens, const int64_t* __restrict__ win,
+                                           int B, int L, int Lp, float* __restrict__ out32, __half* __restrict__ outp,
+                                           int* __restrict__ status) {
   constexpr int Q = kMels / 4;
-  const long rows = (long)B * L, total = rows * Q, plane = rows * kMels;
+  const long rows = (long)B * Lp, total = rows * Q, plane = rows * kMels;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const long row = i / Q;
-    const int b = (int)(row / L), t = (int)(row - (long)b * L);
-    const long off = row * kMels + (i - row * Q) * 4;
+    const int b = (int)(row / Lp), t = (int)(row - (long)b * Lp);
+    const int c = (int)(i - row * Q) * 4;
+    const Rows r = rows_of(win, lens, B, b);
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (t < lens[b]) v = *reinterpret_cast<const float4*>(mels + off);
-    store_quad<OUT, RANGE_IF_STATUS>(v, off, out32, outp, plane, status, FS2_HIFIGAN_RANGE);
+    if (t < r.len) v = *reinterpret_cast<const float4*>(mels + ((long)b * L + r.start + t) * kMels + c);
+    store_quad<OUT, RANGE_IF_STATUS>(v, row * kMels + c, out32, outp, plane, status, FS2_HIFIGAN_RANGE);
   }
 }
 
 // a GEMM operand [B * Lp][C] = lrelu(v, 0.1) with v = x, or the MRF combine v = (x + r) / nk (r nullable: x / nk), for
 // t < lens[b]; +0 past it.  Every row is written: the next GEMM's taps read rows past lens[b] as its zero padding.
-template <int OUT>
-__global__ void hifigan_act_kernel(const float* __restrict__ x, const float* __restrict__ r, int nk, const int64_t* __restrict__ lens,
-                                   int B, int Lp, int C, float* __restrict__ out32, __half* __restrict__ outp, int* __restrict__ status) {
+// A window (WINDOW, win != nullptr): the operand's rows are window win; x and r have ldx rows per utterance in their own
+// window xwin (nullptr: the operand's, ldx = Lp), which holds win's rows; only rows exact_row(margin) are range-checked.
+template <int OUT, bool WINDOW>
+__device__ __forceinline__ void act_loop(const float* __restrict__ x, const float* __restrict__ r, int nk, const int64_t* __restrict__ lens,
+                                         const int64_t* __restrict__ xwin, int ldx, const int64_t* __restrict__ win, int B, int Lp, int C,
+                                         int margin, float* __restrict__ out32, __half* __restrict__ outp, int* __restrict__ status) {
   const int Q = C / 4;
   const long rows = (long)B * Lp, total = rows * Q, plane = rows * C;
   const float fk = (float)nk;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const long row = i / Q;
     const int b = (int)(row / Lp), t = (int)(row - (long)b * Lp);
-    const long off = row * C + (i - row * Q) * 4;
+    const int c = (int)(i - row * Q) * 4;
+    const long off = row * C + c;
+    const Rows w = rows_of(WINDOW ? win : nullptr, lens, B, b);
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (t < lens[b]) {
-      v = *reinterpret_cast<const float4*>(x + off);
+    if (t < w.len) {
+      const long src = WINDOW ? ((long)b * ldx + t + (xwin ? w.start - (int)xwin[b] : 0)) * C + c : off;
+      v = *reinterpret_cast<const float4*>(x + src);
       if (r) {
-        const float4 w = *reinterpret_cast<const float4*>(r + off);
-        v = make_float4(v.x + w.x, v.y + w.y, v.z + w.z, v.w + w.w);
+        const float4 u = *reinterpret_cast<const float4*>(r + src);
+        v = make_float4(v.x + u.x, v.y + u.y, v.z + u.z, v.w + u.w);
       }
       if (nk != 1) v = make_float4(v.x / fk, v.y / fk, v.z / fk, v.w / fk);
       v = make_float4(lrelu(v.x, kSlope), lrelu(v.y, kSlope), lrelu(v.z, kSlope), lrelu(v.w, kSlope));
     }
-    store_quad<OUT, RANGE_IF_STATUS>(v, off, out32, outp, plane, status, FS2_HIFIGAN_RANGE);
+    store_quad<OUT, RANGE_IF_STATUS>(v, off, out32, outp, plane, !WINDOW || exact_row(w, t, margin) ? status : nullptr,
+                                     FS2_HIFIGAN_RANGE);
   }
+}
+
+template <int OUT>
+__global__ void hifigan_act_kernel(const float* __restrict__ x, const float* __restrict__ r, int nk, const int64_t* __restrict__ lens,
+                                   const int64_t* __restrict__ xwin, int ldx, const int64_t* __restrict__ win, int B, int Lp, int C,
+                                   int margin, float* __restrict__ out32, __half* __restrict__ outp, int* __restrict__ status) {
+  if (win) act_loop<OUT, true>(x, r, nk, lens, xwin, ldx, win, B, Lp, C, margin, out32, outp, status);
+  else act_loop<OUT, false>(x, r, nk, lens, xwin, ldx, win, B, Lp, C, margin, out32, outp, status);
 }
 
 // s[i] += r[i] over n floats (n a multiple of 4): the MRF's running sum; rows past lens are +0 in both
@@ -118,26 +193,31 @@ __global__ void hifigan_add_kernel(float* __restrict__ s, const float* __restric
 }
 
 // audio[b, t] = tanh(bias + sum_j sum_c w[j][c] lrelu(x[t + j - 3][c], 0.01)) for t < lens[b], else +0, where x = (S + R) / nk
-// (R nullable) is the last MRF's output, 0 outside [0, lens[b]).  w: [7][C] in dynamic shared memory.
+// (R nullable) is the last MRF's output, 0 outside [0, lens[b]).  w: [7][C] in dynamic shared memory.  x has Lx rows per
+// utterance in window win (nullptr: the whole utterance), audio Lout samples per row, rows ld apart.  A window: audio row b
+// holds samples [start, start + len) of awin, +0 past them.
 __global__ void __launch_bounds__(256) hifigan_post_kernel(const float* __restrict__ S, const float* __restrict__ R, int nk,
-                                                           const int64_t* __restrict__ lens, int B, int Lp, int C,
+                                                           const int64_t* __restrict__ lens, const int64_t* __restrict__ win,
+                                                           const int64_t* __restrict__ awin, int B, int Lx, int Lout, long ld, int C,
                                                            const float* __restrict__ w, const float* __restrict__ bias,
                                                            float* __restrict__ audio) {
   extern __shared__ __align__(16) float ws[];
   for (int i = threadIdx.x; i < kPostTaps * C; i += blockDim.x) ws[i] = w[i];
   __syncthreads();
   const float b0 = __ldg(bias), fk = (float)nk;
-  const long total = (long)B * Lp;
+  const long total = (long)B * Lout;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const int b = (int)(i / Lp), t = (int)(i - (long)b * Lp), n = (int)lens[b];
+    const int b = (int)(i / Lout), t = (int)(i - (long)b * Lout);
+    const Rows r = rows_of(win, lens, B, b);
+    const int a0 = awin ? (int)awin[b] : 0, n = awin ? (int)awin[B + b] : r.n;
     float y = 0.f;
     if (t < n) {
       float acc = b0;
 #pragma unroll 1
       for (int j = 0; j < kPostTaps; ++j) {
-        const int src = t + j - kPostTaps / 2;
-        if (src < 0 || src >= n) continue;
-        const long row = ((long)b * Lp + src) * C;
+        const int src = a0 + t + j - kPostTaps / 2;
+        if (src < 0 || src >= r.n) continue;
+        const long row = ((long)b * Lx + src - r.start) * C;
         for (int q = 0; q < C / 4; ++q) {
           float4 v = __ldg(reinterpret_cast<const float4*>(S + row) + q);
           if (R) {
@@ -154,7 +234,7 @@ __global__ void __launch_bounds__(256) hifigan_post_kernel(const float* __restri
       }
       y = tanhf(acc);
     }
-    audio[i] = y;
+    audio[(long)b * ld + t] = y;
   }
 }
 
@@ -182,8 +262,28 @@ Shape shape_of(const fs2_hifigan_config& c) {
     s.act = std::max(s.act, (long)s.ups.up[i + 1] * s.C[i + 1]);
   }
   s.layers = 2 + s.U + s.U * s.nk * s.per;
+  // the window plan: walking back from the audio, the rows each layer's input needs on each side of the core
+  int R = 0;                                           // the MRF's reach: the largest resblock's
+  for (int j = 0; j < s.nk; ++j) {
+    int r = 0;
+    for (int m = 0; m < s.steps; ++m) r += (c.resblock_kernel_sizes[j] - 1) / 2 * (c.resblock_dilation_sizes[j][m] + (s.type == 1));
+    R = std::max(R, r);
+  }
+  int need = kPostTaps / 2;
+  for (int i = s.U - 1; i >= 0; --i) {
+    need += R;
+    // output rows [-need, 0) of upsampling i's core: row o = u t + p reads input rows t - 1, t (p < u / 2) or t, t + 1
+    const int u = c.upsample_rates[i], o = -need, t = (o - (u - 1)) / u, p = o - t * u;   // floor division of a negative o
+    s.ups.reach[i] = need = -(p < u / 2 ? t - 1 : t);
+    s.ups.halo[i + 1] = u * need;
+  }
+  s.ups.halo[0] = need + kPreTaps / 2;
   return s;
 }
+
+// rows per utterance of level s's window buffer and of upsampling s's input window, for nf frames
+long level_rows(const Shape& sh, int s, long nf) { return nf * sh.ups.up[s] + 2L * sh.ups.halo[s]; }
+long ups_rows(const Shape& sh, int s, long nf) { return nf * sh.ups.up[s] + 2L * sh.ups.reach[s]; }
 
 int validate(const fs2_hifigan_config* c) {
   const char* who = "fs2_hifigan_create";
@@ -217,35 +317,42 @@ int validate(const fs2_hifigan_config* c) {
   return FS2_OK;
 }
 
-// the act producer (x, r, nk as in hifigan_act_kernel) into the operand a
-int act(int kind, const float* x, const float* r, int nk, const int64_t* lens, int B, int Lp, int C, void* a, int* status, cudaStream_t st) {
+// the act producer (x, r, nk, xwin, ldx, win, margin as in hifigan_act_kernel) into the operand a
+int act(int kind, const float* x, const float* r, int nk, const int64_t* lens, const int64_t* xwin, int ldx, const int64_t* win, int B,
+        int Lp, int C, int margin, void* a, int* status, cudaStream_t st) {
   auto k = pick(kind, hifigan_act_kernel<OUT_HILO>, hifigan_act_kernel<OUT_HI>, hifigan_act_kernel<OUT_F32>);
-  k<<<grid_for((long)B * Lp * (C / 4), 256), 256, 0, st>>>(x, r, nk, lens, B, Lp, C, (float*)a, (__half*)a, status);
+  k<<<grid_for((long)B * Lp * (C / 4), 256), 256, 0, st>>>(x, r, nk, lens, xwin, ldx, win, B, Lp, C, margin, (float*)a, (__half*)a, status);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
 
 // lrelu + ConvTranspose1d: x [B * Lin][Cin] (combined with r / nk) -> out [B * Lin][u Cout] = [B * Lin * u][Cout] through the
-// operand a; rows >= lens[b] * u of out written as +0
-int upsample(int mode, const VWeight& w, const float* x, const float* r, int nk, const int64_t* lens, int B, int Lin, int Cin, void* a,
-             float* out, int* status, cudaStream_t st) {
-  int rc = act(out_kind(mode), x, r, nk, lens, B, Lin, Cin, a, status, st);
+// operand a; rows >= lens[b] * u of out written as +0.  A window: the input window (win, lens; Lin rows per utterance) is
+// read from x's own window xwin of ldx rows per utterance.  Every row it reads holds the whole call's values, so all are
+// range-checked.
+int upsample(int mode, const VWeight& w, const float* x, const float* r, int nk, const int64_t* xwin, int ldx, const int64_t* lens,
+             const int64_t* win, int B, int Lin, int Cin, void* a, float* out, int* status, cudaStream_t st) {
+  int rc = act(out_kind(mode), x, r, nk, lens, xwin, ldx, win, B, Lin, Cin, 0, a, status, st);
   return rc ? rc : vweight_gemm(mode, w, a, B, Lin, ACT_NONE, lens, out, st);
 }
 
 // One residual block x -> dest on rows [B * Lp][C]: w = its convolutions in state_dict order, dil its dilations.  Step m
 // writes t[m & 1], the last one dest; dest must differ from x and from the buffer the last step reads (t[(steps - 2) & 1]).
-int resblock(int mode, int type, const VWeight* w, const int* dil, const float* x, const int64_t* lens, int B, int Lp, int C, void* a,
-             float* const* t, float* dest, int* status, cudaStream_t st) {
-  const int steps = type == 1 ? 3 : 2, kind = out_kind(mode);
+// win (nullable): the rows' window; margin: its rows at a side that is not an utterance edge whose values differ from the
+// whole call's on entry, widened here by each convolution's reach.
+int resblock(int mode, int type, const VWeight* w, const int* dil, const float* x, const int64_t* lens, const int64_t* win, int B, int Lp,
+             int C, int margin, void* a, float* const* t, float* dest, int* status, cudaStream_t st) {
+  const int steps = type == 1 ? 3 : 2, kind = out_kind(mode), half = (w[0].taps - 1) / 2;
   const float* X = x;
   int rc;
   for (int m = 0; m < steps; ++m) {
     float* out = m == steps - 1 ? dest : t[m & 1];
-    if ((rc = act(kind, X, nullptr, 1, lens, B, Lp, C, a, status, st))) return rc;
+    if ((rc = act(kind, X, nullptr, 1, lens, nullptr, Lp, win, B, Lp, C, margin, a, status, st))) return rc;
+    margin += half * dil[m];
     if (type == 1) {
       if ((rc = vweight_gemm(mode, w[m], a, B, Lp, ACT_NONE, lens, out, st, nullptr, dil[m]))) return rc;   // h = c1(lrelu(x))
-      if ((rc = act(kind, out, nullptr, 1, lens, B, Lp, C, a, status, st))) return rc;
+      if ((rc = act(kind, out, nullptr, 1, lens, nullptr, Lp, win, B, Lp, C, margin, a, status, st))) return rc;
+      margin += half;
       if ((rc = vweight_gemm(mode, w[3 + m], a, B, Lp, ACT_NONE, lens, out, st, X, 1))) return rc;        // c2(lrelu(h)) + x
     } else {
       if ((rc = vweight_gemm(mode, w[m], a, B, Lp, ACT_NONE, lens, out, st, X, dil[m]))) return rc;       // c(lrelu(x)) + x
@@ -256,17 +363,16 @@ int resblock(int mode, int type, const VWeight* w, const int* dil, const float* 
 }
 
 struct HgPlan {
-  int64_t* lens;      // [U + 1][B]
+  int64_t* lens;      // [U + 1][B]; a window call: the n_wins(U) window descriptors [start | len | n][B]
   void* a;            // GEMM operand
   float* xu;          // the upsampling output of the current stage
   float* s;           // MRF sum
   float* t[2];        // chain buffers
 };
 
-HgPlan plan(Bump& b, const Shape& sh, int B, int L) {
-  const size_t n = (size_t)B * L * sh.act;
+HgPlan carve_plan(Bump& b, size_t lens_bytes, size_t n) {
   HgPlan p;
-  p.lens = (int64_t*)b.bytes((size_t)(sh.U + 1) * B * sizeof(int64_t));
+  p.lens = (int64_t*)b.bytes(lens_bytes);
   p.a = b.floats(n);
   p.xu = b.floats(n);
   p.s = b.floats(n);
@@ -275,12 +381,35 @@ HgPlan plan(Bump& b, const Shape& sh, int B, int L) {
   return p;
 }
 
+HgPlan plan(Bump& b, const Shape& sh, int B, int L) {
+  return carve_plan(b, (size_t)(sh.U + 1) * B * sizeof(int64_t), (size_t)B * L * sh.act);
+}
+
+// A window call's workspace, from B and nf only: five buffers of the largest level buffer per utterance (rows x C over
+// every level; conv_pre's operand, 80 wide, and the upsamplings' operands, r_s <= h_s, fit in it)
+HgPlan window_plan(Bump& b, const Shape& sh, int B, int nf) {
+  long act = level_rows(sh, 0, nf) * kMels;
+  for (int s = 0; s <= sh.U; ++s) act = std::max(act, level_rows(sh, s, nf) * sh.C[s]);
+  return carve_plan(b, (size_t)3 * n_wins(sh.U) * B * sizeof(int64_t), (size_t)B * act);
+}
+
 // a GEMM weight here is [taps][N][K] tap matrices with K = Cin, so vweight_pack_conv packs it at tap_stride = N K
 void set_conv(VWeight& w, int N, int K, int taps) { w.N = N; w.K = K; w.taps = taps; }
 
 int check_size(int math_mode, int B, int L) {
   FS2_REQUIRE(B >= 1 && L >= 1, "fs2_hifigan: need B >= 1 and Lmax >= 1 (got %d, %d)", B, L);
   return check_rows("fs2_hifigan", "B * Lmax * 256", "sample", (long)B * L * kHop, math_mode);
+}
+
+// a window's limits apply to its rows: the GEMMs of level s have B * level_rows(s, nf) rows (the upsamplings' fewer)
+int check_window(int math_mode, const Shape& sh, int B, int nf) {
+  FS2_REQUIRE(B >= 1 && nf >= 1, "fs2_hifigan_window: need B >= 1 and n_frames >= 1 (got %d, %d)", B, nf);
+  int top = 0;
+  for (int s = 1; s <= sh.U; ++s)
+    if (level_rows(sh, s, nf) > level_rows(sh, top, nf)) top = s;
+  char formula[64];
+  snprintf(formula, sizeof formula, "B * (%d * n_frames + %d)", sh.ups.up[top], 2 * sh.ups.halo[top]);
+  return check_rows("fs2_hifigan_window", formula, "window", (long)B * std::min(level_rows(sh, top, nf), 1L << 31), math_mode);
 }
 
 }  // namespace
@@ -301,33 +430,43 @@ struct fs2_hifigan_gen {
 namespace fs2 {
 namespace {
 
-int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const int64_t* olens, int B, int L, float* audio, int* status,
-             cudaStream_t st) {
+// The generator on the plan p: whole utterances (starts == nullptr; level s has L up_s rows per utterance, lens [U + 1][B])
+// or a window of nf frames from starts[b] (level_rows / ups_rows per utterance, the n_wins(U) window descriptors).  Lout
+// audio samples per row, rows ld apart.  Both enqueue the same kernels.
+int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const int64_t* olens, const int64_t* starts, int B, int L,
+             int nf, float* audio, long ld, int* status, cudaStream_t st) {
   const Shape& sh = m->sh;
-  const int mode = m->math_mode, kind = out_kind(mode);
-  auto lens = [&](int s) -> const int64_t* { return p.lens + (long)s * B; };
+  const bool w = starts != nullptr;
+  const int mode = m->math_mode, kind = out_kind(mode), U = sh.U;
+  auto desc = [&](int i) -> const int64_t* { return w ? p.lens + 3L * i * B : nullptr; };
+  auto lens = [&](int i, int s) -> const int64_t* { return w ? p.lens + (3L * i + 1) * B : p.lens + (long)s * B; };   // window i / level s
+  auto rows = [&](int s) { return w ? (int)level_rows(sh, s, nf) : L * sh.ups.up[s]; };
   int rc;
-  hifigan_prep_kernel<<<1, 256, 0, st>>>(olens, B, L, sh.ups, p.lens, status);
+  hifigan_prep_kernel<<<1, 256, 0, st>>>(olens, starts, B, L, nf, sh.ups, p.lens, status);
   FS2_LAUNCH_CHECK();
   {
     auto k = pick(kind, hifigan_mel_operand_kernel<OUT_HILO>, hifigan_mel_operand_kernel<OUT_HI>, hifigan_mel_operand_kernel<OUT_F32>);
-    k<<<grid_for((long)B * L * (kMels / 4), 256), 256, 0, st>>>(mels, lens(0), B, L, (float*)p.a, (__half*)p.a, status);
+    k<<<grid_for((long)B * rows(0) * (kMels / 4), 256), 256, 0, st>>>(mels, lens(win_level(0), 0), desc(win_level(0)), B, L, rows(0),
+                                                                     (float*)p.a, (__half*)p.a, status);
     FS2_LAUNCH_CHECK();
   }
-  if ((rc = vweight_gemm(mode, m->pre, p.a, B, L, ACT_NONE, lens(0), p.t[0], st))) return rc;
+  if ((rc = vweight_gemm(mode, m->pre, p.a, B, rows(0), ACT_NONE, lens(win_level(0), 0), p.t[0], st))) return rc;
   // the stage input: conv_pre's output, then each MRF's (S + r) / nk
   const float* x = p.t[0];
   const float* r = nullptr;
   int nk_in = 1;
-  for (int s = 0; s < sh.U; ++s) {
-    const int Lin = L * sh.ups.up[s], Lp = L * sh.ups.up[s + 1], C = sh.C[s + 1];
-    if ((rc = upsample(mode, m->up[s], x, r, nk_in, lens(s), B, Lin, sh.C[s], p.a, p.xu, status, st))) return rc;
+  for (int s = 0; s < U; ++s) {
+    const int Lin = w ? (int)ups_rows(sh, s, nf) : rows(s), Lp = rows(s + 1), C = sh.C[s + 1], uw = win_ups(U, s), lw = win_level(s + 1);
+    if ((rc = upsample(mode, m->up[s], x, r, nk_in, desc(win_level(s)), rows(s), lens(uw, s), desc(uw), B, Lin, sh.C[s], p.a, p.xu, status,
+                       st)))
+      return rc;
+    const int margin = m->cfg.upsample_rates[s] / 2;   // the rows the edge phases leave wrong at a side that is not an edge
     float* last = p.s;
     for (int j = 0; j < sh.nk; ++j) {
       const int g = s * sh.nk + j;
       last = j == 0 ? p.s : p.t[(sh.steps - 1) & 1];
-      if ((rc = resblock(mode, sh.type, &m->blk[(size_t)g * sh.per], m->cfg.resblock_dilation_sizes[j], p.xu, lens(s + 1), B, Lp, C, p.a,
-                         p.t, last, status, st)))
+      if ((rc = resblock(mode, sh.type, &m->blk[(size_t)g * sh.per], m->cfg.resblock_dilation_sizes[j], p.xu, lens(lw, s + 1), desc(lw), B,
+                         Lp, C, margin, p.a, p.t, last, status, st)))
         return rc;
       if (j >= 1 && j < sh.nk - 1) {
         hifigan_add_kernel<<<grid_for((long)B * Lp * C / 4, 256), 256, 0, st>>>(p.s, last, (long)B * Lp * C);
@@ -338,9 +477,9 @@ int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const
     r = sh.nk > 1 ? last : nullptr;
     nk_in = sh.nk;
   }
-  const int Lout = L * kHop, C = sh.C[sh.U];
-  hifigan_post_kernel<<<grid_for((long)B * Lout, 256), 256, kPostTaps * C * sizeof(float), st>>>(x, r, nk_in, lens(sh.U), B, Lout, C,
-                                                                                                  m->post_w, m->post_b, audio);
+  const int Lout = (w ? nf : L) * kHop, C = sh.C[U];
+  hifigan_post_kernel<<<grid_for((long)B * Lout, 256), 256, kPostTaps * C * sizeof(float), st>>>(
+      x, r, nk_in, lens(win_level(U), U), desc(win_level(U)), desc(win_audio(U)), B, rows(U), Lout, ld, C, m->post_w, m->post_b, audio);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
@@ -432,7 +571,34 @@ int fs2_hifigan(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, int
   Bump b(ws, ws_bytes);
   HgPlan p = plan(b, m->sh, B, Lmax);
   if ((rc = b.check("fs2_hifigan"))) return rc;
-  return generate(m, p, mels, olens, B, Lmax, audio, status, (cudaStream_t)stream);
+  return generate(m, p, mels, olens, nullptr, B, Lmax, 0, audio, (long)Lmax * kHop, status, (cudaStream_t)stream);
+}
+
+int fs2_hifigan_window_workspace_bytes(fs2_hifigan_gen* m, int B, int n_frames, size_t* bytes) {
+  FS2_REQUIRE(m && bytes, "fs2_hifigan_window_workspace_bytes: null argument");
+  int rc = check_window(m->math_mode, m->sh, B, n_frames);
+  if (rc) return rc;
+  Bump b(nullptr, 0);
+  window_plan(b, m->sh, B, n_frames);
+  *bytes = b.off + 256;
+  return FS2_OK;
+}
+
+int fs2_hifigan_window(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax, int n_frames,
+                       float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream) {
+  FS2_REQUIRE(m && mels && olens && starts && audio && status && ws, "fs2_hifigan_window: null argument");
+  FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "fs2_hifigan_window: mels must be 16-byte aligned");
+  int rc = check_window(m->math_mode, m->sh, B, n_frames);
+  if (rc) return rc;
+  FS2_REQUIRE(Lmax >= 1 && (long)Lmax * kHop < (1L << 31), "fs2_hifigan_window: need 1 <= Lmax and Lmax * 256 below 2^31 (got Lmax = %d)",
+              Lmax);
+  FS2_REQUIRE(audio_ld >= (int64_t)n_frames * kHop, "fs2_hifigan_window: audio_ld = %lld below n_frames * 256 = %ld", (long long)audio_ld,
+              (long)n_frames * kHop);
+  Bump b(ws, ws_bytes);
+  HgPlan p = window_plan(b, m->sh, B, n_frames);
+  if ((rc = b.check("fs2_hifigan_window"))) return rc;
+  FS2_REQUIRE(m->loaded, "fs2_hifigan_window: weights not loaded (fs2_hifigan_load)");
+  return generate(m, p, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, (cudaStream_t)stream);
 }
 
 // ---- single layers on the vocoder's own code paths (tests) ----------------------------------------------------------
@@ -468,7 +634,7 @@ int fs2_op_hifigan_resblock(int math_mode, int type, int C, int k, int nd, const
   if (rc) return rc;
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
   for (int i = 0; i < per && !rc; ++i) rc = vweight_pack_conv(w[i], weights[i], biases[i], C, C, k, 0, (long)C * C, st);
-  if (!rc) rc = resblock(math_mode, type, w, dils, x, lens, B, Lp, C, a, t, out, status, st);
+  if (!rc) rc = resblock(math_mode, type, w, dils, x, lens, nullptr, B, Lp, C, 0, a, t, out, status, st);
   cudaFreeAsync(base, st);
   return rc;
 }
@@ -499,7 +665,7 @@ int fs2_op_hifigan_upsample(int math_mode, int Cin, int Cout, int u, const float
   if (rc) return rc;
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
   rc = vweight_pack_conv(wu, w, b, Cin, Cout, 3, u, (long)wu.N * Cin, st);
-  if (!rc) rc = upsample(math_mode, wu, x, nullptr, 1, lens, B, Lin, Cin, a, out, status, st);
+  if (!rc) rc = upsample(math_mode, wu, x, nullptr, 1, nullptr, Lin, lens, nullptr, B, Lin, Cin, a, out, status, st);
   cudaFreeAsync(base, st);
   return rc;
 }
