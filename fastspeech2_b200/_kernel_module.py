@@ -5,6 +5,8 @@ of the three neural vocoders: input and size checks, the whole call, and the win
 from __future__ import annotations
 
 import ctypes as C
+import itertools
+import operator
 import os
 
 import torch
@@ -153,26 +155,47 @@ def normalise_checkpoint(module: nn.Module, sd) -> dict:
 
 # ---- the neural vocoders --------------------------------------------------------------------------------------------
 
+def ups_window_plan(rates, R: int, margin0: int, post: int = 3) -> dict:
+    """The window plan of an upsampling chain (MelGAN, HiFi-GAN; DESIGN.md section 11; csrc/vocoder_window.cuh), walking
+    back from the audio: the last convolution reads `post` rows on each side, each residual stack R, upsampling s (a
+    polyphase ConvTranspose1d of k = 2 u_s) reads reach[s] input rows around its core, and level 0 holds margin0 rows more
+    (the rows the first convolution leaves wrong at a window side that is not an utterance edge).  -> {"reach": [r_s],
+    "halo": [h_s] (rows of level s on each side of its core; h_0 = r_0 + margin0, h_{s+1} = u_s r_s), "R": R}."""
+    reach, halo, need = [0] * len(rates), [0] * (len(rates) + 1), post
+    for s in reversed(range(len(rates))):
+        need += R
+        u = rates[s]
+        t, p = divmod(-need, u)                          # output row -need = u t + p reads t - 1 (p < u / 2) or t
+        reach[s] = need = -(t - 1 if p < u // 2 else t)
+        halo[s + 1] = u * need
+    halo[0] = need + margin0
+    return {"reach": reach, "halo": halo, "R": R}
+
+
 class NeuralVocoder(nn.Module):
     """What MelGANVocoder, HiFiGANVocoder and WaveGlowVocoder share around their C entries: the math mode; the handle,
     reloaded when a parameter changes; the mels / olens and size checks; the whole call with its workspace and status
     check; and the window layer (`window`'s inputs, `stream`'s loop, `forward(chunk_frames=)`).
 
-    A subclass names its C entries (_DESTROY, _WORKSPACE_BYTES, _WINDOW_BYTES) and the prefix of its status bits (_STATUS,
-    e.g. "FS2_MELGAN"), and provides _create() -> handle, _load(handle, device) and _rows(B, Lmax) -> (rows, their
-    formula, their noun).  A whole call is call(h, mels, olens, B, Lmax, audio, status, ws).
+    A subclass names its C entries by their prefix (_NAME: fs2_<_NAME>, fs2_<_NAME>_window, fs2_<_NAME>_destroy, the
+    two *_workspace_bytes and the FS2_<_NAME> status bits) and the frames each utterance runs past olens (_TAIL), and
+    provides _create() -> handle, _load(handle, device) and _rows(B, Lmax) -> (rows, their formula, their noun).  A whole
+    call is call(h, mels, olens, B, Lmax, audio, status, ws), a window call call(h, mels, olens, starts, B, Lmax, n_frames,
+    audio, audio_ld, status, ws).
 
-    Every one has windows: it also provides _window_rows(B, n_frames) -> (rows, their formula); a window call is
-    call(h, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws)."""
+    MelGAN and HiFi-GAN, upsampling chains, also provide _chain() -> (upsample rates, stack reach R, level-0 margin) and
+    take the rest from here: _call and _window_call on their C entries, the window's rows from the chain's plan, and
+    forward, window and stream.  WaveGlow, whose calls carry the noise, has its own calls, window rows and those three."""
 
     HOP = HOP
+    _TAIL = 0
 
     def __init__(self, math_mode: str):
         super().__init__()
         if math_mode not in _lib.MATH_MODES:
             raise ValueError(f"math_mode must be one of {sorted(_lib.MATH_MODES)}")
         self.math_mode = math_mode
-        self._handles = Handles(self._DESTROY)
+        self._handles = Handles(f"fs2_{self._NAME}_destroy")
         self._ws = {}            # device index -> workspace tensor
         self._wws = {}           # device index -> window workspace tensor
         self._epoch = 0
@@ -201,14 +224,15 @@ class NeuralVocoder(nn.Module):
         _lib.check(getattr(_lib.load(), entry)(h, wp, bp, _lib.stream_ptr(device)), entry)
 
     def _workspace(self, h, B: int, L: int, device: torch.device) -> torch.Tensor:
-        return workspace(self._ws, device, query_bytes(self._WORKSPACE_BYTES, h, B, L))
+        return workspace(self._ws, device, query_bytes(f"fs2_{self._NAME}_workspace_bytes", h, B, L))
 
     def _status_table(self):
-        """[(bit, message)] of the status word: <_STATUS>_BAD_LENGTH, _BAD_START where the vocoder has windows, _RANGE."""
-        table = [(getattr(_lib, self._STATUS + "_BAD_LENGTH"), "every olens[b] must lie in [1, Lmax]")]
-        if hasattr(_lib, self._STATUS + "_BAD_START"):
-            table.append((getattr(_lib, self._STATUS + "_BAD_START"), "every starts[b] must be >= 0"))
-        table.append((getattr(_lib, self._STATUS + "_RANGE"),
+        """[(bit, message)] of the status word: FS2_<_NAME>_BAD_LENGTH, _BAD_START where the vocoder has windows, _RANGE."""
+        status = "FS2_" + self._NAME.upper()
+        table = [(getattr(_lib, status + "_BAD_LENGTH"), "every olens[b] must lie in [1, Lmax]")]
+        if hasattr(_lib, status + "_BAD_START"):
+            table.append((getattr(_lib, status + "_BAD_START"), "every starts[b] must be >= 0"))
+        table.append((getattr(_lib, status + "_RANGE"),
                       f"activations exceed the range of the fp16 operand planes in math_mode={self.math_mode!r} "
                       f"(some GEMM input above {65504 / 16:g} in magnitude); use math_mode='fp32' or 'tf32'"))
         return table
@@ -260,9 +284,27 @@ class NeuralVocoder(nn.Module):
         self._check_status(status)
         return audio, olens * self.HOP
 
+    def _call(self, h, mels, olens, B: int, L: int, audio: torch.Tensor, status: torch.Tensor, ws: torch.Tensor) -> None:
+        """The whole call of an upsampling chain: fs2_<_NAME>."""
+        name = f"fs2_{self._NAME}"
+        _lib.check(getattr(_lib.load(), name)(h, _lib.ptr(mels), _lib.ptr(olens), B, L, _lib.ptr(audio), _lib.ptr(status), _lib.ptr(ws),
+                                              ws.numel(), _lib.stream_ptr(mels.device)), name)
+
+    def forward(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int | None = None):
+        """-> (audio [B, Lmax * 256] fp32, alens [B] int64 = olens * 256).
+
+        chunk_frames=k: the same bits, computed as windows of k frames written straight into the output, with the
+        workspace of one window (fs2_<_NAME>_window): in fp32 mode this vocodes batches the whole call refuses.  Still one
+        host read per call: the windows' status words are ORed on the device."""
+        if chunk_frames is not None:
+            mels, olens, B, L = self._window_inputs(mels, olens, chunk_frames)
+            return self._chunked(self._window_call, mels, olens, B, L, chunk_frames)
+        mels, olens, B, L = self._mels_olens(mels, olens)
+        return self._whole(self._call, mels, olens, B, L)
+
     # ---- windows (MelGAN, HiFi-GAN and WaveGlow) ------------------------------------------------------------------
     def _window_workspace(self, h, B: int, n_frames: int, device: torch.device) -> torch.Tensor:
-        return workspace(self._wws, device, query_bytes(self._WINDOW_BYTES, h, B, n_frames))
+        return workspace(self._wws, device, query_bytes(f"fs2_{self._NAME}_window_workspace_bytes", h, B, n_frames))
 
     @staticmethod
     def _check_frames(n_frames) -> None:
@@ -273,6 +315,53 @@ class NeuralVocoder(nn.Module):
         """_check_rows on a window's rows."""
         self._check_frames(n_frames)
         self._check_rows(*self._window_rows(B, n_frames), "window", f"B={B}, n_frames={n_frames}", "use fewer frames per window")
+
+    def _check_extent(self, L: int, rate: int = HOP, noun: str = "samples") -> None:
+        """A window's limit on Lmax, which bounds only the per-utterance rows: (Lmax + _TAIL) * rate below 2^31."""
+        if (L + self._TAIL) * rate >= 1 << 31:
+            lmax = f"(Lmax + {self._TAIL})" if self._TAIL else "Lmax"
+            raise ValueError(f"{lmax} * {rate} must stay below 2^31 {noun} (Lmax={L})")
+
+    def _window_rows(self, B: int, n_frames: int):
+        """An upsampling chain's largest window buffer: B * (up_s * n_frames + 2 h_s) rows for the level s with the most."""
+        rates, R, margin0 = self._chain()
+        ups = itertools.accumulate(rates, operator.mul, initial=1)
+        n, up, h = max((up * n_frames + 2 * h, up, h) for up, h in zip(ups, ups_window_plan(rates, R, margin0)["halo"]))
+        return B * n, f"B * ({up} * n_frames + {2 * h})"
+
+    def _window_inputs(self, mels, olens, n_frames):
+        """_mels_olens with the window's limits in place of the whole call's."""
+        self._check_frames(n_frames)
+
+        def check(B, L):
+            self._check_window_size(B, n_frames)
+            self._check_extent(L)
+        return self._mels_olens(mels, olens, check)
+
+    def _window_call(self, h, mels, olens, starts, B: int, L: int, n_frames: int, audio: torch.Tensor, ld: int, status: torch.Tensor,
+                     ws: torch.Tensor) -> None:
+        """A window call of an upsampling chain: fs2_<_NAME>_window."""
+        name, dev = f"fs2_{self._NAME}_window", mels.device
+        with torch.cuda.device(dev):
+            _lib.check(getattr(_lib.load(), name)(h, _lib.ptr(mels), _lib.ptr(olens), _lib.ptr(starts), B, L, n_frames, audio.data_ptr(), ld,
+                                                  _lib.ptr(status), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)), name)
+
+    def window(self, mels: torch.Tensor, olens: torch.Tensor, starts, n_frames: int):
+        """One window of the audio (DESIGN.md sections 11 and 17): -> (audio [B, n_frames * 256] fp32, alens [B] int64 =
+        clamp(olens - starts, 0, n_frames) * 256).  audio[b, :alens[b]] are samples [starts[b] * 256, ...) of
+        `forward(mels, olens)[0][b]`, bit for bit; the rest is 0.  starts: an int (every utterance), a host list or tensor,
+        or a device tensor.  Only mel frames [starts[b] - r, starts[b] + n_frames + r) below olens[b] are read, r = the
+        first upsampling's reach + 3 (6 for MelGAN, 13 for HiFi-GAN V1, 11 for V3); the workspace depends on B and
+        n_frames only.  One host read per call."""
+        mels, olens, B, L = self._window_inputs(mels, olens, n_frames)
+        return self._window(self._window_call, mels, olens, starts, B, L, n_frames)
+
+    def stream(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int = 32):
+        """Lockstep windows: yields (audio, alens) of `window(mels, olens, k * chunk_frames, chunk_frames)` for k = 0 ..
+        ceil(Lmax / chunk_frames) - 1, the last one cut at Lmax, so that the chunks concatenated along time are
+        `forward(mels, olens)`.  Utterances that have ended give rows of 0 (alens 0)."""
+        self._check_frames(chunk_frames)
+        yield from self._stream(mels, chunk_frames, lambda c0, n: self.window(mels, olens, c0, n))
 
     @staticmethod
     def _starts(starts, B: int, device: torch.device) -> torch.Tensor:

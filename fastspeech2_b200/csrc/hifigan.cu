@@ -33,95 +33,30 @@
 // A GEMM row depends only on its own utterance's input rows, in a fixed K order, and every producer reads rows of its own
 // utterance below lens_s only, so per-utterance results do not depend on the batch.
 //
-// Windows (fs2_hifigan_window, DESIGN.md section 17): the same kernels and GEMMs on a window of each utterance's rows.
-// Walking back from the audio, conv_post reads 3 rows on each side, each MRF R = the largest resblock reach, and
-// upsampling s reads r_s input rows around its core (the polyphase rule above); conv_pre reads 3 frames more.  For the core
-// frames [c0, c1), level s (0 = conv_pre's output, s >= 1 = upsampling s-1's output) holds global rows
-// [c0 up_s - h_s, c1 up_s + h_s) clipped to [0, olens up_s), h_0 = r_0 + 3 and h_{s+1} = u_s r_s, in a buffer of
-// n up_s + 2 h_s rows per utterance; upsampling s reads its input window [c0 up_s - r_s, c1 up_s + r_s) (clipped) out of
-// level s.  Every GEMM runs with lens = the clipped length, so the rows-past-lens and zero-fill rules above give each
-// convolution its padding wherever a buffer side is an utterance edge.  At a side that is not one, level 0 is wrong in its
-// outer 3 rows, level s+1 enters wrong in u_s / 2 rows (the edge phases read outside the operand) and each MRF widens that
-// by R; since u_s r_s >= (what the next layer reads) + u_s / 2, the wrong rows never reach the core.  A window descriptor
-// [start | len | n] x B per buffer (nullptr = the whole utterance: start 0, len = n = lens[b]) maps local rows to global
-// ones, and producers range-check only rows whose values equal the whole call's (exact_row).
+// Windows (fs2_hifigan_window, DESIGN.md section 17): the same kernels and GEMMs on a window of each utterance's rows, on
+// the chain plan of vocoder_window.cuh with R = the largest resblock's reach, level-0 margin 3 (conv_pre's native taps
+// read level-0 rows outside the window) and no tail.  For the core frames [c0, c1), level s holds global rows
+// [c0 up_s - h_s, c1 up_s + h_s) clipped to [0, olens up_s), in a buffer of n up_s + 2 h_s rows per utterance; upsampling s
+// reads its input window [c0 up_s - r_s, c1 up_s + r_s) (clipped) out of level s.  Every GEMM runs with lens = the clipped
+// length, so the rows-past-lens and zero-fill rules above give each convolution its padding wherever a buffer side is an
+// utterance edge.  A window descriptor [start | len | n] x B per buffer (nullptr = the whole utterance: start 0, len = n =
+// lens[b]) maps local rows to global ones, and producers range-check only rows whose values equal the whole call's
+// (exact_row).
 #include <math.h>
 
 #include <algorithm>
 #include <vector>
 
 #include "vocoder_weights.cuh"
+#include "vocoder_window.cuh"
 
 namespace fs2 {
 namespace {
 
-constexpr int kMels = 80, kHop = 256, kPreTaps = 7, kPostTaps = 7, kMaxUps = FS2_HIFIGAN_MAX_UPSAMPLES;
+constexpr int kMels = 80, kHop = 256, kPreTaps = 7, kPostTaps = 7;
 constexpr float kSlope = 0.1f, kPostSlope = 0.01f;   // hifi-gan's LRELU_SLOPE, and F.leaky_relu's default before conv_post
 
 __device__ __forceinline__ float lrelu(float v, float s) { return v > 0.f ? v : v * s; }
-
-// cumulative upsampling of stages 0 .. n, and the window plan (see the top of the file): the upsamplings' input reaches
-// r_s and the level halos h_s
-struct Ups { int n; int up[kMaxUps + 1]; int reach[kMaxUps]; int halo[kMaxUps + 1]; };
-
-// window descriptors of a window call: levels 0 .. U, the upsamplings' input windows, and the audio samples
-__host__ __device__ constexpr int win_level(int s) { return s; }
-__host__ __device__ constexpr int win_ups(int U, int s) { return U + 1 + s; }
-__host__ __device__ constexpr int win_audio(int U) { return 2 * U + 1; }
-__host__ __device__ constexpr int n_wins(int U) { return 2 * U + 2; }
-
-// rows of utterance b in a buffer: global rows [start, start + len) of the utterance's n rows at its rate
-struct Rows { int start, len, n; };
-__device__ __forceinline__ Rows rows_of(const int64_t* __restrict__ win, const int64_t* __restrict__ lens, int B, int b) {
-  if (!win) {
-    const int n = (int)lens[b];
-    return {0, n, n};
-  }
-  return {(int)win[b], (int)win[B + b], (int)win[2 * B + b]};
-}
-// local row t holds the whole call's values: not within `margin` rows of a window side that is not an utterance edge
-__device__ __forceinline__ bool exact_row(const Rows& r, int t, int margin) {
-  return (r.start == 0 || t >= margin) && (r.start + r.len == r.n || t < r.len - margin);
-}
-
-// one CTA: lens[s][b] = olens[b] * up_s for 1 <= olens[b] <= L, else 0 (the utterance is skipped); *status = 0 or
-// FS2_HIFIGAN_BAD_LENGTH.  Runs first, so the producers' range bits land on a cleared word.
-// starts != nullptr (a window of nf frames from starts[b]): lens = the n_wins(U) window descriptors instead, for the core
-// frames [c0, c1) = [starts[b], min(starts[b] + nf, olens[b])); empty (len 0) when that is empty or the utterance is
-// invalid, and FS2_HIFIGAN_BAD_START for starts[b] < 0.
-__global__ void hifigan_prep_kernel(const int64_t* __restrict__ olens, const int64_t* __restrict__ starts, int B, int L, int nf, Ups ups,
-                                    int64_t* __restrict__ lens, int* __restrict__ status) {
-  __shared__ int bad;
-  if (threadIdx.x == 0) bad = 0;
-  __syncthreads();
-  for (int b = threadIdx.x; b < B; b += blockDim.x) {
-    const int64_t n = olens[b];
-    const bool ok = n >= 1 && n <= L;
-    if (!ok) atomicOr(&bad, FS2_HIFIGAN_BAD_LENGTH);
-    if (!starts) {
-      for (int s = 0; s <= ups.n; ++s) lens[(long)s * B + b] = ok ? n * ups.up[s] : 0;
-      continue;
-    }
-    const int64_t c0 = starts[b];
-    if (c0 < 0) atomicOr(&bad, FS2_HIFIGAN_BAD_START);
-    const bool live = ok && c0 >= 0 && c0 < n;
-    const int64_t c1 = live ? min(c0 + nf, n) : 0;
-    auto put = [&](int w, int64_t lo, int64_t hi, int64_t total) {
-      int64_t* d = lens + 3L * w * B + b;
-      d[0] = live ? lo : 0;
-      d[B] = live ? hi - lo : 0;
-      d[2 * B] = live ? total : 0;
-    };
-    for (int s = 0; s <= ups.n; ++s) {
-      const int64_t up = ups.up[s], total = n * up;
-      put(win_level(s), max(c0 * up - ups.halo[s], (int64_t)0), min(c1 * up + ups.halo[s], total), total);
-      if (s < ups.n) put(win_ups(ups.n, s), max(c0 * up - ups.reach[s], (int64_t)0), min(c1 * up + ups.reach[s], total), total);
-    }
-    put(win_audio(ups.n), c0 * kHop, c1 * kHop, n * kHop);
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) *status = bad;
-}
 
 // conv_pre's operand [B * Lp][80]: mel frame start + t of utterance b for t < len (the rows of window win, nullptr: the
 // whole utterance, Lp = L), +0 past it (frames past olens[b] are never read).  Mel rows are L frames apart.
@@ -244,7 +179,7 @@ __global__ void __launch_bounds__(256) hifigan_post_kernel(const float* __restri
 struct Shape {
   int U, nk, type, steps, per;        // upsamplings, resblocks per MRF, resblock type, conv steps and convolutions per resblock
   int C[kMaxUps + 1];                  // stage widths C0 / 2^s
-  Ups ups;
+  UpsPlan ups;
   int layers;                          // convolutions in state_dict order
   long act;                            // floats per frame of the largest stage buffer, max_s up_s * C_s
 };
@@ -253,37 +188,23 @@ Shape shape_of(const fs2_hifigan_config& c) {
   Shape s;
   s.U = c.num_upsamples; s.nk = c.num_kernels; s.type = c.resblock;
   s.steps = s.type == 1 ? 3 : 2; s.per = s.type == 1 ? 6 : 2;
-  s.ups.n = s.U; s.ups.up[0] = 1;
-  s.C[0] = c.upsample_initial_channel;
-  s.act = s.C[0];
-  for (int i = 0; i < s.U; ++i) {
-    s.C[i + 1] = s.C[i] / 2;
-    s.ups.up[i + 1] = s.ups.up[i] * c.upsample_rates[i];
-    s.act = std::max(s.act, (long)s.ups.up[i + 1] * s.C[i + 1]);
-  }
-  s.layers = 2 + s.U + s.U * s.nk * s.per;
-  // the window plan: walking back from the audio, the rows each layer's input needs on each side of the core
   int R = 0;                                           // the MRF's reach: the largest resblock's
   for (int j = 0; j < s.nk; ++j) {
     int r = 0;
     for (int m = 0; m < s.steps; ++m) r += (c.resblock_kernel_sizes[j] - 1) / 2 * (c.resblock_dilation_sizes[j][m] + (s.type == 1));
     R = std::max(R, r);
   }
-  int need = kPostTaps / 2;
-  for (int i = s.U - 1; i >= 0; --i) {
-    need += R;
-    // output rows [-need, 0) of upsampling i's core: row o = u t + p reads input rows t - 1, t (p < u / 2) or t, t + 1
-    const int u = c.upsample_rates[i], o = -need, t = (o - (u - 1)) / u, p = o - t * u;   // floor division of a negative o
-    s.ups.reach[i] = need = -(p < u / 2 ? t - 1 : t);
-    s.ups.halo[i + 1] = u * need;
+  // the window plan: conv_pre's native taps leave its outer 3 rows wrong at a side that is not an utterance edge; no tail
+  s.ups = ups_plan(s.U, c.upsample_rates, R, kPreTaps / 2, kPostTaps / 2, 0);
+  s.C[0] = c.upsample_initial_channel;
+  s.act = s.C[0];
+  for (int i = 0; i < s.U; ++i) {
+    s.C[i + 1] = s.C[i] / 2;
+    s.act = std::max(s.act, (long)s.ups.up[i + 1] * s.C[i + 1]);
   }
-  s.ups.halo[0] = need + kPreTaps / 2;
+  s.layers = 2 + s.U + s.U * s.nk * s.per;
   return s;
 }
-
-// rows per utterance of level s's window buffer and of upsampling s's input window, for nf frames
-long level_rows(const Shape& sh, int s, long nf) { return nf * sh.ups.up[s] + 2L * sh.ups.halo[s]; }
-long ups_rows(const Shape& sh, int s, long nf) { return nf * sh.ups.up[s] + 2L * sh.ups.reach[s]; }
 
 int validate(const fs2_hifigan_config* c) {
   const char* who = "fs2_hifigan_create";
@@ -363,7 +284,7 @@ int resblock(int mode, int type, const VWeight* w, const int* dil, const float* 
 }
 
 struct HgPlan {
-  int64_t* lens;      // [U + 1][B]; a window call: the n_wins(U) window descriptors [start | len | n][B]
+  int64_t* lens;      // [U + 1][B]; a window call: the n_wins(sh.ups) window descriptors [start | len | n][B]
   void* a;            // GEMM operand
   float* xu;          // the upsampling output of the current stage
   float* s;           // MRF sum
@@ -388,9 +309,9 @@ HgPlan plan(Bump& b, const Shape& sh, int B, int L) {
 // A window call's workspace, from B and nf only: five buffers of the largest level buffer per utterance (rows x C over
 // every level; conv_pre's operand, 80 wide, and the upsamplings' operands, r_s <= h_s, fit in it)
 HgPlan window_plan(Bump& b, const Shape& sh, int B, int nf) {
-  long act = level_rows(sh, 0, nf) * kMels;
-  for (int s = 0; s <= sh.U; ++s) act = std::max(act, level_rows(sh, s, nf) * sh.C[s]);
-  return carve_plan(b, (size_t)3 * n_wins(sh.U) * B * sizeof(int64_t), (size_t)B * act);
+  long act = level_rows(sh.ups, 0, nf) * kMels;
+  for (int s = 0; s <= sh.U; ++s) act = std::max(act, level_rows(sh.ups, s, nf) * sh.C[s]);
+  return carve_plan(b, (size_t)3 * n_wins(sh.ups) * B * sizeof(int64_t), (size_t)B * act);
 }
 
 // a GEMM weight here is [taps][N][K] tap matrices with K = Cin, so vweight_pack_conv packs it at tap_stride = N K
@@ -399,17 +320,6 @@ void set_conv(VWeight& w, int N, int K, int taps) { w.N = N; w.K = K; w.taps = t
 int check_size(int math_mode, int B, int L) {
   FS2_REQUIRE(B >= 1 && L >= 1, "fs2_hifigan: need B >= 1 and Lmax >= 1 (got %d, %d)", B, L);
   return check_rows("fs2_hifigan", "B * Lmax * 256", "sample", (long)B * L * kHop, math_mode);
-}
-
-// a window's limits apply to its rows: the GEMMs of level s have B * level_rows(s, nf) rows (the upsamplings' fewer)
-int check_window(int math_mode, const Shape& sh, int B, int nf) {
-  FS2_REQUIRE(B >= 1 && nf >= 1, "fs2_hifigan_window: need B >= 1 and n_frames >= 1 (got %d, %d)", B, nf);
-  int top = 0;
-  for (int s = 1; s <= sh.U; ++s)
-    if (level_rows(sh, s, nf) > level_rows(sh, top, nf)) top = s;
-  char formula[64];
-  snprintf(formula, sizeof formula, "B * (%d * n_frames + %d)", sh.ups.up[top], 2 * sh.ups.halo[top]);
-  return check_rows("fs2_hifigan_window", formula, "window", (long)B * std::min(level_rows(sh, top, nf), 1L << 31), math_mode);
 }
 
 }  // namespace
@@ -431,7 +341,7 @@ namespace fs2 {
 namespace {
 
 // The generator on the plan p: whole utterances (starts == nullptr; level s has L up_s rows per utterance, lens [U + 1][B])
-// or a window of nf frames from starts[b] (level_rows / ups_rows per utterance, the n_wins(U) window descriptors).  Lout
+// or a window of nf frames from starts[b] (level_rows / ups_rows per utterance, the n_wins(sh.ups) window descriptors).  Lout
 // audio samples per row, rows ld apart.  Both enqueue the same kernels.
 int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const int64_t* olens, const int64_t* starts, int B, int L,
              int nf, float* audio, long ld, int* status, cudaStream_t st) {
@@ -440,10 +350,9 @@ int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const
   const int mode = m->math_mode, kind = out_kind(mode), U = sh.U;
   auto desc = [&](int i) -> const int64_t* { return w ? p.lens + 3L * i * B : nullptr; };
   auto lens = [&](int i, int s) -> const int64_t* { return w ? p.lens + (3L * i + 1) * B : p.lens + (long)s * B; };   // window i / level s
-  auto rows = [&](int s) { return w ? (int)level_rows(sh, s, nf) : L * sh.ups.up[s]; };
-  int rc;
-  hifigan_prep_kernel<<<1, 256, 0, st>>>(olens, starts, B, L, nf, sh.ups, p.lens, status);
-  FS2_LAUNCH_CHECK();
+  auto rows = [&](int s) { return w ? (int)level_rows(sh.ups, s, nf) : L * sh.ups.up[s]; };
+  int rc = ups_prep(olens, starts, B, L, nf, sh.ups, p.lens, status, st);
+  if (rc) return rc;
   {
     auto k = pick(kind, hifigan_mel_operand_kernel<OUT_HILO>, hifigan_mel_operand_kernel<OUT_HI>, hifigan_mel_operand_kernel<OUT_F32>);
     k<<<grid_for((long)B * rows(0) * (kMels / 4), 256), 256, 0, st>>>(mels, lens(win_level(0), 0), desc(win_level(0)), B, L, rows(0),
@@ -456,7 +365,8 @@ int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const
   const float* r = nullptr;
   int nk_in = 1;
   for (int s = 0; s < U; ++s) {
-    const int Lin = w ? (int)ups_rows(sh, s, nf) : rows(s), Lp = rows(s + 1), C = sh.C[s + 1], uw = win_ups(U, s), lw = win_level(s + 1);
+    const int Lin = w ? (int)ups_rows(sh.ups, s, nf) : rows(s), Lp = rows(s + 1), C = sh.C[s + 1];
+    const int uw = win_ups(sh.ups, s), lw = win_level(s + 1);
     if ((rc = upsample(mode, m->up[s], x, r, nk_in, desc(win_level(s)), rows(s), lens(uw, s), desc(uw), B, Lin, sh.C[s], p.a, p.xu, status,
                        st)))
       return rc;
@@ -479,7 +389,7 @@ int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const
   }
   const int Lout = (w ? nf : L) * kHop, C = sh.C[U];
   hifigan_post_kernel<<<grid_for((long)B * Lout, 256), 256, kPostTaps * C * sizeof(float), st>>>(
-      x, r, nk_in, lens(win_level(U), U), desc(win_level(U)), desc(win_audio(U)), B, rows(U), Lout, ld, C, m->post_w, m->post_b, audio);
+      x, r, nk_in, lens(win_level(U), U), desc(win_level(U)), desc(win_audio(sh.ups)), B, rows(U), Lout, ld, C, m->post_w, m->post_b, audio);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
@@ -576,7 +486,7 @@ int fs2_hifigan(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, int
 
 int fs2_hifigan_window_workspace_bytes(fs2_hifigan_gen* m, int B, int n_frames, size_t* bytes) {
   FS2_REQUIRE(m && bytes, "fs2_hifigan_window_workspace_bytes: null argument");
-  int rc = check_window(m->math_mode, m->sh, B, n_frames);
+  int rc = check_window_rows("fs2_hifigan_window", m->sh.ups, B, n_frames, m->math_mode);
   if (rc) return rc;
   Bump b(nullptr, 0);
   window_plan(b, m->sh, B, n_frames);
@@ -588,12 +498,9 @@ int fs2_hifigan_window(fs2_hifigan_gen* m, const float* mels, const int64_t* ole
                        float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream) {
   FS2_REQUIRE(m && mels && olens && starts && audio && status && ws, "fs2_hifigan_window: null argument");
   FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "fs2_hifigan_window: mels must be 16-byte aligned");
-  int rc = check_window(m->math_mode, m->sh, B, n_frames);
+  int rc = check_window_rows("fs2_hifigan_window", m->sh.ups, B, n_frames, m->math_mode);
   if (rc) return rc;
-  FS2_REQUIRE(Lmax >= 1 && (long)Lmax * kHop < (1L << 31), "fs2_hifigan_window: need 1 <= Lmax and Lmax * 256 below 2^31 (got Lmax = %d)",
-              Lmax);
-  FS2_REQUIRE(audio_ld >= (int64_t)n_frames * kHop, "fs2_hifigan_window: audio_ld = %lld below n_frames * 256 = %ld", (long long)audio_ld,
-              (long)n_frames * kHop);
+  if ((rc = check_window_extent("fs2_hifigan_window", Lmax, 0, kHop, n_frames, audio_ld))) return rc;
   Bump b(ws, ws_bytes);
   HgPlan p = window_plan(b, m->sh, B, n_frames);
   if ((rc = b.check("fs2_hifigan_window"))) return rc;

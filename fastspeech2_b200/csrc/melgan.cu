@@ -25,17 +25,18 @@
 // own input row and the epilogue stores 0 there.  Every producer reads rows of its own utterance below lens_s only, so
 // per-utterance results do not depend on the batch.
 //
-// Windows (fs2_melgan_window, DESIGN.md section 11): the same kernels and GEMMs on a window of each utterance's rows.
-// Every buffer then holds, per utterance, rows [start, start + len) of the utterance's n rows at its rate (a window
-// descriptor [start | len | n] x B in the workspace; nullptr = the whole utterance, start 0 and len = n = lens[b]).
-// Producers map a local row to its global row, reflect or zero-pad at the utterance's true edges, and read a source
-// outside the window as 0: such rows lie in the halo and are discarded.  Only rows whose values equal the whole call's
-// (all but `margin` rows at a window side that is not an utterance edge) are range-checked.
+// Windows (fs2_melgan_window, DESIGN.md section 11; vocoder_window.cuh): the same kernels and GEMMs on a window of each
+// utterance's rows.  Every buffer then holds, per utterance, rows [start, start + len) of the utterance's n rows at its
+// rate (a window descriptor [start | len | n] x B in the workspace; nullptr = the whole utterance).  Producers map a local
+// row to its global row, reflect or zero-pad at the utterance's true edges, and read a source outside the window as 0:
+// such rows lie in the halo and are discarded.  Only rows whose values equal the whole call's (all but `margin` rows at a
+// window side that is not an utterance edge) are range-checked.
 #include <math.h>
 
 #include <algorithm>
 
 #include "vocoder_weights.cuh"
+#include "vocoder_window.cuh"
 
 namespace fs2 {
 namespace {
@@ -56,85 +57,23 @@ __device__ __forceinline__ float lrelu(float v) { return v > 0.f ? v : v * 0.2f;
 __device__ __forceinline__ float4 lrelu4(float4 v) { return make_float4(lrelu(v.x), lrelu(v.y), lrelu(v.z), lrelu(v.w)); }
 
 // ---- window plan (DESIGN.md section 11) ----
-// rows ConvTranspose s reads on each side of its core, at its input's rate: what the next ResStack (reach 13) and the
-// layers after it need, divided by the stride, plus one row for the phases that read row t - 1 or t + 1
-__host__ __device__ constexpr int reach(int s) { return s == 0 ? 3 : s == 1 ? 4 : s == 2 ? 12 : 9; }
-__host__ __device__ constexpr int stride_of(int s) { return s < 2 ? 8 : 2; }        // kStride[s], usable on the device
+// The chain plan with MelGAN's parameters: a ResStack reads 1 + 3 + 9 rows on each side, the first conv's producer stacks
+// its taps from mel frames (so level 0 has no wrong rows), the last conv reads 3, and 10 tail frames.
 constexpr int kResReach = 1 + 3 + 9, kPostReach = kPostTaps / 2;
-// halo of buffer s on each side of its core: 3 first-conv rows (level 0), else stride * reach of the ConvTranspose that
-// writes it; the ConvTranspose s input window is the level-s core +- reach(s)
-__host__ __device__ constexpr int level_halo(int s) { return s == 0 ? reach(0) : stride_of(s - 1) * reach(s - 1); }
-// rows per utterance of level s and of ConvTranspose s's input window, for n frames; level_rows(s + 1) = stride * convt_rows(s)
-__host__ __device__ constexpr long level_rows(int s, long n) { return n * upsampling(s) + 2 * level_halo(s); }
-__host__ __device__ constexpr long convt_rows(int s, long n) { return n * upsampling(s) + 2 * reach(s); }
-// halo rows whose values differ from the whole call's at a window side that is not an utterance edge: ConvTranspose s's
-// phases at its input window's edge read a row outside it, so level s + 1 starts with stride / 2 such rows; every residual
-// block adds its dilation.  The next layer's input window must lie inside the exact rows:
-__host__ __device__ constexpr int level_margin(int s) { return s == 0 ? 0 : stride_of(s - 1) / 2; }
+constexpr UpsPlan kPlan = ups_plan(kStages, kStride, kResReach, 0, kPostReach, kTail);
+static_assert(kPlan.reach[0] == 3 && kPlan.reach[1] == 4 && kPlan.reach[2] == 12 && kPlan.reach[3] == 9, "DESIGN.md section 11");
+static_assert(kPlan.halo[0] == 3 && kPlan.halo[1] == 24 && kPlan.halo[2] == 32 && kPlan.halo[3] == 24 && kPlan.halo[4] == 18,
+              "DESIGN.md section 11");
+// rows at a window side that is not an utterance edge whose values differ from the whole call's, on entry to level s:
+// ConvTranspose s-1's phases at its input window's edge read a row outside it; every residual block adds its dilation.
+// The next layer's input window must lie inside the exact rows:
+constexpr int level_margin(int s) { return s == 0 ? 0 : kStride[s - 1] / 2; }
 constexpr bool plan_is_exact() {
   for (int s = 1; s <= kStages; ++s)
-    if (level_margin(s) + kResReach > level_halo(s) - (s < kStages ? reach(s) : kPostReach)) return false;
-  return level_margin(0) <= level_halo(0) - reach(0);
+    if (level_margin(s) + kResReach > kPlan.halo[s] - (s < kStages ? kPlan.reach[s] : kPostReach)) return false;
+  return level_margin(0) <= kPlan.halo[0] - kPlan.reach[0];
 }
 static_assert(plan_is_exact(), "a window's halo must cover every layer's reach");
-// window descriptors of a window call: levels 0..4, ConvTranspose 1..3's input windows (ConvTranspose 0 reads all of
-// level 0), and the audio samples [c0 * 256, c1 * 256)
-constexpr int kWins = kStages + 1 + kStages - 1 + 1, kWinAudio = kWins - 1;
-__host__ __device__ constexpr int convt_win(int s) { return s == 0 ? 0 : kStages + s; }
-
-// rows of utterance b in a buffer (see the top of the file)
-struct Rows { int start, len, n; };
-__device__ __forceinline__ Rows rows_of(const int64_t* __restrict__ win, const int64_t* __restrict__ lens, int B, int b) {
-  if (!win) {
-    const int n = (int)lens[b];
-    return {0, n, n};
-  }
-  return {(int)win[b], (int)win[B + b], (int)win[2 * B + b]};
-}
-// local row t holds the whole call's values: not within `margin` rows of a window side that is not an utterance edge
-__device__ __forceinline__ bool exact_row(const Rows& r, int t, int margin) {
-  return (r.start == 0 || t >= margin) && (r.start + r.len == r.n || t < r.len - margin);
-}
-
-// one CTA: lens[s][b] = (olens[b] + 10) * up_s for 1 <= olens[b] <= L, else 0 (the utterance is skipped); *status = 0 or
-// FS2_MELGAN_BAD_LENGTH.  Runs first, so the producers' range bits land on a cleared word.
-// starts != nullptr (a window of nf frames from starts[b]): lens = the kWins window descriptors instead, for the core
-// frames [c0, c1) = [starts[b], min(starts[b] + nf, olens[b])); empty (len 0) when that is empty or the utterance is
-// invalid, and FS2_MELGAN_BAD_START for starts[b] < 0.
-__global__ void melgan_prep_kernel(const int64_t* __restrict__ olens, const int64_t* __restrict__ starts, int B, int L, int nf,
-                                   int64_t* __restrict__ lens, int* __restrict__ status) {
-  __shared__ int bad;
-  if (threadIdx.x == 0) bad = 0;
-  __syncthreads();
-  for (int b = threadIdx.x; b < B; b += blockDim.x) {
-    const int64_t n = olens[b];
-    const bool ok = n >= 1 && n <= L;
-    if (!ok) atomicOr(&bad, FS2_MELGAN_BAD_LENGTH);
-    if (!starts) {
-      for (int s = 0; s <= kStages; ++s) lens[s * B + b] = ok ? (n + kTail) * upsampling(s) : 0;
-      continue;
-    }
-    const int64_t c0 = starts[b];
-    if (c0 < 0) atomicOr(&bad, FS2_MELGAN_BAD_START);
-    const bool live = ok && c0 >= 0 && c0 < n;
-    const int64_t c1 = live ? min(c0 + nf, n) : 0;
-    auto put = [&](int w, int64_t lo, int64_t hi, int s) {
-      int64_t* d = lens + 3L * w * B + b;
-      d[0] = live ? lo : 0;
-      d[B] = live ? hi - lo : 0;
-      d[2 * B] = live ? (n + kTail) * upsampling(s) : 0;
-    };
-    put(0, max(c0 - reach(0), (int64_t)0), c1 + reach(0), 0);
-    for (int s = 0; s < kStages; ++s) {
-      const int64_t lo = max(c0 * upsampling(s) - reach(s), (int64_t)0), hi = c1 * upsampling(s) + reach(s);
-      if (s > 0) put(convt_win(s), lo, hi, s);
-      put(s + 1, lo * stride_of(s), hi * stride_of(s), s + 1);
-    }
-    put(kWinAudio, c0 * upsampling(kStages), c1 * upsampling(kStages), kStages);
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) *status = bad;
-}
 
 // first conv's operand [rows][7 * 80]: tap j of row t = (m + 5) / 5 at frame reflect(t + j - 3), m = the mel frame below
 // olens[b] or the tail value.  Frames past olens[b] are never read (NaN there changes nothing).  A window (win) reads the
@@ -440,7 +379,7 @@ namespace fs2 {
 namespace {
 
 struct MgPlan {
-  int64_t* lens;     // [5][B]; a window call: the kWins window descriptors [start | len | n][B]
+  int64_t* lens;     // [5][B]; a window call: the n_wins(kPlan) window descriptors [start | len | n][B]
   void* a;           // GEMM operand, up to rows * 3C of the widest stage
   float* x[2];       // activations [rows][C], ping-pong
   float* h;          // dilated conv output [rows][C] (unfused route only)
@@ -449,13 +388,13 @@ struct MgPlan {
 // A window call's workspace, from B and nf only: per utterance, the largest operand (rows x K over every producer) and
 // the largest activation (rows x C over every level) of the window's buffers
 MgPlan window_plan(Bump& b, int B, int nf) {
-  long op = level_rows(0, nf) * kMels * kPreTaps, act = level_rows(0, nf) * 512;
+  long op = level_rows(kPlan, 0, nf) * kMels * kPreTaps, act = level_rows(kPlan, 0, nf) * 512;
   for (int s = 0; s < kStages; ++s) {
-    op = std::max(op, std::max(convt_rows(s, nf) * 3 * kCin[s], level_rows(s + 1, nf) * 3 * kCout[s]));
-    act = std::max(act, level_rows(s + 1, nf) * kCout[s]);
+    op = std::max(op, std::max(ups_rows(kPlan, s, nf) * 3 * kCin[s], level_rows(kPlan, s + 1, nf) * 3 * kCout[s]));
+    act = std::max(act, level_rows(kPlan, s + 1, nf) * kCout[s]);
   }
   MgPlan p;
-  p.lens = (int64_t*)b.bytes((size_t)3 * kWins * B * sizeof(int64_t));
+  p.lens = (int64_t*)b.bytes((size_t)3 * n_wins(kPlan) * B * sizeof(int64_t));
   p.a = b.floats((size_t)B * op);
   p.x[0] = b.floats((size_t)B * act);
   p.x[1] = b.floats((size_t)B * act);
@@ -538,7 +477,7 @@ int upsample(int mode, const VWeight& w, const float* x, const int64_t* xwin, in
 }
 
 // The generator on the plan p: whole utterances (starts == nullptr; every buffer (Lmax + 10) * up_s rows per utterance,
-// lens [5][B]) or a window of nf frames from starts[b] (level_rows / convt_rows per utterance, the kWins window
+// lens [5][B]) or a window of nf frames from starts[b] (level_rows / ups_rows per utterance, the n_wins(kPlan) window
 // descriptors).  Lout audio samples per row, rows ld apart.  Both enqueue the same kernels.
 int generate(const fs2_melgan_gen* m, const MgPlan& p, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax,
              int nf, float* audio, long ld, int* status, cudaStream_t st) {
@@ -546,10 +485,9 @@ int generate(const fs2_melgan_gen* m, const MgPlan& p, const float* mels, const 
   const int mode = m->math_mode, kind = out_kind(mode);
   auto desc = [&](int i) -> const int64_t* { return w ? p.lens + 3L * i * B : nullptr; };
   auto lens = [&](int i, int s) -> const int64_t* { return w ? p.lens + (3L * i + 1) * B : p.lens + (long)s * B; };   // window i / level s
-  auto rows = [&](int s) { return w ? (int)level_rows(s, nf) : (Lmax + kTail) * upsampling(s); };
-  int rc;
-  melgan_prep_kernel<<<1, 256, 0, st>>>(olens, starts, B, Lmax, nf, p.lens, status);
-  FS2_LAUNCH_CHECK();
+  auto rows = [&](int s) { return w ? (int)level_rows(kPlan, s, nf) : (Lmax + kTail) * upsampling(s); };
+  int rc = ups_prep(olens, starts, B, Lmax, nf, kPlan, p.lens, status, st);
+  if (rc) return rc;
   {
     auto k = pick(kind, melgan_pre_operand_kernel<OUT_HILO>, melgan_pre_operand_kernel<OUT_HI>, melgan_pre_operand_kernel<OUT_F32>);
     k<<<grid_for((long)B * rows(0) * (kMels * kPreTaps / 4), 256), 256, 0, st>>>(mels, lens(0, 0), desc(0), B, Lmax, rows(0), (float*)p.a,
@@ -559,7 +497,7 @@ int generate(const fs2_melgan_gen* m, const MgPlan& p, const float* mels, const 
   if ((rc = vweight_gemm(mode, m->pre, p.a, B, rows(0), ACT_NONE, lens(0, 0), p.x[0], st))) return rc;
   int cur = 0;
   for (int s = 0; s < kStages; ++s) {
-    const int C = kCout[s], cw = convt_win(s), Lin = w ? (int)convt_rows(s, nf) : rows(s);
+    const int C = kCout[s], cw = win_ups(kPlan, s), Lin = w ? (int)ups_rows(kPlan, s, nf) : rows(s);
     // lrelu, ConvTranspose1d: [B * Lin][s Cout] row-major is [B * Lout][Cout]
     if ((rc = upsample(mode, m->up[s], p.x[cur], desc(s), rows(s), lens(cw, s), desc(cw), B, Lin, kCin[s], p.a, p.x[cur ^ 1], status, st)))
       return rc;
@@ -574,7 +512,7 @@ int generate(const fs2_melgan_gen* m, const MgPlan& p, const float* mels, const 
     }
   }
   const int Lout = (w ? nf : Lmax) * upsampling(kStages);
-  melgan_post_kernel<<<grid_for((long)B * Lout, 256), 256, 0, st>>>(p.x[cur], lens(kStages, kStages), desc(kStages), desc(kWinAudio), B,
+  melgan_post_kernel<<<grid_for((long)B * Lout, 256), 256, 0, st>>>(p.x[cur], lens(kStages, kStages), desc(kStages), desc(win_audio(kPlan)), B,
                                                                    rows(kStages), Lout, ld, m->post_w, m->post_b, audio);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
@@ -583,12 +521,6 @@ int generate(const fs2_melgan_gen* m, const MgPlan& p, const float* mels, const 
 int check_size(const fs2_melgan_gen* m, int B, int L) {
   FS2_REQUIRE(B >= 1 && L >= 1, "fs2_melgan: need B >= 1 and Lmax >= 1 (got %d, %d)", B, L);
   return check_rows("fs2_melgan", "B * (Lmax + 10) * 256", "sample", (long)B * (L + kTail) * upsampling(kStages), m->math_mode);
-}
-
-// a window's limits apply to its rows: the largest buffer, level 4, has B * level_rows(4, nf) rows
-int check_window(const fs2_melgan_gen* m, int B, int nf) {
-  FS2_REQUIRE(B >= 1 && nf >= 1, "fs2_melgan_window: need B >= 1 and n_frames >= 1 (got %d, %d)", B, nf);
-  return check_rows("fs2_melgan_window", "B * (256 * n_frames + 36)", "window", (long)B * level_rows(kStages, nf), m->math_mode);
 }
 
 }  // namespace
@@ -681,7 +613,7 @@ int fs2_melgan(fs2_melgan_gen* m, const float* mels, const int64_t* olens, int B
 
 int fs2_melgan_window_workspace_bytes(fs2_melgan_gen* m, int B, int n_frames, size_t* bytes) {
   FS2_REQUIRE(m && bytes, "fs2_melgan_window_workspace_bytes: null argument");
-  int rc = check_window(m, B, n_frames);
+  int rc = check_window_rows("fs2_melgan_window", kPlan, B, n_frames, m->math_mode);
   if (rc) return rc;
   Bump b(nullptr, 0);
   window_plan(b, B, n_frames);
@@ -693,12 +625,9 @@ int fs2_melgan_window(fs2_melgan_gen* m, const float* mels, const int64_t* olens
                       float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream) {
   FS2_REQUIRE(m && mels && olens && starts && audio && status && ws, "fs2_melgan_window: null argument");
   FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "fs2_melgan_window: mels must be 16-byte aligned");
-  int rc = check_window(m, B, n_frames);
+  int rc = check_window_rows("fs2_melgan_window", kPlan, B, n_frames, m->math_mode);
   if (rc) return rc;
-  FS2_REQUIRE(Lmax >= 1 && ((long)Lmax + kTail) * upsampling(kStages) < (1L << 31),
-              "fs2_melgan_window: need 1 <= Lmax and (Lmax + 10) * 256 below 2^31 (got Lmax = %d)", Lmax);
-  FS2_REQUIRE(audio_ld >= (int64_t)n_frames * upsampling(kStages), "fs2_melgan_window: audio_ld = %lld below n_frames * 256 = %ld",
-              (long long)audio_ld, (long)n_frames * upsampling(kStages));
+  if ((rc = check_window_extent("fs2_melgan_window", Lmax, kTail, upsampling(kStages), n_frames, audio_ld))) return rc;
   Bump b(ws, ws_bytes);
   MgPlan p = window_plan(b, B, n_frames);
   if ((rc = b.check("fs2_melgan_window"))) return rc;

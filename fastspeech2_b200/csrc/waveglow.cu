@@ -37,6 +37,7 @@
 #include <math.h>
 
 #include "vocoder_weights.cuh"
+#include "vocoder_window.cuh"
 
 namespace fs2 {
 namespace {
@@ -662,10 +663,7 @@ int fs2_waveglow_window(fs2_waveglow_net* m, const float* mels, const int64_t* o
   FS2_REQUIRE(isfinite(sigma) && sigma >= 0.0, "fs2_waveglow_window: sigma must be finite and >= 0");
   int rc = check_window(m, B, n_frames);
   if (rc) return rc;
-  FS2_REQUIRE(Lmax >= 1 && (long)Lmax * kSteps < (1L << 31), "fs2_waveglow_window: need 1 <= Lmax and Lmax * 32 below 2^31 (got Lmax = %d)",
-              Lmax);
-  FS2_REQUIRE(audio_ld >= (int64_t)n_frames * kHop, "fs2_waveglow_window: audio_ld = %lld below n_frames * 256 = %ld",
-              (long long)audio_ld, (long)n_frames * kHop);
+  if ((rc = check_window_extent("fs2_waveglow_window", Lmax, 0, kSteps, n_frames, audio_ld))) return rc;
   Bump b(ws, ws_bytes);
   WgPlan p = plan(b, m->math_mode, m->C, B, n_frames + 2 * kHalo, true);
   if ((rc = b.check("fs2_waveglow_window"))) return rc;

@@ -20,7 +20,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from ._kernel_module import HOP, MAX_WAV_VALUE, N_MELS, NeuralVocoder, _WNConv, normalise_checkpoint, read_checkpoint  # noqa: F401
+from ._kernel_module import (HOP, MAX_WAV_VALUE, N_MELS, NeuralVocoder, _WNConv, normalise_checkpoint, read_checkpoint,  # noqa: F401
+                             ups_window_plan)
 
 # hifi-gan's published config_v1.json, config_v2.json and config_v3.json (the fields the generator uses).  V2's widths
 # (128 ... 8) are refused by HiFiGANVocoder; the entry is here for its key list.
@@ -140,9 +141,7 @@ class HiFiGANVocoder(NeuralVocoder):
     GEMMs.  One host read per call (the device-side length and range checks).  `window` / `stream` /
     `forward(chunk_frames=)` give the same audio in windows of frames (DESIGN.md section 17)."""
 
-    _DESTROY, _WORKSPACE_BYTES = "fs2_hifigan_destroy", "fs2_hifigan_workspace_bytes"
-    _WINDOW_BYTES = "fs2_hifigan_window_workspace_bytes"
-    _STATUS = "FS2_HIFIGAN"
+    _NAME = "hifigan"
 
     def __init__(self, config="v1", math_mode: str = "3xf16"):
         super().__init__(math_mode)
@@ -163,21 +162,17 @@ class HiFiGANVocoder(NeuralVocoder):
         each side, each MRF R = its largest resblock's reach, upsampling s reads `reach[s]` input rows around its core, and
         conv_pre 3 frames more.  -> {"reach": [r_s], "halo": [h_s] (rows of level s on each side of its core; h_0 = r_0 + 3
         mel frames, h_{s+1} = u_s r_s), "R": R}."""
+        return ups_window_plan(*self._chain())
+
+    def _chain(self):
+        """The upsample rates; R = the largest resblock's reach; conv_pre's native taps leave its 3 outer rows wrong at a
+        window side that is not an utterance edge."""
         cfg = self.config
         steps = 3 if cfg["resblock"] == "1" else 2
         extra = 1 if cfg["resblock"] == "1" else 0
         R = max(sum((k - 1) // 2 * (d + extra) for d in dil[:steps])
                 for k, dil in zip(cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"]))
-        rates = cfg["upsample_rates"]
-        reach, halo, need = [0] * len(rates), [0] * (len(rates) + 1), 3
-        for s in reversed(range(len(rates))):
-            need += R
-            u = rates[s]
-            t, p = divmod(-need, u)                          # output row -need = u t + p reads t - 1 (p < u / 2) or t
-            reach[s] = need = -(t - 1 if p < u // 2 else t)
-            halo[s + 1] = u * need
-        halo[0] = need + 3
-        return {"reach": reach, "halo": halo, "R": R}
+        return cfg["upsample_rates"], R, 3
 
     def flops_per_frame(self) -> int:
         """Multiply-adds x 2 per mel frame of the generator's convolutions (the transposed ones counted as torch runs them:
@@ -244,65 +239,3 @@ class HiFiGANVocoder(NeuralVocoder):
     def _rows(self, B: int, L: int):
         """fs2_hifigan's largest buffer: B * Lmax * 256 sample rows."""
         return B * L * HOP, f"B * Lmax * {HOP}", "sample"
-
-    @staticmethod
-    def _call(h, mels, olens, B: int, L: int, audio: torch.Tensor, status: torch.Tensor, ws: torch.Tensor) -> None:
-        _lib.check(_lib.load().fs2_hifigan(h, _lib.ptr(mels), _lib.ptr(olens), B, L, _lib.ptr(audio), _lib.ptr(status), _lib.ptr(ws),
-                                           ws.numel(), _lib.stream_ptr(mels.device)), "fs2_hifigan")
-
-    def _window_rows(self, B: int, n_frames: int):
-        """fs2_hifigan_window's largest buffer: B * (up_s * n_frames + 2 h_s) rows for the level s with the most."""
-        halo, up, rows = self.window_plan()["halo"], 1, []
-        for s, h in enumerate(halo):
-            rows.append((up * n_frames + 2 * h, up, h))
-            if s < len(self.config["upsample_rates"]):
-                up *= self.config["upsample_rates"][s]
-        n, up, h = max(rows)
-        return B * n, f"B * ({up} * n_frames + {2 * h})"
-
-    def _window_call(self, h, mels, olens, starts, B: int, L: int, n_frames: int, audio: torch.Tensor, ld: int, status: torch.Tensor,
-                     ws: torch.Tensor) -> None:
-        dev = mels.device
-        with torch.cuda.device(dev):
-            _lib.check(_lib.load().fs2_hifigan_window(h, _lib.ptr(mels), _lib.ptr(olens), _lib.ptr(starts), B, L, n_frames, audio.data_ptr(),
-                                                      ld, _lib.ptr(status), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)),
-                       "fs2_hifigan_window")
-
-    # ---- synthesis ------------------------------------------------------------------------------------------------
-    def forward(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int | None = None):
-        """-> (audio [B, Lmax * 256] fp32, alens [B] int64 = olens * 256).
-
-        chunk_frames=k: the same bits, computed as windows of k frames written straight into the output, with the
-        workspace of one window (fs2_hifigan_window): in fp32 mode this vocodes batches the whole call refuses.  Still one
-        host read per call: the windows' status words are ORed on the device."""
-        if chunk_frames is not None:
-            mels, olens, B, L = self._window_inputs(mels, olens, chunk_frames)
-            return self._chunked(self._window_call, mels, olens, B, L, chunk_frames)
-        mels, olens, B, L = self._mels_olens(mels, olens)
-        return self._whole(self._call, mels, olens, B, L)
-
-    def _window_inputs(self, mels, olens, n_frames):
-        """_mels_olens with the window's limits in place of the whole call's (Lmax bounds only the per-utterance rows)."""
-        self._check_frames(n_frames)
-        def check(B, L):
-            self._check_window_size(B, n_frames)
-            if L * HOP >= 1 << 31:
-                raise ValueError(f"Lmax * {HOP} must stay below 2^31 samples (Lmax={L})")
-        return self._mels_olens(mels, olens, check)
-
-    def window(self, mels: torch.Tensor, olens: torch.Tensor, starts, n_frames: int):
-        """One window of the audio (DESIGN.md section 17): -> (audio [B, n_frames * 256] fp32, alens [B] int64 =
-        clamp(olens - starts, 0, n_frames) * 256).  audio[b, :alens[b]] are samples [starts[b] * 256, ...) of
-        `forward(mels, olens)[0][b]`, bit for bit; the rest is +0.  starts: an int (every utterance), a host list or
-        tensor, or a device tensor.  Only mel frames [starts[b] - h_0, starts[b] + n_frames + h_0) below olens[b] are read
-        (h_0 = window_plan()["halo"][0]: 13 for V1, 11 for V3); the workspace depends on B and n_frames only.  One host
-        read per call."""
-        mels, olens, B, L = self._window_inputs(mels, olens, n_frames)
-        return self._window(self._window_call, mels, olens, starts, B, L, n_frames)
-
-    def stream(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int = 32):
-        """Lockstep windows: yields (audio, alens) of `window(mels, olens, k * chunk_frames, chunk_frames)` for k = 0 ..
-        ceil(Lmax / chunk_frames) - 1, the last one cut at Lmax, so that the chunks concatenated along time are
-        `forward(mels, olens)`.  Utterances that have ended give rows of +0 (alens 0)."""
-        self._check_frames(chunk_frames)
-        yield from self._stream(mels, chunk_frames, lambda c0, n: self.window(mels, olens, c0, n))

@@ -49,8 +49,7 @@ class MelGANVocoder(NeuralVocoder):
     is the hub object's method.  math_mode: "3xf16" (default, fp32-class), "f16", "tf32" or "fp32" for the GEMMs.  One
     host read per call (the device-side length and range checks)."""
 
-    _DESTROY, _WORKSPACE_BYTES, _WINDOW_BYTES = "fs2_melgan_destroy", "fs2_melgan_workspace_bytes", "fs2_melgan_window_workspace_bytes"
-    _STATUS = "FS2_MELGAN"
+    _NAME, _TAIL = "melgan", 10
 
     def __init__(self, math_mode: str = "3xf16"):
         super().__init__(math_mode)
@@ -87,62 +86,14 @@ class MelGANVocoder(NeuralVocoder):
 
     def _rows(self, B: int, L: int):
         """fs2_melgan's largest buffer: B * (Lmax + 10) * 256 sample rows."""
-        return B * (L + 10) * HOP, f"B * (Lmax + 10) * {HOP}", "sample"
+        return B * (L + self._TAIL) * HOP, f"B * (Lmax + {self._TAIL}) * {HOP}", "sample"
 
-    def _window_rows(self, B: int, n_frames: int):
-        """fs2_melgan_window's largest buffer: B * (256 * n_frames + 36) rows."""
-        return B * (n_frames * HOP + 36), "B * (256 * n_frames + 36)"
-
-    def _window_call(self, h, mels, olens, starts, B: int, L: int, n_frames: int, audio: torch.Tensor, ld: int, status: torch.Tensor,
-                     ws: torch.Tensor) -> None:
-        dev = mels.device
-        with torch.cuda.device(dev):
-            _lib.check(_lib.load().fs2_melgan_window(h, _lib.ptr(mels), _lib.ptr(olens), _lib.ptr(starts), B, L, n_frames, audio.data_ptr(), ld,
-                                                     _lib.ptr(status), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev)), "fs2_melgan_window")
-
-    @staticmethod
-    def _call(h, mels, olens, B: int, L: int, audio: torch.Tensor, status: torch.Tensor, ws: torch.Tensor) -> None:
-        _lib.check(_lib.load().fs2_melgan(h, _lib.ptr(mels), _lib.ptr(olens), B, L, _lib.ptr(audio), _lib.ptr(status), _lib.ptr(ws),
-                                          ws.numel(), _lib.stream_ptr(mels.device)), "fs2_melgan")
+    def _chain(self):
+        """The upsampling strides; a ResStack reads 1 + 3 + 9 rows on each side; the first conv's producer reads mel frames
+        for every tap, so level 0 has no wrong rows."""
+        return [s for _, _, s in _STAGES], 1 + 3 + 9, 0
 
     # ---- synthesis ------------------------------------------------------------------------------------------------
-    def forward(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int | None = None):
-        """-> (audio [B, Lmax * 256] fp32, alens [B] int64 = olens * 256).
-
-        chunk_frames=k: the same bits, computed as windows of k frames written straight into the output, with the
-        workspace of one window (fs2_melgan_window): in fp32 mode this vocodes batches the whole call refuses.  Still one
-        host read per call: the windows' status words are ORed on the device."""
-        if chunk_frames is not None:
-            mels, olens, B, L = self._window_inputs(mels, olens, chunk_frames)
-            return self._chunked(self._window_call, mels, olens, B, L, chunk_frames)
-        mels, olens, B, L = self._mels_olens(mels, olens)
-        return self._whole(self._call, mels, olens, B, L)
-
-    def _window_inputs(self, mels, olens, n_frames):
-        """_mels_olens with the window's limits in place of the whole call's (Lmax bounds only the per-utterance rows)."""
-        self._check_frames(n_frames)
-        def check(B, L):
-            self._check_window_size(B, n_frames)
-            if (L + 10) * HOP >= 1 << 31:
-                raise ValueError(f"(Lmax + 10) * {HOP} must stay below 2^31 samples (Lmax={L})")
-        return self._mels_olens(mels, olens, check)
-
-    def window(self, mels: torch.Tensor, olens: torch.Tensor, starts, n_frames: int):
-        """One window of the audio (DESIGN.md section 11): -> (audio [B, n_frames * 256] fp32, alens [B] int64 =
-        clamp(olens - starts, 0, n_frames) * 256).  audio[b, :alens[b]] are samples [starts[b] * 256, ...) of
-        `forward(mels, olens)[0][b]`, bit for bit; the rest is 0.  starts: an int (every utterance), a host list or tensor,
-        or a device tensor.  Only mel frames [starts[b] - 6, starts[b] + n_frames + 6) below olens[b] are read; the
-        workspace depends on B and n_frames only.  One host read per call."""
-        mels, olens, B, L = self._window_inputs(mels, olens, n_frames)
-        return self._window(self._window_call, mels, olens, starts, B, L, n_frames)
-
-    def stream(self, mels: torch.Tensor, olens: torch.Tensor, chunk_frames: int = 32):
-        """Lockstep windows: yields (audio, alens) of `window(mels, olens, k * chunk_frames, chunk_frames)` for k = 0 ..
-        ceil(Lmax / chunk_frames) - 1, the last one cut at Lmax, so that the chunks concatenated along time are
-        `forward(mels, olens)`.  Utterances that have ended give rows of 0 (alens 0)."""
-        self._check_frames(chunk_frames)
-        yield from self._stream(mels, chunk_frames, lambda c0, n: self.window(mels, olens, c0, n))
-
     @staticmethod
     def quantize(audio: torch.Tensor) -> torch.Tensor:
         """The hub object's int16 conversion: * 32768, clamp to [-32768, 32767], truncate toward zero."""

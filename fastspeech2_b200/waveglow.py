@@ -89,9 +89,7 @@ class WaveGlowVocoder(NeuralVocoder):
     lockstep windows whose concatenation is `forward`, and `forward(..., chunk_frames=k)` computes the whole call's bits
     window by window.  A window's workspace depends on B and n_frames only."""
 
-    _DESTROY = "fs2_waveglow_destroy"
-    _WORKSPACE_BYTES, _WINDOW_BYTES = "fs2_waveglow_workspace_bytes", "fs2_waveglow_window_workspace_bytes"
-    _STATUS = "FS2_WAVEGLOW"
+    _NAME = "waveglow"
 
     def __init__(self, n_channels: int = 512, math_mode: str = "3xf16"):
         super().__init__(math_mode)
@@ -258,8 +256,7 @@ class WaveGlowVocoder(NeuralVocoder):
 
         def check(B, L):
             self._check_window_size(B, n_frames)
-            if L * STEPS >= 1 << 31:
-                raise ValueError(f"Lmax * {STEPS} must stay below 2^31 steps (Lmax={L})")
+            self._check_extent(L, STEPS, "steps")
         return self._inputs(mels, olens, sigma, seed, z, check)
 
     @staticmethod

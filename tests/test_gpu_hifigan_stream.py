@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 import torch
 
-import _hifigan_window_plan as P
+import _ups_window_plan as P
 from conftest import GOLDEN
 from fastspeech2_b200 import _lib
 from fastspeech2_b200.hifigan import CONFIGS, HOP, HiFiGANVocoder
@@ -43,8 +43,8 @@ def check_coverage():
     """What the case table must reach for V1 and V3 (tests/test_hifigan_stream_args.py runs this without a GPU)."""
     missing = []
     for name in CONFIG_NAMES:
-        cfg = CONFIGS[name]
-        U, h0 = len(cfg["upsample_rates"]), P.level_halo(cfg, 0)
+        cfg = P.hifigan(CONFIGS[name])
+        U, h0 = len(cfg.rates), P.level_halo(cfg, 0)
         los = {}
         for kind, n in CASES:
             for s, o in zip(_starts(kind, n), OLENS):

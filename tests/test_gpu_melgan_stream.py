@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-import _melgan_window_plan as P
+import _ups_window_plan as P
 from conftest import GOLDEN
 from fastspeech2_b200 import _lib
 from fastspeech2_b200.melgan import HOP, MelGANVocoder
@@ -43,12 +43,12 @@ def check_coverage():
     los = {}
     for kind, n in CASES:
         for s, o in zip(_starts(kind, n), OLENS):
-            for name, (lo, _) in P.windows(s, n, o).items():
+            for name, (lo, _) in P.windows(P.melgan(), s, n, o).items():
                 los.setdefault(name, set()).add(lo)
-    for name in [f"level{s}" for s in range(5)] + [f"convt{s}" for s in range(1, 4)]:
+    for name in [f"level{s}" for s in range(5)] + [f"ups{s}" for s in range(1, 4)]:
         if not any(lo % 128 for lo in los.get(name, ())):
             missing.append(f"{name}: no start row off a 128-row tile boundary")
-    for name in ["level0", "convt1", "convt2", "convt3"]:               # the levels ConvTranspose writes start at s * lo
+    for name in ["level0", "ups1", "ups2", "ups3"]:               # the levels ConvTranspose writes start at s * lo
         if not any(lo % 16 for lo in los.get(name, ())):
             missing.append(f"{name}: no start row off a 16-row boundary")
     starts = [(s, o, n) for kind, n in CASES for s, o in zip(_starts(kind, n), OLENS)]

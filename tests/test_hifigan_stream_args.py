@@ -1,5 +1,5 @@
-"""Windowed HiFi-GAN without a GPU: the window plan (tests/_hifigan_window_plan.py) against the documented numbers and the
-float64 oracle's NaN cone, its exactness over a grid of accepted configs, the window workspace against
+"""Windowed HiFi-GAN without a GPU: the window plan (tests/_ups_window_plan.py) against the documented numbers and the
+float64 oracle's NaN cone, its exactness over a grid of accepted configs and MelGAN's chain, the window workspace against
 fs2_hifigan_window_workspace_bytes, argument validation of the C entry point and of `HiFiGANVocoder.window / stream /
 forward(chunk_frames=)`, and the GPU case table's coverage."""
 import ctypes as C
@@ -10,7 +10,7 @@ import os
 import pytest
 import torch
 
-import _hifigan_window_plan as P
+import _ups_window_plan as P
 from conftest import REPO
 from fastspeech2_b200 import _lib
 from fastspeech2_b200.hifigan import CONFIGS, HiFiGANVocoder, check_config, load_config
@@ -19,13 +19,13 @@ from oracle import hifigan_oracle as O
 
 # ---- the plan's numbers (DESIGN.md section 17) ---------------------------------------------------------------------------
 def test_plan_numbers_for_v1_and_v3():
-    v1, v3 = CONFIGS["v1"], CONFIGS["v3"]
-    assert P.mrf_reach(v1) == 60 and P.mrf_reach(v3) == 45
+    v1, v3 = P.hifigan(CONFIGS["v1"]), P.hifigan(CONFIGS["v3"])
+    assert v1.R == 60 and v3.R == 45
     assert [P.ups_reach(v1, s) for s in range(4)] == [10, 14, 47, 32]
     assert [P.ups_reach(v3, s) for s in range(3)] == [8, 8, 13]
     assert [P.level_halo(v1, s) for s in range(5)] == [13, 80, 112, 94, 64]
     assert [P.level_halo(v3, s) for s in range(4)] == [11, 64, 64, 52]
-    assert P.reaches(v1)["conv_pre"] == 13 and P.reaches(v3)["conv_pre"] == 11
+    assert P.reaches(v1)["pre"] == 13 and P.reaches(v3)["pre"] == 11
     assert [round(100 * P.window_flop_overhead(v1, n), 1) for n in (16, 32, 64, 128)] == [40.0, 20.0, 10.0, 5.0]
     assert [round(100 * P.window_flop_overhead(v3, n), 1) for n in (16, 32, 64, 128)] == [26.6, 13.3, 6.7, 3.3]
     assert round(P.workspace_bytes(v1, 64, 32) / 1e6) == 372 and round(P.workspace_bytes(v3, 64, 32) / 1e6) == 340
@@ -36,11 +36,11 @@ def test_plan_numbers_for_v1_and_v3():
 
 @pytest.mark.parametrize("name", ["v1", "v3"])
 def test_vocoder_plan_and_window_rows_match_the_restated_plan(name):
-    cfg = CONFIGS[name]
+    cfg = P.hifigan(CONFIGS[name])
     v = HiFiGANVocoder(name)
-    U = len(cfg["upsample_rates"])
+    U = len(cfg.rates)
     assert v.window_plan() == {"reach": [P.ups_reach(cfg, s) for s in range(U)], "halo": [P.level_halo(cfg, s) for s in range(U + 1)],
-                               "R": P.mrf_reach(cfg)}
+                               "R": cfg.R}
     for B, n in ((1, 1), (7, 13), (64, 32)):
         assert v._window_rows(B, n)[0] == B * max(P.level_rows(cfg, s, n) for s in range(U + 1))
     assert v._window_rows(1, 32)[1] == f"B * (256 * n_frames + {2 * P.level_halo(cfg, U)})"
@@ -71,7 +71,7 @@ def test_plan_reach_matches_the_nan_cone(name):
     """A NaN mel frame just outside [c0 - h_0, c1 + h_0) leaves the chunk's audio finite; one just inside reaches it."""
     cfg = CONE_CONFIGS[name]
     gen = _generator(cfg)
-    h0 = P.level_halo(cfg, 0)
+    h0 = P.level_halo(P.hifigan(cfg), 0)
     c0, c1 = h0 + 3, h0 + 7
     frames = c1 + h0 + 3
     base = torch.randn(1, 80, frames, generator=torch.Generator().manual_seed(3), dtype=torch.float64) * 2 - 6
@@ -103,33 +103,36 @@ def _rate_lists():
 
 
 def _grid():
+    """Accepted hifi-gan configs as chains, and MelGAN's chain."""
+    yield P.melgan()
     for rates in _rate_lists():
         for resblock, kers, dils in (("1", [3, 7, 11], [[1, 3, 5]] * 3), ("2", [3, 5, 7], [[1, 2], [2, 6], [3, 12]]),
                                      ("1", [1], [[1, 1, 1]]), ("2", [31, 3], [[1024, 7], [1, 1]]), ("1", [5], [[2, 9, 1]])):
-            yield {"resblock": resblock, "upsample_rates": list(rates), "upsample_kernel_sizes": [2 * u for u in rates],
+            cfg = {"resblock": resblock, "upsample_rates": list(rates), "upsample_kernel_sizes": [2 * u for u in rates],
                    "upsample_initial_channel": 32 << len(rates), "resblock_kernel_sizes": kers, "resblock_dilation_sizes": dils}
+            check_config(load_config(cfg))
+            yield P.hifigan(cfg)
 
 
 def test_plan_is_exact_for_every_accepted_config_of_a_grid():
     n = 0
     for cfg in _grid():
-        check_config(load_config(cfg))
         for level, wrong, room in P.exact_margins(cfg):
             assert wrong <= room, (cfg, level)
-        for s, u in enumerate(cfg["upsample_rates"]):
-            need = P.reaches(cfg)[f"mrf{s + 1}"]
+        for s, u in enumerate(cfg.rates):
+            need = P.reaches(cfg)[f"stack{s + 1}"]
             assert u * P.ups_reach(cfg, s) >= need + u // 2, (cfg, s)
             assert P.ups_reach(cfg, s) <= P.level_halo(cfg, s), (cfg, s)    # the upsampling's operand fits in its level
         # every buffer of a window lies inside its level's rows, and each upsampling's input window inside its level's
         for start, nf, olens in ((0, 1, 1), (3, 5, 40), (17, 32, 900), (880, 32, 900)):
             w = P.windows(cfg, start, nf, olens)
-            for s in range(len(cfg["upsample_rates"]) + 1):
+            for s in range(len(cfg.rates) + 1):
                 lo, hi = w[f"level{s}"]
                 assert hi - lo <= P.level_rows(cfg, s, nf)
-                if s < len(cfg["upsample_rates"]):
+                if s < len(cfg.rates):
                     ulo, uhi = w[f"ups{s}"]
                     assert lo <= ulo and uhi <= hi and uhi - ulo <= P.ups_rows(cfg, s, nf)
-                    assert w[f"level{s + 1}"] == (ulo * cfg["upsample_rates"][s], uhi * cfg["upsample_rates"][s])
+                    assert w[f"level{s + 1}"] == (ulo * cfg.rates[s], uhi * cfg.rates[s])
         n += 1
     assert n >= 100
 
@@ -161,7 +164,7 @@ def _ws(lib, h, B, n):
 def test_window_workspace_is_the_plan_and_smaller_than_the_whole_call(handles, name):
     lib = _lib.load()
     h = handles[name, _lib.MATH_3XTF32]
-    cfg = CONFIGS[name]
+    cfg = P.hifigan(CONFIGS[name])
     for B, n in ((1, 1), (1, 32), (7, 13), (64, 16), (64, 32), (64, 64), (3, 901)):
         rc, got = _ws(lib, h, B, n)
         assert rc == 0 and got == P.workspace_bytes(cfg, B, n), (B, n)
@@ -220,7 +223,7 @@ def test_window_entry_rejects_bad_arguments_on_the_host(handles):
     assert call(L=0) == -1 and b"Lmax" in lib.fs2_last_error()
     assert call(L=(1 << 31) // 256) == -1 and b"Lmax" in lib.fs2_last_error()
     assert call(ld=8 * 256 - 1) == -1 and b"audio_ld" in lib.fs2_last_error()
-    need = P.workspace_bytes(CONFIGS["v3"], 2, 8)
+    need = P.workspace_bytes(P.hifigan(CONFIGS["v3"]), 2, 8)
     assert call(ws_bytes=need - 257) == -4 and b"workspace" in lib.fs2_last_error()
     # everything else valid (a row pitch above n_frames * 256 included): only the unloaded weights are left
     assert call(ws_bytes=need, ld=9 * 256) == -1 and b"not loaded" in lib.fs2_last_error()

@@ -262,9 +262,9 @@ def test_melgan_kernels_do_not_spill():
     if not reports:
         pytest.skip("no ptxas reports (library built elsewhere)")
     text = open(reports[0]).read()
-    # instantiations: prep, post (1 each), pre_operand and concat (3 operand kinds), taps (3 x 2), the fused residual block
-    # (4 channel counts x f16 / 3xF16)
-    expected = {"melgan_prep_kernel": 1, "melgan_post_kernel": 1, "melgan_pre_operand_kernel": 3, "melgan_concat_kernel": 3, "melgan_taps_kernel": 6, "melgan_block_kernel": 8}
+    # instantiations: post (1), pre_operand and concat (3 operand kinds), taps (3 x 2), the fused residual block (4 channel
+    # counts x f16 / 3xF16)
+    expected = {"melgan_post_kernel": 1, "melgan_pre_operand_kernel": 3, "melgan_concat_kernel": 3, "melgan_taps_kernel": 6, "melgan_block_kernel": 8}
     for kernel, n in expected.items():
         props = re.findall(r"Function properties for \S*%s\S*\n(.*)" % kernel, text)
         assert len(props) == n, (kernel, len(props))
@@ -282,3 +282,13 @@ def test_shared_weight_pack_kernels_do_not_spill():
         props = re.findall(r"Function properties for \S*%s\S*\n(.*)" % kernel, text)
         assert len(props) == 1, (kernel, len(props))
         assert "0 bytes spill stores, 0 bytes spill loads" in props[0], (kernel, props[0])
+
+
+def test_shared_window_prep_kernel_does_not_spill():
+    """The one prep kernel MelGAN and HiFi-GAN write their lengths and window descriptors with (csrc/vocoder_window.cu)."""
+    reports = glob.glob(os.path.join(REPO, "fastspeech2_b200", "build", "vocoder_window.ptxas.txt"))
+    if not reports:
+        pytest.skip("no ptxas reports (library built elsewhere)")
+    props = re.findall(r"Function properties for (\S*)\n(.*)", open(reports[0]).read())
+    assert len(props) == 1 and "ups_prep_kernel" in props[0][0], props
+    assert "0 bytes spill stores, 0 bytes spill loads" in props[0][1], props[0]

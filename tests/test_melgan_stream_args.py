@@ -1,4 +1,4 @@
-"""Windowed MelGAN without a GPU: the window plan (tests/_melgan_window_plan.py) against the float64 oracle's dependency
+"""Windowed MelGAN without a GPU: the window plan (tests/_ups_window_plan.py) against the float64 oracle's dependency
 cone, the window workspace against fs2_melgan_window_workspace_bytes, argument validation of the C entry point and of
 `MelGANVocoder.window / stream / forward(chunk_frames=)`, the GPU case table's coverage and the ptxas report."""
 import ctypes as C
@@ -9,12 +9,13 @@ import re
 import pytest
 import torch
 
-import _melgan_window_plan as P
+import _ups_window_plan as P
 from conftest import REPO
 from fastspeech2_b200 import _lib
 from fastspeech2_b200.melgan import MelGANVocoder
 from oracle import melgan_oracle as O
 
+MELGAN = P.melgan()
 
 # ---- the reach: the plan against the oracle's dependency cone -------------------------------------------------------
 def _generator():
@@ -23,16 +24,16 @@ def _generator():
 
 
 def _levels(gen, mel):
-    """Forward of the oracle's layers, keeping each layer's input: [('conv0', mel frames), ('convt0', ...), ('res0', ...),
+    """Forward of the oracle's layers, keeping each layer's input: [('pre', mel frames), ('ups0', ...), ('stack1', ...),
     ..., ('post', the last conv's input), ('audio', ...)], each [1, C, rows]."""
     seq = gen.generator
     x = (mel + 5.0) / 5.0
-    out = [("conv0", x)]
+    out = [("pre", x)]
     x = seq[1](seq[0](x))
     for s, i in enumerate((3, 6, 9, 12)):
-        out.append((f"convt{s}", x))
+        out.append((f"ups{s}", x))
         x = seq[i](seq[i - 1](x))
-        out.append((f"res{s}", x))
+        out.append((f"stack{s + 1}", x))
         x = seq[i + 1](x)
     out.append(("post", x))
     out.append(("audio", seq[17](seq[16](seq[15](seq[14](x))))))
@@ -40,12 +41,11 @@ def _levels(gen, mel):
 
 
 def _rate(name):
-    if name in ("conv0", "convt0"):
+    if name == "pre":
         return 1
     if name == "post":
         return 256
-    s = int(name[-1])
-    return P.UP[s] if name.startswith("convt") else P.UP[s + 1]
+    return P.ups(MELGAN)[int(name[-1])]
 
 
 # (frames of the whole input incl. the 10 tail frames, chunk [c0, c1)): interior chunks of 1, 4 and 13 frames, a chunk at
@@ -66,9 +66,9 @@ def test_plan_reach_is_the_oracle_backprop_cone(frames, c0, c1):
     audio = levels[-1][1]
     w = torch.randn(audio[0, 0, c0 * 256: c1 * 256].shape, generator=g, dtype=torch.float64)
     (audio[0, 0, c0 * 256: c1 * 256] * w).sum().backward()
-    reach = P.reaches()
+    reach = P.reaches(MELGAN)
     for name, t in levels[:-1]:
-        grad = mel.grad if name == "conv0" else t.grad
+        grad = mel.grad if name == "pre" else t.grad
         rows = (grad[0].abs().sum(0) != 0).nonzero().flatten()
         up, n = _rate(name), frames * _rate(name)
         want = (max(c0 * up - reach[name], 0), min(c1 * up + reach[name], n))
@@ -80,7 +80,7 @@ def test_plan_reach_matches_the_nan_cone():
     """A NaN mel frame just outside [c0 - 6, c1 + 6) leaves the chunk's audio finite; one just inside reaches it."""
     gen = _generator()
     c0, c1, frames = 15, 19, 34
-    r = P.reaches()["conv0"]
+    r = P.reaches(MELGAN)["pre"]
     assert r == 6
     base = torch.randn(1, 80, frames, generator=torch.Generator().manual_seed(3), dtype=torch.float64) * 2 - 6
     for f, inside in ((c0 - r - 1, False), (c0 - r, True), (c1 + r - 1, True), (c1 + r, False)):
@@ -98,24 +98,25 @@ def test_plan_reach_matches_the_nan_cone():
 
 
 def test_plan_layout_is_exact_and_as_documented():
-    assert P.reaches() == {"conv0": 6, "convt0": 3, "res0": 17, "convt1": 4, "res1": 25, "convt2": 12, "res2": 22,
-                           "convt3": 9, "res3": 16, "post": 3}
-    assert [P.level_halo(s) for s in range(5)] == [3, 24, 32, 24, 18]
-    for s, margin, room in P.exact_margins():
+    assert P.reaches(MELGAN) == {"pre": 6, "ups0": 3, "stack1": 17, "ups1": 4, "stack2": 25, "ups2": 12, "stack3": 22,
+                                 "ups3": 9, "stack4": 16, "post": 3}
+    assert [P.level_halo(MELGAN, s) for s in range(5)] == [3, 24, 32, 24, 18]
+    for s, margin, room in P.exact_margins(MELGAN):
         assert margin <= room, s
     for s in range(4):
-        assert P.level_rows(s + 1, 7) == P.STRIDES[s] * P.convt_rows(s, 7)
-    assert P.level_rows(4, 32) == 256 * 32 + 36
+        assert P.level_rows(MELGAN, s + 1, 7) == MELGAN.rates[s] * P.ups_rows(MELGAN, s, 7)
+    assert P.level_rows(MELGAN, 4, 32) == 256 * 32 + 36
+    assert P.n_windows(MELGAN) == 9                   # ConvTranspose 0's input window is all of level 0
     # every buffer of a window lies inside its level's rows, and the next layer's window inside it
     for start, n, olens in ((0, 1, 1), (3, 5, 40), (17, 32, 900), (890, 32, 900)):
-        w = P.windows(start, n, olens)
+        w = P.windows(MELGAN, start, n, olens)
         lvl = {s: w[f"level{s}"] for s in range(5)}
         for s in range(5):
-            assert lvl[s][1] - lvl[s][0] <= P.level_rows(s, n)
-            assert lvl[s][1] < (olens + 10) * P.UP[s]                      # the right side is never the utterance's edge
+            assert lvl[s][1] - lvl[s][0] <= P.level_rows(MELGAN, s, n)
+            assert lvl[s][1] < (olens + 10) * P.ups(MELGAN)[s]             # the right side is never the utterance's edge
         for s in range(1, 4):
-            lo, hi = w[f"convt{s}"]
-            assert lvl[s][0] <= lo and hi <= lvl[s][1] and hi - lo <= P.convt_rows(s, n)
+            lo, hi = w[f"ups{s}"]
+            assert lvl[s][0] <= lo and hi <= lvl[s][1] and hi - lo <= P.ups_rows(MELGAN, s, n)
 
 
 # ---- the workspace --------------------------------------------------------------------------------------------------
@@ -144,14 +145,14 @@ def test_window_workspace_is_the_plan_and_smaller_than_the_whole_call(handle):
     h = handle[_lib.MATH_3XTF32]
     for B, n in ((1, 1), (1, 32), (7, 13), (64, 16), (64, 32), (64, 64), (3, 901)):
         rc, got = _ws(lib, h, B, n)
-        assert rc == 0 and got == P.workspace_bytes(B, n), (B, n)
+        assert rc == 0 and got == P.workspace_bytes(MELGAN, B, n), (B, n)
         for L in (n + 1, 2 * n, 931):
             if n < L:
                 whole = C.c_size_t()
                 assert lib.fs2_melgan_workspace_bytes(h, B, L, C.byref(whole)) == 0
-                assert whole.value == P.whole_call_workspace_bytes(B, L)
+                assert whole.value == P.whole_call_workspace_bytes(MELGAN, B, L)
                 assert got < whole.value, (B, n, L)
-    assert abs(P.workspace_bytes(64, 32) / 1e9 - 0.415) < 0.001
+    assert abs(P.workspace_bytes(MELGAN, 64, 32) / 1e9 - 0.415) < 0.001
 
 
 @pytest.mark.gpu          # fs2_melgan_create needs a device; the checks themselves run on the host
@@ -201,7 +202,7 @@ def test_window_entry_rejects_bad_arguments_on_the_host(handle):
     assert call(L=0) == -1 and b"Lmax" in lib.fs2_last_error()
     assert call(L=(1 << 31) // 256) == -1 and b"Lmax" in lib.fs2_last_error()
     assert call(ld=8 * 256 - 1) == -1 and b"audio_ld" in lib.fs2_last_error()
-    need = P.workspace_bytes(2, 8)
+    need = P.workspace_bytes(MELGAN, 2, 8)
     assert call(ws_bytes=need - 257) == -4 and b"workspace" in lib.fs2_last_error()
     # everything else valid (a row pitch above n_frames * 256 included): only the unloaded weights are left
     assert call(ws_bytes=need, ld=9 * 256) == -1 and b"not loaded" in lib.fs2_last_error()
@@ -290,6 +291,6 @@ def test_window_support_adds_no_instantiation_and_no_spill():
         pytest.skip("no ptxas reports (library built elsewhere)")
     text = open(reports[0]).read()
     props = re.findall(r"Function properties for (\S*melgan\S*)\n(.*)", text)
-    assert len(props) == 1 + 1 + 3 + 3 + 6 + 8                            # as before windows: runtime arguments only
+    assert len(props) == 1 + 3 + 3 + 6 + 8                                # as before windows: runtime arguments only
     for name, line in props:
         assert "0 bytes spill stores, 0 bytes spill loads" in line, (name, line)

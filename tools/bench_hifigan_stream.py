@@ -11,7 +11,7 @@ paragraph.  Per config (V1, V3), math mode (3xf16, f16) and window size n_frames
                     the whole call (`forward`), whose first sample is ready only when it ends;
   stream_ms         a full lockstep stream of windows (Lmax / n calls, the window's C entry on preallocated buffers) against
                     one `forward`, alternated: the measured overhead, beside the FLOP overhead counted from the window shapes
-                    (tests/_hifigan_window_plan.py);
+                    (tests/_ups_window_plan.py);
   graph / eager     at B = 1, where launches dominate: one window call eager against one replay of a captured graph;
   fp32_chunked      `forward(chunk_frames=64)` in fp32 on filelist64, which the whole call refuses (B * Lmax * 256 above
                     65535 * 128);
@@ -126,7 +126,7 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("needs a CUDA device")
-    import _hifigan_window_plan as P
+    import _ups_window_plan as P
     from fastspeech2_b200 import FeedForwardTransformer, _lib, synthetic_state_dict
     from fastspeech2_b200.hifigan import CONFIGS, HiFiGANVocoder
     from fastspeech2_b200.hparams import load_hp
@@ -225,7 +225,7 @@ def main():
                                "first_audio_ms": first_ms, "first_audio_ms_windows": first_w, "whole_call_ms": whole_ms,
                                "whole_call_ms_windows": whole_w, "window_workspace_bytes": ws_bytes(v, B, n),
                                "whole_call_workspace_bytes": ws_bytes(v, B, L=L),
-                               "flop_overhead_from_shapes": P.window_flop_overhead(cfg, n)}
+                               "flop_overhead_from_shapes": P.window_flop_overhead(P.hifigan(cfg), n)}
                         # a full stream over the paragraph at n = 16 is ~1900 calls: timed at n = 64 only
                         if wname == "filelist64" or n == 64:
                             t = alternate({"stream": s.run, "forward": lambda: v(m, o)}, args.steps, args.rounds)

@@ -96,7 +96,7 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("needs a CUDA device")
-    import _melgan_window_plan as P
+    import _ups_window_plan as P
     from fastspeech2_b200 import FeedForwardTransformer, synthetic_state_dict
     from fastspeech2_b200.hparams import load_hp
     from fastspeech2_b200.melgan import MelGANVocoder
@@ -156,7 +156,7 @@ def main():
                            "first_audio_ms": first_ms, "first_audio_ms_windows": first_w, "whole_call_ms": whole_ms,
                            "whole_call_ms_windows": whole_w, "window_workspace_bytes": ws_bytes(v, B, n),
                            "whole_call_workspace_bytes": ws_bytes(v, B, L=L),
-                           "flop_overhead_from_shapes": P.window_flop_overhead(n)}
+                           "flop_overhead_from_shapes": P.window_flop_overhead(P.melgan(), n)}
                     # a full stream over the paragraph at n = 16 is ~2300 calls: timed at n = 64 only
                     if wname == "filelist64" or n == 64:
                         t = alternate({"stream": s.run, "forward": lambda: v(m, o)}, args.steps, args.rounds)
