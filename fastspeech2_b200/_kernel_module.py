@@ -87,15 +87,15 @@ def read_checkpoint(path_or_dict, wrapper_key: str, what: str) -> dict:
 
 class _WNConv(nn.Module):
     """The parameters of one weight-normalised convolution, registered in `torch.nn.utils.weight_norm`'s order (bias,
-    weight_g, weight_v).  weight = weight_g * weight_v / |weight_v|, the norm taken per index of dim 0: output channels of
+    unless bias=False, weight_g, weight_v).  weight = weight_g * weight_v / |weight_v|, the norm taken per index of dim 0: output channels of
     a Conv1d [Cout, Cin, k], *input* channels of a ConvTranspose1d [Cin, Cout, k]."""
 
-    def __init__(self, cin: int, cout: int, k: int, transposed: bool = False):
+    def __init__(self, cin: int, cout: int, k: int, transposed: bool = False, bias: bool = True):
         super().__init__()
         proto = nn.ConvTranspose1d(cin, cout, k) if transposed else nn.Conv1d(cin, cout, k)   # torch's default init
         v = proto.weight.detach()
         self.transposed = transposed
-        self.bias = nn.Parameter(proto.bias.detach().clone())
+        self.bias = nn.Parameter(proto.bias.detach().clone()) if bias else None
         self.weight_g = nn.Parameter(torch.norm_except_dim(v, 2, 0).clone())
         self.weight_v = nn.Parameter(v.clone())
 
@@ -131,11 +131,14 @@ def normalise_checkpoint(module: nn.Module, sd) -> dict:
             continue
         if f"{p}.weight" in sd and (f"{p}.weight_g" in sd or f"{p}.weight_v" in sd):
             raise ValueError(f"unexpected key {p}.weight alongside {p}.weight_g / weight_v")
-        wanted = [f"{p}.bias"] + ([f"{p}.weight"] if f"{p}.weight" in sd else [f"{p}.weight_g", f"{p}.weight_v"])
-        shapes = {f"{p}.bias": m.bias.shape, f"{p}.weight": m.weight_v.shape, f"{p}.weight_g": m.weight_g.shape,
-                  f"{p}.weight_v": m.weight_v.shape}
+        wanted = [f"{p}.weight"] if f"{p}.weight" in sd else [f"{p}.weight_g", f"{p}.weight_v"]
+        wanted = ([f"{p}.bias"] if m.bias is not None else []) + wanted
+        shapes = {f"{p}.weight": m.weight_v.shape, f"{p}.weight_g": m.weight_g.shape, f"{p}.weight_v": m.weight_v.shape}
+        if m.bias is not None:
+            shapes[f"{p}.bias"] = m.bias.shape
         t = _take(sd, wanted, shapes)
-        out[f"{p}.bias"] = t[f"{p}.bias"]
+        if m.bias is not None:
+            out[f"{p}.bias"] = t[f"{p}.bias"]
         if f"{p}.weight" in t:
             w = t[f"{p}.weight"].contiguous()
             _, norms = torch._weight_norm_interface(w, torch.ones_like(m.weight_g, device="cpu"), 0)
@@ -183,7 +186,8 @@ class NeuralVocoder(nn.Module):
     call is call(h, mels, olens, B, Lmax, audio, status, ws), a window call call(h, mels, olens, starts, B, Lmax, n_frames,
     audio, audio_ld, status, ws).
 
-    MelGAN and HiFi-GAN, upsampling chains, also provide _chain() -> (upsample rates, stack reach R, level-0 margin) and
+    MelGAN, HiFi-GAN and BigVGAN, upsampling chains, also provide _chain() -> (upsample rates, stack reach R, level-0
+    margin[, the last layer's reach when it is not 3]) and
     take the rest from here: _call and _window_call on their C entries, the window's rows from the chain's plan, and
     forward, window and stream.  WaveGlow, whose calls carry the noise, has its own calls, window rows and those three."""
 
@@ -324,9 +328,9 @@ class NeuralVocoder(nn.Module):
 
     def _window_rows(self, B: int, n_frames: int):
         """An upsampling chain's largest window buffer: B * (up_s * n_frames + 2 h_s) rows for the level s with the most."""
-        rates, R, margin0 = self._chain()
+        rates, R, margin0, *post = self._chain()
         ups = itertools.accumulate(rates, operator.mul, initial=1)
-        n, up, h = max((up * n_frames + 2 * h, up, h) for up, h in zip(ups, ups_window_plan(rates, R, margin0)["halo"]))
+        n, up, h = max((up * n_frames + 2 * h, up, h) for up, h in zip(ups, ups_window_plan(rates, R, margin0, *post)["halo"]))
         return B * n, f"B * ({up} * n_frames + {2 * h})"
 
     def _window_inputs(self, mels, olens, n_frames):

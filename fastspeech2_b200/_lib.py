@@ -55,6 +55,8 @@ FS2_WAVEGLOW_BAD_START = 4                           # and of fs2_waveglow_windo
 FS2_HIFIGAN_BAD_LENGTH, FS2_HIFIGAN_RANGE = 1, 2     # bits of fs2_hifigan's device status word
 FS2_HIFIGAN_BAD_START = 4                            # and of fs2_hifigan_window's
 FS2_HIFIGAN_MAX_UPSAMPLES, FS2_HIFIGAN_MAX_KERNELS = 8, 8
+FS2_BIGVGAN_BAD_LENGTH, FS2_BIGVGAN_RANGE, FS2_BIGVGAN_BAD_START = 1, 2, 4   # bits of fs2_bigvgan's / fs2_bigvgan_window's status word
+FS2_BIGVGAN_SNAKE, FS2_BIGVGAN_SNAKEBETA = 0, 1
 
 
 class HiFiGANConfig(C.Structure):
@@ -64,6 +66,11 @@ class HiFiGANConfig(C.Structure):
                 ("upsample_initial_channel", C.c_int32), ("num_kernels", C.c_int32),
                 ("resblock_kernel_sizes", C.c_int32 * FS2_HIFIGAN_MAX_KERNELS), ("num_dilations", C.c_int32),
                 ("resblock_dilation_sizes", (C.c_int32 * 4) * FS2_HIFIGAN_MAX_KERNELS)]
+
+
+class BigVGANConfig(C.Structure):
+    _fields_ = [("gen", HiFiGANConfig), ("activation", C.c_int32), ("snake_logscale", C.c_int32), ("use_tanh_at_final", C.c_int32),
+                ("use_bias_at_final", C.c_int32)]
 
 
 class NoamAdamHp(C.Structure):
@@ -162,6 +169,15 @@ SIGNATURES = {
     "fs2_hifigan_window": [_P, _P, _P, _P, _I, _I, _I, _P, _L, _P, _P, _SZ, _P],
     "fs2_op_hifigan_resblock": [_I, _I, _I, _I, _I, C.POINTER(_I), _P, _P, _I, _I, C.POINTER(_P), C.POINTER(_P), _P, _P, _P],
     "fs2_op_hifigan_upsample": [_I, _I, _I, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P],
+    "fs2_bigvgan_create": [C.POINTER(_P), _I, C.POINTER(BigVGANConfig)],
+    "fs2_bigvgan_load": [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), _P],
+    "fs2_bigvgan_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_bigvgan": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_bigvgan_window_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_bigvgan_window": [_P, _P, _P, _P, _I, _I, _I, _P, _L, _P, _P, _SZ, _P],
+    "fs2_op_bigvgan_act": [_I, _I, _P, _P, _I, _I, C.POINTER(_P), _I, _I, _P, _P, _P],
+    "fs2_op_bigvgan_resblock": [_I, _I, _I, _I, _I, C.POINTER(_I), _P, _P, _I, _I, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), _I, _I, _P,
+                                _P, _P],
     "fs2_waveglow_create": [C.POINTER(_P), _I, _I],
     "fs2_waveglow_load": [_P, C.POINTER(_P), _I, _P],
     "fs2_waveglow_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
@@ -182,7 +198,8 @@ SIGNATURES = {
     "fs2_optim_noam_scalars": [_L, _I, C.POINTER(NoamAdamHp), _P, _P, _P, _P],
 }
 OTHER_SYMBOLS = ("fs2_last_error", "fs2_version", "fs2_destroy", "fs2_kernel_launches", "fs2_profile_label", "fs2_vocoder_destroy",
-                 "fs2_melgan_destroy", "fs2_waveglow_destroy", "fs2_features_destroy", "fs2_hifigan_destroy")
+                 "fs2_melgan_destroy", "fs2_waveglow_destroy", "fs2_features_destroy", "fs2_hifigan_destroy",
+                 "fs2_bigvgan_destroy")
 ALL_SYMBOLS = tuple(SIGNATURES) + OTHER_SYMBOLS
 
 _lib: Optional[C.CDLL] = None
@@ -222,6 +239,8 @@ def load() -> C.CDLL:
     lib.fs2_features_destroy.argtypes = [_P]
     lib.fs2_hifigan_destroy.restype = None
     lib.fs2_hifigan_destroy.argtypes = [_P]
+    lib.fs2_bigvgan_destroy.restype = None
+    lib.fs2_bigvgan_destroy.argtypes = [_P]
     _lib = lib
     return lib
 

@@ -70,6 +70,13 @@ def check_config(cfg: dict) -> None:
     other than "1" or "2"; upsample rates that are odd, whose product is not the hop 256, or whose kernel sizes are not
     twice the rate; a convolution width (upsample_initial_channel / 2^i) that is not a multiple of 32 (this refuses V2) or
     above 2048; even resblock kernel sizes; too few dilations per resblock."""
+    check_rates(cfg)
+    check_widths(cfg, 32)
+    check_resblocks(cfg)
+
+
+def check_rates(cfg: dict) -> None:
+    """check_config's rules before the widths: num_mels, the resblock type, the upsample rates and kernel sizes."""
     if cfg.get("num_mels", N_MELS) != N_MELS:
         raise ValueError(f"config: num_mels must be {N_MELS} (got {cfg['num_mels']})")
     if cfg["resblock"] not in ("1", "2"):
@@ -85,12 +92,20 @@ def check_config(cfg: dict) -> None:
         raise ValueError(f"config: the product of upsample_rates must be the hop {HOP} (got {math.prod(rates)})")
     if len(ks) != len(rates) or any(k != 2 * u for k, u in zip(ks, rates)):
         raise ValueError(f"config: upsample_kernel_sizes must be twice the upsample_rates (got {ks} for {rates})")
-    c0 = cfg["upsample_initial_channel"]
+
+
+def check_widths(cfg: dict, multiple: int) -> None:
+    """Every convolution width upsample_initial_channel / 2^i a multiple of `multiple`, at most 2048."""
+    c0, rates = cfg["upsample_initial_channel"], cfg["upsample_rates"]
     _ints("upsample_initial_channel", [c0])
     widths = [c0 // 2 ** i for i in range(len(rates) + 1)]
-    if c0 > 2048 or c0 % 2 ** len(rates) or any(w % 32 or w < 32 for w in widths):
+    if c0 > 2048 or c0 % 2 ** len(rates) or any(w % multiple or w < multiple for w in widths):
         raise ValueError(f"config: upsample_initial_channel = {c0} gives convolution widths {widths}; every one must be a "
-                         f"multiple of 32 (and at most 2048)")
+                         f"multiple of {multiple} (and at most 2048)")
+
+
+def check_resblocks(cfg: dict) -> None:
+    """check_config's rules after the widths: the resblock kernel sizes and dilations."""
     kers, dils = cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"]
     _ints("resblock_kernel_sizes", kers)
     if not 1 <= len(kers) <= _lib.FS2_HIFIGAN_MAX_KERNELS or any(k < 1 or k > 31 or k % 2 == 0 for k in kers):
@@ -102,6 +117,23 @@ def check_config(cfg: dict) -> None:
         _ints("resblock_dilation_sizes", d)
         if any(v < 1 or v > 1024 for v in d[:need]):
             raise ValueError(f"config: resblock_dilation_sizes must lie in [1, 1024] (got {dils})")
+
+
+def c_config(cfg: dict) -> _lib.HiFiGANConfig:
+    """The fs2_hifigan_config of a checked config."""
+    c = _lib.HiFiGANConfig()
+    c.resblock = int(cfg["resblock"])
+    c.num_upsamples = len(cfg["upsample_rates"])
+    for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
+        c.upsample_rates[i], c.upsample_kernel_sizes[i] = u, k
+    c.upsample_initial_channel = cfg["upsample_initial_channel"]
+    c.num_kernels = len(cfg["resblock_kernel_sizes"])
+    c.num_dilations = 3 if c.resblock == 1 else 2
+    for j, (k, d) in enumerate(zip(cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"])):
+        c.resblock_kernel_sizes[j] = k
+        for m in range(c.num_dilations):
+            c.resblock_dilation_sizes[j][m] = d[m]
+    return c
 
 
 class _ResBlock1(nn.Module):
@@ -212,20 +244,7 @@ class HiFiGANVocoder(NeuralVocoder):
 
     # ---- device state ---------------------------------------------------------------------------------------------
     def _c_config(self) -> _lib.HiFiGANConfig:
-        cfg = self.config
-        c = _lib.HiFiGANConfig()
-        c.resblock = int(cfg["resblock"])
-        c.num_upsamples = len(cfg["upsample_rates"])
-        for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
-            c.upsample_rates[i], c.upsample_kernel_sizes[i] = u, k
-        c.upsample_initial_channel = cfg["upsample_initial_channel"]
-        c.num_kernels = len(cfg["resblock_kernel_sizes"])
-        c.num_dilations = 3 if c.resblock == 1 else 2
-        for j, (k, d) in enumerate(zip(cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"])):
-            c.resblock_kernel_sizes[j] = k
-            for m in range(c.num_dilations):
-                c.resblock_dilation_sizes[j][m] = d[m]
-        return c
+        return c_config(self.config)
 
     def _create(self):
         h = C.c_void_p()

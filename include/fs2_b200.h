@@ -591,6 +591,58 @@ int fs2_op_hifigan_resblock(int math_mode, int type, int C, int k, int nd, const
 int fs2_op_hifigan_upsample(int math_mode, int Cin, int Cout, int u, const float* x, const int64_t* lens, int B, int Lin, const float* w,
                             const float* b, float* out, int* status, void* stream);
 
+/* ---- batched BigVGAN vocoder (DESIGN.md section 18) ----------------------------------------------------------------- */
+/* NVIDIA BigVGAN's generator on log-mels [B, Lmax, 80] with frame counts olens [B], with the call surface of fs2_hifigan:
+ * utterance b is the generator applied to mels[b, :olens[b]] alone (every convolution zero-pads and every Activation1d
+ * replicate-pads at its own edges), olens[b] * 256 samples, bit-identical to a B = 1 call, +0 past them; mel frames past
+ * olens[b] are never read.  No allocation, no synchronisation.  It enqueues 4 + U * (2 + K * G + max(K - 2, 0)) kernels,
+ * as fs2_hifigan: 160 for the 22 kHz base model, 238 for the large ones, in every math mode.  *status: FS2_BIGVGAN_BAD_LENGTH
+ * and FS2_BIGVGAN_RANGE as fs2_hifigan's (and FS2_BIGVGAN_BAD_START for a window). */
+#define FS2_BIGVGAN_BAD_LENGTH 1
+#define FS2_BIGVGAN_RANGE 2
+#define FS2_BIGVGAN_BAD_START 4
+#define FS2_BIGVGAN_SNAKE 0
+#define FS2_BIGVGAN_SNAKEBETA 1
+/* BigVGAN's config.json fields.  gen: the fields it shares with hifi-gan, accepted as fs2_hifigan_create accepts them
+ * except the widths: every upsample_initial_channel / 2^i a multiple of 8, at most 2048 (a width that is not a multiple of
+ * 32 runs zero-padded to the next one).  activation FS2_BIGVGAN_SNAKE or FS2_BIGVGAN_SNAKEBETA; snake_logscale: the
+ * parameters hold log alpha (and log beta); use_tanh_at_final: tanh, else a clamp to [-1, 1]; use_bias_at_final:
+ * conv_post has a bias. */
+typedef struct fs2_bigvgan_config {
+  fs2_hifigan_config gen;
+  int activation;
+  int snake_logscale;
+  int use_tanh_at_final;
+  int use_bias_at_final;
+} fs2_bigvgan_config;
+typedef struct fs2_bigvgan_gen fs2_bigvgan_gen;
+int fs2_bigvgan_create(fs2_bigvgan_gen** out, int math_mode, const fs2_bigvgan_config* cfg);
+void fs2_bigvgan_destroy(fs2_bigvgan_gen* m);
+/* weights[n], biases[n]: as fs2_hifigan_load's, in BigVGAN's state_dict order (conv_pre, ups.{i}.0, resblocks.{j}.convs1 /
+ * convs2 or convs, conv_post); biases[n - 1] is ignored (may be NULL) without use_bias_at_final.  acts[4 a + 0 .. 3]: the
+ * a-th Activation1d in state_dict order (resblocks.{j}.activations.{i}, then activation_post): alpha [C], beta [C] (NULL
+ * for Snake), upsample.filter [12] and downsample.lowpass.filter [12], device fp32. */
+int fs2_bigvgan_load(fs2_bigvgan_gen* m, const float* const* weights, const float* const* biases, const float* const* acts, void* stream);
+int fs2_bigvgan_workspace_bytes(fs2_bigvgan_gen* m, int B, int Lmax, size_t* bytes);
+int fs2_bigvgan(fs2_bigvgan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
+                size_t ws_bytes, void* stream);
+/* A window of the same audio, as fs2_hifigan_window, on the window plan of the config (DESIGN.md section 18). */
+int fs2_bigvgan_window_workspace_bytes(fs2_bigvgan_gen* m, int B, int n_frames, size_t* bytes);
+int fs2_bigvgan_window(fs2_bigvgan_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax,
+                       int n_frames, float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream);
+/* Single BigVGAN layers on fs2_bigvgan's code paths (per-layer tests), packed into a stream-ordered temporary.  status is
+ * set to 0 or FS2_BIGVGAN_RANGE; utterance b is rows t < lens[b] of Lp, rows past it are never read and written as +0.
+ * fs2_op_bigvgan_act: one Activation1d on x [B*Lp][C] (C a multiple of 8, padded to 32 as the vocoder pads it), its four
+ *   tensors as in fs2_bigvgan_load, into out [B*Lp][C]: the GEMM operand of math_mode read back as fp32 ((hi + lo) / 16 in
+ *   the plane modes).
+ * fs2_op_bigvgan_resblock: one AMP block (type 1 or 2) on rows [B*Lp][C] (C a multiple of 32), as fs2_op_hifigan_resblock,
+ *   with acts[4 i + 0 .. 3] its activations in state_dict order. */
+int fs2_op_bigvgan_act(int math_mode, int C, const float* x, const int64_t* lens, int B, int Lp, const float* const* tensors, int snakebeta,
+                       int logscale, float* out, int* status, void* stream);
+int fs2_op_bigvgan_resblock(int math_mode, int type, int C, int k, int nd, const int* dils, const float* x, const int64_t* lens, int B,
+                            int Lp, const float* const* weights, const float* const* biases, const float* const* acts, int snakebeta,
+                            int logscale, float* out, int* status, void* stream);
+
 /* ---- batched WaveGlow vocoder (DESIGN.md section 9) ----------------------------------------------------------------- */
 /* DeepLearningExamples' WaveGlow (n_mel_channels 80, n_flows 12, n_group 8, n_early_every 4, n_early_size 2, WN: 8 layers,
  * kernel 3, n_channels C) in its inverse direction, `infer`, on log-mels [B, Lmax, 80] with frame counts olens [B]:
