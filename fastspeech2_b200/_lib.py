@@ -57,6 +57,7 @@ FS2_HIFIGAN_BAD_START = 4                            # and of fs2_hifigan_window
 FS2_HIFIGAN_MAX_UPSAMPLES, FS2_HIFIGAN_MAX_KERNELS = 8, 8
 FS2_BIGVGAN_BAD_LENGTH, FS2_BIGVGAN_RANGE, FS2_BIGVGAN_BAD_START = 1, 2, 4   # bits of fs2_bigvgan's / fs2_bigvgan_window's status word
 FS2_BIGVGAN_SNAKE, FS2_BIGVGAN_SNAKEBETA = 0, 1
+FS2_ISTFTNET_BAD_LENGTH, FS2_ISTFTNET_RANGE, FS2_ISTFTNET_BAD_START = 1, 2, 4   # bits of fs2_istftnet's / fs2_istftnet_window's status word
 
 
 class HiFiGANConfig(C.Structure):
@@ -71,6 +72,10 @@ class HiFiGANConfig(C.Structure):
 class BigVGANConfig(C.Structure):
     _fields_ = [("gen", HiFiGANConfig), ("activation", C.c_int32), ("snake_logscale", C.c_int32), ("use_tanh_at_final", C.c_int32),
                 ("use_bias_at_final", C.c_int32)]
+
+
+class ISTFTNetConfig(C.Structure):
+    _fields_ = [("gen", HiFiGANConfig), ("istft_n_fft", C.c_int32), ("istft_hop", C.c_int32)]
 
 
 class NoamAdamHp(C.Structure):
@@ -178,6 +183,13 @@ SIGNATURES = {
     "fs2_op_bigvgan_act": [_I, _I, _P, _P, _I, _I, C.POINTER(_P), _I, _I, _P, _P, _P],
     "fs2_op_bigvgan_resblock": [_I, _I, _I, _I, _I, C.POINTER(_I), _P, _P, _I, _I, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), _I, _I, _P,
                                 _P, _P],
+    "fs2_istftnet_create": [C.POINTER(_P), _I, C.POINTER(ISTFTNetConfig)],
+    "fs2_istftnet_load": [_P, C.POINTER(_P), C.POINTER(_P), _P],
+    "fs2_istftnet_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_istftnet": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_istftnet_window_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_istftnet_window": [_P, _P, _P, _P, _I, _I, _I, _P, _L, _P, _P, _SZ, _P],
+    "fs2_op_istftnet_head": [_I, _I, _I, _P, _P, _I, _I, _P, _P, _P, _P],
     "fs2_waveglow_create": [C.POINTER(_P), _I, _I],
     "fs2_waveglow_load": [_P, C.POINTER(_P), _I, _P],
     "fs2_waveglow_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
@@ -199,7 +211,7 @@ SIGNATURES = {
 }
 OTHER_SYMBOLS = ("fs2_last_error", "fs2_version", "fs2_destroy", "fs2_kernel_launches", "fs2_profile_label", "fs2_vocoder_destroy",
                  "fs2_melgan_destroy", "fs2_waveglow_destroy", "fs2_features_destroy", "fs2_hifigan_destroy",
-                 "fs2_bigvgan_destroy")
+                 "fs2_bigvgan_destroy", "fs2_istftnet_destroy")
 ALL_SYMBOLS = tuple(SIGNATURES) + OTHER_SYMBOLS
 
 _lib: Optional[C.CDLL] = None
@@ -241,6 +253,8 @@ def load() -> C.CDLL:
     lib.fs2_hifigan_destroy.argtypes = [_P]
     lib.fs2_bigvgan_destroy.restype = None
     lib.fs2_bigvgan_destroy.argtypes = [_P]
+    lib.fs2_istftnet_destroy.restype = None
+    lib.fs2_istftnet_destroy.argtypes = [_P]
     _lib = lib
     return lib
 

@@ -42,11 +42,16 @@
 // utterance edge.  A window descriptor [start | len | n] x B per buffer (nullptr = the whole utterance: start 0, len = n =
 // lens[b]) maps local rows to global ones, and producers range-check only rows whose values equal the whole call's
 // (exact_row).
+//
+// iSTFTNet (DESIGN.md section 19) is this generator with another head: the same kernels up to the last MRF, then
+// istftnet_head (istftnet.cu) in place of the post kernel, at a last level of 256 / istft_hop rows per frame.  The tables
+// below take the head's hop (1 for HiFi-GAN) and its reach in last-level rows.
 #include <math.h>
 
 #include <algorithm>
 #include <vector>
 
+#include "istftnet.cuh"
 #include "vocoder_weights.cuh"
 #include "vocoder_window.cuh"
 
@@ -184,7 +189,8 @@ struct Shape {
   long act;                            // floats per frame of the largest stage buffer, max_s up_s * C_s
 };
 
-Shape shape_of(const fs2_hifigan_config& c) {
+// n_fft: 0 for HiFi-GAN's post, else iSTFTNet's head of that n_fft and hop
+Shape shape_of(const fs2_hifigan_config& c, int n_fft = 0, int hop = 1) {
   Shape s;
   s.U = c.num_upsamples; s.nk = c.num_kernels; s.type = c.resblock;
   s.steps = s.type == 1 ? 3 : 2; s.per = s.type == 1 ? 6 : 2;
@@ -194,8 +200,9 @@ Shape shape_of(const fs2_hifigan_config& c) {
     for (int m = 0; m < s.steps; ++m) r += (c.resblock_kernel_sizes[j] - 1) / 2 * (c.resblock_dilation_sizes[j][m] + (s.type == 1));
     R = std::max(R, r);
   }
-  // the window plan: conv_pre's native taps leave its outer 3 rows wrong at a side that is not an utterance edge; no tail
-  s.ups = ups_plan(s.U, c.upsample_rates, R, kPreTaps / 2, kPostTaps / 2, 0);
+  // the window plan: conv_pre's native taps leave its outer 3 rows wrong at a side that is not an utterance edge; the head
+  // reads 3 rows (conv_post) or istft_reach rows on each side; no tail
+  s.ups = ups_plan(s.U, c.upsample_rates, R, kPreTaps / 2, n_fft ? istft_reach(n_fft, hop) : kPostTaps / 2, 0);
   s.C[0] = c.upsample_initial_channel;
   s.act = s.C[0];
   for (int i = 0; i < s.U; ++i) {
@@ -206,8 +213,8 @@ Shape shape_of(const fs2_hifigan_config& c) {
   return s;
 }
 
-int validate(const fs2_hifigan_config* c) {
-  const char* who = "fs2_hifigan_create";
+// hop: the head's (1 for HiFi-GAN), so that the rates' product times hop is the frame hop 256
+int validate(const fs2_hifigan_config* c, const char* who, int hop) {
   FS2_REQUIRE(c->resblock == 1 || c->resblock == 2, "%s: resblock must be 1 or 2 (got %d)", who, c->resblock);
   FS2_REQUIRE(c->num_upsamples >= 1 && c->num_upsamples <= kMaxUps, "%s: num_upsamples must lie in [1, %d] (got %d)", who, kMaxUps,
               c->num_upsamples);
@@ -219,7 +226,9 @@ int validate(const fs2_hifigan_config* c) {
                 c->upsample_kernel_sizes[i], u);
     prod *= u;
   }
-  FS2_REQUIRE(prod == kHop, "%s: the product of upsample_rates is %ld, not the hop 256", who, prod);
+  if (hop == 1) FS2_REQUIRE(prod == kHop, "%s: the product of upsample_rates is %ld, not the hop 256", who, prod);
+  else FS2_REQUIRE(prod * hop == kHop, "%s: the product of upsample_rates (%ld) times istft_hop (%d) is %ld, not the hop 256", who, prod, hop,
+                   prod * hop);
   const int C0 = c->upsample_initial_channel;
   FS2_REQUIRE(C0 >= 32 && C0 <= 2048 && C0 % (32 << c->num_upsamples) == 0,
               "%s: upsample_initial_channel = %d must lie in [32, 2048] with every width C0 / 2^i a multiple of 32", who, C0);
@@ -317,9 +326,13 @@ HgPlan window_plan(Bump& b, const Shape& sh, int B, int nf) {
 // a GEMM weight here is [taps][N][K] tap matrices with K = Cin, so vweight_pack_conv packs it at tap_stride = N K
 void set_conv(VWeight& w, int N, int K, int taps) { w.N = N; w.K = K; w.taps = taps; }
 
-int check_size(int math_mode, int B, int L) {
-  FS2_REQUIRE(B >= 1 && L >= 1, "fs2_hifigan: need B >= 1 and Lmax >= 1 (got %d, %d)", B, L);
-  return check_rows("fs2_hifigan", "B * Lmax * 256", "sample", (long)B * L * kHop, math_mode);
+// the whole call's limits on its largest GEMM, B * Lmax * up_U rows (HiFi-GAN: samples)
+int check_size(const char* who, const Shape& sh, int math_mode, int B, int L) {
+  FS2_REQUIRE(B >= 1 && L >= 1, "%s: need B >= 1 and Lmax >= 1 (got %d, %d)", who, B, L);
+  const int up = sh.ups.up[sh.U];
+  char formula[32];
+  snprintf(formula, sizeof formula, "B * Lmax * %d", up);
+  return check_rows(who, formula, up == kHop ? "sample" : "row", (long)B * L * up, math_mode);
 }
 
 }  // namespace
@@ -333,9 +346,12 @@ struct fs2_hifigan_gen {
   void* arena = nullptr; size_t arena_bytes = 0;
   fs2::VWeight pre, up[fs2::kMaxUps];
   std::vector<fs2::VWeight> blk;   // [U * nk][per]: the resblocks' convolutions in state_dict order
-  float* post_w = nullptr;         // [7][C_U]
-  float* post_b = nullptr;
+  float* post_w = nullptr;         // [7][C_U], iSTFTNet: [7][n_fft + 2][C_U]
+  float* post_b = nullptr;         // [1], iSTFTNet: [n_fft + 2]
+  int n_fft = 0, head_hop = 1;     // the head: 0, 1 for HiFi-GAN's post; iSTFTNet's istft_n_fft, istft_hop
 };
+
+struct fs2_istftnet_gen : fs2_hifigan_gen {};
 
 namespace fs2 {
 namespace {
@@ -388,31 +404,29 @@ int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const
     nk_in = sh.nk;
   }
   const int Lout = (w ? nf : L) * kHop, C = sh.C[U];
+  if (m->n_fft)
+    return istftnet_head(x, r, nk_in, lens(win_level(U), U), desc(win_level(U)), desc(win_audio(sh.ups)), B, rows(U), Lout, ld, C, m->n_fft,
+                         m->head_hop, m->post_w, m->post_b, audio, st);
   hifigan_post_kernel<<<grid_for((long)B * Lout, 256), 256, kPostTaps * C * sizeof(float), st>>>(
       x, r, nk_in, lens(win_level(U), U), desc(win_level(U)), desc(win_audio(sh.ups)), B, rows(U), Lout, ld, C, m->post_w, m->post_b, audio);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
 
-}  // namespace
-}  // namespace fs2
-
-using namespace fs2;
-
-extern "C" {
-
-int fs2_hifigan_create(fs2_hifigan_gen** out, int math_mode, const fs2_hifigan_config* cfg) {
-  FS2_REQUIRE(out && cfg, "fs2_hifigan_create: null argument");
-  FS2_REQUIRE(math_mode >= FS2_MATH_FP32 && math_mode <= FS2_MATH_F16, "fs2_hifigan_create: bad math_mode %d", math_mode);
-  int rc = validate(cfg);
+// The entries of both generators, on m's head; name: "fs2_hifigan" or "fs2_istftnet", the prefix of every message.
+template <typename Gen>
+int create_gen(Gen** out, int math_mode, const fs2_hifigan_config* cfg, int n_fft, int hop, const char* who) {
+  int rc = validate(cfg, who, hop);
   if (rc) return rc;
   int dev = 0;
   FS2_CUDA_CHECK(cudaGetDevice(&dev));
-  fs2_hifigan_gen* m = new fs2_hifigan_gen();
+  Gen* m = new Gen();
   m->math_mode = math_mode;
   m->device = dev;
   m->cfg = *cfg;
-  m->sh = shape_of(*cfg);
+  m->n_fft = n_fft;
+  m->head_hop = hop;
+  m->sh = shape_of(*cfg, n_fft, hop);
   const Shape& sh = m->sh;
   set_conv(m->pre, sh.C[0], kMels, kPreTaps);
   for (int s = 0; s < sh.U; ++s) set_conv(m->up[s], cfg->upsample_rates[s] * sh.C[s + 1], sh.C[s], 3);
@@ -424,24 +438,19 @@ int fs2_hifigan_create(fs2_hifigan_gen** out, int math_mode, const fs2_hifigan_c
   return FS2_OK;
 }
 
-void fs2_hifigan_destroy(fs2_hifigan_gen* m) {
-  if (!m) return;
-  if (m->arena) cudaFree(m->arena);
-  delete m;
-}
-
-int fs2_hifigan_load(fs2_hifigan_gen* m, const float* const* weights, const float* const* biases, void* stream) {
-  FS2_REQUIRE(m && weights && biases, "fs2_hifigan_load: null argument");
+int load_gen(fs2_hifigan_gen* m, const float* const* weights, const float* const* biases, void* stream, const char* name) {
+  FS2_REQUIRE(m && weights && biases, "%s_load: null argument", name);
   const Shape& sh = m->sh;
-  for (int i = 0; i < sh.layers; ++i) FS2_REQUIRE(weights[i] && biases[i], "fs2_hifigan_load: layer %d: null tensor", i);
+  for (int i = 0; i < sh.layers; ++i) FS2_REQUIRE(weights[i] && biases[i], "%s_load: layer %d: null tensor", name, i);
   cudaStream_t st = (cudaStream_t)stream;
+  const int O = m->n_fft ? m->n_fft + 2 : 1;   // conv_post's output channels
   m->loaded = false;
   int rc = arena_carve(&m->arena, &m->arena_bytes, st, [&](Bump& b) {
     vweight_carve(b, m->pre, true);
     for (int s = 0; s < sh.U; ++s) vweight_carve(b, m->up[s], true);
     for (auto& w : m->blk) vweight_carve(b, w, true);
-    m->post_w = b.floats((size_t)kPostTaps * sh.C[sh.U]);
-    m->post_b = b.floats(1);
+    m->post_w = b.floats((size_t)kPostTaps * O * sh.C[sh.U]);
+    m->post_b = b.floats(O);
     return FS2_OK;
   });
   if (rc) return rc;
@@ -455,15 +464,15 @@ int fs2_hifigan_load(fs2_hifigan_gen* m, const float* const* weights, const floa
     if ((rc = vweight_pack_conv(w, weights[1 + sh.U + i], biases[1 + sh.U + i], w.K, w.N, w.taps, 0, (long)w.N * w.K, st))) return rc;
   }
   const int C = sh.C[sh.U], last = sh.layers - 1;
-  if ((rc = conv_pack(weights[last], 1, C, kPostTaps, 1, 0, C, C, m->post_w, st))) return rc;
-  FS2_CUDA_CHECK(cudaMemcpyAsync(m->post_b, biases[last], sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if ((rc = conv_pack(weights[last], O, C, kPostTaps, O, 0, (long)O * C, C, m->post_w, st))) return rc;
+  FS2_CUDA_CHECK(cudaMemcpyAsync(m->post_b, biases[last], O * sizeof(float), cudaMemcpyDeviceToDevice, st));
   m->loaded = true;
   return FS2_OK;
 }
 
-int fs2_hifigan_workspace_bytes(fs2_hifigan_gen* m, int B, int Lmax, size_t* bytes) {
-  FS2_REQUIRE(m && bytes, "fs2_hifigan_workspace_bytes: null argument");
-  int rc = check_size(m->math_mode, B, Lmax);
+int workspace_gen(fs2_hifigan_gen* m, int B, int Lmax, size_t* bytes, const char* name) {
+  FS2_REQUIRE(m && bytes, "%s_workspace_bytes: null argument", name);
+  int rc = check_size(name, m->sh, m->math_mode, B, Lmax);
   if (rc) return rc;
   Bump b(nullptr, 0);
   plan(b, m->sh, B, Lmax);
@@ -471,22 +480,24 @@ int fs2_hifigan_workspace_bytes(fs2_hifigan_gen* m, int B, int Lmax, size_t* byt
   return FS2_OK;
 }
 
-int fs2_hifigan(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
-                size_t ws_bytes, void* stream) {
-  FS2_REQUIRE(m && mels && olens && audio && status && ws, "fs2_hifigan: null argument");
-  FS2_REQUIRE(m->loaded, "fs2_hifigan: weights not loaded (fs2_hifigan_load)");
-  FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "fs2_hifigan: mels must be 16-byte aligned");
-  int rc = check_size(m->math_mode, B, Lmax);
+int call_gen(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
+             size_t ws_bytes, void* stream, const char* name) {
+  FS2_REQUIRE(m && mels && olens && audio && status && ws, "%s: null argument", name);
+  FS2_REQUIRE(m->loaded, "%s: weights not loaded (%s_load)", name, name);
+  FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "%s: mels must be 16-byte aligned", name);
+  int rc = check_size(name, m->sh, m->math_mode, B, Lmax);
   if (rc) return rc;
   Bump b(ws, ws_bytes);
   HgPlan p = plan(b, m->sh, B, Lmax);
-  if ((rc = b.check("fs2_hifigan"))) return rc;
+  if ((rc = b.check(name))) return rc;
   return generate(m, p, mels, olens, nullptr, B, Lmax, 0, audio, (long)Lmax * kHop, status, (cudaStream_t)stream);
 }
 
-int fs2_hifigan_window_workspace_bytes(fs2_hifigan_gen* m, int B, int n_frames, size_t* bytes) {
-  FS2_REQUIRE(m && bytes, "fs2_hifigan_window_workspace_bytes: null argument");
-  int rc = check_window_rows("fs2_hifigan_window", m->sh.ups, B, n_frames, m->math_mode);
+int window_workspace_gen(fs2_hifigan_gen* m, int B, int n_frames, size_t* bytes, const char* name) {
+  char who[48];
+  snprintf(who, sizeof who, "%s_window", name);
+  FS2_REQUIRE(m && bytes, "%s_workspace_bytes: null argument", who);
+  int rc = check_window_rows(who, m->sh.ups, B, n_frames, m->math_mode);
   if (rc) return rc;
   Bump b(nullptr, 0);
   window_plan(b, m->sh, B, n_frames);
@@ -494,18 +505,106 @@ int fs2_hifigan_window_workspace_bytes(fs2_hifigan_gen* m, int B, int n_frames, 
   return FS2_OK;
 }
 
-int fs2_hifigan_window(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax, int n_frames,
-                       float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream) {
-  FS2_REQUIRE(m && mels && olens && starts && audio && status && ws, "fs2_hifigan_window: null argument");
-  FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "fs2_hifigan_window: mels must be 16-byte aligned");
-  int rc = check_window_rows("fs2_hifigan_window", m->sh.ups, B, n_frames, m->math_mode);
+int window_gen(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax, int n_frames,
+               float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream, const char* name) {
+  char who[48];
+  snprintf(who, sizeof who, "%s_window", name);
+  FS2_REQUIRE(m && mels && olens && starts && audio && status && ws, "%s: null argument", who);
+  FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "%s: mels must be 16-byte aligned", who);
+  int rc = check_window_rows(who, m->sh.ups, B, n_frames, m->math_mode);
   if (rc) return rc;
-  if ((rc = check_window_extent("fs2_hifigan_window", Lmax, 0, kHop, n_frames, audio_ld))) return rc;
+  if ((rc = check_window_extent(who, Lmax, 0, kHop, n_frames, audio_ld))) return rc;
   Bump b(ws, ws_bytes);
   HgPlan p = window_plan(b, m->sh, B, n_frames);
-  if ((rc = b.check("fs2_hifigan_window"))) return rc;
-  FS2_REQUIRE(m->loaded, "fs2_hifigan_window: weights not loaded (fs2_hifigan_load)");
+  if ((rc = b.check(who))) return rc;
+  FS2_REQUIRE(m->loaded, "%s: weights not loaded (%s_load)", who, name);
   return generate(m, p, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, (cudaStream_t)stream);
+}
+
+static_assert(FS2_ISTFTNET_BAD_LENGTH == FS2_HIFIGAN_BAD_LENGTH && FS2_ISTFTNET_RANGE == FS2_HIFIGAN_RANGE &&
+                  FS2_ISTFTNET_BAD_START == FS2_HIFIGAN_BAD_START,
+              "iSTFTNet runs HiFi-GAN's kernels, which set HiFi-GAN's status bits");
+
+}  // namespace
+}  // namespace fs2
+
+using namespace fs2;
+
+extern "C" {
+
+int fs2_hifigan_create(fs2_hifigan_gen** out, int math_mode, const fs2_hifigan_config* cfg) {
+  FS2_REQUIRE(out && cfg, "fs2_hifigan_create: null argument");
+  FS2_REQUIRE(math_mode >= FS2_MATH_FP32 && math_mode <= FS2_MATH_F16, "fs2_hifigan_create: bad math_mode %d", math_mode);
+  return create_gen(out, math_mode, cfg, 0, 1, "fs2_hifigan_create");
+}
+
+void fs2_hifigan_destroy(fs2_hifigan_gen* m) {
+  if (!m) return;
+  if (m->arena) cudaFree(m->arena);
+  delete m;
+}
+
+int fs2_hifigan_load(fs2_hifigan_gen* m, const float* const* weights, const float* const* biases, void* stream) {
+  return load_gen(m, weights, biases, stream, "fs2_hifigan");
+}
+
+int fs2_hifigan_workspace_bytes(fs2_hifigan_gen* m, int B, int Lmax, size_t* bytes) {
+  return workspace_gen(m, B, Lmax, bytes, "fs2_hifigan");
+}
+
+int fs2_hifigan(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
+                size_t ws_bytes, void* stream) {
+  return call_gen(m, mels, olens, B, Lmax, audio, status, ws, ws_bytes, stream, "fs2_hifigan");
+}
+
+int fs2_hifigan_window_workspace_bytes(fs2_hifigan_gen* m, int B, int n_frames, size_t* bytes) {
+  return window_workspace_gen(m, B, n_frames, bytes, "fs2_hifigan");
+}
+
+int fs2_hifigan_window(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax, int n_frames,
+                       float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream) {
+  return window_gen(m, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws, ws_bytes, stream, "fs2_hifigan");
+}
+
+int fs2_istftnet_create(fs2_istftnet_gen** out, int math_mode, const fs2_istftnet_config* cfg) {
+  const char* who = "fs2_istftnet_create";
+  FS2_REQUIRE(out && cfg, "%s: null argument", who);
+  FS2_REQUIRE(math_mode >= FS2_MATH_FP32 && math_mode <= FS2_MATH_F16, "%s: bad math_mode %d", who, math_mode);
+  const int n = cfg->istft_n_fft, hop = cfg->istft_hop;
+  FS2_REQUIRE(n >= 2 && n % 2 == 0, "%s: istft_n_fft = %d must be even and at least 2", who, n);
+  FS2_REQUIRE(n <= kIstftMaxNfft, "%s: istft_n_fft = %d is above %d, the most the head kernel's shared memory holds", who, n, kIstftMaxNfft);
+  FS2_REQUIRE(hop >= 1 && n % hop == 0 && n / hop >= 2,
+              "%s: istft_hop = %d must divide istft_n_fft = %d with istft_n_fft / istft_hop >= 2 (else the window envelope is 0)", who,
+              hop, n);
+  return create_gen(out, math_mode, &cfg->gen, n, hop, who);
+}
+
+void fs2_istftnet_destroy(fs2_istftnet_gen* m) {
+  if (!m) return;
+  if (m->arena) cudaFree(m->arena);
+  delete m;
+}
+
+int fs2_istftnet_load(fs2_istftnet_gen* m, const float* const* weights, const float* const* biases, void* stream) {
+  return load_gen(m, weights, biases, stream, "fs2_istftnet");
+}
+
+int fs2_istftnet_workspace_bytes(fs2_istftnet_gen* m, int B, int Lmax, size_t* bytes) {
+  return workspace_gen(m, B, Lmax, bytes, "fs2_istftnet");
+}
+
+int fs2_istftnet(fs2_istftnet_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
+                 size_t ws_bytes, void* stream) {
+  return call_gen(m, mels, olens, B, Lmax, audio, status, ws, ws_bytes, stream, "fs2_istftnet");
+}
+
+int fs2_istftnet_window_workspace_bytes(fs2_istftnet_gen* m, int B, int n_frames, size_t* bytes) {
+  return window_workspace_gen(m, B, n_frames, bytes, "fs2_istftnet");
+}
+
+int fs2_istftnet_window(fs2_istftnet_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax, int n_frames,
+                        float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream) {
+  return window_gen(m, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws, ws_bytes, stream, "fs2_istftnet");
 }
 
 // ---- single layers on the vocoder's own code paths (tests) ----------------------------------------------------------

@@ -75,8 +75,10 @@ def check_config(cfg: dict) -> None:
     check_resblocks(cfg)
 
 
-def check_rates(cfg: dict) -> None:
-    """check_config's rules before the widths: num_mels, the resblock type, the upsample rates and kernel sizes."""
+def check_rates(cfg: dict, head_hop: int = 1) -> None:
+    """check_config's rules before the widths: num_mels, the resblock type, the upsample rates and kernel sizes.
+    head_hop: the samples per last-level row of the head (iSTFTNet's gen_istft_hop_size), which the rates' product times
+    must give the hop 256."""
     if cfg.get("num_mels", N_MELS) != N_MELS:
         raise ValueError(f"config: num_mels must be {N_MELS} (got {cfg['num_mels']})")
     if cfg["resblock"] not in ("1", "2"):
@@ -88,8 +90,11 @@ def check_rates(cfg: dict) -> None:
         raise ValueError(f"config: upsample_rates must hold 1 to {_lib.FS2_HIFIGAN_MAX_UPSAMPLES} rates")
     if any(u < 2 or u % 2 for u in rates):
         raise ValueError(f"config: upsample_rates must be even (got {rates})")
-    if math.prod(rates) != HOP:
+    if head_hop == 1 and math.prod(rates) != HOP:
         raise ValueError(f"config: the product of upsample_rates must be the hop {HOP} (got {math.prod(rates)})")
+    if math.prod(rates) * head_hop != HOP:
+        raise ValueError(f"config: the product of upsample_rates times gen_istft_hop_size must be the hop {HOP} "
+                         f"(got {math.prod(rates)} * {head_hop})")
     if len(ks) != len(rates) or any(k != 2 * u for k, u in zip(ks, rates)):
         raise ValueError(f"config: upsample_kernel_sizes must be twice the upsample_rates (got {ks} for {rates})")
 
@@ -149,16 +154,16 @@ class _ResBlock2(nn.Module):
         self.convs = nn.ModuleList([_WNConv(c, c, k) for _ in range(2)])
 
 
-def add_layers(module: nn.Module, cfg: dict) -> nn.Module:
+def add_layers(module: nn.Module, cfg: dict, post_channels: int = 1) -> nn.Module:
     """Registers the generator's parameter holders on module, in hifi-gan's order, so that its state_dict keys are the
-    checkpoint's: conv_pre, ups, resblocks, conv_post.  No check of the config beyond its shapes (the key lists of
-    configs the kernels refuse, such as V2, come from here too)."""
+    checkpoint's: conv_pre, ups, resblocks, conv_post (post_channels outputs: 1, or iSTFTNet's n_fft + 2).  No check of
+    the config beyond its shapes (the key lists of configs the kernels refuse, such as V2, come from here too)."""
     rates, ks, c0 = cfg["upsample_rates"], cfg["upsample_kernel_sizes"], cfg["upsample_initial_channel"]
     block = _ResBlock1 if str(cfg["resblock"]) == "1" else _ResBlock2
     module.conv_pre = _WNConv(N_MELS, c0, 7)
     module.ups = nn.ModuleList([_WNConv(c0 // 2 ** i, c0 // 2 ** (i + 1), k, transposed=True) for i, k in enumerate(ks)])
     module.resblocks = nn.ModuleList([block(c0 // 2 ** (i + 1), k) for i in range(len(rates)) for k in cfg["resblock_kernel_sizes"]])
-    module.conv_post = _WNConv(c0 // 2 ** len(rates), 1, 7)
+    module.conv_post = _WNConv(c0 // 2 ** len(rates), post_channels, 7)
     return module
 
 

@@ -643,6 +643,47 @@ int fs2_op_bigvgan_resblock(int math_mode, int type, int C, int k, int nd, const
                             int Lp, const float* const* weights, const float* const* biases, const float* const* acts, int snakebeta,
                             int logscale, float* out, int* status, void* stream);
 
+/* ---- batched iSTFTNet vocoder (DESIGN.md section 19) ---------------------------------------------------------------- */
+/* rishikksh20/iSTFTNet-pytorch's Generator on log-mels [B, Lmax, 80] with frame counts olens [B], with the call surface of
+ * fs2_hifigan: hifi-gan's generator up to its last MRF (the same kernels), then an inverse-STFT head in place of
+ * conv_post + tanh: y = conv_post(ReflectionPad1d((1, 0))(lrelu(x, 0.01))) with n_fft + 2 channels, and
+ * audio = istft(exp(y[:n_fft/2+1]) * exp(i sin(y[n_fft/2+1:])), n_fft, hop, periodic Hann, center=True).  Utterance b is
+ * the generator applied to mels[b, :olens[b]] alone, olens[b] * 256 samples, bit-identical to a B = 1 call, +0 past them;
+ * mel frames past olens[b] are never read.  The head runs on CUDA cores in fp32 in every math mode.  No allocation, no
+ * synchronisation.  It enqueues 4 + U * (2 + K * G + max(K - 2, 0)) kernels, as fs2_hifigan: 82 for C8C8I.  *status:
+ * FS2_ISTFTNET_BAD_LENGTH and FS2_ISTFTNET_RANGE as fs2_hifigan's (and FS2_ISTFTNET_BAD_START for a window). */
+#define FS2_ISTFTNET_BAD_LENGTH 1
+#define FS2_ISTFTNET_RANGE 2
+#define FS2_ISTFTNET_BAD_START 4
+/* iSTFTNet's config.json fields.  gen: hifi-gan's, accepted as fs2_hifigan_create accepts them except that the product
+ * of the upsample rates times istft_hop must be 256.  istft_n_fft even, at most 16 (the head kernel's shared memory);
+ * istft_hop divides it with istft_n_fft / istft_hop >= 2 (the window envelope is 0 somewhere otherwise). */
+typedef struct fs2_istftnet_config {
+  fs2_hifigan_config gen;
+  int istft_n_fft;
+  int istft_hop;
+} fs2_istftnet_config;
+typedef struct fs2_istftnet_gen fs2_istftnet_gen;
+int fs2_istftnet_create(fs2_istftnet_gen** out, int math_mode, const fs2_istftnet_config* cfg);
+void fs2_istftnet_destroy(fs2_istftnet_gen* m);
+/* weights / biases as fs2_hifigan_load's, conv_post [n_fft + 2, C_U, 7] with its bias [n_fft + 2] */
+int fs2_istftnet_load(fs2_istftnet_gen* m, const float* const* weights, const float* const* biases, void* stream);
+/* fails (FS2_ERR_INVALID) when B * Lmax * (256 / istft_hop) (the last level's rows) reaches 2^31, or exceeds 65535 * 128
+ * in FS2_MATH_FP32 */
+int fs2_istftnet_workspace_bytes(fs2_istftnet_gen* m, int B, int Lmax, size_t* bytes);
+int fs2_istftnet(fs2_istftnet_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
+                 size_t ws_bytes, void* stream);
+/* A window of the same audio, as fs2_hifigan_window, on the window plan of the config with the head's reach
+ * (4 + (n_fft / 2 - 1) / hop last-level rows: 5 for C8C8I). */
+int fs2_istftnet_window_workspace_bytes(fs2_istftnet_gen* m, int B, int n_frames, size_t* bytes);
+int fs2_istftnet_window(fs2_istftnet_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax,
+                        int n_frames, float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream);
+/* The head alone on fs2_istftnet's code path (per-layer tests): x [B*Lp][C] the last MRF's output (C a multiple of 32),
+ * utterance b its rows t < lens[b] (lens[b] in [0, Lp]; a reflected row past lens[b] is 0), conv_post w [n_fft + 2][C][7]
+ * and b [n_fft + 2] (device, torch's layout), into audio [B][Lp * hop]: hop * lens[b] samples, +0 past them. */
+int fs2_op_istftnet_head(int C, int n_fft, int hop, const float* x, const int64_t* lens, int B, int Lp, const float* w, const float* b,
+                         float* audio, void* stream);
+
 /* ---- batched WaveGlow vocoder (DESIGN.md section 9) ----------------------------------------------------------------- */
 /* DeepLearningExamples' WaveGlow (n_mel_channels 80, n_flows 12, n_group 8, n_early_every 4, n_early_size 2, WN: 8 layers,
  * kernel 3, n_channels C) in its inverse direction, `infer`, on log-mels [B, Lmax, 80] with frame counts olens [B]:
