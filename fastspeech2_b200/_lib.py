@@ -58,6 +58,7 @@ FS2_HIFIGAN_MAX_UPSAMPLES, FS2_HIFIGAN_MAX_KERNELS = 8, 8
 FS2_BIGVGAN_BAD_LENGTH, FS2_BIGVGAN_RANGE, FS2_BIGVGAN_BAD_START = 1, 2, 4   # bits of fs2_bigvgan's / fs2_bigvgan_window's status word
 FS2_BIGVGAN_SNAKE, FS2_BIGVGAN_SNAKEBETA = 0, 1
 FS2_ISTFTNET_BAD_LENGTH, FS2_ISTFTNET_RANGE, FS2_ISTFTNET_BAD_START = 1, 2, 4   # bits of fs2_istftnet's / fs2_istftnet_window's status word
+FS2_EVAL_BAD_LENGTH, FS2_EVAL_NONFINITE = 1, 2   # bits of fs2_mcd_dtw's / fs2_path_prosody's status word
 
 
 class HiFiGANConfig(C.Structure):
@@ -158,6 +159,9 @@ SIGNATURES = {
     "fs2_features_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
     "fs2_mel_energy": [_P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _P],
     "fs2_dio": [_P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _P],
+    "fs2_dtw_workspace_bytes": [_I, _I, _I, _I, _I, _I, C.POINTER(_SZ)],
+    "fs2_mcd_dtw": [_P, _P, _I, _P, _P, _I, _I, _I, _P, _I, C.c_double, _P, _P, _P, _P, _P, _P, _SZ, _P],
+    "fs2_path_prosody": [_P, _P, _I, _I, _P, _P, _I, _P, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P],
     "fs2_melgan_create": [C.POINTER(_P), _I],
     "fs2_melgan_load": [_P, C.POINTER(_P), C.POINTER(_P), _P],
     "fs2_melgan_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],

@@ -463,6 +463,43 @@ int fs2_mel_energy(fs2_features* f, const float* wav, const int64_t* lens, int B
 int fs2_dio(fs2_features* f, const float* wav, const int64_t* lens, int B, int Nmax, double* f0, int64_t* plens, int* status,
             void* ws, size_t ws_bytes, void* stream);
 
+/* ---- objective evaluation: MCD under DTW, and F0, voicing and energy errors along its path (DESIGN.md section 20) ---- */
+/* Synthesized log-mels x [B, Lx_max, n_mels] fp32 with xlens [B], reference log-mels y [B, Ly_max, n_mels] with ylens [B]
+ * (the layout fs2_mel_energy writes); rows at or past a length are never read.  Pair b (Lx = xlens[b], Ly = ylens[b]):
+ *   c[t, k]  = sum_{m < n_mels} double(mel[t, m]) * dct[m, k - 1], k = 1..n_cep   (dct: the orthonormal DCT-II basis
+ *              without c0, float64 [n_mels, n_cep], built by the caller)
+ *   d(i, j)  = sqrt(sum_k (cx[i, k] - cy[j, k])^2)
+ *   A(0, 0)  = d(0, 0), A(i, j) = d(i, j) + min over (i-1, j-1), (i-1, j), (i, j-1) that exist, in that order, the first
+ *              minimum winning; no band
+ *   cost[b]  = A(Lx - 1, Ly - 1), plen[b] = P the number of cells on the chosen path, mcd[b] = cost / P * scale
+ *              (scale = 10 sqrt(2) / ln 10 for dB)
+ *   path     NULL, or int32 [B, Lx_max + Ly_max - 1, 2]: the path's (i, j) from (0, 0), -1 past plen[b]
+ * Sums run over increasing m / k with every product and sum rounded (no FMA contraction): float64 restatements with the
+ * same order match bit for bit, and pair b is bit-identical to a B = 1 call.  4 kernels (and a memset) with a path, 3
+ * without; no allocation, no synchronisation.  Data-dependent checks are reported in *status (device int, zeroed):
+ *   FS2_EVAL_BAD_LENGTH  some xlens[b] / ylens[b] outside [1, L_max]; that pair's mcd and cost are NaN, plen 0, path -1;
+ *   FS2_EVAL_NONFINITE   a non-finite log-mel inside a valid region.
+ * Workspace (fs2_dtw_workspace_bytes), with W = min(Lx_max, Ly_max) and every term rounded up to 256 bytes, plus 256:
+ *   8 B (Lx_max + Ly_max) n_cep  +  (W > 1024 ? 36 B W : 0)  +  (with_path ? B (Lx_max + Ly_max - 1) W : 0)
+ * so without a path it grows with Lx_max + Ly_max, not with their product.
+ *
+ * fs2_path_prosody walks each path[b, :plen[b]] ([B, P_max, 2], as fs2_mcd_dtw writes it) in order, with
+ * fx = f0x[b, i] if i < f0x_lens[b] else 0 (f0x [B, Fx] float64), fy likewise, a frame voiced when its F0 > 0, and the
+ * energies ex [B, Ex], ey [B, Ey] fp32:
+ *   counts[b] = (P, cells whose voicing differs, cells voiced on both sides, voiced cells with |fx/fy - 1| > 0.2)  int64
+ *   sums[b]   = (sum (1200 log2(fx/fy))^2 over cells voiced on both sides, sum (ex[i] - ey[j])^2)            float64
+ * FS2_EVAL_BAD_LENGTH in *status: plen[b] outside [0, P_max], a F0 length outside [0, Fx] / [0, Fy], or a path cell
+ * outside [0, Ex) x [0, Ey) (the pair's walk stops there).  One kernel, no workspace. */
+#define FS2_EVAL_BAD_LENGTH 1
+#define FS2_EVAL_NONFINITE 2
+int fs2_dtw_workspace_bytes(int B, int Lx_max, int Ly_max, int n_mels, int n_cep, int with_path, size_t* bytes);
+int fs2_mcd_dtw(const float* x, const int64_t* xlens, int Lx_max, const float* y, const int64_t* ylens, int Ly_max, int B,
+                int n_mels, const double* dct, int n_cep, double scale, double* mcd, double* cost, int64_t* plen, int32_t* path,
+                int* status, void* ws, size_t ws_bytes, void* stream);
+int fs2_path_prosody(const int32_t* path, const int64_t* plen, int B, int P_max, const double* f0x, const int64_t* f0x_lens, int Fx,
+                     const double* f0y, const int64_t* f0y_lens, int Fy, const float* ex, int Ex, const float* ey, int Ey,
+                     int64_t* counts, double* sums, int* status, void* stream);
+
 /* ---- batched MelGAN vocoder (DESIGN.md section 8) ------------------------------------------------------------------- */
 /* seungwonpark/melgan's Generator(mel_channel = 80) on log-mels [B, Lmax, 80] with frame counts olens [B]: utterance b is
  * the generator applied to its own frames mels[b, :olens[b]] followed by 10 frames of -11.5129, every reflection pad at its
