@@ -59,6 +59,8 @@ FS2_BIGVGAN_BAD_LENGTH, FS2_BIGVGAN_RANGE, FS2_BIGVGAN_BAD_START = 1, 2, 4   # b
 FS2_BIGVGAN_SNAKE, FS2_BIGVGAN_SNAKEBETA = 0, 1
 FS2_ISTFTNET_BAD_LENGTH, FS2_ISTFTNET_RANGE, FS2_ISTFTNET_BAD_START = 1, 2, 4   # bits of fs2_istftnet's / fs2_istftnet_window's status word
 FS2_EVAL_BAD_LENGTH, FS2_EVAL_NONFINITE = 1, 2   # bits of fs2_mcd_dtw's / fs2_path_prosody's status word
+FS2_PLAN_BAD_ILENS, FS2_PLAN_BAD_CONTROL, FS2_PLAN_OVERFLOW = 1, 2, 4   # bits of fs2_length_plan_cap's status word
+FS2_SYNTH_VOC_SHIFT = 8                          # fs2_synth_status: the vocoder's bits sit this far up in the word
 
 
 class HiFiGANConfig(C.Structure):
@@ -101,6 +103,8 @@ SIGNATURES = {
     "fs2_length_gather": [_P, _P, _P, _I, _I, _I, _P, _I, _P],
     "fs2_length_plan_ex": [_P, _I, _P, _F, _P, _I, _I, _I, _P, _P, _P, _P, _P],
     "fs2_length_gather_ex": [_P, _P, _P, _I, _I, _I, _P, _I, _P, _P, _P],
+    "fs2_length_plan_cap": [_P, _I, _P, _P, _P, _I, _I, _L, _P, _P, _P, _P, _P, _P],
+    "fs2_synth_status": [_P, _P, _P, _I, _I, _P, _P, _P],
     "fs2_decode": [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _SZ, _P],
     "fs2_decode_ex": [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _SZ, _I, _P],
     "fs2_decode_ctl": [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _SZ, _I, _P],

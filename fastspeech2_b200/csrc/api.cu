@@ -563,6 +563,24 @@ int fs2_length_gather_ex(const float* hs, const int32_t* cum, const int64_t* ile
   return length_gather(hs, cum, ilens, B, Tmax, C, out, Lcap, fac_in, fac_out, (cudaStream_t)stream);
 }
 
+int fs2_length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac, int B,
+                        int Tmax, int64_t Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int32_t* status,
+                        void* stream) {
+  FS2_REQUIRE(ds && ilens && cum && olens && need && status, "fs2_length_plan_cap: null argument");
+  FS2_REQUIRE(B >= 1 && Tmax >= 1, "fs2_length_plan_cap: B=%d and Tmax=%d must be >= 1", B, Tmax);
+  FS2_REQUIRE(Lc >= 1 && Lc <= INT32_MAX, "fs2_length_plan_cap: capacity Lc=%lld must lie in [1, %d] (the prefix sum is int32)",
+              (long long)Lc, INT32_MAX);
+  return length_plan_cap(ds, ds_dtype, ilens, alpha_v, fac, B, Tmax, (long)Lc, cum, olens, need, d_used, status,
+                         (cudaStream_t)stream);
+}
+
+int fs2_synth_status(const int32_t* plan_status, const int32_t* voc_status, const int64_t* olens, int B, int hop,
+                     int32_t* word, int64_t* alens, void* stream) {
+  FS2_REQUIRE(plan_status && olens && word, "fs2_synth_status: null argument");
+  FS2_REQUIRE(B >= 1 && hop >= 1, "fs2_synth_status: B=%d and hop=%d must be >= 1", B, hop);
+  return synth_status(plan_status, voc_status, olens, B, hop, word, alens, (cudaStream_t)stream);
+}
+
 int fs2_decode(fs2_handle* h, const float* hm, const int64_t* olens, const float* es, const float* ps, int B, int L,
                float* before, float* after, float* e_out, float* p_out, int64_t* e_ids, int64_t* p_ids, void* ws,
                size_t ws_bytes, void* stream) {

@@ -163,6 +163,9 @@ int transpose_v(const float* qkv, int B, int L, int C, int heads, float* vt, int
 int length_plan(void* ds, int ds_dtype, const int64_t* ilens, float alpha, const float* alpha_v, int B, int T, int mutate,
                 int32_t* cum, int64_t* olens, int64_t* stats, int64_t* d_used, cudaStream_t st);
 // fac_in [2][B, T] -> fac_out [2][B, Lcap] (both nullable): each frame takes the factors of its source phoneme, 1 past olens
+int length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac, int B, int T,
+                    long Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int* status, cudaStream_t st);
+int synth_status(const int* plan, const int* voc, const int64_t* olens, int B, int hop, int* word, int64_t* alens, cudaStream_t st);
 int length_gather(const float* hs, const int32_t* cum, const int64_t* ilens, int B, int T, int C, float* out, int Lcap,
                   const float* fac_in, float* fac_out, cudaStream_t st);
 

@@ -38,21 +38,44 @@ __device__ __forceinline__ long load_duration(const void* ds, int dtype, long id
   return d;
 }
 
+// What the capacity plan (CAP) adds to the scan: the capacity, the factor planes to check, the per-slot need and the
+// status word.  The plain plan passes none of it.
+struct CapArgs {
+  long Lc;
+  const float* fac;          // [2][B, T] pitch / energy factors checked like alpha_v, or NULL
+  int64_t* need;
+  int* status;
+};
+
+__device__ __forceinline__ bool bad_factor(float a) { return !(isfinite(a) && a > 0.f); }
+
+template <bool CAP>
 __global__ void __launch_bounds__(PLAN_THREADS)
 length_plan_kernel(void* ds, int dtype, const int64_t* __restrict__ ilens, float alpha, const float* __restrict__ alpha_v,
                    int T, int mutate, int32_t* __restrict__ cum, int64_t* __restrict__ olens,
-                   unsigned long long* __restrict__ stats, int64_t* __restrict__ d_used) {
+                   unsigned long long* __restrict__ stats, int64_t* __restrict__ d_used, CapArgs cap) {
   __shared__ long warp_tot[PLAN_THREADS / 32];
   __shared__ long carry_s;
-  __shared__ int any_nonzero, n_negative;
+  __shared__ int any_nonzero, n_negative, bad_control;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  long ilen = ilens[b];
+  const long ilen_in = ilens[b];
+  long ilen = ilen_in;
   if (ilen > T) ilen = T;
   if (ilen < 0) ilen = 0;
   const bool scale = alpha_v || alpha != 1.0f;   // alpha_v: one factor per phoneme [B, T], in place of the scalar
   const long base = (long)b * T;
-  if (tid == 0) { carry_s = 0; any_nonzero = 0; n_negative = 0; }
+  if (tid == 0) { carry_s = 0; any_nonzero = 0; n_negative = 0; bad_control = 0; }
   __syncthreads();
+  if (CAP) {   // the factors of the valid positions must be finite and > 0; a slot with a bad one is emptied below
+    const long plane = (long)gridDim.x * T;
+    int bad = 0;
+    for (long t = tid; t < ilen; t += PLAN_THREADS) {
+      if (alpha_v) bad |= bad_factor(alpha_v[base + t]);
+      if (cap.fac) bad |= bad_factor(cap.fac[base + t]) | bad_factor(cap.fac[plane + base + t]);
+    }
+    if (bad) atomicOr(&bad_control, 1);
+    __syncthreads();
+  }
 
   // pass 1: the reference tests `d.sum() == 0` on the truncated slice (:86).  For integer
   // durations that is "sum of the (possibly negative) values"; for float durations it is the
@@ -101,7 +124,25 @@ length_plan_kernel(void* ds, int dtype, const int64_t* __restrict__ ilens, float
     if (tid == PLAN_THREADS - 1) carry_s = v;
     __syncthreads();
   }
-  if (tid == 0) {
+  if (CAP) {
+    // a slot runs only when 1 <= ilens[b] <= T, its factors are valid and its frames fit the capacity; any other slot
+    // gets olens 0 and an all-zero cum row (the gather then writes it as zeros) and d_used row.  Each thread clears the
+    // positions it wrote above, so no barrier is needed
+    const long need = carry_s;
+    const bool bad_ilen = ilen_in < 0 || ilen_in > T, over = need > cap.Lc;
+    const bool live = ilen_in >= 1 && !bad_ilen && !over && !bad_control;
+    if (!live)
+      for (long t = tid; t < T; t += PLAN_THREADS) {
+        cum[base + t] = 0;
+        if (d_used) d_used[base + t] = 0;
+      }
+    if (tid == 0) {
+      cap.need[b] = need;
+      olens[b] = live ? need : 0;
+      const int bits = (bad_ilen ? FS2_PLAN_BAD_ILENS : 0) | (bad_control ? FS2_PLAN_BAD_CONTROL : 0) | (over ? FS2_PLAN_OVERFLOW : 0);
+      if (bits) atomicOr(cap.status, bits);
+    }
+  } else if (tid == 0) {
     olens[b] = carry_s;
     atomicMax(&stats[0], (unsigned long long)carry_s);
     if (n_negative) atomicAdd(&stats[1], (unsigned long long)n_negative);
@@ -170,8 +211,44 @@ int length_plan(void* ds, int ds_dtype, const int64_t* ilens, float alpha, const
   FS2_REQUIRE(ds_dtype == FS2_DUR_I64 || ds_dtype == FS2_DUR_F32 || ds_dtype == FS2_DUR_I32, "length_plan: bad ds dtype %d", ds_dtype);
   FS2_CUDA_CHECK(cudaMemsetAsync(stats, 0, 2 * sizeof(int64_t), st));
   if (B == 0) return FS2_OK;
-  length_plan_kernel<<<B, PLAN_THREADS, 0, st>>>(ds, ds_dtype, ilens, alpha, alpha_v, T, mutate, cum, olens,
-                                                 reinterpret_cast<unsigned long long*>(stats), d_used);
+  length_plan_kernel<false><<<B, PLAN_THREADS, 0, st>>>(ds, ds_dtype, ilens, alpha, alpha_v, T, mutate, cum, olens,
+                                                        reinterpret_cast<unsigned long long*>(stats), d_used, CapArgs{});
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+int length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac, int B, int T,
+                    long Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int* status, cudaStream_t st) {
+  FS2_REQUIRE(ds_dtype == FS2_DUR_I64 || ds_dtype == FS2_DUR_F32 || ds_dtype == FS2_DUR_I32, "length_plan_cap: bad ds dtype %d", ds_dtype);
+  FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
+  length_plan_kernel<true><<<B, PLAN_THREADS, 0, st>>>(const_cast<void*>(ds), ds_dtype, ilens, 1.0f, alpha_v, T, 0, cum, olens,
+                                                       nullptr, d_used, CapArgs{Lc, fac, need, status});
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+namespace {
+// One warp: word = plan bits | vocoder bits << 8, the vocoder's BAD_LENGTH dropped when some slot has olens 0 (that slot
+// is empty, overflowed or refused, and the vocoder reports exactly that); alens[b] = olens[b] * hop
+__global__ void synth_status_kernel(const int* __restrict__ plan, const int* __restrict__ voc, const int64_t* __restrict__ olens,
+                                    int B, int hop, int* __restrict__ word, int64_t* __restrict__ alens) {
+  int any_empty = 0;
+  for (int b = threadIdx.x; b < B; b += 32) {
+    const int64_t o = olens[b];
+    any_empty |= o == 0;
+    if (alens) alens[b] = o * hop;
+  }
+  any_empty = __any_sync(0xffffffffu, any_empty);
+  if (threadIdx.x == 0) {
+    int v = voc ? *voc : 0;
+    if (any_empty) v &= ~FS2_VOC_BAD_LENGTH;
+    *word = *plan | (v << FS2_SYNTH_VOC_SHIFT);
+  }
+}
+}  // namespace
+
+int synth_status(const int* plan, const int* voc, const int64_t* olens, int B, int hop, int* word, int64_t* alens, cudaStream_t st) {
+  synth_status_kernel<<<1, 32, 0, st>>>(plan, voc, olens, B, hop, word, alens);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }

@@ -647,6 +647,11 @@ class FeedForwardTransformer(nn.Module):
         where the final mels are written (default: a fresh tensor), e.g. a peer-mapped slot of `sharded.PeerGather`."""
         return GraphedForward(self, xs, ilens, olens, ds, es, ps, after_out=after_out)
 
+    def graphed_synthesize(self, B: int, T: int, capacity: int, vocoder=None) -> "GraphedSynthesis":
+        """Capture `synthesize` (and `vocoder`, a MelGAN / HiFi-GAN / BigVGAN / iSTFTNet vocoder, when given) for B slots
+        of T phonemes at `capacity` frames into one CUDA graph that reads nothing back (see GraphedSynthesis)."""
+        return GraphedSynthesis(self, B, T, capacity, vocoder)
+
     def forward(self, xs: torch.Tensor, ilens: torch.Tensor, ys: torch.Tensor, olens: torch.Tensor, ds: torch.Tensor,
                 es: torch.Tensor, ps: torch.Tensor) -> Tuple[torch.Tensor, List[Dict[str, float]]]:
         """Loss computation (fastspeech.py:245-337). Returns (loss, report_keys).  In train mode the loss is attached to
@@ -803,3 +808,211 @@ class GraphedForward:
             if dst.data_ptr() != src.data_ptr():
                 dst.copy_(src, non_blocking=True)
         return self.replay(validate)
+
+
+class GraphedSynthesis:
+    """Per-utterance synthesis (`synthesize`, optionally followed by a neural vocoder) replayed as one CUDA graph at a
+    fixed frame capacity, with no host read (DESIGN.md section 21).
+
+    `synthesize` sizes the decoder by Lmax, which it reads back from the device; here every decoder-side buffer is
+    `capacity` frames long and the capacity length plan (fs2_length_plan_cap) decides on the device which slots run:
+    slot b runs when 1 <= ilens[b] <= T, its control factors are finite and > 0, and need[b] (its planned frame count)
+    <= capacity; every other slot is written as exact zeros (its own row tiles are dead, DESIGN.md section 21).  Captured once for B slots of T phonemes,
+    the current weights, precision and vocoder:
+
+      encoder + duration predictor -> capacity plan -> gather -> variance adaptor, decoder, Postnet at L = capacity
+      [-> vocoder._call at Lmax = capacity] -> status fold
+
+    Static inputs (`self.xs` [B, T], `self.ilens` [B], `self.speed` / `self.pitch` / `self.energy` [B, T] float32, 1.0
+    when not set, which is bit-identical to no control); static outputs, valid until the next replay: mels [B, capacity,
+    80], olens [B], durations [B, T] and need [B], and with a vocoder audio [B, capacity * 256] and alens [B] = olens * 256.
+    A slot that ran is bit-identical to `synthesize` on that utterance alone (and its audio to the vocoder on that);
+    rows past olens[b] and every row of a slot that did not run are +0.
+
+    Validation, as in `GraphedForward`: each replay copies one status word to pinned host memory asynchronously;
+    validate=True checks it at once, "deferred" at the next call or `flush()`, False never.  Bad ilens and bad control
+    factors raise ValueError as `synthesize` does; the vocoder's range bit raises as the vocoder would.  Overflow is not
+    an error: `overflowed()` lists those slots and `need` says what capacity would fit them.  The graph keeps its own
+    workspaces; a change of the model's or the vocoder's parameters after capture (or an eager call that grows the
+    positional tables, which repacks the weights) makes `__call__` raise."""
+
+    def __init__(self, model: FeedForwardTransformer, B: int, T: int, capacity: int, vocoder=None):
+        for name, v in (("B", B), ("T", T), ("capacity", capacity)):
+            if isinstance(v, bool) or not isinstance(v, int) or v < 1:
+                raise ValueError(f"{name} must be an int >= 1 (got {v!r})")
+        if capacity > _lr.INT32_MAX:
+            raise ValueError(f"capacity={capacity} exceeds the length plan's int32 prefix sum ({_lr.INT32_MAX})")
+        if vocoder is not None:
+            from ._kernel_module import NeuralVocoder
+            if not isinstance(vocoder, NeuralVocoder) or not hasattr(vocoder, "_chain"):
+                raise ValueError(f"vocoder must be a NeuralVocoder upsampling chain (MelGAN, HiFi-GAN, BigVGAN or iSTFTNet), got "
+                                 f"{type(vocoder).__name__}: WaveGlow's noise and Griffin-Lim are not captured")
+            vocoder._check_size(B, capacity)
+        dev = model._device()
+        if dev.type != "cuda":
+            raise _lib.Fs2Error(f"model parameters are on {dev}: the H100 path has no CPU fallback, call model.to('cuda')")
+        self.model, self.vocoder, self.device = model, vocoder, dev
+        self.B, self.T, self.capacity = B, T, capacity
+        d = model.dims
+        i64, f32 = dict(dtype=torch.int64, device=dev), dict(dtype=torch.float32, device=dev)
+        self.xs, self.ilens = torch.zeros((B, T), **i64), torch.zeros((B,), **i64)
+        self.speed = torch.ones((B, T), **f32)
+        self._fac = torch.ones((2, B, T), **f32)            # the gather's per-phoneme planes: energy, pitch
+        self.energy, self.pitch = self._fac[0], self._fac[1]
+        self._controlled = False
+        self._hs = torch.empty((B, T, d.adim), **f32)
+        self._d_int = torch.empty((B, T), **i64)
+        self._cum = torch.empty((B, T), dtype=torch.int32, device=dev)
+        self.olens, self.need, self.durations = torch.empty((B,), **i64), torch.empty((B,), **i64), torch.empty((B, T), **i64)
+        self._hm = torch.empty((B, capacity, d.adim), **f32)
+        self._fac_out = torch.empty((2, B, capacity), **f32)
+        self._before, self.mels = torch.empty((B, capacity, d.odim), **f32), torch.empty((B, capacity, d.odim), **f32)
+        self._e_out, self._p_out = torch.empty((B, capacity), **f32), torch.empty((B, capacity), **f32)
+        self._plan_status = torch.empty((1,), dtype=torch.int32, device=dev)
+        self.status = torch.empty((1,), dtype=torch.int32, device=dev)
+        self.audio = self.alens = self._voc_status = None
+        with torch.no_grad():
+            if T > model.encoder.embed[-1].pe.shape[1]:
+                model._extend_pe(model.encoder, T)
+            if capacity > model.decoder.embed[-1].pe.shape[1]:
+                model._extend_pe(model.decoder, capacity)
+            self._h = model._ready(self.xs)
+            n = C.c_size_t()
+            _lib.check(_lib.load().fs2_workspace_bytes(self._h, B, T, capacity, C.byref(n)), "fs2_workspace_bytes")
+            self._ws = torch.empty(int(n.value), dtype=torch.uint8, device=dev)
+            if vocoder is not None:
+                from ._kernel_module import query_bytes
+                self._vh = vocoder._handle(dev)
+                self._vws = torch.empty(query_bytes(f"fs2_{vocoder._NAME}_workspace_bytes", self._vh, B, capacity),
+                                        dtype=torch.uint8, device=dev)
+                self.audio = torch.empty((B, capacity * vocoder.HOP), **f32)
+                self.alens = torch.empty((B,), **i64)
+                self._voc_status = torch.empty((1,), dtype=torch.int32, device=dev)
+                self._voc_fingerprint = vocoder._fingerprint()
+            with torch.cuda.device(dev):
+                for _ in range(2):                  # warm-up on empty slots: kernel attributes, lazily built launch state
+                    self._run()
+                torch.cuda.synchronize(dev)
+                self._fingerprint = model._current_fingerprint()
+                self._params = list(model._sd_cache)
+                self._versions = sum(t._version for t in self._params)
+                self.graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(self.graph):
+                    self._run()
+        self._status_host = torch.empty((1,), dtype=torch.int32).pin_memory()
+        self._status_event = torch.cuda.Event()
+        self._pending = False
+
+    def _run(self) -> None:
+        """The captured sequence, on the static buffers."""
+        lib, P = _lib.load(), _lib.ptr
+        B, T, Lc, d = self.B, self.T, self.capacity, self.model.dims
+        st = _lib.stream_ptr(self.device)
+        flags = _lib.FS2_PER_UTTERANCE
+        _lib.check(lib.fs2_encode_ex(self._h, P(self.xs), P(self.ilens), B, T, P(self._hs), None, P(self._d_int), P(self._ws),
+                                     self._ws.numel(), flags, st), "fs2_encode_ex")
+        _lib.check(lib.fs2_length_plan_cap(P(self._d_int), _lib.FS2_DUR_I64, P(self.ilens), P(self.speed), P(self._fac), B, T, Lc,
+                                           P(self._cum), P(self.olens), P(self.need), P(self.durations), P(self._plan_status), st),
+                   "fs2_length_plan_cap")
+        _lib.check(lib.fs2_length_gather_ex(P(self._hs), P(self._cum), P(self.ilens), B, T, d.adim, P(self._hm), Lc, P(self._fac),
+                                            P(self._fac_out), st), "fs2_length_gather_ex")
+        _lib.check(lib.fs2_decode_ctl(self._h, P(self._hm), P(self.olens), None, None, B, Lc, P(self._before), P(self.mels),
+                                      P(self._e_out), P(self._p_out), None, None, P(self._fac_out[0]), P(self._fac_out[1]),
+                                      P(self._ws), self._ws.numel(), flags, st), "fs2_decode_ctl")
+        hop = 1
+        if self.vocoder is not None:
+            self.vocoder._call(self._vh, self.mels, self.olens, B, Lc, self.audio, self._voc_status, self._vws)
+            hop = self.vocoder.HOP
+        _lib.check(lib.fs2_synth_status(P(self._plan_status), P(self._voc_status), P(self.olens), B, hop, P(self.status),
+                                        P(self.alens), st), "fs2_synth_status")
+
+    @property
+    def outputs(self) -> tuple:
+        """(mels, olens, durations), and with a vocoder (..., audio, alens): the static outputs of the last replay."""
+        out = (self.mels, self.olens, self.durations)
+        return out if self.vocoder is None else out + (self.audio, self.alens)
+
+    @staticmethod
+    def check_request(xs, ilens, B: int, T: int) -> Tuple[int, int]:
+        """The checks of a request that need no device: xs [b, t] with b <= B, t <= T, and ilens [b] (values in [0, t]
+        when on the host; on the device they are checked against T in the status word).  -> (b, t)."""
+        if not torch.is_tensor(xs) or xs.dim() != 2 or xs.shape[0] == 0 or xs.shape[1] == 0:
+            raise ValueError("xs must be a non-empty [b, t] tensor")
+        b, t = int(xs.shape[0]), int(xs.shape[1])
+        if b > B or t > T:
+            raise ValueError(f"a request of b={b} utterances of t={t} phonemes does not fit the graph's B={B}, T={T}")
+        if not torch.is_tensor(ilens) or ilens.dim() != 1 or ilens.shape[0] != b:
+            raise ValueError(f"ilens must be a [b={b}] tensor")
+        if ilens.dtype.is_floating_point or ilens.dtype == torch.bool:
+            raise ValueError("ilens must be an integer tensor")
+        if not ilens.is_cuda and b and (int(ilens.min()) < 0 or int(ilens.max()) > t):
+            raise ValueError(f"every ilens[b] must lie in [0, t={t}] (0 marks an empty slot)")
+        return b, t
+
+    def _check_model(self) -> None:
+        m = self.model
+        if m._epoch != self._fingerprint[0] or sum(t._version for t in self._params) != self._versions:
+            raise RuntimeError("model parameters changed since capture: build a new GraphedSynthesis")
+        if self.vocoder is not None and self.vocoder._fingerprint() != self._voc_fingerprint:
+            raise RuntimeError("vocoder parameters changed since capture: build a new GraphedSynthesis")
+
+    def _raise_for(self, word: int) -> None:
+        if word & _lib.FS2_PLAN_BAD_ILENS:
+            raise ValueError(f"every ilens[b] must lie in [0, T={self.T}] (0 marks an empty slot)")
+        if word & _lib.FS2_PLAN_BAD_CONTROL:
+            raise ValueError("prosody controls: some factor(s) are non-finite or <= 0 (each must be finite and > 0)")
+        voc = word >> _lib.FS2_SYNTH_VOC_SHIFT
+        if voc and self.vocoder is not None:
+            for bit, message in self.vocoder._status_table():
+                if voc & bit:
+                    raise ValueError(message)
+
+    def flush(self) -> None:
+        """Run the outstanding deferred validation (waits for the replay it belongs to)."""
+        if self._pending:
+            self._pending = False
+            self._status_event.synchronize()
+            self._raise_for(int(self._status_host[0]))
+
+    def replay(self, validate=True) -> tuple:
+        """Replay on the current contents of the static inputs; -> `outputs`."""
+        self._check_model()
+        self.flush()
+        with torch.cuda.device(self.device):
+            self.graph.replay()
+            if validate:
+                self._status_host.copy_(self.status, non_blocking=True)
+                self._status_event.record()
+                self._pending = True
+        if validate and validate != "deferred":
+            self.flush()
+        return self.outputs
+
+    def __call__(self, xs, ilens, speed=None, pitch=None, energy=None, validate=True) -> tuple:
+        """Synthesize b <= B requests of t <= T phonemes: xs [b, t] (0 = pad) and ilens [b] are copied into slots 0 .. b-1,
+        slots b .. B-1 become empty.  speed / pitch / energy: None, a number, a [b] or a [b, t] tensor, as in `synthesize`.
+        -> `outputs` (all B slots)."""
+        if validate not in (True, False, "deferred"):
+            raise ValueError(f"validate must be True, False or 'deferred' (got {validate!r})")
+        self._check_model()
+        b, t = self.check_request(xs, ilens, self.B, self.T)
+        controls = _controls_for(b, t, self.device, {"speed": speed, "pitch": pitch, "energy": energy}, ilens)
+        with torch.cuda.device(self.device):
+            self.xs.zero_()
+            self.xs[:b, :t].copy_(xs, non_blocking=True)
+            self.ilens.zero_()
+            self.ilens[:b].copy_(ilens, non_blocking=True)
+            if self._controlled or controls is not None:     # factors stay 1.0 between uncontrolled requests
+                self.speed.fill_(1.0)
+                self._fac.fill_(1.0)
+                for dst, src in zip((self.speed, self.pitch, self.energy), controls or (None,) * 3):
+                    if src is not None:
+                        dst[:b, :t].copy_(src)
+                self._controlled = controls is not None
+        return self.replay(validate)
+
+    def overflowed(self) -> List[int]:
+        """The slots of the last replay whose planned frames (need) exceed the capacity: they were skipped (olens 0), not
+        refused.  One host read."""
+        need, il = torch.stack([self.need, self.ilens]).tolist()
+        return [b for b in range(self.B) if 1 <= il[b] <= self.T and need[b] > self.capacity]

@@ -174,6 +174,34 @@ int fs2_length_plan_ex(void* ds, int ds_dtype, const int64_t* ilens, float alpha
 int fs2_length_gather_ex(const float* hs, const int32_t* cum, const int64_t* ilens, int B, int Tmax, int C, float* out,
                          int Lcap, const float* fac_in, float* fac_out, void* stream);
 
+/* Capacity plan (synthesis replayed from a CUDA graph at a fixed frame capacity Lc, DESIGN.md section 21): the scan of
+ * fs2_length_plan_ex with mutate_ds = 0 and alpha = 1, sized by Lc instead of by a host read, and nothing read back.
+ *   ds, ds_dtype, ilens, alpha_v, d_used: as in fs2_length_plan_ex (alpha_v may be NULL)
+ *   fac     [2][B,Tmax] f32 or NULL: the pitch / energy factors (fs2_length_gather_ex's fac_in), checked like alpha_v
+ *   need    [B] i64 out: the frames slot b plans, computed exactly as fs2_length_plan_ex's olens (speed, all-zero rule)
+ *   olens   [B] i64 out: need[b] when 1 <= ilens[b] <= Tmax, need[b] <= Lc and the slot's factors are valid; else 0
+ *   cum     [B,Tmax] i32 out: fs2_length_plan_ex's where olens[b] = need[b], all zeros where olens[b] = 0, so that
+ *           fs2_length_gather_ex into Lc rows writes such a slot as zeros; d_used is likewise 0 there
+ *   status  one i32 (device) out, zeroed by the call, then the OR of
+ *     FS2_PLAN_BAD_ILENS    some ilens[b] outside [0, Tmax];
+ *     FS2_PLAN_BAD_CONTROL  a factor of alpha_v or fac at t < ilens[b] is non-finite or <= 0;
+ *     FS2_PLAN_OVERFLOW     some need[b] > Lc (informational: that slot is skipped, need says what would fit it).
+ * ilens[b] == 0 marks an empty slot: need and olens 0, no bit.  Needs B, Tmax, Lc >= 1 and Lc <= INT32_MAX (cum is
+ * int32). */
+#define FS2_PLAN_BAD_ILENS 1
+#define FS2_PLAN_BAD_CONTROL 2
+#define FS2_PLAN_OVERFLOW 4
+int fs2_length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac, int B,
+                        int Tmax, int64_t Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int32_t* status,
+                        void* stream);
+/* The status word of one graphed synthesis: *word = *plan_status | (vocoder bits << FS2_SYNTH_VOC_SHIFT), where the
+ * vocoder's bits are *voc_status (NULL: none) without its BAD_LENGTH bit when some olens[b] is 0 (an empty, overflowed or
+ * refused slot, which the vocoder reports as a bad length by design).  alens [B] i64 out or NULL: olens[b] * hop.
+ * Every vocoder's status word has BAD_LENGTH = 1 and RANGE = 2. */
+#define FS2_SYNTH_VOC_SHIFT 8
+int fs2_synth_status(const int32_t* plan_status, const int32_t* voc_status, const int64_t* olens, int B, int hop,
+                     int32_t* word, int64_t* alens, void* stream);
+
 /* ---- stage 3: variance adaptor + mel decoder + Postnet --------------------------------- */
 /* fastspeech.py:195-238.
  *   hm [B,L,adim] f32: length-regulated encoder states (read only)
