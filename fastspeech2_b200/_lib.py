@@ -203,6 +203,8 @@ SIGNATURES = {
     "fs2_waveglow_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
     "fs2_waveglow": [_P, _P, _P, _I, _I, C.c_double, _P, _P, _P, _P, _P, _SZ, _P],
     "fs2_waveglow_noise": [_P, _P, _I, _I, _P, _P],
+    "fs2_op_waveglow_upsample": [_P, _P, _P, _I, _I, _P, _P, _P, _P],
+    "fs2_op_waveglow_flow": [_P, _I, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P],
     "fs2_waveglow_window_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
     "fs2_waveglow_window": [_P, _P, _P, _P, _I, _I, _I, C.c_double, _P, _P, _P, _L, _P, _P, _SZ, _P],
     "fs2_peer_alloc": [_SZ, C.POINTER(_P), _P],

@@ -23,6 +23,7 @@
 // z's channels 0-1 and 2-3 are exactly the early noise prepended after flows 4 and 8, so the concatenation costs nothing.
 // After flow 0 the state is the audio itself ([B, Ls, 8] row-major = [B, Lmax * 256]), so the last flow writes `audio`.
 // Launches per call: 4 + 12 * 41 = 496, plus 1 (the cond planes) in f16 / 3xF16; a window adds 1 (its audio copy).
+// run() is upsample() then flow() per k; the per-stage test entries at the end of the file call the same two functions.
 //
 // A GEMM row depends only on its own input rows (the in-layer GEMM: rows t, t +- 2^i of its own utterance, zero outside
 // [0, olens * 32)), in a fixed K order, so per-utterance results do not depend on the batch.
@@ -64,19 +65,20 @@ __device__ __forceinline__ bool exact_row(const int64_t* __restrict__ win, int B
   return (f0 == 0 || t >= margin) && (f0 + nf == win[kWinN * B + b] || t < ns - margin);
 }
 
-// one CTA: lensF[b] = olens[b], lensS[b] = olens[b] * 32 for 1 <= olens[b] <= L, else 0 (the utterance is skipped);
-// *status = 0 or FS2_WAVEGLOW_BAD_LENGTH.  Runs first, so the producers' range bits land on a cleared word.
-__global__ void wg_prep_kernel(const int64_t* __restrict__ olens, int B, int L, int64_t* __restrict__ lensF,
+// one CTA: lensF[b] = olens[b], lensS[b] (nullable) = olens[b] * 32 for lo <= olens[b] <= L, else 0 (the utterance is
+// skipped); *status = 0 or FS2_WAVEGLOW_BAD_LENGTH.  Runs first, so the producers' range bits land on a cleared word.
+// lo = 1 for the vocoder's calls; the single-layer entries take lo = 0 (an empty utterance is valid there).
+__global__ void wg_prep_kernel(const int64_t* __restrict__ olens, int B, int L, int lo, int64_t* __restrict__ lensF,
                                int64_t* __restrict__ lensS, int* __restrict__ status) {
   __shared__ int bad;
   if (threadIdx.x == 0) bad = 0;
   __syncthreads();
   for (int b = threadIdx.x; b < B; b += blockDim.x) {
     const int64_t n = olens[b];
-    const bool ok = n >= 1 && n <= L;
+    const bool ok = n >= lo && n <= L;
     if (!ok) atomicOr(&bad, 1);
     lensF[b] = ok ? n : 0;
-    lensS[b] = ok ? n * kSteps : 0;
+    if (lensS) lensS[b] = ok ? n * kSteps : 0;
   }
   __syncthreads();
   if (threadIdx.x == 0) *status = bad ? FS2_WAVEGLOW_BAD_LENGTH : 0;
@@ -388,6 +390,19 @@ struct WgPlan {
   float* skip[2];      // skip accumulator [B * Ls][C], ping-pong
 };
 
+// a flow's buffers over `rows` step rows: x, xp, cd, ia, acts, skip and the cond planes (plane modes)
+void plan_wn(Bump& b, WgPlan& p, bool planes, int C, size_t rows) {
+  p.x[0] = b.floats(rows * C);
+  p.x[1] = b.floats(rows * C);
+  p.xp = planes ? (__half*)b.floats(rows * C) : nullptr;
+  p.cd = b.floats(rows * 2 * C);
+  p.ia = b.floats(rows * 2 * C);
+  p.acts = b.floats(rows * C);
+  p.skip[0] = b.floats(rows * C);
+  p.skip[1] = b.floats(rows * C);
+  p.condp = planes ? (__half*)b.floats(rows * kCond) : nullptr;
+}
+
 // buffers of L frames per utterance: the whole call's (L = Lmax) or a window's (window, L = n_frames + 2H)
 WgPlan plan(Bump& b, int mode, int C, int B, int L, bool window = false) {
   const size_t frames = (size_t)B * L, rows = frames * kSteps;
@@ -404,18 +419,12 @@ WgPlan plan(Bump& b, int mode, int C, int B, int L, bool window = false) {
   }
   p.up_a = b.floats(frames * kUpK);                   // fp32 rows, or hi + lo planes: the same bytes
   p.state = b.floats(rows * kGroup);
-  p.x[0] = b.floats(rows * C);
-  p.x[1] = b.floats(rows * C);
-  p.xp = planes ? (__half*)b.floats(rows * C) : nullptr;
-  p.cd = b.floats(rows * 2 * C);
-  p.ia = b.floats(rows * 2 * C);
-  p.acts = b.floats(rows * C);
-  p.skip[0] = b.floats(rows * C);
-  p.skip[1] = b.floats(rows * C);
-  p.condp = planes ? (__half*)b.floats(rows * kCond) : nullptr;
+  plan_wn(b, p, planes, C, rows);
   p.cond = planes && 2 * C >= kCond ? p.ia : b.floats(rows * kCond);    // ia holds rows * 2C floats
   return p;
 }
+
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }   // null counts as aligned
 
 int check_size(const fs2_waveglow_net* m, int B, int L) {
   FS2_REQUIRE(B >= 1 && L >= 1, "fs2_waveglow: need B >= 1 and Lmax >= 1 (got %d, %d)", B, L);
@@ -438,6 +447,77 @@ int launch_flow(K kernel, int c, int C, const float* skip, const float* in, floa
   return FS2_OK;
 }
 
+// flow k's tail (wg_flow_kernel) on the WN skip sum `skip`: columns 8 - c .. 7 of the state `in` into those of `out`
+int flow_tail(const fs2_waveglow_net* m, int k, const float* skip, const float* in, float* out, const int64_t* lens, int B, int Ls,
+              cudaStream_t st) {
+  const WFlow& f = m->flows[k];
+  const int c = flow_channels(k), h = c / 2, o = kGroup - c, C = m->C;
+  return h == 4 ? launch_flow(wg_flow_kernel<4>, c, C, skip, in, out, lens, B, Ls, o, f, st)
+       : h == 3 ? launch_flow(wg_flow_kernel<3>, c, C, skip, in, out, lens, B, Ls, o, f, st)
+                : launch_flow(wg_flow_kernel<2>, c, C, skip, in, out, lens, B, Ls, o, f, st);
+}
+
+// The upsampling on the plan p (L frames per utterance, mels Lm frames apart): the operand of frames t - 3 .. t, the
+// polyphase GEMM into the fp32 cond rows p.cond and, in the plane modes, their planes p.condp with the range check.
+// *cond_a: the cond GEMMs' operand (p.condp or p.cond).
+int upsample(const fs2_waveglow_net* m, const WgPlan& p, const float* mels, int B, int L, int Lm, int* status, cudaStream_t st,
+             const void** cond_a) {
+  const int kind = out_kind(m->math_mode);
+  const bool planes = plane_mode(m->math_mode);
+  const long rows = (long)B * L * kSteps;
+  int rc;
+  {
+    auto k = pick(kind, wg_up_operand_kernel<OUT_HILO>, wg_up_operand_kernel<OUT_HI>, wg_up_operand_kernel<OUT_F32>);
+    k<<<grid_for((long)B * L * (kUpK / 4), 256), 256, 0, st>>>(mels, p.lensF, p.win, B, L, Lm, (float*)p.up_a, (__half*)p.up_a, status);
+    FS2_LAUNCH_CHECK();
+  }
+  if ((rc = vweight_gemm(m->math_mode, m->up, p.up_a, B, L, ACT_NONE, p.lensF, p.cond, st))) return rc;
+  if (planes) {
+    auto k = kind == OUT_HILO ? wg_planes_kernel<OUT_HILO> : wg_planes_kernel<OUT_HI>;
+    k<<<grid_for(rows * (kCond / 4), 256), 256, 0, st>>>(p.cond, p.lensS, B, L * kSteps, kCond, p.condp, status);
+    FS2_LAUNCH_CHECK();
+  }
+  *cond_a = planes ? (const void*)p.condp : (const void*)p.cond;
+  return FS2_OK;
+}
+
+// Flow k of the inverse on the plan p (Ls step rows per utterance, lengths p.lensS): WN k -- start on columns o .. o + h - 1
+// of the state `in`, then per layer the cond and in-layer GEMMs, the gate and the res / skip GEMMs -- and flow_tail from
+// `in` into `out` (which may be `in`).  *wn (nullable): the buffer that holds WN's skip sum (before `end`).
+int flow(const fs2_waveglow_net* m, int k, const WgPlan& p, const void* cond_a, const float* in, float* out, int B, int Ls, int* status,
+         cudaStream_t st, const float** wn = nullptr) {
+  const int kind = out_kind(m->math_mode), C = m->C;
+  const bool planes = plane_mode(m->math_mode);
+  const long rows = (long)B * Ls;
+  const int64_t* win = p.win;
+  const WFlow& f = m->flows[k];
+  const int c = flow_channels(k), h = c / 2, o = kGroup - c;
+  const int exact = (kFlows - 1 - k) * kFlowReach;          // a window's rows are exact this far from an interior side
+  auto start = pick(kind, wg_start_kernel<OUT_HILO>, wg_start_kernel<OUT_HI>, wg_start_kernel<OUT_F32>);
+  auto gate = pick(kind, wg_gate_kernel<OUT_HILO>, wg_gate_kernel<OUT_HI>, wg_gate_kernel<OUT_F32>);
+  int rc;
+  start<<<grid_for(rows * (C / 4), 256), 256, 0, st>>>(in, p.lensS, win, exact, B, Ls, C, o, h, f.start_w, f.start_b, p.x[0], p.xp, status);
+  FS2_LAUNCH_CHECK();
+  int cur = 0, sk = 0;
+  for (int i = 0; i < kLayers; ++i) {
+    if ((rc = vweight_gemm(m->math_mode, f.cond[i], cond_a, B, Ls, ACT_NONE, p.lensS, p.cd, st))) return rc;
+    const void* xa = planes ? (const void*)p.xp : (const void*)p.x[cur];
+    if ((rc = vweight_gemm(m->math_mode, f.in[i], xa, B, Ls, ACT_NONE, p.lensS, p.ia, st, p.cd, 1 << i))) return rc;
+    // layer i's input x is exact at exact + 2^i - 1, its in-layer output (and so acts and the next x) at exact + 2^(i+1) - 1
+    gate<<<grid_for(rows * (C / 4), 256), 256, 0, st>>>(p.ia, planes && i > 0 ? p.x[cur] : nullptr, p.lensS, win, exact + (2 << i) - 1,
+                                                         exact + (1 << i) - 1, B, Ls, C, (float*)p.acts, (__half*)p.acts, status);
+    FS2_LAUNCH_CHECK();
+    if (i < kLayers - 1) {
+      if ((rc = vweight_gemm(m->math_mode, f.res[i], p.acts, B, Ls, ACT_NONE, p.lensS, p.x[cur ^ 1], st, p.x[cur], 1, p.xp))) return rc;
+      cur ^= 1;
+    }
+    if ((rc = vweight_gemm(m->math_mode, f.skip[i], p.acts, B, Ls, ACT_NONE, p.lensS, p.skip[sk ^ 1], st, i ? p.skip[sk] : nullptr))) return rc;
+    sk ^= 1;
+  }
+  if (wn) *wn = p.skip[sk];
+  return flow_tail(m, k, p.skip[sk], in, out, p.lensS, B, Ls, st);
+}
+
 // The inverse flow on the plan p: whole utterances (starts == nullptr; buffers of Lmax frames, audio written by the last
 // flow) or a window of nf frames from starts[b] (buffers of nf + 2H frames, the window descriptors p.win, the core copied
 // out by wg_win_audio_kernel).  audio rows ld samples apart.  Both enqueue the same kernels but the first and the last.
@@ -445,62 +525,21 @@ int run(const fs2_waveglow_net* m, const WgPlan& p, const float* mels, const int
         int nf, double sigma, const int64_t* seeds, const float* z, float* audio, long ld, int* status, cudaStream_t st) {
   const bool window = starts != nullptr;
   const int L = window ? nf + 2 * kHalo : Lmax;
-  const int kind = out_kind(m->math_mode), C = m->C, Ls = L * kSteps;
-  const bool planes = plane_mode(m->math_mode);
+  const int Ls = L * kSteps;
   const long rows = (long)B * Ls;
-  const int64_t* win = p.win;
   int rc;
 
   if (window)
     wg_win_desc_kernel<<<1, 256, 0, st>>>(olens, starts, B, Lmax, nf, p.win, status);
   else
-    wg_prep_kernel<<<1, 256, 0, st>>>(olens, B, Lmax, p.lensF, p.lensS, status);
+    wg_prep_kernel<<<1, 256, 0, st>>>(olens, B, Lmax, 1, p.lensF, p.lensS, status);
   FS2_LAUNCH_CHECK();
-  wg_noise_kernel<<<grid_for(rows * 2, 256), 256, 0, st>>>(z, Lmax * kSteps, seeds, p.lensS, win, 1, B, Ls, sigma, p.state, nullptr);
+  wg_noise_kernel<<<grid_for(rows * 2, 256), 256, 0, st>>>(z, Lmax * kSteps, seeds, p.lensS, p.win, 1, B, Ls, sigma, p.state, nullptr);
   FS2_LAUNCH_CHECK();
-  {
-    auto k = pick(kind, wg_up_operand_kernel<OUT_HILO>, wg_up_operand_kernel<OUT_HI>, wg_up_operand_kernel<OUT_F32>);
-    k<<<grid_for((long)B * L * (kUpK / 4), 256), 256, 0, st>>>(mels, p.lensF, win, B, L, Lmax, (float*)p.up_a, (__half*)p.up_a, status);
-    FS2_LAUNCH_CHECK();
-  }
-  if ((rc = vweight_gemm(m->math_mode, m->up, p.up_a, B, L, ACT_NONE, p.lensF, p.cond, st))) return rc;
-  if (planes) {
-    auto k = kind == OUT_HILO ? wg_planes_kernel<OUT_HILO> : wg_planes_kernel<OUT_HI>;
-    k<<<grid_for(rows * (kCond / 4), 256), 256, 0, st>>>(p.cond, p.lensS, B, Ls, kCond, p.condp, status);
-    FS2_LAUNCH_CHECK();
-  }
-  const void* cond_a = planes ? (const void*)p.condp : (const void*)p.cond;
-  auto start = pick(kind, wg_start_kernel<OUT_HILO>, wg_start_kernel<OUT_HI>, wg_start_kernel<OUT_F32>);
-  auto gate = pick(kind, wg_gate_kernel<OUT_HILO>, wg_gate_kernel<OUT_HI>, wg_gate_kernel<OUT_F32>);
-  for (int k = kFlows - 1; k >= 0; --k) {
-    const WFlow& f = m->flows[k];
-    const int c = flow_channels(k), h = c / 2, o = kGroup - c;
-    const int exact = (kFlows - 1 - k) * kFlowReach;          // a window's rows are exact this far from an interior side
-    start<<<grid_for(rows * (C / 4), 256), 256, 0, st>>>(p.state, p.lensS, win, exact, B, Ls, C, o, h, f.start_w, f.start_b, p.x[0], p.xp,
-                                                         status);
-    FS2_LAUNCH_CHECK();
-    int cur = 0, sk = 0;
-    for (int i = 0; i < kLayers; ++i) {
-      if ((rc = vweight_gemm(m->math_mode, f.cond[i], cond_a, B, Ls, ACT_NONE, p.lensS, p.cd, st))) return rc;
-      const void* xa = planes ? (const void*)p.xp : (const void*)p.x[cur];
-      if ((rc = vweight_gemm(m->math_mode, f.in[i], xa, B, Ls, ACT_NONE, p.lensS, p.ia, st, p.cd, 1 << i))) return rc;
-      // layer i's input x is exact at exact + 2^i - 1, its in-layer output (and so acts and the next x) at exact + 2^(i+1) - 1
-      gate<<<grid_for(rows * (C / 4), 256), 256, 0, st>>>(p.ia, planes && i > 0 ? p.x[cur] : nullptr, p.lensS, win, exact + (2 << i) - 1,
-                                                           exact + (1 << i) - 1, B, Ls, C, (float*)p.acts, (__half*)p.acts, status);
-      FS2_LAUNCH_CHECK();
-      if (i < kLayers - 1) {
-        if ((rc = vweight_gemm(m->math_mode, f.res[i], p.acts, B, Ls, ACT_NONE, p.lensS, p.x[cur ^ 1], st, p.x[cur], 1, p.xp))) return rc;
-        cur ^= 1;
-      }
-      if ((rc = vweight_gemm(m->math_mode, f.skip[i], p.acts, B, Ls, ACT_NONE, p.lensS, p.skip[sk ^ 1], st, i ? p.skip[sk] : nullptr))) return rc;
-      sk ^= 1;
-    }
-    float* dst = k == 0 && !window ? audio : p.state;
-    rc = h == 4 ? launch_flow(wg_flow_kernel<4>, c, C, p.skip[sk], p.state, dst, p.lensS, B, Ls, o, f, st)
-       : h == 3 ? launch_flow(wg_flow_kernel<3>, c, C, p.skip[sk], p.state, dst, p.lensS, B, Ls, o, f, st)
-                : launch_flow(wg_flow_kernel<2>, c, C, p.skip[sk], p.state, dst, p.lensS, B, Ls, o, f, st);
-    if (rc) return rc;
-  }
+  const void* cond_a = nullptr;
+  if ((rc = upsample(m, p, mels, B, L, Lmax, status, st, &cond_a))) return rc;
+  for (int k = kFlows - 1; k >= 0; --k)
+    if ((rc = flow(m, k, p, cond_a, p.state, k == 0 && !window ? audio : p.state, B, Ls, status, st))) return rc;
   if (window) {
     wg_win_audio_kernel<<<grid_for((long)B * nf * kHop, 256), 256, 0, st>>>(p.state, p.win, B, Ls, nf, audio, ld);
     FS2_LAUNCH_CHECK();
@@ -669,6 +708,93 @@ int fs2_waveglow_window(fs2_waveglow_net* m, const float* mels, const int64_t* o
   if ((rc = b.check("fs2_waveglow_window"))) return rc;
   FS2_REQUIRE(m->loaded, "fs2_waveglow_window: weights not loaded (fs2_waveglow_load)");
   return run(m, p, mels, olens, starts, B, Lmax, n_frames, sigma, seeds, z, audio, (long)audio_ld, status, (cudaStream_t)stream);
+}
+
+// ---- stages of the inverse on the vocoder's own code paths (tests) --------------------------------------------------
+// Both run what fs2_waveglow runs for that stage, on a loaded handle's packed weights, with the buffers in a stream-ordered
+// temporary.  The length pass is wg_prep_kernel's with 0 allowed: a length outside [0, L] is 0 and sets
+// FS2_WAVEGLOW_BAD_LENGTH, so it never becomes an out-of-bounds row.
+int fs2_op_waveglow_upsample(fs2_waveglow_net* m, const float* mels, const int64_t* olens, int B, int Lmax, float* cond,
+                             float* cond_planes, int* status, void* stream) {
+  const char* who = "fs2_op_waveglow_upsample";
+  // the checks that need no handle first, so that each refusal names its own cause
+  FS2_REQUIRE(mels && olens && cond && status, "%s: null argument", who);
+  FS2_REQUIRE(B >= 1 && Lmax >= 1, "%s: need B >= 1 and Lmax >= 1 (got %d, %d)", who, B, Lmax);
+  FS2_REQUIRE(aligned16(mels) && aligned16(cond) && aligned16(cond_planes), "%s: mels, cond and cond_planes must be 16-byte aligned", who);
+  FS2_REQUIRE(m && m->loaded, "%s: null or unloaded handle (fs2_waveglow_load)", who);
+  const bool planes = plane_mode(m->math_mode);
+  FS2_REQUIRE(!cond_planes || planes, "%s: cond_planes needs FS2_MATH_F16 or FS2_MATH_3XTF32", who);
+  int rc = check_rows(who, "B * Lmax * 32", "step", (long)B * Lmax * kSteps, m->math_mode);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long rows = (long)B * Lmax * kSteps;
+  WgPlan p{};
+  void* base = nullptr;
+  if ((rc = temp_carve(&base, st, [&](Bump& b) {
+         p.lensF = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
+         p.lensS = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
+         p.up_a = b.floats((size_t)B * Lmax * kUpK);
+         p.condp = planes ? (__half*)b.floats((size_t)rows * kCond) : nullptr;   // hi + lo planes
+       })))
+    return rc;
+  p.cond = cond;
+  auto enqueue = [&]() -> int {      // every error returns here, so that the temporary is released on every path
+    wg_prep_kernel<<<1, 256, 0, st>>>(olens, B, Lmax, 0, p.lensF, p.lensS, status);
+    FS2_LAUNCH_CHECK();
+    // the planes of rows past lens are never written: zeros there (and in f16's unused lo plane) read back as +0
+    if (planes) FS2_CUDA_CHECK(cudaMemsetAsync(p.condp, 0, (size_t)rows * kCond * sizeof(float), st));
+    const void* cond_a = nullptr;
+    int r = upsample(m, p, mels, B, Lmax, Lmax, status, st, &cond_a);
+    if (!r && cond_planes) r = planes_to_rows(p.condp, rows * kCond, cond_planes, st);
+    return r;
+  };
+  rc = enqueue();
+  cudaFreeAsync(base, st);
+  return rc;
+}
+
+int fs2_op_waveglow_flow(fs2_waveglow_net* m, int k, const float* cond, const float* skip_in, const float* state_in, float* state_out,
+                         const int64_t* lens, int B, int Ls, float* wn_out, int* status, void* stream) {
+  const char* who = "fs2_op_waveglow_flow";
+  // the checks that need no handle first, so that each refusal names its own cause
+  FS2_REQUIRE(state_in && state_out && lens && status && (skip_in || cond), "%s: null argument", who);
+  FS2_REQUIRE(!(skip_in && wn_out), "%s: wn_out needs the WN to run (skip_in NULL)", who);
+  FS2_REQUIRE(k >= 0 && k < kFlows, "%s: flow k must lie in [0, %d) (got %d)", who, kFlows, k);
+  FS2_REQUIRE(B >= 1 && Ls >= 1, "%s: need B >= 1 and Ls >= 1 (got %d, %d)", who, B, Ls);
+  FS2_REQUIRE(aligned16(cond) && aligned16(skip_in) && aligned16(state_in) && aligned16(state_out) && aligned16(wn_out),
+              "%s: cond, skip_in, state_in, state_out and wn_out must be 16-byte aligned", who);
+  FS2_REQUIRE(m && m->loaded, "%s: null or unloaded handle (fs2_waveglow_load)", who);
+  int rc = check_rows(who, "B * Ls", "step", (long)B * Ls, m->math_mode);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool planes = plane_mode(m->math_mode);
+  const long rows = (long)B * Ls;
+  WgPlan p{};
+  void* base = nullptr;
+  if ((rc = temp_carve(&base, st, [&](Bump& b) {
+         p.lensS = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
+         if (!skip_in) plan_wn(b, p, planes, m->C, (size_t)rows);
+       })))
+    return rc;
+  auto enqueue = [&]() -> int {      // every error returns here, so that the temporary is released on every path
+    wg_prep_kernel<<<1, 256, 0, st>>>(lens, B, Ls, 0, p.lensS, nullptr, status);
+    FS2_LAUNCH_CHECK();
+    if (skip_in) return flow_tail(m, k, skip_in, state_in, state_out, p.lensS, B, Ls, st);
+    const void* cond_a = cond;
+    if (planes) {     // the cond planes with the range check, as the vocoder's upsampling writes them
+      auto kp = out_kind(m->math_mode) == OUT_HILO ? wg_planes_kernel<OUT_HILO> : wg_planes_kernel<OUT_HI>;
+      kp<<<grid_for(rows * (kCond / 4), 256), 256, 0, st>>>(cond, p.lensS, B, Ls, kCond, p.condp, status);
+      FS2_LAUNCH_CHECK();
+      cond_a = p.condp;
+    }
+    const float* wn = nullptr;
+    int r = flow(m, k, p, cond_a, state_in, state_out, B, Ls, status, st, &wn);
+    if (!r && wn_out) FS2_CUDA_CHECK(cudaMemcpyAsync(wn_out, wn, (size_t)rows * m->C * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return r;
+  };
+  rc = enqueue();
+  cudaFreeAsync(base, st);
+  return rc;
 }
 
 }  // extern "C"

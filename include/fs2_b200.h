@@ -802,6 +802,26 @@ int fs2_waveglow_window(fs2_waveglow_net* m, const float* mels, const int64_t* o
 /* the standard-normal draw a seeded fs2_waveglow call uses: z [B, 8, Lmax * 32], 0 at steps t >= olens[b] * 32.  Element
  * (b, ch, t) is Box-Muller on Philox4x32-10(counter (t, ch / 4, 0, 0), key (seeds[b] mod 2^32, seeds[b] / 2^32)). */
 int fs2_waveglow_noise(const int64_t* seeds, const int64_t* olens, int B, int Lmax, float* z, void* stream);
+/* Stages of the inverse on fs2_waveglow's code paths (per-stage tests), on a loaded handle's packed weights, buffers in a
+ * stream-ordered temporary; no synchronisation.  Lengths (device int64 [B]) outside [0, L] count as 0 and set
+ * FS2_WAVEGLOW_BAD_LENGTH in *status (device int, written by the call; FS2_WAVEGLOW_RANGE as fs2_waveglow's).  Float
+ * pointers 16-byte aligned.  A null or unloaded handle, B or L < 1, misaligned pointers and fs2_waveglow's row limits on
+ * B * L step rows are FS2_ERR_INVALID before anything is enqueued.
+ * fs2_op_waveglow_upsample: the upsampling of mels [B, Lmax, 80] with frame counts olens into cond [B * Lmax * 32][640]
+ *   fp32, the rows the cond GEMMs read (+0 at steps t >= olens[b] * 32; frames past olens[b] are never read).
+ *   cond_planes (nullable, FS2_MATH_F16 / FS2_MATH_3XTF32 only): the same rows as the GEMMs' operand planes read back as
+ *   fp32, (hi + lo) / 16 (hi / 16 in FS2_MATH_F16), +0 past the steps.
+ * fs2_op_waveglow_flow: flow k (0 .. 11, c = 8, 8, 8, 8, 6, 6, 6, 6, 4, 4, 4, 4 channels) of the inverse on the state
+ *   [B * Ls][8] (utterance b its rows t < lens[b], in steps; any Ls >= 1): WN k on cond [B * Ls][640] fp32 rows (their
+ *   planes written with the range check in the plane modes), then end, the affine coupling and the inverse 1x1 conv from
+ *   columns 8 - c .. 7 of state_in into those of state_out (== state_in, or disjoint from it).  Only those columns are
+ *   written, +0 at rows t >= lens[b]; rows past lens[b] of state_in, cond and skip_in are never read.  wn_out [B * Ls][C]
+ *   (nullable): WN's skip sum before end.  skip_in [B * Ls][C] (nullable): the WN is not run, and the flow's tail runs on
+ *   skip_in in its place (cond is then not read and may be NULL; wn_out must be NULL). */
+int fs2_op_waveglow_upsample(fs2_waveglow_net* m, const float* mels, const int64_t* olens, int B, int Lmax, float* cond,
+                             float* cond_planes, int* status, void* stream);
+int fs2_op_waveglow_flow(fs2_waveglow_net* m, int k, const float* cond, const float* skip_in, const float* state_in, float* state_out,
+                         const int64_t* lens, int B, int Ls, float* wn_out, int* status, void* stream);
 
 /* ---- multi-GPU exchange step: gather of the final mel shards on one rank over NVLink peer memory ----------------- */
 /* Replaces what a reference user would write as torch.distributed.gather / all_gather of `after_outs` (the reference has

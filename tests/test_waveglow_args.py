@@ -15,7 +15,7 @@ import torch
 from conftest import GOLDEN, REPO
 from fastspeech2_b200 import _lib
 from fastspeech2_b200 import dropin_run
-from fastspeech2_b200.waveglow import WaveGlowVocoder
+from fastspeech2_b200.waveglow import WaveGlowVocoder, flow_channels
 from oracle import waveglow_oracle as O
 
 
@@ -294,7 +294,7 @@ def test_library_exports_waveglow_entry_points():
     lib = _lib.load()
     header = open(os.path.join(REPO, "include", "fs2_b200.h")).read()
     for name in ("fs2_waveglow_create", "fs2_waveglow_load", "fs2_waveglow_workspace_bytes", "fs2_waveglow", "fs2_waveglow_noise",
-                 "fs2_op_tap_gemm_dil"):
+                 "fs2_op_tap_gemm_dil", "fs2_op_waveglow_upsample", "fs2_op_waveglow_flow"):
         assert hasattr(lib, name) and name in _lib.SIGNATURES, name
         assert f"int {name}(" in header, name
     assert hasattr(lib, "fs2_waveglow_destroy") and "void fs2_waveglow_destroy(" in header
@@ -314,3 +314,66 @@ def test_waveglow_kernels_do_not_spill():
         assert len(props) == n, (kernel, len(props))
         for line in props:
             assert "0 bytes spill stores, 0 bytes spill loads" in line, (kernel, line)
+
+
+# ---- the per-stage entries (tests/test_gpu_waveglow_kernels.py) ----------------------------------------------------
+def _flow(k=0, cond=256, skip=None, state_in=256, state_out=256, lens=256, B=2, Ls=40, wn=None, status=256, h=None):
+    return _lib.load().fs2_op_waveglow_flow(h, k, cond, skip, state_in, state_out, lens, B, Ls, wn, status, None)
+
+
+def _upsample(mels=256, olens=256, B=2, Lmax=5, cond=256, planes=None, status=256, h=None):
+    return _lib.load().fs2_op_waveglow_upsample(h, mels, olens, B, Lmax, cond, planes, status, None)
+
+
+@pytest.mark.parametrize("kw,match", [
+    (dict(state_in=None), "null argument"), (dict(state_out=None), "null argument"), (dict(lens=None), "null argument"),
+    (dict(status=None), "null argument"), (dict(cond=None), "null argument"),
+    (dict(skip=256, wn=512), "wn_out needs the WN"),
+    (dict(k=-1), "flow k"), (dict(k=12), "flow k"),
+    (dict(B=0), "B >= 1 and Ls >= 1"), (dict(Ls=0), "B >= 1 and Ls >= 1"), (dict(Ls=-3), "B >= 1 and Ls >= 1"),
+    (dict(cond=260), "16-byte aligned"), (dict(skip=264, cond=None), "16-byte aligned"), (dict(state_in=257), "16-byte aligned"),
+    (dict(state_out=260), "16-byte aligned"), (dict(wn=268), "16-byte aligned"),
+    ({}, "null or unloaded handle"), (dict(skip=256, cond=None), "null or unloaded handle")])
+def test_flow_entry_refuses_on_the_host(kw, match):
+    """fs2_op_waveglow_flow refuses these before it touches memory (the pointers are never dereferenced); the checks that
+    need no handle run first, so each refusal names its own cause.  An unloaded handle and the row limits are checked on
+    the GPU (test_gpu_waveglow_kernels.test_refusals_that_need_a_handle)."""
+    assert _flow(**kw) == -1
+    assert match.encode() in _lib.load().fs2_last_error()
+
+
+@pytest.mark.parametrize("kw,match", [
+    (dict(mels=None), "null argument"), (dict(olens=None), "null argument"), (dict(cond=None), "null argument"),
+    (dict(status=None), "null argument"), (dict(B=0), "B >= 1 and Lmax >= 1"), (dict(Lmax=0), "B >= 1 and Lmax >= 1"),
+    (dict(mels=264), "16-byte aligned"), (dict(cond=260), "16-byte aligned"), (dict(planes=258), "16-byte aligned"),
+    ({}, "null or unloaded handle")])
+def test_upsample_entry_refuses_on_the_host(kw, match):
+    assert _upsample(**kw) == -1
+    assert match.encode() in _lib.load().fs2_last_error()
+
+
+def test_gpu_case_table_covers_the_tile_widths_flow_widths_and_lengths():
+    """What the per-stage GPU cases reach, restated from the tap GEMM's schedule (tests/test_gpu_tap_gemm.py): res / skip
+    GEMMs (N = C) on 64-, 80- and 128-wide tiles, every flow width, an utterance shorter than each dilation 2^i and not
+    shorter than 2^(i-1), the lengths around one and two row tiles, Ls off the 128-row grid, and a case whose in-layer
+    GEMM has more than 2 x 132 row tiles."""
+    from test_gpu_tap_gemm import H100_SMS, tile_coords, tile_width, tiling
+    import test_gpu_waveglow_kernels as K
+    assert {tile_width(C) for C in K.WN_CS} == {64, 80, 128}        # the whole-flow cases run the GEMMs
+    assert [tile_width(C) for C in K.WN_CS] == [64, 64, 128, 80, 128, 128]
+    assert set(K.WN_CS) <= set(K.TAIL_CS) and {448, 960} <= set(K.TAIL_CS)   # wg_flow_kernel alone at more widths
+    assert 1024 in K.WN_CS and 1024 in K.TAIL_CS                    # wg_flow_kernel's largest shared memory
+    assert all(C % 64 == 0 and 64 <= C <= 1024 for C in K.WN_CS + K.TAIL_CS)
+    assert {flow_channels(k) for k in K.FLOWS} == {4, 6, 8} and O.flow_channels(11) == 4
+    assert {0, 1, 31, 127, 128, 129, 255, 257} <= set(K.LENS) and max(K.LENS) <= K.LS
+    for i in range(1, 8):                                             # dilations 2 .. 128
+        assert any(2 ** (i - 1) <= n < 2 ** i for n in K.LENS), i
+    assert K.LS % 128 != 0
+    B, Ls = K.BIG
+    assert len(K.BIG_LENS) == B and max(K.BIG_LENS) <= Ls
+    t = tiling(B, Ls, 2 * 256, 3, True)                               # the in-layer GEMM of the big case (C = 256)
+    assert t.m_tiles == 3 * 94 and not t.packed
+    live = [mt for mt in range(t.m_tiles) if not tile_coords(t, mt * t.n_tiles, K.BIG_LENS)[3]]
+    assert len(live) == 94 + 93 + 86 > 2 * H100_SMS                   # live row tiles, not only walked ones
+    assert tiling(len(K.LENS), K.LS, 256, 3, True).packed            # the 44-row tails share packed tiles
+    assert min(K.UP_OLENS) == 0 and {1, 2, 3} <= set(K.UP_OLENS)
