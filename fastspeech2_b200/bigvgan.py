@@ -18,16 +18,15 @@ checkpoint file.
 from __future__ import annotations
 
 import ctypes as C
-import json
 import math
-import os
 
 import torch
 import torch.nn as nn
 
 from . import _lib
-from ._kernel_module import HOP, N_MELS, NeuralVocoder, _WNConv, normalise_checkpoint, read_checkpoint, ups_window_plan
-from .hifigan import c_config, check_rates, check_resblocks, check_widths
+from ._kernel_module import HOP, N_MELS, _WNConv  # noqa: F401
+from . import hifigan
+from .hifigan import _Generator, c_config, check_rates, check_resblocks, check_widths
 
 ACT_REACH = 5                    # Activation1d's reach: output row t reads input rows t - 5 .. t + 5
 FILTER_TAPS = 12
@@ -41,33 +40,14 @@ CONFIGS = {
     "v2_22khz_80band_fmax8k_256x": dict(_22K, upsample_rates=[4, 4, 2, 2, 2, 2], upsample_kernel_sizes=[8, 8, 4, 4, 4, 4],
                                         upsample_initial_channel=1536, use_tanh_at_final=False, use_bias_at_final=False),
 }
-_FIELDS = ("resblock", "upsample_rates", "upsample_kernel_sizes", "upsample_initial_channel", "resblock_kernel_sizes",
-           "resblock_dilation_sizes", "activation", "snake_logscale")
 
 
 def load_config(config) -> dict:
     """A BigVGAN config as a dict of the fields the generator uses: from a name of CONFIGS, a dict (e.g. a loaded
     config.json) or the path of a config.json.  Only its form is checked here; `check_config` checks what this library
     runs."""
-    if isinstance(config, str) and config.lower() in CONFIGS:
-        config = CONFIGS[config.lower()]
-    elif isinstance(config, (str, os.PathLike)):
-        with open(config) as f:
-            config = json.load(f)
-    if not isinstance(config, dict):
-        raise ValueError(f"config must be one of {sorted(CONFIGS)}, a dict or the path of a BigVGAN config.json")
-    for k in _FIELDS:
-        if k not in config:
-            raise ValueError(f"config: missing field {k}")
-    out = {"resblock": str(config["resblock"]), "upsample_initial_channel": config["upsample_initial_channel"],
-           "activation": config["activation"], "snake_logscale": config["snake_logscale"],
-           "use_tanh_at_final": config.get("use_tanh_at_final", True), "use_bias_at_final": config.get("use_bias_at_final", True)}
-    for k in ("upsample_rates", "upsample_kernel_sizes", "resblock_kernel_sizes"):
-        out[k] = [v for v in config[k]]
-    out["resblock_dilation_sizes"] = [list(d) for d in config["resblock_dilation_sizes"]]
-    if "num_mels" in config:
-        out["num_mels"] = config["num_mels"]
-    return out
+    return hifigan.load_config(config, CONFIGS, f"one of {sorted(CONFIGS)}", "a BigVGAN", fields=("activation", "snake_logscale"),
+                               defaults={"use_tanh_at_final": True, "use_bias_at_final": True})
 
 
 def check_config(cfg: dict) -> None:
@@ -150,7 +130,7 @@ def add_layers(module: nn.Module, cfg: dict) -> nn.Module:
     return module
 
 
-class BigVGANVocoder(NeuralVocoder):
+class BigVGANVocoder(_Generator):
     """NVIDIA BigVGAN's generator on the H100 kernels.
 
     `forward(mels [B, Lmax, 80], olens [B])` -> (audio [B, Lmax * 256] fp32, alens = olens * 256).  Utterance b is the
@@ -162,6 +142,8 @@ class BigVGANVocoder(NeuralVocoder):
     `forward(chunk_frames=)` give the same audio in windows of frames."""
 
     _NAME = "bigvgan"
+    _ACT_REACH = ACT_REACH
+    _ACT_FLOP = 2 * 6 + FILTER_TAPS        # per channel and input row: 2 x 6 taps up, 12 taps down; the Snake itself not counted
 
     def __init__(self, config="base_22khz_80band", math_mode: str = "3xf16"):
         super().__init__(math_mode)
@@ -171,67 +153,6 @@ class BigVGANVocoder(NeuralVocoder):
         add_layers(self, cfg)
         self._layers = [m for m in self.modules() if isinstance(m, _WNConv)]           # state_dict order
         self._acts = [m for m in self.modules() if isinstance(m, _Activation1d)]      # state_dict order, activation_post last
-
-    def launches(self) -> int:
-        """Kernels one call enqueues: 4 + U * (2 + K * G + max(K - 2, 0)), G = 12 (AMPBlock1) or 4 (AMPBlock2)."""
-        U, K = len(self.config["upsample_rates"]), len(self.config["resblock_kernel_sizes"])
-        G = 12 if self.config["resblock"] == "1" else 4
-        return 4 + U * (2 + K * G + max(K - 2, 0))
-
-    def window_plan(self) -> dict:
-        """The window plan of this config, walking back from the audio: conv_post reads 3 rows of activation_post's output
-        and that 5 more, each MRF R = its largest block's reach with its activations, upsampling s reads `reach[s]` input
-        rows around its core, and conv_pre 3 frames more.  -> {"reach": [r_s], "halo": [h_s], "R": R}."""
-        return ups_window_plan(*self._chain())
-
-    def _chain(self):
-        """The upsample rates; R = the largest block's reach (AMPBlock1 sum_m ((k-1)/2 (d_m + 1) + 2 a), AMPBlock2
-        sum_m ((k-1)/2 d_m + a), a = 5); level-0 margin 3; last-layer reach 3 + a."""
-        cfg = self.config
-        one = cfg["resblock"] == "1"
-        steps = 3 if one else 2
-        R = max(sum((k - 1) // 2 * (d + one) + (2 if one else 1) * ACT_REACH for d in dil[:steps])
-                for k, dil in zip(cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"]))
-        return cfg["upsample_rates"], R, 3, 3 + ACT_REACH
-
-    def flops_per_frame(self) -> int:
-        """FLOP per mel frame: multiply-adds x 2 of the generator's convolutions (the transposed ones counted as torch runs
-        them: Cin * Cout * k per input row) and of the activations' two 12-tap filters (per channel and input row: 2 x 6
-        taps up, 12 taps down); the Snake itself is not counted."""
-        cfg = self.config
-        c0, f = cfg["upsample_initial_channel"], 0
-        f += N_MELS * c0 * 7
-        up = 1
-        one = cfg["resblock"] == "1"
-        convs, acts = (6, 6) if one else (2, 2)
-        act = 2 * 6 + FILTER_TAPS
-        for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
-            cin, cout = c0 // 2 ** i, c0 // 2 ** (i + 1)
-            f += up * cin * cout * k
-            up *= u
-            f += up * sum(convs * cout * cout * kk + acts * cout * act for kk in cfg["resblock_kernel_sizes"])
-        cl = c0 // 2 ** len(cfg["upsample_rates"])
-        f += up * cl * (act + 7)
-        return 2 * f
-
-    # ---- checkpoints ----------------------------------------------------------------------------------------------
-    @classmethod
-    def from_checkpoint(cls, path_or_dict, config=None, math_mode: str = "3xf16") -> "BigVGANVocoder":
-        """A BigVGAN generator checkpoint (`bigvgan_generator.pt`: a dict with "generator") or a bare generator state dict,
-        given as a file path or as the loaded dict.  Either may hold `weight_g` / `weight_v` keys or plain `weight` keys.
-        config: as in the constructor; None reads config.json beside a checkpoint path.  The filters are the checkpoint's
-        own.  A missing, unexpected or wrongly shaped key raises ValueError naming it."""
-        sd = path_or_dict
-        if config is None:
-            if not isinstance(sd, (str, os.PathLike)):
-                raise ValueError("config is required when the checkpoint is given as a dict")
-            path = os.path.join(os.path.dirname(os.path.abspath(sd)), "config.json")
-            if not os.path.exists(path):
-                raise ValueError(f"config is required: no config.json beside {sd}")
-            config = path
-        voc = cls(config, math_mode=math_mode)
-        voc.load_state_dict(normalise_checkpoint(voc, read_checkpoint(sd, "generator", "a generator state dict")))
-        return voc
 
     # ---- device state ---------------------------------------------------------------------------------------------
     def _fingerprint(self):
@@ -247,12 +168,6 @@ class BigVGANVocoder(NeuralVocoder):
         c.use_bias_at_final = int(cfg["use_bias_at_final"])
         return c
 
-    def _create(self):
-        h = C.c_void_p()
-        cfg = self._c_config()
-        _lib.check(_lib.load().fs2_bigvgan_create(C.byref(h), _lib.MATH_MODES[self.math_mode], C.byref(cfg)), "fs2_bigvgan_create")
-        return h.value
-
     def _load(self, h, device: torch.device) -> None:
         def dev(t):
             return None if t is None else t.detach().float().reshape(-1).to(device).contiguous()
@@ -263,7 +178,3 @@ class BigVGANVocoder(NeuralVocoder):
         def ptrs(ts):
             return (C.c_void_p * len(ts))(*[None if t is None else t.data_ptr() for t in ts])
         _lib.check(_lib.load().fs2_bigvgan_load(h, ptrs(ws), ptrs(bs), ptrs(acts), _lib.stream_ptr(device)), "fs2_bigvgan_load")
-
-    def _rows(self, B: int, L: int):
-        """fs2_bigvgan's largest buffer: B * Lmax * 256 sample rows."""
-        return B * L * HOP, f"B * Lmax * {HOP}", "sample"

@@ -46,6 +46,17 @@ __global__ void conv_bias_kernel(const float* __restrict__ b, const float* __res
   for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < N; n += gridDim.x * blockDim.x) dst[n] = b2 ? b[n % Cout] + b2[n] : b[n % Cout];
 }
 
+// dst [A'][B'][k] = src [A][B][k] zero-padded (a torch-layout convolution weight, or with B = k = 1 a bias, or with
+// k = 1 rows of a [rows][B] matrix; A' <= A or B' <= B crops)
+__global__ void pad3_kernel(const float* __restrict__ src, int A, int Bn, int k, float* __restrict__ dst, int Ap, int Bp) {
+  const long total = (long)Ap * Bp * k;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const long ab = i / k;
+    const int j = (int)(i - ab * k), a = (int)(ab / Bp), bb = (int)(ab - (long)a * Bp);
+    dst[i] = a < A && bb < Bn ? src[((long)a * Bn + bb) * k + j] : 0.f;
+  }
+}
+
 }  // namespace
 
 void vweight_carve(Bump& b, VWeight& w, bool bias) {
@@ -81,6 +92,12 @@ int vweight_pack_conv(const VWeight& w, const float* wt, const float* b, int Cin
   conv_bias_kernel<<<grid_for(w.N, 256), 256, 0, st>>>(b, b2, w.N, Cout, w.bias);
   FS2_LAUNCH_CHECK();
   return vweight_planes(w, st);
+}
+
+int pad3(const float* src, int A, int Bn, int k, float* dst, int Ap, int Bp, cudaStream_t st) {
+  pad3_kernel<<<grid_for((long)Ap * Bp * k, 256), 256, 0, st>>>(src, A, Bn, k, dst, Ap, Bp);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
 }
 
 TapGemm vweight_gemm_args(int math_mode, const VWeight& w, const void* a, int B, int L, int act, const int64_t* lens,

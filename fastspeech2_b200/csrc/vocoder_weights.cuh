@@ -1,5 +1,5 @@
 // The library's GEMM weights (the acoustic model in api.cu, the train convolutions in train.cu and the signal modules
-// melgan.cu, hifigan.cu, waveglow.cu, griffin_lim.cu, features.cu): one [taps][N][K] matrix held as fp32 rows (fp32 / tf32 math modes)
+// melgan.cu, hifigan.cu, bigvgan.cu, waveglow.cu, griffin_lim.cu, features.cu): one [taps][N][K] matrix held as fp32 rows (fp32 / tf32 math modes)
 // and as power-of-two-scaled fp16 hi / lo planes (f16 / 3xF16), with an optional bias [N]; the tap-GEMM call over it, the
 // one place that maps a math mode to a tap-GEMM family; and the device arena a module's weights are carved from.
 #pragma once
@@ -33,6 +33,10 @@ int conv_pack(const float* wt, int N, int Cin, int taps, int Cout, int u, long t
 // [Cin, 2 Cin) and its bias added, so that one GEMM over [x | y] computes wt . x + wt2 . y.
 int vweight_pack_conv(const VWeight& w, const float* wt, const float* b, int Cin, int Cout, int taps, int u, long tap_stride, cudaStream_t st,
                       const float* wt2 = nullptr, const float* b2 = nullptr);
+
+// dst [A'][B'][k] = src [A][B][k] zero-padded (a torch-layout convolution weight, or with B = k = 1 a bias, or with k = 1
+// rows of a [rows][B] matrix; A' <= A or B' <= B crops)
+int pad3(const float* src, int A, int Bn, int k, float* dst, int Ap, int Bp, cudaStream_t st);
 
 // The TapGemm of out [B*L][w.N] = act(a [B*L][w.K] (w.taps taps at dilation dil) . w^T + w.bias) (+ resid [B*L][w.N]), a as
 // fp32 rows (fp32 / tf32) or as hi (+ lo) planes (f16 / 3xF16); rows t >= lens[b] are written as 0 (and skipped by the

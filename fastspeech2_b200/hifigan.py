@@ -37,26 +37,38 @@ _FIELDS = ("resblock", "upsample_rates", "upsample_kernel_sizes", "upsample_init
            "resblock_dilation_sizes")
 
 
-def load_config(config) -> dict:
+def load_config(config, configs=None, choices: str = "'v1', 'v2', 'v3'", what: str = "a hifi-gan", fields=(), defaults=None,
+                own=(), own_note: str = "") -> dict:
     """A hifi-gan config as a dict of the fields the generator uses: from "v1" / "v2" / "v3", a dict (e.g. a loaded
     config.json) or the path of a config.json.  Only its form is checked here; `check_config` checks what this library
-    runs."""
-    if isinstance(config, str) and config.lower() in CONFIGS:
-        config = CONFIGS[config.lower()]
+    runs.
+
+    BigVGAN's and iSTFTNet's load_config are this one on their own configs (a name of `configs`, refused as "config must
+    be <choices>, a dict or the path of <what> config.json"), with more fields: `own`, required before hifi-gan's
+    (missing: "config: missing field <k><own_note>"); `fields`, required after them; `defaults`, optional with defaults."""
+    configs = CONFIGS if configs is None else configs
+    if isinstance(config, str) and config.lower() in configs:
+        config = configs[config.lower()]
     elif isinstance(config, (str, os.PathLike)):
         with open(config) as f:
             config = json.load(f)
     if not isinstance(config, dict):
-        raise ValueError("config must be 'v1', 'v2', 'v3', a dict or the path of a hifi-gan config.json")
-    for k in _FIELDS:
+        raise ValueError(f"config must be {choices}, a dict or the path of {what} config.json")
+    for k in own:
+        if k not in config:
+            raise ValueError(f"config: missing field {k}{own_note}")
+    for k in _FIELDS + tuple(fields):
         if k not in config:
             raise ValueError(f"config: missing field {k}")
     out = {"resblock": str(config["resblock"]), "upsample_initial_channel": config["upsample_initial_channel"]}
+    out.update({k: config[k] for k in fields})
+    out.update({k: config.get(k, v) for k, v in (defaults or {}).items()})
     for k in ("upsample_rates", "upsample_kernel_sizes", "resblock_kernel_sizes"):
         out[k] = [v for v in config[k]]
     out["resblock_dilation_sizes"] = [list(d) for d in config["resblock_dilation_sizes"]]
     if "num_mels" in config:
         out["num_mels"] = config["num_mels"]
+    out.update({k: config[k] for k in own})
     return out
 
 
@@ -167,7 +179,94 @@ def add_layers(module: nn.Module, cfg: dict, post_channels: int = 1) -> nn.Modul
     return module
 
 
-class HiFiGANVocoder(NeuralVocoder):
+class _Generator(NeuralVocoder):
+    """What HiFiGANVocoder, BigVGANVocoder and ISTFTNetVocoder share: hifi-gan's generator chain (csrc/hifigan.cu) with
+    the activation before its block convolutions reaching _ACT_REACH rows on each side (lrelu: 0) and costing _ACT_FLOP
+    multiply-adds per channel and row (lrelu: 0).  A subclass sets self.config and self._layers and provides _c_config()."""
+
+    _ACT_REACH = 0
+    _ACT_FLOP = 0
+
+    def launches(self) -> int:
+        """Kernels one call enqueues: 4 + U * (2 + K * G + max(K - 2, 0)), G = 12 (resblock "1") or 4 (resblock "2")."""
+        U, K = len(self.config["upsample_rates"]), len(self.config["resblock_kernel_sizes"])
+        G = 12 if self.config["resblock"] == "1" else 4
+        return 4 + U * (2 + K * G + max(K - 2, 0))
+
+    def window_plan(self) -> dict:
+        """The window plan of this config (DESIGN.md section 17), walking back from the audio: the head reads its reach
+        (conv_post: 3 rows on each side) of the last level, each MRF R = its largest resblock's reach, upsampling s reads
+        `reach[s]` input rows around its core, and conv_pre 3 frames more.  -> {"reach": [r_s], "halo": [h_s] (rows of
+        level s on each side of its core; h_0 = r_0 + 3 mel frames, h_{s+1} = u_s r_s), "R": R}."""
+        return ups_window_plan(*self._chain())
+
+    def _chain(self):
+        """The upsample rates; R = the largest resblock's reach, its activations' included (ResBlock1 sum_m ((k-1)/2
+        (d_m + 1) + 2 a), ResBlock2 sum_m ((k-1)/2 d_m + a), a = _ACT_REACH); conv_pre's native taps leave its 3 outer rows
+        wrong at a window side that is not an utterance edge; the last layer's reach."""
+        cfg, a = self.config, self._ACT_REACH
+        one = cfg["resblock"] == "1"
+        steps = 3 if one else 2
+        R = max(sum((k - 1) // 2 * (d + one) + (2 if one else 1) * a for d in dil[:steps])
+                for k, dil in zip(cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"]))
+        return cfg["upsample_rates"], R, 3, self._post_reach()
+
+    def _post_reach(self) -> int:
+        """Last-level rows the head reads on each side: conv_post's 3, through its activation's reach."""
+        return 3 + self._ACT_REACH
+
+    def flops_per_frame(self) -> int:
+        """FLOP per mel frame: multiply-adds x 2 of the generator's convolutions (the transposed ones counted as torch runs
+        them: Cin * Cout * k per input row) and of its activations (_ACT_FLOP per channel and input row)."""
+        cfg = self.config
+        c0, f = cfg["upsample_initial_channel"], 0
+        f += N_MELS * c0 * 7
+        up = 1
+        convs = 6 if cfg["resblock"] == "1" else 2
+        act = self._ACT_FLOP
+        for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
+            cin, cout = c0 // 2 ** i, c0 // 2 ** (i + 1)
+            f += up * cin * cout * k
+            up *= u
+            f += up * sum(convs * cout * cout * kk + convs * cout * act for kk in cfg["resblock_kernel_sizes"])
+        f += up * (c0 // 2 ** len(cfg["upsample_rates"])) * (act + 7)
+        return 2 * f
+
+    # ---- checkpoints ----------------------------------------------------------------------------------------------
+    @classmethod
+    def from_checkpoint(cls, path_or_dict, config=None, math_mode: str = "3xf16"):
+        """A generator checkpoint (hifi-gan's and iSTFTNet's `g_XXXXXXXX`, BigVGAN's `bigvgan_generator.pt`: a dict with
+        "generator") or a bare generator state dict, given as a file path or as the loaded dict.  Either may hold
+        `weight_g` / `weight_v` keys or plain `weight` keys (after `remove_weight_norm`); BigVGAN's filters are the
+        checkpoint's own.  config: as in the constructor; None reads config.json beside a checkpoint path, as hifi-gan's
+        inference.py does (the dilations cannot be read from the weights).  A missing, unexpected or wrongly shaped key
+        raises ValueError naming it."""
+        sd = path_or_dict
+        if config is None:
+            if not isinstance(sd, (str, os.PathLike)):
+                raise ValueError("config is required when the checkpoint is given as a dict")
+            path = os.path.join(os.path.dirname(os.path.abspath(sd)), "config.json")
+            if not os.path.exists(path):
+                raise ValueError(f"config is required: no config.json beside {sd}")
+            config = path
+        voc = cls(config, math_mode=math_mode)
+        voc.load_state_dict(normalise_checkpoint(voc, read_checkpoint(sd, "generator", "a generator state dict")))
+        return voc
+
+    # ---- device state ---------------------------------------------------------------------------------------------
+    def _create(self):
+        h = C.c_void_p()
+        cfg = self._c_config()
+        name = f"fs2_{self._NAME}_create"
+        _lib.check(getattr(_lib.load(), name)(C.byref(h), _lib.MATH_MODES[self.math_mode], C.byref(cfg)), name)
+        return h.value
+
+    def _rows(self, B: int, L: int):
+        """fs2_<_NAME>'s largest buffer: B * Lmax * 256 sample rows."""
+        return B * L * HOP, f"B * Lmax * {HOP}", "sample"
+
+
+class HiFiGANVocoder(_Generator):
     """jik876/hifi-gan's `Generator(h)` on the H100 kernels.
 
     `forward(mels [B, Lmax, 80], olens [B])` -> (audio [B, Lmax * 256] fp32, alens = olens * 256).  Utterance b is the
@@ -188,78 +287,8 @@ class HiFiGANVocoder(NeuralVocoder):
         add_layers(self, cfg)
         self._layers = [m for m in self.modules() if isinstance(m, _WNConv)]      # state_dict order
 
-    def launches(self) -> int:
-        """Kernels one call enqueues: 4 + U * (2 + K * G + max(K - 2, 0)), G = 12 (resblock "1") or 4 (resblock "2")."""
-        U, K = len(self.config["upsample_rates"]), len(self.config["resblock_kernel_sizes"])
-        G = 12 if self.config["resblock"] == "1" else 4
-        return 4 + U * (2 + K * G + max(K - 2, 0))
-
-    def window_plan(self) -> dict:
-        """The window plan of this config (DESIGN.md section 17), walking back from the audio: conv_post reads 3 rows on
-        each side, each MRF R = its largest resblock's reach, upsampling s reads `reach[s]` input rows around its core, and
-        conv_pre 3 frames more.  -> {"reach": [r_s], "halo": [h_s] (rows of level s on each side of its core; h_0 = r_0 + 3
-        mel frames, h_{s+1} = u_s r_s), "R": R}."""
-        return ups_window_plan(*self._chain())
-
-    def _chain(self):
-        """The upsample rates; R = the largest resblock's reach; conv_pre's native taps leave its 3 outer rows wrong at a
-        window side that is not an utterance edge."""
-        cfg = self.config
-        steps = 3 if cfg["resblock"] == "1" else 2
-        extra = 1 if cfg["resblock"] == "1" else 0
-        R = max(sum((k - 1) // 2 * (d + extra) for d in dil[:steps])
-                for k, dil in zip(cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"]))
-        return cfg["upsample_rates"], R, 3
-
-    def flops_per_frame(self) -> int:
-        """Multiply-adds x 2 per mel frame of the generator's convolutions (the transposed ones counted as torch runs them:
-        Cin * Cout * k per input row)."""
-        cfg = self.config
-        c0, f = cfg["upsample_initial_channel"], 0
-        f += N_MELS * c0 * 7
-        up = 1
-        convs = 6 if cfg["resblock"] == "1" else 2
-        for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
-            cin, cout = c0 // 2 ** i, c0 // 2 ** (i + 1)
-            f += up * cin * cout * k
-            up *= u
-            f += up * sum(convs * cout * cout * kk for kk in cfg["resblock_kernel_sizes"])
-        f += up * (c0 // 2 ** len(cfg["upsample_rates"])) * 7
-        return 2 * f
-
-    # ---- checkpoints ----------------------------------------------------------------------------------------------
-    @classmethod
-    def from_checkpoint(cls, path_or_dict, config=None, math_mode: str = "3xf16") -> "HiFiGANVocoder":
-        """A hifi-gan generator checkpoint (`g_XXXXXXXX`: a dict with "generator") or a bare generator state dict, given as
-        a file path or as the loaded dict.  Either may hold `weight_g` / `weight_v` keys or plain `weight` keys (after
-        `remove_weight_norm`).  config: as in the constructor; None reads config.json beside a checkpoint path, as
-        hifi-gan's inference.py does (the dilations cannot be read from the weights).  A missing, unexpected or wrongly
-        shaped key raises ValueError naming it."""
-        sd = path_or_dict
-        if config is None:
-            if not isinstance(sd, (str, os.PathLike)):
-                raise ValueError("config is required when the checkpoint is given as a dict")
-            path = os.path.join(os.path.dirname(os.path.abspath(sd)), "config.json")
-            if not os.path.exists(path):
-                raise ValueError(f"config is required: no config.json beside {sd}")
-            config = path
-        voc = cls(config, math_mode=math_mode)
-        voc.load_state_dict(normalise_checkpoint(voc, read_checkpoint(sd, "generator", "a generator state dict")))
-        return voc
-
-    # ---- device state ---------------------------------------------------------------------------------------------
     def _c_config(self) -> _lib.HiFiGANConfig:
         return c_config(self.config)
 
-    def _create(self):
-        h = C.c_void_p()
-        cfg = self._c_config()
-        _lib.check(_lib.load().fs2_hifigan_create(C.byref(h), _lib.MATH_MODES[self.math_mode], C.byref(cfg)), "fs2_hifigan_create")
-        return h.value
-
     def _load(self, h, device: torch.device) -> None:
         self._load_layers("fs2_hifigan_load", h, device)
-
-    def _rows(self, B: int, L: int):
-        """fs2_hifigan's largest buffer: B * Lmax * 256 sample rows."""
-        return B * L * HOP, f"B * Lmax * {HOP}", "sample"

@@ -14,13 +14,9 @@ checkpoint file.
 """
 from __future__ import annotations
 
-import ctypes as C
-import json
-import os
-
 import torch
 
-from ._kernel_module import HOP, NeuralVocoder, _WNConv, normalise_checkpoint, read_checkpoint, ups_window_plan
+from ._kernel_module import HOP, _WNConv
 from . import _lib, hifigan
 
 MAX_N_FFT = 16                   # the head kernel's shared memory holds conv_post's outputs for n_fft up to this
@@ -30,26 +26,14 @@ CONFIGS = {
     "v1": dict(hifigan.CONFIGS["v1"], upsample_rates=[8, 8], upsample_kernel_sizes=[16, 16], gen_istft_n_fft=16,
                gen_istft_hop_size=4),
 }
-_ISTFT_FIELDS = ("gen_istft_n_fft", "gen_istft_hop_size")
 
 
 def load_config(config) -> dict:
     """An iSTFTNet config as a dict of the fields the generator uses: from "v1", a dict (e.g. a loaded config.json) or the
     path of a config.json.  A config without gen_istft_n_fft / gen_istft_hop_size (a hifi-gan config) is refused, naming
     the field.  Only its form is checked here; `check_config` checks what this library runs."""
-    if isinstance(config, str) and config.lower() in CONFIGS:
-        config = CONFIGS[config.lower()]
-    elif isinstance(config, (str, os.PathLike)):
-        with open(config) as f:
-            config = json.load(f)
-    if not isinstance(config, dict):
-        raise ValueError(f"config must be one of {sorted(CONFIGS)}, a dict or the path of an iSTFTNet config.json")
-    for k in _ISTFT_FIELDS:
-        if k not in config:
-            raise ValueError(f"config: missing field {k} (a hifi-gan config is not an iSTFTNet one)")
-    out = hifigan.load_config(config)
-    out.update({k: config[k] for k in _ISTFT_FIELDS})
-    return out
+    return hifigan.load_config(config, CONFIGS, f"one of {sorted(CONFIGS)}", "an iSTFTNet", own=("gen_istft_n_fft", "gen_istft_hop_size"),
+                               own_note=" (a hifi-gan config is not an iSTFTNet one)")
 
 
 def check_config(cfg: dict) -> None:
@@ -72,7 +56,7 @@ def check_config(cfg: dict) -> None:
     hifigan.check_resblocks(cfg)
 
 
-class ISTFTNetVocoder(NeuralVocoder):
+class ISTFTNetVocoder(hifigan._Generator):
     """rishikksh20/iSTFTNet-pytorch's `Generator(h)` on the H100 kernels.
 
     `forward(mels [B, Lmax, 80], olens [B])` -> (audio [B, Lmax * 256] fp32, alens = olens * 256).  Utterance b is the
@@ -93,52 +77,20 @@ class ISTFTNetVocoder(NeuralVocoder):
         hifigan.add_layers(self, cfg, cfg["gen_istft_n_fft"] + 2)
         self._layers = [m for m in self.modules() if isinstance(m, _WNConv)]      # state_dict order
 
-    def launches(self) -> int:
-        """Kernels one call enqueues, as HiFi-GAN's: 4 + U * (2 + K * G + max(K - 2, 0)), G = 12 (resblock "1") or 4."""
-        U, K = len(self.config["upsample_rates"]), len(self.config["resblock_kernel_sizes"])
-        G = 12 if self.config["resblock"] == "1" else 4
-        return 4 + U * (2 + K * G + max(K - 2, 0))
-
     def head_reach(self) -> int:
         """Last-level rows the head reads on each side of its samples' rows: frame f reads rows f - 4 .. f + 2 (conv_post's
         taps and the reflected row) and rows [r0, r1) of samples need frames [r0 - e, r1 + e], e = (n_fft / 2 - 1) // hop."""
         return 4 + (self.config["gen_istft_n_fft"] // 2 - 1) // self.config["gen_istft_hop_size"]
 
-    def window_plan(self) -> dict:
-        """The window plan of this config, walking back from the audio: the head reads head_reach() last-level rows on each
-        side, each MRF R, upsampling s reads `reach[s]` input rows around its core, and conv_pre 3 frames more."""
-        return ups_window_plan(*self._chain())
-
-    def _chain(self):
-        """HiFi-GAN's chain of this config (rates, R, level-0 margin 3) with the head's reach as the last layer's."""
-        rates, R, margin0 = hifigan.HiFiGANVocoder._chain(self)
-        return rates, R, margin0, self.head_reach()
+    def _post_reach(self) -> int:
+        return self.head_reach()
 
     def flops_per_frame(self) -> int:
         """Multiply-adds x 2 per mel frame of the generator's convolutions, conv_post's n_fft + 2 outputs included (the
         inverse DFT and overlap-add are not counted)."""
         cfg = self.config
-        return hifigan.HiFiGANVocoder.flops_per_frame(self) + 2 * HOP // cfg["gen_istft_hop_size"] * \
+        return super().flops_per_frame() + 2 * HOP // cfg["gen_istft_hop_size"] * \
             (cfg["upsample_initial_channel"] // 2 ** len(cfg["upsample_rates"])) * 7 * (cfg["gen_istft_n_fft"] + 1)
-
-    # ---- checkpoints ----------------------------------------------------------------------------------------------
-    @classmethod
-    def from_checkpoint(cls, path_or_dict, config=None, math_mode: str = "3xf16") -> "ISTFTNetVocoder":
-        """An iSTFTNet generator checkpoint (`g_XXXXXXXX`: a dict with "generator") or a bare generator state dict, given
-        as a file path or as the loaded dict, with `weight_g` / `weight_v` or plain `weight` keys.  config: as in the
-        constructor; None reads config.json beside a checkpoint path.  A missing, unexpected or wrongly shaped key raises
-        ValueError naming it."""
-        sd = path_or_dict
-        if config is None:
-            if not isinstance(sd, (str, os.PathLike)):
-                raise ValueError("config is required when the checkpoint is given as a dict")
-            path = os.path.join(os.path.dirname(os.path.abspath(sd)), "config.json")
-            if not os.path.exists(path):
-                raise ValueError(f"config is required: no config.json beside {sd}")
-            config = path
-        voc = cls(config, math_mode=math_mode)
-        voc.load_state_dict(normalise_checkpoint(voc, read_checkpoint(sd, "generator", "a generator state dict")))
-        return voc
 
     # ---- device state ---------------------------------------------------------------------------------------------
     def _c_config(self) -> _lib.ISTFTNetConfig:
@@ -147,12 +99,6 @@ class ISTFTNetVocoder(NeuralVocoder):
         c.istft_n_fft = self.config["gen_istft_n_fft"]
         c.istft_hop = self.config["gen_istft_hop_size"]
         return c
-
-    def _create(self):
-        h = C.c_void_p()
-        cfg = self._c_config()
-        _lib.check(_lib.load().fs2_istftnet_create(C.byref(h), _lib.MATH_MODES[self.math_mode], C.byref(cfg)), "fs2_istftnet_create")
-        return h.value
 
     def _load(self, h, device: torch.device) -> None:
         self._load_layers("fs2_istftnet_load", h, device)

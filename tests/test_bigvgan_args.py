@@ -433,8 +433,8 @@ def test_bigvgan_kernels_do_not_spill():
     if not reports:
         pytest.skip("no ptxas reports (library built elsewhere)")
     text = open(reports[0]).read()
-    expected = {"bigvgan_act_kernel": 3, "bigvgan_rows_kernel": 3, "bigvgan_add_kernel": 1, "bigvgan_post_kernel": 1, "act_param_kernel": 1,
-                "pad3_kernel": 1}
+    # the Activation1d kernels only: BigVGAN's chain runs on hifigan.cu's, its padding pack is vocoder_weights.cu's
+    expected = {"bigvgan_act_kernel": 3, "bigvgan_post_kernel": 1, "act_param_kernel": 1}
     for kernel, n in expected.items():
         props = re.findall(r"Function properties for \S*%s\S*\n(.*)" % kernel, text)
         assert len(props) == n, (kernel, len(props))

@@ -273,15 +273,16 @@ def test_melgan_kernels_do_not_spill():
 
 
 def test_shared_weight_pack_kernels_do_not_spill():
-    """The convolution weight pack and bias kernels MelGAN and HiFi-GAN load their checkpoints through (csrc/vocoder_weights.cu)."""
+    """The convolution weight pack, bias and zero-padding kernels MelGAN, HiFi-GAN and BigVGAN load their checkpoints
+    through (csrc/vocoder_weights.cu)."""
     reports = glob.glob(os.path.join(REPO, "fastspeech2_b200", "build", "vocoder_weights.ptxas.txt"))
     if not reports:
         pytest.skip("no ptxas reports (library built elsewhere)")
     text = open(reports[0]).read()
-    for kernel in ("conv_pack_kernel", "conv_bias_kernel"):
+    for kernel in ("conv_pack_kernel", "conv_bias_kernel", "pad3_kernel"):
         props = re.findall(r"Function properties for \S*%s\S*\n(.*)" % kernel, text)
         assert len(props) == 1, (kernel, len(props))
-        assert "0 bytes spill stores, 0 bytes spill loads" in props[0], (kernel, props[0])
+        assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in props[0], (kernel, props[0])
 
 
 def test_shared_window_prep_kernel_does_not_spill():

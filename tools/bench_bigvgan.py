@@ -40,7 +40,8 @@ NAMES = {"base": "base_22khz_80band", "large": "22khz_80band"}
 
 def act_profile(voc, mels, olens, mode: str) -> list:
     """Per stage s: (C'_s, launches, mean device us of one bigvgan_act_kernel launch, HBM-bound us of one launch), the
-    stage found by launch position: the plain-rows producer opens conv_pre (first) and every upsampling."""
+    stage found by launch position: the plain-rows producer (hifigan_act_kernel without lrelu, the generator chain's) opens
+    conv_pre (first) and every upsampling."""
     from torch.profiler import ProfilerActivity, profile
     with torch.no_grad():
         voc(mels, olens)
@@ -48,14 +49,15 @@ def act_profile(voc, mels, olens, mode: str) -> list:
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             voc(mels, olens)
             torch.cuda.synchronize()
-    ev = sorted([e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and "bigvgan" in e.name],
+    ev = sorted([e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
+                 and ("bigvgan" in e.name or "hifigan_act_kernel" in e.name)],
                 key=lambda e: e.time_range.start)
     cfg = voc.config
     U = len(cfg["upsample_rates"])
     per = [[] for _ in range(U)]
     s = -2
     for e in ev:
-        if "bigvgan_rows_kernel" in e.name:
+        if "hifigan_act_kernel" in e.name:
             s += 1
         elif "bigvgan_act_kernel" in e.name and 0 <= s < U:
             per[s].append(e.time_range.elapsed_us())
