@@ -59,7 +59,9 @@ FS2_BIGVGAN_BAD_LENGTH, FS2_BIGVGAN_RANGE, FS2_BIGVGAN_BAD_START = 1, 2, 4   # b
 FS2_BIGVGAN_SNAKE, FS2_BIGVGAN_SNAKEBETA = 0, 1
 FS2_ISTFTNET_BAD_LENGTH, FS2_ISTFTNET_RANGE, FS2_ISTFTNET_BAD_START = 1, 2, 4   # bits of fs2_istftnet's / fs2_istftnet_window's status word
 FS2_EVAL_BAD_LENGTH, FS2_EVAL_NONFINITE = 1, 2   # bits of fs2_mcd_dtw's / fs2_path_prosody's status word
-FS2_PLAN_BAD_ILENS, FS2_PLAN_BAD_CONTROL, FS2_PLAN_OVERFLOW = 1, 2, 4   # bits of fs2_length_plan_cap's status word
+FS2_RS_BAD_LENGTH, FS2_RS_NONFINITE = 1, 2       # bits of fs2_resample's status word
+FS2_RESAMPLE_TABLE = 32769                        # entries of the resampling filter's right wing
+FS2_PLAN_BAD_ILENS,FS2_PLAN_BAD_CONTROL, FS2_PLAN_OVERFLOW = 1, 2, 4   # bits of fs2_length_plan_cap's status word
 FS2_SYNTH_VOC_SHIFT = 8                          # fs2_synth_status: the vocoder's bits sit this far up in the word
 
 
@@ -166,6 +168,8 @@ SIGNATURES = {
     "fs2_dtw_workspace_bytes": [_I, _I, _I, _I, _I, _I, C.POINTER(_SZ)],
     "fs2_mcd_dtw": [_P, _P, _I, _P, _P, _I, _I, _I, _P, _I, C.c_double, _P, _P, _P, _P, _P, _P, _SZ, _P],
     "fs2_path_prosody": [_P, _P, _I, _I, _P, _P, _I, _P, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P],
+    "fs2_resample_workspace_bytes": [_I, _I, _I, _I, _I, C.POINTER(_SZ)],
+    "fs2_resample": [_P, _P, _I, _I, _P, _I, _I, _P, _P, _I, _P, _P, _SZ, _P],
     "fs2_melgan_create": [C.POINTER(_P), _I],
     "fs2_melgan_load": [_P, C.POINTER(_P), C.POINTER(_P), _P],
     "fs2_melgan_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],

@@ -528,6 +528,30 @@ int fs2_path_prosody(const int32_t* path, const int64_t* plen, int B, int P_max,
                      const double* f0y, const int64_t* f0y_lens, int Fy, const float* ex, int Ex, const float* ey, int Ey,
                      int64_t* counts, double* sums, int* status, void* stream);
 
+/* ---- band-limited resampling: librosa 0.7.0's resample (resampy kaiser_best) (DESIGN.md section 22) ---------------- */
+/* Mono utterances x [B, Nmax] fp32 with sample counts lens [B] at sr_orig -> y [B, Mmax] fp32 at sr_new, with
+ * ratio = double(sr_new) / sr_orig, scale = min(1, ratio), 1 / ratio per output step and index_step = int(scale * 512).
+ * table: float64 [FS2_RESAMPLE_TABLE][2], (win[j], delta[j]) interleaved, the kaiser_best right wing (64 zero crossings,
+ * 512 entries each, rolloff 0.9475937167399596, Kaiser beta 14.769656459379492) times ratio when ratio < 1, and its
+ * forward difference (delta[last] = 0), built by the caller.  Utterance b (N = lens[b]):
+ *   n_out    = int(N * ratio) samples computed, olens[b] = ceil(N * ratio), y[b, t] = +0 for t >= n_out
+ *   y[b, t]  = resampy's resample_f: the time register, a running float64 sum of 1 / ratio from 0, gives n and frac; the
+ *              left wing's taps x[n - i], then the right wing's x[n + 1 + k], each weight win[j] + eta * delta[j], each
+ *              product and sum in float64 without FMA, y rounded to float32 after every tap
+ * Samples at or past lens[b] are never read; y[b] is bit-identical to a B = 1 call.  Requires sr_orig != sr_new (equal
+ * rates return the input unchanged, with no call), index_step >= 1, Mmax in [ceil(Nmax * ratio), 2^26) (which keeps the
+ * running sum's rounding far below one input step, so n stays below N).  A memset and 2 kernels; no allocation, no
+ * synchronisation.  Data-dependent checks are reported in *status (device int, zeroed):
+ *   FS2_RS_BAD_LENGTH  some lens[b] outside [1, Nmax], or int(N * ratio) < 1; that row is 0 and olens[b] 0;
+ *   FS2_RS_NONFINITE   a NaN or inf sample within lens[b].
+ * Workspace (fs2_resample_workspace_bytes): the time register, 8 B Mmax rounded up to 256 bytes, plus 256. */
+#define FS2_RS_BAD_LENGTH 1
+#define FS2_RS_NONFINITE 2
+#define FS2_RESAMPLE_TABLE 32769
+int fs2_resample_workspace_bytes(int B, int Nmax, int sr_orig, int sr_new, int Mmax, size_t* bytes);
+int fs2_resample(const float* x, const int64_t* lens, int B, int Nmax, const double* table, int sr_orig, int sr_new, float* y,
+                 int64_t* olens, int Mmax, int* status, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- batched MelGAN vocoder (DESIGN.md section 8) ------------------------------------------------------------------- */
 /* seungwonpark/melgan's Generator(mel_channel = 80) on log-mels [B, Lmax, 80] with frame counts olens [B]: utterance b is
  * the generator applied to its own frames mels[b, :olens[b]] followed by 10 frames of -11.5129, every reflection pad at its
