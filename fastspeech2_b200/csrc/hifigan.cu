@@ -317,18 +317,6 @@ HgPlan carve_plan(Bump& b, size_t lens_bytes, size_t n) {
   return p;
 }
 
-HgPlan plan(Bump& b, const Shape& sh, int B, int L) {
-  return carve_plan(b, (size_t)(sh.U + 1) * B * sizeof(int64_t), (size_t)B * L * sh.act);
-}
-
-// A window call's workspace, from B and nf only: five buffers of the largest level buffer per utterance (rows x C' over
-// every level; conv_pre's operand, 80 wide, and the upsamplings' operands, r_s <= h_s, fit in it)
-HgPlan window_plan(Bump& b, const Shape& sh, int B, int nf) {
-  long act = level_rows(sh.ups, 0, nf) * kMels;
-  for (int s = 0; s <= sh.U; ++s) act = std::max(act, level_rows(sh.ups, s, nf) * sh.Cp[s]);
-  return carve_plan(b, (size_t)3 * n_wins(sh.ups) * B * sizeof(int64_t), (size_t)B * act);
-}
-
 // a GEMM weight here is [taps][N][K] tap matrices with K = Cin, so vweight_pack_conv packs it at tap_stride = N K
 void set_conv(VWeight& w, int N, int K, int taps) { w.N = N; w.K = K; w.taps = taps; }
 
@@ -350,15 +338,6 @@ int pack_conv(const VWeight& w, const float* wt, const float* bias, int Cin, int
     rc = vweight_pack_conv(w, pw, pb, Cip, Cop, taps, u, (long)w.N * w.K, st);
   cudaFreeAsync(base, st);
   return rc;
-}
-
-// the whole call's limits on its largest GEMM, B * Lmax * up_U rows (HiFi-GAN and BigVGAN: samples)
-int check_size(const char* who, const Shape& sh, int math_mode, int B, int L) {
-  FS2_REQUIRE(B >= 1 && L >= 1, "%s: need B >= 1 and Lmax >= 1 (got %d, %d)", who, B, L);
-  const int up = sh.ups.up[sh.U];
-  char formula[32];
-  snprintf(formula, sizeof formula, "B * Lmax * %d", up);
-  return check_rows(who, formula, up == kHop ? "sample" : "row", (long)B * L * up, math_mode);
 }
 
 enum Head { kHeadPost, kHeadIstft, kHeadActPost };   // conv_post + tanh, iSTFTNet's inverse STFT, BigVGAN's activation_post + conv_post
@@ -402,7 +381,7 @@ int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const
   auto desc = [&](int i) -> const int64_t* { return w ? p.lens + 3L * i * B : nullptr; };
   auto lens = [&](int i, int s) -> const int64_t* { return w ? p.lens + (3L * i + 1) * B : p.lens + (long)s * B; };   // window i / level s
   auto rows = [&](int s) { return w ? (int)level_rows(sh.ups, s, nf) : L * sh.ups.up[s]; };
-  int rc = ups_prep(olens, starts, B, L, nf, sh.ups, p.lens, status, st);
+  int rc = ups_prep(olens, starts, B, 1, L, nf, sh.ups, p.lens, status, st);
   if (rc) return rc;
   if ((rc = act(kind, false, mels, nullptr, 1, lens(win_level(0), 0), nullptr, L, desc(win_level(0)), B, rows(0), kMels, 0, p.a, status, st)))
     return rc;
@@ -446,6 +425,24 @@ int generate(const fs2_hifigan_gen* m, const HgPlan& p, const float* mels, const
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
+
+// the generator's side of the shared C entries (vocoder_window.cuh)
+struct HgEntry {
+  using Gen = fs2_hifigan_gen;
+  static const UpsPlan& ups(const Gen* m) { return m->sh.ups; }
+  static HgPlan plan(Bump& b, const Gen* m, int B, int L) {
+    return carve_plan(b, (size_t)(m->sh.U + 1) * B * sizeof(int64_t), (size_t)B * L * m->sh.act);
+  }
+  // A window call's workspace, from B and nf only: five buffers of the largest level buffer per utterance (rows x C' over
+  // every level; conv_pre's operand, 80 wide, and the upsamplings' operands, r_s <= h_s, fit in it)
+  static HgPlan window_plan(Bump& b, const Gen* m, int B, int nf) {
+    const Shape& sh = m->sh;
+    long act = level_rows(sh.ups, 0, nf) * kMels;
+    for (int s = 0; s <= sh.U; ++s) act = std::max(act, level_rows(sh.ups, s, nf) * sh.Cp[s]);
+    return carve_plan(b, (size_t)3 * n_wins(sh.ups) * B * sizeof(int64_t), (size_t)B * act);
+  }
+  static constexpr auto generate = fs2::generate;
+};
 
 // A handle for a validated config with the given head (n_fft, hop: iSTFTNet's; 0, 1 otherwise) and activation
 template <typename Gen>
@@ -516,63 +513,6 @@ int load_gen(fs2_hifigan_gen* m, const float* const* weights, const float* const
   if (m->post_b) FS2_CUDA_CHECK(cudaMemcpyAsync(m->post_b, biases[last], O * sizeof(float), cudaMemcpyDeviceToDevice, st));
   m->loaded = true;
   return FS2_OK;
-}
-
-int workspace_gen(fs2_hifigan_gen* m, int B, int Lmax, size_t* bytes, const char* name) {
-  FS2_REQUIRE(m && bytes, "%s_workspace_bytes: null argument", name);
-  int rc = check_size(name, m->sh, m->math_mode, B, Lmax);
-  if (rc) return rc;
-  Bump b(nullptr, 0);
-  plan(b, m->sh, B, Lmax);
-  *bytes = b.off + 256;
-  return FS2_OK;
-}
-
-int call_gen(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
-             size_t ws_bytes, void* stream, const char* name) {
-  FS2_REQUIRE(m && mels && olens && audio && status && ws, "%s: null argument", name);
-  FS2_REQUIRE(m->loaded, "%s: weights not loaded (%s_load)", name, name);
-  FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "%s: mels must be 16-byte aligned", name);
-  int rc = check_size(name, m->sh, m->math_mode, B, Lmax);
-  if (rc) return rc;
-  Bump b(ws, ws_bytes);
-  HgPlan p = plan(b, m->sh, B, Lmax);
-  if ((rc = b.check(name))) return rc;
-  return generate(m, p, mels, olens, nullptr, B, Lmax, 0, audio, (long)Lmax * kHop, status, (cudaStream_t)stream);
-}
-
-int window_workspace_gen(fs2_hifigan_gen* m, int B, int n_frames, size_t* bytes, const char* name) {
-  char who[48];
-  snprintf(who, sizeof who, "%s_window", name);
-  FS2_REQUIRE(m && bytes, "%s_workspace_bytes: null argument", who);
-  int rc = check_window_rows(who, m->sh.ups, B, n_frames, m->math_mode);
-  if (rc) return rc;
-  Bump b(nullptr, 0);
-  window_plan(b, m->sh, B, n_frames);
-  *bytes = b.off + 256;
-  return FS2_OK;
-}
-
-int window_gen(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax, int n_frames,
-               float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream, const char* name) {
-  char who[48];
-  snprintf(who, sizeof who, "%s_window", name);
-  FS2_REQUIRE(m && mels && olens && starts && audio && status && ws, "%s: null argument", who);
-  FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "%s: mels must be 16-byte aligned", who);
-  int rc = check_window_rows(who, m->sh.ups, B, n_frames, m->math_mode);
-  if (rc) return rc;
-  if ((rc = check_window_extent(who, Lmax, 0, kHop, n_frames, audio_ld))) return rc;
-  Bump b(ws, ws_bytes);
-  HgPlan p = window_plan(b, m->sh, B, n_frames);
-  if ((rc = b.check(who))) return rc;
-  FS2_REQUIRE(m->loaded, "%s: weights not loaded (%s_load)", who, name);
-  return generate(m, p, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, (cudaStream_t)stream);
-}
-
-void destroy_gen(fs2_hifigan_gen* m) {
-  if (!m) return;
-  if (m->arena) cudaFree(m->arena);
-  delete m;
 }
 
 // One residual block on rows [B * Lp][C] (fs2_op_hifigan_resblock; with acts, fs2_op_bigvgan_resblock's AMP block)
@@ -648,21 +588,21 @@ int fs2_hifigan_load(fs2_hifigan_gen* m, const float* const* weights, const floa
 }
 
 int fs2_hifigan_workspace_bytes(fs2_hifigan_gen* m, int B, int Lmax, size_t* bytes) {
-  return workspace_gen(m, B, Lmax, bytes, "fs2_hifigan");
+  return workspace_gen<HgEntry>(m, B, Lmax, bytes, "fs2_hifigan");
 }
 
 int fs2_hifigan(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
                 size_t ws_bytes, void* stream) {
-  return call_gen(m, mels, olens, B, Lmax, audio, status, ws, ws_bytes, stream, "fs2_hifigan");
+  return call_gen<HgEntry>(m, mels, olens, B, Lmax, audio, status, ws, ws_bytes, stream, "fs2_hifigan");
 }
 
 int fs2_hifigan_window_workspace_bytes(fs2_hifigan_gen* m, int B, int n_frames, size_t* bytes) {
-  return window_workspace_gen(m, B, n_frames, bytes, "fs2_hifigan");
+  return window_workspace_gen<HgEntry>(m, B, n_frames, bytes, "fs2_hifigan");
 }
 
 int fs2_hifigan_window(fs2_hifigan_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax, int n_frames,
                        float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream) {
-  return window_gen(m, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws, ws_bytes, stream, "fs2_hifigan");
+  return window_gen<HgEntry>(m, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws, ws_bytes, stream, "fs2_hifigan");
 }
 
 int fs2_istftnet_create(fs2_istftnet_gen** out, int math_mode, const fs2_istftnet_config* cfg) {
@@ -686,21 +626,21 @@ int fs2_istftnet_load(fs2_istftnet_gen* m, const float* const* weights, const fl
 }
 
 int fs2_istftnet_workspace_bytes(fs2_istftnet_gen* m, int B, int Lmax, size_t* bytes) {
-  return workspace_gen(m, B, Lmax, bytes, "fs2_istftnet");
+  return workspace_gen<HgEntry>(m, B, Lmax, bytes, "fs2_istftnet");
 }
 
 int fs2_istftnet(fs2_istftnet_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
                  size_t ws_bytes, void* stream) {
-  return call_gen(m, mels, olens, B, Lmax, audio, status, ws, ws_bytes, stream, "fs2_istftnet");
+  return call_gen<HgEntry>(m, mels, olens, B, Lmax, audio, status, ws, ws_bytes, stream, "fs2_istftnet");
 }
 
 int fs2_istftnet_window_workspace_bytes(fs2_istftnet_gen* m, int B, int n_frames, size_t* bytes) {
-  return window_workspace_gen(m, B, n_frames, bytes, "fs2_istftnet");
+  return window_workspace_gen<HgEntry>(m, B, n_frames, bytes, "fs2_istftnet");
 }
 
 int fs2_istftnet_window(fs2_istftnet_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax, int n_frames,
                         float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream) {
-  return window_gen(m, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws, ws_bytes, stream, "fs2_istftnet");
+  return window_gen<HgEntry>(m, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws, ws_bytes, stream, "fs2_istftnet");
 }
 
 int fs2_bigvgan_create(fs2_bigvgan_gen** out, int math_mode, const fs2_bigvgan_config* cfg) {
@@ -727,21 +667,21 @@ int fs2_bigvgan_load(fs2_bigvgan_gen* m, const float* const* weights, const floa
 }
 
 int fs2_bigvgan_workspace_bytes(fs2_bigvgan_gen* m, int B, int Lmax, size_t* bytes) {
-  return workspace_gen(m, B, Lmax, bytes, "fs2_bigvgan");
+  return workspace_gen<HgEntry>(m, B, Lmax, bytes, "fs2_bigvgan");
 }
 
 int fs2_bigvgan(fs2_bigvgan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
                 size_t ws_bytes, void* stream) {
-  return call_gen(m, mels, olens, B, Lmax, audio, status, ws, ws_bytes, stream, "fs2_bigvgan");
+  return call_gen<HgEntry>(m, mels, olens, B, Lmax, audio, status, ws, ws_bytes, stream, "fs2_bigvgan");
 }
 
 int fs2_bigvgan_window_workspace_bytes(fs2_bigvgan_gen* m, int B, int n_frames, size_t* bytes) {
-  return window_workspace_gen(m, B, n_frames, bytes, "fs2_bigvgan");
+  return window_workspace_gen<HgEntry>(m, B, n_frames, bytes, "fs2_bigvgan");
 }
 
 int fs2_bigvgan_window(fs2_bigvgan_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax, int n_frames,
                        float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream) {
-  return window_gen(m, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws, ws_bytes, stream, "fs2_bigvgan");
+  return window_gen<HgEntry>(m, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws, ws_bytes, stream, "fs2_bigvgan");
 }
 
 // ---- single layers on the vocoders' own code paths (tests) ----------------------------------------------------------

@@ -385,37 +385,6 @@ struct MgPlan {
   float* h;          // dilated conv output [rows][C] (unfused route only)
 };
 
-// A window call's workspace, from B and nf only: per utterance, the largest operand (rows x K over every producer) and
-// the largest activation (rows x C over every level) of the window's buffers
-MgPlan window_plan(Bump& b, int B, int nf) {
-  long op = level_rows(kPlan, 0, nf) * kMels * kPreTaps, act = level_rows(kPlan, 0, nf) * 512;
-  for (int s = 0; s < kStages; ++s) {
-    op = std::max(op, std::max(ups_rows(kPlan, s, nf) * 3 * kCin[s], level_rows(kPlan, s + 1, nf) * 3 * kCout[s]));
-    act = std::max(act, level_rows(kPlan, s + 1, nf) * kCout[s]);
-  }
-  MgPlan p;
-  p.lens = (int64_t*)b.bytes((size_t)3 * n_wins(kPlan) * B * sizeof(int64_t));
-  p.a = b.floats((size_t)B * op);
-  p.x[0] = b.floats((size_t)B * act);
-  p.x[1] = b.floats((size_t)B * act);
-  p.h = b.floats((size_t)B * act);
-  return p;
-}
-
-// per frame of Lp: values of the largest operand (3C at the three late stages, 24576) and activation (8192)
-constexpr long kOperandPerFrame = 3L * 256 * 32, kActPerFrame = 256L * 32;
-
-MgPlan plan(Bump& b, int B, int L, bool fused) {
-  const size_t frames = (size_t)B * (L + kTail);
-  MgPlan p;
-  p.lens = (int64_t*)b.bytes((size_t)(kStages + 1) * B * sizeof(int64_t));
-  p.a = b.floats(frames * kOperandPerFrame);
-  p.x[0] = b.floats(frames * kActPerFrame);
-  p.x[1] = b.floats(frames * kActPerFrame);
-  p.h = fused ? nullptr : b.floats(frames * kActPerFrame);
-  return p;
-}
-
 // the taps producer: operand rows [B * Lp] (window win, lens) from x, ldx rows per utterance in window xwin (nullptr: the
 // operand's own rows, ldx = Lp); margin: see exact_row
 int run_taps(int kind, bool reflect_edges, const float* x, const int64_t* xwin, int ldx, const int64_t* lens, const int64_t* win, int B,
@@ -486,7 +455,7 @@ int generate(const fs2_melgan_gen* m, const MgPlan& p, const float* mels, const 
   auto desc = [&](int i) -> const int64_t* { return w ? p.lens + 3L * i * B : nullptr; };
   auto lens = [&](int i, int s) -> const int64_t* { return w ? p.lens + (3L * i + 1) * B : p.lens + (long)s * B; };   // window i / level s
   auto rows = [&](int s) { return w ? (int)level_rows(kPlan, s, nf) : (Lmax + kTail) * upsampling(s); };
-  int rc = ups_prep(olens, starts, B, Lmax, nf, kPlan, p.lens, status, st);
+  int rc = ups_prep(olens, starts, B, 1, Lmax, nf, kPlan, p.lens, status, st);
   if (rc) return rc;
   {
     auto k = pick(kind, melgan_pre_operand_kernel<OUT_HILO>, melgan_pre_operand_kernel<OUT_HI>, melgan_pre_operand_kernel<OUT_F32>);
@@ -518,10 +487,41 @@ int generate(const fs2_melgan_gen* m, const MgPlan& p, const float* mels, const 
   return FS2_OK;
 }
 
-int check_size(const fs2_melgan_gen* m, int B, int L) {
-  FS2_REQUIRE(B >= 1 && L >= 1, "fs2_melgan: need B >= 1 and Lmax >= 1 (got %d, %d)", B, L);
-  return check_rows("fs2_melgan", "B * (Lmax + 10) * 256", "sample", (long)B * (L + kTail) * upsampling(kStages), m->math_mode);
-}
+// per frame of Lp: values of the largest operand (3C at the three late stages, 24576) and activation (8192)
+constexpr long kOperandPerFrame = 3L * 256 * 32, kActPerFrame = 256L * 32;
+
+// the generator's side of the shared C entries (vocoder_window.cuh)
+struct MgEntry {
+  using Gen = fs2_melgan_gen;
+  static const UpsPlan& ups(const Gen*) { return kPlan; }
+  static MgPlan plan(Bump& b, const Gen*, int B, int L) {
+    const size_t frames = (size_t)B * (L + kTail);
+    MgPlan p;
+    p.lens = (int64_t*)b.bytes((size_t)(kStages + 1) * B * sizeof(int64_t));
+    p.a = b.floats(frames * kOperandPerFrame);
+    p.x[0] = b.floats(frames * kActPerFrame);
+    p.x[1] = b.floats(frames * kActPerFrame);
+    p.h = b.floats(frames * kActPerFrame);
+    return p;
+  }
+  // A window call's workspace, from B and nf only: per utterance, the largest operand (rows x K over every producer) and
+  // the largest activation (rows x C over every level) of the window's buffers
+  static MgPlan window_plan(Bump& b, const Gen*, int B, int nf) {
+    long op = level_rows(kPlan, 0, nf) * kMels * kPreTaps, act = level_rows(kPlan, 0, nf) * 512;
+    for (int s = 0; s < kStages; ++s) {
+      op = std::max(op, std::max(ups_rows(kPlan, s, nf) * 3 * kCin[s], level_rows(kPlan, s + 1, nf) * 3 * kCout[s]));
+      act = std::max(act, level_rows(kPlan, s + 1, nf) * kCout[s]);
+    }
+    MgPlan p;
+    p.lens = (int64_t*)b.bytes((size_t)3 * n_wins(kPlan) * B * sizeof(int64_t));
+    p.a = b.floats((size_t)B * op);
+    p.x[0] = b.floats((size_t)B * act);
+    p.x[1] = b.floats((size_t)B * act);
+    p.h = b.floats((size_t)B * act);
+    return p;
+  }
+  static constexpr auto generate = fs2::generate;
+};
 
 }  // namespace
 }  // namespace fs2
@@ -540,11 +540,7 @@ int fs2_melgan_create(fs2_melgan_gen** out, int math_mode) {
   return FS2_OK;
 }
 
-void fs2_melgan_destroy(fs2_melgan_gen* m) {
-  if (!m) return;
-  if (m->arena) cudaFree(m->arena);
-  delete m;
-}
+void fs2_melgan_destroy(fs2_melgan_gen* m) { destroy_gen(m); }
 
 int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float* const* biases, void* stream) {
   FS2_REQUIRE(m && weights && biases, "fs2_melgan_load: null argument");
@@ -588,51 +584,21 @@ int fs2_melgan_load(fs2_melgan_gen* m, const float* const* weights, const float*
 }
 
 int fs2_melgan_workspace_bytes(fs2_melgan_gen* m, int B, int Lmax, size_t* bytes) {
-  FS2_REQUIRE(m && bytes, "fs2_melgan_workspace_bytes: null argument");
-  int rc = check_size(m, B, Lmax);
-  if (rc) return rc;
-  Bump b(nullptr, 0);
-  plan(b, B, Lmax, false);
-  *bytes = b.off + 256;
-  return FS2_OK;
+  return workspace_gen<MgEntry>(m, B, Lmax, bytes, "fs2_melgan");
 }
 
 int fs2_melgan(fs2_melgan_gen* m, const float* mels, const int64_t* olens, int B, int Lmax, float* audio, int* status, void* ws,
                size_t ws_bytes, void* stream) {
-  FS2_REQUIRE(m && mels && olens && audio && status && ws, "fs2_melgan: null argument");
-  FS2_REQUIRE(m->loaded, "fs2_melgan: weights not loaded (fs2_melgan_load)");
-  FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "fs2_melgan: mels must be 16-byte aligned");
-  int rc = check_size(m, B, Lmax);
-  if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  Bump b(ws, ws_bytes);
-  MgPlan p = plan(b, B, Lmax, false);
-  if ((rc = b.check("fs2_melgan"))) return rc;
-  return generate(m, p, mels, olens, nullptr, B, Lmax, 0, audio, (long)Lmax * upsampling(kStages), status, st);
+  return call_gen<MgEntry>(m, mels, olens, B, Lmax, audio, status, ws, ws_bytes, stream, "fs2_melgan");
 }
 
 int fs2_melgan_window_workspace_bytes(fs2_melgan_gen* m, int B, int n_frames, size_t* bytes) {
-  FS2_REQUIRE(m && bytes, "fs2_melgan_window_workspace_bytes: null argument");
-  int rc = check_window_rows("fs2_melgan_window", kPlan, B, n_frames, m->math_mode);
-  if (rc) return rc;
-  Bump b(nullptr, 0);
-  window_plan(b, B, n_frames);
-  *bytes = b.off + 256;
-  return FS2_OK;
+  return window_workspace_gen<MgEntry>(m, B, n_frames, bytes, "fs2_melgan");
 }
 
 int fs2_melgan_window(fs2_melgan_gen* m, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax, int n_frames,
                       float* audio, int64_t audio_ld, int* status, void* ws, size_t ws_bytes, void* stream) {
-  FS2_REQUIRE(m && mels && olens && starts && audio && status && ws, "fs2_melgan_window: null argument");
-  FS2_REQUIRE((reinterpret_cast<uintptr_t>(mels) & 15) == 0, "fs2_melgan_window: mels must be 16-byte aligned");
-  int rc = check_window_rows("fs2_melgan_window", kPlan, B, n_frames, m->math_mode);
-  if (rc) return rc;
-  if ((rc = check_window_extent("fs2_melgan_window", Lmax, kTail, upsampling(kStages), n_frames, audio_ld))) return rc;
-  Bump b(ws, ws_bytes);
-  MgPlan p = window_plan(b, B, n_frames);
-  if ((rc = b.check("fs2_melgan_window"))) return rc;
-  FS2_REQUIRE(m->loaded, "fs2_melgan_window: weights not loaded (fs2_melgan_load)");
-  return generate(m, p, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, (cudaStream_t)stream);
+  return window_gen<MgEntry>(m, mels, olens, starts, B, Lmax, n_frames, audio, audio_ld, status, ws, ws_bytes, stream, "fs2_melgan");
 }
 
 // ---- single layers on the vocoder's own code paths (tests) ----------------------------------------------------------

@@ -1,4 +1,4 @@
-// The window layer of an upsampling chain (vocoder_window.cuh).
+// The vocoders' window layer (vocoder_window.cuh).
 #include "vocoder_window.cuh"
 
 #include <algorithm>
@@ -9,17 +9,19 @@ namespace fs2 {
 namespace {
 
 constexpr int kBadLength = 1, kBadStart = 4;
-static_assert(FS2_MELGAN_BAD_LENGTH == kBadLength && FS2_HIFIGAN_BAD_LENGTH == kBadLength, "the vocoders' BAD_LENGTH bits differ");
-static_assert(FS2_MELGAN_BAD_START == kBadStart && FS2_HIFIGAN_BAD_START == kBadStart, "the vocoders' BAD_START bits differ");
+static_assert(FS2_MELGAN_BAD_LENGTH == kBadLength && FS2_HIFIGAN_BAD_LENGTH == kBadLength && FS2_WAVEGLOW_BAD_LENGTH == kBadLength,
+              "the vocoders' BAD_LENGTH bits differ");
+static_assert(FS2_MELGAN_BAD_START == kBadStart && FS2_HIFIGAN_BAD_START == kBadStart && FS2_WAVEGLOW_BAD_START == kBadStart,
+              "the vocoders' BAD_START bits differ");
 
-__global__ void ups_prep_kernel(const int64_t* __restrict__ olens, const int64_t* __restrict__ starts, int B, int L, int nf, UpsPlan p,
+__global__ void ups_prep_kernel(const int64_t* __restrict__ olens, const int64_t* __restrict__ starts, int B, int lo, int L, int nf, UpsPlan p,
                                 int64_t* __restrict__ lens, int* __restrict__ status) {
   __shared__ int bad;
   if (threadIdx.x == 0) bad = 0;
   __syncthreads();
   for (int b = threadIdx.x; b < B; b += blockDim.x) {
     const int64_t n = olens[b];
-    const bool ok = n >= 1 && n <= L;
+    const bool ok = n >= lo && n <= L;
     if (!ok) atomicOr(&bad, kBadLength);
     if (!starts) {
       for (int s = 0; s <= p.n; ++s) lens[(long)s * B + b] = ok ? (n + p.tail) * p.up[s] : 0;
@@ -50,11 +52,20 @@ __global__ void ups_prep_kernel(const int64_t* __restrict__ olens, const int64_t
 
 }  // namespace
 
-int ups_prep(const int64_t* olens, const int64_t* starts, int B, int L, int nf, const UpsPlan& p, int64_t* lens, int* status,
+int ups_prep(const int64_t* olens, const int64_t* starts, int B, int lo, int L, int nf, const UpsPlan& p, int64_t* lens, int* status,
              cudaStream_t st) {
-  ups_prep_kernel<<<1, 256, 0, st>>>(olens, starts, B, L, nf, p, lens, status);
+  ups_prep_kernel<<<1, 256, 0, st>>>(olens, starts, B, lo, L, nf, p, lens, status);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
+}
+
+int check_size(const char* who, const UpsPlan& p, int B, int L, int math_mode) {
+  FS2_REQUIRE(B >= 1 && L >= 1, "%s: need B >= 1 and Lmax >= 1 (got %d, %d)", who, B, L);
+  const int up = p.up[p.n];
+  char formula[48];
+  if (p.tail) snprintf(formula, sizeof formula, "B * (Lmax + %d) * %d", p.tail, up);
+  else snprintf(formula, sizeof formula, "B * Lmax * %d", up);
+  return check_rows(who, formula, up == 256 ? "sample" : "row", (long)B * ((long)L + p.tail) * up, math_mode);
 }
 
 int check_window_rows(const char* who, const UpsPlan& p, int B, int nf, int math_mode) {

@@ -30,11 +30,13 @@
 //
 // Windows (fs2_waveglow_window, DESIGN.md section 12): the same kernels and GEMMs on one buffer per utterance that holds
 // global frames [f0, f1) = [max(0, s - H), min(olens, s + n + H)) around the core [s, s + n), H = 96 frames, every buffer
-// (n + 2H) * 32 step rows long (window descriptors [kWinRows][B] in the workspace; nullptr = the whole call).  A flow
-// reaches 255 step rows on each side, so halo rows at a side that is not an utterance edge (f0 > 0, f1 < olens) differ
-// from the whole call's by at most 255 more rows per flow, and the core is exact after all 12.  The noise, the upsampling
-// operand and the cond planes are keyed by global frames and steps, so they are exact everywhere in the buffer; start and
-// gate range-check only rows whose values equal the whole call's (exact_row).
+// (n + 2H) * 32 step rows long.  The window layer (vocoder_window.cuh) describes it as a plan of two levels, the frames
+// and their step rows, each with a halo of H frames: ups_prep writes a descriptor [start | len | n] x B for the frames,
+// the step rows and the core's step rows (nullptr = the whole utterance).  A flow reaches 255 step rows on each side, so
+// halo rows at a side that is not an utterance edge (f0 > 0, f1 < olens) differ from the whole call's by at most 255 more
+// rows per flow, and the core is exact after all 12.  The noise, the upsampling operand and the cond planes are keyed by
+// global frames and steps, so they are exact everywhere in the buffer; start and gate range-check only rows whose values
+// equal the whole call's (exact_row).
 #include <math.h>
 
 #include "vocoder_weights.cuh"
@@ -51,64 +53,15 @@ constexpr int kTensors = 2 + kFlows * kPerFlow;
 // ---- window plan (DESIGN.md section 12) ----
 constexpr int kFlowReach = (1 << kLayers) - 1;                              // 8 k = 3 layers at dilation 2^i: 255 step rows
 constexpr int kHalo = (kFlows * kFlowReach + kSteps - 1) / kSteps;          // 96 frames on each side of a window's core
-static_assert(kHalo * kSteps >= kFlows * kFlowReach, "the halo must cover the 12 flows' reach");
-// window descriptors, one [B] row each: frames and step rows of the buffer (the GEMMs' lens), its first global frame, the
-// utterance's frame count (0 when invalid), the core's first frame in the buffer and its frame count (0: an empty window)
-enum { kWinF, kWinS, kWinF0, kWinN, kWinCore0, kWinCoreN, kWinRows };
+// The window plan (vocoder_window.cuh): level 0 the frames, level 1 their step rows, each with a halo of kHalo frames;
+// the upsampling reads level 0's rows (its reach is the halo, so its input window is level 0's); no tail frames.  The
+// descriptors are level 0's, level 1's and the audio's, all three in the rows of their level (the audio: step rows).
+constexpr UpsPlan kPlan{1, {1, kSteps}, {kHalo}, {kHalo, kSteps * kHalo}, 0};
+static_assert(kPlan.halo[1] >= kFlows * kFlowReach, "the halo must cover the 12 flows' reach");
+static_assert(n_wins(kPlan) == 3 && win_audio(kPlan) == 2, "descriptors of level 0, level 1 and the audio");
+constexpr UpsPlan kStepPlan{0, {1}, {}, {}, 0};                             // fs2_op_waveglow_flow's lengths: step rows
 
 __host__ __device__ inline int flow_channels(int k) { return k < 4 ? 8 : k < 8 ? 6 : 4; }
-
-// local step row t of utterance b's window buffer holds the whole call's values: not within `margin` rows of a side that
-// is not an utterance edge
-__device__ __forceinline__ bool exact_row(const int64_t* __restrict__ win, int B, int b, int t, int margin) {
-  const int64_t f0 = win[kWinF0 * B + b], nf = win[kWinF * B + b], ns = win[kWinS * B + b];
-  return (f0 == 0 || t >= margin) && (f0 + nf == win[kWinN * B + b] || t < ns - margin);
-}
-
-// one CTA: lensF[b] = olens[b], lensS[b] (nullable) = olens[b] * 32 for lo <= olens[b] <= L, else 0 (the utterance is
-// skipped); *status = 0 or FS2_WAVEGLOW_BAD_LENGTH.  Runs first, so the producers' range bits land on a cleared word.
-// lo = 1 for the vocoder's calls; the single-layer entries take lo = 0 (an empty utterance is valid there).
-__global__ void wg_prep_kernel(const int64_t* __restrict__ olens, int B, int L, int lo, int64_t* __restrict__ lensF,
-                               int64_t* __restrict__ lensS, int* __restrict__ status) {
-  __shared__ int bad;
-  if (threadIdx.x == 0) bad = 0;
-  __syncthreads();
-  for (int b = threadIdx.x; b < B; b += blockDim.x) {
-    const int64_t n = olens[b];
-    const bool ok = n >= lo && n <= L;
-    if (!ok) atomicOr(&bad, 1);
-    lensF[b] = ok ? n : 0;
-    if (lensS) lensS[b] = ok ? n * kSteps : 0;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) *status = bad ? FS2_WAVEGLOW_BAD_LENGTH : 0;
-}
-
-// one CTA, a window of nf frames from starts[b]: the kWinRows descriptors (see the top of the file) of the core
-// [starts[b], min(starts[b] + nf, olens[b])), all 0 when that is empty or olens[b] is invalid; *status = 0 or
-// FS2_WAVEGLOW_BAD_LENGTH | FS2_WAVEGLOW_BAD_START (some starts[b] < 0).  Runs first, as wg_prep_kernel does.
-__global__ void wg_win_desc_kernel(const int64_t* __restrict__ olens, const int64_t* __restrict__ starts, int B, int L, int nf,
-                                   int64_t* __restrict__ win, int* __restrict__ status) {
-  __shared__ int bad;
-  if (threadIdx.x == 0) bad = 0;
-  __syncthreads();
-  for (int b = threadIdx.x; b < B; b += blockDim.x) {
-    const int64_t n = olens[b], s = starts[b];
-    const bool ok = n >= 1 && n <= L;
-    if (!ok) atomicOr(&bad, FS2_WAVEGLOW_BAD_LENGTH);
-    if (s < 0) atomicOr(&bad, FS2_WAVEGLOW_BAD_START);
-    const bool live = ok && s >= 0 && s < n;
-    const int64_t c1 = live ? min(s + nf, n) : 0, f0 = live ? max(s - kHalo, (int64_t)0) : 0, f1 = live ? min(c1 + kHalo, n) : 0;
-    win[kWinF * B + b] = f1 - f0;
-    win[kWinS * B + b] = (f1 - f0) * kSteps;
-    win[kWinF0 * B + b] = f0;
-    win[kWinN * B + b] = ok ? n : 0;
-    win[kWinCore0 * B + b] = live ? s - f0 : 0;
-    win[kWinCoreN * B + b] = live ? c1 - s : 0;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) *status = bad;
-}
 
 // Four standard normals for channels 4q .. 4q + 3 of step t of the utterance with seed s: Philox4x32-10 with key
 // (s mod 2^32, s / 2^32) and counter (t, q, 0, 0), Box-Muller on two pairs of 23-bit uniforms in (0, 1).
@@ -125,8 +78,8 @@ __device__ __forceinline__ float4 normal4(uint64_t seed, uint32_t t, uint32_t q)
 
 // The standard-normal draw z [B, 8, Ls] for the steps t < n_b = min(lens[b] * mult, Ls): from zin ([B, 8, ldz]) or from
 // Philox keyed by seeds[b].  state [B * Ls][8] (nullable) = fp32(sigma * z), the product in double and rounded once;
-// zout [B, 8, Ls] (nullable) = z; both 0 for t >= n_b.  zin is never read there.  win (a window): local step t is global
-// step f0 * 32 + t, in zin and in the Philox counter alike.
+// zout [B, 8, Ls] (nullable) = z; both 0 for t >= n_b.  zin is never read there.  win (a window's step rows): local step t
+// is global step start + t, in zin and in the Philox counter alike.
 __global__ void wg_noise_kernel(const float* __restrict__ zin, int ldz, const int64_t* __restrict__ seeds, const int64_t* __restrict__ lens,
                                 const int64_t* __restrict__ win, int mult, int B, int Ls, double sigma, float* __restrict__ state,
                                 float* __restrict__ zout) {
@@ -138,7 +91,7 @@ __global__ void wg_noise_kernel(const float* __restrict__ zin, int ldz, const in
     n = n < 0 ? 0 : (n > Ls ? Ls : n);
     float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
     if (t < n) {
-      const long tg = win ? win[kWinF0 * B + b] * kSteps + t : t;
+      const long tg = (long)rows_of(win, lens, B, b).start + t;
       if (zin) {
         const float* zb = zin + ((long)b * kGroup + 4 * q) * ldz + tg;
         z = make_float4(zb[0], zb[ldz], zb[2L * ldz], zb[3L * ldz]);
@@ -157,9 +110,9 @@ __global__ void wg_noise_kernel(const float* __restrict__ zin, int ldz, const in
 }
 
 // upsampling operand [B * L][4 * 80]: tap j of frame row t = mel frame t - 3 + j of its utterance, 0 outside [0, n).
-// Rows t >= n are not written (the GEMM writes 0 there); frames past olens[b] are never read.  mels has Lm frames per
-// utterance.  win (a window, n = the buffer's frames): row t is global frame f0 + t, and the source is 0 outside
-// [0, olens[b]), so every row equals the whole call's.
+// Rows t >= len are not written (the GEMM writes 0 there); frames past olens[b] are never read.  mels has Lm frames per
+// utterance.  win (a window's frames): row t is global frame start + t, and the source is 0 outside [0, n = olens[b]), so
+// every row equals the whole call's.
 template <int OUT>
 __global__ void wg_up_operand_kernel(const float* __restrict__ mels, const int64_t* __restrict__ lensF, const int64_t* __restrict__ win,
                                      int B, int L, int Lm, float* __restrict__ out32, __half* __restrict__ outp, int* __restrict__ status) {
@@ -168,11 +121,12 @@ __global__ void wg_up_operand_kernel(const float* __restrict__ mels, const int64
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const long row = i / Q;
     const int k = (int)(i - row * Q) * 4, j = k / kMels, c = k - j * kMels;
-    const int b = (int)(row / L), t = (int)(row - (long)b * L), n = (int)lensF[b];
-    if (t >= n) continue;
-    const int src = t - (kUpTaps - 1) + j + (win ? (int)win[kWinF0 * B + b] : 0), lim = win ? (int)win[kWinN * B + b] : n;
+    const int b = (int)(row / L), t = (int)(row - (long)b * L);
+    const Rows r = rows_of(win, lensF, B, b);
+    if (t >= r.len) continue;
+    const int src = r.start + t - (kUpTaps - 1) + j;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (src >= 0 && src < lim) v = *reinterpret_cast<const float4*>(mels + ((long)b * Lm + src) * kMels + c);
+    if (src >= 0 && src < r.n) v = *reinterpret_cast<const float4*>(mels + ((long)b * Lm + src) * kMels + c);
     store_quad<OUT, RANGE_IF_STATUS>(v, row * kUpK + k, out32, outp, plane, status, FS2_WAVEGLOW_RANGE);
   }
 }
@@ -194,7 +148,7 @@ __global__ void wg_planes_kernel(const float* __restrict__ x, const int64_t* __r
 
 // WN start: x[r][n] = bias[n] + sum_{q < h} w[n][q] * state[r][o + q] for t < lens[b], else 0 -- fp32 rows (the residual
 // stream) and, in the plane modes, the in-layer GEMM's operand planes.  Padded rows are written: the dilated taps read them.
-// win / margin (a window): only exact rows are range-checked.
+// win / margin (a window's step rows): only exact rows are range-checked.
 template <int OUT>
 __global__ void wg_start_kernel(const float* __restrict__ state, const int64_t* __restrict__ lens, const int64_t* __restrict__ win,
                                 int margin, int B, int Ls, int C, int o, int h, const float* __restrict__ w, const float* __restrict__ bias,
@@ -219,14 +173,14 @@ __global__ void wg_start_kernel(const float* __restrict__ state, const int64_t* 
     }
     *reinterpret_cast<float4*>(x + row * C + n) = v;
     if (OUT != OUT_F32)
-      store_quad<OUT, RANGE_IF_STATUS>(v, row * C + n, nullptr, xp, plane, !win || exact_row(win, B, b, t, margin) ? status : nullptr,
+      store_quad<OUT, RANGE_IF_STATUS>(v, row * C + n, nullptr, xp, plane, exact_row(rows_of(win, lens, B, b), t, margin) ? status : nullptr,
                                        FS2_WAVEGLOW_RANGE);
   }
 }
 
 // gate: acts[r][c] = tanh(ia[r][c]) * sigmoid(ia[r][C + c]) as the res / skip GEMMs' operand (rows t >= lens[b] are not
 // written).  xchk (nullable, plane modes): the layer's input rows x, written as planes by the previous res GEMM's
-// epilogue, are range-checked here.  win (a window): acts only at rows exact at `margin`, x at `xmargin`.
+// epilogue, are range-checked here.  win (a window's step rows): acts only at rows exact at `margin`, x at `xmargin`.
 template <int OUT>
 __global__ void wg_gate_kernel(const float* __restrict__ ia, const float* __restrict__ xchk, const int64_t* __restrict__ lens,
                                const int64_t* __restrict__ win, int margin, int xmargin, int B, int Ls, int C, float* __restrict__ out32,
@@ -237,14 +191,14 @@ __global__ void wg_gate_kernel(const float* __restrict__ ia, const float* __rest
     const long row = i / Q;
     const int c = (int)(i - row * Q) * 4;
     const int b = (int)(row / Ls), t = (int)(row - (long)b * Ls);
-    if (t >= (int)lens[b]) continue;
+    const Rows r = rows_of(win, lens, B, b);
+    if (t >= r.len) continue;
     const float4 a = *reinterpret_cast<const float4*>(ia + row * 2 * C + c);
     const float4 g = *reinterpret_cast<const float4*>(ia + row * 2 * C + C + c);
     const float4 v = make_float4(tanhf(a.x) * (1.f / (1.f + expf(-g.x))), tanhf(a.y) * (1.f / (1.f + expf(-g.y))),
                                  tanhf(a.z) * (1.f / (1.f + expf(-g.z))), tanhf(a.w) * (1.f / (1.f + expf(-g.w))));
-    store_quad<OUT, RANGE_IF_STATUS>(v, row * C + c, out32, outp, plane, !win || exact_row(win, B, b, t, margin) ? status : nullptr,
-                                     FS2_WAVEGLOW_RANGE);
-    if (xchk && (!win || exact_row(win, B, b, t, xmargin))) {
+    store_quad<OUT, RANGE_IF_STATUS>(v, row * C + c, out32, outp, plane, exact_row(r, t, margin) ? status : nullptr, FS2_WAVEGLOW_RANGE);
+    if (xchk && exact_row(r, t, xmargin)) {
       const float4 x = *reinterpret_cast<const float4*>(xchk + row * C + c);
       if (!(fabsf(x.x) <= kPlaneMax && fabsf(x.y) <= kPlaneMax && fabsf(x.z) <= kPlaneMax && fabsf(x.w) <= kPlaneMax))
         atomicOr(status, FS2_WAVEGLOW_RANGE);
@@ -309,16 +263,17 @@ __global__ void __launch_bounds__(256) wg_flow_kernel(const float* __restrict__ 
   }
 }
 
-// a window's audio: row b (ld samples apart) = the core's samples of the final state [B * Ls][8] (utterance b's samples
-// are contiguous there), then +0 up to nf * 256
-__global__ void wg_win_audio_kernel(const float* __restrict__ state, const int64_t* __restrict__ win, int B, int Ls, int nf,
-                                    float* __restrict__ audio, long ld) {
+// a window's audio: row b (ld samples apart) = the samples of the core's step rows awin in the final state [B * Ls][8]
+// (step rows win; utterance b's samples are contiguous there), then +0 up to nf * 256
+__global__ void wg_win_audio_kernel(const float* __restrict__ state, const int64_t* __restrict__ win, const int64_t* __restrict__ awin,
+                                    int B, int Ls, int nf, float* __restrict__ audio, long ld) {
   const int n = nf * kHop;
   const long total = (long)B * n;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int b = (int)(i / n), t = (int)(i - (long)b * n);
+    const Rows r = rows_of(win, nullptr, B, b), a = rows_of(awin, nullptr, B, b);
     float v = 0.f;
-    if (t < win[kWinCoreN * B + b] * kHop) v = state[(long)b * Ls * kGroup + win[kWinCore0 * B + b] * kHop + t];
+    if (t < a.len * kGroup) v = state[((long)b * Ls + a.start - r.start) * kGroup + t];
     audio[(long)b * ld + t] = v;
   }
 }
@@ -373,9 +328,12 @@ namespace fs2 {
 namespace {
 
 struct WgPlan {
-  int64_t* win;        // a window call: the kWinRows descriptors [kWinRows][B] (lensF and lensS are its first two rows)
-  int64_t* lensF;      // [B] frame lengths (0 for a bad olens[b])
+  int64_t* lens;       // ups_prep's block: the whole call's lengths [2][B] of frames and step rows, or a window call's
+                       // n_wins(kPlan) descriptors [start | len | n][B] of frames, step rows and the audio's step rows
+  int64_t* lensF;      // [B] frame lengths in it (0 for a bad olens[b])
   int64_t* lensS;      // [B] step lengths = lensF * 32
+  int64_t* winF;       // a window call: the descriptors of its frames and its step rows (nullptr: whole utterances)
+  int64_t* winS;
   void* up_a;          // upsampling operand [B * L][320]
   float* cond;         // upsampled mels as fp32 step rows [B * Ls][640].  The plane modes need them only until the
                        // planes are written, before ia is first used, so there they alias ia when its rows hold 640
@@ -408,15 +366,12 @@ WgPlan plan(Bump& b, int mode, int C, int B, int L, bool window = false) {
   const size_t frames = (size_t)B * L, rows = frames * kSteps;
   const bool planes = plane_mode(mode);
   WgPlan p;
-  if (window) {
-    p.win = (int64_t*)b.bytes((size_t)kWinRows * B * sizeof(int64_t));
-    p.lensF = p.win ? p.win + kWinF * B : nullptr;
-    p.lensS = p.win ? p.win + kWinS * B : nullptr;
-  } else {
-    p.win = nullptr;
-    p.lensF = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
-    p.lensS = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
-  }
+  p.lens = (int64_t*)b.bytes((size_t)(window ? 3 * n_wins(kPlan) : kPlan.n + 1) * B * sizeof(int64_t));
+  auto row = [&](int i) { return p.lens ? p.lens + (long)i * B : nullptr; };
+  p.lensF = row(window ? 3 * win_level(0) + 1 : 0);
+  p.lensS = row(window ? 3 * win_level(1) + 1 : 1);
+  p.winF = window ? row(3 * win_level(0)) : nullptr;
+  p.winS = window ? row(3 * win_level(1)) : nullptr;
   p.up_a = b.floats(frames * kUpK);                   // fp32 rows, or hi + lo planes: the same bytes
   p.state = b.floats(rows * kGroup);
   plan_wn(b, p, planes, C, rows);
@@ -468,7 +423,7 @@ int upsample(const fs2_waveglow_net* m, const WgPlan& p, const float* mels, int 
   int rc;
   {
     auto k = pick(kind, wg_up_operand_kernel<OUT_HILO>, wg_up_operand_kernel<OUT_HI>, wg_up_operand_kernel<OUT_F32>);
-    k<<<grid_for((long)B * L * (kUpK / 4), 256), 256, 0, st>>>(mels, p.lensF, p.win, B, L, Lm, (float*)p.up_a, (__half*)p.up_a, status);
+    k<<<grid_for((long)B * L * (kUpK / 4), 256), 256, 0, st>>>(mels, p.lensF, p.winF, B, L, Lm, (float*)p.up_a, (__half*)p.up_a, status);
     FS2_LAUNCH_CHECK();
   }
   if ((rc = vweight_gemm(m->math_mode, m->up, p.up_a, B, L, ACT_NONE, p.lensF, p.cond, st))) return rc;
@@ -489,7 +444,7 @@ int flow(const fs2_waveglow_net* m, int k, const WgPlan& p, const void* cond_a, 
   const int kind = out_kind(m->math_mode), C = m->C;
   const bool planes = plane_mode(m->math_mode);
   const long rows = (long)B * Ls;
-  const int64_t* win = p.win;
+  const int64_t* win = p.winS;
   const WFlow& f = m->flows[k];
   const int c = flow_channels(k), h = c / 2, o = kGroup - c;
   const int exact = (kFlows - 1 - k) * kFlowReach;          // a window's rows are exact this far from an interior side
@@ -519,7 +474,7 @@ int flow(const fs2_waveglow_net* m, int k, const WgPlan& p, const void* cond_a, 
 }
 
 // The inverse flow on the plan p: whole utterances (starts == nullptr; buffers of Lmax frames, audio written by the last
-// flow) or a window of nf frames from starts[b] (buffers of nf + 2H frames, the window descriptors p.win, the core copied
+// flow) or a window of nf frames from starts[b] (buffers of nf + 2H frames, the window descriptors p.lens, the core copied
 // out by wg_win_audio_kernel).  audio rows ld samples apart.  Both enqueue the same kernels but the first and the last.
 int run(const fs2_waveglow_net* m, const WgPlan& p, const float* mels, const int64_t* olens, const int64_t* starts, int B, int Lmax,
         int nf, double sigma, const int64_t* seeds, const float* z, float* audio, long ld, int* status, cudaStream_t st) {
@@ -529,19 +484,16 @@ int run(const fs2_waveglow_net* m, const WgPlan& p, const float* mels, const int
   const long rows = (long)B * Ls;
   int rc;
 
-  if (window)
-    wg_win_desc_kernel<<<1, 256, 0, st>>>(olens, starts, B, Lmax, nf, p.win, status);
-  else
-    wg_prep_kernel<<<1, 256, 0, st>>>(olens, B, Lmax, 1, p.lensF, p.lensS, status);
-  FS2_LAUNCH_CHECK();
-  wg_noise_kernel<<<grid_for(rows * 2, 256), 256, 0, st>>>(z, Lmax * kSteps, seeds, p.lensS, p.win, 1, B, Ls, sigma, p.state, nullptr);
+  if ((rc = ups_prep(olens, starts, B, 1, Lmax, nf, kPlan, p.lens, status, st))) return rc;
+  wg_noise_kernel<<<grid_for(rows * 2, 256), 256, 0, st>>>(z, Lmax * kSteps, seeds, p.lensS, p.winS, 1, B, Ls, sigma, p.state, nullptr);
   FS2_LAUNCH_CHECK();
   const void* cond_a = nullptr;
   if ((rc = upsample(m, p, mels, B, L, Lmax, status, st, &cond_a))) return rc;
   for (int k = kFlows - 1; k >= 0; --k)
     if ((rc = flow(m, k, p, cond_a, p.state, k == 0 && !window ? audio : p.state, B, Ls, status, st))) return rc;
   if (window) {
-    wg_win_audio_kernel<<<grid_for((long)B * nf * kHop, 256), 256, 0, st>>>(p.state, p.win, B, Ls, nf, audio, ld);
+    wg_win_audio_kernel<<<grid_for((long)B * nf * kHop, 256), 256, 0, st>>>(p.state, p.winS, p.lens + 3L * win_audio(kPlan) * B, B, Ls,
+                                                                           nf, audio, ld);
     FS2_LAUNCH_CHECK();
   }
   return FS2_OK;
@@ -567,11 +519,7 @@ int fs2_waveglow_create(fs2_waveglow_net** out, int math_mode, int n_channels) {
   return FS2_OK;
 }
 
-void fs2_waveglow_destroy(fs2_waveglow_net* m) {
-  if (!m) return;
-  if (m->arena) cudaFree(m->arena);
-  delete m;
-}
+void fs2_waveglow_destroy(fs2_waveglow_net* m) { destroy_gen(m); }
 
 int fs2_waveglow_load(fs2_waveglow_net* m, const float* const* t, int n, void* stream) {
   FS2_REQUIRE(m && t, "fs2_waveglow_load: null argument");
@@ -712,8 +660,8 @@ int fs2_waveglow_window(fs2_waveglow_net* m, const float* mels, const int64_t* o
 
 // ---- stages of the inverse on the vocoder's own code paths (tests) --------------------------------------------------
 // Both run what fs2_waveglow runs for that stage, on a loaded handle's packed weights, with the buffers in a stream-ordered
-// temporary.  The length pass is wg_prep_kernel's with 0 allowed: a length outside [0, L] is 0 and sets
-// FS2_WAVEGLOW_BAD_LENGTH, so it never becomes an out-of-bounds row.
+// temporary.  The length pass is ups_prep's with 0 allowed: a length outside [0, L] is 0 and sets FS2_WAVEGLOW_BAD_LENGTH,
+// so it never becomes an out-of-bounds row.
 int fs2_op_waveglow_upsample(fs2_waveglow_net* m, const float* mels, const int64_t* olens, int B, int Lmax, float* cond,
                              float* cond_planes, int* status, void* stream) {
   const char* who = "fs2_op_waveglow_upsample";
@@ -731,16 +679,16 @@ int fs2_op_waveglow_upsample(fs2_waveglow_net* m, const float* mels, const int64
   WgPlan p{};
   void* base = nullptr;
   if ((rc = temp_carve(&base, st, [&](Bump& b) {
-         p.lensF = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
-         p.lensS = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
+         p.lens = (int64_t*)b.bytes((size_t)(kPlan.n + 1) * B * sizeof(int64_t));
          p.up_a = b.floats((size_t)B * Lmax * kUpK);
          p.condp = planes ? (__half*)b.floats((size_t)rows * kCond) : nullptr;   // hi + lo planes
        })))
     return rc;
+  p.lensF = p.lens;
+  p.lensS = p.lens + B;
   p.cond = cond;
   auto enqueue = [&]() -> int {      // every error returns here, so that the temporary is released on every path
-    wg_prep_kernel<<<1, 256, 0, st>>>(olens, B, Lmax, 0, p.lensF, p.lensS, status);
-    FS2_LAUNCH_CHECK();
+    if (int r = ups_prep(olens, nullptr, B, 0, Lmax, 0, kPlan, p.lens, status, st)) return r;
     // the planes of rows past lens are never written: zeros there (and in f16's unused lo plane) read back as +0
     if (planes) FS2_CUDA_CHECK(cudaMemsetAsync(p.condp, 0, (size_t)rows * kCond * sizeof(float), st));
     const void* cond_a = nullptr;
@@ -772,13 +720,12 @@ int fs2_op_waveglow_flow(fs2_waveglow_net* m, int k, const float* cond, const fl
   WgPlan p{};
   void* base = nullptr;
   if ((rc = temp_carve(&base, st, [&](Bump& b) {
-         p.lensS = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));
+         p.lensS = (int64_t*)b.bytes((size_t)B * sizeof(int64_t));      // ups_prep's block for kStepPlan
          if (!skip_in) plan_wn(b, p, planes, m->C, (size_t)rows);
        })))
     return rc;
   auto enqueue = [&]() -> int {      // every error returns here, so that the temporary is released on every path
-    wg_prep_kernel<<<1, 256, 0, st>>>(lens, B, Ls, 0, p.lensS, nullptr, status);
-    FS2_LAUNCH_CHECK();
+    if (int r = ups_prep(lens, nullptr, B, 0, Ls, 0, kStepPlan, p.lensS, status, st)) return r;
     if (skip_in) return flow_tail(m, k, skip_in, state_in, state_out, p.lensS, B, Ls, st);
     const void* cond_a = cond;
     if (planes) {     // the cond planes with the range check, as the vocoder's upsampling writes them

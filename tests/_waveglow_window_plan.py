@@ -9,7 +9,7 @@ STEPS = HOP // N_GROUP                       # 32 step rows per frame
 N_FLOWS, N_LAYERS, KERNEL = 12, 8, 3
 DILATIONS = [2 ** i for i in range(N_LAYERS)]
 UP_KERNEL, UP_STRIDE = 1024, 256             # ConvTranspose1d(80, 80, 1024, stride 256)
-N_DESC = 6                                   # window descriptors per utterance (kWinRows)
+N_WINS = 3                                   # window descriptors [start | len | n]: frames, step rows, the audio
 
 
 def layer_reach(i: int) -> int:
@@ -111,12 +111,13 @@ def _carve(sizes) -> int:
 def workspace_bytes(C: int, planes: bool, B: int, n_frames: int) -> int:
     """fs2_waveglow_window_workspace_bytes: the window descriptors, then the whole call's buffers for B utterances of
     n + 2H frames, each 256-byte aligned, plus 256 bytes of slack for the base pointer's alignment."""
-    return _carve([N_DESC * B * 8] + _buffers(C, B * buffer_frames(n_frames), planes))
+    return _carve([3 * N_WINS * B * 8] + _buffers(C, B * buffer_frames(n_frames), planes))
 
 
 def whole_call_workspace_bytes(C: int, planes: bool, B: int, L: int) -> int:
-    """fs2_waveglow_workspace_bytes: the two length vectors and the buffers for B utterances of Lmax frames."""
-    return _carve([B * 8, B * 8] + _buffers(C, B * L, planes))
+    """fs2_waveglow_workspace_bytes: the lengths [2][B] of frames and step rows and the buffers for B utterances of Lmax
+    frames."""
+    return _carve([2 * B * 8] + _buffers(C, B * L, planes))
 
 
 def window_flop_overhead(n_frames: int, sides: int = 2) -> float:

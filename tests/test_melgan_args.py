@@ -286,7 +286,8 @@ def test_shared_weight_pack_kernels_do_not_spill():
 
 
 def test_shared_window_prep_kernel_does_not_spill():
-    """The one prep kernel MelGAN and HiFi-GAN write their lengths and window descriptors with (csrc/vocoder_window.cu)."""
+    """The one prep kernel MelGAN, HiFi-GAN and WaveGlow write their lengths and window descriptors with
+    (csrc/vocoder_window.cu)."""
     reports = glob.glob(os.path.join(REPO, "fastspeech2_b200", "build", "vocoder_window.ptxas.txt"))
     if not reports:
         pytest.skip("no ptxas reports (library built elsewhere)")

@@ -126,7 +126,7 @@ def _ws(lib, h, B, n):
 
 
 @pytest.mark.gpu          # fs2_waveglow_create needs a device; the checks themselves run on the host
-def test_window_workspace_is_the_plan_and_independent_of_lmax(handle):
+def test_window_workspace_is_the_shared_plan_and_independent_of_lmax(handle):
     lib = _lib.load()
     for (mode, C_), h in handle.items():
         planes = mode != _lib.MATH_FP32
@@ -313,16 +313,15 @@ def test_case_table_reaches_every_window_shape():
 
 
 # ---- ptxas ----------------------------------------------------------------------------------------------------------
-def test_window_kernels_do_not_spill():
+def test_window_audio_kernel_does_not_spill():
     reports = glob.glob(os.path.join(REPO, "fastspeech2_b200", "build", "waveglow.ptxas.txt"))
     if not reports:
         pytest.skip("no ptxas reports (library built elsewhere)")
     text = open(reports[0]).read()
-    for kernel in ("wg_win_desc_kernel", "wg_win_audio_kernel"):
-        props = re.findall(r"Function properties for \S*%s\S*\n(.*)" % kernel, text)
-        assert len(props) == 1, (kernel, len(props))
-        assert "0 bytes spill stores, 0 bytes spill loads" in props[0], (kernel, props[0])
+    props = re.findall(r"Function properties for \S*wg_win_audio_kernel\S*\n(.*)", text)
+    assert len(props) == 1, len(props)
+    assert "0 bytes spill stores, 0 bytes spill loads" in props[0], props[0]
     props = re.findall(r"Function properties for (\S*wg_\S*)\n(.*)", text)
-    assert len(props) == 19 + 2                            # the whole call's 19 instantiations and the two window kernels
+    assert len(props) == 18 + 1                            # the whole call's 18 instantiations and the window's audio copy
     for name, line in props:
         assert "0 bytes spill stores, 0 bytes spill loads" in line, (name, line)
