@@ -61,6 +61,8 @@ FS2_ISTFTNET_BAD_LENGTH, FS2_ISTFTNET_RANGE, FS2_ISTFTNET_BAD_START = 1, 2, 4   
 FS2_EVAL_BAD_LENGTH, FS2_EVAL_NONFINITE = 1, 2   # bits of fs2_mcd_dtw's / fs2_path_prosody's status word
 FS2_RS_BAD_LENGTH, FS2_RS_NONFINITE = 1, 2       # bits of fs2_resample's status word
 FS2_WORLD_BAD_LENGTH, FS2_WORLD_NONFINITE, FS2_WORLD_F0_RANGE = 1, 2, 4   # bits of fs2_stonemask's / fs2_cheaptrick's / fs2_mcep's
+FS2_ALIGN_BAD_LENGTH, FS2_ALIGN_INFEASIBLE, FS2_ALIGN_NONFINITE = 1, 2, 4   # bits of the fs2_align_* status word
+FS2_ALIGN_DIM, FS2_ALIGN_MAX_T = 80, 1024
 FS2_RESAMPLE_TABLE = 32769                        # entries of the resampling filter's right wing
 FS2_PLAN_BAD_ILENS,FS2_PLAN_BAD_CONTROL, FS2_PLAN_OVERFLOW = 1, 2, 4   # bits of fs2_length_plan_cap's status word
 FS2_SYNTH_VOC_SHIFT = 8                          # fs2_synth_status: the vocoder's bits sit this far up in the word
@@ -181,6 +183,13 @@ SIGNATURES = {
     "fs2_mcep": [C.POINTER(WorldConfig), _P, _P, _I, _I, _P, _P, _I, _P, _P, _P, _SZ, _P],
     "fs2_resample_workspace_bytes": [_I, _I, _I, _I, _I, C.POINTER(_SZ)],
     "fs2_resample": [_P, _P, _I, _I, _P, _I, _I, _P, _P, _I, _P, _P, _SZ, _P],
+    "fs2_align_workspace_bytes": [_I, _I, _I, C.POINTER(_SZ)],
+    "fs2_align_logprob": [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_align_logprob_backward": [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _SZ, _P],
+    "fs2_align_forward_sum": [_P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _SZ, _P],
+    "fs2_align_mas": [_P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _SZ, _P],
+    "fs2_align_bin_loss": [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _SZ, _P],
+    "fs2_align_mask_rows": [_P, _P, _I, _I, _I, _P, _P],
     "fs2_melgan_create": [C.POINTER(_P), _I],
     "fs2_melgan_load": [_P, C.POINTER(_P), C.POINTER(_P), _P],
     "fs2_melgan_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],

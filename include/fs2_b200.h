@@ -594,6 +594,52 @@ int fs2_resample_workspace_bytes(int B, int Nmax, int sr_orig, int sr_new, int M
 int fs2_resample(const float* x, const int64_t* lens, int B, int Nmax, const double* table, int sr_orig, int sr_new, float* y,
                  int64_t* olens, int Mmax, int* status, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- unsupervised duration aligner: forward-sum attention and MAS (DESIGN.md section 24) -------------------------- */
+/* The hot path of Badlani et al.'s alignment module (FastPitch 1.1) for a ragged batch; fastspeech2_b200/aligner.py drives
+ * it.  q [B, L, FS2_ALIGN_DIM] fp32 (frames), k [B, T, FS2_ALIGN_DIM] fp32 (phonemes); utterance b has M = olens[b]
+ * frames and N = ilens[b] phonemes.  Rows at or past the lengths are never read.
+ *   fs2_align_logprob           logp [B, L, T] = log_softmax_{t < N}(-0.0005 sum_c (q[l,c] - k[t,c])^2)
+ *                               + (float)log(betabinom(N, l + 1, M - l).pmf(t) + 1e-8) (prior in float64, lgamma) for
+ *                               l < M, t < N; +0 elsewhere
+ *   fs2_align_logprob_backward  dq [B, L, D], dk [B, T, D] from dlogp [B, L, T] (rows past the lengths +0); dk sums the
+ *                               frames in ascending order
+ *   fs2_align_forward_sum       loss [B]: CTC NLL of the labels 1..N over M frames of log_softmax([-1, logp[l, :N]])
+ *                               (blank 0), divided by N (ctc_loss reduction="mean", zero_infinity=True on one utterance);
+ *                               dlogp [B, L, T] (nullable) = dloss[b] (NULL: 1) * its gradient, (softmax - posterior
+ *                               occupancy) / N on the label columns, +0 elsewhere
+ *   fs2_align_mas               FastPitch's mas_width1 on log soft = logp - lse (lse per frame in float64, rounded once):
+ *                               row 0 starts at t = 0, v[l,t] = log soft[l,t] + max(v[l-1,t], v[l-1,t-1]) with t - 1
+ *                               winning ties, backtracked from (M-1, N-1).  durations [B, T] int64 (each >= 1 for t < N,
+ *                               summing to M; 0 past N), path [B, L] int32 (phoneme of each frame; -1 past M)
+ *   fs2_align_bin_loss          loss [B] = -sum_{l<M} log(max(soft[l, path[l]], 1e-12)) / M; dlogp (nullable) =
+ *                               dloss[b] (NULL: 1) * its gradient, +0 elsewhere
+ *   fs2_align_mask_rows         y[b, t, :] = x[b, t, :] for t < lens[b], +0 past it (x may be y)
+ * Float32 on the CUDA cores; no floating-point atomics, every sum in a fixed order that depends on the utterance's own
+ * lengths only: utterance b is bit-identical to a B = 1 call.  No allocation, no synchronisation.  Data-dependent checks
+ * are reported in *status (device int, zeroed by the call); each affected utterance's outputs are 0 (durations 0, path -1):
+ *   FS2_ALIGN_BAD_LENGTH   ilens[b] outside [1, T] or olens[b] outside [1, L] (bin loss: or a path index outside [0, N));
+ *   FS2_ALIGN_INFEASIBLE   olens[b] < ilens[b]: no monotonic alignment gives every phoneme a frame;
+ *   FS2_ALIGN_NONFINITE    a NaN or inf in the rows an entry reads (q, k; or logp).
+ * Sizes: B in [1, 65535], L in [1, 2^20], T in [1, FS2_ALIGN_MAX_T].  Workspace (fs2_align_workspace_bytes, one size
+ * for every entry, 256-byte aligned): align256(4 B) + align256(4 B L) + 4 B L (2 T + 1) bytes. */
+#define FS2_ALIGN_DIM 80
+#define FS2_ALIGN_MAX_T 1024
+#define FS2_ALIGN_BAD_LENGTH 1
+#define FS2_ALIGN_INFEASIBLE 2
+#define FS2_ALIGN_NONFINITE 4
+int fs2_align_workspace_bytes(int B, int L, int T, size_t* bytes);
+int fs2_align_logprob(const float* q, const float* k, const int64_t* ilens, const int64_t* olens, int B, int L, int T, float* logp,
+                      int* status, void* ws, size_t ws_bytes, void* stream);
+int fs2_align_logprob_backward(const float* q, const float* k, const int64_t* ilens, const int64_t* olens, int B, int L, int T,
+                               const float* dlogp, float* dq, float* dk, int* status, void* ws, size_t ws_bytes, void* stream);
+int fs2_align_forward_sum(const float* logp, const int64_t* ilens, const int64_t* olens, int B, int L, int T, const float* dloss,
+                          float* loss, float* dlogp, int* status, void* ws, size_t ws_bytes, void* stream);
+int fs2_align_mas(const float* logp, const int64_t* ilens, const int64_t* olens, int B, int L, int T, int64_t* durations,
+                  int32_t* path, int* status, void* ws, size_t ws_bytes, void* stream);
+int fs2_align_bin_loss(const float* logp, const int32_t* path, const int64_t* ilens, const int64_t* olens, int B, int L, int T,
+                       const float* dloss, float* loss, float* dlogp, int* status, void* ws, size_t ws_bytes, void* stream);
+int fs2_align_mask_rows(const float* x, const int64_t* lens, int B, int L, int C, float* y, void* stream);
+
 /* ---- batched MelGAN vocoder (DESIGN.md section 8) ------------------------------------------------------------------- */
 /* seungwonpark/melgan's Generator(mel_channel = 80) on log-mels [B, Lmax, 80] with frame counts olens [B]: utterance b is
  * the generator applied to its own frames mels[b, :olens[b]] followed by 10 frames of -11.5129, every reflection pad at its
