@@ -65,6 +65,7 @@ FS2_ALIGN_BAD_LENGTH, FS2_ALIGN_INFEASIBLE, FS2_ALIGN_NONFINITE = 1, 2, 4   # bi
 FS2_ALIGN_DIM, FS2_ALIGN_MAX_T = 80, 1024
 FS2_RESAMPLE_TABLE = 32769                        # entries of the resampling filter's right wing
 FS2_PLAN_BAD_ILENS,FS2_PLAN_BAD_CONTROL, FS2_PLAN_OVERFLOW = 1, 2, 4   # bits of fs2_length_plan_cap's status word
+FS2_PLAN_BAD_SPEAKER = 8                          # and of fs2_length_plan_cap_spk's
 FS2_SYNTH_VOC_SHIFT = 8                          # fs2_synth_status: the vocoder's bits sit this far up in the word
 
 
@@ -109,11 +110,13 @@ SIGNATURES = {
     "fs2_workspace_bytes": [_P, _I, _I, _I, C.POINTER(_SZ)],
     "fs2_encode": [_P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _P],
     "fs2_encode_ex": [_P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _I, _P],
+    "fs2_encode_spk": [_P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _I, _P],
     "fs2_length_plan": [_P, _I, _P, _F, _I, _I, _I, _P, _P, _P, _P],
     "fs2_length_gather": [_P, _P, _P, _I, _I, _I, _P, _I, _P],
     "fs2_length_plan_ex": [_P, _I, _P, _F, _P, _I, _I, _I, _P, _P, _P, _P, _P],
     "fs2_length_gather_ex": [_P, _P, _P, _I, _I, _I, _P, _I, _P, _P, _P],
     "fs2_length_plan_cap": [_P, _I, _P, _P, _P, _I, _I, _L, _P, _P, _P, _P, _P, _P],
+    "fs2_length_plan_cap_spk": [_P, _I, _P, _P, _P, _P, _I, _I, _I, _L, _P, _P, _P, _P, _P, _P],
     "fs2_synth_status": [_P, _P, _P, _I, _I, _P, _P, _P],
     "fs2_decode": [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _SZ, _P],
     "fs2_decode_ex": [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _SZ, _I, _P],
@@ -153,6 +156,9 @@ SIGNATURES = {
     "fs2_embed_posenc": [_P, _P, _I, _P, _P, _I, _I, _I, _P, _P],
     "fs2_embed_backward": [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P],
     "fs2_posenc_add": [_P, _P, _P, _I, _I, _I, _P, _P],
+    "fs2_speaker_add": [_P, _P, _P, _I, _I, _I, _I, _P, _P],
+    "fs2_speaker_add_backward_ws_bytes": [_I, _I, C.POINTER(_SZ)],
+    "fs2_speaker_add_backward": [_P, _P, _I, _I, _I, _I, _P, _P, _SZ, _P],
     "fs2_onehot_linear_forward": [_P, _P, _P, _P, _L, _I, _I, _P, _P],
     "fs2_onehot_linear_backward": [_P, _P, _L, _I, _I, _P, _P, _P],
     "fs2_length_regulator_backward": [_P, _P, _P, _I, _I, _I, _I, _P, _P],

@@ -5,7 +5,8 @@ al., "One TTS Alignment To Rule Them All" (2021), as FastPitch 1.1 builds it, tr
     python -m fastspeech2_b200.aligner extract -c config.yaml --filelist FILE [-d DATA_DIR] -p aligner.pt --out NEW_FILELIST
 
 Filelist lines are the reference's five `|` fields: text, boundaries, durations, phonemes, wav name (fields 1 and 2 may
-be empty).  Mels are read from `{data_dir}/mels/{id}.npy` of a `preprocess` tree, id = the wav name up to its first dot,
+be empty), optionally followed by a sixth, the speaker name (`python -m fastspeech2_b200.speakers tag`), which `extract`
+carries through.  Mels are read from `{data_dir}/mels/{id}.npy` of a `preprocess` tree, id = the wav name up to its first dot,
 as the reference's `TTSDataset` does.  `extract` writes the same lines with field 2 replaced by the durations found by
 monotonic alignment search, which sum to the mel's frame count, so the reference's loader trains on them unchanged (its
 last-duration correction then changes nothing).  Field 1 becomes the start frame 0 followed by the cumulative end frame
@@ -44,11 +45,13 @@ STATUS_MESSAGES = [(_lib.FS2_ALIGN_BAD_LENGTH, "lengths outside [1, T] / [1, L] 
 
 # ---- filelists -------------------------------------------------------------------------------------------------------
 class Line:
-    """One filelist line: text | boundaries | durations | phonemes | wav name."""
-    __slots__ = ("text", "boundaries", "durations", "phonemes", "wav")
+    """One filelist line: text | boundaries | durations | phonemes | wav name [| speaker name]."""
+    __slots__ = ("text", "boundaries", "durations", "phonemes", "wav", "speaker")
 
-    def __init__(self, text: str, boundaries: Optional[List[int]], durations: Optional[List[int]], phonemes: List[str], wav: str):
+    def __init__(self, text: str, boundaries: Optional[List[int]], durations: Optional[List[int]], phonemes: List[str], wav: str,
+                 speaker: Optional[str] = None):
         self.text, self.boundaries, self.durations, self.phonemes, self.wav = text, boundaries, durations, phonemes, wav
+        self.speaker = speaker
 
     @property
     def id(self) -> str:
@@ -56,10 +59,16 @@ class Line:
 
 
 def parse_line(line: str, where: str = "line") -> Line:
-    """A filelist line -> Line; empty fields 1 and 2 give None.  Raises ValueError naming `where` on a malformed line."""
+    """A filelist line -> Line; empty fields 1 and 2 give None, and a line without the sixth (speaker) field gives
+    speaker None.  Raises ValueError naming `where` on a malformed line."""
     f = line.rstrip("\r\n").split("|")
-    if len(f) != 5:
-        raise ValueError(f"{where}: expected 5 '|'-separated fields, found {len(f)}")
+    if len(f) not in (5, 6):
+        raise ValueError(f"{where}: expected 5 '|'-separated fields, found {len(f)} (a sixth, the speaker name, is optional)")
+    speaker = None
+    if len(f) == 6:
+        speaker = f[5].strip()
+        if not speaker:
+            raise ValueError(f"{where}: empty speaker field")
     ints = []
     for k in (1, 2):
         try:
@@ -73,7 +82,7 @@ def parse_line(line: str, where: str = "line") -> Line:
         raise ValueError(f"{where}: no wav name")
     if ints[1] is not None and len(ints[1]) != len(phonemes):
         raise ValueError(f"{where}: {len(ints[1])} durations for {len(phonemes)} phonemes")
-    return Line(f[0], ints[0], ints[1], phonemes, f[4].strip())
+    return Line(f[0], ints[0], ints[1], phonemes, f[4].strip(), speaker)
 
 
 def read_filelist(path: str) -> List[Line]:
@@ -82,10 +91,12 @@ def read_filelist(path: str) -> List[Line]:
 
 
 def format_line(line: Line, durations: Sequence[int]) -> str:
-    """`line` with field 2 = durations and field 1 = 0 followed by their cumulative end frames."""
+    """`line` with field 2 = durations and field 1 = 0 followed by their cumulative end frames (and its speaker field,
+    if it has one)."""
     d = [int(v) for v in durations]
     ends = np.cumsum([0] + d).tolist()
-    return "|".join([line.text, " ".join(map(str, ends)), " ".join(map(str, d)), " ".join(line.phonemes), line.wav])
+    fields = [line.text, " ".join(map(str, ends)), " ".join(map(str, d)), " ".join(line.phonemes), line.wav]
+    return "|".join(fields + ([line.speaker] if line.speaker is not None else []))
 
 
 def build_symbols(lines: Sequence[Line]) -> List[str]:

@@ -75,6 +75,7 @@ struct fs2_handle {
   const float* e_bins = nullptr; const float* p_bins = nullptr;
   const float* e_tab = nullptr; const float* e_tab_bias = nullptr;
   const float* p_tab = nullptr; const float* p_tab_bias = nullptr;
+  const float* spk_table = nullptr; int n_speakers = 0;   // optional speaker_embed.weight [n_speakers, adim]
   // decoder side
   fs2::VWeight dec_in; fs2::Norm dec_in_ln; const float* dec_pe = nullptr; const float* dec_alpha = nullptr;
   fs2::VWeight feat_out;
@@ -135,6 +136,9 @@ RowNorm masked(RowNorm r, const int64_t* zlens, int L) {
   return r;
 }
 
+// the speaker add of the last encoder LayerNorm (RowNorm::spk_table); table == nullptr: none
+struct SpeakerAdd { const float* table = nullptr; const int64_t* ids = nullptr; int n = 0; };
+
 struct BlockBufs {
   float *x, *y;            // fp32 rows [rows, C]: block input / output ping-pong (the residual stream)
   float *qkv, *vt, *ctx, *hid;   // fp32 families: q|k|v rows, transposed V, context, conv-FFN hidden
@@ -146,7 +150,7 @@ struct BlockBufs {
 // only for the residual stream (x, y), and residual + LayerNorm run as a row kernel after each projection.  On entry w.xp
 // holds the planes of w.x; on exit it holds the planes of *result.
 int run_blocks(const std::vector<Block>& blocks, const BlockBufs& w, const int64_t* lens, const int64_t* zlens, int B, int L,
-               int C, int heads, int mode, bool is_dec, cudaStream_t st, float** result) {
+               int C, int heads, int mode, bool is_dec, cudaStream_t st, float** result, const SpeakerAdd& spk = SpeakerAdd()) {
   const int64_t rows = (int64_t)B * L;
   const int c_qkv = is_dec ? P_DEC_QKV : P_ENC_QKV, c_att = is_dec ? P_DEC_ATTN : P_ENC_ATTN;
   const int c_out = is_dec ? P_DEC_OUT : P_ENC_OUT, c_w1 = is_dec ? P_DEC_W1 : P_ENC_W1, c_w2 = is_dec ? P_DEC_W2 : P_ENC_W2;
@@ -189,6 +193,7 @@ int run_blocks(const std::vector<Block>& blocks, const BlockBufs& w, const int64
       return rc;
     RowNorm r2 = masked(make_norm(k.ln2, y, C, rows, C, x, C), zlens, L);
     if (planes) { r2.split_out = w.xp; r2.split_lo = x3; }   // planes of the block output: A operand of the next q|k|v / mel projection
+    if (spk.table && &k == &blocks.back()) { r2.spk_table = spk.table; r2.spk = spk.ids; r2.n_spk = spk.n; r2.spk_L = L; }
     if ((rc = norm_rows(r2, st))) return rc;
   }
   *result = x;
@@ -352,6 +357,16 @@ struct Packer {
       if ((rc = copy("energy_embed.bias", c.adim, &h->e_tab_bias))) return rc;
       if ((rc = copy("pitch_embed.bias", c.adim, &h->p_tab_bias))) return rc;
     }
+    // optional speaker table (multi-speaker models): n read off the tensor
+    h->spk_table = nullptr; h->n_speakers = 0;
+    if (const fs2_weight_desc* sp = find(m, "speaker_embed.weight")) {
+      if (sp->ndim != 2 || sp->shape[0] < 1 || sp->shape[0] > INT32_MAX || sp->shape[1] != c.adim || sp->dtype != 0) {
+        set_error("fs2_load_weights: 'speaker_embed.weight' must be float32 [n >= 1, adim=%d]", c.adim);
+        return FS2_ERR_INVALID;
+      }
+      if ((rc = copy("speaker_embed.weight", sp->shape[0] * c.adim, &h->spk_table))) return rc;
+      h->n_speakers = (int)sp->shape[0];
+    }
     // decoder (fastspeech.py:119-136; input layer core/encoder.py:118-125)
     if ((rc = dense("decoder.embed.0.weight", "decoder.embed.0.bias", c.ddim, c.adim, 1, &h->dec_in))) return rc;
     if ((rc = norm("decoder.embed.1.", c.ddim, 1e-5f, &h->dec_in_ln))) return rc;
@@ -514,9 +529,17 @@ int fs2_encode(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B, in
 
 int fs2_encode_ex(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B, int Tmax, float* hs, float* d_log,
                   int64_t* d_int, void* ws, size_t ws_bytes, int flags, void* stream) {
+  return fs2_encode_spk(h, xs, ilens, nullptr, B, Tmax, hs, d_log, d_int, ws, ws_bytes, flags, stream);
+}
+
+int fs2_encode_spk(fs2_handle* h, const int64_t* xs, const int64_t* ilens, const int64_t* spk, int B, int Tmax, float* hs,
+                   float* d_log, int64_t* d_int, void* ws, size_t ws_bytes, int flags, void* stream) {
   FS2_REQUIRE(h && xs && ilens && hs && ws, "fs2_encode: null argument");
   FS2_REQUIRE((flags & ~FS2_PER_UTTERANCE) == 0, "fs2_encode_ex: unknown flags 0x%x", flags);
   if (!h->loaded) { set_error("fs2_encode: weights not loaded"); return FS2_ERR_NOT_LOADED; }
+  FS2_REQUIRE(!h->spk_table || spk, "fs2_encode: the model has a speaker table (%d speakers): pass speaker ids (fs2_encode_spk)",
+              h->n_speakers);
+  FS2_REQUIRE(h->spk_table || !spk, "fs2_encode_spk: speaker ids given but the model has no speaker table");
   FS2_REQUIRE(Tmax <= h->enc_pe_len, "fs2_encode: Tmax=%d exceeds the positional table (%d rows)", Tmax, h->enc_pe_len);
   FS2_DEVICE_GUARD(h);
   cudaStream_t st = (cudaStream_t)stream;
@@ -533,8 +556,10 @@ int fs2_encode_ex(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B,
   { ProfScope prof_scope(P_EMBED, 0, (planes ? 12.0 : 8.0) * B * Tmax * c.adim, st);
     if ((rc = embed_posenc(xs, h->emb, c.idim, h->enc_pe, h->enc_alpha, B, Tmax, c.adim, p.w.x, planes ? p.w.xp : nullptr, zlens, st))) return rc; }
   float* enc_out = nullptr;
+  SpeakerAdd sa;
+  sa.table = h->spk_table; sa.ids = spk; sa.n = h->n_speakers;
   if ((rc = run_blocks(h->enc, p.w, ilens, zlens, B, Tmax, c.adim, c.aheads, planes ? MATH_3XTF32 : FS2_MATH_FP32, false, st,
-                       &enc_out))) return rc;
+                       &enc_out, sa))) return rc;
   FS2_CUDA_CHECK(cudaMemcpyAsync(hs, enc_out, (size_t)B * Tmax * c.adim * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (d_log || d_int)
     if ((rc = run_predictor(h->dur, enc_out, planes ? p.w.xp : nullptr, c.adim, B, Tmax, p.t1, p.t2, p.t2p, ilens, zlens, d_log, d_int, nullptr, st))) return rc;
@@ -566,12 +591,20 @@ int fs2_length_gather_ex(const float* hs, const int32_t* cum, const int64_t* ile
 int fs2_length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac, int B,
                         int Tmax, int64_t Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int32_t* status,
                         void* stream) {
+  return fs2_length_plan_cap_spk(ds, ds_dtype, ilens, alpha_v, fac, nullptr, 0, B, Tmax, Lc, cum, olens, need, d_used, status,
+                                 stream);
+}
+
+int fs2_length_plan_cap_spk(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac,
+                            const int64_t* spk, int n_speakers, int B, int Tmax, int64_t Lc, int32_t* cum, int64_t* olens,
+                            int64_t* need, int64_t* d_used, int32_t* status, void* stream) {
   FS2_REQUIRE(ds && ilens && cum && olens && need && status, "fs2_length_plan_cap: null argument");
+  FS2_REQUIRE(!spk || n_speakers >= 1, "fs2_length_plan_cap_spk: speaker ids need n_speakers >= 1 (got %d)", n_speakers);
   FS2_REQUIRE(B >= 1 && Tmax >= 1, "fs2_length_plan_cap: B=%d and Tmax=%d must be >= 1", B, Tmax);
   FS2_REQUIRE(Lc >= 1 && Lc <= INT32_MAX, "fs2_length_plan_cap: capacity Lc=%lld must lie in [1, %d] (the prefix sum is int32)",
               (long long)Lc, INT32_MAX);
-  return length_plan_cap(ds, ds_dtype, ilens, alpha_v, fac, B, Tmax, (long)Lc, cum, olens, need, d_used, status,
-                         (cudaStream_t)stream);
+  return length_plan_cap(ds, ds_dtype, ilens, alpha_v, fac, spk, n_speakers, B, Tmax, (long)Lc, cum, olens, need, d_used,
+                         status, (cudaStream_t)stream);
 }
 
 int fs2_synth_status(const int32_t* plan_status, const int32_t* voc_status, const int64_t* olens, int B, int hop,

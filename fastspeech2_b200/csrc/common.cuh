@@ -128,6 +128,10 @@ struct RowNorm {
   const int64_t* lens;            // optional mask (needs L > 0): rows t >= lens[b] write 0 to the head, out and split_out
   __half* split_out;              // optional operand planes of y (scaled by kPlaneScale): hi at [row][C], lo at [rows + row][C]
   int split_lo;                   // write the lo plane too (3xF16 consumer)
+  // optional speaker table (the last encoder LayerNorm of a multi-speaker model): y += spk_table[spk[row / spk_L]], one
+  // fp32 add after gamma / beta, before out, split_out and the head.  An id outside [0, n_spk) adds nothing; masked rows
+  // (lens) still write 0
+  const float* spk_table; const int64_t* spk; int n_spk; int spk_L;
 };
 int row_norm(const RowNorm& r, cudaStream_t st);
 
@@ -162,9 +166,10 @@ int transpose_v(const float* qkv, int B, int L, int C, int heads, float* vt, int
 // alpha_v (nullable): per-phoneme factors [B, T] in place of the scalar alpha; d_used (nullable): [B, T] frame counts expanded
 int length_plan(void* ds, int ds_dtype, const int64_t* ilens, float alpha, const float* alpha_v, int B, int T, int mutate,
                 int32_t* cum, int64_t* olens, int64_t* stats, int64_t* d_used, cudaStream_t st);
-// fac_in [2][B, T] -> fac_out [2][B, Lcap] (both nullable): each frame takes the factors of its source phoneme, 1 past olens
-int length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac, int B, int T,
-                    long Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int* status, cudaStream_t st);
+// spk (nullable) [B]: a non-empty slot whose id lies outside [0, n_spk) is emptied and sets FS2_PLAN_BAD_SPEAKER
+int length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac, const int64_t* spk,
+                    int n_spk, int B, int T, long Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int* status,
+                    cudaStream_t st);
 int synth_status(const int* plan, const int* voc, const int64_t* olens, int B, int hop, int* word, int64_t* alens, cudaStream_t st);
 int length_gather(const float* hs, const int32_t* cum, const int64_t* ilens, int B, int T, int C, float* out, int Lcap,
                   const float* fac_in, float* fac_out, cudaStream_t st);

@@ -77,6 +77,11 @@ __global__ void row_norm_kernel(RowNorm r) {
   long bidx = r.L > 0 ? row / r.L : 0;
   const bool padded = r.lens && (long)t >= r.lens[bidx];
   const float alpha = r.pe ? __ldg(r.alpha) : 0.f;
+  const float* srow = nullptr;    // this row's speaker vector, if any
+  if (r.spk_table) {
+    const int64_t id = __ldg(r.spk + row / r.spk_L);
+    if (id >= 0 && id < r.n_spk) srow = r.spk_table + id * C;
+  }
   float dot = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
@@ -91,6 +96,10 @@ __global__ void row_norm_kernel(RowNorm r) {
       float4 p = __ldg(reinterpret_cast<const float4*>(r.pe + (long)t * C + c));
       y.x = __fadd_rn(y.x, __fmul_rn(alpha, p.x)); y.y = __fadd_rn(y.y, __fmul_rn(alpha, p.y));
       y.z = __fadd_rn(y.z, __fmul_rn(alpha, p.z)); y.w = __fadd_rn(y.w, __fmul_rn(alpha, p.w));
+    }
+    if (srow) {   // hs + E[spk]: one fp32 add
+      float4 e = __ldg(reinterpret_cast<const float4*>(srow + c));
+      y.x = __fadd_rn(y.x, e.x); y.y = __fadd_rn(y.y, e.y); y.z = __fadd_rn(y.z, e.z); y.w = __fadd_rn(y.w, e.w);
     }
     if (r.head_w) {
       float4 w = __ldg(reinterpret_cast<const float4*>(r.head_w + c));
@@ -297,6 +306,7 @@ int row_norm(const RowNorm& r, cudaStream_t st) {
   FS2_REQUIRE(r.ldx % 4 == 0 && (!r.out || r.ldo % 4 == 0) && (!r.resid || r.ldr % 4 == 0), "row_norm: strides must be 16-byte multiples");
   FS2_REQUIRE(!r.split_out || (reinterpret_cast<uintptr_t>(r.split_out) & 7) == 0, "row_norm: operand planes must be 8-byte aligned");
   FS2_REQUIRE(!r.lens || r.L > 0, "row_norm: lens needs L > 0");
+  FS2_REQUIRE(!r.spk_table || (r.spk && r.spk_L > 0), "row_norm: a speaker table needs ids and rows per utterance");
   int grid = (int)((r.rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA);
   if (r.C == 256) { FS2_CUDA_CHECK(launch_pdl(row_norm_kernel<2>, dim3(grid), dim3(256), 0, st, r)); }
   else if (r.C == 384) { FS2_CUDA_CHECK(launch_pdl(row_norm_kernel<3>, dim3(grid), dim3(256), 0, st, r)); }

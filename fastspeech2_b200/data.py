@@ -9,11 +9,15 @@
   mel length cuts it.  (The reference ships a BinnedLengthSampler, dataloader.py:121-150, but never instantiates it.)
 
 Items are the reference's `TTSDataset.__getitem__` tuples (dataloader.py:47-74):
-  (phoneme ids [T] int, mel [L, n_mels] float, id str, mel_len int, durations [T] int, energy [L] float, pitch [L] float).
+  (phoneme ids [T] int, mel [L, n_mels] float, id str, mel_len int, durations [T] int, energy [L] float, pitch [L] float),
+optionally followed by an 8th element, the speaker id (multi-speaker models, DESIGN.md section 25).  When every item of a
+batch has it, `collate_tts` and `PinnedCollator` return a 10th element, speakers [B] int64; with 7-element items the
+9-tuple is unchanged.  `FilelistDataset` reads such items from a `preprocess` tree.
 """
 from __future__ import annotations
 
-from typing import Iterator, List, Optional, Sequence, Tuple
+import os
+from typing import Dict, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -21,6 +25,16 @@ import torch
 
 def _lens(batch) -> Tuple[List[int], List[int]]:
     return [int(np.shape(it[0])[0]) for it in batch], [int(np.shape(it[1])[0]) for it in batch]
+
+
+def _speakers(batch) -> Optional[List[int]]:
+    """The batch's speaker ids (8th item element), or None when the items have 7 elements."""
+    n = {len(it) for it in batch}
+    if n == {7}:
+        return None
+    if n != {8}:
+        raise ValueError(f"items must all have 7 elements, or all 8 (with the speaker id); got lengths {sorted(n)}")
+    return [int(it[7]) for it in batch]
 
 
 def _fill(batch, inputs, mels, durations, energys, pitches, labels):
@@ -50,7 +64,9 @@ def collate_tts(batch: Sequence[tuple]):
     labels = torch.zeros(B, L, dtype=torch.float32)
     _fill(batch, inputs, mels, durations, energys, pitches, labels)
     ids = [it[2] for it in batch]
-    return inputs, torch.tensor(il, dtype=torch.int64), mels, labels, torch.tensor(ol, dtype=torch.int64), ids, durations, energys, pitches
+    out = (inputs, torch.tensor(il, dtype=torch.int64), mels, labels, torch.tensor(ol, dtype=torch.int64), ids, durations, energys, pitches)
+    spk = _speakers(batch)
+    return out if spk is None else out + (torch.tensor(spk, dtype=torch.int64),)
 
 
 class _Collated(tuple):
@@ -75,7 +91,8 @@ class PinnedCollator:
         self.slots = [dict(inputs=mk((max_batch, max_T), torch.int64), durations=mk((max_batch, max_T), torch.int64),
                            mels=mk((max_batch, max_L, n_mels), torch.float32), labels=mk((max_batch, max_L), torch.float32),
                            energys=mk((max_batch, max_L), torch.float32), pitches=mk((max_batch, max_L), torch.float32),
-                           ilens=mk((max_batch,), torch.int64), olens=mk((max_batch,), torch.int64), event=None)
+                           ilens=mk((max_batch,), torch.int64), olens=mk((max_batch,), torch.int64),
+                           speakers=mk((max_batch,), torch.int64), event=None)
                       for _ in range(max(1, int(slots)))]
         self._next = 0
 
@@ -101,7 +118,13 @@ class PinnedCollator:
         _fill(batch, inputs, mels, durations, energys, pitches, labels)
         ilens, olens = s["ilens"][:B], s["olens"][:B]
         ilens.copy_(torch.tensor(il)); olens.copy_(torch.tensor(ol))
-        out = _Collated((inputs, ilens, mels, labels, olens, [it[2] for it in batch], durations, energys, pitches))
+        items = (inputs, ilens, mels, labels, olens, [it[2] for it in batch], durations, energys, pitches)
+        spk = _speakers(batch)
+        if spk is not None:
+            speakers = s["speakers"][:B]
+            speakers.copy_(torch.tensor(spk, dtype=torch.int64))
+            items = items + (speakers,)
+        out = _Collated(items)
         out.slot = idx
         return out
 
@@ -172,3 +195,55 @@ class BucketBatchSampler:
             tot += int(ls.max()) * len(batch)
             pad += int(ls.max()) * len(batch) - int(ls.sum())
         return pad / max(tot, 1)
+
+
+class FilelistDataset:
+    """The reference's `TTSDataset` (dataloader.py:34-74) on a `preprocess` tree, plus the speaker id.
+
+    `filelist`: 5- or 6-field lines (aligner.parse_line); `data_dir`: holds mels/, energy/ and pitch/{id}.npy;
+    `symbols`: the phoneme table (aligner.build_symbols -- the reference's 68-symbol table belongs to its text front-end);
+    `speaker_map` ({name: id}, speakers.build_map / load_map) or None for a single-speaker corpus.  Item i is
+    (phoneme ids, mel [L, n_mels], id, L, durations, energy, pitch[, speaker id]) with the reference loader's corrections:
+    durations cut to the phonemes and the last one stretched so that they sum to L, remove_outlier on energy and pitch."""
+
+    def __init__(self, filelist: str, data_dir: str, symbols: Sequence[str], speaker_map: Optional[Dict[str, int]] = None):
+        from .aligner import read_filelist
+        self.lines = read_filelist(filelist)
+        self.data_dir = data_dir
+        self.table = {s: i for i, s in enumerate(symbols)}
+        self.speaker_map = speaker_map
+        for ln in self.lines:
+            if ln.durations is None:
+                raise ValueError(f"{ln.wav}: no durations (run `python -m fastspeech2_b200.aligner extract` first)")
+        if speaker_map is not None:
+            from .speakers import speaker_of
+            missing = sorted({speaker_of(ln) for ln in self.lines} - set(speaker_map))
+            if missing:
+                raise ValueError(f"speakers {missing[:5]} are not in the speaker map")
+
+    def __len__(self) -> int:
+        return len(self.lines)
+
+    def __getitem__(self, index: int) -> tuple:
+        from .aligner import encode
+        from .preprocess import remove_outlier
+        ln = self.lines[index]
+        x = encode(ln, list(self.table))
+        path = lambda kind: os.path.join(self.data_dir, kind, ln.id + ".npy")
+        mel = np.load(path("mels"))
+        L = int(mel.shape[1])
+        d = list(ln.durations)[: len(x)]
+        d[-1] = d[-1] + (L - sum(d))                       # dataloader.py:64-65
+        if d[-1] < 0:
+            raise ValueError(f"{ln.wav}: durations sum past the mel's {L} frames")
+        e = remove_outlier(np.load(path("energy")))
+        p = remove_outlier(np.load(path("pitch")))
+        item = (x, mel.T, ln.id, L, np.array(d, dtype=np.int64), e, p)
+        if self.speaker_map is None:
+            return item
+        from .speakers import speaker_of
+        return item + (self.speaker_map[speaker_of(ln)],)
+
+    def mel_lengths(self) -> List[int]:
+        """Frames per item (BucketBatchSampler's lengths), read from the mel files' headers."""
+        return [int(np.load(os.path.join(self.data_dir, "mels", ln.id + ".npy"), mmap_mode="r").shape[1]) for ln in self.lines]

@@ -35,6 +35,7 @@ fused tf32 tensor-core kernels that store only the row log-sum-exp (DESIGN.md §
 from __future__ import annotations
 
 import ctypes as C
+import inspect
 import os
 from typing import Any, Dict, List, Optional, Sequence, Tuple
 
@@ -287,6 +288,63 @@ def _control_violations(controls: Tuple, ilens: torch.Tensor, T: int) -> torch.T
     return torch.stack(bad).sum()
 
 
+def n_speakers_from_hp(hp: Any) -> int:
+    """hp.model.n_speakers: absent, None or 0 is a single-speaker model."""
+    v = _get(_get(hp, "model"), "n_speakers", 0)
+    if v is None:
+        return 0
+    if isinstance(v, bool) or not isinstance(v, int) or v < 0:
+        raise ValueError(f"hp.model.n_speakers must be an int >= 0, got {v!r}")
+    return int(v)
+
+
+def _speaker_ids(n_speakers: int, speakers: Any, B: int, dev: torch.device) -> Optional[torch.Tensor]:
+    """Speakers of a call -> None (single-speaker model) or a contiguous int64 [B] tensor on `dev`.  Everything that needs
+    no device read is checked here; ids on the device are range-checked in the caller's single host read."""
+    if n_speakers == 0:
+        if speakers is not None:
+            raise ValueError("speakers were given but the model has no speaker table (hp.model.n_speakers is 0)")
+        return None
+    if speakers is None:
+        raise ValueError(f"the model has {n_speakers} speakers: pass the speaker ids (speakers=)")
+    if not torch.is_tensor(speakers) or speakers.dtype != torch.int64:
+        raise ValueError(f"speakers must be an int64 tensor, got {getattr(speakers, 'dtype', type(speakers).__name__)}")
+    if speakers.dim() != 1 or speakers.shape[0] != B:
+        raise ValueError(f"speakers must be [B={B}], got {tuple(speakers.shape)}")
+    if not speakers.is_cuda:
+        _check_speaker_range(int(((speakers < 0) | (speakers >= n_speakers)).sum()), n_speakers)
+    return speakers.to(dev).contiguous()
+
+
+def _speaker_violations(spk: torch.Tensor, n_speakers: int) -> torch.Tensor:
+    """Device scalar: how many ids lie outside [0, n_speakers)."""
+    return ((spk < 0) | (spk >= n_speakers)).sum().view(1)
+
+
+def _check_speaker_range(bad: int, n_speakers: int) -> None:
+    if bad:
+        raise ValueError(f"speakers: {bad} id(s) outside [0, n_speakers={n_speakers})")
+
+
+def _one_speaker(speaker: Any) -> Optional[torch.Tensor]:
+    """`inference`'s speaker: None, a Python int or a 0-d int64 tensor -> None or a [1] tensor."""
+    if speaker is None:
+        return None
+    if torch.is_tensor(speaker):
+        if speaker.dim() != 0:
+            raise ValueError(f"speaker must be an int or a 0-d tensor, got shape {tuple(speaker.shape)}")
+        return speaker.reshape(1)
+    if isinstance(speaker, bool) or not isinstance(speaker, int):
+        raise ValueError(f"speaker must be an int or a 0-d int64 tensor, got {type(speaker).__name__}")
+    return torch.tensor([speaker], dtype=torch.int64)
+
+
+def _without(fn, name: str) -> inspect.Signature:
+    """fn's signature without the parameter `name`."""
+    sig = inspect.signature(fn)
+    return sig.replace(parameters=[p for p in sig.parameters.values() if p.name != name])
+
+
 # ------------------------------------------------------------------------------------------------
 class FeedForwardTransformer(nn.Module):
     """Feed-forward Transformer TTS (FastSpeech2) on H100.  See module docstring."""
@@ -308,13 +366,20 @@ class FeedForwardTransformer(nn.Module):
             hp = load_hp_str(checkpoint["hp_str"])
         idim = int(sd["encoder.embed.0.weight"].shape[0])
         odim = int(_get(_get(hp, "audio"), "num_mels"))
-        model = cls(idim, odim, hp, precision=precision, train_precision=train_precision, train_attention=train_attention)
+        # the speaker count comes from the table: an hp_str written before multi-speaker models lacks the key
+        table = sd.get("speaker_embed.weight")
+        n_spk = int(table.shape[0]) if table is not None else 0
+        n_hp = n_speakers_from_hp(hp)
+        if n_hp and n_hp != n_spk:
+            raise ValueError(f"hp.model.n_speakers = {n_hp} but the checkpoint's speaker table has {n_spk} rows")
+        model = cls(idim, odim, hp, precision=precision, train_precision=train_precision, train_attention=train_attention,
+                    n_speakers=n_spk)
         model.load_state_dict(sd, strict="model" in checkpoint)
         model.eval()
         return model.to(device) if device is not None else model
 
     def __init__(self, idim: int, odim: int, hp: Dict, precision: Optional[str] = None, train_precision: Optional[str] = None,
-                 train_attention: Optional[str] = None):
+                 train_attention: Optional[str] = None, n_speakers: Optional[int] = None):
         super().__init__()
         dims = dims_from_hp(idim, odim, hp)
         self.dims = dims
@@ -354,6 +419,14 @@ class FeedForwardTransformer(nn.Module):
         _init_like_reference(self, str(_get(m, "transformer_init", "pytorch")))
         self.encoder.embed[-1].alpha.data = torch.tensor(float(_get(m, "initial_encoder_alpha", 1.0)))
         self.decoder.embed[-1].alpha.data = torch.tensor(float(_get(m, "initial_decoder_alpha", 1.0)))
+        # multi-speaker (DESIGN.md section 25): one learned vector per speaker added to the encoder output.  Created last, so
+        # the reference's 225 keys keep their order, the new key comes after feat_out, and the other parameters draw the
+        # same initial values as in a single-speaker model; nn.Embedding's N(0, 1) init, no padding row
+        self.n_speakers = n_speakers_from_hp(hp) if n_speakers is None else int(n_speakers)
+        if self.n_speakers < 0:
+            raise ValueError(f"n_speakers must be >= 0, got {self.n_speakers}")
+        if self.n_speakers:
+            self.speaker_embed = nn.Embedding(self.n_speakers, A)
 
         self.postnet_dropout_rate = float(_get(m, "postnet_dropout_rate", 0.5))
         self.duration_dropout_rate = float(_get(m, "duration_predictor_dropout_rate", 0.1))
@@ -470,7 +543,7 @@ class FeedForwardTransformer(nn.Module):
                  es: torch.Tensor = None, ps: torch.Tensor = None, is_inference: bool = False,
                  _one_hot: bool = True, _defer_check: Optional[list] = None, _after_out: Optional[torch.Tensor] = None,
                  per_utterance: bool = False, _olens_out: Optional[list] = None,
-                 _controls: Optional[Tuple] = None) -> Sequence[torch.Tensor]:
+                 _controls: Optional[Tuple] = None, speakers: Optional[torch.Tensor] = None) -> Sequence[torch.Tensor]:
         """The reference's `_forward` (fastspeech.py:169-243).  `per_utterance=True` (not in the reference) makes every
         utterance's result independent of its batch mates: utterance b is bit-identical to the B = 1 call on
         `xs[b:b+1, :ilens[b]]` (teacher-forced: with its es / ps sliced to olens[b]), in inference the decoder is masked by
@@ -479,13 +552,15 @@ class FeedForwardTransformer(nn.Module):
         olens[b] == sum(ds[b, :ilens[b]]).  `_olens_out` (list): receives the olens the decoder ran with.
         `_controls` (from `_controls_for`): prosody factors (speed, pitch, energy) per phoneme, in inference only, and
         only where an utterance's result does not depend on its batch mates (per_utterance, or B = 1); the returned
-        durations are then the frame counts actually expanded."""
+        durations are then the frame counts actually expanded.  `speakers` (multi-speaker models, DESIGN.md section 25):
+        int64 [B] ids in [0, n_speakers); E[speakers[b]] is added to the encoder output at every row (reference semantics)
+        or at rows t < ilens[b] (per_utterance)."""
         # the handle-less ABI stages (LengthRegulator, losses, ...) run on the CURRENT device like any CUDA library call:
         # select the device the data lives on for the whole call, leave the caller's current device untouched
         if xs.is_cuda and torch.cuda.current_device() != (xs.device.index or 0):
             with torch.cuda.device(xs.device):
                 return self._forward(xs, ilens, olens, ds, es, ps, is_inference, _one_hot, _defer_check, _after_out,
-                                     per_utterance, _olens_out, _controls)
+                                     per_utterance, _olens_out, _controls, speakers)
         if _controls is not None:
             if not is_inference:
                 raise ValueError("prosody controls apply to inference only (teacher-forced durations, energy and pitch are given)")
@@ -494,6 +569,9 @@ class FeedForwardTransformer(nn.Module):
                                  "batch semantics an utterance's result depends on its batch mates")
         if per_utterance:
             self._check_ilens(xs, ilens)
+        if xs.dim() != 2:
+            raise ValueError("xs must be [B, Tmax]")
+        spk = _speaker_ids(self.n_speakers, speakers, int(xs.shape[0]), xs.device)
         h = self._ready(xs)
         lib = _lib.load()
         dev, d = xs.device, self.dims
@@ -525,8 +603,8 @@ class FeedForwardTransformer(nn.Module):
         hs = torch.empty((B, T, d.adim), **f32)
         d_log = None if is_inference else torch.empty((B, T), **f32)
         d_int = torch.empty((B, T), dtype=torch.int64, device=dev) if is_inference else None
-        _lib.check(lib.fs2_encode_ex(h, _lib.ptr(xs), _lib.ptr(ilens), B, T, _lib.ptr(hs), _lib.ptr(d_log), _lib.ptr(d_int),
-                                     _lib.ptr(ws), ws.numel(), flags, st), "fs2_encode_ex")
+        _lib.check(lib.fs2_encode_spk(h, _lib.ptr(xs), _lib.ptr(ilens), _lib.ptr(spk), B, T, _lib.ptr(hs), _lib.ptr(d_log),
+                                      _lib.ptr(d_int), _lib.ptr(ws), ws.numel(), flags, st), "fs2_encode_spk")
 
         # stage 2: length regulator
         speed, pitch, energy = _controls if _controls is not None else (None, None, None)
@@ -542,7 +620,11 @@ class FeedForwardTransformer(nn.Module):
                 words.append(torch.stack([ilens.min(), ilens.max()]))
             if _controls is not None:
                 words.append(_control_violations(_controls, ilens, T).view(1))
+            if spk is not None:     # and the speaker range
+                words.append(_speaker_violations(spk, self.n_speakers))
             vals = torch.cat(words).tolist() if len(words) > 1 else stats.tolist()  # the single host sync of inference
+            if spk is not None:
+                _check_speaker_range(vals.pop(), self.n_speakers)
             if _controls is not None and vals[-1]:
                 raise ValueError(f"prosody controls: {vals[-1]} factor(s) are non-finite or <= 0 (each must be finite and > 0)")
             if per_utterance:
@@ -604,16 +686,20 @@ class FeedForwardTransformer(nn.Module):
         # teacher-forced: validate what the reference would have tripped over with shape errors
         # (mask widths are max(lengths): utils/util.py:262-272), one host read at the end.
         chk_dev = torch.stack([stats[0], stats[1], ilens.max(), olens_dec.max()])
+        if spk is not None:     # the speaker range rides in the same transfer
+            chk_dev = torch.cat([chk_dev, _speaker_violations(spk, self.n_speakers)])
         if _defer_check is not None:          # CUDA-graph capture: no host read here, the caller validates after replay
             _defer_check.append((chk_dev, T, L))
             return before, after, d_log, e_out, p_out
         if per_utterance:   # + the ilens range and olens == sum(ds) (the zero rows of hm end at sum(ds)), same transfer
             chk = torch.cat([chk_dev, torch.stack([ilens.min(), (olens_dec != olens_lr).sum()])]).tolist()
-            self._check_ilens_range(chk[4], chk[2], T)
-            if chk[5]:
-                raise ValueError(f"per_utterance: olens differs from sum(ds) in {chk[5]} utterance(s)")
+            self._check_ilens_range(chk[-2], chk[2], T)
+            if chk[-1]:
+                raise ValueError(f"per_utterance: olens differs from sum(ds) in {chk[-1]} utterance(s)")
         else:
             chk = chk_dev.tolist()
+        if spk is not None:
+            _check_speaker_range(chk[4], self.n_speakers)
         self._validate_lengths(chk[:4], T, L)
         return before, after, d_log, e_out, p_out
 
@@ -653,16 +739,17 @@ class FeedForwardTransformer(nn.Module):
         return GraphedSynthesis(self, B, T, capacity, vocoder)
 
     def forward(self, xs: torch.Tensor, ilens: torch.Tensor, ys: torch.Tensor, olens: torch.Tensor, ds: torch.Tensor,
-                es: torch.Tensor, ps: torch.Tensor) -> Tuple[torch.Tensor, List[Dict[str, float]]]:
+                es: torch.Tensor, ps: torch.Tensor, speakers: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, List[Dict[str, float]]]:
         """Loss computation (fastspeech.py:245-337). Returns (loss, report_keys).  In train mode the loss is attached to
         the autograd graph of the train path (fastspeech2_b200/train.py) so `loss.backward()` fills `.grad` of every
-        parameter the reference trains; `self.dropout_masks` (a train.MaskSource) may be set to inject masks."""
+        parameter the reference trains; `self.dropout_masks` (a train.MaskSource) may be set to inject masks.
+        `speakers`: int64 [B] ids of a multi-speaker model (required there, refused otherwise)."""
         if xs.is_cuda and torch.cuda.current_device() != (xs.device.index or 0):
             with torch.cuda.device(xs.device):
-                return self.forward(xs, ilens, ys, olens, ds, es, ps)
+                return self.forward(xs, ilens, ys, olens, ds, es, ps, speakers)
         if self.training:
             from .train import train_forward
-            return train_forward(self, xs, ilens, ys, olens, ds, es, ps, masks=self.dropout_masks)
+            return train_forward(self, xs, ilens, ys, olens, ds, es, ps, masks=self.dropout_masks, speakers=speakers)
         self._ready(xs)
         lib = _lib.load()
         dev = xs.device
@@ -672,7 +759,8 @@ class FeedForwardTransformer(nn.Module):
         xs = xs[:, :tmax]  # fastspeech.py:266-267
         ds_t = ds[:, :tmax].contiguous() if ds.shape[1] != tmax else ds
         es_t, ps_t = es[:, :lmax], ps[:, :lmax]
-        before, after, d_outs, e_outs, p_outs = self._forward(xs, ilens, olens, ds_t, es_t, ps_t, is_inference=False)
+        before, after, d_outs, e_outs, p_outs = self._forward(xs, ilens, olens, ds_t, es_t, ps_t, is_inference=False,
+                                                              speakers=speakers)
         if ds_t is not ds and ds_t.shape == ds[:, :tmax].shape:
             ds[:, :tmax].copy_(ds_t)
         B, T = xs.shape
@@ -690,13 +778,19 @@ class FeedForwardTransformer(nn.Module):
         names = ["l1_loss", "before_loss", "after_loss", "duration_loss", "energy_loss", "pitch_loss", "loss"]
         return out7[6], [{k: v} for k, v in zip(names, vals)]
 
-    def inference(self, x: torch.Tensor) -> torch.Tensor:
-        """x [T] int64 -> mel [L, odim] (fastspeech.py:339-357)."""
+    def inference(self, x: torch.Tensor, speaker=None) -> torch.Tensor:
+        """x [T] int64 -> mel [L, odim] (fastspeech.py:339-357).  speaker: the id (an int or a 0-d int64 tensor) of a
+        multi-speaker model."""
         ilens = torch.tensor([x.shape[0]], dtype=torch.long, device=x.device)
-        _, outs, _, _, _ = self._forward(x.unsqueeze(0), ilens, is_inference=True, _one_hot=False)
+        _, outs, _, _, _ = self._forward(x.unsqueeze(0), ilens, is_inference=True, _one_hot=False, speakers=_one_speaker(speaker))
         return outs[0]
 
-    def inference_controlled(self, x: torch.Tensor, *, speed=None, pitch=None, energy=None) -> torch.Tensor:
+    # `forward` and `inference` report the reference's signatures to introspection (fastspeech.py:245-254, :339, what
+    # drop-in launchers check); `speakers` / `speaker` are extra keywords that only multi-speaker models use
+    forward.__signature__ = _without(forward, "speakers")
+    inference.__signature__ = _without(inference, "speaker")
+
+    def inference_controlled(self, x: torch.Tensor, *, speed=None, pitch=None, energy=None, speaker=None) -> torch.Tensor:
         """`inference` with prosody controls (not in the reference, whose `_forward` passes alpha = 1 to its
         LengthRegulator and pitch / energy predictors; `inference` itself keeps the reference's signature).  Each control
         is None, a number or a [T] tensor of per-phoneme factors, finite and > 0.  speed multiplies the predicted
@@ -714,10 +808,11 @@ class FeedForwardTransformer(nn.Module):
                 ctl[k] = v[None, :]
         controls = _controls_for(1, int(x.shape[0]), x.device, ctl)
         ilens = torch.tensor([x.shape[0]], dtype=torch.long, device=x.device)
-        _, outs, _, _, _ = self._forward(x.unsqueeze(0), ilens, is_inference=True, _one_hot=False, _controls=controls)
+        _, outs, _, _, _ = self._forward(x.unsqueeze(0), ilens, is_inference=True, _one_hot=False, _controls=controls,
+                                         speakers=_one_speaker(speaker))
         return outs[0]
 
-    def synthesize(self, xs: torch.Tensor, ilens: torch.Tensor, *, speed=None, pitch=None,
+    def synthesize(self, xs: torch.Tensor, ilens: torch.Tensor, *, speakers=None, speed=None, pitch=None,
                    energy=None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Per-utterance batched inference (not in the reference): xs [B, Tmax] int64 (0 = pad), ilens [B] with
         1 <= ilens[b] <= Tmax -> (mels [B, Lmax, odim], olens [B] int64, durations [B, Tmax] int64), all on the device.
@@ -726,14 +821,15 @@ class FeedForwardTransformer(nn.Module):
         speed / pitch / energy: prosody controls as in `inference_controlled`, each None, a number, a [B] tensor (per
         utterance) or a [B, Tmax] tensor (per phoneme; entries past ilens[b] are ignored).  Utterance b is then
         bit-identical to `inference_controlled` on it with its slice of the controls.  durations are the frame counts expanded (after speed and
-        the all-zero rule): durations.sum(1) == olens."""
+        the all-zero rule): durations.sum(1) == olens.  speakers: int64 [B] ids of a multi-speaker model; utterance b is
+        then bit-identical to `inference` on it with speaker speakers[b]."""
         if xs.dim() != 2:
             raise ValueError("xs must be [B, Tmax]")
         controls = _controls_for(int(xs.shape[0]), int(xs.shape[1]), xs.device,
                                  {"speed": speed, "pitch": pitch, "energy": energy}, ilens)
         got: list = []
         _, after, dur, _, _ = self._forward(xs, ilens, is_inference=True, _one_hot=False, per_utterance=True, _olens_out=got,
-                                            _controls=controls)
+                                            _controls=controls, speakers=speakers)
         return after, got[0], dur
 
 
@@ -824,7 +920,8 @@ class GraphedSynthesis:
       [-> vocoder._call at Lmax = capacity] -> status fold
 
     Static inputs (`self.xs` [B, T], `self.ilens` [B], `self.speed` / `self.pitch` / `self.energy` [B, T] float32, 1.0
-    when not set, which is bit-identical to no control); static outputs, valid until the next replay: mels [B, capacity,
+    when not set, which is bit-identical to no control; `self.speakers` [B] int64 on a multi-speaker model, whose ids the
+    plan checks on the device, so changing only the speakers between replays needs no recapture); static outputs, valid until the next replay: mels [B, capacity,
     80], olens [B], durations [B, T] and need [B], and with a vocoder audio [B, capacity * 256] and alens [B] = olens * 256.
     A slot that ran is bit-identical to `synthesize` on that utterance alone (and its audio to the vocoder on that);
     rows past olens[b] and every row of a slot that did not run are +0.
@@ -856,6 +953,7 @@ class GraphedSynthesis:
         d = model.dims
         i64, f32 = dict(dtype=torch.int64, device=dev), dict(dtype=torch.float32, device=dev)
         self.xs, self.ilens = torch.zeros((B, T), **i64), torch.zeros((B,), **i64)
+        self.speakers = torch.zeros((B,), **i64) if model.n_speakers else None
         self.speed = torch.ones((B, T), **f32)
         self._fac = torch.ones((2, B, T), **f32)            # the gather's per-phoneme planes: energy, pitch
         self.energy, self.pitch = self._fac[0], self._fac[1]
@@ -909,11 +1007,11 @@ class GraphedSynthesis:
         B, T, Lc, d = self.B, self.T, self.capacity, self.model.dims
         st = _lib.stream_ptr(self.device)
         flags = _lib.FS2_PER_UTTERANCE
-        _lib.check(lib.fs2_encode_ex(self._h, P(self.xs), P(self.ilens), B, T, P(self._hs), None, P(self._d_int), P(self._ws),
-                                     self._ws.numel(), flags, st), "fs2_encode_ex")
-        _lib.check(lib.fs2_length_plan_cap(P(self._d_int), _lib.FS2_DUR_I64, P(self.ilens), P(self.speed), P(self._fac), B, T, Lc,
-                                           P(self._cum), P(self.olens), P(self.need), P(self.durations), P(self._plan_status), st),
-                   "fs2_length_plan_cap")
+        _lib.check(lib.fs2_encode_spk(self._h, P(self.xs), P(self.ilens), P(self.speakers), B, T, P(self._hs), None, P(self._d_int),
+                                      P(self._ws), self._ws.numel(), flags, st), "fs2_encode_spk")
+        _lib.check(lib.fs2_length_plan_cap_spk(P(self._d_int), _lib.FS2_DUR_I64, P(self.ilens), P(self.speed), P(self._fac),
+                                               P(self.speakers), self.model.n_speakers, B, T, Lc, P(self._cum), P(self.olens),
+                                               P(self.need), P(self.durations), P(self._plan_status), st), "fs2_length_plan_cap_spk")
         _lib.check(lib.fs2_length_gather_ex(P(self._hs), P(self._cum), P(self.ilens), B, T, d.adim, P(self._hm), Lc, P(self._fac),
                                             P(self._fac_out), st), "fs2_length_gather_ex")
         _lib.check(lib.fs2_decode_ctl(self._h, P(self._hm), P(self.olens), None, None, B, Lc, P(self._before), P(self.mels),
@@ -961,6 +1059,8 @@ class GraphedSynthesis:
             raise ValueError(f"every ilens[b] must lie in [0, T={self.T}] (0 marks an empty slot)")
         if word & _lib.FS2_PLAN_BAD_CONTROL:
             raise ValueError("prosody controls: some factor(s) are non-finite or <= 0 (each must be finite and > 0)")
+        if word & _lib.FS2_PLAN_BAD_SPEAKER:
+            _check_speaker_range(1, self.model.n_speakers)
         voc = word >> _lib.FS2_SYNTH_VOC_SHIFT
         if voc and self.vocoder is not None:
             for bit, message in self.vocoder._status_table():
@@ -988,20 +1088,25 @@ class GraphedSynthesis:
             self.flush()
         return self.outputs
 
-    def __call__(self, xs, ilens, speed=None, pitch=None, energy=None, validate=True) -> tuple:
+    def __call__(self, xs, ilens, speakers=None, speed=None, pitch=None, energy=None, validate=True) -> tuple:
         """Synthesize b <= B requests of t <= T phonemes: xs [b, t] (0 = pad) and ilens [b] are copied into slots 0 .. b-1,
-        slots b .. B-1 become empty.  speed / pitch / energy: None, a number, a [b] or a [b, t] tensor, as in `synthesize`.
+        slots b .. B-1 become empty.  speakers: int64 [b] ids of a multi-speaker model (ids on the device are checked in the
+        status word).  speed / pitch / energy: None, a number, a [b] or a [b, t] tensor, as in `synthesize`.
         -> `outputs` (all B slots)."""
         if validate not in (True, False, "deferred"):
             raise ValueError(f"validate must be True, False or 'deferred' (got {validate!r})")
         self._check_model()
         b, t = self.check_request(xs, ilens, self.B, self.T)
+        spk = _speaker_ids(self.model.n_speakers, speakers, b, self.device)
         controls = _controls_for(b, t, self.device, {"speed": speed, "pitch": pitch, "energy": energy}, ilens)
         with torch.cuda.device(self.device):
             self.xs.zero_()
             self.xs[:b, :t].copy_(xs, non_blocking=True)
             self.ilens.zero_()
             self.ilens[:b].copy_(ilens, non_blocking=True)
+            if spk is not None:
+                self.speakers.zero_()
+                self.speakers[:b].copy_(spk, non_blocking=True)
             if self._controlled or controls is not None:     # factors stay 1.0 between uncontrolled requests
                 self.speed.fill_(1.0)
                 self._fac.fill_(1.0)

@@ -222,16 +222,19 @@ class PeerGather:
         self._base = 0
 
 
-def synthesize_sharded(model, xs: torch.Tensor, ilens: torch.Tensor, group: Optional[dist.ProcessGroup] = None):
+def synthesize_sharded(model, xs: torch.Tensor, ilens: torch.Tensor, group: Optional[dist.ProcessGroup] = None,
+                       speakers: Optional[torch.Tensor] = None):
     """Batched `is_inference=True` synthesis of a global batch: every rank passes the same global
-    `xs [B,T]` / `ilens [B]`, runs its shard and receives all mels.  Returns (mels, olens)."""
+    `xs [B,T]` / `ilens [B]` (and, for a multi-speaker model, `speakers [B]`), runs its shard and receives all mels.
+    Returns (mels, olens)."""
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     lo, hi = shard_bounds(xs.shape[0], rank, world)
     il = ilens[lo:hi]
     t = int(il.max()) if hi > lo else 0
     with torch.no_grad():
-        _, after, d_outs, _, _ = model._forward(xs[lo:hi, :t].contiguous(), il, is_inference=True, _one_hot=False)
+        _, after, d_outs, _, _ = model._forward(xs[lo:hi, :t].contiguous(), il, is_inference=True, _one_hot=False,
+                                                speakers=None if speakers is None else speakers[lo:hi])
     olens = d_outs.sum(dim=1)
     if world == 1:
         return after, olens

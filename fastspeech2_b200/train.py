@@ -405,6 +405,41 @@ class RowDotFn(torch.autograd.Function):
         return dx, dw.reshape(ctx.wshape), db, None
 
 
+class SpeakerAddFn(torch.autograd.Function):
+    """hs + E[spk].unsqueeze(1) over every row t < T (DESIGN.md section 25); E [n, C].  The table's gradient comes from the
+    deterministic fs2_speaker_add_backward (per-utterance column sums, then one ordered sum per speaker, no atomics)."""
+
+    @staticmethod
+    def forward(ctx, x, spk, table):
+        x = _c(x)
+        B, T, C_ = x.shape
+        out = torch.empty_like(x)
+        _chk(_lib.load().fs2_speaker_add(x.data_ptr(), spk.data_ptr(), _c(table.detach()).data_ptr(), B, T, C_, table.shape[0], out.data_ptr(),
+                                         _st(x)), "fs2_speaker_add")
+        ctx.save_for_backward(spk)
+        ctx.meta = (B, T, C_, table.shape[0])
+        return out
+
+    @staticmethod
+    def backward(ctx, dy):
+        (spk,) = ctx.saved_tensors
+        B, T, C_, n = ctx.meta
+        dy = _c(dy)
+        dtab = torch.zeros((n, C_), dtype=torch.float32, device=dy.device)
+        nbytes = speaker_add_ws_bytes(B, C_)
+        ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=dy.device)
+        _chk(_lib.load().fs2_speaker_add_backward(dy.data_ptr(), spk.data_ptr(), B, T, C_, n, dtab.data_ptr(), ws.data_ptr(), nbytes, _st(dy)),
+             "fs2_speaker_add_backward")
+        return dy, None, dtab
+
+
+def speaker_add_ws_bytes(B: int, C_: int) -> int:
+    """Workspace bytes of fs2_speaker_add_backward for B utterances of C channels."""
+    n = C.c_size_t(0)
+    _chk(_lib.load().fs2_speaker_add_backward_ws_bytes(int(B), int(C_), C.byref(n)), "fs2_speaker_add_backward_ws_bytes")
+    return int(n.value)
+
+
 class LengthRegulatorFn(torch.autograd.Function):
     """length_regulator.py:38-95 with the ground-truth durations; backward = per-phoneme sum of its frames' gradients."""
 
@@ -571,9 +606,10 @@ def _predictor(pred, x, lens, rate: float, masks: MaskSource, math: int = _lib.M
     return RowDotFn.apply(x, pred.linear.weight, pred.linear.bias, lens)
 
 
-def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskSource] = None):
+def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskSource] = None, speakers=None):
     """`FeedForwardTransformer.forward` in train mode (fastspeech.py:245-337 -> _forward :169-243).  Returns
-    (loss 0-d tensor attached to the autograd graph, report_keys)."""
+    (loss 0-d tensor attached to the autograd graph, report_keys).  `speakers`: int64 [B] ids of a multi-speaker model."""
+    from .fastspeech import _check_speaker_range, _speaker_ids, _speaker_violations
     lib = _lib.load()
     dev = xs.device
     if dev.type != "cuda":
@@ -584,7 +620,12 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
     d = model.dims
     ilens = ilens.to(device=dev, dtype=torch.int64).contiguous()
     olens = olens.to(device=dev, dtype=torch.int64).contiguous()
-    tmax, lmax = torch.stack([ilens.max(), olens.max()]).tolist()
+    spk = _speaker_ids(model.n_speakers, speakers, int(xs.shape[0]), dev)
+    if spk is None:
+        tmax, lmax = torch.stack([ilens.max(), olens.max()]).tolist()
+    else:       # the speaker range rides in the same host read
+        tmax, lmax, bad = torch.cat([torch.stack([ilens.max(), olens.max()]), _speaker_violations(spk, model.n_speakers)]).tolist()
+        _check_speaker_range(bad, model.n_speakers)
     xs = xs[:, :tmax].to(torch.int64).contiguous()                                            # fastspeech.py:266-267
     ds = ds[:, :tmax].contiguous()
     es = es[:, :lmax].to(torch.float32).contiguous()
@@ -601,6 +642,8 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
     x = EmbedFn.apply(xs, model.encoder.embed[0].weight, enc_pos.alpha, enc_pos.pe)
     x = _drop(x, ER, masks)                                                                   # embedding.py:120
     hs = _fft_blocks(model.encoder, x, ilens, d.aheads, ER, masks, math, flash)
+    if spk is not None:     # hs + E[spk] at every row, fp32 in both train precisions
+        hs = SpeakerAddFn.apply(hs, spk, model.speaker_embed.weight)
     # duration predictor on the encoder states, then LengthRegulator with the ground-truth durations (:209-211)
     d_outs = _predictor(model.duration_predictor, hs, ilens, model.duration_dropout_rate, masks, math)
     hm = LengthRegulatorFn.apply(hs, ds, ilens, L)

@@ -141,6 +141,19 @@ int fs2_encode(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B, in
 int fs2_encode_ex(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B, int Tmax, float* hs, float* d_log,
                   int64_t* d_int, void* ws, size_t ws_bytes, int flags, void* stream);
 
+/* Multi-speaker encoder (DESIGN.md section 25).  fs2_load_weights takes an optional "speaker_embed.weight" [n, adim]
+ * (n >= 1 read off the tensor; fs2_config does not change).  With such a table loaded,
+ *   hs[b, t, :] = LN_last(...)[b, t, :] + table[spk[b], :]
+ * one fp32 add in the epilogue of the last encoder block's second LayerNorm, so the duration predictor, the returned hs
+ * and everything downstream see the sum.  Without FS2_PER_UTTERANCE the add covers every row t < Tmax (the reference's
+ * `hs + E[spk].unsqueeze(1)`); with it only rows t < ilens[b], and the padding stays exact 0.
+ *   spk [B] i64 (device): ids in [0, n).  An id outside that range adds nothing (and is never read past the table): the
+ *       caller checks ids (fs2_length_plan_cap_spk does so on the device).
+ * fs2_encode_ex is the spk = NULL case.  spk == NULL with a table loaded, and spk != NULL without one, are
+ * FS2_ERR_INVALID. */
+int fs2_encode_spk(fs2_handle* h, const int64_t* xs, const int64_t* ilens, const int64_t* spk, int B, int Tmax, float* hs,
+                   float* d_log, int64_t* d_int, void* ws, size_t ws_bytes, int flags, void* stream);
+
 /* ---- stage 2: LengthRegulator (needs no handle) ---------------------------------------- */
 /* core/duration_modeling/length_regulator.py:38-95 + utils/util.py:91-104.
  * Plan: per utterance, optionally scale by alpha (round half to even, :58-59), truncate to
@@ -191,9 +204,16 @@ int fs2_length_gather_ex(const float* hs, const int32_t* cum, const int64_t* ile
 #define FS2_PLAN_BAD_ILENS 1
 #define FS2_PLAN_BAD_CONTROL 2
 #define FS2_PLAN_OVERFLOW 4
+#define FS2_PLAN_BAD_SPEAKER 8
 int fs2_length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac, int B,
                         int Tmax, int64_t Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int32_t* status,
                         void* stream);
+/* fs2_length_plan_cap for a multi-speaker model; fs2_length_plan_cap is the spk = NULL case.
+ *   spk [B] i64 (device) or NULL, n_speakers >= 1 when spk is given: a slot with ilens[b] != 0 whose id lies outside
+ *       [0, n_speakers) gets olens 0 (written as zeros, like a bad-ilens slot) and sets FS2_PLAN_BAD_SPEAKER. */
+int fs2_length_plan_cap_spk(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac,
+                            const int64_t* spk, int n_speakers, int B, int Tmax, int64_t Lc, int32_t* cum, int64_t* olens,
+                            int64_t* need, int64_t* d_used, int32_t* status, void* stream);
 /* The status word of one graphed synthesis: *word = *plan_status | (vocoder bits << FS2_SYNTH_VOC_SHIFT), where the
  * vocoder's bits are *voc_status (NULL: none) without its BAD_LENGTH bit when some olens[b] is 0 (an empty, overflowed or
  * refused slot, which the vocoder reports as a bad length by design).  alens [B] i64 out or NULL: olens[b] * hop.
@@ -383,6 +403,18 @@ int fs2_embed_posenc(const int64_t* xs, const float* table, int n_sym, const flo
 int fs2_embed_backward(const int64_t* xs /* NULL: positional part only */, const float* dy, const float* pe, int B, int T, int C, int n_sym,
                        float* dtable /* += or NULL */, float* dalpha /* += */, void* stream);
 int fs2_posenc_add(const float* x, const float* pe, const float* alpha, int B, int T, int C, float* y, void* stream);
+/* Speaker table of the train step (DESIGN.md section 25): y[b,t,:] = x[b,t,:] + table[spk[b],:] at every t < T, one fp32
+ * add (an id outside [0, n) adds nothing), and its backward into the table:
+ *   dtable[s,:] += sum over b with spk[b] == s of sum_{t < T} dy[b,t,:]
+ * Deterministic, without atomics: per-utterance column sums over T in a fixed tree order into the workspace [B, C], then
+ * one thread per (first utterance of a speaker, column) adds that speaker's partials in ascending b and writes dtable
+ * once.  Rows of speakers absent from the batch (and out-of-range ids) are left untouched; the same dy always gives the
+ * same bits.  ws: at least fs2_speaker_add_backward_ws_bytes(B, C) bytes, 16-byte aligned, contents on entry unused.
+ * C % 4 == 0 (forward); B, T >= 0; a short workspace is FS2_ERR_INVALID. */
+int fs2_speaker_add(const float* x, const int64_t* spk, const float* table, int B, int T, int C, int n, float* y, void* stream);
+int fs2_speaker_add_backward_ws_bytes(int B, int C, size_t* bytes);
+int fs2_speaker_add_backward(const float* dy, const int64_t* spk, int B, int T, int C, int n, float* dtable /* += */, void* ws,
+                             size_t ws_bytes, void* stream);
 /* pitch / energy embedding = Linear(n_bins -> C) on a one-hot (fastspeech.py:102,113,218-219), W [C, n_bins] */
 int fs2_onehot_linear_forward(const float* x, const int64_t* ids, const float* W, const float* b, int64_t rows, int C, int n_bins, float* y,
                               void* stream);
