@@ -96,6 +96,17 @@ class NoamAdamHp(C.Structure):
     _fields_ = [(n, C.c_double) for n in ("rate_scale", "warmup_pow", "beta1", "beta2", "eps")]
 
 
+class RowNormDesc(C.Structure):
+    """fs2_row_norm_desc: the row LayerNorm and its fusions (fs2_op_row_norm); unset pointers are NULL, unset ints 0."""
+    _fields_ = [("x", C.c_void_p), ("ldx", C.c_int32), ("resid", C.c_void_p), ("ldr", C.c_int32),
+                ("gamma", C.c_void_p), ("beta", C.c_void_p), ("eps", C.c_float), ("rows", C.c_int64), ("C", C.c_int32),
+                ("out", C.c_void_p), ("ldo", C.c_int32), ("relu_after", C.c_int32),
+                ("pe", C.c_void_p), ("alpha", C.c_void_p), ("L", C.c_int32),
+                ("head_w", C.c_void_p), ("head_b", C.c_void_p), ("head_out", C.c_void_p), ("dur_out", C.c_void_p),
+                ("head_scale", C.c_void_p), ("lens", C.c_void_p), ("split_out", C.c_void_p), ("split_lo", C.c_int32),
+                ("spk_table", C.c_void_p), ("spk", C.c_void_p), ("n_spk", C.c_int32), ("spk_L", C.c_int32)]
+
+
 FS2_OPTIM_CHUNK = 65536                           # elements per chunk of the optimizer's parameter table
 _P, _I, _F, _L, _SZ = C.c_void_p, C.c_int, C.c_float, C.c_int64, C.c_size_t
 
@@ -131,6 +142,8 @@ SIGNATURES = {
     "fs2_op_attention_planes": [_I, _P, _P, _I, _P, _I, _I, _I, _I, _P, _P, _P],
     "fs2_op_gemm_layernorm": [_I, _P, _L, _I, _I, _P, _P, _P, _P, _P, _F, _P, _P, _P],
     "fs2_op_layernorm": [_P, _P, _P, _P, _F, _L, _I, _P, _P],
+    "fs2_op_row_norm": [C.POINTER(RowNormDesc), _P],
+    "fs2_op_variance_embed_add": [_P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _L, _I, _P, _P, _I, _P, _P, _P, _I, _P],
     "fs2_dropout_mask": [_P, _L, _F, C.c_uint64, C.c_uint64, _P],
     "fs2_dropout_apply": [_P, _P, _F, _P, _L, _P],
     "fs2_act_backward": [_P, _P, _I, _P, _L, _P],
@@ -153,7 +166,7 @@ SIGNATURES = {
     "fs2_attn_train_ws_bytes": [_I, _I, _I, _I, C.POINTER(_SZ)],
     "fs2_attn_train_forward": [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P, C.c_uint64, C.c_uint64, _P, _P, _P, _SZ, _P],
     "fs2_attn_train_backward": [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P, C.c_uint64, C.c_uint64, _P, _P, _P, _P, _SZ, _P],
-    "fs2_embed_posenc": [_P, _P, _I, _P, _P, _I, _I, _I, _P, _P],
+    "fs2_embed_posenc": [_P, _P, _I, _P, _P, _I, _I, _I, _P, _P, _P, _P],
     "fs2_embed_backward": [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P],
     "fs2_posenc_add": [_P, _P, _P, _I, _I, _I, _P, _P],
     "fs2_speaker_add": [_P, _P, _P, _I, _I, _I, _I, _P, _P],
@@ -295,8 +308,20 @@ def load() -> C.CDLL:
     lib.fs2_bigvgan_destroy.argtypes = [_P]
     lib.fs2_istftnet_destroy.restype = None
     lib.fs2_istftnet_destroy.argtypes = [_P]
+    lib.fs2_embed_posenc = _embed_posenc_with_optional_planes(lib.fs2_embed_posenc)
     _lib = lib
     return lib
+
+
+def _embed_posenc_with_optional_planes(fn):
+    """fs2_embed_posenc took no planes and lens before they were added to it: the binding still accepts that form,
+    (xs, table, n_sym, pe, alpha, B, T, C, out, stream), and passes both as NULL."""
+    def call(*args):
+        if len(args) == len(fn.argtypes) - 2:
+            args = args[:-1] + (None, None) + args[-1:]
+        return fn(*args)
+    call.argtypes = fn.argtypes
+    return call
 
 
 def check(rc: int, what: str) -> None:

@@ -859,5 +859,26 @@ int fs2_op_layernorm(const float* x, const float* resid, const float* g, const f
   r.resid = resid; r.ldr = C;
   return row_norm(r, (cudaStream_t)stream);
 }
+int fs2_op_row_norm(const fs2_row_norm_desc* d, void* stream) {
+  FS2_REQUIRE(d, "fs2_op_row_norm: null descriptor");
+  FS2_REQUIRE(d->out || d->split_out || d->head_w, "fs2_op_row_norm: no output (out, split_out or head_w)");
+  RowNorm r;
+  r.x = d->x; r.ldx = d->ldx; r.resid = d->resid; r.ldr = d->ldr; r.gamma = d->gamma; r.beta = d->beta; r.eps = d->eps;
+  r.rows = d->rows; r.C = d->C; r.out = d->out; r.ldo = d->ldo; r.relu_after = d->relu_after;
+  r.pe = d->pe; r.alpha = d->alpha; r.L = d->L;
+  r.head_w = d->head_w; r.head_b = d->head_b; r.head_out = d->head_out; r.dur_out = d->dur_out; r.head_scale = d->head_scale;
+  r.lens = d->lens; r.split_out = reinterpret_cast<__half*>(d->split_out); r.split_lo = d->split_lo;
+  r.spk_table = d->spk_table; r.spk = d->spk; r.n_spk = d->n_spk; r.spk_L = d->spk_L;
+  return row_norm(r, (cudaStream_t)stream);
+}
+int fs2_op_variance_embed_add(const float* hm, const float* e_val, const float* p_val, const float* e_bins, const float* p_bins,
+                              int n_edges, const float* e_tab, const float* e_bias, const float* p_tab, const float* p_bias,
+                              int64_t rows, int C, float* out, void* planes, int planes_lo, int64_t* e_ids, int64_t* p_ids,
+                              const int64_t* lens, int L, void* stream) {
+  FS2_REQUIRE(hm && e_val && p_val && e_bins && p_bins && e_tab && e_bias && p_tab && p_bias && (out || planes),
+              "fs2_op_variance_embed_add: null argument");
+  return variance_embed_add(hm, e_val, p_val, e_bins, p_bins, n_edges, e_tab, e_bias, p_tab, p_bias, rows, C, out,
+                            reinterpret_cast<__half*>(planes), planes_lo, e_ids, p_ids, lens, L, (cudaStream_t)stream);
+}
 
 }  // extern "C"

@@ -289,8 +289,20 @@ __global__ void fold_batchnorm_kernel(const float* gamma, const float* beta, con
 
 }  // namespace
 
+// The kernels above move rows as float4 (operand planes as uint2): every such pointer must be null or 16-byte (8-byte)
+// aligned, checked before a launch so that a bad pointer is an FS2_ERR_INVALID naming the field, not a misaligned access.
+#define FS2_REQUIRE_ALIGNED(p, bytes, who, name) \
+  FS2_REQUIRE((reinterpret_cast<uintptr_t>(p) & ((bytes) - 1)) == 0, "%s: %s must be %d-byte aligned", who, name, bytes)
+
 int embed_posenc(const int64_t* xs, const float* table, int n_sym, const float* pe, const float* alpha, int B, int T,
                  int C, float* out, __half* planes, const int64_t* lens, cudaStream_t st) {
+  const char* who = "embed_posenc";
+  FS2_REQUIRE(C == 256 || C == 384, "%s: C=%d unsupported (256 or 384)", who, C);
+  FS2_REQUIRE(n_sym > 0, "%s: n_sym must be positive (ids outside [0, n_sym) read row 0)", who);
+  FS2_REQUIRE_ALIGNED(table, 16, who, "table");
+  FS2_REQUIRE_ALIGNED(pe, 16, who, "pe");
+  FS2_REQUIRE_ALIGNED(out, 16, who, "out");
+  FS2_REQUIRE_ALIGNED(planes, 8, who, "planes");
   long rows = (long)B * T;
   if (rows == 0) return FS2_OK;
   int grid = (int)((rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA);
@@ -302,11 +314,29 @@ int embed_posenc(const int64_t* xs, const float* table, int n_sym, const float* 
 }
 
 int row_norm(const RowNorm& r, cudaStream_t st) {
+  const char* who = "row_norm";
+  FS2_REQUIRE(r.C == 256 || r.C == 384, "%s: C=%d unsupported (256 or 384)", who, r.C);
+  FS2_REQUIRE(r.x, "%s: x is null", who);
+  FS2_REQUIRE(r.gamma && r.beta, "%s: gamma and beta are required (null argument)", who);
+  FS2_REQUIRE(r.ldx % 4 == 0, "%s: ldx must be a multiple of 4 floats", who);
+  FS2_REQUIRE(!r.resid || r.ldr % 4 == 0, "%s: ldr must be a multiple of 4 floats", who);
+  FS2_REQUIRE(!r.out || r.ldo % 4 == 0, "%s: ldo must be a multiple of 4 floats", who);
+  FS2_REQUIRE_ALIGNED(r.x, 16, who, "x");
+  FS2_REQUIRE_ALIGNED(r.resid, 16, who, "resid");
+  FS2_REQUIRE_ALIGNED(r.out, 16, who, "out");
+  FS2_REQUIRE_ALIGNED(r.gamma, 16, who, "gamma");
+  FS2_REQUIRE_ALIGNED(r.beta, 16, who, "beta");
+  FS2_REQUIRE_ALIGNED(r.pe, 16, who, "pe");
+  FS2_REQUIRE_ALIGNED(r.head_w, 16, who, "head_w");
+  FS2_REQUIRE_ALIGNED(r.spk_table, 16, who, "spk_table");
+  FS2_REQUIRE_ALIGNED(r.split_out, 8, who, "split_out");
+  FS2_REQUIRE(!r.pe || (r.alpha && r.L > 0), "%s: pe needs alpha and L > 0 (pe row t = row %% L)", who);
+  FS2_REQUIRE(!r.lens || r.L > 0, "%s: lens needs L > 0", who);
+  FS2_REQUIRE(!r.head_w || r.head_b, "%s: head_w needs head_b", who);
+  FS2_REQUIRE(!(r.head_out || r.dur_out || r.head_scale) || r.head_w,
+              "%s: head_out, dur_out and head_scale need head_w and head_b", who);
+  FS2_REQUIRE(!r.spk_table || (r.spk && r.spk_L > 0), "%s: a speaker table (spk_table) needs ids and rows per utterance", who);
   if (r.rows == 0) return FS2_OK;
-  FS2_REQUIRE(r.ldx % 4 == 0 && (!r.out || r.ldo % 4 == 0) && (!r.resid || r.ldr % 4 == 0), "row_norm: strides must be 16-byte multiples");
-  FS2_REQUIRE(!r.split_out || (reinterpret_cast<uintptr_t>(r.split_out) & 7) == 0, "row_norm: operand planes must be 8-byte aligned");
-  FS2_REQUIRE(!r.lens || r.L > 0, "row_norm: lens needs L > 0");
-  FS2_REQUIRE(!r.spk_table || (r.spk && r.spk_L > 0), "row_norm: a speaker table needs ids and rows per utterance");
   int grid = (int)((r.rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA);
   if (r.C == 256) { FS2_CUDA_CHECK(launch_pdl(row_norm_kernel<2>, dim3(grid), dim3(256), 0, st, r)); }
   else if (r.C == 384) { FS2_CUDA_CHECK(launch_pdl(row_norm_kernel<3>, dim3(grid), dim3(256), 0, st, r)); }
@@ -323,8 +353,9 @@ int bucketize(const float* vals, const float* bins, int n_edges, int64_t n, int6
 }
 
 int one_hot(const int64_t* ids, int64_t n, int n_bins, float* out, cudaStream_t st) {
+  FS2_REQUIRE(n_bins > 0 && n_bins % 4 == 0, "one_hot: n_bins must be a positive multiple of 4");
+  FS2_REQUIRE_ALIGNED(out, 16, "one_hot", "out");
   if (n == 0) return FS2_OK;
-  FS2_REQUIRE(n_bins % 4 == 0, "one_hot: n_bins must be a multiple of 4");
   one_hot_kernel<<<(int)((n + ROWS_PER_CTA - 1) / ROWS_PER_CTA), 256, 0, st>>>(ids, n, n_bins, out);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
@@ -334,8 +365,18 @@ int variance_embed_add(const float* hm, const float* e_val, const float* p_val, 
                        int n_edges, const float* e_tab, const float* e_bias, const float* p_tab, const float* p_bias,
                        int64_t rows, int C, float* out, __half* planes, int planes_lo, int64_t* e_ids, int64_t* p_ids,
                        const int64_t* lens, int L, cudaStream_t st) {
+  const char* who = "variance_embed_add";
+  FS2_REQUIRE(C == 256 || C == 384, "%s: C=%d unsupported (256 or 384)", who, C);
+  FS2_REQUIRE(n_edges >= 0, "%s: n_edges must be >= 0", who);
+  FS2_REQUIRE_ALIGNED(hm, 16, who, "hm");
+  FS2_REQUIRE_ALIGNED(e_tab, 16, who, "e_tab");
+  FS2_REQUIRE_ALIGNED(e_bias, 16, who, "e_bias");
+  FS2_REQUIRE_ALIGNED(p_tab, 16, who, "p_tab");
+  FS2_REQUIRE_ALIGNED(p_bias, 16, who, "p_bias");
+  FS2_REQUIRE_ALIGNED(out, 16, who, "out");
+  FS2_REQUIRE_ALIGNED(planes, 8, who, "planes");
+  FS2_REQUIRE(!lens || L > 0, "%s: lens needs L > 0", who);
   if (rows == 0) return FS2_OK;
-  FS2_REQUIRE(!lens || L > 0, "variance_embed_add: lens needs L > 0");
   int grid = (int)((rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA);
   if (C == 256) {
     FS2_CUDA_CHECK(launch_pdl(variance_embed_add_kernel<2>, dim3(grid), dim3(256), 0, st, hm, e_val, p_val, e_bins, p_bins, n_edges, e_tab, e_bias, p_tab,

@@ -679,9 +679,9 @@ int fs2_embed_backward(const int64_t* xs, const float* dy, const float* pe, int 
   return FS2_OK;
 }
 int fs2_embed_posenc(const int64_t* xs, const float* table, int n_sym, const float* pe, const float* alpha, int B, int T, int C, float* out,
-                     void* stream) {
+                     void* planes, const int64_t* lens, void* stream) {
   FS2_REQUIRE(xs && table && pe && alpha && out, "fs2_embed_posenc: null argument");
-  return embed_posenc(xs, table, n_sym, pe, alpha, B, T, C, out, nullptr, nullptr, (cudaStream_t)stream);
+  return embed_posenc(xs, table, n_sym, pe, alpha, B, T, C, out, reinterpret_cast<__half*>(planes), lens, (cudaStream_t)stream);
 }
 int fs2_posenc_add(const float* x, const float* pe, const float* alpha, int B, int T, int C, float* y, void* stream) {
   FS2_REQUIRE(x && pe && alpha && y, "fs2_posenc_add: null argument");

@@ -337,7 +337,7 @@ class EmbedFn(torch.autograd.Function):
         out = torch.empty((B, T, C_), dtype=torch.float32, device=xs.device)
         pe2 = _c(pe.reshape(-1, C_))
         _chk(_lib.load().fs2_embed_posenc(xs.data_ptr(), _c(table.detach()).data_ptr(), table.shape[0], pe2.data_ptr(), alpha.detach().reshape(1).data_ptr(),
-                                          B, T, C_, out.data_ptr(), _st(xs)), "fs2_embed_posenc")
+                                          B, T, C_, out.data_ptr(), None, None, _st(xs)), "fs2_embed_posenc")
         ctx.save_for_backward(xs, pe2)
         ctx.meta = (B, T, C_, table.shape[0])
         return out

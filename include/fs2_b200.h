@@ -322,6 +322,46 @@ int fs2_op_attention_planes(int math_mode, const void* qkp, const void* vtp, int
 /* y = LayerNorm_C(x (+resid)) * g + b over the last dim (C in {256,384}) */
 int fs2_op_layernorm(const float* x, const float* resid, const float* g, const float* b, float eps, int64_t rows, int C,
                      float* out, void* stream);
+/* The row LayerNorm kernel with every fusion the stages use (csrc/rowwise.cu), one warp per row of C in {256, 384}:
+ *   v = x[row] (+ resid[row])                                     statistics in fp32, rstd = 1 / sqrtf(var + eps)
+ *   y = (v - mean) * rstd * gamma + beta
+ *   y = relu(y)                                        relu_after != 0
+ *   y = y + (alpha * pe[row % L])                      pe != NULL (needs alpha and L > 0), one rounding per op
+ *   y = y + spk_table[spk[row / spk_L]]                spk_table != NULL; ids outside [0, n_spk) add nothing
+ *   s = y . head_w + *head_b                           head_w != NULL: head_out[row] = s, or fp32(s * head_scale[row]);
+ *                                                      dur_out[row] = (int64) max(rint(expf(s) - 1), 0), half to even
+ *   rows t = row % L >= lens[row / L] (lens != NULL, L > 0) write 0 to out, split_out, head_out and dur_out.
+ * Outputs: out [rows][ldo] fp32; split_out fp16 operand planes of y scaled by 16, hi at [row][C] and, when split_lo, lo at
+ * [rows + row][C].  x, resid, out, gamma, beta, pe, head_w and spk_table must be 16-byte aligned, split_out 8-byte
+ * aligned, and ldx, ldr, ldo multiples of 4; head_out, dur_out and head_scale need head_w and head_b.  A call that breaks
+ * any of these returns FS2_ERR_INVALID, naming the field, before anything is launched. */
+typedef struct fs2_row_norm_desc {
+  const float* x; int32_t ldx;
+  const float* resid; int32_t ldr;
+  const float* gamma; const float* beta; float eps;
+  int64_t rows; int32_t C;
+  float* out; int32_t ldo;
+  int32_t relu_after;
+  const float* pe; const float* alpha; int32_t L;
+  const float* head_w; const float* head_b; float* head_out; int64_t* dur_out;
+  const float* head_scale;
+  const int64_t* lens;
+  void* split_out; int32_t split_lo;
+  const float* spk_table; const int64_t* spk; int32_t n_spk; int32_t spk_L;
+} fs2_row_norm_desc;
+int fs2_op_row_norm(const fs2_row_norm_desc* d, void* stream);
+/* hs + pitch_embed(one_hot(p_ids)) + energy_embed(one_hot(e_ids)) (fastspeech.py:218-219) as the decode stage runs it,
+ * over rows = B * L rows of C in {256, 384}:
+ *   id = torch.bucketize(val, bins) over n_edges sorted edges (NaN -> n_edges)
+ *   out[row] = (hm[row] + (p_tab[p_id] + p_bias)) + (e_tab[e_id] + e_bias)
+ * e_tab / p_tab [n_edges + 1][C]: row i is column i of the embedding Linear's weight.  e_ids / p_ids (nullable) receive
+ * the ids.  lens (nullable, with L > 0): rows t = row % L >= lens[row / L] get zero rows and ids -1.  planes (nullable)
+ * fp16 operand planes of out scaled by 16, hi at [row][C] and, when planes_lo, lo at [rows + row][C].  hm, the tables,
+ * the biases and out must be 16-byte aligned, planes 8-byte aligned (FS2_ERR_INVALID otherwise). */
+int fs2_op_variance_embed_add(const float* hm, const float* e_val, const float* p_val, const float* e_bins, const float* p_bins,
+                              int n_edges, const float* e_tab, const float* e_bias, const float* p_tab, const float* p_bias,
+                              int64_t rows, int C, float* out, void* planes, int planes_lo, int64_t* e_ids, int64_t* p_ids,
+                              const int64_t* lens, int L, void* stream);
 
 /* ---- train mode (SURVEY.md section 8f-1): dropout, BatchNorm batch statistics and the backward of every stage ------- */
 /* What `model.train(); loss, _ = model(...); loss.backward()` of train_fastspeech.py:100-123 needs; fp32 on CUDA cores
@@ -397,9 +437,13 @@ int fs2_attn_train_forward(const float* q, const float* k, const float* v, const
 int fs2_attn_train_backward(const float* q, const float* k, const float* v, const float* out, const float* lse, const float* dout,
                             const int64_t* lens, int B, int L, int C, int heads, float p_drop, const uint8_t* dmask, uint64_t seed,
                             uint64_t offset, float* dq, float* dk, float* dv, void* ws, size_t ws_bytes, void* stream);
-/* encoder input (fastspeech.py:65-67 + embedding.py:105-120 before its dropout) and its backward; decoder-side x + alpha*pe */
+/* encoder input (fastspeech.py:65-67 + embedding.py:105-120 before its dropout) and its backward; decoder-side x + alpha*pe.
+ * fs2_embed_posenc: out[b,t] = table[id] + (alpha * pe[t]), id = xs[b,t] (ids outside [0, n_sym) read row 0), C in
+ * {256, 384}.  planes (nullable): hi + lo fp16 operand planes of out scaled by 16, [2][B*T][C]; lens (nullable) [B]: rows
+ * t >= lens[b] are written as zeros, as fs2_encode_ex does in per-utterance mode.  table, pe and out must be 16-byte
+ * aligned, planes 8-byte aligned (FS2_ERR_INVALID otherwise). */
 int fs2_embed_posenc(const int64_t* xs, const float* table, int n_sym, const float* pe, const float* alpha, int B, int T, int C, float* out,
-                     void* stream);
+                     void* planes, const int64_t* lens, void* stream);
 int fs2_embed_backward(const int64_t* xs /* NULL: positional part only */, const float* dy, const float* pe, int B, int T, int C, int n_sym,
                        float* dtable /* += or NULL */, float* dalpha /* += */, void* stream);
 int fs2_posenc_add(const float* x, const float* pe, const float* alpha, int B, int T, int C, float* y, void* stream);

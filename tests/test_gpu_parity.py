@@ -359,20 +359,6 @@ def test_fused_gemm_layernorm_vs_torch(prec, N, rows, K, with_resid):
         assert float(((planes - out).abs() - rel * out.abs()).max()) <= 1e-6, float((planes - out).abs().max())
 
 
-@pytest.mark.parametrize("C", [256, 384])
-def test_layernorm_vs_torch(C):
-    g = torch.Generator().manual_seed(C)
-    x, r = torch.randn(1000, C, generator=g) * 3, torch.randn(1000, C, generator=g)
-    w, b = torch.randn(C, generator=g), torch.randn(C, generator=g)
-    want = torch.nn.functional.layer_norm(x + r, (C,), w, b, 1e-5)
-    out = torch.empty(1000, C, device="cuda")
-    lib = _lib.load()
-    xc, rc, wc, bc = x.cuda(), r.cuda(), w.cuda(), b.cuda()
-    _lib.check(lib.fs2_op_layernorm(_lib.ptr(xc), _lib.ptr(rc), _lib.ptr(wc), _lib.ptr(bc), 1e-5, 1000, C, _lib.ptr(out),
-                                    _lib.stream_ptr(out.device)), "fs2_op_layernorm")
-    close(out, want, dict(max=1e-5, mean=1e-6), "layernorm")
-
-
 # ---- edge cases -------------------------------------------------------------------------------------
 @pytest.mark.parametrize("prec", PRECISIONS)
 def test_edge_shapes_vs_oracle(models, weights, prec):

@@ -4,6 +4,8 @@ import ctypes
 import json
 import os
 import re
+import shutil
+import subprocess
 
 import pytest
 import torch
@@ -112,3 +114,37 @@ def test_library_rejects_bad_arguments_without_a_gpu():
     lib = _lib.load()
     assert lib.fs2_length_gather(None, None, None, 1, 1, 256, None, 8, None) == -1
     assert b"null" in lib.fs2_last_error()
+
+
+@pytest.mark.skipif(shutil.which("gcc") is None, reason="gcc not available")
+def test_row_norm_desc_layout_matches_header(tmp_path):
+    """_lib.RowNormDesc has fs2_row_norm_desc's fields in order, at the header's offsets and size; the row-kernel entries
+    take as many arguments as the header declares."""
+    header = open(os.path.join(REPO, "include", "fs2_b200.h")).read()
+    fields = [n for n, _ in _lib.RowNormDesc._fields_]
+    src = tmp_path / "layout.c"
+    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "fs2_b200.h"\nint main(void) {\n'
+                   + "".join(f'  printf("%zu ", offsetof(fs2_row_norm_desc, {n}));\n' for n in fields)
+                   + '  printf("%zu\\n", sizeof(fs2_row_norm_desc));\n  return 0;\n}\n')
+    exe = str(tmp_path / "layout")
+    r = subprocess.run(["gcc", "-std=c99", "-I", os.path.join(REPO, "include"), str(src), "-o", exe], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    got = [int(v) for v in subprocess.run([exe], capture_output=True, text=True, check=True).stdout.split()]
+    want = [getattr(_lib.RowNormDesc, n).offset for n in fields] + [ctypes.sizeof(_lib.RowNormDesc)]
+    assert got == want
+    body = re.search(r"typedef struct fs2_row_norm_desc \{(.*?)\} fs2_row_norm_desc;", header, re.S).group(1)
+    assert re.findall(r"\**(\w+)\s*[;,]", body) == fields
+    for name in ("fs2_op_row_norm", "fs2_op_variance_embed_add", "fs2_embed_posenc"):
+        params = re.search(rf"int {name}\((.*?)\);", header, re.S).group(1)
+        assert len(params.split(",")) == len(_lib.SIGNATURES[name]), name
+
+
+def test_embed_posenc_binding_takes_both_forms():
+    """The binding passes planes and lens as NULL when a caller omits them (the entry's form before they existed); either
+    form reaches the library, which refuses the null xs before any launch."""
+    lib = _lib.load()
+    a = 0x10000
+    assert lib.fs2_embed_posenc(None, a, 10, a, a, 2, 4, 256, a, None) == -1 and b"null" in lib.fs2_last_error()
+    assert lib.fs2_embed_posenc(None, a, 10, a, a, 2, 4, 256, a, None, None, None) == -1 and b"null" in lib.fs2_last_error()
+    with pytest.raises(TypeError):
+        lib.fs2_embed_posenc(None, a, 10, a, a, 2, 4, 256, a, None, None)
