@@ -178,6 +178,24 @@ SIGNATURES = {
     "fs2_rowdot": [_P, _P, _P, _P, _L, _I, _I, _P, _P],
     "fs2_rowdot_backward": [_P, _P, _P, _P, _L, _I, _I, _P, _P, _P, _P],
     "fs2_loss_backward": [_P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P],
+    "fs2_colsum_det_ws_bytes": [_L, _I, C.POINTER(_SZ)],
+    "fs2_colsum_det": [_P, _L, _I, _P, _P, _SZ, _P],
+    "fs2_conv_wgrad_det_ws_bytes": [_I, _I, _I, _I, _I, C.POINTER(_SZ)],
+    "fs2_conv_wgrad_det": [_P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_layernorm_backward_det_ws_bytes": [_L, _I, C.POINTER(_SZ)],
+    "fs2_layernorm_backward_det": [_P, _P, _P, _F, _L, _I, _P, _P, _P, _P, _SZ, _P],
+    "fs2_batchnorm_train_det_ws_bytes": [_L, _I, C.POINTER(_SZ)],
+    "fs2_batchnorm_train_det": [_P, _L, _I, _P, _P, _F, _F, _I, _P, _P, _P, _P, _P, _SZ, _P],
+    "fs2_batchnorm_backward_det_ws_bytes": [_L, _I, C.POINTER(_SZ)],
+    "fs2_batchnorm_backward_det": [_P, _P, _P, _P, _F, _L, _I, _P, _P, _P, _P, _SZ, _P],
+    "fs2_embed_backward_det_ws_bytes": [_I, _I, _I, _I, C.POINTER(_SZ)],
+    "fs2_embed_backward_det": [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_onehot_linear_backward_det_ws_bytes": [_L, _I, _I, C.POINTER(_SZ)],
+    "fs2_onehot_linear_backward_det": [_P, _P, _L, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_rowdot_backward_det_ws_bytes": [_L, _I, C.POINTER(_SZ)],
+    "fs2_rowdot_backward_det": [_P, _P, _P, _P, _L, _I, _I, _P, _P, _P, _P, _SZ, _P],
+    "fs2_masked_losses_det_ws_bytes": [_I, _I, _I, _I, C.POINTER(_SZ)],
+    "fs2_masked_losses_det": [_P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _SZ, _P],
     "fs2_stft_frames": [_P, _I, _I, _I, _I, _I, _P, _P],
     "fs2_stft_magphase": [_P, _I, _I, _I, _I, _P, _P, _P],
     "fs2_istft_recombine": [_P, _P, _I, _I, _I, _I, _P, _P],

@@ -306,12 +306,15 @@ class Aligner(nn.Module):
             raise ValueError("inputs must be CUDA tensors on one device (the aligner has no CPU path)")
         return xs.to(torch.int64).contiguous(), ilens.to(torch.int64).contiguous(), mels.contiguous(), olens.to(torch.int64).contiguous()
 
-    def keys_queries(self, xs, ilens, mels, olens):
-        """(k [B, T, 80], q [B, L, 80]) on the library's kernels, differentiable in the parameters."""
+    def keys_queries(self, xs, ilens, mels, olens, deterministic: bool = False):
+        """(k [B, T, 80], q [B, L, 80]) on the library's kernels, differentiable in the parameters.  `deterministic`: the
+        embedding and bias gradients are summed in a fixed order (the deterministic train mode, DESIGN.md §26)."""
         tf32, relu, none = _lib.MATH_TF32, _train.ACT_RELU, _train.ACT_NONE
         B, T = xs.shape
         zero = torch.zeros((1,), dtype=torch.float32, device=xs.device)
-        h = _train.EmbedFn.apply(xs, self.embed.weight, zero, torch.zeros((T, EMB), dtype=torch.float32, device=xs.device))
+        det = bool(deterministic)
+        tf32 = _train.conv_math(tf32, det)
+        h = _train.EmbedFn.apply(xs, self.embed.weight, zero, torch.zeros((T, EMB), dtype=torch.float32, device=xs.device), det)
         h = _train.ConvFn.apply(MaskRowsFn.apply(h, ilens), self.key_conv1.weight, self.key_conv1.bias, relu, None, tf32)
         k = _train.ConvFn.apply(MaskRowsFn.apply(h, ilens), self.key_conv2.weight, self.key_conv2.bias, none, None, tf32)
         m = _train.ConvFn.apply(MaskRowsFn.apply(mels, olens), self.query_conv1.weight, self.query_conv1.bias, relu, None, tf32)
@@ -319,13 +322,15 @@ class Aligner(nn.Module):
         q = _train.ConvFn.apply(MaskRowsFn.apply(m, olens), self.query_conv3.weight, self.query_conv3.bias, none, None, tf32)
         return k, q
 
-    def loss(self, xs, ilens, mels, olens, bin_weight: float = 0.0):
+    def loss(self, xs, ilens, mels, olens, bin_weight: float = 0.0, deterministic: bool = False):
         """(loss, forward-sum mean, bin mean or None, status): the batch means of the per-utterance losses, loss =
         forward-sum + bin_weight * bin (the binarization loss and its MAS are skipped when bin_weight is 0).  status is
-        an int32 device tensor of the entries' status words; nothing is read back to the host."""
+        an int32 device tensor of the entries' status words; nothing is read back to the host.  `deterministic`: see
+        keys_queries (also on whenever torch.are_deterministic_algorithms_enabled())."""
         xs, ilens, mels, olens = self._inputs(xs, ilens, mels, olens)
         status = torch.zeros((7,), dtype=torch.int32, device=xs.device)
-        k, q = self.keys_queries(xs, ilens, mels, olens)
+        det = bool(deterministic) or torch.are_deterministic_algorithms_enabled()
+        k, q = self.keys_queries(xs, ilens, mels, olens, det)
         logp = AlignLogProbFn.apply(q, k, ilens, olens, status)
         fs = ForwardSumFn.apply(logp, ilens, olens, status).mean()
         if not bin_weight:
@@ -388,9 +393,12 @@ class Corpus:
 
 
 def train(corpus: Corpus, n_symbols: int, steps: int, batch: int = 32, bin_start: Optional[int] = None, seed: int = 0,
-          warmup: int = 4000, factor: float = 1.0, grad_clip: float = 1.0, device="cuda", log=print, log_every: int = 100):
+          warmup: int = 4000, factor: float = 1.0, grad_clip: float = 1.0, device="cuda", log=print, log_every: int = 100,
+          deterministic: bool = False):
     """Trains an Aligner for `steps` steps of `batch` utterances (length-bucketed) with NoamAdam(model size 256, factor,
     warmup), clipping at grad_clip; the binarization loss is weighted 1 from step bin_start on (default steps // 2).
+    `deterministic` (or torch.use_deterministic_algorithms(True)): every gradient is summed in a fixed order, so the same
+    corpus and seed give the same weights bit for bit (DESIGN.md §26).
     Returns (model, [(step, loss, forward-sum, bin or None)] at every log_every-th step)."""
     if not corpus.lines:
         raise ValueError("no trainable lines in the corpus")
@@ -405,7 +413,8 @@ def train(corpus: Corpus, n_symbols: int, steps: int, batch: int = 32, bin_start
         for idx in sampler:
             if step >= steps:
                 break
-            loss, fs, bl, status = model.loss(*corpus.batch(idx, device), bin_weight=1.0 if step >= bin_start else 0.0)
+            loss, fs, bl, status = model.loss(*corpus.batch(idx, device), bin_weight=1.0 if step >= bin_start else 0.0,
+                                              deterministic=deterministic)
             opt.zero_grad()
             loss.backward()
             opt.clip_and_step(grad_clip)
@@ -495,6 +504,8 @@ def main(argv=None) -> None:
     t.add_argument("--steps", type=int, default=20000)
     t.add_argument("--bin-start", type=int, default=None, help="step from which the binarization loss is on (default: steps / 2)")
     t.add_argument("-o", "--out", required=True, help="checkpoint to write")
+    t.add_argument("--deterministic", action="store_true",
+                   help="sum every gradient in a fixed order, so a rerun gives the same checkpoint bit for bit")
     e = sub.choices["extract"]
     e.add_argument("-p", "--checkpoint", required=True, help="aligner checkpoint written by train")
     e.add_argument("--out", required=True, help="filelist to write")
@@ -507,7 +518,7 @@ def main(argv=None) -> None:
     if args.cmd == "train":
         symbols = build_symbols(lines)
         corpus = Corpus(lines, symbols, data_dir, log=lambda m: print(m, file=sys.stderr))
-        model, _ = train(corpus, len(symbols), args.steps, args.batch, args.bin_start)
+        model, _ = train(corpus, len(symbols), args.steps, args.batch, args.bin_start, deterministic=args.deterministic)
         save(args.out, model, symbols, args.steps)
         return
     model, symbols, _ = load(args.checkpoint)

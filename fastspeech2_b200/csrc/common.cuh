@@ -179,6 +179,42 @@ int masked_losses(const float* before, const float* after, const float* ys, int 
                   const int64_t* ilens, const int64_t* olens, int B, int T, int L, int odim, float* out7, void* scratch,
                   cudaStream_t st);
 
+// ---- deterministic train mode (DESIGN.md section 26): ordered sums, no floating-point atomics ----
+// dw[n][k][j] += sum over q < splits, in ascending q, of part[q][j][n][k] (wgrad_tc.cu); taps = N = 1 sums rows of [splits][K]
+int ordered_reduce(const float* part, int splits, int taps, int N, int K, float* dw, cudaStream_t st);
+// out[k] = sum_{i < n} part[k * sk + i * si], k < K, in double, in a fixed order (train.cu)
+int ordered_sum_f64(const double* part, long n, long si, long sk, int K, double* out, cudaStream_t st);
+// workspace of masked_losses_det and its carve (train.cu)
+size_t loss_det_ws_bytes(int B, int T, int L, int odim);
+int loss_det_carve(void* ws, int B, int T, int L, int odim, double** acc, double** mel, long* n_mel, double** seq, long* n_seq);
+int masked_losses_det(const float* before, const float* after, const float* ys, int ld_ys_time, const float* d_out,
+                      const void* ds, int ds_dtype, const float* e_out, const float* p_out, const float* es, const float* ps,
+                      const int64_t* ilens, const int64_t* olens, int B, int T, int L, int odim, float* out7, void* ws,
+                      cudaStream_t st);
+// the bodies of the ordered train entries (train.cu); the C entries with their argument checks are in train_det.cu
+size_t colsum_det_bytes(long rows, int C);
+int colsum_det(const float* x, long rows, int C, float* out, void* ws, cudaStream_t st);
+size_t conv_wgrad_det_bytes(int B, int L, int N, int K, int taps, bool bias);
+int conv_wgrad_det(const float* dy, const float* x, int B, int L, int N, int K, int taps, float* dw, float* dbias, void* ws, cudaStream_t st);
+size_t layernorm_backward_det_bytes(long rows, int C);
+int layernorm_backward_det(const float* x, const float* dy, const float* gamma, float eps, long rows, int C, float* dx, float* dgamma,
+                           float* dbeta, void* ws, cudaStream_t st);
+size_t batchnorm_det_bytes(long rows, int C);
+int batchnorm_train_det(const float* x, long rows, int C, const float* gamma, const float* beta, float eps, float momentum, int act,
+                        float* running_mean, float* running_var, float* stats, float* y, void* ws, cudaStream_t st);
+int batchnorm_backward_det(const float* x, const float* dy, const float* stats, const float* gamma, float eps, long rows, int C, float* dx,
+                           float* dgamma, float* dbeta, void* ws, cudaStream_t st);
+size_t embed_backward_det_bytes(long rows, int C, int n_sym, bool table);
+int embed_backward_det(const int64_t* xs, const float* dy, const float* pe, int B, int T, int C, int n_sym, float* dtable, float* dalpha,
+                       void* ws, cudaStream_t st);
+size_t onehot_linear_backward_det_bytes(long rows, int C, int n_bins, bool bias);
+int onehot_linear_backward_det(const int64_t* ids, const float* dy, long rows, int C, int n_bins, float* dW, float* dbias, void* ws,
+                               cudaStream_t st);
+size_t rowdot_backward_det_bytes(long rows, int C);
+int rowdot_backward_det(const float* x, const float* w, const float* dy, const int64_t* lens, long rows, int L, int C, float* dx, float* dw,
+                        float* dbias, void* ws, cudaStream_t st);
+int scatter_max_ids();   // largest id range (n_sym, n_bins) of the ordered scatter
+
 // weight repacking helpers (pack.cu)
 int pack_conv_weight(const float* src, int N, int K, int taps, const float* scale /*[N] or null*/, float* dst,
                      cudaStream_t st);  // src [N][K][taps] -> dst [taps][N][K] * scale[n]

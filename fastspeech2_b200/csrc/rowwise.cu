@@ -198,11 +198,25 @@ __global__ void variance_embed_add_kernel(const float* __restrict__ hm, const fl
 
 // ---- masked losses (fastspeech.py:277-333) ---------------------------------------------------
 // acc[0..4] (double): sum|before-ys|, sum|after-ys|, sum(d-log(ds+1))^2, sum(e-es)^2, sum(p-ps)^2
+// kOrdered (deterministic train mode, DESIGN.md section 26): acc is the partial table [sums][grid.y][grid.x]: each block adds
+// its warps' sums in warp order and stores one double per sum; ordered_sum_f64 then adds the blocks in a fixed order.
+template <bool kOrdered>
 __device__ __forceinline__ void block_accumulate(float v, double* dst) {
   v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0 && v != 0.f) atomicAdd(dst, (double)v);
+  if constexpr (kOrdered) {
+    __shared__ float sw[32];
+    __syncthreads();                      // the previous sum's readers are done with sw
+    if ((threadIdx.x & 31) == 0) sw[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double t = 0.0;
+      for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += (double)sw[w];
+      dst[(long)blockIdx.y * gridDim.x + blockIdx.x] = t;
+    }
+  } else if ((threadIdx.x & 31) == 0 && v != 0.f) atomicAdd(dst, (double)v);
 }
 
+template <bool kOrdered>
 __global__ void loss_mel_kernel(const float* __restrict__ before, const float* __restrict__ after,
                                 const float* __restrict__ ys, int ld_ys_time, const int64_t* __restrict__ olens, int L,
                                 int odim, double* acc) {
@@ -219,10 +233,12 @@ __global__ void loss_mel_kernel(const float* __restrict__ before, const float* _
     s0 += (fabsf(x0.x - y.x) + fabsf(x0.y - y.y)) + (fabsf(x0.z - y.z) + fabsf(x0.w - y.w));
     s1 += (fabsf(x1.x - y.x) + fabsf(x1.y - y.y)) + (fabsf(x1.z - y.z) + fabsf(x1.w - y.w));
   }
-  block_accumulate(s0, acc + 0);
-  block_accumulate(s1, acc + 1);
+  const long nb = kOrdered ? (long)gridDim.x * gridDim.y : 1;   // distance between two sums' slots
+  block_accumulate<kOrdered>(s0, acc + 0 * nb);
+  block_accumulate<kOrdered>(s1, acc + 1 * nb);
 }
 
+template <bool kOrdered>
 __global__ void loss_seq_kernel(const float* __restrict__ d_out, const void* __restrict__ ds, int ds_dtype,
                                 const float* __restrict__ e_out, const float* __restrict__ p_out,
                                 const float* __restrict__ es, const float* __restrict__ ps,
@@ -243,9 +259,11 @@ __global__ void loss_seq_kernel(const float* __restrict__ d_out, const void* __r
     float de = e_out[o] - es[o], dp = p_out[o] - ps[o];
     se += de * de; sp += dp * dp;
   }
-  block_accumulate(sd, acc + 2);
-  block_accumulate(se, acc + 3);
-  block_accumulate(sp, acc + 4);
+  const long nb = kOrdered ? (long)gridDim.x * gridDim.y : 1;
+  double* a = kOrdered ? acc : acc + 2;   // the ordered table of this kernel holds its three sums only
+  block_accumulate<kOrdered>(sd, a + 0 * nb);
+  block_accumulate<kOrdered>(se, a + 1 * nb);
+  block_accumulate<kOrdered>(sp, a + 2 * nb);
 }
 
 __global__ void loss_finalize_kernel(const double* acc, const int64_t* ilens, const int64_t* olens, int B, int odim,
@@ -390,23 +408,45 @@ int variance_embed_add(const float* hm, const float* e_val, const float* p_val, 
   return FS2_OK;
 }
 
-int masked_losses(const float* before, const float* after, const float* ys, int ld_ys_time, const float* d_out,
-                  const void* ds, int ds_dtype, const float* e_out, const float* p_out, const float* es, const float* ps,
-                  const int64_t* ilens, const int64_t* olens, int B, int T, int L, int odim, float* out7, void* scratch,
-                  cudaStream_t st) {
+// kOrdered: scratch is the workspace of loss_det_ws_bytes (the five sums, then the two kernels' partial tables)
+template <bool kOrdered>
+int masked_losses_impl(const float* before, const float* after, const float* ys, int ld_ys_time, const float* d_out,
+                       const void* ds, int ds_dtype, const float* e_out, const float* p_out, const float* es, const float* ps,
+                       const int64_t* ilens, const int64_t* olens, int B, int T, int L, int odim, float* out7, void* scratch,
+                       cudaStream_t st) {
   double* acc = reinterpret_cast<double*>(scratch);
+  double *mel = nullptr, *seq = nullptr;
+  long n_mel = 0, n_seq = 0;
+  if (kOrdered) loss_det_carve(scratch, B, T, L, odim, &acc, &mel, &n_mel, &seq, &n_seq);
   FS2_REQUIRE(odim % 4 == 0 && (reinterpret_cast<uintptr_t>(ys) & 15) == 0, "masked_losses: odim must be a multiple of 4 and ys 16-byte aligned");
   FS2_CUDA_CHECK(cudaMemsetAsync(acc, 0, 8 * sizeof(double), st));
   if (B > 0) {
     dim3 g1(grid_for((long)L * odim / 4, 256, 32), B), g2(grid_for(L > T ? L : T, 256, 16), B);
-    loss_mel_kernel<<<g1, 256, 0, st>>>(before, after, ys, ld_ys_time, olens, L, odim, acc);
+    loss_mel_kernel<kOrdered><<<g1, 256, 0, st>>>(before, after, ys, ld_ys_time, olens, L, odim, kOrdered ? mel : acc);
     FS2_LAUNCH_CHECK();
-    loss_seq_kernel<<<g2, 256, 0, st>>>(d_out, ds, ds_dtype, e_out, p_out, es, ps, ilens, olens, T, L, acc);
+    loss_seq_kernel<kOrdered><<<g2, 256, 0, st>>>(d_out, ds, ds_dtype, e_out, p_out, es, ps, ilens, olens, T, L, kOrdered ? seq : acc);
     FS2_LAUNCH_CHECK();
+    int rc;
+    if (kOrdered && ((rc = ordered_sum_f64(mel, n_mel, 1, n_mel, 2, acc, st)) || (rc = ordered_sum_f64(seq, n_seq, 1, n_seq, 3, acc + 2, st))))
+      return rc;
   }
   loss_finalize_kernel<<<1, 1, 0, st>>>(acc, ilens, olens, B, odim, out7);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
+}
+int masked_losses(const float* before, const float* after, const float* ys, int ld_ys_time, const float* d_out,
+                  const void* ds, int ds_dtype, const float* e_out, const float* p_out, const float* es, const float* ps,
+                  const int64_t* ilens, const int64_t* olens, int B, int T, int L, int odim, float* out7, void* scratch,
+                  cudaStream_t st) {
+  return masked_losses_impl<false>(before, after, ys, ld_ys_time, d_out, ds, ds_dtype, e_out, p_out, es, ps, ilens, olens, B, T, L, odim,
+                                   out7, scratch, st);
+}
+int masked_losses_det(const float* before, const float* after, const float* ys, int ld_ys_time, const float* d_out,
+                      const void* ds, int ds_dtype, const float* e_out, const float* p_out, const float* es, const float* ps,
+                      const int64_t* ilens, const int64_t* olens, int B, int T, int L, int odim, float* out7, void* ws,
+                      cudaStream_t st) {
+  return masked_losses_impl<true>(before, after, ys, ld_ys_time, d_out, ds, ds_dtype, e_out, p_out, es, ps, ilens, olens, B, T, L, odim,
+                                  out7, ws, st);
 }
 
 int pack_conv_weight(const float* src, int N, int K, int taps, const float* scale, float* dst, cudaStream_t st) {

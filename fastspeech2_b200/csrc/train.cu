@@ -43,6 +43,9 @@ __global__ void add_kernel(const float* __restrict__ a, const float* __restrict_
 }
 
 // ---- column sums: out[c] (+)= sum_r x[r, c]  (bias gradients) ----------------------------------------------------------------
+// kOrdered (the deterministic train mode, DESIGN.md section 26): out is the partial table [grid.y][C], one store per column
+// and grid.y block instead of the atomic; ordered_reduce then adds the partials in ascending grid.y.
+template <bool kOrdered>
 __global__ void colsum_kernel(const float* __restrict__ x, long rows, int C, float* __restrict__ out) {
   // block = 256 threads = 32 columns x 8 row-lanes; grid (C/32 ceil, row chunks)
   __shared__ float red[8][33];
@@ -56,7 +59,8 @@ __global__ void colsum_kernel(const float* __restrict__ x, long rows, int C, flo
     float t = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) t += red[i][threadIdx.x & 31];
-    atomicAdd(out + c, t);
+    if constexpr (kOrdered) out[(long)blockIdx.y * C + c] = t;
+    else atomicAdd(out + c, t);
   }
 }
 
@@ -64,7 +68,10 @@ __global__ void colsum_kernel(const float* __restrict__ x, long rows, int C, flo
 // dW[n][k][j] += sum_{b,t} dy[b,t,n] * x[b, t + j - pad, k]   (x zero outside [0,L)); output in the REFERENCE's layout
 // [N][K][taps] (nn.Conv1d weight; taps == 1 is nn.Linear's [N][K]).  64 x 64 output tile per CTA, the reduction over the
 // B*L rows is split over gridDim.z chunks and combined with atomicAdd (the gradient buffer is zero-initialised by autograd).
+// kOrdered: with several chunks dw is the partial table [chunks][taps][N][K] (wgrad_tc.cu's layout, summed by ordered_reduce);
+// with one chunk each output has one writer, which adds its tile straight into dw.
 constexpr int WG_T = 64, WG_KM = 16;
+template <bool kOrdered>
 __global__ void __launch_bounds__(256)
 wgrad_kernel(const float* __restrict__ dy, int ldy, const float* __restrict__ x, int ldx, int B, int L, int N, int K, int taps,
              int chunks, float* __restrict__ dw) {
@@ -108,7 +115,11 @@ wgrad_kernel(const float* __restrict__ dy, int ldy, const float* __restrict__ x,
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const int n = n0 + ty * 4 + i, k = k0 + tx * 4 + q;
-      if (n < N && k < K) atomicAdd(dw + ((long)n * K + k) * taps + j, acc[i][q]);
+      if (n < N && k < K) {
+        if constexpr (!kOrdered) atomicAdd(dw + ((long)n * K + k) * taps + j, acc[i][q]);
+        else if (chunks == 1) dw[((long)n * K + k) * taps + j] += acc[i][q];
+        else dw[(((long)chunk * taps + j) * N + n) * K + k] = acc[i][q];
+      }
     }
 }
 // reference layout [N][K][taps] -> dgrad operand in kernel layout [taps][K][N] with the taps reversed:
@@ -123,14 +134,18 @@ __global__ void pack_dgrad_weight_kernel(const float* __restrict__ w, int N, int
 
 // ---- LayerNorm backward (nn.LayerNorm over the last dim; encoder.py:37-38, modules.py:112-120) ---------------------------------
 // x: the saved INPUT rows [rows, C]; dy, gamma -> dx; dgamma, dbeta accumulated with atomics (one partial sum per CTA).
-template <int NV>
+// kOrdered: each warp stores its sums as one row of shared memory, the rows are added in warp order, and dgamma / dbeta
+// are the partial tables [grid][C] (one row per CTA, summed across CTAs in CTA order by the caller).
+template <int NV, bool kOrdered>
 __global__ void __launch_bounds__(256)
 layernorm_backward_kernel(const float* __restrict__ x, const float* __restrict__ dy, const float* __restrict__ gamma, float eps, long rows,
                           float* __restrict__ dx, float* __restrict__ dgamma, float* __restrict__ dbeta) {
-  constexpr int C = NV * 128;
-  __shared__ float sg[C], sb[C];
-  for (int i = threadIdx.x; i < C; i += blockDim.x) { sg[i] = 0.f; sb[i] = 0.f; }
-  __syncthreads();
+  constexpr int C = NV * 128, WR = kOrdered ? 8 : 1;
+  __shared__ float sg[WR * C], sb[WR * C];
+  if constexpr (!kOrdered) {
+    for (int i = threadIdx.x; i < C; i += blockDim.x) { sg[i] = 0.f; sb[i] = 0.f; }
+    __syncthreads();
+  }
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   float4 g4[NV];
 #pragma unroll
@@ -174,19 +189,36 @@ layernorm_backward_kernel(const float* __restrict__ x, const float* __restrict__
       *reinterpret_cast<float4*>(dx + row * C + i * 128 + lane * 4) = o;
     }
   }
+  if constexpr (kOrdered) {
 #pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int c = i * 128 + lane * 4;
-    atomicAdd(&sg[c], ag[i].x); atomicAdd(&sg[c + 1], ag[i].y); atomicAdd(&sg[c + 2], ag[i].z); atomicAdd(&sg[c + 3], ag[i].w);
-    atomicAdd(&sb[c], ab[i].x); atomicAdd(&sb[c + 1], ab[i].y); atomicAdd(&sb[c + 2], ab[i].z); atomicAdd(&sb[c + 3], ab[i].w);
+    for (int i = 0; i < NV; ++i) {
+      *reinterpret_cast<float4*>(sg + wid * C + i * 128 + lane * 4) = ag[i];
+      *reinterpret_cast<float4*>(sb + wid * C + i * 128 + lane * 4) = ab[i];
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < C; i += blockDim.x) {
+      float g = sg[i], b = sb[i];
+#pragma unroll
+      for (int w = 1; w < 8; ++w) { g += sg[w * C + i]; b += sb[w * C + i]; }
+      dgamma[(long)blockIdx.x * C + i] = g; dbeta[(long)blockIdx.x * C + i] = b;
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+      const int c = i * 128 + lane * 4;
+      atomicAdd(&sg[c], ag[i].x); atomicAdd(&sg[c + 1], ag[i].y); atomicAdd(&sg[c + 2], ag[i].z); atomicAdd(&sg[c + 3], ag[i].w);
+      atomicAdd(&sb[c], ab[i].x); atomicAdd(&sb[c + 1], ab[i].y); atomicAdd(&sb[c + 2], ab[i].z); atomicAdd(&sb[c + 3], ab[i].w);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < C; i += blockDim.x) { atomicAdd(dgamma + i, sg[i]); atomicAdd(dbeta + i, sb[i]); }
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < C; i += blockDim.x) { atomicAdd(dgamma + i, sg[i]); atomicAdd(dbeta + i, sb[i]); }
 }
 
 // ---- BatchNorm1d in train mode over rows of [rows, C] (modules.py:283-348: the Postnet's BatchNorm1d sees [B, C, L], i.e. its
 // statistics run over all B*L frames of a channel, padded frames included) ----------------------------------------------------
 // stats[0..C) = mean, stats[C..2C) = biased variance; also updates running_mean / running_var (momentum, unbiased variance)
+// kOrdered (here and in bn_backward_sums): part is the double table [grid.y][2C], summed in grid.y order by ordered_sum_f64
+template <bool kOrdered>
 __global__ void bn_stats_kernel(const float* __restrict__ x, long rows, int C, float* __restrict__ part /*[2][C] double-sum as float pairs*/) {
   // grid (C/32 ceil, chunks): partial sums and sums of squares in double
   __shared__ double r1[8][33], r2[8][33];
@@ -200,8 +232,13 @@ __global__ void bn_stats_kernel(const float* __restrict__ x, long rows, int C, f
     double a = 0.0, b = 0.0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) { a += r1[i][threadIdx.x & 31]; b += r2[i][threadIdx.x & 31]; }
-    atomicAdd(reinterpret_cast<double*>(part) + c, a);
-    atomicAdd(reinterpret_cast<double*>(part) + C + c, b);
+    if constexpr (kOrdered) {
+      double* p = reinterpret_cast<double*>(part) + (long)blockIdx.y * 2 * C;
+      p[c] = a; p[C + c] = b;
+    } else {
+      atomicAdd(reinterpret_cast<double*>(part) + c, a);
+      atomicAdd(reinterpret_cast<double*>(part) + C + c, b);
+    }
   }
 }
 __global__ void bn_finalize_kernel(const double* __restrict__ part, long rows, int C, float momentum, float* __restrict__ stats,
@@ -230,6 +267,7 @@ __global__ void bn_apply_kernel(const float* __restrict__ x, const float* __rest
 }
 // backward: sums[0..C) = sum dy, sums[C..2C) = sum dy * xhat (double), then
 // dx = gamma * rstd / M * (M dy - sum dy - xhat * sum(dy xhat)); dgamma = sum dy xhat; dbeta = sum dy
+template <bool kOrdered>
 __global__ void bn_backward_sums_kernel(const float* __restrict__ x, const float* __restrict__ dy, const float* __restrict__ stats, float eps,
                                         long rows, int C, double* __restrict__ sums) {
   __shared__ double r1[8][33], r2[8][33];
@@ -248,9 +286,12 @@ __global__ void bn_backward_sums_kernel(const float* __restrict__ x, const float
     double a = 0.0, b = 0.0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) { a += r1[i][threadIdx.x & 31]; b += r2[i][threadIdx.x & 31]; }
-    atomicAdd(sums + c, a); atomicAdd(sums + C + c, b);
+    if constexpr (kOrdered) { double* p = sums + (long)blockIdx.y * 2 * C; p[c] = a; p[C + c] = b; }
+    else { atomicAdd(sums + c, a); atomicAdd(sums + C + c, b); }
   }
 }
+// kOrdered: dgamma / dbeta have one writer per channel and take a plain read-add-store
+template <bool kOrdered>
 __global__ void bn_backward_apply_kernel(const float* __restrict__ x, const float* __restrict__ dy, const float* __restrict__ stats,
                                          const float* __restrict__ gamma, float eps, long rows, int C, const double* __restrict__ sums,
                                          float* __restrict__ dx, float* __restrict__ dgamma, float* __restrict__ dbeta) {
@@ -260,7 +301,10 @@ __global__ void bn_backward_apply_kernel(const float* __restrict__ x, const floa
     const int c = (int)(i % C);
     const float rstd = 1.0f / sqrtf(stats[C + c] + eps), xh = (x[i] - stats[c]) * rstd;
     dx[i] = gamma[c] * rstd * (dy[i] - (float)sums[c] * invM - xh * (float)sums[C + c] * invM);
-    if (i < C) { atomicAdd(dgamma + c, (float)sums[C + c]); atomicAdd(dbeta + c, (float)sums[c]); }
+    if (i < C) {
+      if constexpr (kOrdered) { dgamma[c] += (float)sums[C + c]; dbeta[c] += (float)sums[c]; }
+      else { atomicAdd(dgamma + c, (float)sums[C + c]); atomicAdd(dbeta + c, (float)sums[c]); }
+    }
   }
 }
 
@@ -355,6 +399,8 @@ __global__ void attn_softmax_backward_kernel(const float* __restrict__ p, const 
 // ---- embedding / positional encoding backward (fastspeech.py:65-67, embedding.py:105-120) ---------------------------------------
 // dtable[id] += dy[row] (id != padding_idx 0: nn.Embedding(padding_idx=0) keeps that row's gradient at zero);
 // dalpha += sum dy * pe[t]
+// kOrdered: dalpha is the per-row partial table [rows] and the table is left to the ordered scatter (scatter_* below)
+template <bool kOrdered>
 __global__ void embed_backward_kernel(const int64_t* __restrict__ xs, const float* __restrict__ dy, const float* __restrict__ pe, long rows, int T,
                                       int C, int n_sym, float* __restrict__ dtable, float* __restrict__ dalpha) {
   const long row = (long)blockIdx.x * 8 + (threadIdx.x >> 5);
@@ -364,12 +410,15 @@ __global__ void embed_backward_kernel(const int64_t* __restrict__ xs, const floa
     const long id = xs ? xs[row] : 0; const int t = (int)(row % T);
     for (int c = lane; c < C; c += 32) {
       const float g = dy[row * C + c];
-      if (dtable && id > 0 && id < n_sym) atomicAdd(dtable + id * C + c, g);
+      if constexpr (!kOrdered)
+        if (dtable && id > 0 && id < n_sym) atomicAdd(dtable + id * C + c, g);
       da += g * pe[(long)t * C + c];
     }
   }
   da = warp_sum(da);
-  if (lane == 0 && da != 0.f) atomicAdd(dalpha, da);
+  if constexpr (kOrdered) {
+    if (lane == 0 && row < rows) dalpha[row] = da;
+  } else if (lane == 0 && da != 0.f) atomicAdd(dalpha, da);
 }
 // y[row, :] = x[row, :] + alpha * pe[row % T, :]   (ScaledPositionalEncoding on the decoder input, embedding.py:105-120)
 __global__ void posenc_add_kernel(const float* __restrict__ x, const float* __restrict__ pe, const float* __restrict__ alpha, long rows, int T, int C,
@@ -427,10 +476,18 @@ __global__ void rowdot_kernel(const float* __restrict__ x, const float* __restri
   s = warp_sum(s) + bias[0];
   if (lane == 0) y[row] = (lens && (row % L) >= lens[row / L]) ? 0.f : s;
 }
+// kOrdered: one shared row of dw per warp, added in warp order; dw is the partial table [grid][C] and dbias [grid] (the
+// CTA's warps in order), summed across CTAs in CTA order by the caller
+template <bool kOrdered>
 __global__ void rowdot_backward_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ dy, const int64_t* __restrict__ lens,
                                        long rows, int L, int C, float* __restrict__ dx, float* __restrict__ dw, float* __restrict__ dbias) {
-  __shared__ float sw[384];
-  for (int i = threadIdx.x; i < C; i += blockDim.x) sw[i] = 0.f;
+  constexpr int WR = kOrdered ? 8 : 1;
+  __shared__ float sw[WR * 384];
+  if constexpr (kOrdered) {
+    for (int i = threadIdx.x; i < WR * 384; i += blockDim.x) sw[i] = 0.f;
+  } else {
+    for (int i = threadIdx.x; i < C; i += blockDim.x) sw[i] = 0.f;
+  }
   __syncthreads();
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   float db = 0.f;
@@ -438,13 +495,156 @@ __global__ void rowdot_backward_kernel(const float* __restrict__ x, const float*
     const float g = (lens && (row % L) >= lens[row / L]) ? 0.f : dy[row];
     for (int c = lane; c < C; c += 32) {
       dx[row * C + c] = g * w[c];
-      atomicAdd(&sw[c], g * x[row * C + c]);
+      if constexpr (kOrdered) sw[wid * 384 + c] += g * x[row * C + c];
+      else atomicAdd(&sw[c], g * x[row * C + c]);
     }
     if (lane == 0) db += g;
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dw + i, sw[i]);
-  if (lane == 0 && db != 0.f) atomicAdd(dbias, db);
+  if constexpr (kOrdered) {
+    __shared__ float sdb[8];
+    for (int i = threadIdx.x; i < C; i += blockDim.x) {
+      float s = sw[i];
+#pragma unroll
+      for (int k = 1; k < 8; ++k) s += sw[k * 384 + i];
+      dw[(long)blockIdx.x * C + i] = s;
+    }
+    if (lane == 0) sdb[wid] = db;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float s = sdb[0];
+#pragma unroll
+      for (int k = 1; k < 8; ++k) s += sdb[k];
+      dbias[blockIdx.x] = s;
+    }
+  } else {
+    for (int i = threadIdx.x; i < C; i += blockDim.x) atomicAdd(dw + i, sw[i]);
+    if (lane == 0 && db != 0.f) atomicAdd(dbias, db);
+  }
+}
+
+// ---- ordered scatter by id (deterministic train mode): a stable counting sort of the rows by id, then per-id sums ------------
+// Rows whose id lies outside [lo, n) are dropped (embedding: lo = 1 skips the padding id 0).  Every order below depends
+// only on the ids and the shapes:
+//   scatter_hist:  per chunk of SC_ROWS rows, the count of each id (shared integer counters whose values are not read
+//                  until the block is done) -> cnt[id][chunk];
+//   scatter_scan:  one CTA: exclusive scan of cnt in (id, chunk) order -> the first sorted slot of each (id, chunk); the
+//                  first slot of each id, and the first group of each id when its rows are cut into groups of SC_GROUP;
+//   scatter_rank:  per chunk, row r goes to slot off[id][chunk] + (rows of its chunk before r with the same id), so the
+//                  sorted list holds each id's rows in ascending row order;
+//   scatter_group_sum: one CTA per (group, 128 columns) sums the group's rows in ascending order -> gpart[group][C];
+//   scatter_id_sum:    one thread per (id, column) sums that id's groups in ascending order and adds the total once.
+constexpr int SC_ROWS = 256, SC_GROUP = 256, SC_COLS = 128, SC_MAX_IDS = 8192;
+
+__global__ void scatter_hist_kernel(const int64_t* __restrict__ ids, long rows, int lo, int n, int chunks, int* __restrict__ cnt) {
+  __shared__ int h[SC_MAX_IDS];
+  for (int i = threadIdx.x; i < n; i += blockDim.x) h[i] = 0;
+  __syncthreads();
+  const long r = (long)blockIdx.x * SC_ROWS + threadIdx.x;
+  if (r < rows) {
+    const int64_t id = ids[r];
+    if (id >= lo && id < n) atomicAdd(&h[id], 1);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < n; i += blockDim.x) cnt[(long)i * chunks + blockIdx.x] = h[i];
+}
+__global__ void __launch_bounds__(1024) scatter_scan_kernel(int* __restrict__ cnt, int n, int chunks, int* __restrict__ id_start,
+                                                            int* __restrict__ grp_start) {
+  __shared__ int s[1024];
+  const long len = (long)n * chunks, per = (len + 1023) / 1024;
+  const long b = threadIdx.x * per, e = b + per < len ? b + per : len;
+  int t = 0;
+  for (long i = b; i < e; ++i) t += cnt[i];
+  s[threadIdx.x] = t;
+  __syncthreads();
+  for (int off = 1; off < 1024; off <<= 1) {
+    const int v = threadIdx.x >= off ? s[threadIdx.x - off] : 0;
+    __syncthreads();
+    s[threadIdx.x] += v;
+    __syncthreads();
+  }
+  int run = threadIdx.x ? s[threadIdx.x - 1] : 0;
+  for (long i = b; i < e; ++i) { const int c = cnt[i]; cnt[i] = run; run += c; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const int total = s[1023];
+    int g = 0;
+    for (int id = 0; id < n; ++id) {
+      const int st = cnt[(long)id * chunks], en = id + 1 < n ? cnt[(long)(id + 1) * chunks] : total;
+      id_start[id] = st; grp_start[id] = g;
+      g += (en - st + SC_GROUP - 1) / SC_GROUP;
+    }
+    id_start[n] = total; grp_start[n] = g;
+  }
+}
+__global__ void scatter_rank_kernel(const int64_t* __restrict__ ids, long rows, int lo, int n, int chunks, const int* __restrict__ off,
+                                    int* __restrict__ sorted) {
+  __shared__ int sid[SC_ROWS];
+  const long r = (long)blockIdx.x * SC_ROWS + threadIdx.x;
+  int id = -1;
+  if (r < rows) {
+    const int64_t v = ids[r];
+    if (v >= lo && v < n) id = (int)v;
+  }
+  sid[threadIdx.x] = id;
+  __syncthreads();
+  if (id < 0) return;
+  int rank = 0;
+  for (int j = 0; j < (int)threadIdx.x; ++j) rank += sid[j] == id;
+  sorted[off[(long)id * chunks + blockIdx.x] + rank] = (int)r;
+}
+// grid (max groups, ceil(C / SC_COLS)), block SC_COLS
+__global__ void scatter_group_sum_kernel(const float* __restrict__ dy, int C, int n, const int* __restrict__ id_start,
+                                         const int* __restrict__ grp_start, const int* __restrict__ sorted, float* __restrict__ gpart) {
+  __shared__ int srow[SC_GROUP];
+  __shared__ int sid;
+  const int g = blockIdx.x;
+  if (g >= grp_start[n]) return;
+  if (threadIdx.x == 0) {   // the id whose groups contain g: the last id with grp_start[id] <= g
+    int a = 0, b = n - 1;
+    while (a < b) { const int m = (a + b + 1) / 2; if (grp_start[m] <= g) a = m; else b = m - 1; }
+    sid = a;
+  }
+  __syncthreads();
+  const int id = sid;
+  const int r0 = id_start[id] + (g - grp_start[id]) * SC_GROUP, r1 = min(r0 + SC_GROUP, id_start[id + 1]);
+  for (int i = threadIdx.x; i < r1 - r0; i += blockDim.x) srow[i] = sorted[r0 + i];
+  __syncthreads();
+  const int c = blockIdx.y * SC_COLS + threadIdx.x;
+  if (c >= C) return;
+  float s = 0.f;
+#pragma unroll 8
+  for (int i = 0; i < r1 - r0; ++i) s += dy[(long)srow[i] * C + c];
+  gpart[(long)g * C + c] = s;
+}
+// out[id * ors + c * ocs] += sum of the id's groups, ascending; ids without rows are not touched
+__global__ void scatter_id_sum_kernel(const float* __restrict__ gpart, int C, int n, const int* __restrict__ grp_start, float* __restrict__ out,
+                                      long ors, long ocs) {
+  const int id = blockIdx.x, c = blockIdx.y * SC_COLS + threadIdx.x;
+  if (c >= C) return;
+  const int g0 = grp_start[id], g1 = grp_start[id + 1];
+  if (g0 == g1) return;
+  float s = 0.f;
+#pragma unroll 8
+  for (int g = g0; g < g1; ++g) s += gpart[(long)g * C + c];
+  out[id * ors + c * ocs] += s;
+}
+
+// K sums out[k] = sum_{i < n} part[k * sk + i * si] in double: thread t takes i = t, t + 256, ... in order, then a fixed
+// halving tree over the 256 threads; one CTA per sum
+__global__ void __launch_bounds__(256) ordered_sum_f64_kernel(const double* __restrict__ part, long n, long si, long sk, double* __restrict__ out) {
+  __shared__ double s[256];
+  const long k = blockIdx.x;
+  double a = 0.0;
+  for (long i = threadIdx.x; i < n; i += 256) a += part[k * sk + i * si];
+  s[threadIdx.x] = a;
+  __syncthreads();
+#pragma unroll
+  for (int h = 128; h > 0; h >>= 1) {
+    if ((int)threadIdx.x < h) s[threadIdx.x] += s[threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) out[k] = s[0];
 }
 
 // ---- loss backward (fastspeech.py:277-324 with use_masking): upstream g = dL/dloss ----------------------------------------------
@@ -511,7 +711,285 @@ int conv_dgrad(const char* who, int math_mode, const float* dy, int B, int L, in
   return vweight_gemm(math_mode, pw, dy, B, L, ACT_NONE, nullptr, dx, st);
 }
 
+// ---- launch geometry shared by the default and the ordered entries ------------------------------------------------------------
+long colsum_chunks(long rows) { return rows / 512 + 1 > 64 ? 64 : rows / 512 + 1; }
+int warp_row_ctas(long rows) { return (int)(rows / 8 + 1 > 132 * 4 ? 132 * 4 : rows / 8 + 1); }   // layernorm / rowdot backward
+long bn_chunks(long rows) { return rows / 256 + 1 < 128 ? rows / 256 + 1 : 128; }
+int wgrad_chunks(long M, int tiles) {
+  int chunks = (132 * 4 + tiles - 1) / tiles;
+  const long max_chunks = (M + 255) / 256;
+  if (chunks > max_chunks) chunks = (int)max_chunks;
+  if (chunks < 1) chunks = 1;
+  return chunks;
+}
+int wgrad_tiles(int N, int K, int taps) { return ((N + WG_T - 1) / WG_T) * ((K + WG_T - 1) / WG_T) * taps; }
+
+// kOrdered: part [colsum_chunks(rows)][C] floats
+template <bool kOrdered>
+int colsum_impl(const float* x, long rows, int C, float* out, float* part, cudaStream_t st) {
+  if (rows == 0) return FS2_OK;
+  dim3 grid((C + 31) / 32, (unsigned)colsum_chunks(rows));
+  colsum_kernel<kOrdered><<<grid, 256, 0, st>>>(x, rows, C, kOrdered ? part : out);
+  FS2_LAUNCH_CHECK();
+  if (kOrdered) return ordered_reduce(part, (int)grid.y, 1, 1, C, out, st);
+  return FS2_OK;
+}
+
+// Workspace carves of the ordered entries (Bump over NULL counts the bytes; every carve 256-byte aligned)
+struct WgradDetWs { float* part; float* colsum; };
+WgradDetWs wgrad_det_ws(Bump& w, int B, int L, int N, int K, int taps, bool bias) {
+  const long M = (long)B * L;
+  const int chunks = wgrad_chunks(M, wgrad_tiles(N, K, taps));
+  WgradDetWs r;
+  r.part = chunks > 1 ? w.floats((size_t)chunks * taps * N * K) : nullptr;
+  r.colsum = bias ? w.floats((size_t)colsum_chunks(M) * N) : nullptr;
+  return r;
+}
+struct RowsDetWs { float* a; float* b; float* colsum; };   // layernorm: a = dgamma, b = dbeta partials; rowdot: a = dw, b = dbias
+RowsDetWs layernorm_det_ws(Bump& w, long rows, int C) {
+  const int ctas = warp_row_ctas(rows);
+  RowsDetWs r;
+  r.a = w.floats((size_t)ctas * C); r.b = w.floats((size_t)ctas * C); r.colsum = w.floats((size_t)colsum_chunks(ctas) * C);
+  return r;
+}
+RowsDetWs rowdot_det_ws(Bump& w, long rows, int C) {
+  const int ctas = warp_row_ctas(rows);
+  RowsDetWs r;
+  r.a = w.floats((size_t)ctas * C); r.b = w.floats((size_t)ctas); r.colsum = w.floats((size_t)colsum_chunks(ctas) * C);
+  return r;
+}
+struct BnDetWs { double* part; double* sums; };
+BnDetWs bn_det_ws(Bump& w, long rows, int C) {
+  BnDetWs r;
+  r.part = w.doubles((size_t)bn_chunks(rows) * 2 * C); r.sums = w.doubles((size_t)2 * C);
+  return r;
+}
+struct ScatterWs { int* cnt; int* id_start; int* grp_start; int* sorted; float* gpart; };
+long scatter_chunks(long rows) { return (rows + SC_ROWS - 1) / SC_ROWS; }
+long scatter_max_groups(long rows, int n) { return (rows + SC_GROUP - 1) / SC_GROUP + n; }
+ScatterWs scatter_ws(Bump& w, long rows, int C, int n) {
+  ScatterWs r;
+  const long chunks = scatter_chunks(rows);
+  r.cnt = (int*)w.bytes((size_t)n * chunks * sizeof(int));
+  r.id_start = (int*)w.bytes((size_t)(n + 1) * sizeof(int));
+  r.grp_start = (int*)w.bytes((size_t)(n + 1) * sizeof(int));
+  r.sorted = (int*)w.bytes((size_t)rows * sizeof(int));
+  r.gpart = w.floats((size_t)scatter_max_groups(rows, n) * C);
+  return r;
+}
+struct EmbedDetWs { float* da; float* colsum; ScatterWs sc; };
+EmbedDetWs embed_det_ws(Bump& w, long rows, int C, int n_sym, bool table) {
+  EmbedDetWs r;
+  r.da = w.floats((size_t)rows); r.colsum = w.floats((size_t)colsum_chunks(rows));
+  r.sc = table ? scatter_ws(w, rows, C, n_sym) : ScatterWs{};
+  return r;
+}
+struct OnehotDetWs { ScatterWs sc; float* colsum; };
+OnehotDetWs onehot_det_ws(Bump& w, long rows, int C, int n_bins, bool bias) {
+  OnehotDetWs r;
+  r.sc = scatter_ws(w, rows, C, n_bins);
+  r.colsum = bias ? w.floats((size_t)colsum_chunks(rows) * C) : nullptr;
+  return r;
+}
+struct LossDetWs { double* acc; double* mel; double* seq; long n_mel, n_seq; };
+LossDetWs loss_det_ws(Bump& w, int B, int T, int L, int odim) {
+  LossDetWs r;
+  r.n_mel = (long)grid_for((long)L * odim / 4, 256, 32) * B;
+  r.n_seq = (long)grid_for(L > T ? L : T, 256, 16) * B;
+  r.acc = w.doubles(8); r.mel = w.doubles((size_t)2 * r.n_mel); r.seq = w.doubles((size_t)3 * r.n_seq);
+  return r;
+}
+
+// out[id * ors + c * ocs] += sum of dy[r, c] over the rows r with ids[r] == id in [lo, n), in ascending row order per id
+int scatter_rows(const int64_t* ids, const float* dy, long rows, int C, int lo, int n, float* out, long ors, long ocs, const ScatterWs& w,
+                 cudaStream_t st) {
+  if (rows == 0) return FS2_OK;
+  const long chunks = scatter_chunks(rows);
+  scatter_hist_kernel<<<(unsigned)chunks, SC_ROWS, 0, st>>>(ids, rows, lo, n, (int)chunks, w.cnt);
+  FS2_LAUNCH_CHECK();
+  scatter_scan_kernel<<<1, 1024, 0, st>>>(w.cnt, n, (int)chunks, w.id_start, w.grp_start);
+  FS2_LAUNCH_CHECK();
+  scatter_rank_kernel<<<(unsigned)chunks, SC_ROWS, 0, st>>>(ids, rows, lo, n, (int)chunks, w.cnt, w.sorted);
+  FS2_LAUNCH_CHECK();
+  const unsigned cb = (C + SC_COLS - 1) / SC_COLS;
+  scatter_group_sum_kernel<<<dim3((unsigned)scatter_max_groups(rows, n), cb), SC_COLS, 0, st>>>(dy, C, n, w.id_start, w.grp_start, w.sorted, w.gpart);
+  FS2_LAUNCH_CHECK();
+  scatter_id_sum_kernel<<<dim3(n, cb), SC_COLS, 0, st>>>(w.gpart, C, n, w.grp_start, out, ors, ocs);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+template <bool kOrdered>
+int conv_wgrad_impl(const float* dy, const float* x, int B, int L, int N, int K, int taps, float* dw, float* dbias, const WgradDetWs& w,
+                    cudaStream_t st) {
+  const long M = (long)B * L;
+  if (M == 0) return FS2_OK;
+  const int chunks = wgrad_chunks(M, wgrad_tiles(N, K, taps));
+  dim3 grid((N + WG_T - 1) / WG_T, (K + WG_T - 1) / WG_T, taps * chunks);
+  const bool staged = kOrdered && chunks > 1;
+  wgrad_kernel<kOrdered><<<grid, 256, 0, st>>>(dy, N, x, K, B, L, N, K, taps, chunks, staged ? w.part : dw);
+  FS2_LAUNCH_CHECK();
+  int rc;
+  if (staged && (rc = ordered_reduce(w.part, chunks, taps, N, K, dw, st))) return rc;
+  if (dbias) return colsum_impl<kOrdered>(dy, M, N, dbias, w.colsum, st);
+  return FS2_OK;
+}
+
+template <bool kOrdered>
+int layernorm_backward_impl(const float* x, const float* dy, const float* gamma, float eps, long rows, int C, float* dx, float* dgamma,
+                            float* dbeta, const RowsDetWs& w, cudaStream_t st) {
+  if (rows == 0) return FS2_OK;
+  const int grid = warp_row_ctas(rows);
+  float* pg = kOrdered ? w.a : dgamma;
+  float* pb = kOrdered ? w.b : dbeta;
+  if (C == 256) layernorm_backward_kernel<2, kOrdered><<<grid, 256, 0, st>>>(x, dy, gamma, eps, rows, dx, pg, pb);
+  else if (C == 384) layernorm_backward_kernel<3, kOrdered><<<grid, 256, 0, st>>>(x, dy, gamma, eps, rows, dx, pg, pb);
+  else { set_error("fs2_layernorm_backward: C=%d unsupported (256 or 384)", C); return FS2_ERR_INVALID; }
+  FS2_LAUNCH_CHECK();
+  int rc;
+  if (kOrdered && ((rc = colsum_impl<true>(w.a, grid, C, dgamma, w.colsum, st)) || (rc = colsum_impl<true>(w.b, grid, C, dbeta, w.colsum, st))))
+    return rc;
+  return FS2_OK;
+}
+
+template <bool kOrdered>
+int batchnorm_train_impl(const float* x, long rows, int C, const float* gamma, const float* beta, float eps, float momentum, int act,
+                         float* running_mean, float* running_var, float* stats, float* y, void* scratch, const BnDetWs& w, cudaStream_t st) {
+  if (!kOrdered) FS2_CUDA_CHECK(cudaMemsetAsync(scratch, 0, (size_t)2 * C * sizeof(double), st));
+  dim3 grid((C + 31) / 32, (unsigned)(rows / 256 + 1 > 128 ? 128 : rows / 256 + 1));
+  bn_stats_kernel<kOrdered><<<grid, 256, 0, st>>>(x, rows, C, kOrdered ? reinterpret_cast<float*>(w.part) : reinterpret_cast<float*>(scratch));
+  FS2_LAUNCH_CHECK();
+  const double* sums = kOrdered ? w.sums : reinterpret_cast<const double*>(scratch);
+  if (kOrdered) {
+    ordered_sum_f64_kernel<<<2 * C, 256, 0, st>>>(w.part, grid.y, 2L * C, 1, w.sums);
+    FS2_LAUNCH_CHECK();
+  }
+  bn_finalize_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, rows, C, momentum, stats, running_mean, running_var);
+  FS2_LAUNCH_CHECK();
+  bn_apply_kernel<<<grid_for(rows * C, 256), 256, 0, st>>>(x, stats, gamma, beta, eps, rows, C, act, y);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+template <bool kOrdered>
+int batchnorm_backward_impl(const float* x, const float* dy, const float* stats, const float* gamma, float eps, long rows, int C, float* dx,
+                            float* dgamma, float* dbeta, void* scratch, const BnDetWs& w, cudaStream_t st) {
+  if (!kOrdered) FS2_CUDA_CHECK(cudaMemsetAsync(scratch, 0, (size_t)2 * C * sizeof(double), st));
+  dim3 grid((C + 31) / 32, (unsigned)(rows / 256 + 1 > 128 ? 128 : rows / 256 + 1));
+  bn_backward_sums_kernel<kOrdered><<<grid, 256, 0, st>>>(x, dy, stats, eps, rows, C, kOrdered ? w.part : reinterpret_cast<double*>(scratch));
+  FS2_LAUNCH_CHECK();
+  const double* sums = kOrdered ? w.sums : reinterpret_cast<const double*>(scratch);
+  if (kOrdered) {
+    ordered_sum_f64_kernel<<<2 * C, 256, 0, st>>>(w.part, grid.y, 2L * C, 1, w.sums);
+    FS2_LAUNCH_CHECK();
+  }
+  bn_backward_apply_kernel<kOrdered><<<grid_for(rows * C, 256), 256, 0, st>>>(x, dy, stats, gamma, eps, rows, C, sums, dx, dgamma, dbeta);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+template <bool kOrdered>
+int rowdot_backward_impl(const float* x, const float* w, const float* dy, const int64_t* lens, long rows, int L, int C, float* dx, float* dw,
+                         float* dbias, const RowsDetWs& ws, cudaStream_t st) {
+  if (rows == 0) return FS2_OK;
+  const int grid = warp_row_ctas(rows);
+  rowdot_backward_kernel<kOrdered><<<grid, 256, 0, st>>>(x, w, dy, lens, rows, L, C, dx, kOrdered ? ws.a : dw, kOrdered ? ws.b : dbias);
+  FS2_LAUNCH_CHECK();
+  int rc;
+  if (kOrdered && ((rc = colsum_impl<true>(ws.a, grid, C, dw, ws.colsum, st)) || (rc = colsum_impl<true>(ws.b, grid, 1, dbias, ws.colsum, st))))
+    return rc;
+  return FS2_OK;
+}
+
 }  // namespace
+
+int ordered_sum_f64(const double* part, long n, long si, long sk, int K, double* out, cudaStream_t st) {
+  if (K == 0) return FS2_OK;
+  ordered_sum_f64_kernel<<<K, 256, 0, st>>>(part, n, si, sk, out);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+// ---- the ordered entries' bodies (the C entries and their argument checks are in train_det.cu); `*_det_bytes` is the
+// workspace the body carves, every carve 256-byte aligned from the start of ws --------------------------------------------------
+template <class F>
+size_t counted(F carve) { Bump w(nullptr, 0); carve(w); return w.off; }
+
+size_t colsum_det_bytes(long rows, int C) { return rows == 0 ? 0 : counted([&](Bump& w) { w.floats((size_t)colsum_chunks(rows) * C); }); }
+int colsum_det(const float* x, long rows, int C, float* out, void* ws, cudaStream_t st) {
+  return colsum_impl<true>(x, rows, C, out, reinterpret_cast<float*>(ws), st);
+}
+size_t conv_wgrad_det_bytes(int B, int L, int N, int K, int taps, bool bias) {
+  return (long)B * L == 0 ? 0 : counted([&](Bump& w) { wgrad_det_ws(w, B, L, N, K, taps, bias); });
+}
+int conv_wgrad_det(const float* dy, const float* x, int B, int L, int N, int K, int taps, float* dw, float* dbias, void* ws, cudaStream_t st) {
+  Bump w(ws, 0);
+  return conv_wgrad_impl<true>(dy, x, B, L, N, K, taps, dw, dbias, wgrad_det_ws(w, B, L, N, K, taps, dbias != nullptr), st);
+}
+size_t layernorm_backward_det_bytes(long rows, int C) { return rows == 0 ? 0 : counted([&](Bump& w) { layernorm_det_ws(w, rows, C); }); }
+int layernorm_backward_det(const float* x, const float* dy, const float* gamma, float eps, long rows, int C, float* dx, float* dgamma,
+                           float* dbeta, void* ws, cudaStream_t st) {
+  Bump w(ws, 0);
+  return layernorm_backward_impl<true>(x, dy, gamma, eps, rows, C, dx, dgamma, dbeta, layernorm_det_ws(w, rows, C), st);
+}
+size_t batchnorm_det_bytes(long rows, int C) { return counted([&](Bump& w) { bn_det_ws(w, rows, C); }); }
+int batchnorm_train_det(const float* x, long rows, int C, const float* gamma, const float* beta, float eps, float momentum, int act,
+                        float* running_mean, float* running_var, float* stats, float* y, void* ws, cudaStream_t st) {
+  Bump w(ws, 0);
+  return batchnorm_train_impl<true>(x, rows, C, gamma, beta, eps, momentum, act, running_mean, running_var, stats, y, nullptr,
+                                    bn_det_ws(w, rows, C), st);
+}
+int batchnorm_backward_det(const float* x, const float* dy, const float* stats, const float* gamma, float eps, long rows, int C, float* dx,
+                           float* dgamma, float* dbeta, void* ws, cudaStream_t st) {
+  Bump w(ws, 0);
+  return batchnorm_backward_impl<true>(x, dy, stats, gamma, eps, rows, C, dx, dgamma, dbeta, nullptr, bn_det_ws(w, rows, C), st);
+}
+size_t embed_backward_det_bytes(long rows, int C, int n_sym, bool table) {
+  return rows == 0 ? 0 : counted([&](Bump& w) { embed_det_ws(w, rows, C, n_sym, table); });
+}
+int embed_backward_det(const int64_t* xs, const float* dy, const float* pe, int B, int T, int C, int n_sym, float* dtable, float* dalpha,
+                       void* ws, cudaStream_t st) {
+  const long rows = (long)B * T;
+  if (rows == 0) return FS2_OK;
+  Bump w(ws, 0);
+  const EmbedDetWs r = embed_det_ws(w, rows, C, n_sym, dtable != nullptr);
+  embed_backward_kernel<true><<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(xs, dy, pe, rows, T, C, n_sym, nullptr, r.da);
+  FS2_LAUNCH_CHECK();
+  int rc = colsum_impl<true>(r.da, rows, 1, dalpha, r.colsum, st);
+  if (rc || !dtable) return rc;
+  return scatter_rows(xs, dy, rows, C, 1, n_sym, dtable, C, 1, r.sc, st);
+}
+size_t onehot_linear_backward_det_bytes(long rows, int C, int n_bins, bool bias) {
+  return rows == 0 ? 0 : counted([&](Bump& w) { onehot_det_ws(w, rows, C, n_bins, bias); });
+}
+int onehot_linear_backward_det(const int64_t* ids, const float* dy, long rows, int C, int n_bins, float* dW, float* dbias, void* ws,
+                               cudaStream_t st) {
+  if (rows == 0) return FS2_OK;
+  Bump w(ws, 0);
+  const OnehotDetWs r = onehot_det_ws(w, rows, C, n_bins, dbias != nullptr);
+  int rc = scatter_rows(ids, dy, rows, C, 0, n_bins, dW, 1, n_bins, r.sc, st);
+  if (rc || !dbias) return rc;
+  return colsum_impl<true>(dy, rows, C, dbias, r.colsum, st);
+}
+size_t rowdot_backward_det_bytes(long rows, int C) { return rows == 0 ? 0 : counted([&](Bump& w) { rowdot_det_ws(w, rows, C); }); }
+int rowdot_backward_det(const float* x, const float* w, const float* dy, const int64_t* lens, long rows, int L, int C, float* dx, float* dw,
+                        float* dbias, void* ws, cudaStream_t st) {
+  Bump b(ws, 0);
+  return rowdot_backward_impl<true>(x, w, dy, lens, rows, L, C, dx, dw, dbias, rowdot_det_ws(b, rows, C), st);
+}
+int scatter_max_ids() { return SC_MAX_IDS; }
+
+size_t loss_det_ws_bytes(int B, int T, int L, int odim) {
+  Bump w(nullptr, 0);
+  loss_det_ws(w, B, T, L, odim);
+  return w.off;
+}
+int loss_det_carve(void* ws, int B, int T, int L, int odim, double** acc, double** mel, long* n_mel, double** seq, long* n_seq) {
+  Bump w(ws, 0);
+  const LossDetWs r = loss_det_ws(w, B, T, L, odim);
+  *acc = r.acc; *mel = r.mel; *n_mel = r.n_mel; *seq = r.seq; *n_seq = r.n_seq;
+  return FS2_OK;
+}
+
 }  // namespace fs2
 
 using namespace fs2;
@@ -555,11 +1033,7 @@ int fs2_add(const float* a, const float* b, float* y, int64_t n, void* stream) {
 }
 int fs2_colsum(const float* x, int64_t rows, int C, float* out, void* stream) {
   FS2_REQUIRE(x && out && C > 0, "fs2_colsum: bad argument");
-  if (rows == 0) return FS2_OK;
-  dim3 grid((C + 31) / 32, (unsigned)(rows / 512 + 1 > 64 ? 64 : rows / 512 + 1));
-  colsum_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, rows, C, out);
-  FS2_LAUNCH_CHECK();
-  return FS2_OK;
+  return colsum_impl<false>(x, rows, C, out, nullptr, (cudaStream_t)stream);
 }
 /* Conv1d / Linear in the reference's weight layout w [N][K][taps]:
  *   forward   out = act(conv(x, w) + bias) (+ resid)        (packs w into the kernel layout, then the fp32 tap-GEMM)
@@ -590,57 +1064,24 @@ int fs2_conv_dgrad_ex(const float* dy, int B, int L, int N, const float* w, int 
 int fs2_conv_wgrad(const float* dy, const float* x, int B, int L, int N, int K, int taps, float* dw, float* dbias, void* stream) {
   FS2_REQUIRE(dy && x && dw, "fs2_conv_wgrad: null argument");
   FS2_REQUIRE(B >= 0 && L >= 0 && N > 0 && K > 0 && taps > 0 && (taps & 1) == 1, "fs2_conv_wgrad: need B, L >= 0, N, K > 0 and odd taps");
-  cudaStream_t st = (cudaStream_t)stream;
-  const long M = (long)B * L;
-  if (M == 0) return FS2_OK;
-  const int tiles = ((N + WG_T - 1) / WG_T) * ((K + WG_T - 1) / WG_T) * taps;
-  int chunks = (132 * 4 + tiles - 1) / tiles;
-  const long max_chunks = (M + 255) / 256;
-  if (chunks > max_chunks) chunks = (int)max_chunks;
-  if (chunks < 1) chunks = 1;
-  dim3 grid((N + WG_T - 1) / WG_T, (K + WG_T - 1) / WG_T, taps * chunks);
-  wgrad_kernel<<<grid, 256, 0, st>>>(dy, N, x, K, B, L, N, K, taps, chunks, dw);
-  FS2_LAUNCH_CHECK();
-  if (dbias) return fs2_colsum(dy, M, N, dbias, stream);
-  return FS2_OK;
+  return conv_wgrad_impl<false>(dy, x, B, L, N, K, taps, dw, dbias, WgradDetWs{}, (cudaStream_t)stream);
 }
 int fs2_layernorm_backward(const float* x, const float* dy, const float* gamma, float eps, int64_t rows, int C, float* dx, float* dgamma,
                            float* dbeta, void* stream) {
   FS2_REQUIRE(x && dy && gamma && dx && dgamma && dbeta, "fs2_layernorm_backward: null argument");
-  if (rows == 0) return FS2_OK;
-  const int grid = (int)(rows / 8 + 1 > 132 * 4 ? 132 * 4 : rows / 8 + 1);
-  if (C == 256) layernorm_backward_kernel<2><<<grid, 256, 0, (cudaStream_t)stream>>>(x, dy, gamma, eps, rows, dx, dgamma, dbeta);
-  else if (C == 384) layernorm_backward_kernel<3><<<grid, 256, 0, (cudaStream_t)stream>>>(x, dy, gamma, eps, rows, dx, dgamma, dbeta);
-  else { set_error("fs2_layernorm_backward: C=%d unsupported (256 or 384)", C); return FS2_ERR_INVALID; }
-  FS2_LAUNCH_CHECK();
-  return FS2_OK;
+  return layernorm_backward_impl<false>(x, dy, gamma, eps, rows, C, dx, dgamma, dbeta, RowsDetWs{}, (cudaStream_t)stream);
 }
 /* BatchNorm1d, training: stats [2*C] out (mean, biased var), running stats updated in place; scratch >= 4*C doubles, zeroed here */
 int fs2_batchnorm_train(const float* x, int64_t rows, int C, const float* gamma, const float* beta, float eps, float momentum, int act,
                         float* running_mean, float* running_var, float* stats, float* y, void* scratch, void* stream) {
   FS2_REQUIRE(x && gamma && beta && stats && y && scratch && rows > 0, "fs2_batchnorm_train: bad argument");
-  cudaStream_t st = (cudaStream_t)stream;
-  FS2_CUDA_CHECK(cudaMemsetAsync(scratch, 0, (size_t)2 * C * sizeof(double), st));
-  dim3 grid((C + 31) / 32, (unsigned)(rows / 256 + 1 > 128 ? 128 : rows / 256 + 1));
-  bn_stats_kernel<<<grid, 256, 0, st>>>(x, rows, C, reinterpret_cast<float*>(scratch));
-  FS2_LAUNCH_CHECK();
-  bn_finalize_kernel<<<(C + 127) / 128, 128, 0, st>>>(reinterpret_cast<const double*>(scratch), rows, C, momentum, stats, running_mean, running_var);
-  FS2_LAUNCH_CHECK();
-  bn_apply_kernel<<<grid_for(rows * C, 256), 256, 0, st>>>(x, stats, gamma, beta, eps, rows, C, act, y);
-  FS2_LAUNCH_CHECK();
-  return FS2_OK;
+  return batchnorm_train_impl<false>(x, rows, C, gamma, beta, eps, momentum, act, running_mean, running_var, stats, y, scratch, BnDetWs{},
+                                     (cudaStream_t)stream);
 }
 int fs2_batchnorm_backward(const float* x, const float* dy, const float* stats, const float* gamma, float eps, int64_t rows, int C, float* dx,
                            float* dgamma, float* dbeta, void* scratch, void* stream) {
   FS2_REQUIRE(x && dy && stats && gamma && dx && dgamma && dbeta && scratch && rows > 0, "fs2_batchnorm_backward: bad argument");
-  cudaStream_t st = (cudaStream_t)stream;
-  FS2_CUDA_CHECK(cudaMemsetAsync(scratch, 0, (size_t)2 * C * sizeof(double), st));
-  dim3 grid((C + 31) / 32, (unsigned)(rows / 256 + 1 > 128 ? 128 : rows / 256 + 1));
-  bn_backward_sums_kernel<<<grid, 256, 0, st>>>(x, dy, stats, eps, rows, C, reinterpret_cast<double*>(scratch));
-  FS2_LAUNCH_CHECK();
-  bn_backward_apply_kernel<<<grid_for(rows * C, 256), 256, 0, st>>>(x, dy, stats, gamma, eps, rows, C, reinterpret_cast<const double*>(scratch), dx, dgamma, dbeta);
-  FS2_LAUNCH_CHECK();
-  return FS2_OK;
+  return batchnorm_backward_impl<false>(x, dy, stats, gamma, eps, rows, C, dx, dgamma, dbeta, scratch, BnDetWs{}, (cudaStream_t)stream);
 }
 /* strided batched fp32 GEMM over z = (b, h): C = alpha * A . B with every operand given by (pointer, batch stride, head stride,
  * row stride, column stride) in floats */
@@ -674,7 +1115,7 @@ int fs2_embed_backward(const int64_t* xs, const float* dy, const float* pe, int 
   FS2_REQUIRE(dy && pe && dalpha && (xs || !dtable), "fs2_embed_backward: null argument");
   const long rows = (long)B * T;
   if (rows == 0) return FS2_OK;
-  embed_backward_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>(xs, dy, pe, rows, T, C, n_sym, dtable, dalpha);
+  embed_backward_kernel<false><<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>(xs, dy, pe, rows, T, C, n_sym, dtable, dalpha);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
@@ -725,11 +1166,7 @@ int fs2_rowdot(const float* x, const float* w, const float* bias, const int64_t*
 int fs2_rowdot_backward(const float* x, const float* w, const float* dy, const int64_t* lens, int64_t rows, int L, int C, float* dx, float* dw,
                         float* dbias, void* stream) {
   FS2_REQUIRE(x && w && dy && dx && dw && dbias && L > 0 && C <= 384, "fs2_rowdot_backward: bad argument");
-  if (rows == 0) return FS2_OK;
-  const int grid = (int)(rows / 8 + 1 > 132 * 4 ? 132 * 4 : rows / 8 + 1);
-  rowdot_backward_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, w, dy, lens, rows, L, C, dx, dw, dbias);
-  FS2_LAUNCH_CHECK();
-  return FS2_OK;
+  return rowdot_backward_impl<false>(x, w, dy, lens, rows, L, C, dx, dw, dbias, RowsDetWs{}, (cudaStream_t)stream);
 }
 int fs2_loss_backward(const float* before, const float* after, const float* ys, int ld_ys_time, const float* d_out, const void* ds, int ds_dtype,
                       const float* e_out, const float* p_out, const float* es, const float* ps, const int64_t* ilens, const int64_t* olens,

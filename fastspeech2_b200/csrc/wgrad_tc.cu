@@ -252,6 +252,13 @@ int wgrad_plan(int B, int L, int N, int K, int taps, WgradPlan* pl, const char* 
 }
 
 }  // namespace
+
+int ordered_reduce(const float* part, int splits, int taps, int N, int K, float* dw, cudaStream_t st) {
+  wgrad_reduce_kernel<<<grid_for((long)taps * N * K, 256), 256, 0, st>>>(part, splits, taps, N, K, dw);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
 }  // namespace fs2
 
 using namespace fs2;
@@ -303,8 +310,7 @@ int fs2_conv_wgrad_tc(const float* dy, const float* x, int B, int L, int N, int 
   const int grid = pl.units < sm_count_current() ? pl.units : sm_count_current();
   wgrad_tc_kernel<<<grid, WT_THREADS, WT_SMEM, st>>>(mdy, mx[0], mx[1], mx[2], mx[3], p);
   FS2_LAUNCH_CHECK();
-  wgrad_reduce_kernel<<<grid_for((long)taps * N * K, 256), 256, 0, st>>>(part, pl.splits, taps, N, K, dw);
-  FS2_LAUNCH_CHECK();
+  if ((rc = ordered_reduce(part, pl.splits, taps, N, K, dw, st))) return rc;
   if (dbias) return fs2_colsum(dy, (int64_t)B * L, N, dbias, stream);
   return FS2_OK;
 }

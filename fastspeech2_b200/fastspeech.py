@@ -31,6 +31,12 @@ the step stay fp32 (DESIGN.md §10).
 Train attention (`train_attention=` / FS2_TRAIN_ATTENTION): "materialized" (default) runs the train step's attention as
 fp32 batched products over a stored [B, heads, L, L] score tensor; "flash" (needs train_precision="tf32") runs it on
 fused tf32 tensor-core kernels that store only the row log-sum-exp (DESIGN.md §13).
+
+Deterministic training (`train_deterministic=` / FS2_TRAIN_DETERMINISTIC=1): every gradient, the loss and report, the
+BatchNorm running statistics and so the optimizer state are summed in a fixed order, so the same weights, batches and
+`torch.manual_seed` give the same bits on every run (DESIGN.md §26).  Off by default: its sums round differently from
+the default path's.  A step also runs this way whenever `torch.are_deterministic_algorithms_enabled()`.  It covers the
+eval-mode `forward` loss as well.
 """
 from __future__ import annotations
 
@@ -74,6 +80,22 @@ def resolve_train_attention(train_attention: Optional[str] = None, train_precisi
         raise ValueError(f"train_attention='flash' needs train_precision='tf32', got {train_precision!r}: the fused attention's products "
                          "are 1xTF32 on the tensor cores, which the fp32 train mode does not allow (it has no fp32-class flash kernel)")
     return mode
+
+
+def resolve_train_deterministic(train_deterministic: Optional[bool] = None) -> bool:
+    """The model's deterministic train mode: the argument, else FS2_TRAIN_DETERMINISTIC ("1" / "true" / "yes" / "on" turn it
+    on; "", "0", "false", "no", "off" leave it off).  torch.use_deterministic_algorithms(True) turns a step deterministic
+    regardless (train.deterministic_step), so False here never overrides torch's flag."""
+    if train_deterministic is not None:
+        if not isinstance(train_deterministic, bool):
+            raise ValueError(f"train_deterministic must be a bool or None, got {train_deterministic!r}")
+        return train_deterministic
+    v = os.environ.get("FS2_TRAIN_DETERMINISTIC", "").strip().lower()
+    if v in ("1", "true", "yes", "on"):
+        return True
+    if v in ("", "0", "false", "no", "off"):
+        return False
+    raise ValueError(f"FS2_TRAIN_DETERMINISTIC must be 1 or 0 (true / false), got {v!r}")
 
 
 def _get(node: Any, key: str, default: Any = None) -> Any:
@@ -351,7 +373,7 @@ class FeedForwardTransformer(nn.Module):
 
     @classmethod
     def from_checkpoint(cls, checkpoint, hp=None, precision: Optional[str] = None, device=None, train_precision: Optional[str] = None,
-                        train_attention: Optional[str] = None):
+                        train_attention: Optional[str] = None, train_deterministic: Optional[bool] = None):
         """Build the model from a reference checkpoint: a path or the loaded dict `{"model": state_dict, "optim": ..,
         "step": .., "hp_str": .., "githash": ..}` that train_fastspeech.py:235-244 writes (or a bare state_dict, the
         `--old_model` case of inference.py:161-163).  `hp` defaults to the checkpoint's own `hp_str` like
@@ -373,13 +395,13 @@ class FeedForwardTransformer(nn.Module):
         if n_hp and n_hp != n_spk:
             raise ValueError(f"hp.model.n_speakers = {n_hp} but the checkpoint's speaker table has {n_spk} rows")
         model = cls(idim, odim, hp, precision=precision, train_precision=train_precision, train_attention=train_attention,
-                    n_speakers=n_spk)
+                    n_speakers=n_spk, train_deterministic=train_deterministic)
         model.load_state_dict(sd, strict="model" in checkpoint)
         model.eval()
         return model.to(device) if device is not None else model
 
     def __init__(self, idim: int, odim: int, hp: Dict, precision: Optional[str] = None, train_precision: Optional[str] = None,
-                 train_attention: Optional[str] = None, n_speakers: Optional[int] = None):
+                 train_attention: Optional[str] = None, n_speakers: Optional[int] = None, train_deterministic: Optional[bool] = None):
         super().__init__()
         dims = dims_from_hp(idim, odim, hp)
         self.dims = dims
@@ -395,6 +417,7 @@ class FeedForwardTransformer(nn.Module):
             raise ValueError(f"precision must be one of {sorted(_lib.MATH_MODES)}")
         self.train_precision = resolve_train_precision(train_precision)
         self.train_attention = resolve_train_attention(train_attention, self.train_precision)
+        self.train_deterministic = resolve_train_deterministic(train_deterministic)
         if self.train_attention == "flash":
             for name, width in (("adim", dims.adim), ("ddim", dims.ddim)):
                 if width % dims.aheads or width // dims.aheads not in FLASH_HEAD_WIDTHS:
@@ -747,8 +770,8 @@ class FeedForwardTransformer(nn.Module):
         if xs.is_cuda and torch.cuda.current_device() != (xs.device.index or 0):
             with torch.cuda.device(xs.device):
                 return self.forward(xs, ilens, ys, olens, ds, es, ps, speakers)
+        from .train import deterministic_step, masked_losses, train_forward
         if self.training:
-            from .train import train_forward
             return train_forward(self, xs, ilens, ys, olens, ds, es, ps, masks=self.dropout_masks, speakers=speakers)
         self._ready(xs)
         lib = _lib.load()
@@ -768,12 +791,15 @@ class FeedForwardTransformer(nn.Module):
         ys_c = ys.to(dtype=torch.float32, device=dev).contiguous()
         es_c, ps_c = es_t.to(torch.float32).contiguous(), ps_t.to(torch.float32).contiguous()
         ds_c = ds_t.contiguous()
-        out7 = torch.empty((7,), dtype=torch.float32, device=dev)
-        scratch = torch.empty((16,), dtype=torch.float64, device=dev)
-        _lib.check(lib.fs2_masked_losses(_lib.ptr(before), _lib.ptr(after), _lib.ptr(ys_c), int(ys_c.shape[1]), _lib.ptr(d_outs),
-                                         _lib.ptr(ds_c), _lib.dur_dtype(ds_c), _lib.ptr(e_outs), _lib.ptr(p_outs), _lib.ptr(es_c),
-                                         _lib.ptr(ps_c), _lib.ptr(ilens.contiguous()), _lib.ptr(olens.contiguous()), B, T, L,
-                                         self.odim, _lib.ptr(out7), _lib.ptr(scratch), _lib.stream_ptr(dev)), "fs2_masked_losses")
+        if deterministic_step(self):
+            out7 = masked_losses(before, after, d_outs, e_outs, p_outs, ys_c, ds_c, es_c, ps_c, ilens.contiguous(), olens.contiguous(), True)
+        else:
+            out7 = torch.empty((7,), dtype=torch.float32, device=dev)
+            scratch = torch.empty((16,), dtype=torch.float64, device=dev)
+            _lib.check(lib.fs2_masked_losses(_lib.ptr(before), _lib.ptr(after), _lib.ptr(ys_c), int(ys_c.shape[1]), _lib.ptr(d_outs),
+                                             _lib.ptr(ds_c), _lib.dur_dtype(ds_c), _lib.ptr(e_outs), _lib.ptr(p_outs), _lib.ptr(es_c),
+                                             _lib.ptr(ps_c), _lib.ptr(ilens.contiguous()), _lib.ptr(olens.contiguous()), B, T, L,
+                                             self.odim, _lib.ptr(out7), _lib.ptr(scratch), _lib.stream_ptr(dev)), "fs2_masked_losses")
         vals = out7.tolist()
         names = ["l1_loss", "before_loss", "after_loss", "duration_loss", "energy_loss", "pitch_loss", "loss"]
         return out7[6], [{k: v} for k, v in zip(names, vals)]

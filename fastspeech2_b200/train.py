@@ -10,6 +10,11 @@ dropout sites and BatchNorm batch statistics follow the reference modules line b
 `train_forward`).  With `train_attention="flash"` (tf32 only) self-attention runs on the fused tensor-core kernels of
 csrc/attention_train_tc.cu (`FlashAttentionFn`, DESIGN.md §13) instead of the materialized `AttentionFn`.
 
+Deterministic mode (`det=True` on the Functions below, `conv_math(math, True)` for ConvFn, DESIGN.md §26): every sum that the default kernels take with
+floating-point atomics runs on the library's `_det` twins instead, which add per-CTA partials from a workspace in a fixed
+order.  `train_forward` turns it on for a model built with `train_deterministic` and whenever
+`torch.are_deterministic_algorithms_enabled()`; the same weights, batches and seed then give the same bits every run.
+
 Dropout masks come from `MaskSource`: the library's Philox kernel in production, or masks injected by a test so that the
 reference (with `torch.nn.functional.dropout` patched to consume the same list) and this path drop the same elements.
 """
@@ -23,8 +28,10 @@ import torch
 
 from . import _lib
 from . import length_regulator as _lr
+from ._kernel_module import query_bytes
 
 ACT_NONE, ACT_RELU, ACT_TANH = 0, 1, 2
+DET_SUMS = 0x100     # or'ed into ConvFn's `math`: its weight and bias gradients take the ordered sums (conv_math)
 
 
 def _st(t: torch.Tensor) -> int:
@@ -41,6 +48,18 @@ def _chk(rc: int, what: str) -> None:
 
 def _c(t: torch.Tensor) -> torch.Tensor:
     return t if t.is_contiguous() else t.contiguous()
+
+
+def _det_ws(entry: str, device, *shape):
+    """(workspace, bytes) of the ordered entry `entry` for `shape` (its `_ws_bytes` query), from the caching allocator."""
+    nbytes = query_bytes(entry + "_ws_bytes", *shape)
+    return torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=device), nbytes
+
+
+def deterministic_step(model) -> bool:
+    """Whether a train step of `model` sums in the fixed order of the `_det` entries: the model's `train_deterministic`,
+    or torch's own flag (`torch.use_deterministic_algorithms(True)`) at the time of the step."""
+    return bool(getattr(model, "train_deterministic", False)) or torch.are_deterministic_algorithms_enabled()
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -87,7 +106,9 @@ class MaskSource:
 class ConvFn(torch.autograd.Function):
     """out = act(conv1d_same(x, w) + bias) (+ resid); x [B,L,K], w [N,K,taps] (nn.Conv1d) or [N,K] (nn.Linear).
     `math`: _lib.MATH_FP32 (CUDA cores) or _lib.MATH_TF32 (forward and input gradient on the tap GEMM's tf32 family,
-    weight gradient on the tensor-core wgrad kernel; the bias gradient is the same column sum in both)."""
+    weight gradient on the tensor-core wgrad kernel; the bias gradient is the same column sum in both).
+    `math | DET_SUMS` (conv_math): weight and bias gradients summed in a fixed order (fs2_conv_wgrad_det; tf32:
+    fs2_colsum_det for the bias)."""
 
     @staticmethod
     def forward(ctx, x, w, bias, act, resid, math=_lib.MATH_FP32):
@@ -97,6 +118,7 @@ class ConvFn(torch.autograd.Function):
         N = w.shape[0]
         taps = w.shape[2] if w.dim() == 3 else 1
         assert not (act != ACT_NONE and resid is not None)
+        det, math = bool(math & DET_SUMS), math & ~DET_SUMS
         if math not in (_lib.MATH_FP32, _lib.MATH_TF32):
             raise ValueError(f"ConvFn: math mode {math} is neither MATH_FP32 nor MATH_TF32")
         out = torch.empty((B, L, N), dtype=torch.float32, device=x.device)
@@ -111,6 +133,7 @@ class ConvFn(torch.autograd.Function):
         ctx.save_for_backward(x, wc, out if act != ACT_NONE else None)
         ctx.meta = (B, L, K, N, taps, int(act), bias is not None, resid is not None, w.shape)
         ctx.math = math
+        ctx.det = bool(det)
         return out
 
     @staticmethod
@@ -139,11 +162,23 @@ class ConvFn(torch.autograd.Function):
             if tf32:
                 nbytes = wgrad_tc_ws_bytes(B, L, N, K, taps)
                 ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=dy.device)
-                _chk(lib.fs2_conv_wgrad_tc(g.data_ptr(), x.data_ptr(), B, L, N, K, taps, dw.data_ptr(), _p(db), ws.data_ptr(), nbytes, _st(dy)),
-                     "fs2_conv_wgrad_tc")
+                _chk(lib.fs2_conv_wgrad_tc(g.data_ptr(), x.data_ptr(), B, L, N, K, taps, dw.data_ptr(), _p(None if ctx.det else db), ws.data_ptr(),
+                                           nbytes, _st(dy)), "fs2_conv_wgrad_tc")
+                if ctx.det and db is not None:      # the tf32 weight gradient is ordered already; its bias column sum is not
+                    ws, nbytes = _det_ws("fs2_colsum_det", dy.device, B * L, N)
+                    _chk(lib.fs2_colsum_det(g.data_ptr(), B * L, N, db.data_ptr(), ws.data_ptr(), nbytes, _st(dy)), "fs2_colsum_det")
+            elif ctx.det:
+                ws, nbytes = _det_ws("fs2_conv_wgrad_det", dy.device, B, L, N, K, taps)
+                _chk(lib.fs2_conv_wgrad_det(g.data_ptr(), x.data_ptr(), B, L, N, K, taps, dw.data_ptr(), _p(db), ws.data_ptr(), nbytes, _st(dy)),
+                     "fs2_conv_wgrad_det")
             else:
                 _chk(lib.fs2_conv_wgrad(g.data_ptr(), x.data_ptr(), B, L, N, K, taps, dw.data_ptr(), _p(db), _st(dy)), "fs2_conv_wgrad")
         return dx, dw, db, None, (dy if has_resid else None), None
+
+
+def conv_math(math: int, det: bool) -> int:
+    """ConvFn's `math` argument: the math mode, with DET_SUMS when the step takes the ordered sums."""
+    return math | DET_SUMS if det else math
 
 
 def wgrad_tc_ws_bytes(B: int, L: int, N: int, K: int, taps: int) -> int:
@@ -155,7 +190,7 @@ def wgrad_tc_ws_bytes(B: int, L: int, N: int, K: int, taps: int) -> int:
 
 class LayerNormFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, gamma, beta, eps):
+    def forward(ctx, x, gamma, beta, eps, det=False):
         lib = _lib.load()
         x = _c(x)
         C_ = x.shape[-1]
@@ -165,6 +200,7 @@ class LayerNormFn(torch.autograd.Function):
                                   _st(x)), "fs2_op_layernorm")
         ctx.save_for_backward(x, gamma.detach())
         ctx.eps = float(eps)
+        ctx.det = bool(det)
         return out
 
     @staticmethod
@@ -177,9 +213,13 @@ class LayerNormFn(torch.autograd.Function):
         dx = torch.empty_like(x)
         dg = torch.zeros((C_,), dtype=torch.float32, device=x.device)
         db = torch.zeros((C_,), dtype=torch.float32, device=x.device)
-        _chk(lib.fs2_layernorm_backward(x.data_ptr(), dy.data_ptr(), _c(gamma).data_ptr(), ctx.eps, rows, C_, dx.data_ptr(), dg.data_ptr(), db.data_ptr(),
-                                        _st(x)), "fs2_layernorm_backward")
-        return dx, dg, db, None
+        args = (x.data_ptr(), dy.data_ptr(), _c(gamma).data_ptr(), ctx.eps, rows, C_, dx.data_ptr(), dg.data_ptr(), db.data_ptr())
+        if ctx.det:
+            ws, nbytes = _det_ws("fs2_layernorm_backward_det", x.device, rows, C_)
+            _chk(lib.fs2_layernorm_backward_det(*args, ws.data_ptr(), nbytes, _st(x)), "fs2_layernorm_backward_det")
+        else:
+            _chk(lib.fs2_layernorm_backward(*args, _st(x)), "fs2_layernorm_backward")
+        return dx, dg, db, None, None
 
 
 class AddFn(torch.autograd.Function):
@@ -331,7 +371,7 @@ class EmbedFn(torch.autograd.Function):
     """nn.Embedding(padding_idx=0) + x + alpha * pe (fastspeech.py:65-67, embedding.py:105-120, before its dropout)."""
 
     @staticmethod
-    def forward(ctx, xs, table, alpha, pe):
+    def forward(ctx, xs, table, alpha, pe, det=False):
         B, T = xs.shape
         C_ = table.shape[1]
         out = torch.empty((B, T, C_), dtype=torch.float32, device=xs.device)
@@ -340,6 +380,7 @@ class EmbedFn(torch.autograd.Function):
                                           B, T, C_, out.data_ptr(), None, None, _st(xs)), "fs2_embed_posenc")
         ctx.save_for_backward(xs, pe2)
         ctx.meta = (B, T, C_, table.shape[0])
+        ctx.det = bool(det)
         return out
 
     @staticmethod
@@ -349,16 +390,20 @@ class EmbedFn(torch.autograd.Function):
         dy = _c(dy)
         dtab = torch.zeros((n_sym, C_), dtype=torch.float32, device=dy.device)
         dalpha = torch.zeros((1,), dtype=torch.float32, device=dy.device)
-        _chk(_lib.load().fs2_embed_backward(xs.data_ptr(), dy.data_ptr(), pe2.data_ptr(), B, T, C_, n_sym, dtab.data_ptr(), dalpha.data_ptr(), _st(dy)),
-             "fs2_embed_backward")
-        return None, dtab, dalpha.reshape(()), None
+        args = (xs.data_ptr(), dy.data_ptr(), pe2.data_ptr(), B, T, C_, n_sym, dtab.data_ptr(), dalpha.data_ptr())
+        if ctx.det:
+            ws, nbytes = _det_ws("fs2_embed_backward_det", dy.device, B, T, C_, n_sym)
+            _chk(_lib.load().fs2_embed_backward_det(*args, ws.data_ptr(), nbytes, _st(dy)), "fs2_embed_backward_det")
+        else:
+            _chk(_lib.load().fs2_embed_backward(*args, _st(dy)), "fs2_embed_backward")
+        return None, dtab, dalpha.reshape(()), None, None
 
 
 class PosEncFn(torch.autograd.Function):
     """x + alpha * pe[:T] (ScaledPositionalEncoding of the decoder input layer, before its dropout)."""
 
     @staticmethod
-    def forward(ctx, x, alpha, pe):
+    def forward(ctx, x, alpha, pe, det=False):
         x = _c(x)
         B, T, C_ = x.shape
         pe2 = _c(pe.reshape(-1, C_))
@@ -366,6 +411,7 @@ class PosEncFn(torch.autograd.Function):
         _chk(_lib.load().fs2_posenc_add(x.data_ptr(), pe2.data_ptr(), alpha.detach().reshape(1).data_ptr(), B, T, C_, out.data_ptr(), _st(x)), "fs2_posenc_add")
         ctx.save_for_backward(pe2)
         ctx.meta = (B, T, C_)
+        ctx.det = bool(det)
         return out
 
     @staticmethod
@@ -374,15 +420,20 @@ class PosEncFn(torch.autograd.Function):
         B, T, C_ = ctx.meta
         dy = _c(dy)
         dalpha = torch.zeros((1,), dtype=torch.float32, device=dy.device)
-        _chk(_lib.load().fs2_embed_backward(None, dy.data_ptr(), pe2.data_ptr(), B, T, C_, 0, None, dalpha.data_ptr(), _st(dy)), "fs2_embed_backward")
-        return dy, dalpha.reshape(()), None
+        args = (None, dy.data_ptr(), pe2.data_ptr(), B, T, C_, 0, None, dalpha.data_ptr())
+        if ctx.det:
+            ws, nbytes = _det_ws("fs2_embed_backward_det", dy.device, B, T, C_, 0)
+            _chk(_lib.load().fs2_embed_backward_det(*args, ws.data_ptr(), nbytes, _st(dy)), "fs2_embed_backward_det")
+        else:
+            _chk(_lib.load().fs2_embed_backward(*args, _st(dy)), "fs2_embed_backward")
+        return dy, dalpha.reshape(()), None, None
 
 
 class RowDotFn(torch.autograd.Function):
     """Linear(C -> 1).squeeze(-1), masked_fill(pad, 0): the predictors' heads."""
 
     @staticmethod
-    def forward(ctx, x, w, bias, lens):
+    def forward(ctx, x, w, bias, lens, det=False):
         x = _c(x)
         B, L, C_ = x.shape
         y = torch.empty((B, L), dtype=torch.float32, device=x.device)
@@ -390,6 +441,7 @@ class RowDotFn(torch.autograd.Function):
         _chk(_lib.load().fs2_rowdot(x.data_ptr(), wv.data_ptr(), _c(bias.detach()).data_ptr(), _p(lens), B * L, L, C_, y.data_ptr(), _st(x)), "fs2_rowdot")
         ctx.save_for_backward(x, wv, lens)
         ctx.wshape = w.shape
+        ctx.det = bool(det)
         return y
 
     @staticmethod
@@ -400,9 +452,13 @@ class RowDotFn(torch.autograd.Function):
         dx = torch.empty_like(x)
         dw = torch.zeros((C_,), dtype=torch.float32, device=x.device)
         db = torch.zeros((1,), dtype=torch.float32, device=x.device)
-        _chk(_lib.load().fs2_rowdot_backward(x.data_ptr(), wv.data_ptr(), dy.data_ptr(), _p(lens), B * L, L, C_, dx.data_ptr(), dw.data_ptr(), db.data_ptr(),
-                                             _st(x)), "fs2_rowdot_backward")
-        return dx, dw.reshape(ctx.wshape), db, None
+        args = (x.data_ptr(), wv.data_ptr(), dy.data_ptr(), _p(lens), B * L, L, C_, dx.data_ptr(), dw.data_ptr(), db.data_ptr())
+        if ctx.det:
+            ws, nbytes = _det_ws("fs2_rowdot_backward_det", x.device, B * L, C_)
+            _chk(_lib.load().fs2_rowdot_backward_det(*args, ws.data_ptr(), nbytes, _st(x)), "fs2_rowdot_backward_det")
+        else:
+            _chk(_lib.load().fs2_rowdot_backward(*args, _st(x)), "fs2_rowdot_backward")
+        return dx, dw.reshape(ctx.wshape), db, None, None
 
 
 class SpeakerAddFn(torch.autograd.Function):
@@ -468,7 +524,7 @@ class OneHotLinearAddFn(torch.autograd.Function):
     """hs + Linear(n_bins -> C)(one_hot(ids)) (fastspeech.py:218-219); W [C, n_bins], b [C]."""
 
     @staticmethod
-    def forward(ctx, x, ids, W, b):
+    def forward(ctx, x, ids, W, b, det=False):
         x = _c(x)
         rows, C_ = x.numel() // x.shape[-1], x.shape[-1]
         out = torch.empty_like(x)
@@ -476,6 +532,7 @@ class OneHotLinearAddFn(torch.autograd.Function):
                                                    out.data_ptr(), _st(x)), "fs2_onehot_linear_forward")
         ctx.save_for_backward(ids)
         ctx.meta = (rows, C_, W.shape[1])
+        ctx.det = bool(det)
         return out
 
     @staticmethod
@@ -485,27 +542,36 @@ class OneHotLinearAddFn(torch.autograd.Function):
         dy = _c(dy)
         dW = torch.zeros((C_, nb), dtype=torch.float32, device=dy.device)
         db = torch.zeros((C_,), dtype=torch.float32, device=dy.device)
-        _chk(_lib.load().fs2_onehot_linear_backward(ids.data_ptr(), dy.data_ptr(), rows, C_, nb, dW.data_ptr(), db.data_ptr(), _st(dy)),
-             "fs2_onehot_linear_backward")
-        return dy, None, dW, db
+        args = (ids.data_ptr(), dy.data_ptr(), rows, C_, nb, dW.data_ptr(), db.data_ptr())
+        if ctx.det:
+            ws, nbytes = _det_ws("fs2_onehot_linear_backward_det", dy.device, rows, C_, nb)
+            _chk(_lib.load().fs2_onehot_linear_backward_det(*args, ws.data_ptr(), nbytes, _st(dy)), "fs2_onehot_linear_backward_det")
+        else:
+            _chk(_lib.load().fs2_onehot_linear_backward(*args, _st(dy)), "fs2_onehot_linear_backward")
+        return dy, None, dW, db, None
 
 
 class BatchNormFn(torch.autograd.Function):
     """BatchNorm1d in train mode over all B*L rows of a channel (+ optional tanh); updates the running statistics."""
 
     @staticmethod
-    def forward(ctx, x, gamma, beta, running_mean, running_var, eps, momentum, act):
+    def forward(ctx, x, gamma, beta, running_mean, running_var, eps, momentum, act, det=False):
         x = _c(x)
         C_ = x.shape[-1]
         rows = x.numel() // C_
         y = torch.empty_like(x)
         stats = torch.empty((2 * C_,), dtype=torch.float32, device=x.device)
-        scratch = torch.empty((4 * C_,), dtype=torch.float64, device=x.device)
-        _chk(_lib.load().fs2_batchnorm_train(x.data_ptr(), rows, C_, _c(gamma.detach()).data_ptr(), _c(beta.detach()).data_ptr(), float(eps), float(momentum),
-                                             int(act), running_mean.data_ptr(), running_var.data_ptr(), stats.data_ptr(), y.data_ptr(), scratch.data_ptr(),
-                                             _st(x)), "fs2_batchnorm_train")
+        args = (x.data_ptr(), rows, C_, _c(gamma.detach()).data_ptr(), _c(beta.detach()).data_ptr(), float(eps), float(momentum), int(act),
+                running_mean.data_ptr(), running_var.data_ptr(), stats.data_ptr(), y.data_ptr())
+        if det:
+            ws, nbytes = _det_ws("fs2_batchnorm_train_det", x.device, rows, C_)
+            _chk(_lib.load().fs2_batchnorm_train_det(*args, ws.data_ptr(), nbytes, _st(x)), "fs2_batchnorm_train_det")
+        else:
+            scratch = torch.empty((4 * C_,), dtype=torch.float64, device=x.device)
+            _chk(_lib.load().fs2_batchnorm_train(*args, scratch.data_ptr(), _st(x)), "fs2_batchnorm_train")
         ctx.save_for_backward(x, stats, gamma.detach(), y if act != ACT_NONE else None)
         ctx.meta = (rows, C_, float(eps), int(act))
+        ctx.det = bool(det)
         return y
 
     @staticmethod
@@ -521,10 +587,14 @@ class BatchNormFn(torch.autograd.Function):
         dx = torch.empty_like(x)
         dg = torch.zeros((C_,), dtype=torch.float32, device=x.device)
         db = torch.zeros((C_,), dtype=torch.float32, device=x.device)
-        scratch = torch.empty((4 * C_,), dtype=torch.float64, device=x.device)
-        _chk(lib.fs2_batchnorm_backward(x.data_ptr(), g.data_ptr(), stats.data_ptr(), _c(gamma).data_ptr(), eps, rows, C_, dx.data_ptr(), dg.data_ptr(),
-                                        db.data_ptr(), scratch.data_ptr(), _st(x)), "fs2_batchnorm_backward")
-        return dx, dg, db, None, None, None, None, None
+        args = (x.data_ptr(), g.data_ptr(), stats.data_ptr(), _c(gamma).data_ptr(), eps, rows, C_, dx.data_ptr(), dg.data_ptr(), db.data_ptr())
+        if ctx.det:
+            ws, nbytes = _det_ws("fs2_batchnorm_backward_det", x.device, rows, C_)
+            _chk(lib.fs2_batchnorm_backward_det(*args, ws.data_ptr(), nbytes, _st(x)), "fs2_batchnorm_backward_det")
+        else:
+            scratch = torch.empty((4 * C_,), dtype=torch.float64, device=x.device)
+            _chk(lib.fs2_batchnorm_backward(*args, scratch.data_ptr(), _st(x)), "fs2_batchnorm_backward")
+        return dx, dg, db, None, None, None, None, None, None
 
 
 class LossFn(torch.autograd.Function):
@@ -532,16 +602,9 @@ class LossFn(torch.autograd.Function):
     differentiable through element 6 only (the scalar the training loop back-propagates)."""
 
     @staticmethod
-    def forward(ctx, before, after, d_outs, e_outs, p_outs, ys, ds, es, ps, ilens, olens):
-        lib = _lib.load()
+    def forward(ctx, before, after, d_outs, e_outs, p_outs, ys, ds, es, ps, ilens, olens, det=False):
         before, after, d_outs, e_outs, p_outs = (_c(t) for t in (before, after, d_outs, e_outs, p_outs))
-        B, L, odim = before.shape
-        T = d_outs.shape[1]
-        out7 = torch.empty((7,), dtype=torch.float32, device=before.device)
-        scratch = torch.empty((16,), dtype=torch.float64, device=before.device)
-        _chk(lib.fs2_masked_losses(before.data_ptr(), after.data_ptr(), ys.data_ptr(), int(ys.shape[1]), d_outs.data_ptr(), ds.data_ptr(), _lib.dur_dtype(ds),
-                                   e_outs.data_ptr(), p_outs.data_ptr(), es.data_ptr(), ps.data_ptr(), ilens.data_ptr(), olens.data_ptr(), B, T, L, odim,
-                                   out7.data_ptr(), scratch.data_ptr(), _st(before)), "fs2_masked_losses")
+        out7 = masked_losses(before, after, d_outs, e_outs, p_outs, ys, ds, es, ps, ilens, olens, det)
         ctx.save_for_backward(before, after, d_outs, e_outs, p_outs, ys, ds, es, ps, ilens, olens)
         return out7
 
@@ -557,7 +620,25 @@ class LossFn(torch.autograd.Function):
         _chk(lib.fs2_loss_backward(before.data_ptr(), after.data_ptr(), ys.data_ptr(), int(ys.shape[1]), d_outs.data_ptr(), ds.data_ptr(), _lib.dur_dtype(ds),
                                    e_outs.data_ptr(), p_outs.data_ptr(), es.data_ptr(), ps.data_ptr(), ilens.data_ptr(), olens.data_ptr(), B, T, L, odim,
                                    g.data_ptr(), gb.data_ptr(), ga.data_ptr(), gd.data_ptr(), ge.data_ptr(), gp.data_ptr(), _st(before)), "fs2_loss_backward")
-        return gb, ga, gd, ge, gp, None, None, None, None, None, None
+        return gb, ga, gd, ge, gp, None, None, None, None, None, None, None
+
+
+def masked_losses(before, after, d_outs, e_outs, p_outs, ys, ds, es, ps, ilens, olens, det: bool = False) -> torch.Tensor:
+    """The 7 report values of fs2_masked_losses (contiguous CUDA inputs, ys [B, >= L, odim]); `det`: fs2_masked_losses_det,
+    whose five sums are added in a fixed order."""
+    lib = _lib.load()
+    B, L, odim = before.shape
+    T = d_outs.shape[1]
+    out7 = torch.empty((7,), dtype=torch.float32, device=before.device)
+    args = (before.data_ptr(), after.data_ptr(), ys.data_ptr(), int(ys.shape[1]), d_outs.data_ptr(), ds.data_ptr(), _lib.dur_dtype(ds),
+            e_outs.data_ptr(), p_outs.data_ptr(), es.data_ptr(), ps.data_ptr(), ilens.data_ptr(), olens.data_ptr(), B, T, L, odim, out7.data_ptr())
+    if det:
+        ws, nbytes = _det_ws("fs2_masked_losses_det", before.device, B, T, L, odim)
+        _chk(lib.fs2_masked_losses_det(*args, ws.data_ptr(), nbytes, _st(before)), "fs2_masked_losses_det")
+    else:
+        scratch = torch.empty((16,), dtype=torch.float64, device=before.device)
+        _chk(lib.fs2_masked_losses(*args, scratch.data_ptr(), _st(before)), "fs2_masked_losses")
+    return out7
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -569,41 +650,44 @@ def _drop(x: torch.Tensor, p: float, masks: MaskSource, channel_first: bool = Fa
     return DropoutFn.apply(x, masks.next(tuple(x.shape), p, x.device), p)
 
 
-def _fft_blocks(stack, x, lens, heads: int, rate: float, masks: MaskSource, math: int = _lib.MATH_FP32, flash: bool = False):
+def _fft_blocks(stack, x, lens, heads: int, rate: float, masks: MaskSource, math: int = _lib.MATH_FP32, flash: bool = False,
+                det: bool = False):
     """core/encoder.py:46-71 (post-LN, concat_after=False) x num_blocks.  `flash`: attention on the fused tf32 kernels
-    (FlashAttentionFn) instead of the materialized AttentionFn."""
+    (FlashAttentionFn) instead of the materialized AttentionFn.  `det`: the ordered sums of the deterministic mode."""
     B, L, C_ = x.shape
+    cm = conv_math(math, det)
     for blk in stack.encoders_:
         a = blk.self_attn
-        q = ConvFn.apply(x, a.linear_q.weight, a.linear_q.bias, ACT_NONE, None, math)        # attention.py:48-50
-        k = ConvFn.apply(x, a.linear_k.weight, a.linear_k.bias, ACT_NONE, None, math)
-        v = ConvFn.apply(x, a.linear_v.weight, a.linear_v.bias, ACT_NONE, None, math)
+        q = ConvFn.apply(x, a.linear_q.weight, a.linear_q.bias, ACT_NONE, None, cm)   # attention.py:48-50
+        k = ConvFn.apply(x, a.linear_k.weight, a.linear_k.bias, ACT_NONE, None, cm)
+        v = ConvFn.apply(x, a.linear_v.weight, a.linear_v.bias, ACT_NONE, None, cm)
         if flash:
             dmask, seed, off = masks.attention((B, heads, L, L), rate, x.device) if rate > 0 else (None, 0, 0)   # attention.py:69
             ctx = FlashAttentionFn.apply(q, k, v, lens, heads, rate, dmask, seed, off)
         else:
             dmask = masks.next((B, heads, L, L), rate, x.device) if rate > 0 else None       # attention.py:69
             ctx = AttentionFn.apply(q, k, v, lens, heads, rate, dmask)
-        att = ConvFn.apply(ctx, a.linear_out.weight, a.linear_out.bias, ACT_NONE, None, math)  # attention.py:74
+        att = ConvFn.apply(ctx, a.linear_out.weight, a.linear_out.bias, ACT_NONE, None, cm)   # attention.py:74
         x = AddFn.apply(x, _drop(att, rate, masks))                                           # encoder.py:60
-        x = LayerNormFn.apply(x, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)             # encoder.py:62
+        x = LayerNormFn.apply(x, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps, det)        # encoder.py:62
         f = blk.feed_forward
-        h = ConvFn.apply(x, f.w_1.weight, f.w_1.bias, ACT_RELU, None, math)                   # modules.py:247
+        h = ConvFn.apply(x, f.w_1.weight, f.w_1.bias, ACT_RELU, None, cm)              # modules.py:247
         h = _drop(h, rate, masks)                                                             # modules.py:248
-        y = ConvFn.apply(h, f.w_2.weight, f.w_2.bias, ACT_NONE, None, math)
+        y = ConvFn.apply(h, f.w_2.weight, f.w_2.bias, ACT_NONE, None, cm)
         x = AddFn.apply(x, _drop(y, rate, masks))                                             # encoder.py:67
-        x = LayerNormFn.apply(x, blk.norm2.weight, blk.norm2.bias, blk.norm2.eps)             # encoder.py:69
+        x = LayerNormFn.apply(x, blk.norm2.weight, blk.norm2.bias, blk.norm2.eps, det)        # encoder.py:69
     return x
 
 
-def _predictor(pred, x, lens, rate: float, masks: MaskSource, math: int = _lib.MATH_FP32):
+def _predictor(pred, x, lens, rate: float, masks: MaskSource, math: int = _lib.MATH_FP32, det: bool = False):
     """duration_predictor.py:64-86 / variance_predictor.py:39-78: [conv -> ReLU -> LayerNorm(channels) -> Dropout] x n, Linear -> 1, mask."""
+    cm = conv_math(math, det)
     for layer in pred.conv:
         conv, ln = layer[0], layer[2].layer_norm
-        x = ConvFn.apply(x, conv.weight, conv.bias, ACT_RELU, None, math)
-        x = LayerNormFn.apply(x, ln.weight, ln.bias, ln.eps)
+        x = ConvFn.apply(x, conv.weight, conv.bias, ACT_RELU, None, cm)
+        x = LayerNormFn.apply(x, ln.weight, ln.bias, ln.eps, det)
         x = _drop(x, rate, masks, channel_first=True)
-    return RowDotFn.apply(x, pred.linear.weight, pred.linear.bias, lens)
+    return RowDotFn.apply(x, pred.linear.weight, pred.linear.bias, lens, det)
 
 
 def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskSource] = None, speakers=None):
@@ -617,6 +701,8 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
     masks = masks or MaskSource(seed=int(torch.initial_seed()) & 0xFFFFFFFF)
     math = _lib.MATH_TF32 if model.train_precision == "tf32" else _lib.MATH_FP32
     flash = model.train_attention == "flash"
+    det = deterministic_step(model)
+    cm = conv_math(math, det)
     d = model.dims
     ilens = ilens.to(device=dev, dtype=torch.int64).contiguous()
     olens = olens.to(device=dev, dtype=torch.int64).contiguous()
@@ -639,48 +725,48 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
 
     # encoder (fastspeech.py:180-184): Embedding + scaled positional encoding + dropout, FFT blocks
     enc_pos = model.encoder.embed[-1]
-    x = EmbedFn.apply(xs, model.encoder.embed[0].weight, enc_pos.alpha, enc_pos.pe)
+    x = EmbedFn.apply(xs, model.encoder.embed[0].weight, enc_pos.alpha, enc_pos.pe, det)
     x = _drop(x, ER, masks)                                                                   # embedding.py:120
-    hs = _fft_blocks(model.encoder, x, ilens, d.aheads, ER, masks, math, flash)
+    hs = _fft_blocks(model.encoder, x, ilens, d.aheads, ER, masks, math, flash, det)
     if spk is not None:     # hs + E[spk] at every row, fp32 in both train precisions
         hs = SpeakerAddFn.apply(hs, spk, model.speaker_embed.weight)
     # duration predictor on the encoder states, then LengthRegulator with the ground-truth durations (:209-211)
-    d_outs = _predictor(model.duration_predictor, hs, ilens, model.duration_dropout_rate, masks, math)
+    d_outs = _predictor(model.duration_predictor, hs, ilens, model.duration_dropout_rate, masks, math, det)
     hm = LengthRegulatorFn.apply(hs, ds, ilens, L)
-    e_outs = _predictor(model.energy_predictor.predictor, hm, olens, PR, masks, math)               # :212-215
-    p_outs = _predictor(model.pitch_predictor.predictor, hm, olens, PR, masks, math)
+    e_outs = _predictor(model.energy_predictor.predictor, hm, olens, PR, masks, math, det)          # :212-215
+    p_outs = _predictor(model.pitch_predictor.predictor, hm, olens, PR, masks, math, det)
     # hs + pitch_embed(one_hot(ps)) + energy_embed(one_hot(es)) (:200-206,218-219); bucket ids from the library's bucketize
     e_ids = torch.empty((B, L), dtype=torch.int64, device=dev)
     p_ids = torch.empty((B, L), dtype=torch.int64, device=dev)
     eb, pb = model.energy_predictor.energy_bins, model.pitch_predictor.pitch_bins
     _chk(lib.fs2_bucketize(es.data_ptr(), eb.data_ptr(), eb.numel(), es.numel(), e_ids.data_ptr(), _st(es)), "fs2_bucketize")
     _chk(lib.fs2_bucketize(ps.data_ptr(), pb.data_ptr(), pb.numel(), ps.numel(), p_ids.data_ptr(), _st(ps)), "fs2_bucketize")
-    hm = OneHotLinearAddFn.apply(hm, p_ids, model.pitch_embed.weight, model.pitch_embed.bias)
-    hm = OneHotLinearAddFn.apply(hm, e_ids, model.energy_embed.weight, model.energy_embed.bias)
+    hm = OneHotLinearAddFn.apply(hm, p_ids, model.pitch_embed.weight, model.pitch_embed.bias, det)
+    hm = OneHotLinearAddFn.apply(hm, e_ids, model.energy_embed.weight, model.energy_embed.bias, det)
     # decoder input layer (core/encoder.py:118-125): Linear -> LayerNorm -> Dropout -> ReLU -> scaled positional encoding (+ dropout)
     emb = model.decoder.embed
-    z = ConvFn.apply(hm, emb[0].weight, emb[0].bias, ACT_NONE, None, math)
-    z = LayerNormFn.apply(z, emb[1].weight, emb[1].bias, emb[1].eps)
+    z = ConvFn.apply(hm, emb[0].weight, emb[0].bias, ACT_NONE, None, cm)
+    z = LayerNormFn.apply(z, emb[1].weight, emb[1].bias, emb[1].eps, det)
     z = _drop(z, DR, masks)
     z = ReluFn.apply(z)
-    z = PosEncFn.apply(z, emb[4].alpha, emb[4].pe)
+    z = PosEncFn.apply(z, emb[4].alpha, emb[4].pe, det)
     z = _drop(z, DR, masks)
-    z = _fft_blocks(model.decoder, z, olens, d.aheads, DR, masks, math, flash)
-    before = ConvFn.apply(z, model.feat_out.weight, model.feat_out.bias, ACT_NONE, None, math)  # :228-230
+    z = _fft_blocks(model.decoder, z, olens, d.aheads, DR, masks, math, flash, det)
+    before = ConvFn.apply(z, model.feat_out.weight, model.feat_out.bias, ACT_NONE, None, cm)   # :228-230
     # Postnet (modules.py:283-359): [conv(no bias) -> BatchNorm1d(batch statistics) -> tanh -> dropout] x 4, conv -> BN -> dropout; + residual
     y = before
     n_post = len(model.postnet.postnet)
     for i, layer in enumerate(model.postnet.postnet):
         conv, bn = layer[0], layer[1]
         last = i == n_post - 1
-        y = ConvFn.apply(y, conv.weight, None, ACT_NONE, None, math)
+        y = ConvFn.apply(y, conv.weight, None, ACT_NONE, None, cm)
         y = BatchNormFn.apply(y, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, bn.momentum if bn.momentum is not None else 0.1,
-                              ACT_NONE if last else ACT_TANH)
+                              ACT_NONE if last else ACT_TANH, det)
         with torch.no_grad():
             bn.num_batches_tracked += 1
         y = _drop(y, POST, masks, channel_first=True)
     after = AddFn.apply(before, y)                                                            # :236-238
-    out7 = LossFn.apply(before, after, d_outs, e_outs, p_outs, ys, ds, es, ps, ilens, olens)
+    out7 = LossFn.apply(before, after, d_outs, e_outs, p_outs, ys, ds, es, ps, ilens, olens, det)
     vals = out7.detach().tolist()
     names = ["l1_loss", "before_loss", "after_loss", "duration_loss", "energy_loss", "pitch_loss", "loss"]
     return out7[6], [{k: v} for k, v in zip(names, vals)]

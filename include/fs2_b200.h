@@ -476,6 +476,61 @@ int fs2_loss_backward(const float* before, const float* after, const float* ys, 
                       int B, int T, int L, int odim, const float* grad_loss, float* g_before, float* g_after, float* g_d, float* g_e, float* g_p,
                       void* stream);
 
+/* ---- deterministic train mode (DESIGN.md section 26) ------------------------------------------------------------------
+ * The ordered twin of every train entry that sums with floating-point atomics.  Same arguments and results as the entry
+ * without _det, plus a caller-owned workspace: each partial sum (per CTA, chunk, block or row) is stored there and the
+ * partials are added in ascending index order through a fixed tree, so the order of every floating-point sum depends
+ * only on the shapes and on the id and length tensors -- not on timing, workspace contents, pointers or the SM count.
+ * The same inputs give the same bits on every run and every H100.  No floating-point atomics run on this path.
+ * The rounding differs from the entry without _det (the sums are grouped differently); the default entries are unchanged.
+ *
+ * ws: at least the _ws_bytes answer for the same shape, 16-byte aligned, contents on entry unused (a call whose answer
+ * is 0 may pass NULL).  Every argument error -- a null pointer, a bad size, a short or misaligned workspace -- is
+ * FS2_ERR_INVALID before anything is launched.  Workspace bounds (floats are 4 bytes, doubles 8, ints 4; every region
+ * rounded up to 256 bytes; M = B * L rows, gy(r) = min(r / 512 + 1, 64), ctas(r) = min(r / 8 + 1, 528)):
+ *   colsum               gy(rows) * C floats                                        (0 when rows == 0)
+ *   conv_wgrad           chunks * taps * N * K floats when chunks > 1 (fs2_conv_wgrad's split of the M rows), then
+ *                        gy(M) * N floats for dbias                                 (0 when M == 0)
+ *   layernorm_backward   2 * ctas(rows) * C + gy(ctas(rows)) * C floats             (0 when rows == 0)
+ *   batchnorm_*          min(rows / 256 + 1, 128) * 2C + 2C doubles
+ *   embed_backward       rows + gy(rows) floats, then n_sym * ceil(rows / 256) + 2 (n_sym + 1) + rows ints and
+ *                        (ceil(rows / 256) + n_sym) * C floats for the table's counting sort (rows = B * T)
+ *   onehot_linear        the counting sort with n_bins ids, then gy(rows) * C floats for dbias
+ *   rowdot_backward      ctas(rows) * (C + 1) + gy(ctas(rows)) * C floats          (0 when rows == 0)
+ *   masked_losses        8 + 2 B g1 + 3 B g2 doubles, g1 / g2 the loss kernels' grid widths
+ * The table gradients (embed_backward, onehot_linear_backward) go through a stable counting sort of the rows by id: each
+ * id's rows are added in ascending row order in groups of 256, and the groups in ascending order.  Rows whose id lies
+ * outside [1, n_sym) (embedding: id 0 is padding) or [0, n_bins) (one-hot) add nothing; n_sym, n_bins <= 8192, rows < 2^31.
+ * fs2_conv_wgrad_tc already sums in a fixed order; its ordered form is dbias = NULL plus fs2_colsum_det. */
+int fs2_colsum_det_ws_bytes(int64_t rows, int C, size_t* bytes);
+int fs2_colsum_det(const float* x, int64_t rows, int C, float* out /* += */, void* ws, size_t ws_bytes, void* stream);
+int fs2_conv_wgrad_det_ws_bytes(int B, int L, int N, int K, int taps, size_t* bytes);
+int fs2_conv_wgrad_det(const float* dy, const float* x, int B, int L, int N, int K, int taps, float* dw /* += */, float* dbias /* += or NULL */,
+                       void* ws, size_t ws_bytes, void* stream);
+int fs2_layernorm_backward_det_ws_bytes(int64_t rows, int C, size_t* bytes);
+int fs2_layernorm_backward_det(const float* x, const float* dy, const float* gamma, float eps, int64_t rows, int C, float* dx,
+                               float* dgamma /* += */, float* dbeta /* += */, void* ws, size_t ws_bytes, void* stream);
+int fs2_batchnorm_train_det_ws_bytes(int64_t rows, int C, size_t* bytes);
+int fs2_batchnorm_train_det(const float* x, int64_t rows, int C, const float* gamma, const float* beta, float eps, float momentum, int act,
+                            float* running_mean, float* running_var, float* stats, float* y, void* ws, size_t ws_bytes, void* stream);
+int fs2_batchnorm_backward_det_ws_bytes(int64_t rows, int C, size_t* bytes);
+int fs2_batchnorm_backward_det(const float* x, const float* dy, const float* stats, const float* gamma, float eps, int64_t rows, int C,
+                               float* dx, float* dgamma /* += */, float* dbeta /* += */, void* ws, size_t ws_bytes, void* stream);
+int fs2_embed_backward_det_ws_bytes(int B, int T, int C, int n_sym, size_t* bytes);
+int fs2_embed_backward_det(const int64_t* xs /* NULL: positional part only */, const float* dy, const float* pe, int B, int T, int C, int n_sym,
+                           float* dtable /* += or NULL */, float* dalpha /* += */, void* ws, size_t ws_bytes, void* stream);
+int fs2_onehot_linear_backward_det_ws_bytes(int64_t rows, int C, int n_bins, size_t* bytes);
+int fs2_onehot_linear_backward_det(const int64_t* ids, const float* dy, int64_t rows, int C, int n_bins, float* dW /* += */,
+                                   float* dbias /* += or NULL */, void* ws, size_t ws_bytes, void* stream);
+int fs2_rowdot_backward_det_ws_bytes(int64_t rows, int C, size_t* bytes);
+int fs2_rowdot_backward_det(const float* x, const float* w, const float* dy, const int64_t* lens, int64_t rows, int L, int C, float* dx,
+                            float* dw /* += */, float* dbias /* += */, void* ws, size_t ws_bytes, void* stream);
+int fs2_masked_losses_det_ws_bytes(int B, int Tmax, int L, int odim, size_t* bytes);
+int fs2_masked_losses_det(const float* before, const float* after, const float* ys, int ld_ys_time, const float* d_out,
+                          const void* ds, int ds_dtype, const float* e_out, const float* p_out, const float* es,
+                          const float* ps, const int64_t* ilens, const int64_t* olens, int B, int Tmax, int L, int odim,
+                          float* out7, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- vocoder hand-off (SURVEY.md section 8f-2): the STFT / inverse STFT Griffin-Lim iterates ------------------------- */
 /* utils/stft.py:82-151 without cuFFT, like the reference (which runs them as conv1d / conv_transpose1d with Fourier bases):
  * the two GEMMs go through fs2_op_tap_gemm, these are the kernels around them.  fastspeech2_b200/vocoder.py drives them.
