@@ -66,6 +66,8 @@ FS2_ALIGN_DIM, FS2_ALIGN_MAX_T = 80, 1024
 FS2_RESAMPLE_TABLE = 32769                        # entries of the resampling filter's right wing
 FS2_PLAN_BAD_ILENS,FS2_PLAN_BAD_CONTROL, FS2_PLAN_OVERFLOW = 1, 2, 4   # bits of fs2_length_plan_cap's status word
 FS2_PLAN_BAD_SPEAKER = 8                          # and of fs2_length_plan_cap_spk's
+FS2_SPEMB_NONFINITE = 16                          # fs2_spemb_project's / fs2_encode_spemb's status bit, and fs2_length_plan_cap_spemb's
+FS2_SPEMB_MAX_DIM = 4096                          # the largest speaker-embedding width D
 FS2_SYNTH_VOC_SHIFT = 8                          # fs2_synth_status: the vocoder's bits sit this far up in the word
 
 
@@ -122,12 +124,14 @@ SIGNATURES = {
     "fs2_encode": [_P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _P],
     "fs2_encode_ex": [_P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _I, _P],
     "fs2_encode_spk": [_P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _SZ, _I, _P],
+    "fs2_encode_spemb": [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _SZ, _I, _P, _P, _P],
     "fs2_length_plan": [_P, _I, _P, _F, _I, _I, _I, _P, _P, _P, _P],
     "fs2_length_gather": [_P, _P, _P, _I, _I, _I, _P, _I, _P],
     "fs2_length_plan_ex": [_P, _I, _P, _F, _P, _I, _I, _I, _P, _P, _P, _P, _P],
     "fs2_length_gather_ex": [_P, _P, _P, _I, _I, _I, _P, _I, _P, _P, _P],
     "fs2_length_plan_cap": [_P, _I, _P, _P, _P, _I, _I, _L, _P, _P, _P, _P, _P, _P],
     "fs2_length_plan_cap_spk": [_P, _I, _P, _P, _P, _P, _I, _I, _I, _L, _P, _P, _P, _P, _P, _P],
+    "fs2_length_plan_cap_spemb": [_P, _I, _P, _P, _P, _P, _I, _P, _I, _I, _L, _P, _P, _P, _P, _P, _P],
     "fs2_synth_status": [_P, _P, _P, _I, _I, _P, _P, _P],
     "fs2_decode": [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _SZ, _P],
     "fs2_decode_ex": [_P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _SZ, _I, _P],
@@ -143,6 +147,7 @@ SIGNATURES = {
     "fs2_op_gemm_layernorm": [_I, _P, _L, _I, _I, _P, _P, _P, _P, _P, _F, _P, _P, _P],
     "fs2_op_layernorm": [_P, _P, _P, _P, _F, _L, _I, _P, _P],
     "fs2_op_row_norm": [C.POINTER(RowNormDesc), _P],
+    "fs2_op_row_norm_spemb": [C.POINTER(RowNormDesc), _P, _P],
     "fs2_op_variance_embed_add": [_P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _L, _I, _P, _P, _I, _P, _P, _P, _I, _P],
     "fs2_dropout_mask": [_P, _L, _F, C.c_uint64, C.c_uint64, _P],
     "fs2_dropout_apply": [_P, _P, _F, _P, _L, _P],
@@ -172,6 +177,8 @@ SIGNATURES = {
     "fs2_speaker_add": [_P, _P, _P, _I, _I, _I, _I, _P, _P],
     "fs2_speaker_add_backward_ws_bytes": [_I, _I, C.POINTER(_SZ)],
     "fs2_speaker_add_backward": [_P, _P, _I, _I, _I, _I, _P, _P, _SZ, _P],
+    "fs2_spemb_project": [_P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P],
+    "fs2_spemb_project_backward": [_P, _P, _I, _I, _I, _P, _P, _P],
     "fs2_onehot_linear_forward": [_P, _P, _P, _P, _L, _I, _I, _P, _P],
     "fs2_onehot_linear_backward": [_P, _P, _L, _I, _I, _P, _P, _P],
     "fs2_length_regulator_backward": [_P, _P, _P, _I, _I, _I, _I, _P, _P],

@@ -76,6 +76,7 @@ struct fs2_handle {
   const float* e_tab = nullptr; const float* e_tab_bias = nullptr;
   const float* p_tab = nullptr; const float* p_tab_bias = nullptr;
   const float* spk_table = nullptr; int n_speakers = 0;   // optional speaker_embed.weight [n_speakers, adim]
+  const float* spemb_w = nullptr; const float* spemb_b = nullptr; int spemb_dim = 0;   // optional spk_embed_proj [adim, D], [adim]
   // decoder side
   fs2::VWeight dec_in; fs2::Norm dec_in_ln; const float* dec_pe = nullptr; const float* dec_alpha = nullptr;
   fs2::VWeight feat_out;
@@ -136,8 +137,8 @@ RowNorm masked(RowNorm r, const int64_t* zlens, int L) {
   return r;
 }
 
-// the speaker add of the last encoder LayerNorm (RowNorm::spk_table); table == nullptr: none
-struct SpeakerAdd { const float* table = nullptr; const int64_t* ids = nullptr; int n = 0; };
+// the speaker adds of the last encoder LayerNorm (RowNorm::spk_table, RowNorm::spk_vec); nullptr: none
+struct SpeakerAdd { const float* table = nullptr; const int64_t* ids = nullptr; int n = 0; const float* vec = nullptr; };
 
 struct BlockBufs {
   float *x, *y;            // fp32 rows [rows, C]: block input / output ping-pong (the residual stream)
@@ -194,6 +195,7 @@ int run_blocks(const std::vector<Block>& blocks, const BlockBufs& w, const int64
     RowNorm r2 = masked(make_norm(k.ln2, y, C, rows, C, x, C), zlens, L);
     if (planes) { r2.split_out = w.xp; r2.split_lo = x3; }   // planes of the block output: A operand of the next q|k|v / mel projection
     if (spk.table && &k == &blocks.back()) { r2.spk_table = spk.table; r2.spk = spk.ids; r2.n_spk = spk.n; r2.spk_L = L; }
+    if (spk.vec && &k == &blocks.back()) { r2.spk_vec = spk.vec; r2.spk_L = L; }
     if ((rc = norm_rows(r2, st))) return rc;
   }
   *result = x;
@@ -367,6 +369,23 @@ struct Packer {
       if ((rc = copy("speaker_embed.weight", sp->shape[0] * c.adim, &h->spk_table))) return rc;
       h->n_speakers = (int)sp->shape[0];
     }
+    // optional speaker-embedding projection (DESIGN.md section 27): D read off the weight, the bias must come with it
+    h->spemb_w = h->spemb_b = nullptr; h->spemb_dim = 0;
+    {
+      const fs2_weight_desc* pw = find(m, "spk_embed_proj.weight");
+      const fs2_weight_desc* pb = find(m, "spk_embed_proj.bias");
+      if (pw || pb) {
+        if (!pw || !pb || pw->ndim != 2 || pw->shape[0] != c.adim || pw->shape[1] < 1 || pw->shape[1] > FS2_SPEMB_MAX_DIM ||
+            pw->dtype != 0 || pb->ndim != 1 || pb->shape[0] != c.adim || pb->dtype != 0) {
+          set_error("fs2_load_weights: 'spk_embed_proj.weight' [adim=%d, D in [1, %d]] and 'spk_embed_proj.bias' [adim] must "
+                    "both be float32", c.adim, FS2_SPEMB_MAX_DIM);
+          return FS2_ERR_INVALID;
+        }
+        if ((rc = copy("spk_embed_proj.weight", pw->shape[1] * c.adim, &h->spemb_w))) return rc;
+        if ((rc = copy("spk_embed_proj.bias", c.adim, &h->spemb_b))) return rc;
+        h->spemb_dim = (int)pw->shape[1];
+      }
+    }
     // decoder (fastspeech.py:119-136; input layer core/encoder.py:118-125)
     if ((rc = dense("decoder.embed.0.weight", "decoder.embed.0.bias", c.ddim, c.adim, 1, &h->dec_in))) return rc;
     if ((rc = norm("decoder.embed.1.", c.ddim, 1e-5f, &h->dec_in_ln))) return rc;
@@ -394,8 +413,9 @@ struct Packer {
 
 // Workspace layouts.  A tensor exists either as fp32 rows (fp32 / tf32 families) or as fp16 operand planes [2][rows][K]
 // (plane families) -- the same bytes, so the two views alias one allocation.
-struct EncodePlan { BlockBufs w; float *t1, *t2; __half* t2p; };
-EncodePlan plan_encode(const fs2_config& c, Bump& b, int B, int T) {
+struct EncodePlan { BlockBufs w; float *t1, *t2; __half* t2p; float* v; };
+// spemb: the handle has a speaker-embedding projection, whose per-utterance vectors v [B, adim] then live here too
+EncodePlan plan_encode(const fs2_config& c, Bump& b, int B, int T, bool spemb) {
   const int64_t rows = (int64_t)B * T;
   EncodePlan p;
   p.w.x = b.floats(rows * c.adim); p.w.y = b.floats(rows * c.adim);
@@ -405,6 +425,7 @@ EncodePlan plan_encode(const fs2_config& c, Bump& b, int B, int T) {
   p.w.ctx = b.floats(rows * c.adim); p.w.ctxp = (__half*)p.w.ctx;
   p.w.hid = b.floats(rows * c.eunits); p.w.hidp = (__half*)p.w.hid;
   p.t1 = b.floats(rows * c.pred_chans); p.t2 = b.floats(rows * c.pred_chans); p.t2p = (__half*)p.t2;
+  p.v = spemb ? b.floats((int64_t)B * c.adim) : nullptr;
   return p;
 }
 struct DecodePlan { BlockBufs w; float *hm2, *t1, *t2, *q1, *q2; __half *hmp, *hm2p, *t2p, *beforep; };
@@ -423,6 +444,19 @@ DecodePlan plan_decode(const fs2_config& c, Bump& b, int B, int L) {
   p.q1 = b.floats(rows * c.postnet_chans); p.q2 = b.floats(rows * c.postnet_chans);
   p.beforep = (__half*)b.floats(rows * c.odim);
   return p;
+}
+
+// the RowNorm of an fs2_row_norm_desc (the header's copy of its fields) plus a per-utterance vector
+RowNorm row_norm_of(const fs2_row_norm_desc& d, const float* spk_vec) {
+  RowNorm r;
+  r.x = d.x; r.ldx = d.ldx; r.resid = d.resid; r.ldr = d.ldr; r.gamma = d.gamma; r.beta = d.beta; r.eps = d.eps;
+  r.rows = d.rows; r.C = d.C; r.out = d.out; r.ldo = d.ldo; r.relu_after = d.relu_after;
+  r.pe = d.pe; r.alpha = d.alpha; r.L = d.L;
+  r.head_w = d.head_w; r.head_b = d.head_b; r.head_out = d.head_out; r.dur_out = d.dur_out; r.head_scale = d.head_scale;
+  r.lens = d.lens; r.split_out = reinterpret_cast<__half*>(d.split_out); r.split_lo = d.split_lo;
+  r.spk_table = d.spk_table; r.spk = d.spk; r.n_spk = d.n_spk; r.spk_L = d.spk_L;
+  r.spk_vec = spk_vec;
+  return r;
 }
 
 }  // namespace
@@ -516,7 +550,7 @@ int fs2_load_weights(fs2_handle* h, const fs2_weight_desc* w, int n, void* strea
 int fs2_workspace_bytes(fs2_handle* h, int B, int Tmax, int Lmax, size_t* out) {
   FS2_REQUIRE(h && out && B >= 0 && Tmax >= 0 && Lmax >= 0, "fs2_workspace_bytes: bad argument");
   Bump e(nullptr, 0), d(nullptr, 0);
-  plan_encode(h->cfg, e, B, Tmax);
+  plan_encode(h->cfg, e, B, Tmax, h->spemb_w != nullptr);
   plan_decode(h->cfg, d, B, Lmax);
   *out = (e.off > d.off ? e.off : d.off) + 1024;
   return FS2_OK;
@@ -534,19 +568,30 @@ int fs2_encode_ex(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B,
 
 int fs2_encode_spk(fs2_handle* h, const int64_t* xs, const int64_t* ilens, const int64_t* spk, int B, int Tmax, float* hs,
                    float* d_log, int64_t* d_int, void* ws, size_t ws_bytes, int flags, void* stream) {
+  return fs2_encode_spemb(h, xs, ilens, spk, nullptr, 0, B, Tmax, hs, d_log, d_int, ws, ws_bytes, flags, nullptr, nullptr, stream);
+}
+
+int fs2_encode_spemb(fs2_handle* h, const int64_t* xs, const int64_t* ilens, const int64_t* spk, const float* spembs, int D, int B,
+                     int Tmax, float* hs, float* d_log, int64_t* d_int, void* ws, size_t ws_bytes, int flags, int32_t* bad,
+                     int32_t* status, void* stream) {
   FS2_REQUIRE(h && xs && ilens && hs && ws, "fs2_encode: null argument");
   FS2_REQUIRE((flags & ~FS2_PER_UTTERANCE) == 0, "fs2_encode_ex: unknown flags 0x%x", flags);
   if (!h->loaded) { set_error("fs2_encode: weights not loaded"); return FS2_ERR_NOT_LOADED; }
   FS2_REQUIRE(!h->spk_table || spk, "fs2_encode: the model has a speaker table (%d speakers): pass speaker ids (fs2_encode_spk)",
               h->n_speakers);
   FS2_REQUIRE(h->spk_table || !spk, "fs2_encode_spk: speaker ids given but the model has no speaker table");
+  FS2_REQUIRE(!h->spemb_w || spembs, "fs2_encode: the model has a speaker-embedding projection (D=%d): pass spembs "
+              "(fs2_encode_spemb)", h->spemb_dim);
+  FS2_REQUIRE(h->spemb_w || !spembs, "fs2_encode_spemb: speaker embeddings given but the model has no projection "
+              "(spk_embed_proj)");
+  FS2_REQUIRE(!spembs || D == h->spemb_dim, "fs2_encode_spemb: D=%d but the loaded projection takes D=%d", D, h->spemb_dim);
   FS2_REQUIRE(Tmax <= h->enc_pe_len, "fs2_encode: Tmax=%d exceeds the positional table (%d rows)", Tmax, h->enc_pe_len);
   FS2_DEVICE_GUARD(h);
   cudaStream_t st = (cudaStream_t)stream;
   const fs2_config& c = h->cfg;
   t_prof = &h->prof;
   Bump b(ws, ws_bytes);
-  EncodePlan p = plan_encode(c, b, B, Tmax);
+  EncodePlan p = plan_encode(c, b, B, Tmax, h->spemb_w != nullptr);
   int rc = b.check("fs2_encode");
   if (rc) return rc;
   // the encoder's output feeds round() in the duration predictor: exact fp32 FMA in FS2_MATH_FP32,
@@ -558,6 +603,10 @@ int fs2_encode_spk(fs2_handle* h, const int64_t* xs, const int64_t* ilens, const
   float* enc_out = nullptr;
   SpeakerAdd sa;
   sa.table = h->spk_table; sa.ids = spk; sa.n = h->n_speakers;
+  if (spembs) {
+    if ((rc = spemb_project(h->spemb_w, h->spemb_b, spembs, B, D, c.adim, p.v, nullptr, bad, status, st))) return rc;
+    sa.vec = p.v;
+  }
   if ((rc = run_blocks(h->enc, p.w, ilens, zlens, B, Tmax, c.adim, c.aheads, planes ? MATH_3XTF32 : FS2_MATH_FP32, false, st,
                        &enc_out, sa))) return rc;
   FS2_CUDA_CHECK(cudaMemcpyAsync(hs, enc_out, (size_t)B * Tmax * c.adim * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -598,12 +647,19 @@ int fs2_length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, cons
 int fs2_length_plan_cap_spk(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac,
                             const int64_t* spk, int n_speakers, int B, int Tmax, int64_t Lc, int32_t* cum, int64_t* olens,
                             int64_t* need, int64_t* d_used, int32_t* status, void* stream) {
+  return fs2_length_plan_cap_spemb(ds, ds_dtype, ilens, alpha_v, fac, spk, n_speakers, nullptr, B, Tmax, Lc, cum, olens, need,
+                                   d_used, status, stream);
+}
+
+int fs2_length_plan_cap_spemb(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac,
+                              const int64_t* spk, int n_speakers, const int32_t* spemb_bad, int B, int Tmax, int64_t Lc,
+                              int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int32_t* status, void* stream) {
   FS2_REQUIRE(ds && ilens && cum && olens && need && status, "fs2_length_plan_cap: null argument");
   FS2_REQUIRE(!spk || n_speakers >= 1, "fs2_length_plan_cap_spk: speaker ids need n_speakers >= 1 (got %d)", n_speakers);
   FS2_REQUIRE(B >= 1 && Tmax >= 1, "fs2_length_plan_cap: B=%d and Tmax=%d must be >= 1", B, Tmax);
   FS2_REQUIRE(Lc >= 1 && Lc <= INT32_MAX, "fs2_length_plan_cap: capacity Lc=%lld must lie in [1, %d] (the prefix sum is int32)",
               (long long)Lc, INT32_MAX);
-  return length_plan_cap(ds, ds_dtype, ilens, alpha_v, fac, spk, n_speakers, B, Tmax, (long)Lc, cum, olens, need, d_used,
+  return length_plan_cap(ds, ds_dtype, ilens, alpha_v, fac, spk, n_speakers, spemb_bad, B, Tmax, (long)Lc, cum, olens, need, d_used,
                          status, (cudaStream_t)stream);
 }
 
@@ -862,14 +918,12 @@ int fs2_op_layernorm(const float* x, const float* resid, const float* g, const f
 int fs2_op_row_norm(const fs2_row_norm_desc* d, void* stream) {
   FS2_REQUIRE(d, "fs2_op_row_norm: null descriptor");
   FS2_REQUIRE(d->out || d->split_out || d->head_w, "fs2_op_row_norm: no output (out, split_out or head_w)");
-  RowNorm r;
-  r.x = d->x; r.ldx = d->ldx; r.resid = d->resid; r.ldr = d->ldr; r.gamma = d->gamma; r.beta = d->beta; r.eps = d->eps;
-  r.rows = d->rows; r.C = d->C; r.out = d->out; r.ldo = d->ldo; r.relu_after = d->relu_after;
-  r.pe = d->pe; r.alpha = d->alpha; r.L = d->L;
-  r.head_w = d->head_w; r.head_b = d->head_b; r.head_out = d->head_out; r.dur_out = d->dur_out; r.head_scale = d->head_scale;
-  r.lens = d->lens; r.split_out = reinterpret_cast<__half*>(d->split_out); r.split_lo = d->split_lo;
-  r.spk_table = d->spk_table; r.spk = d->spk; r.n_spk = d->n_spk; r.spk_L = d->spk_L;
-  return row_norm(r, (cudaStream_t)stream);
+  return row_norm(row_norm_of(*d, nullptr), (cudaStream_t)stream);
+}
+int fs2_op_row_norm_spemb(const fs2_row_norm_desc* d, const float* spk_vec, void* stream) {
+  FS2_REQUIRE(d, "fs2_op_row_norm_spemb: null descriptor");
+  FS2_REQUIRE(d->out || d->split_out || d->head_w, "fs2_op_row_norm_spemb: no output (out, split_out or head_w)");
+  return row_norm(row_norm_of(*d, spk_vec), (cudaStream_t)stream);
 }
 int fs2_op_variance_embed_add(const float* hm, const float* e_val, const float* p_val, const float* e_bins, const float* p_bins,
                               int n_edges, const float* e_tab, const float* e_bias, const float* p_tab, const float* p_bias,

@@ -132,8 +132,16 @@ struct RowNorm {
   // fp32 add after gamma / beta, before out, split_out and the head.  An id outside [0, n_spk) adds nothing; masked rows
   // (lens) still write 0
   const float* spk_table; const int64_t* spk; int n_spk; int spk_L;
+  // optional per-utterance vector (projected external speaker embeddings, DESIGN.md section 27): y += spk_vec[row / spk_L],
+  // one more fp32 add after the table's, so y = (LN + E[spk]) + v; needs spk_L > 0
+  const float* spk_vec;
 };
 int row_norm(const RowNorm& r, cudaStream_t st);
+// v [B, A] = W [A, D] . normalize(e [B, D]) + bias (spembs.cu); en [B, D] (nullable) receives the normalised embeddings,
+// bad [B] (nullable) 1 where e_b holds a non-finite value or its sum of squares overflows fp32, else 0; status (nullable)
+// |= FS2_SPEMB_NONFINITE then
+int spemb_project(const float* W, const float* bias, const float* e, int B, int D, int A, float* v, float* en, int32_t* bad,
+                  int32_t* status, cudaStream_t st);
 
 // lens (nullable): rows t >= lens[b] are written as zeros (per-utterance mode)
 int embed_posenc(const int64_t* xs, const float* table, int n_sym, const float* pe, const float* alpha, int B, int T,
@@ -166,9 +174,10 @@ int transpose_v(const float* qkv, int B, int L, int C, int heads, float* vt, int
 // alpha_v (nullable): per-phoneme factors [B, T] in place of the scalar alpha; d_used (nullable): [B, T] frame counts expanded
 int length_plan(void* ds, int ds_dtype, const int64_t* ilens, float alpha, const float* alpha_v, int B, int T, int mutate,
                 int32_t* cum, int64_t* olens, int64_t* stats, int64_t* d_used, cudaStream_t st);
-// spk (nullable) [B]: a non-empty slot whose id lies outside [0, n_spk) is emptied and sets FS2_PLAN_BAD_SPEAKER
+// spk (nullable) [B]: a non-empty slot whose id lies outside [0, n_spk) is emptied and sets FS2_PLAN_BAD_SPEAKER;
+// spemb_bad (nullable) [B]: a non-empty slot with spemb_bad[b] != 0 is emptied and sets FS2_SPEMB_NONFINITE
 int length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac, const int64_t* spk,
-                    int n_spk, int B, int T, long Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int* status,
+                    int n_spk, const int32_t* spemb_bad, int B, int T, long Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int* status,
                     cudaStream_t st);
 int synth_status(const int* plan, const int* voc, const int64_t* olens, int B, int hop, int* word, int64_t* alens, cudaStream_t st);
 int length_gather(const float* hs, const int32_t* cum, const int64_t* ilens, int B, int T, int C, float* out, int Lcap,

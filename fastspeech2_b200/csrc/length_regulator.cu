@@ -47,6 +47,7 @@ struct CapArgs {
   int* status;
   const int64_t* spk;        // [B] speaker ids checked against [0, n_spk), or NULL
   int n_spk;
+  const int32_t* spemb_bad;  // [B] non-finite speaker embeddings (fs2_spemb_project's bad), or NULL
 };
 
 __device__ __forceinline__ bool bad_factor(float a) { return !(isfinite(a) && a > 0.f); }
@@ -133,7 +134,8 @@ length_plan_kernel(void* ds, int dtype, const int64_t* __restrict__ ilens, float
     const long need = carry_s;
     const bool bad_ilen = ilen_in < 0 || ilen_in > T, over = need > cap.Lc;
     const bool bad_spk = cap.spk && ilen_in != 0 && (cap.spk[b] < 0 || cap.spk[b] >= cap.n_spk);   // empty slots need no id
-    const bool live = ilen_in >= 1 && !bad_ilen && !over && !bad_control && !bad_spk;
+    const bool bad_spemb = cap.spemb_bad && ilen_in != 0 && cap.spemb_bad[b] != 0;                  // nor an embedding
+    const bool live = ilen_in >= 1 && !bad_ilen && !over && !bad_control && !bad_spk && !bad_spemb;
     if (!live)
       for (long t = tid; t < T; t += PLAN_THREADS) {
         cum[base + t] = 0;
@@ -143,7 +145,7 @@ length_plan_kernel(void* ds, int dtype, const int64_t* __restrict__ ilens, float
       cap.need[b] = need;
       olens[b] = live ? need : 0;
       const int bits = (bad_ilen ? FS2_PLAN_BAD_ILENS : 0) | (bad_control ? FS2_PLAN_BAD_CONTROL : 0) | (over ? FS2_PLAN_OVERFLOW : 0) |
-                       (bad_spk ? FS2_PLAN_BAD_SPEAKER : 0);
+                       (bad_spk ? FS2_PLAN_BAD_SPEAKER : 0) | (bad_spemb ? FS2_SPEMB_NONFINITE : 0);
       if (bits) atomicOr(cap.status, bits);
     }
   } else if (tid == 0) {
@@ -222,12 +224,12 @@ int length_plan(void* ds, int ds_dtype, const int64_t* ilens, float alpha, const
 }
 
 int length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac, const int64_t* spk,
-                    int n_spk, int B, int T, long Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int* status,
+                    int n_spk, const int32_t* spemb_bad, int B, int T, long Lc, int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int* status,
                     cudaStream_t st) {
   FS2_REQUIRE(ds_dtype == FS2_DUR_I64 || ds_dtype == FS2_DUR_F32 || ds_dtype == FS2_DUR_I32, "length_plan_cap: bad ds dtype %d", ds_dtype);
   FS2_CUDA_CHECK(cudaMemsetAsync(status, 0, sizeof(int), st));
   length_plan_kernel<true><<<B, PLAN_THREADS, 0, st>>>(const_cast<void*>(ds), ds_dtype, ilens, 1.0f, alpha_v, T, 0, cum, olens,
-                                                       nullptr, d_used, CapArgs{Lc, fac, need, status, spk, n_spk});
+                                                       nullptr, d_used, CapArgs{Lc, fac, need, status, spk, n_spk, spemb_bad});
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }

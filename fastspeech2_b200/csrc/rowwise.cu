@@ -46,7 +46,9 @@ __global__ void embed_posenc_kernel(const int64_t* __restrict__ xs, const float*
 // ---- LayerNorm over channels with optional residual / ReLU / pos-enc / scalar head ----------
 // encoder.py:60-69 (eps 1e-5), encoder.py:119-125, modules.py:112-120 (eps 1e-12),
 // duration_predictor.py:75-84, variance_predictor.py:50-51,75-78.
-template <int NV>
+// kSpk: the speaker adds (spk_table, spk_vec) are compiled in; only the last encoder LayerNorm of a model with a speaker
+// table or speaker embeddings launches that instantiation, so every other row norm carries no speaker code at all
+template <int NV, bool kSpk>
 __global__ void row_norm_kernel(RowNorm r) {
   pdl_trigger(); pdl_wait();
   long row = (long)blockIdx.x * ROWS_PER_CTA + (threadIdx.x >> 5);
@@ -78,10 +80,11 @@ __global__ void row_norm_kernel(RowNorm r) {
   const bool padded = r.lens && (long)t >= r.lens[bidx];
   const float alpha = r.pe ? __ldg(r.alpha) : 0.f;
   const float* srow = nullptr;    // this row's speaker vector, if any
-  if (r.spk_table) {
+  if (kSpk && r.spk_table) {
     const int64_t id = __ldg(r.spk + row / r.spk_L);
     if (id >= 0 && id < r.n_spk) srow = r.spk_table + id * C;
   }
+  const float* vrow = kSpk && r.spk_vec ? r.spk_vec + (row / r.spk_L) * C : nullptr;   // this utterance's projected embedding
   float dot = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
@@ -97,8 +100,12 @@ __global__ void row_norm_kernel(RowNorm r) {
       y.x = __fadd_rn(y.x, __fmul_rn(alpha, p.x)); y.y = __fadd_rn(y.y, __fmul_rn(alpha, p.y));
       y.z = __fadd_rn(y.z, __fmul_rn(alpha, p.z)); y.w = __fadd_rn(y.w, __fmul_rn(alpha, p.w));
     }
-    if (srow) {   // hs + E[spk]: one fp32 add
+    if (kSpk && srow) {   // hs + E[spk]: one fp32 add
       float4 e = __ldg(reinterpret_cast<const float4*>(srow + c));
+      y.x = __fadd_rn(y.x, e.x); y.y = __fadd_rn(y.y, e.y); y.z = __fadd_rn(y.z, e.z); y.w = __fadd_rn(y.w, e.w);
+    }
+    if (kSpk && vrow) {   // (hs + E[spk]) + v: one more fp32 add
+      float4 e = __ldg(reinterpret_cast<const float4*>(vrow + c));
       y.x = __fadd_rn(y.x, e.x); y.y = __fadd_rn(y.y, e.y); y.z = __fadd_rn(y.z, e.z); y.w = __fadd_rn(y.w, e.w);
     }
     if (r.head_w) {
@@ -347,6 +354,7 @@ int row_norm(const RowNorm& r, cudaStream_t st) {
   FS2_REQUIRE_ALIGNED(r.pe, 16, who, "pe");
   FS2_REQUIRE_ALIGNED(r.head_w, 16, who, "head_w");
   FS2_REQUIRE_ALIGNED(r.spk_table, 16, who, "spk_table");
+  FS2_REQUIRE_ALIGNED(r.spk_vec, 16, who, "spk_vec");
   FS2_REQUIRE_ALIGNED(r.split_out, 8, who, "split_out");
   FS2_REQUIRE(!r.pe || (r.alpha && r.L > 0), "%s: pe needs alpha and L > 0 (pe row t = row %% L)", who);
   FS2_REQUIRE(!r.lens || r.L > 0, "%s: lens needs L > 0", who);
@@ -354,10 +362,14 @@ int row_norm(const RowNorm& r, cudaStream_t st) {
   FS2_REQUIRE(!(r.head_out || r.dur_out || r.head_scale) || r.head_w,
               "%s: head_out, dur_out and head_scale need head_w and head_b", who);
   FS2_REQUIRE(!r.spk_table || (r.spk && r.spk_L > 0), "%s: a speaker table (spk_table) needs ids and rows per utterance", who);
+  FS2_REQUIRE(!r.spk_vec || r.spk_L > 0, "%s: per-utterance vectors (spk_vec) need rows per utterance (spk_L > 0)", who);
   if (r.rows == 0) return FS2_OK;
   int grid = (int)((r.rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA);
-  if (r.C == 256) { FS2_CUDA_CHECK(launch_pdl(row_norm_kernel<2>, dim3(grid), dim3(256), 0, st, r)); }
-  else if (r.C == 384) { FS2_CUDA_CHECK(launch_pdl(row_norm_kernel<3>, dim3(grid), dim3(256), 0, st, r)); }
+  const bool spk = r.spk_table || r.spk_vec;
+  void (*k2)(RowNorm) = spk ? row_norm_kernel<2, true> : row_norm_kernel<2, false>;
+  void (*k3)(RowNorm) = spk ? row_norm_kernel<3, true> : row_norm_kernel<3, false>;
+  if (r.C == 256) { FS2_CUDA_CHECK(launch_pdl(k2, dim3(grid), dim3(256), 0, st, r)); }
+  else if (r.C == 384) { FS2_CUDA_CHECK(launch_pdl(k3, dim3(grid), dim3(256), 0, st, r)); }
   else { set_error("row_norm: C=%d unsupported (256 or 384)", r.C); return FS2_ERR_INVALID; }
   FS2_LAUNCH_CHECK();
   return FS2_OK;

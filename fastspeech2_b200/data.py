@@ -12,7 +12,10 @@ Items are the reference's `TTSDataset.__getitem__` tuples (dataloader.py:47-74):
   (phoneme ids [T] int, mel [L, n_mels] float, id str, mel_len int, durations [T] int, energy [L] float, pitch [L] float),
 optionally followed by an 8th element, the speaker id (multi-speaker models, DESIGN.md section 25).  When every item of a
 batch has it, `collate_tts` and `PinnedCollator` return a 10th element, speakers [B] int64; with 7-element items the
-9-tuple is unchanged.  `FilelistDataset` reads such items from a `preprocess` tree.
+9-tuple is unchanged.  A 9th element is the utterance's speaker embedding, float32 [D] (models with spk_embed_dim,
+DESIGN.md section 27), after the speaker id or None when there is no speaker table; when every item has it, the 10th
+element is speakers [B] int64 or None, and an 11th follows, spembs [B, D] float32.  `FilelistDataset` reads such items
+from a `preprocess` tree.
 """
 from __future__ import annotations
 
@@ -28,13 +31,29 @@ def _lens(batch) -> Tuple[List[int], List[int]]:
 
 
 def _speakers(batch) -> Optional[List[int]]:
-    """The batch's speaker ids (8th item element), or None when the items have 7 elements."""
+    """The batch's speaker ids (8th item element), or None when the items have 7 elements (or 9 with None there)."""
     n = {len(it) for it in batch}
     if n == {7}:
         return None
-    if n != {8}:
-        raise ValueError(f"items must all have 7 elements, or all 8 (with the speaker id); got lengths {sorted(n)}")
+    if n not in ({8}, {9}):
+        raise ValueError(f"items must all have 7 elements, all 8 (with the speaker id) or all 9 (speaker id or None, then the "
+                         f"speaker embedding); got lengths {sorted(n)}")
+    if n == {9} and all(it[7] is None for it in batch):
+        return None
+    if any(it[7] is None for it in batch):
+        raise ValueError("items must all carry a speaker id or all carry None")
     return [int(it[7]) for it in batch]
+
+
+def _spembs(batch) -> Optional[np.ndarray]:
+    """The batch's speaker embeddings (9th item element) as float32 [B, D], or None when the items have fewer elements."""
+    if len(batch[0]) != 9:
+        return None
+    out = [np.asarray(it[8], dtype=np.float32) for it in batch]
+    shapes = {e.shape for e in out}
+    if len(shapes) != 1 or len(next(iter(shapes))) != 1:
+        raise ValueError(f"speaker embeddings must all be [D] with one D, got shapes {sorted(shapes)}")
+    return np.stack(out)
 
 
 def _fill(batch, inputs, mels, durations, energys, pitches, labels):
@@ -66,7 +85,11 @@ def collate_tts(batch: Sequence[tuple]):
     ids = [it[2] for it in batch]
     out = (inputs, torch.tensor(il, dtype=torch.int64), mels, labels, torch.tensor(ol, dtype=torch.int64), ids, durations, energys, pitches)
     spk = _speakers(batch)
-    return out if spk is None else out + (torch.tensor(spk, dtype=torch.int64),)
+    spe = _spembs(batch)
+    spk_t = None if spk is None else torch.tensor(spk, dtype=torch.int64)
+    if spe is not None:
+        return out + (spk_t, torch.from_numpy(spe))
+    return out if spk is None else out + (spk_t,)
 
 
 class _Collated(tuple):
@@ -83,7 +106,8 @@ class PinnedCollator:
     can never overwrite host memory an earlier asynchronous copy is still reading (with `slots` batches in flight).
     """
 
-    def __init__(self, max_batch: int, max_T: int, max_L: int, n_mels: int = 80, pin: Optional[bool] = None, slots: int = 2):
+    def __init__(self, max_batch: int, max_T: int, max_L: int, n_mels: int = 80, pin: Optional[bool] = None, slots: int = 2,
+                 spk_embed_dim: int = 0):
         pin = torch.cuda.is_available() if pin is None else pin
         mk = lambda shape, dt: torch.zeros(shape, dtype=dt).pin_memory() if pin else torch.zeros(shape, dtype=dt)
         self.cap = (max_batch, max_T, max_L)
@@ -92,8 +116,10 @@ class PinnedCollator:
                            mels=mk((max_batch, max_L, n_mels), torch.float32), labels=mk((max_batch, max_L), torch.float32),
                            energys=mk((max_batch, max_L), torch.float32), pitches=mk((max_batch, max_L), torch.float32),
                            ilens=mk((max_batch,), torch.int64), olens=mk((max_batch,), torch.int64),
-                           speakers=mk((max_batch,), torch.int64), event=None)
+                           speakers=mk((max_batch,), torch.int64), event=None,
+                           spembs=mk((max_batch, spk_embed_dim), torch.float32) if spk_embed_dim else None)
                       for _ in range(max(1, int(slots)))]
+        self.spk_embed_dim = int(spk_embed_dim)
         self._next = 0
 
     def __call__(self, batch: Sequence[tuple]):
@@ -120,9 +146,18 @@ class PinnedCollator:
         ilens.copy_(torch.tensor(il)); olens.copy_(torch.tensor(ol))
         items = (inputs, ilens, mels, labels, olens, [it[2] for it in batch], durations, energys, pitches)
         spk = _speakers(batch)
+        spe = _spembs(batch)
+        speakers = None
         if spk is not None:
             speakers = s["speakers"][:B]
             speakers.copy_(torch.tensor(spk, dtype=torch.int64))
+        if spe is not None:
+            if spe.shape[1] != self.spk_embed_dim:
+                raise ValueError(f"speaker embeddings of D={spe.shape[1]}, but the collator holds spk_embed_dim={self.spk_embed_dim}")
+            spembs = s["spembs"][:B]
+            spembs.copy_(torch.from_numpy(spe))
+            items = items + (speakers, spembs)
+        elif speakers is not None:
             items = items + (speakers,)
         out = _Collated(items)
         out.slot = idx
@@ -198,20 +233,25 @@ class BucketBatchSampler:
 
 
 class FilelistDataset:
-    """The reference's `TTSDataset` (dataloader.py:34-74) on a `preprocess` tree, plus the speaker id.
+    """The reference's `TTSDataset` (dataloader.py:34-74) on a `preprocess` tree, plus the speaker id and embedding.
 
     `filelist`: 5- or 6-field lines (aligner.parse_line); `data_dir`: holds mels/, energy/ and pitch/{id}.npy;
     `symbols`: the phoneme table (aligner.build_symbols -- the reference's 68-symbol table belongs to its text front-end);
     `speaker_map` ({name: id}, speakers.build_map / load_map) or None for a single-speaker corpus.  Item i is
     (phoneme ids, mel [L, n_mels], id, L, durations, energy, pitch[, speaker id]) with the reference loader's corrections:
-    durations cut to the phonemes and the last one stretched so that they sum to L, remove_outlier on energy and pitch."""
+    durations cut to the phonemes and the last one stretched so that they sum to L, remove_outlier on energy and pitch.
+    `spemb_dir` (DESIGN.md section 27): a directory of `{id}.npy` speaker embeddings, one float32 [D] per utterance (id =
+    the wav name up to its first dot), from any extractor; items then carry it as a 9th element, after the speaker id or
+    None."""
 
-    def __init__(self, filelist: str, data_dir: str, symbols: Sequence[str], speaker_map: Optional[Dict[str, int]] = None):
+    def __init__(self, filelist: str, data_dir: str, symbols: Sequence[str], speaker_map: Optional[Dict[str, int]] = None,
+                 spemb_dir: Optional[str] = None):
         from .aligner import read_filelist
         self.lines = read_filelist(filelist)
         self.data_dir = data_dir
         self.table = {s: i for i, s in enumerate(symbols)}
         self.speaker_map = speaker_map
+        self.spemb_dir = spemb_dir
         for ln in self.lines:
             if ln.durations is None:
                 raise ValueError(f"{ln.wav}: no durations (run `python -m fastspeech2_b200.aligner extract` first)")
@@ -239,11 +279,30 @@ class FilelistDataset:
         e = remove_outlier(np.load(path("energy")))
         p = remove_outlier(np.load(path("pitch")))
         item = (x, mel.T, ln.id, L, np.array(d, dtype=np.int64), e, p)
-        if self.speaker_map is None:
-            return item
-        from .speakers import speaker_of
-        return item + (self.speaker_map[speaker_of(ln)],)
+        spk = None
+        if self.speaker_map is not None:
+            from .speakers import speaker_of
+            spk = self.speaker_map[speaker_of(ln)]
+        if self.spemb_dir is None:
+            return item if spk is None else item + (spk,)
+        return item + (spk, load_spemb(os.path.join(self.spemb_dir, ln.id + ".npy")))
+
+    def spemb_dim(self) -> int:
+        """D of the first utterance's embedding (spemb_dir given), else 0."""
+        if self.spemb_dir is None or not self.lines:
+            return 0
+        return int(load_spemb(os.path.join(self.spemb_dir, self.lines[0].id + ".npy")).shape[0])
 
     def mel_lengths(self) -> List[int]:
         """Frames per item (BucketBatchSampler's lengths), read from the mel files' headers."""
         return [int(np.load(os.path.join(self.data_dir, "mels", ln.id + ".npy"), mmap_mode="r").shape[1]) for ln in self.lines]
+
+
+def load_spemb(path: str) -> np.ndarray:
+    """One speaker embedding file: a [D] (or [1, D]) array of any float dtype -> float32 [D]."""
+    e = np.load(path)
+    if e.ndim == 2 and e.shape[0] == 1:
+        e = e[0]
+    if e.ndim != 1 or e.shape[0] < 1 or not np.issubdtype(e.dtype, np.floating):
+        raise ValueError(f"{path}: a speaker embedding must be a float [D] array, got {e.dtype} {e.shape}")
+    return e.astype(np.float32)

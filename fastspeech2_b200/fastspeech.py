@@ -361,10 +361,63 @@ def _one_speaker(speaker: Any) -> Optional[torch.Tensor]:
     return torch.tensor([speaker], dtype=torch.int64)
 
 
-def _without(fn, name: str) -> inspect.Signature:
-    """fn's signature without the parameter `name`."""
+SPEMB_INTEGRATION_TYPES = ("add",)
+
+
+def spk_embed_dim_from_hp(hp: Any) -> int:
+    """hp.model.spk_embed_dim: absent, None or 0 is a model without speaker embeddings; else D in [1, 4096].
+    hp.model.spk_embed_integration_type, when set, must be "add" (ESPnet2's default)."""
+    m = _get(hp, "model")
+    kind = _get(m, "spk_embed_integration_type", None)
+    if kind is not None and kind not in SPEMB_INTEGRATION_TYPES:
+        raise ValueError(f"hp.model.spk_embed_integration_type must be one of {list(SPEMB_INTEGRATION_TYPES)}, got {kind!r}")
+    v = _get(m, "spk_embed_dim", 0)
+    return _check_spk_embed_dim(0 if v is None else v, "hp.model.spk_embed_dim")
+
+
+def _check_spk_embed_dim(v: Any, what: str) -> int:
+    if isinstance(v, bool) or not isinstance(v, int) or not (v == 0 or 1 <= v <= _lib.FS2_SPEMB_MAX_DIM):
+        raise ValueError(f"{what} must be 0 (none) or an int in [1, {_lib.FS2_SPEMB_MAX_DIM}], got {v!r}")
+    return int(v)
+
+
+def _spemb_tensor(D: int, spembs: Any, B: int, dev: torch.device) -> Optional[torch.Tensor]:
+    """Speaker embeddings of a call -> None (model without spk_embed_dim) or a contiguous float32 [B, D] tensor on `dev`,
+    detached (embeddings are data).  Non-finite values are found on the device (fs2_spemb_project's status bit)."""
+    if D == 0:
+        if spembs is not None:
+            raise ValueError("speaker embeddings were given but the model has no projection (hp.model.spk_embed_dim is 0)")
+        return None
+    if spembs is None:
+        raise ValueError(f"the model takes {D}-dim speaker embeddings: pass them (spembs= / spemb=)")
+    if not torch.is_tensor(spembs) or spembs.dtype != torch.float32:
+        raise ValueError(f"spembs must be a float32 tensor, got {getattr(spembs, 'dtype', type(spembs).__name__)}")
+    if spembs.dim() != 2 or tuple(spembs.shape) != (B, D):
+        raise ValueError(f"spembs must be [B={B}, D={D}], got {tuple(spembs.shape)}")
+    if spembs.device != dev:
+        raise ValueError(f"spembs must be on {dev} with the model's input, got {spembs.device}")
+    return spembs.detach().contiguous()
+
+
+def _one_spemb(spemb: Any) -> Any:
+    """`inference`'s spemb [D] -> [1, D] (anything else is left to _spemb_tensor to refuse)."""
+    if torch.is_tensor(spemb) and spemb.dim() == 1:
+        return spemb[None]
+    if torch.is_tensor(spemb):
+        raise ValueError(f"spemb must be a [D] tensor, got shape {tuple(spemb.shape)}")
+    return spemb
+
+
+def _check_spemb_status(word: int) -> None:
+    if word & _lib.FS2_SPEMB_NONFINITE:
+        raise ValueError("spembs: some speaker embedding(s) hold non-finite values, or values so large (above ~1.8e19) that "
+                         "their fp32 sum of squares overflows")
+
+
+def _without(fn, *names: str) -> inspect.Signature:
+    """fn's signature without the parameters `names`."""
     sig = inspect.signature(fn)
-    return sig.replace(parameters=[p for p in sig.parameters.values() if p.name != name])
+    return sig.replace(parameters=[p for p in sig.parameters.values() if p.name not in names])
 
 
 # ------------------------------------------------------------------------------------------------
@@ -394,14 +447,21 @@ class FeedForwardTransformer(nn.Module):
         n_hp = n_speakers_from_hp(hp)
         if n_hp and n_hp != n_spk:
             raise ValueError(f"hp.model.n_speakers = {n_hp} but the checkpoint's speaker table has {n_spk} rows")
+        # and the speaker-embedding width from the projection (DESIGN.md section 27)
+        proj = sd.get("spk_embed_proj.weight")
+        d_spe = int(proj.shape[1]) if proj is not None else 0
+        d_hp = spk_embed_dim_from_hp(hp)
+        if d_hp and d_hp != d_spe:
+            raise ValueError(f"hp.model.spk_embed_dim = {d_hp} but the checkpoint's spk_embed_proj.weight takes D = {d_spe}")
         model = cls(idim, odim, hp, precision=precision, train_precision=train_precision, train_attention=train_attention,
-                    n_speakers=n_spk, train_deterministic=train_deterministic)
+                    n_speakers=n_spk, train_deterministic=train_deterministic, spk_embed_dim=d_spe)
         model.load_state_dict(sd, strict="model" in checkpoint)
         model.eval()
         return model.to(device) if device is not None else model
 
     def __init__(self, idim: int, odim: int, hp: Dict, precision: Optional[str] = None, train_precision: Optional[str] = None,
-                 train_attention: Optional[str] = None, n_speakers: Optional[int] = None, train_deterministic: Optional[bool] = None):
+                 train_attention: Optional[str] = None, n_speakers: Optional[int] = None, train_deterministic: Optional[bool] = None,
+                 spk_embed_dim: Optional[int] = None):
         super().__init__()
         dims = dims_from_hp(idim, odim, hp)
         self.dims = dims
@@ -450,6 +510,13 @@ class FeedForwardTransformer(nn.Module):
             raise ValueError(f"n_speakers must be >= 0, got {self.n_speakers}")
         if self.n_speakers:
             self.speaker_embed = nn.Embedding(self.n_speakers, A)
+        # external speaker embeddings (DESIGN.md section 27): ESPnet2's spk_embed_proj, created after everything else (the
+        # speaker table included), so its two keys come last and every other parameter draws the same initial values;
+        # nn.Linear's default init
+        d_hp = spk_embed_dim_from_hp(hp)
+        self.spk_embed_dim = d_hp if spk_embed_dim is None else _check_spk_embed_dim(spk_embed_dim, "spk_embed_dim")
+        if self.spk_embed_dim:
+            self.spk_embed_proj = nn.Linear(self.spk_embed_dim, A)
 
         self.postnet_dropout_rate = float(_get(m, "postnet_dropout_rate", 0.5))
         self.duration_dropout_rate = float(_get(m, "duration_predictor_dropout_rate", 0.1))
@@ -566,7 +633,8 @@ class FeedForwardTransformer(nn.Module):
                  es: torch.Tensor = None, ps: torch.Tensor = None, is_inference: bool = False,
                  _one_hot: bool = True, _defer_check: Optional[list] = None, _after_out: Optional[torch.Tensor] = None,
                  per_utterance: bool = False, _olens_out: Optional[list] = None,
-                 _controls: Optional[Tuple] = None, speakers: Optional[torch.Tensor] = None) -> Sequence[torch.Tensor]:
+                 _controls: Optional[Tuple] = None, speakers: Optional[torch.Tensor] = None,
+                 spembs: Optional[torch.Tensor] = None) -> Sequence[torch.Tensor]:
         """The reference's `_forward` (fastspeech.py:169-243).  `per_utterance=True` (not in the reference) makes every
         utterance's result independent of its batch mates: utterance b is bit-identical to the B = 1 call on
         `xs[b:b+1, :ilens[b]]` (teacher-forced: with its es / ps sliced to olens[b]), in inference the decoder is masked by
@@ -577,13 +645,14 @@ class FeedForwardTransformer(nn.Module):
         only where an utterance's result does not depend on its batch mates (per_utterance, or B = 1); the returned
         durations are then the frame counts actually expanded.  `speakers` (multi-speaker models, DESIGN.md section 25):
         int64 [B] ids in [0, n_speakers); E[speakers[b]] is added to the encoder output at every row (reference semantics)
-        or at rows t < ilens[b] (per_utterance)."""
+        or at rows t < ilens[b] (per_utterance).  `spembs` (models with spk_embed_dim = D, DESIGN.md section 27): float32
+        [B, D] on the device; W . normalize(spembs[b]) + bias is added after the table, over the same rows."""
         # the handle-less ABI stages (LengthRegulator, losses, ...) run on the CURRENT device like any CUDA library call:
         # select the device the data lives on for the whole call, leave the caller's current device untouched
         if xs.is_cuda and torch.cuda.current_device() != (xs.device.index or 0):
             with torch.cuda.device(xs.device):
                 return self._forward(xs, ilens, olens, ds, es, ps, is_inference, _one_hot, _defer_check, _after_out,
-                                     per_utterance, _olens_out, _controls, speakers)
+                                     per_utterance, _olens_out, _controls, speakers, spembs)
         if _controls is not None:
             if not is_inference:
                 raise ValueError("prosody controls apply to inference only (teacher-forced durations, energy and pitch are given)")
@@ -595,6 +664,7 @@ class FeedForwardTransformer(nn.Module):
         if xs.dim() != 2:
             raise ValueError("xs must be [B, Tmax]")
         spk = _speaker_ids(self.n_speakers, speakers, int(xs.shape[0]), xs.device)
+        spe = _spemb_tensor(self.spk_embed_dim, spembs, int(xs.shape[0]), xs.device)
         h = self._ready(xs)
         lib = _lib.load()
         dev, d = xs.device, self.dims
@@ -626,8 +696,14 @@ class FeedForwardTransformer(nn.Module):
         hs = torch.empty((B, T, d.adim), **f32)
         d_log = None if is_inference else torch.empty((B, T), **f32)
         d_int = torch.empty((B, T), dtype=torch.int64, device=dev) if is_inference else None
-        _lib.check(lib.fs2_encode_spk(h, _lib.ptr(xs), _lib.ptr(ilens), _lib.ptr(spk), B, T, _lib.ptr(hs), _lib.ptr(d_log),
-                                      _lib.ptr(d_int), _lib.ptr(ws), ws.numel(), flags, st), "fs2_encode_spk")
+        if spe is None:
+            _lib.check(lib.fs2_encode_spk(h, _lib.ptr(xs), _lib.ptr(ilens), _lib.ptr(spk), B, T, _lib.ptr(hs), _lib.ptr(d_log),
+                                          _lib.ptr(d_int), _lib.ptr(ws), ws.numel(), flags, st), "fs2_encode_spk")
+        else:
+            spe_status = torch.zeros((1,), dtype=torch.int32, device=dev)
+            _lib.check(lib.fs2_encode_spemb(h, _lib.ptr(xs), _lib.ptr(ilens), _lib.ptr(spk), _lib.ptr(spe), self.spk_embed_dim, B, T,
+                                            _lib.ptr(hs), _lib.ptr(d_log), _lib.ptr(d_int), _lib.ptr(ws), ws.numel(), flags, None,
+                                            _lib.ptr(spe_status), st), "fs2_encode_spemb")
 
         # stage 2: length regulator
         speed, pitch, energy = _controls if _controls is not None else (None, None, None)
@@ -645,7 +721,11 @@ class FeedForwardTransformer(nn.Module):
                 words.append(_control_violations(_controls, ilens, T).view(1))
             if spk is not None:     # and the speaker range
                 words.append(_speaker_violations(spk, self.n_speakers))
+            if spe is not None:     # and the embeddings' status word
+                words.append(spe_status.to(torch.int64))
             vals = torch.cat(words).tolist() if len(words) > 1 else stats.tolist()  # the single host sync of inference
+            if spe is not None:
+                _check_spemb_status(vals.pop())
             if spk is not None:
                 _check_speaker_range(vals.pop(), self.n_speakers)
             if _controls is not None and vals[-1]:
@@ -711,6 +791,8 @@ class FeedForwardTransformer(nn.Module):
         chk_dev = torch.stack([stats[0], stats[1], ilens.max(), olens_dec.max()])
         if spk is not None:     # the speaker range rides in the same transfer
             chk_dev = torch.cat([chk_dev, _speaker_violations(spk, self.n_speakers)])
+        if spe is not None:     # and the embeddings' status word, last
+            chk_dev = torch.cat([chk_dev, spe_status.to(torch.int64)])
         if _defer_check is not None:          # CUDA-graph capture: no host read here, the caller validates after replay
             _defer_check.append((chk_dev, T, L))
             return before, after, d_log, e_out, p_out
@@ -721,6 +803,8 @@ class FeedForwardTransformer(nn.Module):
                 raise ValueError(f"per_utterance: olens differs from sum(ds) in {chk[-1]} utterance(s)")
         else:
             chk = chk_dev.tolist()
+        if spe is not None:
+            _check_spemb_status(chk[4 + (spk is not None)])
         if spk is not None:
             _check_speaker_range(chk[4], self.n_speakers)
         self._validate_lengths(chk[:4], T, L)
@@ -762,17 +846,19 @@ class FeedForwardTransformer(nn.Module):
         return GraphedSynthesis(self, B, T, capacity, vocoder)
 
     def forward(self, xs: torch.Tensor, ilens: torch.Tensor, ys: torch.Tensor, olens: torch.Tensor, ds: torch.Tensor,
-                es: torch.Tensor, ps: torch.Tensor, speakers: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, List[Dict[str, float]]]:
+                es: torch.Tensor, ps: torch.Tensor, speakers: Optional[torch.Tensor] = None,
+                spembs: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, List[Dict[str, float]]]:
         """Loss computation (fastspeech.py:245-337). Returns (loss, report_keys).  In train mode the loss is attached to
         the autograd graph of the train path (fastspeech2_b200/train.py) so `loss.backward()` fills `.grad` of every
         parameter the reference trains; `self.dropout_masks` (a train.MaskSource) may be set to inject masks.
-        `speakers`: int64 [B] ids of a multi-speaker model (required there, refused otherwise)."""
+        `speakers`: int64 [B] ids of a multi-speaker model (required there, refused otherwise).  `spembs`: float32 [B, D]
+        speaker embeddings of a model with spk_embed_dim = D (required there, refused otherwise); they get no gradient."""
         if xs.is_cuda and torch.cuda.current_device() != (xs.device.index or 0):
             with torch.cuda.device(xs.device):
-                return self.forward(xs, ilens, ys, olens, ds, es, ps, speakers)
+                return self.forward(xs, ilens, ys, olens, ds, es, ps, speakers, spembs)
         from .train import deterministic_step, masked_losses, train_forward
         if self.training:
-            return train_forward(self, xs, ilens, ys, olens, ds, es, ps, masks=self.dropout_masks, speakers=speakers)
+            return train_forward(self, xs, ilens, ys, olens, ds, es, ps, masks=self.dropout_masks, speakers=speakers, spembs=spembs)
         self._ready(xs)
         lib = _lib.load()
         dev = xs.device
@@ -783,7 +869,7 @@ class FeedForwardTransformer(nn.Module):
         ds_t = ds[:, :tmax].contiguous() if ds.shape[1] != tmax else ds
         es_t, ps_t = es[:, :lmax], ps[:, :lmax]
         before, after, d_outs, e_outs, p_outs = self._forward(xs, ilens, olens, ds_t, es_t, ps_t, is_inference=False,
-                                                              speakers=speakers)
+                                                              speakers=speakers, spembs=spembs)
         if ds_t is not ds and ds_t.shape == ds[:, :tmax].shape:
             ds[:, :tmax].copy_(ds_t)
         B, T = xs.shape
@@ -804,19 +890,21 @@ class FeedForwardTransformer(nn.Module):
         names = ["l1_loss", "before_loss", "after_loss", "duration_loss", "energy_loss", "pitch_loss", "loss"]
         return out7[6], [{k: v} for k, v in zip(names, vals)]
 
-    def inference(self, x: torch.Tensor, speaker=None) -> torch.Tensor:
+    def inference(self, x: torch.Tensor, speaker=None, spemb=None) -> torch.Tensor:
         """x [T] int64 -> mel [L, odim] (fastspeech.py:339-357).  speaker: the id (an int or a 0-d int64 tensor) of a
-        multi-speaker model."""
+        multi-speaker model; spemb: the float32 [D] speaker embedding of a model with spk_embed_dim = D."""
         ilens = torch.tensor([x.shape[0]], dtype=torch.long, device=x.device)
-        _, outs, _, _, _ = self._forward(x.unsqueeze(0), ilens, is_inference=True, _one_hot=False, speakers=_one_speaker(speaker))
+        _, outs, _, _, _ = self._forward(x.unsqueeze(0), ilens, is_inference=True, _one_hot=False, speakers=_one_speaker(speaker),
+                                         spembs=_one_spemb(spemb))
         return outs[0]
 
     # `forward` and `inference` report the reference's signatures to introspection (fastspeech.py:245-254, :339, what
-    # drop-in launchers check); `speakers` / `speaker` are extra keywords that only multi-speaker models use
-    forward.__signature__ = _without(forward, "speakers")
-    inference.__signature__ = _without(inference, "speaker")
+    # drop-in launchers check); `speakers` / `speaker` and `spembs` / `spemb` are extra keywords that only multi-speaker
+    # models and models with speaker embeddings use
+    forward.__signature__ = _without(forward, "speakers", "spembs")
+    inference.__signature__ = _without(inference, "speaker", "spemb")
 
-    def inference_controlled(self, x: torch.Tensor, *, speed=None, pitch=None, energy=None, speaker=None) -> torch.Tensor:
+    def inference_controlled(self, x: torch.Tensor, *, speed=None, pitch=None, energy=None, speaker=None, spemb=None) -> torch.Tensor:
         """`inference` with prosody controls (not in the reference, whose `_forward` passes alpha = 1 to its
         LengthRegulator and pitch / energy predictors; `inference` itself keeps the reference's signature).  Each control
         is None, a number or a [T] tensor of per-phoneme factors, finite and > 0.  speed multiplies the predicted
@@ -835,11 +923,11 @@ class FeedForwardTransformer(nn.Module):
         controls = _controls_for(1, int(x.shape[0]), x.device, ctl)
         ilens = torch.tensor([x.shape[0]], dtype=torch.long, device=x.device)
         _, outs, _, _, _ = self._forward(x.unsqueeze(0), ilens, is_inference=True, _one_hot=False, _controls=controls,
-                                         speakers=_one_speaker(speaker))
+                                         speakers=_one_speaker(speaker), spembs=_one_spemb(spemb))
         return outs[0]
 
     def synthesize(self, xs: torch.Tensor, ilens: torch.Tensor, *, speakers=None, speed=None, pitch=None,
-                   energy=None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                   energy=None, spembs=None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Per-utterance batched inference (not in the reference): xs [B, Tmax] int64 (0 = pad), ilens [B] with
         1 <= ilens[b] <= Tmax -> (mels [B, Lmax, odim], olens [B] int64, durations [B, Tmax] int64), all on the device.
         durations[b], olens[b] and mels[b, :olens[b]] are bit-identical to what `inference(xs[b, :ilens[b]])` computes,
@@ -848,14 +936,15 @@ class FeedForwardTransformer(nn.Module):
         utterance) or a [B, Tmax] tensor (per phoneme; entries past ilens[b] are ignored).  Utterance b is then
         bit-identical to `inference_controlled` on it with its slice of the controls.  durations are the frame counts expanded (after speed and
         the all-zero rule): durations.sum(1) == olens.  speakers: int64 [B] ids of a multi-speaker model; utterance b is
-        then bit-identical to `inference` on it with speaker speakers[b]."""
+        then bit-identical to `inference` on it with speaker speakers[b].  spembs: float32 [B, D] speaker embeddings of a
+        model with spk_embed_dim = D; utterance b is then bit-identical to `inference` on it with spemb=spembs[b]."""
         if xs.dim() != 2:
             raise ValueError("xs must be [B, Tmax]")
         controls = _controls_for(int(xs.shape[0]), int(xs.shape[1]), xs.device,
                                  {"speed": speed, "pitch": pitch, "energy": energy}, ilens)
         got: list = []
         _, after, dur, _, _ = self._forward(xs, ilens, is_inference=True, _one_hot=False, per_utterance=True, _olens_out=got,
-                                            _controls=controls, speakers=speakers)
+                                            _controls=controls, speakers=speakers, spembs=spembs)
         return after, got[0], dur
 
 
@@ -947,7 +1036,8 @@ class GraphedSynthesis:
 
     Static inputs (`self.xs` [B, T], `self.ilens` [B], `self.speed` / `self.pitch` / `self.energy` [B, T] float32, 1.0
     when not set, which is bit-identical to no control; `self.speakers` [B] int64 on a multi-speaker model, whose ids the
-    plan checks on the device, so changing only the speakers between replays needs no recapture); static outputs, valid until the next replay: mels [B, capacity,
+    plan checks on the device, so changing only the speakers between replays needs no recapture; `self.spembs` [B, D]
+    float32 on a model with speaker embeddings, likewise, whose non-finite slots the plan empties); static outputs, valid until the next replay: mels [B, capacity,
     80], olens [B], durations [B, T] and need [B], and with a vocoder audio [B, capacity * 256] and alens [B] = olens * 256.
     A slot that ran is bit-identical to `synthesize` on that utterance alone (and its audio to the vocoder on that);
     rows past olens[b] and every row of a slot that did not run are +0.
@@ -980,6 +1070,9 @@ class GraphedSynthesis:
         i64, f32 = dict(dtype=torch.int64, device=dev), dict(dtype=torch.float32, device=dev)
         self.xs, self.ilens = torch.zeros((B, T), **i64), torch.zeros((B,), **i64)
         self.speakers = torch.zeros((B,), **i64) if model.n_speakers else None
+        D = model.spk_embed_dim
+        self.spembs = torch.zeros((B, D), **f32) if D else None
+        self._spemb_bad = torch.zeros((B,), dtype=torch.int32, device=dev) if D else None
         self.speed = torch.ones((B, T), **f32)
         self._fac = torch.ones((2, B, T), **f32)            # the gather's per-phoneme planes: energy, pitch
         self.energy, self.pitch = self._fac[0], self._fac[1]
@@ -1033,11 +1126,20 @@ class GraphedSynthesis:
         B, T, Lc, d = self.B, self.T, self.capacity, self.model.dims
         st = _lib.stream_ptr(self.device)
         flags = _lib.FS2_PER_UTTERANCE
-        _lib.check(lib.fs2_encode_spk(self._h, P(self.xs), P(self.ilens), P(self.speakers), B, T, P(self._hs), None, P(self._d_int),
-                                      P(self._ws), self._ws.numel(), flags, st), "fs2_encode_spk")
-        _lib.check(lib.fs2_length_plan_cap_spk(P(self._d_int), _lib.FS2_DUR_I64, P(self.ilens), P(self.speed), P(self._fac),
-                                               P(self.speakers), self.model.n_speakers, B, T, Lc, P(self._cum), P(self.olens),
-                                               P(self.need), P(self.durations), P(self._plan_status), st), "fs2_length_plan_cap_spk")
+        if self.spembs is None:
+            _lib.check(lib.fs2_encode_spk(self._h, P(self.xs), P(self.ilens), P(self.speakers), B, T, P(self._hs), None,
+                                          P(self._d_int), P(self._ws), self._ws.numel(), flags, st), "fs2_encode_spk")
+            _lib.check(lib.fs2_length_plan_cap_spk(P(self._d_int), _lib.FS2_DUR_I64, P(self.ilens), P(self.speed), P(self._fac),
+                                                   P(self.speakers), self.model.n_speakers, B, T, Lc, P(self._cum), P(self.olens),
+                                                   P(self.need), P(self.durations), P(self._plan_status), st), "fs2_length_plan_cap_spk")
+        else:   # a slot whose embedding is non-finite is emptied by the plan, which sets FS2_SPEMB_NONFINITE
+            _lib.check(lib.fs2_encode_spemb(self._h, P(self.xs), P(self.ilens), P(self.speakers), P(self.spembs),
+                                            self.model.spk_embed_dim, B, T, P(self._hs), None, P(self._d_int), P(self._ws),
+                                            self._ws.numel(), flags, P(self._spemb_bad), None, st), "fs2_encode_spemb")
+            _lib.check(lib.fs2_length_plan_cap_spemb(P(self._d_int), _lib.FS2_DUR_I64, P(self.ilens), P(self.speed), P(self._fac),
+                                                     P(self.speakers), self.model.n_speakers, P(self._spemb_bad), B, T, Lc,
+                                                     P(self._cum), P(self.olens), P(self.need), P(self.durations),
+                                                     P(self._plan_status), st), "fs2_length_plan_cap_spemb")
         _lib.check(lib.fs2_length_gather_ex(P(self._hs), P(self._cum), P(self.ilens), B, T, d.adim, P(self._hm), Lc, P(self._fac),
                                             P(self._fac_out), st), "fs2_length_gather_ex")
         _lib.check(lib.fs2_decode_ctl(self._h, P(self._hm), P(self.olens), None, None, B, Lc, P(self._before), P(self.mels),
@@ -1087,6 +1189,7 @@ class GraphedSynthesis:
             raise ValueError("prosody controls: some factor(s) are non-finite or <= 0 (each must be finite and > 0)")
         if word & _lib.FS2_PLAN_BAD_SPEAKER:
             _check_speaker_range(1, self.model.n_speakers)
+        _check_spemb_status(word)
         voc = word >> _lib.FS2_SYNTH_VOC_SHIFT
         if voc and self.vocoder is not None:
             for bit, message in self.vocoder._status_table():
@@ -1114,16 +1217,19 @@ class GraphedSynthesis:
             self.flush()
         return self.outputs
 
-    def __call__(self, xs, ilens, speakers=None, speed=None, pitch=None, energy=None, validate=True) -> tuple:
+    def __call__(self, xs, ilens, speakers=None, speed=None, pitch=None, energy=None, validate=True, spembs=None) -> tuple:
         """Synthesize b <= B requests of t <= T phonemes: xs [b, t] (0 = pad) and ilens [b] are copied into slots 0 .. b-1,
         slots b .. B-1 become empty.  speakers: int64 [b] ids of a multi-speaker model (ids on the device are checked in the
-        status word).  speed / pitch / energy: None, a number, a [b] or a [b, t] tensor, as in `synthesize`.
+        status word).  speed / pitch / energy: None, a number, a [b] or a [b, t] tensor, as in `synthesize`.  spembs:
+        float32 [b, D] speaker embeddings of a model with spk_embed_dim = D, copied into the static `self.spembs`; a
+        non-empty slot with a non-finite embedding comes out as zeros and the status word raises ValueError.
         -> `outputs` (all B slots)."""
         if validate not in (True, False, "deferred"):
             raise ValueError(f"validate must be True, False or 'deferred' (got {validate!r})")
         self._check_model()
         b, t = self.check_request(xs, ilens, self.B, self.T)
         spk = _speaker_ids(self.model.n_speakers, speakers, b, self.device)
+        spe = _spemb_tensor(self.model.spk_embed_dim, spembs, b, self.device)
         controls = _controls_for(b, t, self.device, {"speed": speed, "pitch": pitch, "energy": energy}, ilens)
         with torch.cuda.device(self.device):
             self.xs.zero_()
@@ -1133,6 +1239,9 @@ class GraphedSynthesis:
             if spk is not None:
                 self.speakers.zero_()
                 self.speakers[:b].copy_(spk, non_blocking=True)
+            if spe is not None:
+                self.spembs.zero_()
+                self.spembs[:b].copy_(spe, non_blocking=True)
             if self._controlled or controls is not None:     # factors stay 1.0 between uncontrolled requests
                 self.speed.fill_(1.0)
                 self._fac.fill_(1.0)

@@ -223,9 +223,10 @@ class PeerGather:
 
 
 def synthesize_sharded(model, xs: torch.Tensor, ilens: torch.Tensor, group: Optional[dist.ProcessGroup] = None,
-                       speakers: Optional[torch.Tensor] = None):
+                       speakers: Optional[torch.Tensor] = None, spembs: Optional[torch.Tensor] = None):
     """Batched `is_inference=True` synthesis of a global batch: every rank passes the same global
-    `xs [B,T]` / `ilens [B]` (and, for a multi-speaker model, `speakers [B]`), runs its shard and receives all mels.
+    `xs [B,T]` / `ilens [B]` (and, for a multi-speaker model, `speakers [B]`; for a model with speaker embeddings,
+    `spembs [B, D]`), runs its shard and receives all mels.
     Returns (mels, olens)."""
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
@@ -234,7 +235,8 @@ def synthesize_sharded(model, xs: torch.Tensor, ilens: torch.Tensor, group: Opti
     t = int(il.max()) if hi > lo else 0
     with torch.no_grad():
         _, after, d_outs, _, _ = model._forward(xs[lo:hi, :t].contiguous(), il, is_inference=True, _one_hot=False,
-                                                speakers=None if speakers is None else speakers[lo:hi])
+                                                speakers=None if speakers is None else speakers[lo:hi],
+                                                spembs=None if spembs is None else spembs[lo:hi])
     olens = d_outs.sum(dim=1)
     if world == 1:
         return after, olens

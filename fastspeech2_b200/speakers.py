@@ -1,6 +1,7 @@
 """Speaker names and ids of a multi-speaker corpus (DESIGN.md section 25).
 
     python -m fastspeech2_b200.speakers tag IN OUT [--map speakers.json]
+    python -m fastspeech2_b200.speakers average --filelist F --spemb-dir D -o OUT
 
 `tag` appends the speaker name as a sixth `|` field to every line of the filelist IN and writes OUT, plus the map
 {name: id} (default: speakers.json beside OUT).  The speaker name is the wav name up to its first `_`, which fits VCTK's
@@ -8,6 +9,10 @@
 reference's `TTSDataset` reads fields 0-4 by index and ignores the rest, so the tagged filelist still trains a
 single-speaker model on the reference's loader.  Ids are the sorted names numbered 0 .. n-1, so the same set of speakers
 always gives the same map; `hp.model.n_speakers` is its length.
+
+`average` (DESIGN.md section 27) writes one `{speaker}.npy` per speaker of the filelist F to OUT: the mean of that
+speaker's L2-normalised utterance embeddings `{D}/{id}.npy` (id = the wav name up to its first dot), float32 [D].  This is
+ESPnet2's usual way to synthesize a speaker from several recordings: pass the result as `spemb=`.
 """
 from __future__ import annotations
 
@@ -15,6 +20,8 @@ import argparse
 import json
 import os
 from typing import Dict, Iterable, List, Optional
+
+import numpy as np
 
 from .aligner import Line, parse_line, read_filelist
 
@@ -73,6 +80,30 @@ def tag(src: str, dst: str, map_path: Optional[str] = None) -> Dict[str, int]:
     return mapping
 
 
+def average(filelist: str, spemb_dir: str, out_dir: Optional[str] = None) -> Dict[str, np.ndarray]:
+    """{speaker: mean of the speaker's normalised utterance embeddings}, float32 [D], summed in float64 in filelist order;
+    each written to `{out_dir}/{speaker}.npy` when out_dir is given."""
+    from .data import load_spemb
+    sums: Dict[str, np.ndarray] = {}
+    counts: Dict[str, int] = {}
+    for ln in read_filelist(filelist):
+        e = load_spemb(os.path.join(spemb_dir, ln.id + ".npy")).astype(np.float64)
+        if not np.isfinite(e).all():
+            raise ValueError(f"{ln.wav}: its speaker embedding holds non-finite values")
+        e = e / max(float(np.linalg.norm(e)), 1e-12)
+        name = speaker_of(ln)
+        if name in sums and sums[name].shape != e.shape:
+            raise ValueError(f"{ln.wav}: a [{e.shape[0]}] embedding, but speaker {name} has [{sums[name].shape[0]}] ones")
+        sums[name] = sums[name] + e if name in sums else e
+        counts[name] = counts.get(name, 0) + 1
+    out = {name: (sums[name] / counts[name]).astype(np.float32) for name in sorted(sums)}
+    if out_dir is not None:
+        os.makedirs(out_dir, exist_ok=True)
+        for name, e in out.items():
+            np.save(os.path.join(out_dir, name + ".npy"), e)
+    return out
+
+
 def main(argv=None) -> None:
     ap = argparse.ArgumentParser(prog="python -m fastspeech2_b200.speakers", description=__doc__.split("\n\n")[0])
     sub = ap.add_subparsers(dest="cmd", required=True)
@@ -80,7 +111,15 @@ def main(argv=None) -> None:
     t.add_argument("src", help="filelist in the reference's five-field format")
     t.add_argument("dst", help="filelist to write")
     t.add_argument("--map", default=None, help="speaker map to write (default: speakers.json beside dst)")
+    a = sub.add_parser("average", help="write each speaker's mean normalised embedding as {speaker}.npy")
+    a.add_argument("--filelist", required=True, help="filelist whose utterances are averaged (the speaker field or wav name)")
+    a.add_argument("--spemb-dir", required=True, help="directory of {id}.npy utterance embeddings")
+    a.add_argument("-o", "--out", required=True, help="directory to write {speaker}.npy to")
     args = ap.parse_args(argv)
+    if args.cmd == "average":
+        means = average(args.filelist, args.spemb_dir, args.out)
+        print(json.dumps({"speakers": len(means), "out": args.out}))
+        return
     mapping = tag(args.src, args.dst, args.map)
     print(json.dumps({"speakers": len(mapping), "filelist": args.dst}))
 

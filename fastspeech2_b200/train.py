@@ -489,6 +489,57 @@ class SpeakerAddFn(torch.autograd.Function):
         return dy, None, dtab
 
 
+class SpembAddFn(torch.autograd.Function):
+    """hs + v.unsqueeze(1) over every row t < T, v = W . normalize(e) + bias the projected speaker embeddings (DESIGN.md
+    section 27; `spemb_project` computes v and the normalised e).  The add is fs2_speaker_add with ids 0 .. B-1 and v as
+    the table, one fp32 add.  Backward: dv[b] = sum_t dy[b, t] (fs2_speaker_add_backward with those ids, a fixed tree
+    order), then fs2_spemb_project_backward: dW += sum_b dv[b] (x) e_hat[b], dbias += sum_b dv[b], b ascending.  No
+    atomics, so it is deterministic in every train mode.  The embeddings get no gradient."""
+
+    @staticmethod
+    def forward(ctx, x, v, en, weight, bias):
+        x = _c(x)
+        B, T, C_ = x.shape
+        ids = torch.arange(B, dtype=torch.int64, device=x.device)
+        out = torch.empty_like(x)
+        _chk(_lib.load().fs2_speaker_add(x.data_ptr(), ids.data_ptr(), v.data_ptr(), B, T, C_, max(B, 1), out.data_ptr(), _st(x)),
+             "fs2_speaker_add")
+        ctx.save_for_backward(ids, en)
+        ctx.meta = (B, T, C_, int(en.shape[1]))
+        return out
+
+    @staticmethod
+    def backward(ctx, dy):
+        ids, en = ctx.saved_tensors
+        B, T, C_, D = ctx.meta
+        dy = _c(dy)
+        lib = _lib.load()
+        dv = torch.zeros((B, C_), dtype=torch.float32, device=dy.device)
+        nbytes = speaker_add_ws_bytes(B, C_)
+        ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=dy.device)
+        _chk(lib.fs2_speaker_add_backward(dy.data_ptr(), ids.data_ptr(), B, T, C_, max(B, 1), dv.data_ptr(), ws.data_ptr(), nbytes,
+                                          _st(dy)), "fs2_speaker_add_backward")
+        dW = torch.zeros((C_, D), dtype=torch.float32, device=dy.device)
+        db = torch.zeros((C_,), dtype=torch.float32, device=dy.device)
+        _chk(lib.fs2_spemb_project_backward(dv.data_ptr(), en.data_ptr(), B, D, C_, dW.data_ptr(), db.data_ptr(), _st(dy)),
+             "fs2_spemb_project_backward")
+        return dy, None, None, dW, db
+
+
+def spemb_project(weight: torch.Tensor, bias: torch.Tensor, spembs: torch.Tensor):
+    """fs2_spemb_project: (v [B, adim], e_hat [B, D], status [1] int32) for float32 [B, D] embeddings on the device.
+    status has FS2_SPEMB_NONFINITE set when some embedding holds a non-finite value or its fp32 sum of squares overflows."""
+    B, D = spembs.shape
+    A = int(weight.shape[0])
+    dev = spembs.device
+    v = torch.empty((B, A), dtype=torch.float32, device=dev)
+    en = torch.empty((B, D), dtype=torch.float32, device=dev)
+    status = torch.zeros((1,), dtype=torch.int32, device=dev)
+    _chk(_lib.load().fs2_spemb_project(_c(weight.detach()).data_ptr(), _c(bias.detach()).data_ptr(), _c(spembs).data_ptr(), B, D, A,
+                                       v.data_ptr(), en.data_ptr(), None, status.data_ptr(), _st(spembs)), "fs2_spemb_project")
+    return v, en, status
+
+
 def speaker_add_ws_bytes(B: int, C_: int) -> int:
     """Workspace bytes of fs2_speaker_add_backward for B utterances of C channels."""
     n = C.c_size_t(0)
@@ -690,10 +741,11 @@ def _predictor(pred, x, lens, rate: float, masks: MaskSource, math: int = _lib.M
     return RowDotFn.apply(x, pred.linear.weight, pred.linear.bias, lens, det)
 
 
-def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskSource] = None, speakers=None):
+def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskSource] = None, speakers=None, spembs=None):
     """`FeedForwardTransformer.forward` in train mode (fastspeech.py:245-337 -> _forward :169-243).  Returns
-    (loss 0-d tensor attached to the autograd graph, report_keys).  `speakers`: int64 [B] ids of a multi-speaker model."""
-    from .fastspeech import _check_speaker_range, _speaker_ids, _speaker_violations
+    (loss 0-d tensor attached to the autograd graph, report_keys).  `speakers`: int64 [B] ids of a multi-speaker model;
+    `spembs`: float32 [B, D] speaker embeddings of a model with spk_embed_dim = D."""
+    from .fastspeech import _check_spemb_status, _check_speaker_range, _spemb_tensor, _speaker_ids, _speaker_violations
     lib = _lib.load()
     dev = xs.device
     if dev.type != "cuda":
@@ -707,11 +759,24 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
     ilens = ilens.to(device=dev, dtype=torch.int64).contiguous()
     olens = olens.to(device=dev, dtype=torch.int64).contiguous()
     spk = _speaker_ids(model.n_speakers, speakers, int(xs.shape[0]), dev)
-    if spk is None:
+    spe = _spemb_tensor(model.spk_embed_dim, spembs, int(xs.shape[0]), dev)
+    if spe is not None:     # projected first, so that its status word rides in the host read below
+        proj = model.spk_embed_proj
+        spe_v, spe_en, spe_status = spemb_project(proj.weight, proj.bias, spe)
+    if spk is None and spe is None:
         tmax, lmax = torch.stack([ilens.max(), olens.max()]).tolist()
-    else:       # the speaker range rides in the same host read
-        tmax, lmax, bad = torch.cat([torch.stack([ilens.max(), olens.max()]), _speaker_violations(spk, model.n_speakers)]).tolist()
-        _check_speaker_range(bad, model.n_speakers)
+    else:       # the speaker range and the embeddings' status word ride in the same host read
+        words = [torch.stack([ilens.max(), olens.max()])]
+        if spk is not None:
+            words.append(_speaker_violations(spk, model.n_speakers))
+        if spe is not None:
+            words.append(spe_status.to(torch.int64))
+        vals = torch.cat(words).tolist()
+        tmax, lmax = vals[:2]
+        if spe is not None:
+            _check_spemb_status(vals.pop())
+        if spk is not None:
+            _check_speaker_range(vals[2], model.n_speakers)
     xs = xs[:, :tmax].to(torch.int64).contiguous()                                            # fastspeech.py:266-267
     ds = ds[:, :tmax].contiguous()
     es = es[:, :lmax].to(torch.float32).contiguous()
@@ -730,6 +795,8 @@ def train_forward(model, xs, ilens, ys, olens, ds, es, ps, masks: Optional[MaskS
     hs = _fft_blocks(model.encoder, x, ilens, d.aheads, ER, masks, math, flash, det)
     if spk is not None:     # hs + E[spk] at every row, fp32 in both train precisions
         hs = SpeakerAddFn.apply(hs, spk, model.speaker_embed.weight)
+    if spe is not None:     # (hs + E[spk]) + v at every row, fp32 in both train precisions
+        hs = SpembAddFn.apply(hs, spe_v, spe_en, model.spk_embed_proj.weight, model.spk_embed_proj.bias)
     # duration predictor on the encoder states, then LengthRegulator with the ground-truth durations (:209-211)
     d_outs = _predictor(model.duration_predictor, hs, ilens, model.duration_dropout_rate, masks, math, det)
     hm = LengthRegulatorFn.apply(hs, ds, ilens, L)

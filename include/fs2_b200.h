@@ -154,6 +154,25 @@ int fs2_encode_ex(fs2_handle* h, const int64_t* xs, const int64_t* ilens, int B,
 int fs2_encode_spk(fs2_handle* h, const int64_t* xs, const int64_t* ilens, const int64_t* spk, int B, int Tmax, float* hs,
                    float* d_log, int64_t* d_int, void* ws, size_t ws_bytes, int flags, void* stream);
 
+/* External speaker embeddings (DESIGN.md section 27; ESPnet2's `spembs`, integration type "add").  fs2_load_weights takes
+ * an optional "spk_embed_proj.weight" [adim, D] with "spk_embed_proj.bias" [adim] (D in [1, FS2_SPEMB_MAX_DIM] read off
+ * the tensor; fs2_config does not change).  With them loaded,
+ *   v[b, :] = W . (spembs[b, :] / max(||spembs[b, :]||_2, 1e-12)) + bias          (fs2_spemb_project, fp32, every mode)
+ *   hs[b, t, :] = (LN_last(...)[b, t, :] + table[spk[b], :]) + v[b, :]
+ * the second add in the same epilogue as the speaker table's, after it, each add rounded once.  Rows covered as for the
+ * table: every t < Tmax, or with FS2_PER_UTTERANCE only t < ilens[b].
+ *   spembs [B, D] f32 (device), D must equal the loaded projection's.
+ *   bad [B] i32 out or NULL: 1 where spembs[b] holds a non-finite value or its fp32 sum of squares overflows (elements
+ *       above ~1.8e19, which would otherwise normalise to 0), else 0.
+ *   status i32 or NULL: |= FS2_SPEMB_NONFINITE when some spembs[b] is flagged so (the caller zeroes it).
+ * The workspace (fs2_workspace_bytes) then includes B * adim floats for v.  fs2_encode_spk is the spembs = NULL case.
+ * spembs == NULL with a projection loaded, and spembs != NULL without one, are FS2_ERR_INVALID. */
+#define FS2_SPEMB_NONFINITE 16
+#define FS2_SPEMB_MAX_DIM 4096
+int fs2_encode_spemb(fs2_handle* h, const int64_t* xs, const int64_t* ilens, const int64_t* spk, const float* spembs, int D, int B,
+                     int Tmax, float* hs, float* d_log, int64_t* d_int, void* ws, size_t ws_bytes, int flags, int32_t* bad,
+                     int32_t* status, void* stream);
+
 /* ---- stage 2: LengthRegulator (needs no handle) ---------------------------------------- */
 /* core/duration_modeling/length_regulator.py:38-95 + utils/util.py:91-104.
  * Plan: per utterance, optionally scale by alpha (round half to even, :58-59), truncate to
@@ -214,6 +233,11 @@ int fs2_length_plan_cap(const void* ds, int ds_dtype, const int64_t* ilens, cons
 int fs2_length_plan_cap_spk(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac,
                             const int64_t* spk, int n_speakers, int B, int Tmax, int64_t Lc, int32_t* cum, int64_t* olens,
                             int64_t* need, int64_t* d_used, int32_t* status, void* stream);
+/* fs2_length_plan_cap_spk with the per-slot flags of fs2_encode_spemb's `bad` (NULL: none): a slot with ilens[b] != 0 and
+ * spemb_bad[b] != 0 gets olens 0 (written as zeros) and sets FS2_SPEMB_NONFINITE in the status word. */
+int fs2_length_plan_cap_spemb(const void* ds, int ds_dtype, const int64_t* ilens, const float* alpha_v, const float* fac,
+                              const int64_t* spk, int n_speakers, const int32_t* spemb_bad, int B, int Tmax, int64_t Lc,
+                              int32_t* cum, int64_t* olens, int64_t* need, int64_t* d_used, int32_t* status, void* stream);
 /* The status word of one graphed synthesis: *word = *plan_status | (vocoder bits << FS2_SYNTH_VOC_SHIFT), where the
  * vocoder's bits are *voc_status (NULL: none) without its BAD_LENGTH bit when some olens[b] is 0 (an empty, overflowed or
  * refused slot, which the vocoder reports as a bad length by design).  alens [B] i64 out or NULL: olens[b] * hop.
@@ -350,6 +374,10 @@ typedef struct fs2_row_norm_desc {
   const float* spk_table; const int64_t* spk; int32_t n_spk; int32_t spk_L;
 } fs2_row_norm_desc;
 int fs2_op_row_norm(const fs2_row_norm_desc* d, void* stream);
+/* fs2_op_row_norm with a per-utterance vector (RowNorm::spk_vec, DESIGN.md section 27): y += spk_vec[row / spk_L] after
+ * the speaker table's add, one fp32 add; spk_vec [rows / spk_L, C] f32, 16-byte aligned, needs spk_L > 0.  spk_vec == NULL
+ * is fs2_op_row_norm. */
+int fs2_op_row_norm_spemb(const fs2_row_norm_desc* d, const float* spk_vec, void* stream);
 /* hs + pitch_embed(one_hot(p_ids)) + energy_embed(one_hot(e_ids)) (fastspeech.py:218-219) as the decode stage runs it,
  * over rows = B * L rows of C in {256, 384}:
  *   id = torch.bucketize(val, bins) over n_edges sorted edges (NaN -> n_edges)
@@ -459,6 +487,18 @@ int fs2_speaker_add(const float* x, const int64_t* spk, const float* table, int 
 int fs2_speaker_add_backward_ws_bytes(int B, int C, size_t* bytes);
 int fs2_speaker_add_backward(const float* dy, const int64_t* spk, int B, int T, int C, int n, float* dtable /* += */, void* ws,
                              size_t ws_bytes, void* stream);
+/* External speaker embeddings (DESIGN.md section 27), spembs.cu.  Deterministic, fp32, no atomics on floats.
+ * fs2_spemb_project: v [B, adim] = W [adim, D] . normalize(spembs [B, D]) + bias [adim], one CTA per utterance, every sum
+ *   in an order fixed by D alone, so v[b] depends only on spembs[b].  en [B, D] out or NULL: the normalised embeddings
+ *   (the backward's input); bad [B] i32 out or NULL: 1 where spembs[b] is non-finite or its fp32 sum of squares
+ *   overflows, else 0; status i32 or NULL:
+ *   |= FS2_SPEMB_NONFINITE then.  D in [1, FS2_SPEMB_MAX_DIM], B >= 0.
+ * fs2_spemb_project_backward: dW [adim, D] += sum_b dv[b] (x) en[b] and dbias [adim] += sum_b dv[b], b ascending; dv [B, adim]
+ *   is the per-utterance sum of the output gradient (fs2_speaker_add_backward with ids 0 .. B-1 gives it). */
+int fs2_spemb_project(const float* W, const float* bias, const float* spembs, int B, int D, int adim, float* v, float* en,
+                      int32_t* bad, int32_t* status, void* stream);
+int fs2_spemb_project_backward(const float* dv, const float* en, int B, int D, int adim, float* dW /* += */,
+                               float* dbias /* += */, void* stream);
 /* pitch / energy embedding = Linear(n_bins -> C) on a one-hot (fastspeech.py:102,113,218-219), W [C, n_bins] */
 int fs2_onehot_linear_forward(const float* x, const int64_t* ids, const float* W, const float* b, int64_t rows, int C, int n_bins, float* y,
                               void* stream);
