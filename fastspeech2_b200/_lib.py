@@ -68,6 +68,8 @@ FS2_PLAN_BAD_ILENS,FS2_PLAN_BAD_CONTROL, FS2_PLAN_OVERFLOW = 1, 2, 4   # bits of
 FS2_PLAN_BAD_SPEAKER = 8                          # and of fs2_length_plan_cap_spk's
 FS2_SPEMB_NONFINITE = 16                          # fs2_spemb_project's / fs2_encode_spemb's status bit, and fs2_length_plan_cap_spemb's
 FS2_SPEMB_MAX_DIM = 4096                          # the largest speaker-embedding width D
+FS2_ECAPA_BAD_LENGTH, FS2_ECAPA_RANGE = 1, 2       # bits of fs2_ecapa's / fs2_op_ecapa_stage's status word
+FS2_ECAPA_MAX_BLOCKS, FS2_ECAPA_MAX_SCALE = 8, 16
 FS2_SYNTH_VOC_SHIFT = 8                          # fs2_synth_status: the vocoder's bits sit this far up in the word
 
 
@@ -92,6 +94,12 @@ class ISTFTNetConfig(C.Structure):
 class WorldConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("sample_rate", "fft_size", "order")] + \
                [(n, C.c_double) for n in ("frame_period", "q1", "alpha")]
+
+
+class ECAPAConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("n_mels", "channels", "n_blocks", "scale", "se_channels", "attention_channels",
+                                         "mfa_channels", "lin_neurons", "global_context")] + \
+               [("kernel_sizes", C.c_int32 * (FS2_ECAPA_MAX_BLOCKS + 2)), ("dilations", C.c_int32 * (FS2_ECAPA_MAX_BLOCKS + 2))]
 
 
 class NoamAdamHp(C.Structure):
@@ -275,6 +283,12 @@ SIGNATURES = {
     "fs2_op_waveglow_flow": [_P, _I, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P],
     "fs2_waveglow_window_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
     "fs2_waveglow_window": [_P, _P, _P, _P, _I, _I, _I, C.c_double, _P, _P, _P, _L, _P, _P, _SZ, _P],
+    "fs2_ecapa_create": [C.POINTER(_P), _I, C.POINTER(ECAPAConfig)],
+    "fs2_ecapa_n_tensors": [C.POINTER(ECAPAConfig)],
+    "fs2_ecapa_load": [_P, C.POINTER(_P), _I, _P],
+    "fs2_ecapa_workspace_bytes": [_P, _I, _I, C.POINTER(_SZ)],
+    "fs2_ecapa": [_P, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
+    "fs2_op_ecapa_stage": [_P, _I, _P, _P, _I, _I, _P, _P, _P, _SZ, _P],
     "fs2_peer_alloc": [_SZ, C.POINTER(_P), _P],
     "fs2_peer_free": [_P],
     "fs2_peer_open": [_P, C.POINTER(_P)],
@@ -289,7 +303,7 @@ SIGNATURES = {
 }
 OTHER_SYMBOLS = ("fs2_last_error", "fs2_version", "fs2_destroy", "fs2_kernel_launches", "fs2_profile_label", "fs2_vocoder_destroy",
                  "fs2_melgan_destroy", "fs2_waveglow_destroy", "fs2_features_destroy", "fs2_hifigan_destroy",
-                 "fs2_bigvgan_destroy", "fs2_istftnet_destroy")
+                 "fs2_bigvgan_destroy", "fs2_istftnet_destroy", "fs2_ecapa_destroy")
 ALL_SYMBOLS = tuple(SIGNATURES) + OTHER_SYMBOLS
 
 _lib: Optional[C.CDLL] = None
@@ -333,6 +347,8 @@ def load() -> C.CDLL:
     lib.fs2_bigvgan_destroy.argtypes = [_P]
     lib.fs2_istftnet_destroy.restype = None
     lib.fs2_istftnet_destroy.argtypes = [_P]
+    lib.fs2_ecapa_destroy.restype = None
+    lib.fs2_ecapa_destroy.argtypes = [_P]
     lib.fs2_embed_posenc = _embed_posenc_with_optional_planes(lib.fs2_embed_posenc)
     _lib = lib
     return lib

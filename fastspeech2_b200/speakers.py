@@ -2,6 +2,8 @@
 
     python -m fastspeech2_b200.speakers tag IN OUT [--map speakers.json]
     python -m fastspeech2_b200.speakers average --filelist F --spemb-dir D -o OUT
+    python -m fastspeech2_b200.speakers embed --checkpoint embedding_model.ckpt -d WAV_DIR -o SPEMB_DIR [--budget SAMPLES]
+                                              [--math-mode M]
 
 `tag` appends the speaker name as a sixth `|` field to every line of the filelist IN and writes OUT, plus the map
 {name: id} (default: speakers.json beside OUT).  The speaker name is the wav name up to its first `_`, which fits VCTK's
@@ -13,6 +15,12 @@ always gives the same map; `hp.model.n_speakers` is its length.
 `average` (DESIGN.md section 27) writes one `{speaker}.npy` per speaker of the filelist F to OUT: the mean of that
 speaker's L2-normalised utterance embeddings `{D}/{id}.npy` (id = the wav name up to its first dot), float32 [D].  This is
 ESPnet2's usual way to synthesize a speaker from several recordings: pass the result as `spemb=`.
+
+`embed` (DESIGN.md section 28) writes one float32 [D] `{id}.npy` per wav of WAV_DIR (id = the wav name up to its first
+dot, the rule of `preprocess` and `FilelistDataset(spemb_dir=)`): SpeechBrain's ECAPA-TDNN embedding of the utterance, on
+the library's kernels (`fastspeech2_b200.ecapa`), in batches of at most --budget padded samples.  Files at another rate
+than 16 kHz are resampled on the GPU with the library's resampler (`preprocess --resample`'s, librosa 0.7's kaiser_best
+semantics), not torchaudio's, so their embeddings differ from a SpeechBrain user's in that step.
 """
 from __future__ import annotations
 
@@ -104,6 +112,41 @@ def average(filelist: str, spemb_dir: str, out_dir: Optional[str] = None) -> Dic
     return out
 
 
+def embed(checkpoint, wav_dir: str, out_dir: str, budget: int = 1 << 24, math_mode: str = "3xf16", device="cuda",
+          log=print) -> int:
+    """Write `{out_dir}/{id}.npy` for every wav of wav_dir; returns how many were written."""
+    import glob
+
+    import torch
+
+    from .ecapa import SAMPLE_RATE, ECAPAEncoder
+    from .preprocess import batches, gpu_resampler
+    enc = ECAPAEncoder.from_checkpoint(checkpoint, math_mode=math_mode)
+    resample = gpu_resampler(device)
+    paths = sorted(glob.glob(os.path.join(wav_dir, "*.wav")))
+    if not paths:
+        raise ValueError(f"{wav_dir}: no .wav files")
+    os.makedirs(out_dir, exist_ok=True)
+    n = 0
+    for rate, items in batches(paths, SAMPLE_RATE, budget, resample=True):
+        ids = [i for i, _ in items]
+        wavs = [w for _, w in items]
+        if rate != SAMPLE_RATE:
+            wavs = resample(wavs, rate, SAMPLE_RATE)
+        for i, w in zip(ids, wavs):
+            if len(w) < enc.min_samples:
+                raise ValueError(f"{i}: {len(w)} samples at 16 kHz, the encoder needs at least {enc.min_samples}")
+        x = np.zeros((len(wavs), max(len(w) for w in wavs)), dtype=np.float32)
+        for b, w in enumerate(wavs):
+            x[b, : len(w)] = w
+        e = enc(torch.from_numpy(x).to(device), torch.tensor([len(w) for w in wavs], device=device)).cpu().numpy()
+        for b, i in enumerate(ids):
+            np.save(os.path.join(out_dir, i + ".npy"), e[b].astype(np.float32))
+        n += len(ids)
+        log(f"embed: {n} / {len(paths)}")
+    return n
+
+
 def main(argv=None) -> None:
     ap = argparse.ArgumentParser(prog="python -m fastspeech2_b200.speakers", description=__doc__.split("\n\n")[0])
     sub = ap.add_subparsers(dest="cmd", required=True)
@@ -115,7 +158,17 @@ def main(argv=None) -> None:
     a.add_argument("--filelist", required=True, help="filelist whose utterances are averaged (the speaker field or wav name)")
     a.add_argument("--spemb-dir", required=True, help="directory of {id}.npy utterance embeddings")
     a.add_argument("-o", "--out", required=True, help="directory to write {speaker}.npy to")
+    e = sub.add_parser("embed", help="write each wav's ECAPA-TDNN speaker embedding as {id}.npy")
+    e.add_argument("--checkpoint", required=True, help="SpeechBrain's embedding_model.ckpt (spkrec-ecapa-voxceleb)")
+    e.add_argument("-d", "--wav-dir", required=True, help="directory of .wav files (any rate; resampled to 16 kHz on the GPU)")
+    e.add_argument("-o", "--out", required=True, help="directory to write {id}.npy to")
+    e.add_argument("--budget", type=int, default=1 << 24, help="padded samples per batch (default 2^24)")
+    e.add_argument("--math-mode", default="3xf16", help="fp32, tf32, 3xf16 or f16 (default 3xf16)")
     args = ap.parse_args(argv)
+    if args.cmd == "embed":
+        n = embed(args.checkpoint, args.wav_dir, args.out, args.budget, args.math_mode, log=lambda m: None)
+        print(json.dumps({"embedded": n, "out": args.out}))
+        return
     if args.cmd == "average":
         means = average(args.filelist, args.spemb_dir, args.out)
         print(json.dumps({"speakers": len(means), "out": args.out}))

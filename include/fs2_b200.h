@@ -1166,6 +1166,49 @@ int fs2_optim_clip_noam_adam(const fs2_optim_entry* table, const int64_t* numel,
 int fs2_optim_noam_scalars(int64_t step0, int count, const fs2_noam_adam_hp* hp, double* lr, float* step_size,
                            float* bc2_sqrt, void* stream);
 
+/* ---- batched ECAPA-TDNN speaker encoder (DESIGN.md section 28) ----------------------------------------------------- */
+/* SpeechBrain's ECAPA_TDNN with its Fbank(n_mels) + sentence mean-normalisation front end, on 16 kHz audio wavs [B, Nmax]
+ * with sample counts lens [B]: emb [B, lin_neurons] fp32, row b the network applied to wavs[b, :lens[b]] alone (T_b =
+ * 1 + lens[b] / 160 frames, every "same" convolution reflect-padded at the utterance's own edges, every mean over its own
+ * frames).  emb[b] is bit-identical to a B = 1 call in every math mode; samples past lens[b] are never read.  No
+ * allocation, no synchronisation, no floating-point atomics: a call can be graph-captured and repeats bit for bit.
+ * math_mode FS2_MATH_*: every convolution GEMM; the front end and the per-utterance reductions run in fp32.
+ * *status (device int, written by the call):
+ *   FS2_ECAPA_BAD_LENGTH  some lens[b] outside [(min_frames - 1) * 160, Nmax]; that row of emb is 0
+ *   FS2_ECAPA_RANGE       an fp16 operand plane (f16 / 3xF16 modes) would saturate: some GEMM input above 4094 */
+#define FS2_ECAPA_BAD_LENGTH 1
+#define FS2_ECAPA_RANGE 2
+#define FS2_ECAPA_MAX_BLOCKS 8
+#define FS2_ECAPA_MAX_SCALE 16
+typedef struct fs2_ecapa_config {
+  int32_t n_mels, channels, n_blocks, scale, se_channels, attention_channels, mfa_channels, lin_neurons, global_context;
+  /* [0]: block 0, [1 .. n_blocks]: the SE-Res2Net blocks' Res2Net convolutions, [n_blocks + 1]: the MFA (k must be 1) */
+  int32_t kernel_sizes[FS2_ECAPA_MAX_BLOCKS + 2], dilations[FS2_ECAPA_MAX_BLOCKS + 2];
+} fs2_ecapa_config;
+typedef struct fs2_ecapa_model fs2_ecapa_model;
+/* channels a multiple of 16 * scale, n_mels, mfa_channels and attention_channels multiples of 16, odd kernel sizes */
+int fs2_ecapa_create(fs2_ecapa_model** out, int math_mode, const fs2_ecapa_config* cfg);
+void fs2_ecapa_destroy(fs2_ecapa_model* m);
+/* tensors fs2_ecapa_load takes: 4 + n_blocks * (12 + 4 * (scale - 1)) + 14 */
+int fs2_ecapa_n_tensors(const fs2_ecapa_config* cfg);
+/* t[n]: device fp32 tensors in this order, convolutions in torch's layout [Cout, Cin, k], every BatchNorm (eval) as its
+ * per-channel scale s = gamma / sqrt(var + eps) and shift beta - mean * s:
+ *   block 0: w, b, s, t;  per SE-Res2Net block: tdnn1 w, b, s, t; Res2Net j = 1 .. scale - 1: w, b, s, t; tdnn2 w, b, s, t;
+ *   se conv1 w, b; se conv2 w, b;  mfa w, b, s, t;  asp.tdnn w [A, 3M (M without global context), 1], b, s, t;
+ *   asp.conv w, b;  asp_bn s, t;  fc w, b.
+ * Copied and packed into the handle; the tensors may be freed afterwards.  Synchronises the stream once. */
+int fs2_ecapa_load(fs2_ecapa_model* m, const float* const* t, int n, void* stream);
+/* fails (FS2_ERR_INVALID) when B * (1 + Nmax / 160) reaches 2^31 (65535 * 128 in FS2_MATH_FP32), or a GEMM operand's
+ * elements reach 2^31 */
+int fs2_ecapa_workspace_bytes(fs2_ecapa_model* m, int B, int Nmax, size_t* bytes);
+int fs2_ecapa(fs2_ecapa_model* m, const float* wavs, const int64_t* lens, int B, int Nmax, float* emb, int* status, void* ws, size_t ws_bytes,
+              void* stream);
+/* One stage of fs2_ecapa (per-layer tests): 0 the front end (audio [B][L], lens in samples -> features [B][1 + L / 160][n_mels]);
+ * 1 block 0; 1 + i SE-Res2Net block i; n_blocks + 2 the MFA; n_blocks + 3 the attentive statistics pooling ([B][2M]).
+ * Stages >= 1 take rows [B * L][width] with frame counts lens; output rows past lens[b] are unspecified. */
+int fs2_op_ecapa_stage(fs2_ecapa_model* m, int stage, const float* in, const int64_t* lens, int B, int L, float* out, int* status, void* ws,
+                       size_t ws_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
